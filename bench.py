@@ -5,7 +5,7 @@ BASELINE config as a sub-record (`configs`): C3 (6 x Radial, forward + inverse),
 the ranks), C5 (RealNVP logpdf, N=2^22 TOTAL sharded, ending in the path's ONE collective, b2b_allreduce_sum_f64,
 INSIDE the timed region), each with an in-run oracle check on a 1024-column sample.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input.  Prints ONE JSON line (rank 0).
   value      whole-job samples/s with the batch resident in HBM (CUDA events, max over ranks)
@@ -54,7 +54,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth"
 
 
 def pick_threads(layers):
@@ -107,7 +107,7 @@ def cpu_baseline(nthreads=None, repeats=5, cols=NCOLS):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -266,21 +266,21 @@ def run_configs(B, torch, dist, world, rank, comm, peak, iters, warmup):
                                     r.standard_normal((Dd, K - 1)).astype(f32), 3.0)
     W, H, Dv = rqs.knots()
     orqs = O.Layer("rqs", dict(widths=W, heights=H, derivs=Dv))
-    # the shard (64 MiB / world per pass) is L2-sized: rotate over enough buffer pairs to exceed L2 (126 MB) twice over
+    # the shard (64 MiB / world per pass) is L2-sized: rotate over enough buffer pairs to exceed L2 (50 MB) twice over
     pair_bytes = 2 * N * Dd * 4
-    nbuf = max(4, int(2 * 126e6 / pair_bytes) + 1)
+    nbuf = max(4, int(2 * 50e6 / pair_bytes) + 1)
     xs = [batch(Dd, N, 1.5) for _ in range(nbuf)]
     ys = [B.colmajor_empty(Dd, N) for _ in range(nbuf)]
     lj = torch.empty(N, device="cuda")
 
-    # one shard of this pass is 5-40 us of GPU time -- less than the Python + driver launch path -- so the rotation over
+    # one shard of this pass is tens of microseconds of GPU time -- less than the Python + driver launch path -- so the rotation over
     # the buffer pairs is captured once into a CUDA graph and replayed (the entry points are launch-only, capture-safe)
     def rot_f():
         for i in range(nbuf):
             B.run_chain(rqs, xs[i], y=ys[i], logjac=lj)
 
     g_f = B.GraphedCalls(rot_f)
-    ms = timed(g_f, max(iters // 2, 3)) / nbuf
+    ms = timed(g_f, iters) / nbuf
     del g_f
     B.run_chain(rqs, xs[0], y=ys[0], logjac=lj)
     cols = sample_cols(N)
@@ -300,7 +300,7 @@ def run_configs(B, torch, dist, world, rank, comm, peak, iters, warmup):
             B.run_chain(irqs, ys[i], y=xr[i], logjac=lj)
 
     g_i = B.GraphedCalls(rot_i)
-    ms = timed(g_i, max(iters // 2, 3)) / nbuf
+    ms = timed(g_i, iters) / nbuf
     del g_i
     B.run_chain(irqs, ys[0], y=xr[0], logjac=lj)
     xo, ljio = orqs.inverse(ys[0][:, ct].cpu().numpy().astype(np.float64))
@@ -370,10 +370,21 @@ def run_configs(B, torch, dist, world, rank, comm, peak, iters, warmup):
     return out
 
 
+def dump_outputs(out_dir, torch, y, lj, ncols=1 << 14):
+    """The headline step's outputs as float32 .npy files: logjac in full (4 MiB), y on a fixed, seeded sample of
+    `ncols` columns (8 MiB at D = 128), so that two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    cols = torch.as_tensor(np.sort(np.random.default_rng(11).choice(y.shape[1], ncols, replace=False)), device=y.device)
+    np.save(os.path.join(out_dir, "y.npy"), y[:, cols].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "logjac.npy"), lj.cpu().numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20,
+                    help="timed steps of the headline chain, of its host-parameter and per-layer legs, and of every "
+                         "config sub-record (a C4 step replays the whole buffer rotation once)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--variant", type=int, default=0, help="kernel variant (0 auto, 1 v0 lane-group, 2 v1 interpreter, 3 unrolled planar)")
@@ -382,7 +393,10 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the C3/C4/C5 sub-records")
     ap.add_argument("--no-numa", action="store_true", help="do not bind the rank to its GPU's NUMA node")
     ap.add_argument("--profile", action="store_true",
-                    help="profiling runs (under ncu): only the warm-up and the timed headline steps, no JSON contract line")
+                    help="profiling runs: only the warm-up and the timed headline steps, no JSON contract line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last headline step returned: logjac.npy (all N "
+                         "columns) and y.npy (the D rows of 16384 columns drawn with a fixed seed, ascending), float32")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -403,7 +417,7 @@ def main():
     local = local_rank if args.no_numa else device_for_rank(local_rank)
     torch.cuda.set_device(local)
     # every rank next to its GPU: CPU affinity + preferred memory node BEFORE any pinned host allocation (the 8-rank
-    # e2e leg of round 1 crossed the inter-socket link with half of its copies)
+    # e2e leg otherwise crosses the inter-socket link with half of its copies)
     try:
         affinity0 = os.sched_getaffinity(0)
     except AttributeError:
@@ -455,6 +469,8 @@ def main():
     ms_total = float(ms)
     clocks = sampler.stop() if sampler else None
     value = world * NCOLS * steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, y, lj)
 
     if args.profile:
         if rank == 0:
@@ -526,28 +542,19 @@ def main():
     peak, peak_src = measured_peaks()
     configs = None
     if not args.no_configs:
-        configs = run_configs(B, torch, dist, world, rank, comm, peak, iters=max(min(steps, 10), 5), warmup=3)
+        configs = run_configs(B, torch, dist, world, rank, comm, peak, iters=steps, warmup=warmup)
 
     if rank == 0:
         ms_step = ms_total / steps
         bytes_fused = NCOLS * 4 * (2 * D + 1)  # read column + write column + write logjac, once per chain launch
         achieved = bytes_fused / (ms_step * 1e-3) / 1e9
         bytes_layerwise = NCOLS * 4 * (NLAYERS * (2 * D + 1) + (NLAYERS - 1))
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            try:
-                tj = json.load(open(tpath))
-                traffic = tj.get("chain_kernel_dram_bytes_per_launch")
-                traffic_src = tj.get("source")
-            except Exception:
-                traffic = None
         line = {
             "metric": METRIC, "value": value, "unit": "samples/s", "n_gpus": world, "steps": steps, "warmup": warmup,
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "chain": "one fused chain launch per step (column read once, written once); parameters device-resident",
-                       "l2": "inputs_larger_than_L2 (x, y 512 MiB each per GPU; L2 126 MB)",
+                       "l2": "inputs_larger_than_L2 (x, y 512 MiB each per GPU; L2 50 MB)",
                        "parallelism": f"columns sharded, {world} rank(s), no data-path collective",
                        "kernel_variant": args.variant, "numa": numa, "cuda_device_of_rank0": local},
             "gpu_launches": int(launches_per_step * steps),
@@ -559,7 +566,7 @@ def main():
                     # what the copies ask of the host memory system (DMA reads + writes of pinned DRAM, all ranks)
                     "host_dram_gbs": e2e_value * (2 * D * 4 + 4) / 1e9},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peak_src})",
+                         "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peak_src})",
                          "kernel": "planar_dev_kernel: fused 8-layer chain, 1 launch/step", "algorithmic_bytes_per_launch": bytes_fused,
                          "accounting": "chain-fused: 4*(2D+1) B/sample per launch"},
             "host_resident_parameters": {"ms_per_step": ms_hostparams, "samples_per_s": NCOLS / (ms_hostparams * 1e-3),

@@ -1,4 +1,4 @@
-"""bijectors.jl_b200 -- B200-native batched bijector evaluation path behind Bijectors.jl's Transform API.
+"""bijectors.jl_b200 -- H100-native batched bijector evaluation path behind Bijectors.jl's Transform API.
 
 Import name: ``bijectors_jl_b200`` (the directory name contains a dot; ``bijectors_jl_b200.py`` at the
 repository root registers this package under that name).

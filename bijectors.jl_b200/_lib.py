@@ -151,7 +151,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  bijectors.jl_b200 has no CPU fallback."
+                "(nvcc, sm_90a).  bijectors.jl_b200 has no CPU fallback."
             )
         handle = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL)
         for name, (res, args) in _SIGS.items():

@@ -387,7 +387,7 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
   P.L = L;
   P.accumulate = accumulate_logjac ? 1 : 0;
   long long grid = (N + F64_WARPS - 1) / F64_WARPS;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   if (sum_out) {
     if (!workspace || workspace_bytes < 4096 * sizeof(double)) return B2B_EWORKSPACE;
     P.partials = static_cast<double*>(workspace);

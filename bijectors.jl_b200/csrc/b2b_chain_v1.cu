@@ -1,7 +1,7 @@
 // v1 fused column-local chain kernel: TMA-staged, THREAD-PER-COLUMN.
 //
 // Why: in the v0 (lane-group) kernel an 8-layer chain costs ~250 warp-instructions per column (cross-lane
-// reductions, selects, broadcasts, redundant transcendental work) and the kernel is issue-bound at ~45 % of
+// reductions, selects, broadcasts, redundant transcendental work) and the kernel is issue-bound well below
 // the HBM roofline.  Here one thread owns one whole column in registers, so a row reduction is a private
 // FFMA chain (no shuffles), per-column scalars (tanh, log1p, find_alpha) are computed exactly once, and
 // every layer parameter read is a warp-uniform shared-memory broadcast.
@@ -64,10 +64,10 @@ static int plan_v1(B2BChainParams& p, V1Plan& plan) {
   int nw, tpc, cpt = 1;
   if (D == 256) { plan.kernel = chain_v1_kernel<256, 4, 1, 12>; nw = 12; tpc = 4; }
   else if (D == 128) {
-    // default: one thread per column (measured fastest: 4.4-4.5 G samples/s on C2).  Chains with per-row layers
+    // default: one thread per column.  Chains with per-row layers
     // (RQS, Stacked) use two lanes per column.  B2B_V1_CFG=2218 selects the build with two lanes per column and
     // TWO columns per thread (every parameter load serves two columns: LDS wavefronts -36 %, but more scalar work
-    // per warp; measured 4.06 G samples/s), 2112 the 2-lane / 12-warp build (3.7 G samples/s).
+    // per warp), 2112 the 2-lane / 12-warp build.
     if (cfg == 2218 && !per_row) { plan.kernel = chain_v1_kernel<128, 2, 2, 8>; nw = 8; tpc = 2; cpt = 2; }
     else if (cfg == 2112 || per_row) { plan.kernel = chain_v1_kernel<128, 2, 1, 12>; nw = 12; tpc = 2; }
     else { plan.kernel = chain_v1_kernel<128, 1, 1, 8>; nw = 8; tpc = 1; }

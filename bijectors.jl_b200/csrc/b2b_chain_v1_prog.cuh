@@ -22,13 +22,13 @@ __device__ __forceinline__ void planar_apply(float2 (&x)[CPT][D / TPC / 2], cons
     const float4 w = w4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      acc[cc][(r & 1) * 2 + 0] = __ffma2_rn(make_float2(w.x, w.y), x[cc][i], acc[cc][(r & 1) * 2 + 0]);
-      acc[cc][(r & 1) * 2 + 1] = __ffma2_rn(make_float2(w.z, w.w), x[cc][i + 1], acc[cc][(r & 1) * 2 + 1]);
+      acc[cc][(r & 1) * 2 + 0] = b2b_ffma2(make_float2(w.x, w.y), x[cc][i], acc[cc][(r & 1) * 2 + 0]);
+      acc[cc][(r & 1) * 2 + 1] = b2b_ffma2(make_float2(w.z, w.w), x[cc][i + 1], acc[cc][(r & 1) * 2 + 1]);
     }
   }
   float2 t2[CPT];
   B2B_FOR_COLS {
-    const float2 s = __fadd2_rn(__fadd2_rn(acc[cc][0], acc[cc][1]), __fadd2_rn(acc[cc][2], acc[cc][3]));
+    const float2 s = b2b_fadd2(b2b_fadd2(acc[cc][0], acc[cc][1]), b2b_fadd2(acc[cc][2], acc[cc][3]));
     const float wz = part_sum<TPC>(s.x + s.y);  // aT_b(w, z), utils.jl:2
     float t, s2;
     if (!inverse) {
@@ -45,8 +45,8 @@ __device__ __forceinline__ void planar_apply(float2 (&x)[CPT][D / TPC / 2], cons
     const float4 u = u4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      x[cc][i] = __ffma2_rn(make_float2(u.x, u.y), t2[cc], x[cc][i]);  // planar_layer.jl:78 / :124
-      x[cc][i + 1] = __ffma2_rn(make_float2(u.z, u.w), t2[cc], x[cc][i + 1]);
+      x[cc][i] = b2b_ffma2(make_float2(u.x, u.y), t2[cc], x[cc][i]);  // planar_layer.jl:78 / :124
+      x[cc][i + 1] = b2b_ffma2(make_float2(u.z, u.w), t2[cc], x[cc][i + 1]);
     }
   }
 }
@@ -62,8 +62,8 @@ __device__ __forceinline__ void batchnorm_apply(float2 (&x)[CPT][D / TPC / 2], c
     const float4 a = A4[c.prm(ql, r)], k = C4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      x[cc][i] = __ffma2_rn(x[cc][i], make_float2(a.x, a.y), make_float2(k.x, k.y));
-      x[cc][i + 1] = __ffma2_rn(x[cc][i + 1], make_float2(a.z, a.w), make_float2(k.z, k.w));
+      x[cc][i] = b2b_ffma2(x[cc][i], make_float2(a.x, a.y), make_float2(k.x, k.y));
+      x[cc][i + 1] = b2b_ffma2(x[cc][i + 1], make_float2(a.z, a.w), make_float2(k.z, k.w));
     }
   }
   const float ljc = sp[4 * D];

@@ -10,7 +10,7 @@
 // coalesced global reads, every thread computes a 4(j) x 2(s,t) x 2(col) register block of the
 // conditioner GEMM reading W through the read-only path (uniform addresses -> one sector per request,
 // W stays L1/L2 resident), the epilogue applies exp/FMA in place on the x₁ rows of the tile and the
-// tile is written back coalesced.  This is the exact-fp32 path; the tensor-core path (3xTF32 tcgen05)
+// tile is written back coalesced.  This is the exact-fp32 path; the tensor-core path (fp16-split wgmma)
 // lives in b2b_coupling_tc.cu and is cross-checked against this kernel.
 #include <cuda_runtime.h>
 

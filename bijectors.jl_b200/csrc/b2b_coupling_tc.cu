@@ -1,28 +1,28 @@
-// Affine coupling layer on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM).
+// Affine coupling layer on the Hopper tensor cores (wgmma, accumulators in registers).
 //
 // Reference: Coupling (src/bijectors/coupling.jl:206-228) with θ(x₂) = Shift(t) ∘ Scale(exp.(s)),
 // [s; t] = W·x₂ + c (scale.jl:13,31; shift.jl:14,21) mapped over the columns of the batch; see
 // b2b_coupling.cu for the exact-fp32 SIMT version this kernel is cross-checked against.
 //
 // The conditioner is a GEMM  [s;t](2·n1 x T) = W(2·n1 x n2) · X₂(n2 x T)  per tile of T = 64 columns:
-// 65.5 kFLOP per 2 KB sample at D = 256 (AI ≈ 32 FLOP/B), i.e. compute-bound on the fp32 CUDA cores at about
-// a third of the HBM roofline, hence tensor cores.  Plain TF32/BF16 cannot hold the 1e-5 parity bar, so both
+// 65.5 kFLOP per 2 KB sample at D = 256 (AI ≈ 32 FLOP/B), i.e. compute-bound on the fp32 CUDA cores,
+// hence tensor cores.  Plain TF32/BF16 cannot hold the 1e-5 parity bar, so both
 // operands are split into an fp16 "hi" and an fp16 "lo" half (22 mantissa bits together) after an EXACT
 // power-of-two rescale (W by one global 2^k, every x₂ column by its own 2^k, undone in the epilogue), and
-// three products hi·hi + hi·lo + lo·hi are accumulated in fp32 in TMEM (the dropped lo·lo term is 2^-22).
+// three products hi·hi + hi·lo + lo·hi are accumulated in fp32 (the dropped lo·lo term is 2^-22).
 //
-// Warp roles of the persistent CTA (544 threads, one CTA per SM; the roles are latency-bound, so each gets 8 warps):
-//   warps 0-7  epilogue : tcgen05.ld s/t rows out of TMEM (thread = row j = 32·(warp%4)+lane, columns
-//                         32·(warp/4)..+31 of the tile), add c, read x₁ from global (prefetched one chunk ahead),
-//                         y₁ = exp(s)·x₁ + t (or the inverse) and store -- 512 B contiguous per column
-//   warps 8-15 producers: coalesced float4 loads of the x₂ rows (prefetched one tile ahead), per-column scale
+// Warp roles of the persistent CTA (512 threads = 4 warpgroups, one CTA per SM):
+//   warpgroups 0-1  consumers: warpgroup g issues the wgmma.mma_async m64n64k16 chain (48 per tile at n2 = 128) for
+//                         rows 64g..64g+63 of both the s and the t block, so the s and t value of one (row, column)
+//                         sit in the same accumulator slot of the same thread.  x₁ of the tile is requested before
+//                         the MMAs are issued; the epilogue then adds c, forms y₁ = exp(s)·x₁ + t (or the inverse)
+//                         and stores -- each warp store covers 16 rows (64 B) of each of 8 columns
+//   warpgroups 2-3  producers: coalesced float4 loads of the x₂ rows (prefetched one tile ahead), per-column scale
 //                         (REDUX max of the float bit patterns), hi/lo split, store into the K-major 128B-swizzled
-//                         UMMA operand layout, logjac = wsum·x₂ + Σc in fp32 (Σ_j s_j = (Σ_j W_j)·x₂ + Σ_j c_j),
+//                         wgmma operand layout, logjac = wsum·x₂ + Σc in fp32 (Σ_j s_j = (Σ_j W_j)·x₂ + Σ_j c_j),
 //                         pass-through rows when y != x
-//   warp  16   MMA      : one elected lane issues 48 tcgen05.mma (M128 N64 K16, kind::f16) per tile
 // W (both halves, both M tiles) stays resident in shared memory for the lifetime of the CTA (128 KB at
-// n2 = 128); x₂ operand stages and TMEM accumulator stages are double buffered and handed over with
-// mbarriers (tcgen05.commit on the MMA side).
+// n2 = 128, loaded once by bulk copies); x₂ operand stages are double buffered and handed over with mbarriers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -33,15 +33,13 @@
 
 namespace b2b {
 
-constexpr int TC_T = 64;              // batch columns per tile == UMMA N
+constexpr int TC_T = 64;              // batch columns per tile == wgmma N
 constexpr int TC_STAGES = 2;          // x₂ operand stages in shared memory
-constexpr int TC_ACC = 2;             // accumulator stages in TMEM
 constexpr int TC_SCALE_SLOTS = 4;     // per-column scale slots (producer may run 4 tiles ahead of the epilogue)
 constexpr int TC_ABLK = 128 * 128;    // one [128 rows x 64 k] fp16 block, 128B-swizzled, 16 KB
 constexpr int TC_BBLK = TC_T * 128;   // one [64 rows x 64 k] fp16 block, 8 KB
-constexpr int TC_THREADS = 544;
-constexpr int TC_PROD_WARPS = 8, TC_EPI_WARPS = 8, TC_MMA_WARP = 16;
-constexpr int TC_TMEM_COLS = 256;     // 2 stages x (s: 64 + t: 64) fp32 columns
+constexpr int TC_THREADS = 512;
+constexpr int TC_PROD_WARPS = 8, TC_EPI_WARPS = 8;  // consumers are warps 0-7, producers warps 8-15
 
 struct TcParams {
   const float* x;
@@ -85,40 +83,32 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulators across the wgmma fence / wait
+__device__ __forceinline__ void wg_fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// D(64 x 64, fp32) (+)= A(64 x 16) · B(16 x 64), fp16 operands K-major in shared memory; `accumulate` = 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): K-major operand, 128-byte
-// swizzle, 8-row groups 1024 B apart: start>>4 | LBO(=1, unused)<<16 | SBO(1024>>4)<<32 | version 1<<46 | SW128(2)<<61
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// wgmma shared-memory matrix descriptor: K-major operand, 128-byte swizzle, 8-row groups 1024 B apart:
+// start>>4 | LBO(=1, unused for swizzled K-major)<<16 | SBO(1024>>4)<<32 | SW128(1)<<62
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// UMMA instruction descriptor (InstrDescriptor): D=f32 (1<<4), A=B=f16 (0), K-major both, N>>3 at bit 17, M>>4 at bit 24
-constexpr uint32_t TC_IDESC = (1u << 4) | ((uint32_t)(TC_T >> 3) << 17) | ((128u >> 4) << 24);
 
 // byte offset of the 8-byte group holding k' .. k'+3 of row `row` inside one 128B-swizzled [rows x 64] fp16 block
 __device__ __forceinline__ int sw128_off(int row, int kprime) {
@@ -184,9 +174,8 @@ __global__ void __launch_bounds__(1024) coupling_prep_kernel(const float* __rest
 // Template parameters: LD > 0 = compile-time leading dimension of BOTH x and y (the dense D = 256 batches of the
 // BASELINE configuration: every per-column address becomes an immediate offset), 0 = run-time strides; FOLD = a
 // neighbouring BatchNorm is folded in (per-row affine before / after); INV = inverse law.
-// Round-2 rewrite of the producer / epilogue loops: the round-1 kernel executed ~150 instructions per x₂ column and ~44
-// per x₁ element (64-bit address products, per-column bounds tests and clamps, run-time mode flags, register spills)
-// and was issue / instruction-cache bound at 46 % of the HBM roofline.  This kernel only ever sees WHOLE tiles (the
+// Per-column bounds tests, clamps, 64-bit address products and run-time mode flags make a kernel like this one issue /
+// instruction-cache bound, so this kernel only ever sees WHOLE tiles (the
 // launcher hands the < 64 ragged columns at the end of a batch to the exact-fp32 kernel), so there is no bounds logic
 // at all, and addresses are a per-tile pointer plus immediates.
 template <int LD, bool FOLD, bool INV>
@@ -200,73 +189,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) coupling_tc_kernel(const __grid
   unsigned char* sB = base + a_bytes;
   float* colscale = reinterpret_cast<float*>(sB + TC_STAGES * b_stage);   // [TC_SCALE_SLOTS][TC_T]
   uint64_t* bars = reinterpret_cast<uint64_t*>(colscale + TC_SCALE_SLOTS * TC_T);
-  // bars: [0..1] b_full, [2..3] b_empty, [4..5] acc_full, [6..7] acc_empty, [8] w_ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
+  // bars: [0..1] b_full, [2..3] b_empty, [4] w_ready
   const long long ldx = LD ? LD : P.ldx, ldy = LD ? LD : P.ldy;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
       bar_init(sm_u32(&bars[0 + s]), TC_PROD_WARPS);
-      bar_init(sm_u32(&bars[2 + s]), 1);  // tcgen05.commit
+      bar_init(sm_u32(&bars[2 + s]), TC_EPI_WARPS);  // every consumer warp, once its MMAs have read the stage
     }
-    for (int a = 0; a < TC_ACC; ++a) {
-      bar_init(sm_u32(&bars[4 + a]), 1);  // tcgen05.commit
-      bar_init(sm_u32(&bars[6 + a]), TC_EPI_WARPS);
-    }
-    bar_init(sm_u32(&bars[8]), 1);
+    bar_init(sm_u32(&bars[4]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == TC_MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sm_u32(tmem_slot)),
-                 "r"((uint32_t)TC_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const long long my_tiles = (P.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
 
-  if (warp == TC_MMA_WARP) {
-    // ================================ MMA issuer ================================
-    if (lane == 0) {
-      const uint32_t wbar = sm_u32(&bars[8]);
-      bar_expect_tx(wbar, (uint32_t)a_bytes);
-      for (int off = 0; off < a_bytes; off += TC_ABLK) bulk_g2s(sm_u32(sA + off), P.wimg + off, TC_ABLK, wbar);
-      bar_wait(wbar, 0);
-      for (long long i = 0; i < my_tiles; ++i) {
-        const int s = (int)(i & 1), a = (int)(i & 1);
-        const uint32_t ph = (uint32_t)((i >> 1) & 1);
-        bar_wait(sm_u32(&bars[0 + s]), ph);      // x₂ operand stage filled
-        bar_wait(sm_u32(&bars[6 + a]), ph ^ 1);  // accumulator stage drained by the epilogue
-        tc_fence_after();
-        const uint32_t bB = sm_u32(sB + s * b_stage);
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          const uint32_t d_tmem = tmem_base + (uint32_t)(a * 2 * TC_T + mt * TC_T);
-          uint32_t acc = 0;
-          // smallest terms first: lo·hi, hi·lo, hi·hi
-#pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {
-            const int pa = prod == 0 ? 1 : 0, pb = prod == 1 ? 1 : 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-              const uint32_t aaddr = sm_u32(sA) + (uint32_t)(((mt * 2 + pa) * nkb + kb) * TC_ABLK);
-              const uint32_t baddr = bB + (uint32_t)((pb * nkb + kb) * TC_BBLK);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {  // 4 K-steps of 16 fp16 (32 B) inside the 128-byte swizzle atom
-                tc_mma_f16(d_tmem, umma_desc_k_sw128(aaddr + 32 * j), umma_desc_k_sw128(baddr + 32 * j), TC_IDESC, acc);
-                acc = 1;
-              }
-            }
-          }
-        }
-        tc_commit(sm_u32(&bars[2 + s]));  // operand stage may be refilled
-        tc_commit(sm_u32(&bars[4 + a]));  // accumulators ready for the epilogue
-      }
-    }
-  } else if (warp >= TC_EPI_WARPS) {
+  if (warp >= TC_EPI_WARPS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 112;" ::: "memory");  // registers go to the consumers
     // ================================ producers ================================
     // Warp p converts columns [8p, 8p+8) of every tile.  Lane l holds the float4 #l of a column (rows
     // row2+4l..+3).  The per-column maximum (operand scale) is ONE redux.sync on the float bit patterns (monotonic
@@ -398,101 +337,107 @@ __global__ void __launch_bounds__(TC_THREADS, 1) coupling_tc_kernel(const __grid
       if (write_y2) yt += tstride * ldy;
     }
   } else {
-    // ================================ epilogue ================================
-    // Thread = TMEM lane = row j of s / t; warp w covers rows 32·(w%4)..+31 and columns 32·(w/4)..+31 of the tile
-    // as two chunks of 16 columns.  x₁ of the row is prefetched ONE tile ahead (buffers A/B = the two chunks).
-    const int j = (warp & 3) * 32 + lane;
-    const int chalf = warp >> 2;  // which 32-column half of the tile
-    const bool rowok = j < P.n1;
-    const int jr = rowok ? j : 0;  // clamp: loads stay in bounds, stores are predicated
-    const float cs_j = (rowok && P.cvec) ? P.cvec[j] : 0.f;
-    const float ct_j = (rowok && P.cvec) ? P.cvec[P.n1 + j] : 0.f;
-    float preA_j = 1.f, preC_j = 0.f, postA_j = 1.f, postC_j = 0.f;
-    if (FOLD && rowok) {
-      preA_j = P.fold[P.row1 + j];
-      preC_j = P.fold[P.D + P.row1 + j];
-      postA_j = P.fold[2 * P.D + P.row1 + j];
-      postC_j = P.fold[3 * P.D + P.row1 + j];
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 144;" ::: "memory");  // 64 accumulators + 32 x₁ values per thread
+    // ================================ consumers ================================
+    // Warpgroup g owns rows 64g..64g+63 of s and of t.  In the m64n64 accumulator layout, thread (warp w, lane l) of
+    // the warpgroup holds rows j0 = 64g + 16(w%4) + l/4 and j0 + 8, columns 8i + 2(l%4) + {0, 1} (i = 0..7):
+    // slot 4i + 2h + e is (row j0 + 8h, column 8i + 2(l%4) + e), identically for s and t.
+    const int g = warp >> 2;
+    const int j0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);  // first of this thread's two columns in every group of 8
+    float cs_j[2], ct_j[2], preA_j[2], preC_j[2], postA_j[2], postC_j[2];
+    bool store_j[2];
+    int jr[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = j0 + 8 * h;
+      const bool rowok = j < P.n1;
+      jr[h] = rowok ? j : 0;  // clamp: loads stay in bounds, stores are predicated
+      store_j[h] = P.y != nullptr && rowok;
+      cs_j[h] = (rowok && P.cvec) ? P.cvec[j] : 0.f;
+      ct_j[h] = (rowok && P.cvec) ? P.cvec[P.n1 + j] : 0.f;
+      preA_j[h] = 1.f, preC_j[h] = 0.f, postA_j[h] = 1.f, postC_j[h] = 0.f;
+      if (FOLD && rowok) {
+        preA_j[h] = P.fold[P.row1 + j];
+        preC_j[h] = P.fold[P.D + P.row1 + j];
+        postA_j[h] = P.fold[2 * P.D + P.row1 + j];
+        postC_j[h] = P.fold[3 * P.D + P.row1 + j];
+      }
     }
-    const bool do_store = P.y != nullptr && rowok;
     const long long tstride = (long long)gridDim.x * TC_T;
-    long long c0 = (long long)blockIdx.x * TC_T + chalf * 32;  // first column of this warp in the current tile
-    const float* xr = P.x + P.row1 + jr + c0 * ldx;
-    float* yr = P.y ? P.y + P.row1 + jr + c0 * ldy : nullptr;
-    auto load_chunk = [&](float (&buf)[16], const float* src) {
-#pragma unroll
-      for (int n = 0; n < 16; ++n) buf[n] = __ldcs(src + n * ldx);
-    };
-    float xa[16], xb[16];
-#pragma unroll
-    for (int n = 0; n < 16; ++n) xa[n] = xb[n] = 0.f;
-    if (my_tiles > 0) {
-      load_chunk(xa, xr);
-      load_chunk(xb, xr + 16 * ldx);
+    const float* xr = P.x + P.row1 + (long long)blockIdx.x * TC_T * ldx + cq * ldx;
+    float* yr = P.y ? P.y + P.row1 + (long long)blockIdx.x * TC_T * ldy + cq * ldy : nullptr;
+    const uint32_t wbar = sm_u32(&bars[4]);
+    if (threadIdx.x == 0) {
+      bar_expect_tx(wbar, (uint32_t)a_bytes);
+      for (int off = 0; off < a_bytes; off += TC_ABLK) bulk_g2s(sm_u32(sA + off), P.wimg + off, TC_ABLK, wbar);
     }
+    bar_wait(wbar, 0);
+    const uint32_t aW = sm_u32(sA) + (uint32_t)(g * 64 * 128);  // rows 64g.. of a 128-row block: 8 swizzle atoms in
+
     for (long long i = 0; i < my_tiles; ++i) {
-      const int a = (int)(i & 1);
+      const int s = (int)(i & 1);
       const uint32_t ph = (uint32_t)((i >> 1) & 1);
-      const float* cs = colscale + (int)(i & (TC_SCALE_SLOTS - 1)) * TC_T + chalf * 32;
-      const bool more = i + 1 < my_tiles;
-      bar_wait(sm_u32(&bars[4 + a]), ph);
-      tc_fence_after();
-      const uint32_t t_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(a * 2 * TC_T + chalf * 32);
-      auto finish = [&](const uint32_t (&rs)[16], const uint32_t (&rt)[16], float (&xbuf)[16], int chl) {
-        float outv[16];
+      // x₁ of this tile: requested first, in flight while the stage fills and the MMAs run
+      float xv[32];
 #pragma unroll
-        for (int n4 = 0; n4 < 4; ++n4) {
-          const float4 f4 = *reinterpret_cast<const float4*>(cs + chl * 16 + n4 * 4);
-          const float ff[4] = {f4.x, f4.y, f4.z, f4.w};
+      for (int q = 0; q < 8; ++q)
 #pragma unroll
-          for (int m = 0; m < 4; ++m) {
-            const int n = n4 * 4 + m;
-            const float sv = fmaf(__uint_as_float(rs[n]), ff[m], cs_j);
-            const float tv = fmaf(__uint_as_float(rt[n]), ff[m], ct_j);
-            const float xv = FOLD ? fmaf(xbuf[n], preA_j, preC_j) : xbuf[n];
-            float out;
-            if (!INV) out = fmaf(__expf(sv), xv, tv);  // exp(s)·x₁ + t  (scale.jl:13, shift.jl:14)
-            else out = (xv - tv) * __expf(-sv);         // inv.(a) .* (y₁ + (−t))  (scale.jl:16, shift.jl:12)
-            outv[n] = FOLD ? fmaf(out, postA_j, postC_j) : out;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) xv[4 * q + 2 * h + e] = __ldcs(xr + (8 * q + e) * ldx + jr[h]);
+      float accs[32], acct[32];
+      bar_wait(sm_u32(&bars[0 + s]), ph);  // x₂ operand stage filled
+      const uint32_t bB = sm_u32(sB + s * b_stage);
+      wg_fence_acc(accs);
+      wg_fence_acc(acct);
+      wg_fence();
+      // smallest terms first: lo·hi, hi·lo, hi·hi
+#pragma unroll
+      for (int prod = 0; prod < 3; ++prod) {
+        const int pa = prod == 0 ? 1 : 0, pb = prod == 1 ? 1 : 0;
+        for (int kb = 0; kb < nkb; ++kb) {  // nkb is left rolled: unrolled, the chain spills in every variant
+          const uint32_t as = aW + (uint32_t)(((0 * 2 + pa) * nkb + kb) * TC_ABLK);
+          const uint32_t at = aW + (uint32_t)(((1 * 2 + pa) * nkb + kb) * TC_ABLK);
+          const uint32_t baddr = bB + (uint32_t)((pb * nkb + kb) * TC_BBLK);
+          const uint32_t first = prod == 0 && kb == 0;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {  // 4 K-steps of 16 fp16 (32 B) inside the 128-byte swizzle atom
+            const uint64_t bd = gmma_desc_k_sw128(baddr + 32 * j);
+            wgmma_m64n64k16(accs, gmma_desc_k_sw128(as + 32 * j), bd, first && j == 0 ? 0u : 1u);
+            wgmma_m64n64k16(acct, gmma_desc_k_sw128(at + 32 * j), bd, first && j == 0 ? 0u : 1u);
           }
         }
-        // refill this buffer with the same chunk of the next tile
-        if (more) load_chunk(xbuf, xr + (tstride + chl * 16) * ldx);
-        if (do_store) {
-          float* dst = yr + chl * 16 * ldy;
-#pragma unroll
-          for (int n = 0; n < 16; ++n) __stcs(dst + n * ldy, outv[n]);
-        }
-      };
-      {
-        uint32_t rs[16], rt[16];
-        tc_ld16(t_lane, rs);
-        tc_ld16(t_lane + TC_T, rt);
-        tc_wait_ld();
-        finish(rs, rt, xa, 0);
       }
-      {
-        uint32_t rs[16], rt[16];
-        tc_ld16(t_lane + 16, rs);
-        tc_ld16(t_lane + TC_T + 16, rt);
-        tc_wait_ld();
-        finish(rs, rt, xb, 1);
-      }
-      tc_fence_before();
+      wg_commit();
+      wg_wait0();
+      wg_fence_acc(accs);
+      wg_fence_acc(acct);
       __syncwarp();
-      if (lane == 0) bar_arrive(sm_u32(&bars[6 + a]));
-      c0 += tstride;
+      if (lane == 0) bar_arrive(sm_u32(&bars[2 + s]));  // operand stage may be refilled
+
+      const float* cs = colscale + (int)(i & (TC_SCALE_SLOTS - 1)) * TC_T + cq;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float2 f2 = *reinterpret_cast<const float2*>(cs + 8 * q);
+        const float ff[2] = {f2.x, f2.y};
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = 4 * q + 2 * h + e;
+            const float sv = fmaf(accs[n], ff[e], cs_j[h]);
+            const float tv = fmaf(acct[n], ff[e], ct_j[h]);
+            const float x1 = FOLD ? fmaf(xv[n], preA_j[h], preC_j[h]) : xv[n];
+            float out;
+            if (!INV) out = fmaf(__expf(sv), x1, tv);  // exp(s)·x₁ + t  (scale.jl:13, shift.jl:14)
+            else out = (x1 - tv) * __expf(-sv);         // inv.(a) .* (y₁ + (−t))  (scale.jl:16, shift.jl:12)
+            if (store_j[h]) __stcs(yr + (8 * q + e) * ldy + jr[h], FOLD ? fmaf(out, postA_j[h], postC_j[h]) : out);
+          }
+      }
       xr += tstride * ldx;
       if (yr) yr += tstride * ldy;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == TC_MMA_WARP) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TC_TMEM_COLS)
-                 : "memory");
   }
 }
 
@@ -547,22 +492,22 @@ int b2b_launch_coupling_affine_tc(const b2b_layer_desc& d, const float* fold, co
   P.fold = fold;
   P.cvec = d.p1;
   P.N = N;
+  P.nkb = nkb;
   P.ldx = ldx;
   P.ldy = ldy;
   P.tiles = N / TC_T;
   P.D = D;
   P.n1 = n1;
   P.n2 = n2;
-  P.nkb = nkb;
   P.row1 = row1;
   P.row2 = row2;
   P.accumulate = accumulate;
   P.inverse = d.inverse;
   const size_t smem = (size_t)4 * nkb * TC_ABLK + (size_t)TC_STAGES * 2 * nkb * TC_BBLK +
-                      TC_SCALE_SLOTS * TC_T * sizeof(float) + 16 * sizeof(uint64_t) + 1024;
-  typedef void (*kernel_t)(const TcParams);
+                      TC_SCALE_SLOTS * TC_T * sizeof(float) + 8 * sizeof(uint64_t) + 1024;
   const bool dense256 = ldx == 256 && (!y || ldy == 256);
   const bool inv = d.inverse != 0, fd = fold != nullptr;
+  typedef void (*kernel_t)(const TcParams);
   kernel_t kernel;
   if (dense256) {
     kernel = fd ? (inv ? coupling_tc_kernel<256, true, true> : coupling_tc_kernel<256, true, false>)

@@ -13,8 +13,8 @@
 // exact fp32 on the CUDA cores: a persistent CTA per SM, tiles of 32 columns transposed into shared memory, the CTA's
 // partial W̄ (2·n1 x n2 <= 256 x 128 floats) lives in REGISTERS for the whole launch (128 accumulators per thread) and is
 // written once; a second kernel sums the per-CTA partials in a fixed order (deterministic).  Two programs: the generic one
-// below (any n1, n2 <= 128, scalar loads) and the float4 / FFMA2 one for n1, n2 multiples of 4.  The tensor-core (fp16-split
-// tcgen05) form of the forward kernel has not been carried over to the reverse mode (DESIGN §8).
+// below (any n1, n2 <= 128, scalar loads) and the float4 / float2-pair one for n1, n2 multiples of 4.  The tensor-core (fp16-split
+// wgmma) form of the forward kernel has not been carried over to the reverse mode (DESIGN §8).
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -178,13 +178,12 @@ __global__ void __launch_bounds__(CV_THREADS, 1) coupling_vjp_kernel(const __gri
 //   [s; t]   thread = 4 s rows + the matching 4 t rows x 4 columns: per k two float4 of W (L1) + one float4 of x₂ -> 32 FMA
 //   x̄₂       thread = 4 rows of x₂ x 4 columns: per 4 j four float4 of W + four float4 of [s̄; t̄]              -> 64 FMA
 //   W̄        warp = 32 rows of [s̄; t̄], lane = 4 rows of x₂: per 4 columns 32 broadcast float4 + 4 float4     -> 512 FMA
-// and every FMA is one half of a packed FFMA2 (row pairs of W / of [s̄; t̄] against a broadcast scalar, or even/odd-j
-// partial sums), which halves the issue slots the arithmetic takes.
+// and every FMA is one half of a float2-pair b2b_ffma2 (row pairs of W / of [s̄; t̄] against a broadcast scalar, or even/odd-j
+// partial sums).
 // The tiles are 32 floats wide with the 16-byte chunks XOR-swizzled by the row (chunk ^ (row & 7)) instead of padded:
 // conflict-free for the row-wise float4 reads, the lane-per-row reads of the W̄ product and the transposing stores alike,
 // and the CTA stays under 100 KB of shared memory -- which leaves 156 KB of L1 for W (128 KB at n1 = n2 = 128), read
-// through L1 by every tile.  Measured (ncu, D = 256, N = 2^19): 3.5 ms, three quarters of W's sectors hit L1, the rest
-// (L2 latency, two warps per scheduler) is what `long_scoreboard` shows; streaming W through shared memory with bulk
+// through L1 by every tile; streaming W through shared memory with bulk
 // copies was tried and was slower.
 constexpr int CF_LD = CV_TC;
 
@@ -215,7 +214,7 @@ __device__ __forceinline__ int cf_chunk(int r, int ch) { return r * CF_LD + ((ch
 __device__ __forceinline__ int cf_elem(int r, int c) { return r * CF_LD + ((((c >> 2) ^ (r & 7)) << 2) | (c & 3)); }
 
 // [s̄; t̄] tile: rows stored in interleaved PAIRS -- a 16-byte chunk holds {row 2p, row 2p+1} x {col 2h, col 2h+1} -- so that
-// a float4 is two packed-FFMA2 operands (row pairs against a broadcast scalar).  Chunk h of pair p sits at h ^ (h >> 3).
+// a float4 is two b2b_ffma2 operands (row pairs against a broadcast scalar).  Chunk h of pair p sits at h ^ (h >> 3).
 __device__ __forceinline__ int sb_chunk(int p, int h) { return p * 64 + ((h ^ (h >> 3)) << 2); }
 __device__ __forceinline__ int sb_elem(int row, int col) { return sb_chunk(row >> 1, col >> 1) + ((col & 1) << 1) + (row & 1); }
 __device__ __forceinline__ float2 bc2(float v) { return make_float2(v, v); }
@@ -294,10 +293,10 @@ __global__ void __launch_bounds__(CV_THREADS, 1) coupling_vjp_fast_kernel(const 
         const float xq[4] = {xv.x, xv.y, xv.z, xv.w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          sv[0][q] = __ffma2_rn(ws0, bc2(xq[q]), sv[0][q]);
-          sv[1][q] = __ffma2_rn(ws1, bc2(xq[q]), sv[1][q]);
-          tv[0][q] = __ffma2_rn(wt0, bc2(xq[q]), tv[0][q]);
-          tv[1][q] = __ffma2_rn(wt1, bc2(xq[q]), tv[1][q]);
+          sv[0][q] = b2b_ffma2(ws0, bc2(xq[q]), sv[0][q]);
+          sv[1][q] = b2b_ffma2(ws1, bc2(xq[q]), sv[1][q]);
+          tv[0][q] = b2b_ffma2(wt0, bc2(xq[q]), tv[0][q]);
+          tv[1][q] = b2b_ffma2(wt1, bc2(xq[q]), tv[1][q]);
         }
       }
     }
@@ -377,14 +376,14 @@ __global__ void __launch_bounds__(CV_THREADS, 1) coupling_vjp_fast_kernel(const 
         for (int i = 0; i < 4; ++i) {
           const float4 w = ld4g(wr[i] + j);
           const float2 w0 = make_float2(w.x, w.y), w1 = make_float2(w.z, w.w);
-          a[i][0] = __ffma2_rn(w0, make_float2(p00.x, p00.y), a[i][0]);
-          a[i][1] = __ffma2_rn(w0, make_float2(p00.z, p00.w), a[i][1]);
-          a[i][2] = __ffma2_rn(w0, make_float2(p01.x, p01.y), a[i][2]);
-          a[i][3] = __ffma2_rn(w0, make_float2(p01.z, p01.w), a[i][3]);
-          a[i][0] = __ffma2_rn(w1, make_float2(p10.x, p10.y), a[i][0]);
-          a[i][1] = __ffma2_rn(w1, make_float2(p10.z, p10.w), a[i][1]);
-          a[i][2] = __ffma2_rn(w1, make_float2(p11.x, p11.y), a[i][2]);
-          a[i][3] = __ffma2_rn(w1, make_float2(p11.z, p11.w), a[i][3]);
+          a[i][0] = b2b_ffma2(w0, make_float2(p00.x, p00.y), a[i][0]);
+          a[i][1] = b2b_ffma2(w0, make_float2(p00.z, p00.w), a[i][1]);
+          a[i][2] = b2b_ffma2(w0, make_float2(p01.x, p01.y), a[i][2]);
+          a[i][3] = b2b_ffma2(w0, make_float2(p01.z, p01.w), a[i][3]);
+          a[i][0] = b2b_ffma2(w1, make_float2(p10.x, p10.y), a[i][0]);
+          a[i][1] = b2b_ffma2(w1, make_float2(p10.z, p10.w), a[i][1]);
+          a[i][2] = b2b_ffma2(w1, make_float2(p11.x, p11.y), a[i][2]);
+          a[i][3] = b2b_ffma2(w1, make_float2(p11.z, p11.w), a[i][3]);
         }
       }
 #pragma unroll
@@ -420,10 +419,10 @@ __global__ void __launch_bounds__(CV_THREADS, 1) coupling_vjp_fast_kernel(const 
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
               float2 t = acc[ip][q];
-              t = __ffma2_rn(make_float2(a0.x, a0.y), bc2(bq[q].x), t);
-              t = __ffma2_rn(make_float2(a0.z, a0.w), bc2(bq[q].y), t);
-              t = __ffma2_rn(make_float2(a1.x, a1.y), bc2(bq[q].z), t);
-              t = __ffma2_rn(make_float2(a1.z, a1.w), bc2(bq[q].w), t);
+              t = b2b_ffma2(make_float2(a0.x, a0.y), bc2(bq[q].x), t);
+              t = b2b_ffma2(make_float2(a0.z, a0.w), bc2(bq[q].y), t);
+              t = b2b_ffma2(make_float2(a1.x, a1.y), bc2(bq[q].z), t);
+              t = b2b_ffma2(make_float2(a1.z, a1.w), bc2(bq[q].w), t);
               acc[ip][q] = t;
             }
           }
@@ -591,7 +590,7 @@ static int sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 148;
+  return sms > 0 ? sms : 132;
 }
 
 }  // namespace b2b

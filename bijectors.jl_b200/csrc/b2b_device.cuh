@@ -123,7 +123,7 @@ __device__ inline void planar_table_piece(float c, int i, float* tab) {
 }
 
 // the safeguarded iteration as an out-of-line call: the unrolled 8-layer program would otherwise carry eight inlined
-// copies of a loop it almost never runs (ncu: 96 KB of SASS, no_instruction 0.72 warps/issue -- instruction-cache misses)
+// copies of a loop it almost never runs and become instruction-cache bound
 static __device__ __noinline__ float find_alpha_ts_call(float t, float c, float b, float* th, float* s2) {
   float th_, s2_;
   const float x = find_alpha_ts(t, c, b, th_, s2_);
@@ -327,8 +327,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // RQS tables staged by ALL threads of the CTA, one (row, knot) pair per thread: the per-warp version below walks the
-// KP knots of a row serially (KP x ~8 dependent-latency global loads and two divisions: ~15 us, a fifth of the
-// RQS kernel's run time with the other warps idle at the barrier).  Same table layout as stage_layer(B2B_RQS).
+// KP knots of a row serially (KP x ~8 dependent-latency global loads and two divisions, with the other warps
+// idle at the barrier).  Same table layout as stage_layer(B2B_RQS).
 __device__ inline void stage_rqs_cta(const b2b_layer_desc& d, float* sm, int D, int Dp, int tid, int nthreads) {
   const int K1 = d.n0, KP = rqs_kp(K1);
   float* Sw = sm;

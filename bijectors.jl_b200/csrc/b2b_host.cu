@@ -90,7 +90,7 @@ extern "C" int b2b_host_ctx_destroy(b2b_host_ctx* c) {
 // ---------------------------------------------------------------------------------------------------
 // NUMA placement of the calling thread next to a GPU.  On the 2-socket HGX hosts every GPU hangs off one socket's PCIe
 // root complexes; a pinned host buffer that lives on the OTHER socket makes every H2D / D2H copy cross the inter-socket
-// link, which is what capped the 8-rank host-buffer throughput in round 1 (SCALE_r01: 0.24 efficiency).  This binds the
+// link, which caps the host-buffer throughput when several ranks share a box.  This binds the
 // calling thread (CPU affinity + preferred memory node) to the NUMA node of `device`, so that pinned buffers allocated
 // afterwards (cudaHostAlloc / torch pin_memory from this thread) and the host ctx's staging land on the local node.
 // Linux only; every step is best effort (returns B2B_OK with *node_out = -1 when the topology is not exposed).

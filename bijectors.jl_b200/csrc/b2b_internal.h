@@ -18,6 +18,20 @@ struct B2BChainParams {
   b2b_layer_desc layers[B2B_MAX_CHAIN];
 };
 
+#ifdef __CUDACC__
+// Element-wise float2 arithmetic of the paired-column kernels.  sm_90 has no packed FP32 instruction, so each is two
+// scalar operations; the _rn intrinsics keep every product and sum individually rounded (no contraction).
+__device__ __forceinline__ float2 b2b_ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 b2b_fadd2(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 b2b_fmul2(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+#endif
+
 // number of floats of staged (derived) parameters a layer needs for padded depth Dp
 static inline int b2b_layer_smem_floats(const b2b_layer_desc& d, int Dp) {
   switch (d.kind) {

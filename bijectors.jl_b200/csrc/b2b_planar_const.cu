@@ -1,17 +1,17 @@
 // Chains of <= 8 PlanarLayers as ONE UNROLLED program on the TMA pipeline (b2b_v1_pipeline.cuh).
 //
-// Why: the layer interpreter (b2b_chain_v1.cu) runs the 8-layer D = 128 headline chain at 72 % of the HBM roofline
-// (rolled layer loop, switch on the layer kind, generic fragment mapping).  Specialising the program on (D, L,
-// direction) and unrolling the layers reaches 85-89 %.  Parameter operands:
+// Why: the layer interpreter (b2b_chain_v1.cu) pays for a rolled layer loop, a switch on the layer kind and a generic
+// fragment mapping on the 8-layer D = 128 headline chain; specialising the program on (D, L, direction) and unrolling
+// the layers removes that overhead.  Parameter operands:
 //   device-resident parameters (DevSrc, every b2b_chain_run_f32 segment made of PlanarLayers): each CTA derives û /
 //       wᵀû in its prologue into shared memory and all operands are warp-uniform LDS broadcasts -- one launch, no
 //       library-owned device state;
 //   host-resident parameters (ArgSrc, b2b_planar_chain_hostparams_f32): derived on the host, passed BY VALUE as kernel
-//       arguments, i.e. CONSTANT-BANK operands (LDCU -> uniform register -> FFMA2: no LSU work).  The first-level
+//       arguments, i.e. CONSTANT-BANK operands (LDC -> FFMA operand: no LSU work).  The first-level
 //       constant cache holds ~4 KB, so the 8 KB of an 8-layer D = 128 chain is split: w in shared memory, û in the
-//       constant bank (MODE 2).  This is the fastest form (88-89 %).
-// A __constant__ slot filled per call from device parameters (prep kernel + copy) was measured too: the extra
-// launch + copy-engine hop costs 13 us per call, more than constant operands gain over shared-memory ones at D >= 64.
+//       constant bank (MODE 2).
+// A __constant__ slot filled per call from device parameters (prep kernel + copy) is not used: the extra
+// launch + copy-engine hop costs more per call than constant operands gain over shared-memory ones at D >= 64.
 //
 // Reference semantics: planar_layer.jl:65-80 (get_u_hat, forward), :102-110 (logabsdetjac), :112-127 + :160-185
 // (inverse through find_alpha).
@@ -45,8 +45,8 @@ struct ArgSrc {
 // Device-resident parameters: the kernel derives û / wᵀû itself (get_u_hat, planar_layer.jl:65-70, one warp per layer
 // in the prologue of every CTA) into shared memory and runs the unrolled program on the shared-memory copy -- one
 // launch, no library-owned device state.  (Measured: for the unrolled program the shared-memory operands are as fast
-// as the constant-bank ones at D >= 64 -- 85 % vs 86 % of the roofline at D = 128 -- and a separate preparation
-// kernel + copy into a __constant__ slot costs 13 us per call, more than it gains.)
+// as the constant-bank ones at D >= 64, and a separate preparation
+// kernel + copy into a __constant__ slot costs more per call than it gains.)
 template <int D, int L>
 struct DevSrc {
   static constexpr bool kDerive = true;
@@ -98,10 +98,10 @@ struct PlanarConstProg {
         float4 w;
         if constexpr (WS) w = w4[i];
         else w = make_float4(src.w(l, 4 * i), src.w(l, 4 * i + 1), src.w(l, 4 * i + 2), src.w(l, 4 * i + 3));
-        acc[(i & 1) * 2 + 0] = __ffma2_rn(make_float2(w.x, w.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
-        acc[(i & 1) * 2 + 1] = __ffma2_rn(make_float2(w.z, w.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
+        acc[(i & 1) * 2 + 0] = b2b_ffma2(make_float2(w.x, w.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
+        acc[(i & 1) * 2 + 1] = b2b_ffma2(make_float2(w.z, w.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
       }
-      const float2 s = __fadd2_rn(__fadd2_rn(acc[0], acc[1]), __fadd2_rn(acc[2], acc[3]));
+      const float2 s = b2b_fadd2(b2b_fadd2(acc[0], acc[1]), b2b_fadd2(acc[2], acc[3]));
       const float wz = s.x + s.y;  // aT_b(w, z), utils.jl:2
       float cc_, bb;
       if constexpr (SS) {
@@ -128,8 +128,8 @@ struct PlanarConstProg {
         float4 u;
         if constexpr (US) u = u4[i];
         else u = make_float4(src.uh(l, 4 * i), src.uh(l, 4 * i + 1), src.uh(l, 4 * i + 2), src.uh(l, 4 * i + 3));
-        x[0][2 * i] = __ffma2_rn(make_float2(u.x, u.y), t2, x[0][2 * i]);  // planar_layer.jl:78 / :124
-        x[0][2 * i + 1] = __ffma2_rn(make_float2(u.z, u.w), t2, x[0][2 * i + 1]);
+        x[0][2 * i] = b2b_ffma2(make_float2(u.x, u.y), t2, x[0][2 * i]);  // planar_layer.jl:78 / :124
+        x[0][2 * i + 1] = b2b_ffma2(make_float2(u.z, u.w), t2, x[0][2 * i + 1]);
       }
     }
   }

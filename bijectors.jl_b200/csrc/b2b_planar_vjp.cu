@@ -49,10 +49,10 @@ struct PlanarVjpProg {
 #pragma unroll
       for (int i = 0; i < D / 4; ++i) {
         const float4 w = w4[i];
-        acc[(i & 1) * 2 + 0] = __ffma2_rn(make_float2(w.x, w.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
-        acc[(i & 1) * 2 + 1] = __ffma2_rn(make_float2(w.z, w.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
+        acc[(i & 1) * 2 + 0] = b2b_ffma2(make_float2(w.x, w.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
+        acc[(i & 1) * 2 + 1] = b2b_ffma2(make_float2(w.z, w.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
       }
-      const float2 s = __fadd2_rn(__fadd2_rn(acc[0], acc[1]), __fadd2_rn(acc[2], acc[3]));
+      const float2 s = b2b_fadd2(b2b_fadd2(acc[0], acc[1]), b2b_fadd2(acc[2], acc[3]));
       const float cc_ = params[2 * L * D + l], bb = params[2 * L * D + L + l];
       if (DIR == 0) tanh_sech2(s.x + s.y + bb, st.t[l], st.s2[l]);
       else find_alpha_ts(s.x + s.y, cc_, bb, st.t[l], st.s2[l]);  // planar_layer.jl:121
@@ -62,8 +62,8 @@ struct PlanarVjpProg {
 #pragma unroll
         for (int i = 0; i < D / 4; ++i) {
           const float4 u = u4[i];
-          x[0][2 * i] = __ffma2_rn(make_float2(u.x, u.y), t2, x[0][2 * i]);
-          x[0][2 * i + 1] = __ffma2_rn(make_float2(u.z, u.w), t2, x[0][2 * i + 1]);
+          x[0][2 * i] = b2b_ffma2(make_float2(u.x, u.y), t2, x[0][2 * i]);
+          x[0][2 * i + 1] = b2b_ffma2(make_float2(u.z, u.w), t2, x[0][2 * i + 1]);
         }
       }
     }
@@ -82,10 +82,10 @@ struct PlanarVjpProg {
 #pragma unroll
       for (int i = 0; i < D / 4; ++i) {
         const float4 u = u4[i];
-        acc[(i & 1) * 2 + 0] = __ffma2_rn(make_float2(u.x, u.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
-        acc[(i & 1) * 2 + 1] = __ffma2_rn(make_float2(u.z, u.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
+        acc[(i & 1) * 2 + 0] = b2b_ffma2(make_float2(u.x, u.y), x[0][2 * i], acc[(i & 1) * 2 + 0]);
+        acc[(i & 1) * 2 + 1] = b2b_ffma2(make_float2(u.z, u.w), x[0][2 * i + 1], acc[(i & 1) * 2 + 1]);
       }
-      const float2 s = __fadd2_rn(__fadd2_rn(acc[0], acc[1]), __fadd2_rn(acc[2], acc[3]));
+      const float2 s = b2b_fadd2(b2b_fadd2(acc[0], acc[1]), b2b_fadd2(acc[2], acc[3]));
       const float d = s.x + s.y;  // û_lᵀ ȳ_{l+1}
       const float c = params[2 * L * D + l], s2 = st.s2[l], t = st.t[l];
       const float rden = __frcp_rn(fmaf(c, s2, 1.0f));
@@ -96,8 +96,8 @@ struct PlanarVjpProg {
 #pragma unroll
       for (int i = 0; i < D / 4; ++i) {
         const float4 w = w4[i];
-        x[0][2 * i] = __ffma2_rn(make_float2(w.x, w.y), g2, x[0][2 * i]);
-        x[0][2 * i + 1] = __ffma2_rn(make_float2(w.z, w.w), g2, x[0][2 * i + 1]);
+        x[0][2 * i] = b2b_ffma2(make_float2(w.x, w.y), g2, x[0][2 * i]);
+        x[0][2 * i + 1] = b2b_ffma2(make_float2(w.z, w.w), g2, x[0][2 * i + 1]);
       }
     }
     if (col < N) {
@@ -216,7 +216,7 @@ __global__ void __launch_bounds__(PG_THREADS)
 // K2 for dense batches (ld == D): chunks of PGB_CH columns of x, ȳ and the per-column scalars are contiguous in global
 // memory, so one elected thread streams them into a 4-stage shared-memory ring with three 1-D bulk copies per chunk
 // (cp.async.bulk + mbarrier full/empty pairs); the 8 warps consume from shared memory.  This keeps ~100 KB in flight
-// per SM -- the register-staged kernel above is bound by load latency (3 TB/s).
+// per SM -- the register-staged kernel above is bound by load latency.
 constexpr int PGB_CH = 16;      // columns per chunk
 constexpr int PGB_STAGES = 4;
 template <int D, int L>
@@ -589,7 +589,7 @@ int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long
   const HPShape sh = hp_shape(D, Lp);
   V1Geom g;
   static const int vjp_nw = getenv("B2B_VJP_NW") ? atoi(getenv("B2B_VJP_NW")) : 0;
-  // D = 128 x 8 layers: two-tensor slots are 32 KB; 7 warps leave room for 3 of them (8 warps: 2, 40 % slower)
+  // D = 128 x 8 layers: two-tensor slots are 32 KB; 7 warps leave room for 3 of them (8 warps: 2)
   const int nw = (D == 128 && Lp == 8) ? ((vjp_nw == 6 || vjp_nw == 8) ? vjp_nw : 7) : sh.nw;
   int rc = v1_geometry(D, p.N, nw, 32, (size_t)((2 * Lp * D + 2 * Lp + 3) & ~3), g, 2);
   if (rc != 0) return rc;

@@ -1,6 +1,6 @@
 // INVERSE chains of <= 8 RadialLayers as ONE UNROLLED program on the TMA pipeline, specialised on (D, L) -- the radial
-// counterpart of b2b_planar_const.cu (BASELINE config 3, inverse: 79 % -> 84 % of the roofline).  The forward direction
-// stays in the layer interpreter, which is faster there (87 % vs 80 %: the unrolled forward program spills at 12 warps).
+// counterpart of b2b_planar_const.cu (BASELINE config 3, inverse).  The forward direction stays in the layer
+// interpreter: an unrolled forward program of this shape spills at 12 warps.
 // Reference semantics: radial_layer.jl:43-72 (forward), :88-102,124-129 (inverse), see radial_apply.
 #include "b2b_v1_pipeline.cuh"
 

@@ -6,12 +6,11 @@
 // at the recovered point (interface.jl:276-281).
 //
 // Per element the work is a bin search plus ~25 flops, i.e. the layer is bound by instruction issue and by
-// shared-memory wavefronts, not by HBM.  What this program does about it (round-1 kernel: ~78 instructions and 17+
-// wavefronts per element, 36 % of the HBM roofline):
+// shared-memory wavefronts, not by HBM.  What this program does about it:
 //   * ONE 48-byte record per (row, bin): {w_k, 1/w | w, h_k, Δy | s}{d_k, d_k1}{probe knot, aux} -- one LDS.128 + one
 //     LDS.64 (6 wavefronts, the minimum for six lane-divergent numbers) fetch everything the element needs; with a
 //     48-byte stride the nine bins of a row start in nine different 16-byte bank groups, so the lane-divergent fetch is
-//     conflict-free (the 32-byte stride of round 1 was 2-3-way conflicted);
+//     conflict-free (a 32-byte stride is 2-3-way conflicted);
 //   * the bin search walks the K - 1 INTERIOR knots only (log2(K) dependent probes instead of log2(2K)), the probes live
 //     in the records themselves so the running bin index IS the byte offset of the record (no index -> address
 //     arithmetic, no clamp), and the first knot is compared separately (only raw three-argument-constructor knots can
@@ -92,7 +91,7 @@ __device__ inline void stage_rqs_records(const b2b_layer_desc& d, float* sm, int
 // Shared-memory loads by 32-bit shared-space address: the running record offset is then ONE register that the search
 // updates with predicated adds and every load uses directly (generic addressing cost an extra three-input add per
 // dependent probe and a select + add per step).  NOT volatile: volatile asm statements keep their program order, which
-// serialises the 32 elements of a column (measured: 48 % instead of 57 % of the roofline).
+// serialises the 32 elements of a column.
 __device__ __forceinline__ float lds_f32(uint32_t a) {
   float v;
   asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));

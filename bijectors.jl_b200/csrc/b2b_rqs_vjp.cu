@@ -274,7 +274,7 @@ static RqvShape rqv_shape(int K1, int D) {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   int per_sm = (int)((size_t)(227 * 1024) / (s.smem + 1024));
   if (per_sm > 3) per_sm = 3;  // 80 registers x 256 threads: three CTAs per SM
   if (per_sm < 1) per_sm = 1;

@@ -74,7 +74,7 @@ extern "C" int b2b_randn_f32(float* z, const float* mu, const float* sigma, uint
   V1Gen g{seed, offset, column_offset, mu, sigma};
   const long long total = N * ((D + 3) / 4);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   randn_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream_)>>>(z, g, D, N, ld);
   return (int)cudaGetLastError();
 }

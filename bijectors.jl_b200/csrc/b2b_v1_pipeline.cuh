@@ -93,7 +93,7 @@ struct V1Extra {
 };
 
 // Register layout of one thread: it owns rows [h*EPT, (h+1)*EPT) (h = part index, TPC parts per column) of CPT
-// columns, as float2 pairs so that the packed sm_100 FP32 pipe (FFMA2: two fp32 results per issue slot) does
+// columns, as float2 pairs (b2b_ffma2 and friends: two scalar fp32 operations each on sm_90) that do
 // the per-row work.  Every layer parameter that is loaded from shared memory is used for all CPT columns of the
 // thread: at D = 128 (TPC = 2, CPT = 2) that halves the LDS wavefronts per column, which is what bounds the
 // one-column-per-thread mapping.  Box ql (of NQT = EPT/32 boxes) slot r holds the LOGICAL 16-byte chunk r ^ rot
@@ -137,15 +137,15 @@ __device__ __forceinline__ void radial_apply(float2 (&x)[CPT][D / TPC / 2], cons
     const float4 z0 = z4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      const float2 d0 = __ffma2_rn(make_float2(z0.x, z0.y), m1, x[cc][i]);
-      const float2 d1 = __ffma2_rn(make_float2(z0.z, z0.w), m1, x[cc][i + 1]);
-      acc[cc][(r & 1) * 2 + 0] = __ffma2_rn(d0, d0, acc[cc][(r & 1) * 2 + 0]);
-      acc[cc][(r & 1) * 2 + 1] = __ffma2_rn(d1, d1, acc[cc][(r & 1) * 2 + 1]);
+      const float2 d0 = b2b_ffma2(make_float2(z0.x, z0.y), m1, x[cc][i]);
+      const float2 d1 = b2b_ffma2(make_float2(z0.z, z0.w), m1, x[cc][i + 1]);
+      acc[cc][(r & 1) * 2 + 0] = b2b_ffma2(d0, d0, acc[cc][(r & 1) * 2 + 0]);
+      acc[cc][(r & 1) * 2 + 1] = b2b_ffma2(d1, d1, acc[cc][(r & 1) * 2 + 1]);
     }
   }
   float2 g2[CPT];
   B2B_FOR_COLS {
-    const float2 s = __fadd2_rn(__fadd2_rn(acc[cc][0], acc[cc][1]), __fadd2_rn(acc[cc][2], acc[cc][3]));
+    const float2 s = b2b_fadd2(b2b_fadd2(acc[cc][0], acc[cc][1]), b2b_fadd2(acc[cc][2], acc[cc][3]));
     const float nrm = sqrtf(part_sum<TPC>(s.x + s.y));  // radial_layer.jl:49 / :125
     float r_ = nrm;
     if (inverse) {
@@ -170,10 +170,10 @@ __device__ __forceinline__ void radial_apply(float2 (&x)[CPT][D / TPC / 2], cons
     const float4 z0 = z4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      const float2 d0 = __ffma2_rn(make_float2(z0.x, z0.y), m1, x[cc][i]);
-      const float2 d1 = __ffma2_rn(make_float2(z0.z, z0.w), m1, x[cc][i + 1]);
-      x[cc][i] = __ffma2_rn(g2[cc], d0, x[cc][i]);
-      x[cc][i + 1] = __ffma2_rn(g2[cc], d1, x[cc][i + 1]);
+      const float2 d0 = b2b_ffma2(make_float2(z0.x, z0.y), m1, x[cc][i]);
+      const float2 d1 = b2b_ffma2(make_float2(z0.z, z0.w), m1, x[cc][i + 1]);
+      x[cc][i] = b2b_ffma2(g2[cc], d0, x[cc][i]);
+      x[cc][i + 1] = b2b_ffma2(g2[cc], d1, x[cc][i + 1]);
     }
   }
 }
@@ -193,14 +193,14 @@ __device__ __forceinline__ void mvnormal_apply(const float2 (&x)[CPT][D / TPC / 
     const float4 mu = mu4[c.prm(ql, r)], is = is4[c.prm(ql, r)];
     const int i = (ql * 8 + r) * 2;
     B2B_FOR_COLS {
-      const float2 z0 = __fmul2_rn(__ffma2_rn(make_float2(mu.x, mu.y), m1, x[cc][i]), make_float2(is.x, is.y));
-      const float2 z1 = __fmul2_rn(__ffma2_rn(make_float2(mu.z, mu.w), m1, x[cc][i + 1]), make_float2(is.z, is.w));
-      acc[cc][0] = __ffma2_rn(z0, z0, acc[cc][0]);
-      acc[cc][1] = __ffma2_rn(z1, z1, acc[cc][1]);
+      const float2 z0 = b2b_fmul2(b2b_ffma2(make_float2(mu.x, mu.y), m1, x[cc][i]), make_float2(is.x, is.y));
+      const float2 z1 = b2b_fmul2(b2b_ffma2(make_float2(mu.z, mu.w), m1, x[cc][i + 1]), make_float2(is.z, is.w));
+      acc[cc][0] = b2b_ffma2(z0, z0, acc[cc][0]);
+      acc[cc][1] = b2b_ffma2(z1, z1, acc[cc][1]);
     }
   }
   B2B_FOR_COLS {
-    const float2 s = __fadd2_rn(acc[cc][0], acc[cc][1]);
+    const float2 s = b2b_fadd2(acc[cc][0], acc[cc][1]);
     lj[cc] += sp[2 * D] - 0.5f * part_sum<TPC>(s.x + s.y);
   }
 }
@@ -241,8 +241,8 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t
 __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
   const float u1 = fmaf(__uint2float_rn(a), 2.3283064365386963e-10f, 1.1641532182693481e-10f);
   const float u2 = fmaf(__uint2float_rn(b), 2.3283064365386963e-10f, 1.1641532182693481e-10f);
-  // special-function-unit forms (lg2, sqrt, sin, cos: one MUFU each): the library-accurate logf / sincospif made the
-  // generator 2.5x slower than the chain it feeds; their absolute error (~2^-21) is far below the 1e-5 parity bar
+  // special-function-unit forms (lg2, sqrt, sin, cos: one MUFU each): the library-accurate logf / sincospif cost several
+  // times the instructions; their absolute error (~2^-21) is far below the 1e-5 parity bar
   const float r = sqrtf(-1.3862943611198906f * __log2f(u1));  // sqrt(−2·ln u1)
   const float ang = 6.283185307179586f * u2 - 3.141592653589793f;  // 2π·u2 − π in (−π, π]: the accurate range of MUFU.SIN/COS
   z0 = -r * __cosf(ang);                                            // cos(2π u2) = −cos(2π u2 − π)
@@ -314,8 +314,7 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
   };
   // tiles of this CTA: global tile id = blockIdx.x + j * gridDim.x
   const long long my_tiles = (E.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
-  // The first P tile loads are issued BEFORE the parameters are staged: the DRAM latency of the first tiles (and, for
-  // the 20-60 us kernels, a visible share of the run time) overlaps the prologue arithmetic (get_u_hat, spline records).
+  // The first P tile loads are issued BEFORE the parameters are staged: the DRAM latency of the first tiles overlaps the prologue arithmetic (get_u_hat, spline records).
   if (threadIdx.x == 0 && !GEN) {
     for (int i = 0; i < E.n_in; ++i) mbar_init(smem_u32(&bars[i]), 1);
     fence_mbar_init();

@@ -430,7 +430,7 @@ class GraphedCalls:
     """A fixed sequence of chain launches captured ONCE into a CUDA graph and replayed with one graph launch.
 
     Every entry point of libb2b.so is launch-only on the caller's stream (no host synchronisation, no library-owned
-    device state), so it is stream-capture safe; for launch-bound work -- a 20 us spline pass on one shard of an 8-way
+    device state), so it is stream-capture safe; for launch-bound work -- a short spline pass on one shard of an 8-way
     sharded batch costs less GPU time than the Python + driver launch path -- replaying a captured graph removes the
     per-launch host cost (SURVEY §8(b): "graph-captured sequence").  `fn` must issue the same launches on the same
     buffers every time (shapes, pointers and parameters tensors are baked into the graph; parameter VALUES are read at

@@ -4,7 +4,7 @@
 # (ext/BijectorsB200Ext.jl; `[weakdeps] CUDA`, `[extensions] BijectorsB200Ext = "CUDA"`), so every method below is a
 # more specific method of Bijectors' OWN generic functions on Bijectors' OWN layer types parametrised by CuArrays --
 # no type piracy.  Bijectors.jl has no FFI/plugin registry: "plugging in" = dispatch (src/interface.jl:144,156,183,265).
-# NOT runnable in the build container (no Julia toolchain exists there); the identical C ABI is exercised by the
+# Not exercised by the test suite (it has no Julia toolchain); the identical C ABI is exercised by the
 # Python/ctypes harness in bijectors.jl_b200/ (tests/, bench.py), and tests/test_host_logic.py parses every `ccall` in
 # this file and checks symbol, arity and argument classes against include/b2b.h.
 #

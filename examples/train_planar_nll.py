@@ -1,8 +1,8 @@
-"""The reference's flow-training example (docs/src/flows.md:40-110) on the B200 path: a PlanarLayer flow on 2-D data,
+"""The reference's flow-training example (docs/src/flows.md:40-110) on the H100 path: a PlanarLayer flow on 2-D data,
 trained by gradient descent on the negative log-likelihood −Σ logpdf(transformed(MvNormal(2, 1), flow), data).
 The reference differentiates with ForwardDiff; here torch.autograd drives b2b_planar_chain_vjp_f32 (reverse mode).
 
-    python examples/train_planar_nll.py            # needs a B200 (no CPU fallback)
+    python examples/train_planar_nll.py            # needs an H100 (no CPU fallback)
 """
 import math
 import os

@@ -1,5 +1,5 @@
 /*
- * b2b.h -- C ABI of libb2b.so: the B200-native batched bijector evaluation path.
+ * b2b.h -- C ABI of libb2b.so: the H100-native batched bijector evaluation path.
  *
  * This is the drop-in boundary for the hot path of TuringLang/Bijectors.jl (v0.16.2): batched
  * `with_logabsdet_jacobian` / `transform` / `logabsdetjac` / `logpdf` of normalising-flow layers over a
@@ -87,7 +87,7 @@ extern "C" {
  *                    (W column-major; rows 0..n1-1 give s, rows n1..2n1-1 give t; idx = PartitionMask rows.
  *                     n2 / n3 = first row of idx1 / idx2 when that list is the contiguous range
  *                     first..first+len-1 (then the pointer may be NULL), else -1.  Contiguous masks with
- *                     n1 <= 128 and n2 in {64,128} run on the tensor cores (tcgen05) when workspace is given.)
+ *                     n1 <= 128 and n2 in {64,128} run on the tensor cores (wgmma) when workspace is given.)
  * BATCHNORM          b[D]        logs[D]     m[D]        v[D]     -               -             -     -    eps
  * PERMUTE            -           -           -           -        dst_of_src[D]   -             -     -    -
  *                    (y[dst_of_src[i]] = x[i], i.e. Permute(indices) of permute.jl:90-100, 0-based)
@@ -356,8 +356,7 @@ int b2b_host_unregister(void* ptr);
 int b2b_numa_bind_to_device(int32_t device, int32_t* node_out, int32_t* ncpus_out);
 /* NUMA node of the PCIe root complex that serves CUDA device `device` (-1 when not exposed).  A launcher that starts
  * fewer ranks than the box has GPUs can use it to spread the ranks over the sockets: the host-buffer path is bound by
- * host DRAM bandwidth per socket (measured: four B200s behind one socket reach 0.52 of four times the single-GPU
- * throughput, two behind each socket 0.88). */
+ * host DRAM bandwidth per socket. */
 int b2b_device_numa_node(int32_t device, int32_t* node_out);
 
 /* ---- multi-GPU: the ONE collective of the path (SURVEY §8(e)) -----------------------------------

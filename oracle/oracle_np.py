@@ -18,7 +18,7 @@ the build container, so the reference itself cannot be executed here: this resta
 Values in the reference tests that depend on Julia RNG streams (``randn`` after ``seed!``, ``StableRNG``)
 are NOT reproducible without Julia: for those inputs parity is "pinned by property, not by value".
 
-Arithmetic that lives in third-party Julia packages (not under /root/reference; no Manifest is vendored,
+Arithmetic that lives in third-party Julia packages (not in the reference repository; no Manifest is vendored,
 only compat ranges in Project.toml) is restated from its published maths:
   LogExpFunctions (compat 0.3.3, 1.0)  log1pexp, softmax
   Roots (compat 1.3.15, 2, 3)          find_zero(..., A42()) -> any bracketing solver converging to

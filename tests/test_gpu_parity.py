@@ -649,15 +649,20 @@ def test_rand_and_shapes(B):
     assert not B.isclosedform(B.inverse(B.PlanarLayer(4))) and B.isclosedform(flow)
 
 
-@pytest.mark.parametrize("D,n1,row1,n2,row2", [(256, 128, 0, 128, 128), (256, 128, 128, 128, 0), (128, 64, 0, 64, 64),
-                                                (256, 64, 0, 128, 128), (192, 100, 64, 64, 0)])
-def test_coupling_tensor_core_path(B, D, n1, row1, n2, row2):
-    """The tcgen05 path (fp16 hi/lo split, 3 products, fp32 TMEM accumulation) against the oracle and against the
+_TC_SHORT = 64 * 37 + 29  # at most one 64-column tile per CTA
+_TC_LONG = 64 * 132 * 9 + 29  # nine tiles per CTA on 132 SMs: the stage barriers and the column-scale ring wrap
+_TC_CASES = [(256, 128, 0, 128, 128, _TC_SHORT), (256, 128, 128, 128, 0, _TC_SHORT), (128, 64, 0, 64, 64, _TC_SHORT),
+             (256, 64, 0, 128, 128, _TC_SHORT), (192, 100, 64, 64, 0, _TC_SHORT), (256, 128, 0, 128, 128, _TC_LONG)]
+
+
+@pytest.mark.parametrize("D,n1,row1,n2,row2,N", _TC_CASES,
+                         ids=["-".join(map(str, c[:5])) + ("" if c[5] == _TC_SHORT else "-many_tiles") for c in _TC_CASES])
+def test_coupling_tensor_core_path(B, D, n1, row1, n2, row2, N):
+    """The wgmma path (fp16 hi/lo split, 3 products, fp32 register accumulation) against the oracle and against the
     exact-fp32 CUDA-core kernel; masks with pass-through rows (x₃), out-of-place, in-place, N tail."""
     import torch
 
     rng = np.random.default_rng(D + n1 + row1)
-    N = 64 * 37 + 29
     idx1 = list(range(row1 + 1, row1 + n1 + 1))
     idx2 = list(range(row2 + 1, row2 + n2 + 1))
     W = (rng.standard_normal((2 * n1, n2)) * 0.3 / np.sqrt(n2)).astype(f32)
@@ -696,10 +701,13 @@ def test_coupling_tensor_core_path(B, D, n1, row1, n2, row2):
     # inverse (against the float64 oracle applied to the SAME float32 y), in place, accumulating the log-Jacobian
     yh = B.to_numpy(y).copy()
     xo, ljio = ol.inverse(yh[:, ok].astype(np.float64))
+    # the many-tile batch draws columns with s down to about -17, where y₁ − t cancels and exp(−s) amplifies it: there the
+    # float32 restatement of the reference is itself ~2e-3 away from float64, so that case is held to gate()
+    tol = RTOL if N == _TC_SHORT else gate(ol.inverse(yh[:, ok])[0], xo)
     acc = lj.clone()
     yi, acc = B.with_logabsdet_jacobian_(B.inverse(cl), y, None, acc)
     assert yi.data_ptr() == y.data_ptr()
-    assert rel(B.to_numpy(yi)[:, ok], xo) <= RTOL, rel(B.to_numpy(yi)[:, ok], xo)
+    assert rel(B.to_numpy(yi)[:, ok], xo) <= tol, (rel(B.to_numpy(yi)[:, ok], xo), tol)
     assert float(acc[torch.as_tensor(ok, device="cuda")].abs().max()) <= 1e-4 * max(1.0, float(np.abs(ljo).max()))
     # logabsdetjac alone (no D x N store)
     assert rel(B.to_numpy(B.logabsdetjac(cl, xd)), ljo) <= RTOL
@@ -736,7 +744,7 @@ def test_realnvp_config5_shape(B):
     n_folded = B.lib().b2b_last_launch_count()
     xo, ljo = O.chain_forward(ora_layers, yv.astype(np.float64))
     assert rel(B.to_numpy(xs), xo) <= RTOL and rel(B.to_numpy(ljf), ljo) <= RTOL
-    # BatchNorm layers ride inside the coupling launches: 4 x (fold table + W image + tcgen05 kernel), no BN launch
+    # BatchNorm layers ride inside the coupling launches: 4 x (fold table + W image + wgmma kernel), no BN launch
     assert n_folded == 12, n_folded
     B.lib().b2b_set_kernel_variant(100)  # same chain with the BatchNorm layers as their own launches
     try:

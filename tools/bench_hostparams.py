@@ -31,4 +31,4 @@ for name, flow in (("device", dev), ("host", host), ("device-inv", B.inverse(dev
         ts.append(e0.elapsed_time(e1))
     t = float(np.median(ts[3:]))
     gb = 4.0 * (2 * D + 1) * N / 1e9
-    print(f"{name:11s} D={D} L={L}  {t:.4f} ms  {N / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s  ({gb / t * 1e3 / 6570.9 * 100:.1f} % of 6570.9)")
+    print(f"{name:11s} D={D} L={L}  {t:.4f} ms  {N / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s  ({gb / t * 1e3 / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")

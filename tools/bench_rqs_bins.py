@@ -39,5 +39,5 @@ for K in (8, 6, 10, 16, 20):
         finally:
             B.lib().b2b_set_kernel_variant(0)
     gb = 4.0 * N * (2 * D + 1) / 1e9
-    print(f"K={K:2d}  program fwd {row[0][0]*1e3:6.1f} us ({gb/row[0][0]*1e3/6570.9*100:4.1f} %)  inv {row[0][1]*1e3:6.1f} us ({gb/row[0][1]*1e3/6570.9*100:4.1f} %)"
+    print(f"K={K:2d}  program fwd {row[0][0]*1e3:6.1f} us ({gb/row[0][0]*1e3/3350.0*100:4.1f} %)  inv {row[0][1]*1e3:6.1f} us ({gb/row[0][1]*1e3/3350.0*100:4.1f} %)"
           f"   interpreter fwd {row[1][0]*1e3:6.1f} us  inv {row[1][1]*1e3:6.1f} us")

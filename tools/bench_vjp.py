@@ -32,7 +32,7 @@ for name, pg in (("xbar only", False), ("xbar + parameter cotangents", True)):
     # x, ybar and the scalars (twice: skinny reductions + S statistics)
     gb = 4.0 * N * (3 * D + 1 + 3 * L) / 1e9 + (4.0 * N * (2 * D + 6 * L) / 1e9 if pg else 0.0)
     print(f"{name:30s} D={D} L={L}  {t:.4f} ms  {N / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s "
-          f"({gb / t * 1e3 / 6570.9 * 100:.1f} % of 6570.9)")
+          f"({gb / t * 1e3 / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")
 
 # radial chain (BASELINE C3 shape: 6 layers, D = 64)
 Dr, Lr = 64, 6
@@ -52,7 +52,7 @@ for it in range(11):
 t = float(np.median(ts[3:]))
 gb = 4.0 * N * (3 * Dr + 1) / 1e9
 print(f"radial VJP (xbar + parameter cotangents) D={Dr} L={Lr}  {t:.4f} ms  {N / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s "
-      f"({gb / t * 1e3 / 6570.9 * 100:.1f} % of 6570.9)")
+      f"({gb / t * 1e3 / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")
 
 
 def timed(fn, reps=11):
@@ -78,7 +78,7 @@ for name, t_ in (("forward", spl), ("inverse", B.inverse(spl))):
     t = timed(lambda: B.rqs_vjp(t_, xq, ybq, ljb))
     gb = 4.0 * N * (3 * Dq + 1) / 1e9
     print(f"RQS VJP {name} D={Dq} K={K}  {t:.4f} ms  {N / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s "
-          f"({gb / t * 1e3 / 6570.9 * 100:.1f} % of 6570.9)")
+          f"({gb / t * 1e3 / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")
 
 # RealNVP layer kinds (BASELINE C5 shape: D = 256, n1 = n2 = 128; N = 2^19)
 Dc, Nc = 256, 1 << 19
@@ -92,4 +92,4 @@ gb = 4.0 * Nc * (3 * Dc + 1) / 1e9
 for name, fn in (("coupling VJP", lambda: B.coupling_vjp(cl, xc, ybc, ljc)), ("batchnorm VJP", lambda: B.batchnorm_vjp(bn, xc, ybc, ljc))):
     t = timed(fn)
     print(f"{name} D={Dc} N=2^19  {t:.4f} ms  {Nc / t / 1e6:.2f} G samples/s  {gb / t * 1e3:.0f} GB/s "
-          f"({gb / t * 1e3 / 6570.9 * 100:.1f} % of 6570.9)")
+          f"({gb / t * 1e3 / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Register / stack / spill table of every kernel in libb2b.so from the -Xptxas -v logs the Makefile keeps
-(csrc/*.o.ptxas.log):  python tools/ptxas_table.py > profiles/r02_ptxas_registers.txt"""
+(csrc/*.o.ptxas.log):  python tools/ptxas_table.py"""
 import glob
 import os
 import re
@@ -25,7 +25,7 @@ for log in sorted(glob.glob(os.path.join(ROOT, "bijectors.jl_b200", "csrc", "*.p
             rows.append((name, int(m.group(1)), stack, st, ld))
             name = None
 names = subprocess.run(["cu++filt"] + [r[0] for r in rows], capture_output=True, text=True).stdout.splitlines()
-print("# -Xptxas -v of every kernel in libb2b.so at the round-2 HEAD: registers / stack frame / spill stores / spill loads (bytes)")
+print("# -Xptxas -v of every kernel in libb2b.so registers / stack frame / spill stores / spill loads (bytes)")
 out = []
 for (mangled, regs, stack, st, ld), dn in zip(rows, names):
     dn = re.sub(r"\(.*$", "", dn.replace("void ", "").replace("b2b::", "").replace("(int)", "").replace("(bool)", ""))

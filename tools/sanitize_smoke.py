@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Tiny invocation of every kernel family, meant to run under compute-sanitizer on the GPU box:
+"""Tiny invocation of every kernel family, meant to run under compute-sanitizer:
    compute-sanitizer --tool memcheck python tools/sanitize_smoke.py"""
 import os
 import sys

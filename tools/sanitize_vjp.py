@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Tiny invocation of every round-2 kernel family that is not in sanitize_smoke.py, for compute-sanitizer on the GPU box:
+"""Tiny invocation of every kernel family that is not in sanitize_smoke.py, for compute-sanitizer:
    compute-sanitizer --tool memcheck python tools/sanitize_vjp.py
 reverse mode (radial both directions + mixed, coupling fast / generic, BatchNorm, RQS both directions, planar runs),
 the in-kernel sampler, Float64 chains, Logit / Truncated blocks, exact-L planar programs, padded spline tables."""
