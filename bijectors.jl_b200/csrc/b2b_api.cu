@@ -13,7 +13,7 @@ int b2b_chain_grid_size_v1(const B2BChainParams& p);
 
 static thread_local int g_last_launches = 0;
 // kernel selection of b2b_set_kernel_variant: per calling thread (no mutable process-global state)
-static thread_local int g_variant = 0;           // fused chain kernel: 0 auto, 1 v0, 2 v1 interpreter, 3 unrolled planar
+static thread_local int g_variant = 0;           // fused chain kernel: 0 auto, 1 v0, 2 v1 interpreter, 3 planar chain
 static thread_local int g_fold_bn = 1;            // fold BatchNorm neighbours into coupling launches (hundreds digit 1 disables)
 static thread_local int g_coupling_variant = 0;  // coupling: 0 auto (tensor cores when possible), 1 force the fp32 CUDA-core kernel
 
@@ -93,7 +93,7 @@ static thread_local int g_fused_launches = 1;
 static int launch_fused(B2BChainParams& p, cudaStream_t stream) {
   int rc = B2B_EUNSUPPORTED;
   g_fused_launches = 1;
-  // segments made of <= 8 PlanarLayers: the unrolled planar kernel (variant 3 forces, 1 / 2 disable)
+  // segments made of <= 8 PlanarLayers: the fused planar chain kernel (variant 3 forces, 1 / 2 disable)
   if (g_variant == 0 || g_variant == 3) {
     rc = b2b_launch_planar_chain_const(p, stream);
     if (rc == B2B_OK) {

@@ -97,7 +97,7 @@ __device__ __forceinline__ float find_alpha_ts(float t, float c, float b, float&
   return x;
 }
 
-// Table-driven find_alpha for the unrolled planar kernels.  With u = α + b and s = t + b the equation reads
+// Table-driven find_alpha for the fused planar chain kernels.  With u = α + b and s = t + b the equation reads
 // u + c·tanh(u) = s, so the root is a ONE-dimensional function u = G_c(s) of the column's scalar s for a fixed layer.
 // Every CTA tabulates G_c on [−R, R] (R = 9.5 + |c|; beyond it tanh is ±1 in fp32 and u = s ∓ c exactly) as PT_N cubic
 // Hermite pieces (nodes solved with find_alpha_ts, slope 1/(1 + c·sech²u)) in its prologue; a column then takes
@@ -122,8 +122,9 @@ __device__ inline void planar_table_piece(float c, int i, float* tab) {
   if (i == 0) reinterpret_cast<float4*>(tab)[PT_N] = make_float4(R, (float)PT_N / (2.0f * R), 0.f, 0.f);
 }
 
-// the safeguarded iteration as an out-of-line call: the unrolled 8-layer program would otherwise carry eight inlined
-// copies of a loop it almost never runs and become instruction-cache bound
+// the safeguarded iteration as an out-of-line call: the planar layer loop would otherwise carry an inlined copy of a
+// loop it almost never runs in its hot body (inlined into each layer of the former unrolled 8-layer program, it made
+// the kernel instruction-cache bound)
 static __device__ __noinline__ float find_alpha_ts_call(float t, float c, float b, float* th, float* s2) {
   float th_, s2_;
   const float x = find_alpha_ts(t, c, b, th_, s2_);

@@ -55,14 +55,14 @@ static inline int b2b_layer_smem_floats(const b2b_layer_desc& d, int Dp) {
 int b2b_launch_chain_v0(const B2BChainParams& p, cudaStream_t stream);
 // v1: TMA-staged thread-per-column fused interpreter (D in {32,64,128}); returns B2B_EUNSUPPORTED otherwise
 int b2b_launch_chain_v1(const B2BChainParams& p, cudaStream_t stream);
-// constant-bank planar chains (b2b_planar_const.cu).  hostparams: `L` in {1,2,4,8} layers, derived parameters packed
+// fused planar chains (b2b_planar_const.cu).  hostparams: `L` in 1..8 layers, derived parameters packed
 // w[L][D] | û[L][D] | c[L] | b[L] in HOST memory, bit l of invmask = inverse of layer l.
 int b2b_launch_planar_hostparams(const B2BChainParams& p, int L, const float* packed, int invmask,
                                  cudaStream_t stream);
 // device-resident parameters: p.layers must be 1..8 PLANAR layers; B2B_EUNSUPPORTED when not applicable
 int b2b_launch_planar_chain_const(const B2BChainParams& p, cudaStream_t stream);
 int b2b_planar_const_grid_size(const B2BChainParams& p);
-// number of planar layers when the constant-bank path applies to the segment `p`, else 0
+// number of planar layers when the fused planar chain kernel applies to the segment `p`, else 0
 int b2b_planar_const_layers(const B2BChainParams& p);
 // reverse mode of a forward radial chain (b2b_radial_vjp.cu)
 size_t b2b_radial_vjp_workspace(int L, int D);

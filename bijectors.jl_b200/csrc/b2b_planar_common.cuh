@@ -12,9 +12,9 @@ constexpr int HP_MAX_D = 128;
 
 // get_u_hat (planar_layer.jl:65-70) of the layers P.layers[0..nreal) into shared memory, packed for (D, L):
 // w[L][D] | û[L][D] | c[L] | b[L]; layers nreal..L-1 are identity padding.  One warp per layer.
-template <int D, int L>
-__device__ __forceinline__ void planar_derive_smem(const B2BChainParams& P, int nreal, float* params, int warp, int lane,
-                                                   int nw) {
+template <int D>
+__device__ __forceinline__ void planar_derive_smem(const B2BChainParams& P, int nreal, int L, float* params, int warp,
+                                                   int lane, int nw) {
   for (int l = warp; l < L; l += nw) {
     float* w_out = params + l * D;
     float* u_out = params + L * D + l * D;
@@ -86,16 +86,7 @@ static __global__ void __launch_bounds__(HP_MAX_L * 32)
 }
 
 // ---- host side: launch shapes -------------------------------------------------------------------------------
-struct HPShape {
-  int nw, mode;
-};
-
-// warps per CTA as in the interpreter (register budget); MODE 2 when w and û exceed ~4 KB of constants
-static HPShape hp_shape(int D, int L) {
-  HPShape s;
-  s.nw = D == 128 ? 8 : (D == 64 ? 12 : 16);
-  s.mode = (2 * D * L * 4 > 4096) ? 2 : 0;
-  return s;
-}
+// warps per CTA as in the interpreter (register budget)
+static int hp_warps(int D) { return D == 128 ? 8 : (D == 64 ? 12 : 16); }
 
 }  // namespace b2b

@@ -34,7 +34,7 @@ struct PlanarVjpProg {
   float* scal;     // [N][3][L]: g | t | l̄·s/(1+c·s)
   long long N;
   __device__ __forceinline__ void stage(float* params, int warp, int lane, int nw) const {
-    planar_derive_smem<D, L>(P, nreal, params, warp, lane, nw);
+    planar_derive_smem<D>(P, nreal, L, params, warp, lane, nw);
   }
   // forward recompute on the x fragment: t_l, s_l
   __device__ __forceinline__ void phase1(float2 (&x)[1][D / 2], const ColCtx<D, 1>&, const float* params,
@@ -586,11 +586,10 @@ int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long
   wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
   const VjpWs ws = vjp_carve(wsb, Lp, D, p.N);
 
-  const HPShape sh = hp_shape(D, Lp);
   V1Geom g;
   static const int vjp_nw = getenv("B2B_VJP_NW") ? atoi(getenv("B2B_VJP_NW")) : 0;
   // D = 128 x 8 layers: two-tensor slots are 32 KB; 7 warps leave room for 3 of them (8 warps: 2)
-  const int nw = (D == 128 && Lp == 8) ? ((vjp_nw == 6 || vjp_nw == 8) ? vjp_nw : 7) : sh.nw;
+  const int nw = (D == 128 && Lp == 8) ? ((vjp_nw == 6 || vjp_nw == 8) ? vjp_nw : 7) : hp_warps(D);
   int rc = v1_geometry(D, p.N, nw, 32, (size_t)((2 * Lp * D + 2 * Lp + 3) & ~3), g, 2);
   if (rc != 0) return rc;
   CUtensorMap mx, mxb, myb;

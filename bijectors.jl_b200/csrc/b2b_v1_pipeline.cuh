@@ -1,5 +1,5 @@
 // TMA tile pipeline shared by the thread-per-column kernels (b2b_chain_v1.cu: layer interpreter,
-// b2b_planar_const.cu: constant-bank planar chains).  See b2b_chain_v1.cu for the design notes.
+// b2b_planar_const.cu: fused planar chains).  See b2b_chain_v1.cu for the design notes.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
