@@ -5,7 +5,7 @@ repository root registers this package under that name).
 """
 from ._lib import B2BError, LIB_PATH, exported_symbols, lib  # noqa: F401
 from .interface import (  # noqa: F401
-    Bijector, Columnwise, Composed, ComposedFunction, GraphedCalls, Inverse, Transform, colmajor_empty, columnwise, compose, flatten,
+    Bijector, Columnwise, Composed, ComposedFunction, GraphedCalls, Inverse, Transform, chain_vjp, colmajor_empty, columnwise, compose, flatten,
     from_numpy,
     inverse, isclosedform, isinvertible, logabsdetjac, logabsdetjac_, planar_chain_vjp, radial_chain_vjp, coupling_vjp, batchnorm_vjp, rqs_vjp, run_chain, to_numpy, transform, transform_,
     with_logabsdet_jacobian, with_logabsdet_jacobian_,
@@ -15,7 +15,7 @@ from .layers import (  # noqa: F401
     RationalQuadraticSpline, Scale, Shift, Stacked, TruncatedBijector, coupling, elementwise,
 )
 from .transformed_distribution import (  # noqa: F401
-    MvNormal, TransformedDistribution, logpdf, logpdf_sum, rand, transformed,
+    MvNormal, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, transformed,
 )
 from . import autograd, distributed  # noqa: F401
 

@@ -96,6 +96,9 @@ _SIGS = {
     "b2b_rqs_vjp_workspace_bytes": (c_size_t, [c_int32, c_int32]),
     "b2b_rqs_vjp_f32": (c_int, [POINTER(LayerDesc)] + [c_void_p] * 7 +
                         [c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "b2b_chain_vjp_workspace_bytes": (c_size_t, [POINTER(LayerDesc), c_int32, c_int32, c_int64]),
+    "b2b_chain_vjp_f32": (c_int, [POINTER(LayerDesc), c_int32] + [c_void_p] * 5 +
+                          [c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "b2b_radial_fwd_f32": (c_int, [_F32P] * 6 + [c_int32, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "b2b_radial_inv_f32": (c_int, [_F32P] * 6 + [c_int32, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "b2b_rqs_fwd_f32": (c_int, [_F32P] * 6 + [c_int32, c_int32, c_int64, c_int64, c_int64, c_int, c_void_p]),

@@ -1,5 +1,6 @@
-"""torch.autograd glue for planar flows: makes ``with_logabsdet_jacobian`` of a PlanarLayer chain (either direction)
-differentiable by routing the backward pass to ``b2b_planar_chain_vjp_f32`` -- the role the AD extensions play for the
+"""torch.autograd glue: makes ``with_logabsdet_jacobian`` of a PlanarLayer chain (either direction), of the other per-kind
+modules and -- through ``Flow`` -- of any chain differentiable by routing the backward pass to the library's VJP entry
+points (``b2b_planar_chain_vjp_f32`` ... ``b2b_chain_vjp_f32``) -- the role the AD extensions play for the
 reference (ext/BijectorsChainRulesCoreExt.jl, docs/src/flows.md:93-100).  No arithmetic on batches happens here."""
 from __future__ import annotations
 
@@ -7,7 +8,10 @@ from typing import List, Sequence, Tuple
 
 import torch
 
-from .interface import Composed, batchnorm_vjp, colmajor_empty, coupling_vjp, inverse, planar_chain_vjp, radial_chain_vjp, rqs_vjp, run_chain
+from . import _lib
+from ._lib import B2BError
+from .interface import (Composed, Inverse, _chain_vjp_raw, _trainable_slots, batchnorm_vjp, colmajor_empty, coupling_vjp, flatten,
+                        inverse, planar_chain_vjp, radial_chain_vjp, rqs_vjp, run_chain)
 from .layers import (AffineConditioner, Coupling, InvertibleBatchNorm, PartitionMask, PlanarLayer, RadialLayer,
                      RationalQuadraticSpline)
 
@@ -300,3 +304,97 @@ class SplineLayer(torch.nn.Module):
 
     def inverse(self, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         return _SplineFn.apply(y, *self.knots(), True)
+
+
+# ---- any chain: one b2b_chain_vjp_f32 call per backward ------------------------------------------------------------------
+def _trainable_tensors(leaf) -> List[torch.Tensor]:
+    """The device tensors of a leaf's trainable fields (Functors' trainable set of the reference's layer structs)."""
+    lay = leaf.orig if isinstance(leaf, Inverse) else leaf
+    if isinstance(lay, PlanarLayer):
+        return [lay.w, lay.u, lay.b]
+    if isinstance(lay, RadialLayer):
+        return [getattr(lay, "α_"), getattr(lay, "β"), lay.z_0]
+    if isinstance(lay, RationalQuadraticSpline):
+        return [lay.widths, lay.heights, lay.derivatives]
+    if isinstance(lay, Coupling):
+        return [t for t in (lay.θ.W, lay.θ.c) if t is not None]
+    if isinstance(lay, InvertibleBatchNorm):
+        if lay.training:
+            raise B2BError(_lib.B2B_EUNSUPPORTED, "Flow: InvertibleBatchNorm in training mode has no reverse mode on the device")
+        return [lay.b, lay.logs]
+    return []
+
+
+class _ChainFn(torch.autograd.Function):
+    """with_logabsdet_jacobian of a whole chain (plus, for logpdf, the terminal MvNormal); backward = ONE
+    b2b_chain_vjp_f32 call whose parameter cotangents are routed to the parameters by device address."""
+
+    @staticmethod
+    def forward(ctx, x, t, extra, want_y: bool, *params):
+        xc = _colmajor(x.detach())
+        D = xc.shape[0]
+        y, lj = run_chain(t, xc, want_y=want_y, extra_descs=extra)
+        descs = list(t._descs(False, D, torch.float32)) + list(extra)
+        owner = {p.data_ptr(): k for k, p in enumerate(params) if ctx.needs_input_grad[4 + k]}
+        # a parameter can appear in several descriptors (a layer used twice): its cotangent is the sum
+        ctx.want = [(l, i, owner[getattr(d, f"p{i}")]) for l, d in enumerate(descs) for i in _trainable_slots(d)
+                    if getattr(d, f"p{i}") in owner]
+        ctx.t, ctx.descs, ctx.extra, ctx.want_y, ctx.shapes = t, descs, extra, want_y, [p.shape for p in params]
+        ctx.save_for_backward(xc)
+        return (y, lj) if want_y else lj
+
+    @staticmethod
+    def backward(ctx, *grads):
+        (xc,) = ctx.saved_tensors
+        ybar, ljbar = grads if ctx.want_y else (None, grads[0])
+        yb = _colmajor(ybar) if ybar is not None else None
+        lb = ljbar.contiguous() if ljbar is not None else None
+        xbar, bars = _chain_vjp_raw(ctx.descs, xc, yb, lb, [(l, i) for l, i, _ in ctx.want])
+        out: List = [None] * len(ctx.shapes)
+        for l, i, k in ctx.want:
+            g = bars[(l, i)].reshape(ctx.shapes[k])
+            out[k] = g if out[k] is None else out[k] + g
+        return (xbar, None, None, None, *out)
+
+
+class Flow(torch.nn.Module):
+    """A trainable flow made of ANY chain of the supported layers -- `Stacked(ibs) ∘ PlanarLayer(2)`, spline flows with
+    permutations, coupling flows with bounded outputs -- over an optional MvNormal base.  Its parameters are the trainable
+    fields of every leaf of ``flatten(transform)`` (w/u/b, α_/β/z_0, processed RQS knots, W/c, b/logs) and μ, σ of the
+    base when it has them, registered on the leaves' own device storage: an optimiser step is what the next launch reads.
+    ``forward(x)`` / ``inverse(y)`` return (result, logjac); ``logpdf(y)`` is logpdf(transformed(base, transform), y) and
+    ``nll(y)`` = −Σ logpdf.  Each is one autograd Function whose backward is one b2b_chain_vjp_f32 call.  A training-mode
+    InvertibleBatchNorm raises (it has no reverse mode here)."""
+
+    def __init__(self, transform, base=None):
+        super().__init__()
+        from .transformed_distribution import MvNormal
+
+        self.transform, self.base = transform, base
+        tensors, seen = [], set()
+        for leaf in flatten(transform):
+            for t in _trainable_tensors(leaf):
+                if t.data_ptr() not in seen:
+                    seen.add(t.data_ptr())
+                    tensors.append(t)
+        if isinstance(base, MvNormal):
+            tensors += [t for t in (base.mu, base.sigma) if t is not None]
+        self.params = torch.nn.ParameterList([torch.nn.Parameter(t) for t in tensors])  # shares the leaves' storage
+
+    def _base(self, D, device):
+        from .transformed_distribution import MvNormal
+
+        return self.base if self.base is not None else MvNormal(D, device=device)
+
+    def forward(self, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        return _ChainFn.apply(x, self.transform, (), True, *self.params)
+
+    def inverse(self, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        return _ChainFn.apply(y, inverse(self.transform), (), True, *self.params)
+
+    def logpdf(self, y: torch.Tensor) -> torch.Tensor:
+        term = self._base(y.shape[0], y.device)._terminal_desc()
+        return _ChainFn.apply(y, inverse(self.transform), (term,), False, *self.params)
+
+    def nll(self, y: torch.Tensor) -> torch.Tensor:
+        return -self.logpdf(y).sum()

@@ -4,6 +4,8 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
+#include <utility>
 #include <vector>
 
 #include "b2b_internal.h"
@@ -618,4 +620,417 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
                                              workspace, workspace_bytes, &launches, stream);
   if (rc == B2B_OK) g_last_launches = launches;
   return rc;
+}
+
+// ---- reverse mode of any chain ------------------------------------------------------------------------------------------
+// The chain is cut into VJP segments, each differentiated by an existing per-kind kernel or by the elementwise-run kernel:
+// planar runs of one direction (<= 8), radial runs (<= 8, mixed directions), single RQS / coupling / eval-BatchNorm layers,
+// and runs of <= 8 STACKED_EW / PERMUTE layers optionally closed by the terminal MVNORMAL_DIAG.  The forward is recomputed
+// once, segment by segment, storing each segment's input (at ld = D); then the segments are differentiated last to first,
+// the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
+namespace {
+
+enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW };
+
+struct VSeg {
+  int kind, begin, end;
+  int Dk;  // rows the segment's kernel runs at: planar runs at D not in {32, 64, 128} are embedded in the next of them
+};
+
+size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+size_t mat_bytes(int D, long long N) { return al256((size_t)D * (size_t)N * sizeof(float)); }
+
+int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& segs) {
+  segs.clear();
+  for (int l = 0; l < L;) {
+    VSeg s{VK_EW, l, l + 1, D};
+    int& e = s.end;
+    switch (layers[l].kind) {
+      case B2B_PLANAR:
+        if (D > 128) return B2B_EUNSUPPORTED;
+        while (e < L && e - l < 8 && layers[e].kind == B2B_PLANAR && (layers[e].inverse != 0) == (layers[l].inverse != 0)) ++e;
+        s.kind = VK_PLANAR;
+        s.Dk = D <= 32 ? 32 : D <= 64 ? 64 : 128;
+        break;
+      case B2B_RADIAL:
+        if (D > 128) return B2B_EUNSUPPORTED;
+        while (e < L && e - l < 8 && layers[e].kind == B2B_RADIAL) ++e;
+        s.kind = VK_RADIAL;
+        break;
+      case B2B_RQS:
+        if (D > 256 || layers[l].n0 > 64) return B2B_EUNSUPPORTED;
+        s.kind = VK_RQS;
+        break;
+      case B2B_COUPLING_AFFINE:
+        if (layers[l].n0 > 128 || layers[l].n1 > 128) return B2B_EUNSUPPORTED;
+        s.kind = VK_COUPLING;
+        break;
+      case B2B_BATCHNORM:
+        if (D > 1024) return B2B_EUNSUPPORTED;
+        s.kind = VK_BN;
+        break;
+      default:  // PERMUTE / STACKED_EW (or the terminal MVNORMAL_DIAG alone)
+        if (D > 1024) return B2B_EUNSUPPORTED;
+        e = l;
+        while (e < L && e - l < 8 && (layers[e].kind == B2B_PERMUTE || layers[e].kind == B2B_STACKED_EW)) ++e;
+        if (e < L && layers[e].kind == B2B_MVNORMAL_DIAG) ++e;
+        if (e == l) return B2B_EINVAL;  // not a layer kind of include/b2b.h
+        s.kind = VK_EW;
+    }
+    segs.push_back(s);
+    l = e;
+  }
+  return B2B_OK;
+}
+
+// floats of parameter-cotangent scratch (each array rounded up to 64 floats) and bytes of kernel workspace of a segment
+size_t seg_param_floats(const b2b_layer_desc* layers, const VSeg& s, int D) {
+  const size_t n = (size_t)(s.end - s.begin);
+  auto r = [](size_t f) { return (f + 63) & ~(size_t)63; };
+  const b2b_layer_desc& d = layers[s.begin];
+  switch (s.kind) {
+    case VK_PLANAR: return 4 * r(n * s.Dk) + r(n);  // w̄, ū, b̄ as the kernel writes them (+ padded w, u)
+    case VK_RADIAL: return 2 * r(n) + r(n * D);
+    case VK_RQS: return 3 * r((size_t)D * d.n0);
+    case VK_COUPLING: return r((size_t)2 * d.n0 * d.n1) + r((size_t)2 * d.n0);
+    case VK_BN: return 2 * r(D);
+    default: return 0;
+  }
+}
+
+size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long long N) {
+  const int n = s.end - s.begin;
+  const b2b_layer_desc& d = layers[s.begin];
+  switch (s.kind) {
+    case VK_PLANAR: return b2b_planar_vjp_workspace(n, s.Dk, N);
+    case VK_RADIAL: return b2b_radial_vjp_workspace(n, D);
+    case VK_RQS: return b2b_rqs_vjp_workspace_bytes(d.n0, D);
+    case VK_COUPLING: return b2b_coupling_affine_vjp_workspace_bytes(d.n0, d.n1);
+    case VK_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
+    default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
+  }
+}
+
+// workspace: [checkpoints of segments 1..S-1][2 cotangent buffers][staged x][3 padded planar buffers][parameter scratch]
+//            [kernel workspace], each 256-aligned, + 256 of alignment slack
+struct VLayout {
+  size_t ckpt, ncot, stage, pad, param, kern, total;
+  int Dk_pad;  // rows of the padded planar buffers (0: none)
+};
+
+VLayout vjp_layout(const b2b_layer_desc* layers, const std::vector<VSeg>& segs, int D, long long N) {
+  VLayout v{};
+  const size_t S = segs.size(), m = mat_bytes(D, N);
+  v.ckpt = (S - 1) * m;
+  v.ncot = (S == 1 && segs[0].kind == VK_EW) ? 0 : 2;
+  // the planar kernels read x through TMA: an x they cannot read is copied (into a free checkpoint when there is one)
+  v.stage = (S == 1 && segs[0].kind == VK_PLANAR && segs[0].Dk == D) ? m : 0;
+  size_t pf = 0;
+  for (const VSeg& s : segs) {
+    if (s.kind == VK_PLANAR && s.Dk != D) v.Dk_pad = s.Dk;
+    pf = std::max(pf, seg_param_floats(layers, s, D));
+    v.kern = std::max(v.kern, al256(seg_kernel_bytes(layers, s, D, N)));
+  }
+  v.pad = v.Dk_pad ? 3 * mat_bytes(v.Dk_pad, N) : 0;
+  v.param = al256(pf * sizeof(float));
+  v.total = v.ckpt + v.ncot * m + v.stage + v.pad + v.param + v.kern + 256;
+  return v;
+}
+
+bool tma_ok(const float* p, long long ld) { return p && (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 4 == 0; }
+
+// elements of parameter slot i of layer d (the cotangent has the parameter's shape)
+size_t slot_len(const b2b_layer_desc& d, int i, int D) {
+  switch (d.kind) {
+    case B2B_PLANAR: return i == 2 ? 1 : D;
+    case B2B_RADIAL: return i == 2 ? D : 1;
+    case B2B_RQS: return (size_t)D * d.n0;
+    case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
+    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
+  }
+}
+
+}  // namespace
+
+extern "C" size_t b2b_chain_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N) {
+  if (!layers || L < 1 || L > B2B_MAX_CHAIN || D < 1 || N < 0) return 0;
+  for (int l = 0; l < L; ++l)
+    if (validate_layer(layers[l], D, l == L - 1) != B2B_OK) return 0;
+  std::vector<VSeg> segs;
+  if (vjp_segments(layers, L, D, segs) != B2B_OK) return 0;
+  return vjp_layout(layers, segs, D, N).total;
+}
+
+extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const float* x, const float* ybar,
+                                 const float* ljbar, float* xbar, float* const* param_bars, int32_t D, int64_t N,
+                                 int64_t ldx, int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes,
+                                 void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  g_last_launches = 0;
+  if (!layers || L < 1 || L > B2B_MAX_CHAIN || D < 1 || N < 0) return B2B_EINVAL;
+  for (int l = 0; l < L; ++l) {
+    const int rc = validate_layer(layers[l], D, l == L - 1);
+    if (rc != B2B_OK) return rc;
+  }
+  auto bar = [&](int l, int i) -> float* { return param_bars ? param_bars[4 * l + i] : nullptr; };
+  // trainable slots: PLANAR w u b, RADIAL α_ β z_0, RQS widths heights derivatives, COUPLING W c, BATCHNORM b logs,
+  // MVNORMAL_DIAG μ σ (when given); a cotangent of anything else is not computed
+  for (int l = 0; l < L && param_bars; ++l)
+    for (int i = 0; i < 4; ++i) {
+      if (!bar(l, i)) continue;
+      const b2b_layer_desc& d = layers[l];
+      switch (d.kind) {
+        case B2B_PLANAR:
+        case B2B_RADIAL:
+        case B2B_RQS:
+          if (i == 3) return B2B_EUNSUPPORTED;
+          break;
+        case B2B_COUPLING_AFFINE:
+          if (i >= 2) return B2B_EUNSUPPORTED;
+          if (i == 1 && !d.p1) return B2B_EINVAL;
+          break;
+        case B2B_BATCHNORM:
+          if (i >= 2) return B2B_EUNSUPPORTED;
+          break;
+        case B2B_MVNORMAL_DIAG:
+          if (i >= 2) return B2B_EUNSUPPORTED;
+          if (!(i == 0 ? d.p0 : d.p1)) return B2B_EINVAL;
+          break;
+        default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
+      }
+    }
+  std::vector<VSeg> segs;
+  int rc = vjp_segments(layers, L, D, segs);
+  if (rc != B2B_OK) return rc;
+  int launches = 0;
+  if (N == 0) {  // empty batch: the requested cotangents are zero
+    for (int l = 0; l < L && param_bars; ++l)
+      for (int i = 0; i < 4; ++i)
+        if (bar(l, i)) {
+          const cudaError_t e = cudaMemsetAsync(bar(l, i), 0, slot_len(layers[l], i, D) * sizeof(float), stream);
+          if (e != cudaSuccess) return (int)e;
+          ++launches;
+        }
+    g_last_launches = launches;
+    return B2B_OK;
+  }
+  if (!x || !xbar || ldx < D || ldxbar < D || (ybar && ldybar < D)) return B2B_EINVAL;
+  {  // x̄ is written while x and ȳ are still being read
+    auto range = [&](const void* p, long long ld) {
+      const char* a = static_cast<const char*>(p);
+      return std::make_pair(a, a + ((size_t)(N - 1) * (size_t)ld + (size_t)D) * sizeof(float));
+    };
+    const auto xb = range(xbar, ldxbar), xr = range(x, ldx);
+    if (xb.first < xr.second && xr.first < xb.second) return B2B_EINVAL;
+    if (ybar) {
+      const auto yr = range(ybar, ldybar);
+      if (xb.first < yr.second && yr.first < xb.second) return B2B_EINVAL;
+    }
+  }
+  const VLayout lay = vjp_layout(layers, segs, D, N);
+  if (!workspace || workspace_bytes < lay.total) return B2B_EWORKSPACE;
+  const int S = (int)segs.size();
+  const size_t m = mat_bytes(D, N);
+  char* ws = static_cast<char*>(workspace);
+  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
+  std::vector<float*> ckpt(S, nullptr);
+  for (int s = 1; s < S; ++s) ckpt[s] = reinterpret_cast<float*>(ws + (size_t)(s - 1) * m);
+  ws += lay.ckpt;
+  float* G[2] = {nullptr, nullptr};
+  for (size_t k = 0; k < lay.ncot; ++k) G[k] = reinterpret_cast<float*>(ws + k * m);
+  ws += lay.ncot * m;
+  float* stage = lay.stage ? reinterpret_cast<float*>(ws) : nullptr;
+  ws += lay.stage;
+  float* pad[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < 3 && lay.Dk_pad; ++k) pad[k] = reinterpret_cast<float*>(ws + (size_t)k * mat_bytes(lay.Dk_pad, N));
+  ws += lay.pad;
+  float* scratch = reinterpret_cast<float*>(ws);
+  ws += lay.param;
+  void* kws = ws;
+  const size_t kws_bytes = lay.kern;
+  const size_t F = sizeof(float);
+  cudaError_t e;
+#define B2B_VJP_CUDA(call)                    \
+  do {                                        \
+    if ((e = (call)) != cudaSuccess) return (int)e; \
+    ++launches;                               \
+  } while (0)
+
+  // 1. forward recompute: the input of every segment after the first
+  for (int s = 0; s + 1 < S; ++s) {
+    rc = b2b_chain_run_f32(layers + segs[s].begin, segs[s].end - segs[s].begin, s == 0 ? x : ckpt[s], ckpt[s + 1],
+                           nullptr, nullptr, D, N, s == 0 ? ldx : D, D, 0, nullptr, 0, stream);
+    if (rc != B2B_OK) return rc;
+    launches += g_last_launches;
+  }
+  // 2. reverse sweep
+  for (int s = S - 1; s >= 0; --s) {
+    const VSeg& sg = segs[s];
+    const int n = sg.end - sg.begin;
+    const b2b_layer_desc* ls = layers + sg.begin;
+    const float* in = s == 0 ? x : ckpt[s];
+    long long ldin = s == 0 ? ldx : D;
+    const float* cin = s == S - 1 ? ybar : G[(s + 1) & 1];
+    long long ldcin = s == S - 1 ? ldybar : D;
+    float* out = s == 0 ? xbar : G[s & 1];
+    const long long ldout = s == 0 ? ldxbar : D;
+    float* cstage = G[(s + 1) & 1];  // free while this segment runs: holds a zero / realigned ȳ
+    auto stage_cot = [&](int rows) -> int {  // cin := zeros (ȳ == NULL) or a copy at ld = rows
+      if (!cin) B2B_VJP_CUDA(cudaMemsetAsync(cstage, 0, (size_t)D * N * F, stream));
+      else B2B_VJP_CUDA(cudaMemcpy2DAsync(cstage, (size_t)rows * F, cin, (size_t)ldcin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
+      cin = cstage;
+      ldcin = rows;
+      return B2B_OK;
+    };
+    int nl = 0;
+    if (sg.kind == VK_PLANAR) {
+      const int Dk = sg.Dk;
+      const size_t r64 = ((size_t)n * Dk + 63) & ~(size_t)63;
+      float *wb = nullptr, *ub = nullptr, *bb = nullptr;
+      bool want = false;
+      for (int j = 0; j < n; ++j) want = want || bar(sg.begin + j, 0) || bar(sg.begin + j, 1) || bar(sg.begin + j, 2);
+      if (want) {
+        wb = scratch;
+        ub = scratch + r64;
+        bb = scratch + 2 * r64;
+      }
+      B2BChainParams p;
+      memset(&p, 0, sizeof(p));
+      p.N = N;
+      p.D = Dk;
+      p.L = n;
+      for (int j = 0; j < n; ++j) p.layers[j] = ls[j];
+      float* o = out;
+      long long ldo = ldout;
+      if (Dk != D) {
+        // embedded in Dk rows: w, u padded with zeros give the same map on the first D rows (wᵀz, wᵀu, ‖w‖² and those
+        // rows of û are unchanged) and leave the zero rows of x at zero
+        float* wp = scratch + 2 * r64 + 64;
+        float* up = wp + r64;
+        const float* src[16];
+        float* dst[16];
+        int len[16], dlen[16];
+        for (int j = 0; j < n; ++j) {
+          src[2 * j] = ls[j].p0;
+          dst[2 * j] = wp + (size_t)j * Dk;
+          src[2 * j + 1] = ls[j].p1;
+          dst[2 * j + 1] = up + (size_t)j * Dk;
+          len[2 * j] = len[2 * j + 1] = D;
+          dlen[2 * j] = dlen[2 * j + 1] = Dk;
+          p.layers[j].p0 = wp + (size_t)j * Dk;
+          p.layers[j].p1 = up + (size_t)j * Dk;
+        }
+        if ((rc = b2b_launch_copy_list(2 * n, src, dst, len, dlen, stream)) != B2B_OK) return rc;
+        ++launches;
+        const size_t pitch = (size_t)Dk * F, zrows = (size_t)(Dk - D) * F;
+        B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[0], pitch, in, (size_t)ldin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
+        B2B_VJP_CUDA(cudaMemset2DAsync(pad[0] + D, pitch, 0, zrows, N, stream));
+        if (cin) {
+          B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[1], pitch, cin, (size_t)ldcin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
+          B2B_VJP_CUDA(cudaMemset2DAsync(pad[1] + D, pitch, 0, zrows, N, stream));
+        } else {
+          B2B_VJP_CUDA(cudaMemsetAsync(pad[1], 0, (size_t)Dk * N * F, stream));
+        }
+        in = pad[0];
+        ldin = Dk;
+        cin = pad[1];
+        ldcin = Dk;
+        o = pad[2];
+        ldo = Dk;
+      } else {
+        if (!tma_ok(in, ldin)) {
+          float* st = S >= 2 ? ckpt[1] : stage;  // segment 1's checkpoint is no longer needed
+          B2B_VJP_CUDA(cudaMemcpy2DAsync(st, (size_t)D * F, in, (size_t)ldin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
+          in = st;
+          ldin = D;
+        }
+        if (!tma_ok(cin, ldcin) && (rc = stage_cot(D)) != B2B_OK) return rc;
+        if (!tma_ok(o, ldo)) {
+          o = G[s & 1];
+          ldo = D;
+        }
+      }
+      p.x = in;
+      p.ldx = ldin;
+      rc = b2b_launch_planar_chain_vjp(p, cin, ldcin, ljbar, o, ldo, wb, ub, bb, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+      if (o != out) B2B_VJP_CUDA(cudaMemcpy2DAsync(out, (size_t)ldout * F, o, (size_t)ldo * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
+      if (want) {
+        const float* src[24];
+        float* dst[24];
+        int len[24], dlen[24], c = 0;
+        for (int j = 0; j < n; ++j)
+          for (int i = 0; i < 3; ++i)
+            if (float* d = bar(sg.begin + j, i)) {
+              src[c] = i == 0 ? wb + (size_t)j * Dk : i == 1 ? ub + (size_t)j * Dk : bb + j;
+              dst[c] = d;
+              len[c] = dlen[c] = i == 2 ? 1 : D;
+              ++c;
+            }
+        if ((rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream)) != B2B_OK) return rc;
+        ++launches;
+      }
+    } else if (sg.kind == VK_RADIAL) {
+      if (!cin && (rc = stage_cot(D)) != B2B_OK) return rc;
+      float* ab = scratch;
+      float* bb = scratch + 64 * ((n + 63) / 64);
+      float* zb = bb + 64 * ((n + 63) / 64);
+      B2BChainParams p;
+      memset(&p, 0, sizeof(p));
+      p.x = in;
+      p.ldx = ldin;
+      p.N = N;
+      p.D = D;
+      p.L = n;
+      for (int j = 0; j < n; ++j) p.layers[j] = ls[j];
+      rc = b2b_launch_radial_chain_vjp(p, cin, ldcin, ljbar, out, ldout, ab, bb, zb, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+      const float* src[24];
+      float* dst[24];
+      int len[24], dlen[24], c = 0;
+      for (int j = 0; j < n; ++j)
+        for (int i = 0; i < 3; ++i)
+          if (float* d = bar(sg.begin + j, i)) {
+            src[c] = i == 0 ? ab + j : i == 1 ? bb + j : zb + (size_t)j * D;
+            dst[c] = d;
+            len[c] = dlen[c] = i == 2 ? D : 1;
+            ++c;
+          }
+      if (c) {
+        if ((rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream)) != B2B_OK) return rc;
+        ++launches;
+      }
+    } else if (sg.kind == VK_EW) {
+      const bool mvn = ls[n - 1].kind == B2B_MVNORMAL_DIAG;
+      rc = b2b_launch_ew_vjp(ls, n, in, ldin, cin, ldcin, ljbar, out, ldout, mvn ? bar(sg.end - 1, 0) : nullptr,
+                             mvn ? bar(sg.end - 1, 1) : nullptr, D, N, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+    } else {  // one RQS, coupling or eval-BatchNorm layer: its own entry point (two launches each)
+      if (!cin && (rc = stage_cot(D)) != B2B_OK) return rc;
+      const b2b_layer_desc& d = ls[0];
+      float* pb[3];
+      size_t off = 0;
+      for (int i = 0; i < 3; ++i) {  // cotangents the caller did not ask for go to scratch
+        pb[i] = bar(sg.begin, i);
+        if (!pb[i] && (sg.kind == VK_RQS || i < 2)) {
+          pb[i] = scratch + off;
+          off += (slot_len(d, i, D) + 63) & ~(size_t)63;
+        }
+      }
+      if (sg.kind == VK_RQS)
+        rc = b2b_rqs_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], pb[2], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
+      else if (sg.kind == VK_COUPLING)
+        rc = b2b_coupling_affine_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
+      else
+        rc = b2b_batchnorm_eval_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
+      if (rc != B2B_OK) return rc;
+      launches += 2;
+    }
+  }
+#undef B2B_VJP_CUDA
+  g_last_launches = launches;
+  return B2B_OK;
 }

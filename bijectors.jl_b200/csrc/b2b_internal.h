@@ -80,6 +80,15 @@ size_t b2b_planar_vjp_workspace(int L, int D, long long N);
 int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
                                 float* xbar, long long ldxb, float* wbar, float* ubar, float* bbar, void* workspace,
                                 size_t workspace_bytes, int* launches, cudaStream_t stream);
+// reverse mode of an elementwise run (b2b_ew_vjp.cu): <= 8 STACKED_EW / PERMUTE layers, optionally closed by the terminal
+// MVNORMAL_DIAG.  ybar, ljbar may be NULL (zeros); mubar / sigmabar (D, or NULL) need b2b_ew_vjp_workspace(D, 1) bytes.
+size_t b2b_ew_vjp_workspace(int D, int want_mvn_params);
+int b2b_launch_ew_vjp(const b2b_layer_desc* layers, int L, const float* x, long long ldx, const float* ybar,
+                      long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* mubar, float* sigmabar,
+                      int D, long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
+// one launch copying up to 24 small device vectors: dst[k][0, len[k]) = src[k][0, len[k]), zero up to dst_len[k]
+int b2b_launch_copy_list(int n, const float* const* src, float* const* dst, const int* len, const int* dst_len,
+                         cudaStream_t stream);
 // number of CTAs the v0/v1 launch of `p` will use (size of the partials array)
 int b2b_chain_grid_size(const B2BChainParams& p);
 // deterministic final sum of per-CTA partials into *sum_out

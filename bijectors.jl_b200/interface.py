@@ -762,3 +762,111 @@ def isclosedform(t) -> bool:
     if isinstance(t, (ComposedFunction, Composed)):
         return all(isclosedform(b) for b in flatten(t))
     return True
+
+
+# --------------------------------------------------------------------------------------------------
+# reverse mode of any chain: b2b_chain_vjp_f32
+# --------------------------------------------------------------------------------------------------
+
+# names of the trainable descriptor slots p0..p3 of each kind (the reference's field names)
+_SLOT_NAMES = {
+    _lib.PLANAR: ("w", "u", "b"),
+    _lib.RADIAL: ("α_", "β", "z_0"),
+    _lib.RQS: ("widths", "heights", "derivatives"),
+    _lib.COUPLING_AFFINE: ("W", "c"),
+    _lib.BATCHNORM: ("b", "logs"),
+    _lib.MVNORMAL_DIAG: ("μ", "σ"),
+}
+
+
+def _trainable_slots(d) -> List[int]:
+    """Slots of descriptor ``d`` that have a cotangent (absent optional parameters have none)."""
+    names = _SLOT_NAMES.get(d.kind, ())
+    return [i for i in range(len(names)) if getattr(d, f"p{i}")]
+
+
+def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
+    """Shape of the device tensor behind slot i of ``d`` (the storage layout the library reads)."""
+    if d.kind == _lib.PLANAR:
+        return (1,) if i == 2 else (D,)
+    if d.kind == _lib.RADIAL:
+        return (D,) if i == 2 else (1,)
+    if d.kind == _lib.RQS:
+        return (d.n0, D)  # column-major D × K+1
+    if d.kind == _lib.COUPLING_AFFINE:
+        return (d.n1, 2 * d.n0) if i == 0 else (2 * d.n0,)  # W column-major (2n1 × n2)
+    return (D,)
+
+
+def _chain_vjp_raw(descs, x: torch.Tensor, ybar: Optional[torch.Tensor], ljbar: Optional[torch.Tensor], want):
+    """One b2b_chain_vjp_f32 call.  ``want``: (descriptor index, slot) pairs.  Returns (xbar, {(l, i): cotangent in the
+    storage shape of that parameter})."""
+    D, N, ldx = _batch_view(x)
+    if not x.is_cuda or x.dtype != torch.float32:
+        raise ValueError("chain_vjp: x must be a Float32 device batch")
+    ldyb = D
+    if ybar is not None:
+        Dy, Ny, ldyb = _batch_view(ybar)
+        if (Dy, Ny) != (D, N) or not ybar.is_cuda or ybar.dtype != torch.float32:
+            raise ValueError("chain_vjp: ybar must be a Float32 device batch of x's shape")
+    if ljbar is not None and (ljbar.numel() != N or ljbar.dtype != torch.float32 or not ljbar.is_contiguous()):
+        raise ValueError("ljbar must be a contiguous float32 vector of length N")
+    arr = _desc_array(descs)
+    L = len(descs)
+    bars = {}
+    ptrs = (ctypes.c_void_p * (4 * L))()
+    for l, i in want:
+        t = torch.empty(_slot_shape(descs[l], i, D), dtype=torch.float32, device=x.device)
+        bars[(l, i)] = t
+        ptrs[4 * l + i] = t.data_ptr()
+    xbar = torch.empty_like(x) if x.dim() == 1 else colmajor_empty(D, N, x.device)
+    L_ = lib()
+    ws_bytes = L_.b2b_chain_vjp_workspace_bytes(arr, L, D, N)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device) if ws_bytes else None
+    rc = L_.b2b_chain_vjp_f32(
+        arr, L, x.data_ptr(), ybar.data_ptr() if ybar is not None else None,
+        ljbar.data_ptr() if ljbar is not None else None, xbar.data_ptr(), ctypes.cast(ptrs, ctypes.c_void_p) if want else None,
+        D, N, ldx, ldyb, _batch_view(xbar)[2], ws.data_ptr() if ws is not None else None, ws_bytes, _stream())
+    check(rc, "b2b_chain_vjp_f32")
+    return xbar, bars
+
+
+def _leaf_descs(t, D: int):
+    """(descriptors of ``t`` in application order, number of descriptors of each leaf of flatten(t))."""
+    descs, counts = [], []
+    for leaf in flatten(t):
+        ds = list(leaf._descs(False, D, torch.float32))
+        descs += ds
+        counts.append(len(ds))
+    return descs, counts
+
+
+def _leaf_grads(descs, counts, bars) -> List[dict]:
+    """One dict per leaf, keyed by the reference's field names; RQS knots as D × K+1 and W as (2n1 × n2)."""
+    grads, k = [], 0
+    for c in counts:
+        g = {}
+        for l in range(k, k + c):
+            d = descs[l]
+            for i in _trainable_slots(d):
+                t = bars[(l, i)]
+                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind == _lib.RQS or (d.kind == _lib.COUPLING_AFFINE and i == 0)) else t
+        grads.append(g)
+        k += c
+    return grads
+
+
+def chain_vjp(t, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Optional[torch.Tensor] = None):
+    """Vector-Jacobian product of ``with_logabsdet_jacobian(t, x)`` for ANY chain the forward accepts -- every layer kind,
+    either direction, mixed: what the reference's reverse-mode AD computes when a flow is trained
+    (docs/src/flows.md:93-100).  ``ybar`` (D×N) / ``ljbar`` (N) are the cotangents of the two outputs (None = zeros).
+    One b2b_chain_vjp_f32 call.  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)`` (application
+    order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives`` (D×K+1),
+    ``W/c``, ``b/logs``, and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
+    D = _batch_view(x)[0]
+    descs, counts = _leaf_descs(t, D)
+    if not descs:
+        raise ValueError("empty chain")
+    want = [(l, i) for l, d in enumerate(descs) for i in _trainable_slots(d)]
+    xbar, bars = _chain_vjp_raw(descs, x, ybar, ljbar, want)
+    return xbar, _leaf_grads(descs, counts, bars)

@@ -320,6 +320,44 @@ function rqs_vjp(b, x::CuMatrix{Float32}, ȳ::CuMatrix{Float32}, l̄::CuVector{F
     return x̄, W̄, H̄, D̄
 end
 
+# Reverse mode of ANY device chain (b2b_chain_vjp_f32): `f` (or inverse(f) with inv=true); ȳ, l̄ the cotangents of
+# (y, logjac), `nothing` = zeros.  Returns x̄ and, per descriptor in application order, the cotangents of its trainable
+# fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, BatchNorm b logs, the
+# terminal MvNormal's μ σ) in the fields' shapes; `nothing` for fields without one.
+function vjp_slots(d::LayerDesc, D::Integer)
+    z(dims...) = CUDA.zeros(Float32, dims...)
+    d.kind == PLANAR && return (z(D), z(D), z(1))
+    d.kind == RADIAL && return (z(1), z(1), z(D))
+    d.kind == RQS && return (z(D, d.n0), z(D, d.n0), z(D, d.n0))
+    d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
+    d.kind == BATCHNORM && return (z(D), z(D))
+    d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
+    return ()
+end
+chain_vjp(f, x::CuMatrix{Float32}, ȳ, l̄; inv::Bool=false) = chain_vjp(descs(f, inv), x, ȳ, l̄)
+function chain_vjp(ds::Vector{LayerDesc}, x::CuMatrix{Float32}, ȳ, l̄)
+    L, (D, N) = length(ds), size(x)
+    bars = [vjp_slots(d, D) for d in ds]
+    ptrs = Ptr{Cvoid}[i <= length(b) && b[i] !== nothing ? Ptr{Cvoid}(UInt(pointer(b[i]))) : C_NULL for b in bars for i in 1:4]
+    x̄ = similar(x)
+    nbytes = ccall((:b2b_chain_vjp_workspace_bytes, libb2b), Csize_t, (Ptr{LayerDesc}, Int32, Int32, Int64), ds, L, D, N)
+    ws = CuVector{UInt8}(undef, nbytes)
+    GC.@preserve ds bars ptrs ws ȳ l̄ check(ccall((:b2b_chain_vjp_f32, libb2b), Cint,
+        (Ptr{LayerDesc}, Int32, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Ptr{Ptr{Cvoid}}, Int32,
+         Int64, Int64, Int64, Int64, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+        ds, L, pointer(x), ȳ === nothing ? NULLF : pointer(ȳ), l̄ === nothing ? NULLF : pointer(l̄), pointer(x̄), ptrs,
+        D, N, stride(x, 2), ȳ === nothing ? D : stride(ȳ, 2), stride(x̄, 2), pointer(ws), nbytes, stream_handle()))
+    return x̄, bars
+end
+# Reverse mode of logpdf(td, y) with cotangent l̄ of the logpdf vector: (ȳ, flow cotangents in flow order, (μ̄, σ̄)).
+function logpdf_vjp(td::TransformedDistribution{<:MvNormal}, y::CuMatrix{Float32}, l̄::CuVector{Float32})
+    ds = descs(td.transform, true)
+    μ, σ = cu(Float32.(mean(td.dist))), cu(Float32.(sqrt.(var(td.dist))))
+    push!(ds, LayerDesc(MVNORMAL_DIAG, 0, 0, 0, 0, 0, 0f0, 0f0, pointer(μ), pointer(σ), NULLF, NULLF, NULLI, NULLI))
+    ȳ, bars = GC.@preserve μ σ chain_vjp(ds, y, nothing, l̄)
+    return ȳ, reverse(bars[1:end-1]), bars[end]
+end
+
 # rand(rng, td, n) (src/transformed_distribution.jl:212-224): the base samples are generated INSIDE the chain kernel
 # (Philox4x32-10 + Box-Muller); `seed` plays the role of rng, `column_offset` continues one stream across column shards.
 function device_rand(td::TransformedDistribution{<:MvNormal}, n::Integer; seed::UInt64=rand(UInt64), offset::UInt64=UInt64(0),

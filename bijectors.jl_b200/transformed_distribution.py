@@ -139,3 +139,25 @@ def rand(td, n: int, seed: Optional[int] = None, offset: int = 0, column_offset:
     else:
         y, lj = _sample(td.dist, td.transform, n, seed, offset, column_offset, with_logjac)
     return (y, lj) if with_logjac else y
+
+
+def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[torch.Tensor] = None):
+    """Reverse mode of ``logpdf(td, y)``: one b2b_chain_vjp_f32 call through inverse(td.transform) and the terminal
+    MvNormal.  ``lpbar`` (N, None = ones) is the cotangent of the logpdf vector.  Returns ``(ybar, flow_grads, base_grads)``:
+    ``flow_grads`` one dict per leaf of ``flatten(td.transform)`` in FLOW order (see chain_vjp for the keys) and
+    ``base_grads`` = {"μ", "σ"} for the base parameters that are given; all summed over the columns of this batch."""
+    from .interface import _chain_vjp_raw, _leaf_descs, _leaf_grads, _trainable_slots
+
+    D, N, _ = _batch_view(y)
+    if D != len(td.dist):
+        raise ValueError(f"DimensionMismatch: distribution has {len(td.dist)} dims, input has {D}")
+    if lpbar is None:
+        lpbar = torch.ones((N,), dtype=torch.float32, device=y.device)
+    descs, counts = _leaf_descs(inverse(td.transform), D)
+    descs.append(td.dist._terminal_desc())
+    want = [(l, i) for l, d in enumerate(descs) for i in _trainable_slots(d)]
+    ybar, bars = _chain_vjp_raw(descs, y, None, lpbar, want)
+    flow = _leaf_grads(descs, counts, bars)[::-1]
+    T = len(descs) - 1
+    base = {name: bars[(T, i)] for i, name in enumerate(("μ", "σ")) if (T, i) in bars}
+    return ybar, flow, base

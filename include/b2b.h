@@ -231,6 +231,30 @@ size_t b2b_rqs_vjp_workspace_bytes(int32_t K1, int32_t D);
 int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar, float* xbar,
                     float* widths_bar, float* heights_bar, float* derivs_bar, int32_t D, int64_t N, int64_t ldx,
                     int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes, void* stream);
+/* Reverse mode of b2b_chain_run_f32: the vector-Jacobian product through ANY chain it accepts -- layers in application
+ * order with their `inverse` flags, optionally ending in the terminal B2B_MVNORMAL_DIAG (then the logjac output is
+ * logpdf).  What the reference's reverse-mode AD computes for `with_logabsdet_jacobian(flow, x)` or
+ * `logpdf(transformed(base, flow), y)` (docs/src/flows.md:93-100).
+ * Inputs: `x`, the batch the chain was applied to; `ybar` (D x N) the cotangent of the y that b2b_chain_run_f32 writes
+ * for the same chain (NULL = zeros, the usual case for logpdf); `ljbar` (N) the cotangent of logjac / logpdf (NULL =
+ * zeros).  Outputs: `xbar` (D x N, required, must not overlap `x` or `ybar`: B2B_EINVAL) and, when `param_bars` != NULL,
+ * 4*L pointers: entry 4l+i receives the cotangent of layers[l].p<i> in the shape and layout of p<i> (NULL entries are not
+ * computed), summed over the N columns in a fixed order (deterministic; a multi-GPU caller all-reduces them).
+ * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c;
+ * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL).  Any other
+ * non-NULL entry (BatchNorm m / v, PERMUTE, STACKED_EW) returns B2B_EUNSUPPORTED.
+ * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
+ * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling /
+ * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
+ * differentiates.  The forward is recomputed once to checkpoint each segment's input, then the segments are
+ * differentiated last to first.  Limits are the kernels': planar and radial D <= 128, RQS D <= 256 and K1 <= 64, coupling
+ * n1, n2 <= 128, BatchNorm and elementwise runs D <= 1024 (else B2B_EUNSUPPORTED).  N == 0 zeroes the requested parameter
+ * cotangents.  Launch-only on `stream`, no allocation (CUDA-graph capturable).  workspace: b2b_chain_vjp_workspace_bytes
+ * (0 = unsupported chain); b2b_last_launch_count counts every kernel, copy and fill enqueued. */
+size_t b2b_chain_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N);
+int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const float* x, const float* ybar, const float* ljbar,
+                      float* xbar, float* const* param_bars, int32_t D, int64_t N, int64_t ldx, int64_t ldybar,
+                      int64_t ldxbar, void* workspace, size_t workspace_bytes, void* stream);
 /* RadialLayer: radial_layer.jl:58-72 (fwd), :88-102,124-129 (inverse) */
 int b2b_radial_fwd_f32(const float* x, float* y, float* logjac, const float* alpha_raw,
                        const float* beta, const float* z0, int32_t D, int64_t N, int64_t ldx,

@@ -1,0 +1,152 @@
+"""Float64 restatements of the reverse mode of the elementwise layers (Stacked laws, Permute), of the terminal MvNormal and
+of whole mixed chains -- the references of b2b_chain_vjp_f32.  They compose the per-kind VJPs of oracle/oracle_np.py and
+are themselves checked against central finite differences (tests/test_oracle_chain_vjp.py)."""
+from __future__ import annotations
+
+import numpy as np
+
+from oracle import oracle_np as O
+
+EW = O.EW
+
+
+def _law_deriv(op, inverse, x):
+    """(f′, ∂log|f′|/∂x) of one Stacked law at x (float64): what AD of the reference's formulas gives, including
+    _clamp's zero derivative outside [lb, ub] (Bijectors.jl:95-100) and LeakyReLU's identity branch at 0."""
+    code = op[0]
+    a = float(op[1]) if len(op) > 1 else 0.0
+    b = float(op[2]) if len(op) > 2 else 0.0
+    one, zero = np.ones_like(x), np.zeros_like(x)
+    if code in (EW.EXP, EW.LOG):
+        if (code == EW.EXP) != inverse:
+            return np.exp(x), one
+        return 1 / x, -1 / x
+    if code == EW.SCALE:
+        return one * (1 / a if inverse else a), zero
+    if code == EW.LEAKY_RELU:
+        al = 1 / a if inverse else a
+        return np.where(x < 0, al, 1.0), zero
+    if code == EW.LOGIT:
+        if not inverse:
+            return 1 / (x - a) + 1 / (b - x), 1 / (b - x) - 1 / (x - a)
+        s = O._logistic(x)
+        return (b - a) * s * (1 - s), 1 - 2 * s
+    if code == EW.TRUNCATED:
+        lo, hi = np.isfinite(a), np.isfinite(b)
+        if not inverse:
+            inside = (x >= a) & (x <= b)
+            xc = np.where(inside, x, (a if lo else 0.0) + 0.5)  # any interior point: the result is masked
+            if lo and hi:
+                f, d = 1 / (xc - a) + 1 / (b - xc), 1 / (b - xc) - 1 / (xc - a)
+            elif lo:
+                f, d = 1 / (xc - a), -1 / (xc - a)
+            elif hi:
+                f, d = -1 / (b - xc), 1 / (b - xc)
+            else:
+                f, d = one, zero
+            return np.where(inside, f, 0.0), np.where(inside, d, 0.0)
+        if lo and hi:
+            s = O._logistic(x)
+            xo, f, d = (b - a) * s + a, (b - a) * s * (1 - s), 1 - 2 * s
+        elif lo or hi:
+            e = np.exp(x)
+            xo, f, d = (e + a if lo else b - e), (e if lo else -e), one
+        else:
+            xo, f, d = x, one, zero
+        return np.where((xo < a) | (xo > b), 0.0, f), d
+    return one, zero  # IDENTITY, SHIFT
+
+
+def stacked_vjp(ops, ranges, x, ybar, ljbar, inverse=False):
+    """Input cotangent of with_logabsdet_jacobian(Stacked(laws, ranges), x) (or of its inverse): x̄ = ȳ·f′ + l̄·∂log|f′|/∂x
+    per element.  ``ops`` / ``ranges`` as in oracle_np.stacked_forward; x, ybar (D, N), ljbar (N,)."""
+    x = np.asarray(x)
+    xbar = np.empty_like(x)
+    lb = np.asarray(ljbar, x.dtype)[None, :]
+    for op, (lo, hi) in zip(ops, ranges):
+        f, d = _law_deriv(op, inverse, x[lo - 1:hi])
+        xbar[lo - 1:hi] = ybar[lo - 1:hi] * f + lb * d
+    return xbar
+
+
+def permute_vjp(A, ybar, inverse=False):
+    """Input cotangent of Permute(A) (y = A x, permute.jl:152) or of its inverse (x = Aᵀ y, :153): Aᵀ ȳ or A x̄."""
+    A = np.asarray(A, np.float64)
+    return (A @ ybar) if inverse else (A.T @ ybar)
+
+
+def mvnormal_diag_logpdf_vjp(mu, sigma, x, lpbar):
+    """Cotangents (x̄, μ̄, σ̄) of logpdf(MvNormal(μ, Diagonal(σ²)), x) with cotangent lpbar (N,) of the logpdf vector:
+    q = (x − μ)/σ, x̄ = −l̄·q/σ, μ̄ = Σ_n l̄·q/σ, σ̄ = Σ_n l̄·(q² − 1)/σ."""
+    x = np.asarray(x)
+    D, dt = x.shape[0], x.dtype
+    mu = np.zeros(D, dt) if mu is None else np.asarray(mu, dt)
+    sigma = np.ones(D, dt) if sigma is None else np.asarray(sigma, dt)
+    q = (x - mu[:, None]) / sigma[:, None]
+    lb = np.asarray(lpbar, dt)[None, :]
+    g = lb * q / sigma[:, None]
+    return -g, g.sum(axis=1), (lb * (q * q - 1) / sigma[:, None]).sum(axis=1)
+
+
+def _layer_vjp(lay: O.Layer, inv: bool, x, ybar, ljbar):
+    """(x̄, parameter cotangents as a dict keyed like the device grads) of one oracle layer applied to x."""
+    p, k = lay.params, lay.kind
+    if k == "planar":
+        fn = O.planar_inverse_chain_vjp if inv else O.planar_chain_vjp
+        xb, g = fn([(p["w"], p["u"], p["b"])], x, ybar, ljbar)
+        return xb, dict(w=g[0][0], u=g[0][1], b=g[0][2])
+    if k == "radial":
+        xb, g = O.radial_chain_vjp_dir([(p["alpha_raw"], p["beta"], p["z0"])], [inv], x, ybar, ljbar)
+        return xb, {"α_": g[0][0], "β": g[0][1], "z_0": g[0][2]}
+    if k == "rqs":
+        xb, W, H, Dv = O.rqs_vjp(p["widths"], p["heights"], p["derivs"], x, ybar, ljbar, inverse=inv)
+        return xb, dict(widths=W, heights=H, derivatives=Dv)
+    if k == "coupling_affine":
+        xb, W, c = O.coupling_affine_vjp(p["idx1"], p["idx2"], p["W"], p["c"], x, ybar, ljbar, inverse=inv)
+        return xb, dict(W=W, c=c)
+    if k == "batchnorm":
+        xb, b, ls = O.batchnorm_eval_vjp(p["bn"], x, ybar, ljbar, inverse=inv)
+        return xb, dict(b=b, logs=ls)
+    if k == "permute":
+        return permute_vjp(p["A"], ybar, inverse=inv), {}
+    if k == "stacked":
+        return stacked_vjp(p["ops"], p["ranges"], x, ybar, ljbar, inverse=inv), {}
+    raise ValueError(k)
+
+
+def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, terminal=False, dtype=np.float64):
+    """Reverse mode of a chain applied in the given order (layer l inverted when inverse_flags[l]), optionally closed by
+    the terminal MvNormal(μ, σ) (then the log-Jacobian output is logpdf).  ybar (D, N) or None (zeros), ljbar (N,).
+    Evaluated in `dtype` (float32 gives the reference's own float32 error for the parity gate).
+    Returns (x̄, [grads dict per layer], {"μ": …, "σ": …} or {})."""
+    x = np.asarray(x, dtype)
+    N = x.shape[1]
+    lb = np.zeros(N, dtype) if ljbar is None else np.asarray(ljbar, dtype)
+    inputs, cur = [], x
+    for lay, inv in zip(layers, inverse_flags):
+        inputs.append(cur)
+        cur = (lay.inverse if inv else lay.forward)(cur)[0]
+    g = np.zeros_like(cur) if ybar is None else np.asarray(ybar, dtype)
+    base = {}
+    if terminal:
+        gx, gm, gs = mvnormal_diag_logpdf_vjp(mu, sigma, cur, lb)
+        g = g + gx
+        if mu is not None:
+            base["μ"] = gm
+        if sigma is not None:
+            base["σ"] = gs
+    grads = [None] * len(layers)
+    for l in reversed(range(len(layers))):
+        g, grads[l] = _layer_vjp(layers[l], inverse_flags[l], inputs[l], g, lb)
+    return g, grads, base
+
+
+def chain_logjac(layers, inverse_flags, x, mu=None, sigma=None, terminal=False):
+    """(y, logjac or logpdf) of the same chain in float64 (for finite differences)."""
+    cur, lj = np.asarray(x, np.float64), 0.0
+    for lay, inv in zip(layers, inverse_flags):
+        cur, l = (lay.inverse if inv else lay.forward)(cur)
+        lj = lj + l
+    if terminal:
+        lj = lj + O.mvnormal_diag_logpdf(mu, sigma, cur)
+    return cur, lj

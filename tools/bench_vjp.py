@@ -1,5 +1,10 @@
-"""Times the reverse-mode (VJP) path of the headline chain: 8 x PlanarLayer, D=128, N=2^20."""
+"""Times the reverse-mode (VJP) path of the headline chain: 8 x PlanarLayer, D=128, N=2^20.
+`python tools/bench_vjp.py chain` times b2b_chain_vjp_f32 instead, as device time of graph-captured calls: (a) the
+elementwise-run kernel alone on Stacked(Logit + exp rows) + Permute + MvNormal, (b) the logpdf gradient of
+inverse(8 x Planar) + MvNormal through logpdf_vjp against planar_chain_vjp with the base density's cotangent in torch, the
+two routes alternated."""
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -7,6 +12,70 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bijectors_jl_b200 as B
+
+
+def bench_chain():
+    D, N, L = 128, 1 << 20, 8
+    rng = np.random.default_rng(0)
+    try:
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        power = "unknown"
+    print(f"card: {torch.cuda.get_device_name()}, power limit: {power}")
+
+    def device_ms(fn, reps=20):
+        """Device time of one call: the call is captured once into a CUDA graph (no host work in the timed window) and
+        the graph is replayed `reps` times between two events.  Every D x N operand is 512 MiB, far beyond the 50 MB L2,
+        so back-to-back replays read from HBM."""
+        g = B.GraphedCalls(fn)
+        g()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            g()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def report(name, t, nbytes):
+        gbs = nbytes / t / 1e6
+        print(f"{name}  D={D} N=2^20  {t:.4f} ms  {gbs:.0f} GB/s  ({gbs / 3350.0 * 100:.1f} % of the 3350 GB/s H100 data sheet)")
+
+    # (a) the elementwise-run kernel: Stacked(Logit rows | exp rows) + Permute + MvNormal(μ, σ), ȳ = NULL, l̄ = 1 -- one
+    # segment, so the call is the kernel plus the tiny fixed-order finalize of μ̄, σ̄
+    st = B.Stacked([B.Logit(0.0, 1.0), B.elementwise("exp")], [(1, D // 2), (D // 2 + 1, D)])
+    base = B.MvNormal(D, mu=(rng.standard_normal(D) * 0.1).astype(np.float32), sigma=rng.uniform(0.8, 1.2, D).astype(np.float32))
+    td = B.transformed(base, B.inverse(B.Composed(st, B.Permute((rng.permutation(D) + 1).tolist()))))
+    y = B.from_numpy(np.concatenate([rng.uniform(0.05, 0.95, (D // 2, N)), rng.standard_normal((D // 2, N))]).astype(np.float32))
+    ones = torch.ones(N, device="cuda")
+    report("(a) elementwise-run VJP kernel (Stacked + Permute + MvNormal, with μ̄, σ̄)", device_ms(lambda: B.logpdf_vjp(td, y, ones)),
+           4.0 * N * (2 * D + 1))
+    # (b) logpdf gradient of inverse(8 x Planar) + MvNormal: one chain_vjp call vs today's route, both as device time
+    flow = B.Composed(*[B.PlanarLayer((rng.standard_normal(D) / np.sqrt(D)).astype(np.float32),
+                                      (rng.standard_normal(D) / np.sqrt(D)).astype(np.float32),
+                                      rng.standard_normal(1).astype(np.float32)) for _ in range(L)])
+    tdp = B.transformed(B.MvNormal(D), flow)
+    yp = B.from_numpy(rng.standard_normal((D, N)).astype(np.float32))
+
+    def today():
+        x, _ = B.run_chain(B.inverse(flow), yp)  # the base density's cotangent is −x (torch)
+        B.planar_chain_vjp(B.inverse(flow), yp, (-x).t().contiguous().t(), ones)
+
+    ta, tb = [], []
+    for _ in range(3):
+        ta.append(device_ms(lambda: B.logpdf_vjp(tdp, yp, ones)))
+        tb.append(device_ms(today))
+    t_new, t_old = float(np.median(ta)), float(np.median(tb))
+    report("(b) logpdf gradient, chain_vjp (ȳ + parameter cotangents)", t_new, 4.0 * N * (2 * D + 1))
+    report("(b) logpdf gradient, planar_chain_vjp + torch base density", t_old, 4.0 * N * (2 * D + 1))
+    print(f"(b) ratio today / chain_vjp: {t_old / t_new:.3f}  (per-run medians: chain_vjp {ta}, today {tb})")
+
+
+if len(sys.argv) > 1 and sys.argv[1] == "chain":
+    bench_chain()
+    sys.exit(0)
 
 D, N, L = int(sys.argv[1]) if len(sys.argv) > 1 else 128, 1 << 20, int(sys.argv[2]) if len(sys.argv) > 2 else 8
 rng = np.random.default_rng(0)
