@@ -169,13 +169,51 @@ extern "C" size_t b2b_coupling_workspace_bytes(int32_t n1, int32_t n2) {
   return b ? align_up(b, 1024) + 1024 : 0;
 }
 
+// A launch of the chain: a run of fusable layers, or one coupling layer (with the BatchNorm neighbours folded into it).
+struct Seg {
+  int begin, end;
+  bool coupling;
+  int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
+};
+
+// Cuts the chain into launches before anything is enqueued: single coupling layers, and maximal runs of fusable layers
+// whose staged parameters fit one fused kernel (a run is ended before the layer that would cross the shared-memory budget,
+// so the terminal MvNormal stays in the last segment).  B2B_EUNSUPPORTED when one layer alone does not fit.
+static int plan_segments(const b2b_layer_desc* layers, int32_t L, int32_t D, std::vector<Seg>& segs) {
+  segs.clear();
+  for (int l = 0; l < L;) {
+    if (layers[l].kind == B2B_COUPLING_AFFINE) {
+      if (!b2b_coupling_affine_fits(layers[l].n0, layers[l].n1, D)) return B2B_EUNSUPPORTED;
+      segs.push_back({l, l + 1, true, -1, -1});
+      ++l;
+      continue;
+    }
+    int e = l;
+    while (e < L && fusable(layers[e].kind)) ++e;
+    for (int b = l; b < e;) {
+      if (b2b_chain_v0_smem_bytes(layers + b, 1, D) > B2B_V0_SMEM_MAX) return B2B_EUNSUPPORTED;
+      int k = b + 1;
+      while (k < e && b2b_chain_v0_smem_bytes(layers + b, k + 1 - b, D) <= B2B_V0_SMEM_MAX) ++k;
+      segs.push_back({b, k, false, -1, -1});
+      b = k;
+    }
+    l = e;
+  }
+  return B2B_OK;
+}
+
+int b2b_chain_segment_count(const b2b_layer_desc* layers, int32_t L, int32_t D) {
+  std::vector<Seg> segs;
+  const int rc = plan_segments(layers, L, D, segs);
+  return rc != B2B_OK ? rc : (int)segs.size();
+}
+
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
                                             int want_y, int want_sum) {
   size_t bytes = chain_tc_bytes(layers, L, D);
-  bool has_coupling = false;
-  for (int l = 0; l < L; ++l) has_coupling |= layers[l].kind == B2B_COUPLING_AFFINE;
   // a D x N scratch matrix is needed only when y == NULL but the chain has more than one segment
-  if (!want_y && has_coupling && L > 1) bytes += align_up((size_t)D * (size_t)N * sizeof(float), 1024);
+  if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
+    bytes += align_up((size_t)D * (size_t)N * sizeof(float), 1024);
   if (want_sum) bytes += 4096 * sizeof(double);
   return bytes;
 }
@@ -209,23 +247,10 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG;
   if (sum_out && !logjac && !terminal) return B2B_EINVAL;
 
-  // segments: maximal runs of fusable layers, and single coupling layers
-  struct Seg {
-    int begin, end;
-    bool coupling;
-    int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
-  };
   std::vector<Seg> segs;
-  for (int l = 0; l < L;) {
-    if (layers[l].kind == B2B_COUPLING_AFFINE) {
-      segs.push_back({l, l + 1, true, -1, -1});
-      ++l;
-    } else {
-      int e = l;
-      while (e < L && fusable(layers[e].kind)) ++e;
-      segs.push_back({l, e, false, -1, -1});
-      l = e;
-    }
+  {
+    const int rc = plan_segments(layers, L, D, segs);
+    if (rc != B2B_OK) return rc;
   }
   // workspace carve-up
   char* ws = static_cast<char*>(workspace);
@@ -662,7 +687,7 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
         s.kind = VK_RQS;
         break;
       case B2B_COUPLING_AFFINE:
-        if (layers[l].n0 > 128 || layers[l].n1 > 128) return B2B_EUNSUPPORTED;
+        if (!b2b_coupling_affine_vjp_fits(layers[l], D)) return B2B_EUNSUPPORTED;
         s.kind = VK_COUPLING;
         break;
       case B2B_BATCHNORM:
@@ -679,6 +704,13 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
     }
     segs.push_back(s);
     l = e;
+  }
+  // the forward recompute runs every segment but the last through b2b_chain_run_f32: it must accept them, so that the
+  // workspace query and the call refuse the same chains, before anything is launched
+  std::vector<Seg> fwd;
+  for (size_t k = 0; k + 1 < segs.size(); ++k) {
+    const int rc = plan_segments(layers + segs[k].begin, segs[k].end - segs[k].begin, D, fwd);
+    if (rc != B2B_OK) return rc;
   }
   return B2B_OK;
 }

@@ -415,6 +415,26 @@ struct V0Plan {
   bool ok;
 };
 
+constexpr int V0_BLOCK = 256;
+
+// Shared-memory layout of a v0 launch: every layer's derived parameters at padded depth Dp (soff[l], when given), then
+// the per-warp permute scratch (*scratch_off, -1 when no layer permutes).  Returns the floats staged.
+static size_t v0_layout(const b2b_layer_desc* layers, int L, int D, int* soff, int* scratch_off) {
+  const V0Config cfg = pick_config(D);
+  const int Dp = 4 * cfg.G * cfg.V;
+  const int cpw = (32 / cfg.G) * cfg.C;
+  size_t off = 0;
+  bool need_scratch = false;
+  for (int l = 0; l < L; ++l) {
+    if (soff) soff[l] = (int)off;
+    off += (b2b_layer_smem_floats(layers[l], Dp) + 3) & ~3;
+    if (layers[l].kind == B2B_PERMUTE) need_scratch = true;
+  }
+  if (scratch_off) *scratch_off = need_scratch ? (int)off : -1;
+  if (need_scratch) off += (size_t)(V0_BLOCK / 32) * cpw * Dp;
+  return off;
+}
+
 static int plan_v0(B2BChainParams& p, V0Plan& plan) {
   if (p.D < 1 || p.D > 1024) return B2B_EUNSUPPORTED;
   const V0Config cfg = pick_config(p.D);
@@ -423,21 +443,9 @@ static int plan_v0(B2BChainParams& p, V0Plan& plan) {
   const bool vec = (p.D % 4 == 0) && (p.ldx % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.x) & 15) == 0) &&
                    (!p.y || ((p.ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.y) & 15) == 0)));
   plan.kernel = vec ? pick_kernel<true>(cfg) : pick_kernel<false>(cfg);
-  plan.block = 256;
-  int off = 0;
-  bool need_scratch = false;
-  for (int l = 0; l < p.L; ++l) {
-    p.soff[l] = off;
-    off += (b2b_layer_smem_floats(p.layers[l], Dp) + 3) & ~3;
-    if (p.layers[l].kind == B2B_PERMUTE) need_scratch = true;
-  }
-  p.scratch_off = -1;
-  if (need_scratch) {
-    p.scratch_off = off;
-    off += (plan.block / 32) * cpw * Dp;
-  }
-  plan.smem = (size_t)off * sizeof(float);
-  if (plan.smem > 200 * 1024) return B2B_EUNSUPPORTED;
+  plan.block = V0_BLOCK;
+  plan.smem = v0_layout(p.layers, p.L, p.D, p.soff, &p.scratch_off) * sizeof(float);
+  if (plan.smem > B2B_V0_SMEM_MAX) return B2B_EUNSUPPORTED;
   plan.Dp = Dp;
   plan.cpw = cpw;
   cudaError_t e = cudaSuccess;
@@ -460,6 +468,11 @@ static int plan_v0(B2BChainParams& p, V0Plan& plan) {
 }
 
 }  // namespace b2b
+
+size_t b2b_chain_v0_smem_bytes(const b2b_layer_desc* layers, int L, int D) {
+  if (D < 1 || D > 1024) return SIZE_MAX;
+  return b2b::v0_layout(layers, L, D, nullptr, nullptr) * sizeof(float);
+}
 
 int b2b_chain_grid_size_v0(const B2BChainParams& p) {
   B2BChainParams q = p;

@@ -6,12 +6,14 @@
 //   inverse : x₁ = inv.(exp(s)) ⊙ (y₁ − t), logjac = −Σ_j s_j
 // x₂ (rows idx2) and x₃ (the remaining rows) pass through unchanged (combine, coupling.jl:125).
 //
-// A CTA owns a tile of TC columns.  The tile is transposed into shared memory ([row][col], padded) with
-// coalesced global reads, every thread computes a 4(j) x 2(s,t) x 2(col) register block of the
-// conditioner GEMM reading W through the read-only path (uniform addresses -> one sector per request,
-// W stays L1/L2 resident), the epilogue applies exp/FMA in place on the x₁ rows of the tile and the
-// tile is written back coalesced.  This is the exact-fp32 path; the tensor-core path (fp16-split wgmma)
-// lives in b2b_coupling_tc.cu and is cross-checked against this kernel.
+// A CTA owns a tile of TC columns.  The tile is transposed into shared memory ([row][col], padded), every thread
+// computes a 4(j) x 2(s,t) x 2(col) register block of the conditioner GEMM reading W through the read-only path (uniform
+// addresses -> one sector per request, W stays L1/L2 resident), the epilogue applies exp/FMA in place on the x₁ rows and
+// the tile is written back.  Two programs: coupling_affine_full_kernel stages all D rows (coalesced reads and writes of
+// whole columns) when they fit; coupling_affine_rows_kernel stages only the x₂ and x₁ rows and copies the pass-through
+// rows x₃ global to global (through the folded BatchNorm affines when there are any; skipped in place without them), so
+// its shared memory -- and the limit -- depends on n1 + n2 only, not on D.  This is the exact-fp32 path; the tensor-core
+// path (fp16-split wgmma) lives in b2b_coupling_tc.cu and is cross-checked against this kernel.
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -24,8 +26,78 @@ constexpr int CP_TC = 64;       // columns per tile
 constexpr int CP_LD = CP_TC + 1;  // padded row stride of the smem tile
 constexpr int CP_THREADS = 256;
 
+// Conditioner GEMM [s; t] = W·x₂ + c and the affine epilogue on x₁, in place in shared memory, for one 64-column tile;
+// leaves the column sums of s of this warp in red[warp][*].  The two programs stage rows differently: x₂ row k lives at
+// X2 + row2(k)·CP_LD, x₁ row j at X1 + row1(j)·CP_LD.
+template <bool INV, class Row2, class Row1>
+__device__ __forceinline__ void coupling_tile(const float* X2, float* X1, Row2 row2, Row1 row1, const float* __restrict__ W,
+                                              const float* __restrict__ cvec, int n1, int n2, bool wvec, float* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int ldw = 2 * n1;
+  const int cA = lane, cB = lane + 32;
+  float sumA = 0.f, sumB = 0.f;
+  for (int jb = 4 * warp; jb < n1; jb += 4 * (CP_THREADS / 32)) {
+    float sA[4] = {0.f, 0.f, 0.f, 0.f}, sB[4] = {0.f, 0.f, 0.f, 0.f};
+    float tA[4] = {0.f, 0.f, 0.f, 0.f}, tB[4] = {0.f, 0.f, 0.f, 0.f};
+    if (wvec) {
+#pragma unroll 4
+      for (int k = 0; k < n2; ++k) {
+        const int r2 = row2(k);
+        const float xa = X2[r2 * CP_LD + cA], xb = X2[r2 * CP_LD + cB];
+        const float4 ws = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + jb));
+        const float4 wt = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + n1 + jb));
+        sA[0] = fmaf(ws.x, xa, sA[0]); sB[0] = fmaf(ws.x, xb, sB[0]);
+        sA[1] = fmaf(ws.y, xa, sA[1]); sB[1] = fmaf(ws.y, xb, sB[1]);
+        sA[2] = fmaf(ws.z, xa, sA[2]); sB[2] = fmaf(ws.z, xb, sB[2]);
+        sA[3] = fmaf(ws.w, xa, sA[3]); sB[3] = fmaf(ws.w, xb, sB[3]);
+        tA[0] = fmaf(wt.x, xa, tA[0]); tB[0] = fmaf(wt.x, xb, tB[0]);
+        tA[1] = fmaf(wt.y, xa, tA[1]); tB[1] = fmaf(wt.y, xb, tB[1]);
+        tA[2] = fmaf(wt.z, xa, tA[2]); tB[2] = fmaf(wt.z, xb, tB[2]);
+        tA[3] = fmaf(wt.w, xa, tA[3]); tB[3] = fmaf(wt.w, xb, tB[3]);
+      }
+    } else {
+      for (int k = 0; k < n2; ++k) {
+        const int r2 = row2(k);
+        const float xa = X2[r2 * CP_LD + cA], xb = X2[r2 * CP_LD + cB];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          if (jb + q < n1) {
+            const float ws = __ldg(W + (size_t)k * ldw + jb + q);
+            const float wt = __ldg(W + (size_t)k * ldw + n1 + jb + q);
+            sA[q] = fmaf(ws, xa, sA[q]); sB[q] = fmaf(ws, xb, sB[q]);
+            tA[q] = fmaf(wt, xa, tA[q]); tB[q] = fmaf(wt, xb, tB[q]);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int j = jb + q;
+      if (j < n1) {
+        const float cs = cvec ? __ldg(cvec + j) : 0.f, ct = cvec ? __ldg(cvec + n1 + j) : 0.f;
+        const int r1 = row1(j);
+        const float s_a = sA[q] + cs, s_b = sB[q] + cs, t_a = tA[q] + ct, t_b = tB[q] + ct;
+        const float xa = X1[r1 * CP_LD + cA], xb = X1[r1 * CP_LD + cB];
+        if (!INV) {
+          X1[r1 * CP_LD + cA] = fmaf(expf(s_a), xa, t_a);  // exp(s)·x₁ + t  (scale.jl:13, shift.jl:14)
+          X1[r1 * CP_LD + cB] = fmaf(expf(s_b), xb, t_b);
+        } else {
+          X1[r1 * CP_LD + cA] = (xa - t_a) / expf(s_a);  // inv.(a) .* (y₁ + (−t))  (scale.jl:16, shift.jl:12)
+          X1[r1 * CP_LD + cB] = (xb - t_b) / expf(s_b);
+        }
+        sumA += s_a;
+        sumB += s_b;
+      }
+    }
+  }
+  red[warp * CP_TC + cA] = sumA;
+  red[warp * CP_TC + cB] = sumB;
+}
+
+// Layers whose D rows fit shared memory (D <= 777 at n2 = 128) stage the whole tile: every row is read and written
+// coalesced, column by column.
 template <bool INV>
-__global__ void __launch_bounds__(CP_THREADS) coupling_affine_kernel(
+__global__ void __launch_bounds__(CP_THREADS) coupling_affine_full_kernel(
     const float* __restrict__ x, float* __restrict__ y, float* __restrict__ logjac,
     const int32_t* __restrict__ idx1, const int32_t* __restrict__ idx2, const float* __restrict__ W,
     const float* __restrict__ cvec, const float* __restrict__ fold, int D, int n1, int n2, int row1, int row2,
@@ -38,7 +110,6 @@ __global__ void __launch_bounds__(CP_THREADS) coupling_affine_kernel(
   for (int k = threadIdx.x; k < n2; k += CP_THREADS) sidx2[k] = idx2 ? idx2[k] : row2 + k;
   const bool wvec = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
   const long long tiles = (N + CP_TC - 1) / CP_TC;
-  const int ldw = 2 * n1;
 
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const long long col0 = tile * CP_TC;
@@ -59,64 +130,8 @@ __global__ void __launch_bounds__(CP_THREADS) coupling_affine_kernel(
     }
     __syncthreads();
     // ---- conditioner GEMM + epilogue -------------------------------------------------------------
-    const int cA = lane, cB = lane + 32;
-    float sumA = 0.f, sumB = 0.f;
-    for (int jb = 4 * warp; jb < n1; jb += 4 * (CP_THREADS / 32)) {
-      float sA[4] = {0.f, 0.f, 0.f, 0.f}, sB[4] = {0.f, 0.f, 0.f, 0.f};
-      float tA[4] = {0.f, 0.f, 0.f, 0.f}, tB[4] = {0.f, 0.f, 0.f, 0.f};
-      if (wvec) {
-#pragma unroll 4
-        for (int k = 0; k < n2; ++k) {
-          const int r2 = sidx2[k];
-          const float xa = X[r2 * CP_LD + cA], xb = X[r2 * CP_LD + cB];
-          const float4 ws = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + jb));
-          const float4 wt = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + n1 + jb));
-          sA[0] = fmaf(ws.x, xa, sA[0]); sB[0] = fmaf(ws.x, xb, sB[0]);
-          sA[1] = fmaf(ws.y, xa, sA[1]); sB[1] = fmaf(ws.y, xb, sB[1]);
-          sA[2] = fmaf(ws.z, xa, sA[2]); sB[2] = fmaf(ws.z, xb, sB[2]);
-          sA[3] = fmaf(ws.w, xa, sA[3]); sB[3] = fmaf(ws.w, xb, sB[3]);
-          tA[0] = fmaf(wt.x, xa, tA[0]); tB[0] = fmaf(wt.x, xb, tB[0]);
-          tA[1] = fmaf(wt.y, xa, tA[1]); tB[1] = fmaf(wt.y, xb, tB[1]);
-          tA[2] = fmaf(wt.z, xa, tA[2]); tB[2] = fmaf(wt.z, xb, tB[2]);
-          tA[3] = fmaf(wt.w, xa, tA[3]); tB[3] = fmaf(wt.w, xb, tB[3]);
-        }
-      } else {
-        for (int k = 0; k < n2; ++k) {
-          const int r2 = sidx2[k];
-          const float xa = X[r2 * CP_LD + cA], xb = X[r2 * CP_LD + cB];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (jb + q < n1) {
-              const float ws = __ldg(W + (size_t)k * ldw + jb + q);
-              const float wt = __ldg(W + (size_t)k * ldw + n1 + jb + q);
-              sA[q] = fmaf(ws, xa, sA[q]); sB[q] = fmaf(ws, xb, sB[q]);
-              tA[q] = fmaf(wt, xa, tA[q]); tB[q] = fmaf(wt, xb, tB[q]);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int j = jb + q;
-        if (j < n1) {
-          const float cs = cvec ? __ldg(cvec + j) : 0.f, ct = cvec ? __ldg(cvec + n1 + j) : 0.f;
-          const int r1 = idx1 ? __ldg(idx1 + j) : row1 + j;
-          const float s_a = sA[q] + cs, s_b = sB[q] + cs, t_a = tA[q] + ct, t_b = tB[q] + ct;
-          const float xa = X[r1 * CP_LD + cA], xb = X[r1 * CP_LD + cB];
-          if (!INV) {
-            X[r1 * CP_LD + cA] = fmaf(expf(s_a), xa, t_a);  // exp(s)·x₁ + t  (scale.jl:13, shift.jl:14)
-            X[r1 * CP_LD + cB] = fmaf(expf(s_b), xb, t_b);
-          } else {
-            X[r1 * CP_LD + cA] = (xa - t_a) / expf(s_a);  // inv.(a) .* (y₁ + (−t))  (scale.jl:16, shift.jl:12)
-            X[r1 * CP_LD + cB] = (xb - t_b) / expf(s_b);
-          }
-          sumA += s_a;
-          sumB += s_b;
-        }
-      }
-    }
-    red[warp * CP_TC + cA] = sumA;
-    red[warp * CP_TC + cB] = sumB;
+    coupling_tile<INV>(X, X, [&](int k) { return sidx2[k]; }, [&](int j) { return idx1 ? __ldg(idx1 + j) : row1 + j; },
+                       W, cvec, n1, n2, wvec, red);
     __syncthreads();
     // ---- write back --------------------------------------------------------------------------------
     if (y) {
@@ -128,6 +143,110 @@ __global__ void __launch_bounds__(CP_THREADS) coupling_affine_kernel(
             for (int r = lane; r < D; r += 32) __stcs(yc + r, fmaf(X[r * CP_LD + c], fold[2 * D + r], fold[3 * D + r]));
           } else {
             for (int r = lane; r < D; r += 32) __stcs(yc + r, X[r * CP_LD + c]);
+          }
+        }
+      }
+    }
+    if (logjac && threadIdx.x < CP_TC) {
+      const long long col = col0 + threadIdx.x;
+      if (col < N) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < CP_THREADS / 32; ++w) s += red[w * CP_TC + threadIdx.x];
+        const float base = (accumulate ? logjac[col] : 0.f) + (fold ? fold[4 * D] : 0.f);
+        logjac[col] = INV ? base - s : base + s;  // Σ log|exp(s)| = Σ s  (scale.jl:31)
+      }
+    }
+  }
+}
+
+// Wider layers stage only the rows they read.  Three CTAs per SM leave 85 registers per thread: no spills.
+template <bool INV>
+__global__ void __launch_bounds__(CP_THREADS, 3) coupling_affine_rows_kernel(
+    const float* __restrict__ x, float* __restrict__ y, float* __restrict__ logjac,
+    const int32_t* __restrict__ idx1, const int32_t* __restrict__ idx2, const float* __restrict__ W,
+    const float* __restrict__ cvec, const float* __restrict__ fold, int D, int n1, int n2, int row1, int row2,
+    long long N, long long ldx, long long ldy, int accumulate) {
+  // x and y may alias (in place): every element is read before it is written, by the same CTA
+  extern __shared__ float smem[];
+  float* X2 = smem;                                      // [n2][CP_LD]  conditioner input x₂ (folded)
+  float* X1 = X2 + (size_t)n2 * CP_LD;                   // [n1][CP_LD]  x₁ (folded), transformed in place
+  float* red = X1 + (size_t)n1 * CP_LD;                  // [8][CP_TC]
+  int* sidx2 = reinterpret_cast<int*>(red + 8 * CP_TC);  // [n2]
+  int* sidx1 = sidx2 + n2;                               // [n1]
+  unsigned* coupled = reinterpret_cast<unsigned*>(sidx1 + n1);  // [ceil(D/32)] bit r: row r is in idx1 or idx2
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // pass-through rows exist when the two index lists do not cover the column; without a fold an in-place call leaves
+  // them (and x₂) where they are
+  const bool has_x3 = n1 + n2 < D;
+  const bool copy_through = y && (fold || y != x);
+  const int nwords = (D + 31) >> 5;
+  if (has_x3 && copy_through)
+    for (int k = threadIdx.x; k < nwords; k += CP_THREADS) coupled[k] = 0u;
+  for (int k = threadIdx.x; k < n2; k += CP_THREADS) sidx2[k] = idx2 ? idx2[k] : row2 + k;
+  for (int k = threadIdx.x; k < n1; k += CP_THREADS) sidx1[k] = idx1 ? idx1[k] : row1 + k;
+  __syncthreads();
+  if (has_x3 && copy_through) {
+    for (int k = threadIdx.x; k < n2; k += CP_THREADS) atomicOr(&coupled[sidx2[k] >> 5], 1u << (sidx2[k] & 31));
+    for (int k = threadIdx.x; k < n1; k += CP_THREADS) atomicOr(&coupled[sidx1[k] >> 5], 1u << (sidx1[k] & 31));
+  }
+  const bool wvec = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
+  const long long tiles = (N + CP_TC - 1) / CP_TC;
+
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long col0 = tile * CP_TC;
+    __syncthreads();  // previous tile fully written back / index tables visible
+    // ---- load + transpose x₂ and x₁; pass-through rows go straight to y ---------------------------------------
+    for (int c = warp; c < CP_TC; c += CP_THREADS / 32) {
+      const long long col = col0 + c;
+      if (col < N) {
+        const float* xc = x + col * ldx;
+        if (fold) {
+          for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = fmaf(__ldcs(xc + sidx2[k]), fold[sidx2[k]], fold[D + sidx2[k]]);
+          if (y)  // the log-Jacobian needs x₂ only
+            for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = fmaf(__ldcs(xc + sidx1[k]), fold[sidx1[k]], fold[D + sidx1[k]]);
+        } else {
+          for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = __ldcs(xc + sidx2[k]);
+          if (y)
+            for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = __ldcs(xc + sidx1[k]);
+        }
+        if (has_x3 && copy_through) {
+          float* yc = y + col * ldy;
+          for (int r = lane; r < D; r += 32) {
+            if ((coupled[r >> 5] >> (r & 31)) & 1u) continue;
+            const float v = __ldcs(xc + r);
+            // pre- then post-BatchNorm affine: exactly what the rows would get had they been staged
+            __stcs(yc + r, fold ? fmaf(fmaf(v, fold[r], fold[D + r]), fold[2 * D + r], fold[3 * D + r]) : v);
+          }
+        }
+      } else {
+        for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = 0.f;
+        for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = 0.f;
+      }
+    }
+    __syncthreads();
+    // ---- conditioner GEMM + epilogue -------------------------------------------------------------
+    coupling_tile<INV>(X2, X1, [](int k) { return k; }, [](int j) { return j; }, W, cvec, n1, n2, wvec, red);
+    __syncthreads();
+    // ---- write back x₁ (and x₂ unless it is already in place) ---------------------------------------------------------
+    if (y) {
+      for (int c = warp; c < CP_TC; c += CP_THREADS / 32) {
+        const long long col = col0 + c;
+        if (col < N) {
+          float* yc = y + col * ldy;
+          if (fold) {
+            for (int k = lane; k < n1; k += 32) {
+              const int r = sidx1[k];
+              __stcs(yc + r, fmaf(X1[k * CP_LD + c], fold[2 * D + r], fold[3 * D + r]));
+            }
+            for (int k = lane; k < n2; k += 32) {
+              const int r = sidx2[k];
+              __stcs(yc + r, fmaf(X2[k * CP_LD + c], fold[2 * D + r], fold[3 * D + r]));
+            }
+          } else {
+            for (int k = lane; k < n1; k += 32) __stcs(yc + sidx1[k], X1[k * CP_LD + c]);
+            if (copy_through)
+              for (int k = lane; k < n2; k += 32) __stcs(yc + sidx2[k], X2[k * CP_LD + c]);
           }
         }
       }
@@ -184,7 +303,17 @@ __global__ void __launch_bounds__(256) bn_fold_prep_kernel(b2b_layer_desc pre, i
   }
 }
 
+// coupling_affine_rows_kernel: x₂ and x₁ tiles, the column-sum slab, both index tables and the coupled-row bitmap
+static size_t coupling_smem_bytes(int n1, int n2, int D) {
+  return ((size_t)(n1 + n2) * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int) +
+         (size_t)((D + 31) / 32) * sizeof(unsigned);
+}
+
 }  // namespace b2b
+
+bool b2b_coupling_affine_fits(int n1, int n2, int D) {
+  return b2b::coupling_smem_bytes(n1, n2, D) <= 200 * 1024;
+}
 
 int b2b_launch_bn_fold_prep(const b2b_layer_desc* pre, const b2b_layer_desc* post, int D, float* out,
                             cudaStream_t stream) {
@@ -201,9 +330,12 @@ int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const
   const int n1 = d.n0, n2 = d.n1;
   if (n1 < 1 || n2 < 1 || n1 + n2 > D || !d.p0) return B2B_EINVAL;
   if ((!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-  const size_t smem = ((size_t)D * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)n2 * sizeof(int);
-  if (smem > 200 * 1024) return B2B_EUNSUPPORTED;
-  auto kern = d.inverse ? coupling_affine_kernel<true> : coupling_affine_kernel<false>;
+  if (!b2b_coupling_affine_fits(n1, n2, D)) return B2B_EUNSUPPORTED;
+  const size_t smem_full = ((size_t)D * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)n2 * sizeof(int);
+  const bool full = smem_full <= 200 * 1024;
+  const size_t smem = full ? smem_full : coupling_smem_bytes(n1, n2, D);
+  auto kern = full ? (d.inverse ? coupling_affine_full_kernel<true> : coupling_affine_full_kernel<false>)
+                   : (d.inverse ? coupling_affine_rows_kernel<true> : coupling_affine_rows_kernel<false>);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   int dev = 0, sms = 0, per_sm = 0;

@@ -586,6 +586,18 @@ __global__ void __launch_bounds__(256) bn_vjp_finalize_kernel(const float* __res
   }
 }
 
+// float4 path: n1, n2 multiples of 4 and a 16-byte aligned W (its leading dimension 2·n1 is then a multiple of 4 too)
+static bool vjp_fast(const b2b_layer_desc& d) {
+  return d.n0 % 4 == 0 && d.n1 % 4 == 0 && (reinterpret_cast<uintptr_t>(d.p0) & 15) == 0;
+}
+
+// both programs stage the layer's input and output cotangent tiles over all D rows
+static size_t vjp_smem_bytes(const b2b_layer_desc& d, int D) {
+  const int n1 = d.n0, n2 = d.n1;
+  return vjp_fast(d) ? ((size_t)(2 * D + 1 + ((2 * n1 + 31) & ~31)) * CF_LD + CV_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int)
+                     : ((size_t)2 * D * CV_LD + (size_t)2 * n1 * CV_LD + CV_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int);
+}
+
 static int sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
@@ -594,6 +606,10 @@ static int sm_count() {
 }
 
 }  // namespace b2b
+
+bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D) {
+  return d.n0 <= 128 && d.n1 <= 128 && b2b::vjp_smem_bytes(d, D) <= 220 * 1024;
+}
 
 extern "C" size_t b2b_coupling_affine_vjp_workspace_bytes(int32_t n1, int32_t n2) {
   if (n1 < 1 || n1 > 128 || n2 < 1 || n2 > 128) return 0;
@@ -610,7 +626,7 @@ extern "C" int b2b_coupling_affine_vjp_f32(const b2b_layer_desc* layer, const fl
   const b2b_layer_desc& d = *layer;
   const int n1 = d.n0, n2 = d.n1;
   if (!d.p0 || n1 < 1 || n2 < 1 || n1 + n2 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-  if (n1 > 128 || n2 > 128) return B2B_EUNSUPPORTED;
+  if (!b2b_coupling_affine_vjp_fits(d, D)) return B2B_EUNSUPPORTED;
   if (N == 0) {
     cudaMemsetAsync(Wbar, 0, sizeof(float) * (size_t)2 * n1 * n2, stream);
     return (int)cudaMemsetAsync(cbar, 0, sizeof(float) * 2 * n1, stream);
@@ -642,11 +658,8 @@ extern "C" int b2b_coupling_affine_vjp_f32(const b2b_layer_desc* layer, const fl
   const long long tiles = (N + CV_TC - 1) / CV_TC;
   long long grid = sm_count();
   if (grid > tiles) grid = tiles;
-  // float4 path: n1, n2 multiples of 4 and a 16-byte aligned W (its leading dimension 2·n1 is then a multiple of 4 too)
-  const bool fast = n1 % 4 == 0 && n2 % 4 == 0 && (reinterpret_cast<uintptr_t>(d.p0) & 15) == 0;
-  const size_t smem = fast ? ((size_t)(2 * D + 1 + ((2 * n1 + 31) & ~31)) * CF_LD + CV_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int)
-                           : ((size_t)2 * D * CV_LD + (size_t)2 * n1 * CV_LD + CV_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int);
-  if (smem > 220 * 1024) return B2B_EUNSUPPORTED;
+  const bool fast = vjp_fast(d);
+  const size_t smem = vjp_smem_bytes(d, D);
   void (*kernel)(const CvParams);
   if (!fast) kernel = d.inverse ? coupling_vjp_kernel<true> : coupling_vjp_kernel<false>;
   else if (d.n3 < 0) kernel = d.inverse ? coupling_vjp_fast_kernel<true, false> : coupling_vjp_fast_kernel<false, false>;

@@ -189,8 +189,11 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
     c->hsum_cap = nchunks;
   }
   int launches = 0;
-  bool has_coupling = false;
-  for (int l = 0; l < L; ++l) has_coupling |= layers[l].kind == B2B_COUPLING_AFFINE;
+  // a logjac-only call still needs the D x N intermediate when the chain runs as several launches (a coupling layer, or
+  // a run of layers split at the fused kernels' shared-memory budget): the staging buffer doubles as that scratch
+  const int nseg = b2b_chain_segment_count(layers, L, D);
+  if (nseg < 0) return nseg;
+  const bool stage_y = y_host != nullptr || nseg > 1;
   for (long long k = 0; k < nchunks; ++k) {
     const int s = (int)(k % c->n_streams);
     cudaStream_t st = c->streams[s];
@@ -200,9 +203,7 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
                                     cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) return (int)e;
     const bool want_lj = logjac_host != nullptr || (sum_host && layers[L - 1].kind != B2B_MVNORMAL_DIAG);
-    // in place; a logjac-only call still needs the D x N intermediate when the chain has several segments (a
-    // coupling layer splits it), so the staging buffer doubles as that scratch
-    const int rc = b2b_chain_run_f32(layers, L, c->dx[s], (y_host || has_coupling) ? c->dx[s] : nullptr,
+    const int rc = b2b_chain_run_f32(layers, L, c->dx[s], stage_y ? c->dx[s] : nullptr,  // in place
                                      (want_lj || layers[L - 1].kind == B2B_MVNORMAL_DIAG) ? c->dlj[s] : nullptr,
                                      sum_host ? c->dsum[s] : nullptr, D, n, D, D, 0, c->dws[s], kWsBytes, st);
     if (rc != B2B_OK) return rc;

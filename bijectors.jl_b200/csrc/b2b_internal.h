@@ -51,8 +51,17 @@ static inline int b2b_layer_smem_floats(const b2b_layer_desc& d, int Dp) {
 }
 
 // ---- launchers (each returns a cudaError_t as int, or a negative B2B_E* code) ---------------------
-// v0: lane-group direct-global fused interpreter (any D <= 1024)
+// v0: lane-group direct-global fused interpreter (any D <= 1024 whose staged parameters fit B2B_V0_SMEM_MAX)
 int b2b_launch_chain_v0(const B2BChainParams& p, cudaStream_t stream);
+// Dynamic shared memory v0 stages for the fused run layers[0..L) at D (SIZE_MAX when D is out of range).  Every other
+// fused kernel stages at least as much for the runs it accepts, so a run within B2B_V0_SMEM_MAX always has a kernel:
+// the chain orchestrator ends a fused segment before the layer that would cross the budget.
+#define B2B_V0_SMEM_MAX (200 * 1024)
+size_t b2b_chain_v0_smem_bytes(const b2b_layer_desc* layers, int L, int D);
+// Launch segments b2b_chain_run_f32 cuts a chain into (before BatchNorm neighbours are folded into coupling launches), or
+// a negative B2B_E* code when a layer fits no kernel.  With y == NULL a chain of more than one segment needs a D x N
+// intermediate between them (b2b_api.cu).
+int b2b_chain_segment_count(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // v1: TMA-staged thread-per-column fused interpreter (D in {32,64,128}); returns B2B_EUNSUPPORTED otherwise
 int b2b_launch_chain_v1(const B2BChainParams& p, cudaStream_t stream);
 // fused planar chains (b2b_planar_const.cu).  hostparams: `L` in 1..8 layers, derived parameters packed
@@ -80,6 +89,9 @@ size_t b2b_planar_vjp_workspace(int L, int D, long long N);
 int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
                                 float* xbar, long long ldxb, float* wbar, float* ubar, float* bbar, void* workspace,
                                 size_t workspace_bytes, int* launches, cudaStream_t stream);
+// reverse mode of one affine coupling layer (b2b_coupling_vjp.cu): whether its kernel takes the layer at D (n1, n2 <= 128
+// and the D-row input / cotangent tiles within shared memory: D <= 747 at n1 = n2 = 128)
+bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D);
 // reverse mode of an elementwise run (b2b_ew_vjp.cu): <= 8 STACKED_EW / PERMUTE layers, optionally closed by the terminal
 // MVNORMAL_DIAG.  ybar, ljbar may be NULL (zeros); mubar / sigmabar (D, or NULL) need b2b_ew_vjp_workspace(D, 1) bytes.
 size_t b2b_ew_vjp_workspace(int D, int want_mvn_params);
@@ -101,7 +113,9 @@ int b2b_launch_coupling_affine_tc(const b2b_layer_desc& d, const float* fold, co
                                   void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 int b2b_launch_bn_fold_prep(const b2b_layer_desc* pre, const b2b_layer_desc* post, int D, float* out,
                             cudaStream_t stream);
-// affine coupling, exact-fp32 CUDA-core kernel (any index lists)
+// affine coupling, exact-fp32 CUDA-core kernel (any index lists; it stages the n1 + n2 rows it reads, so the limit is
+// b2b_coupling_affine_fits, independent of D and N)
+bool b2b_coupling_affine_fits(int n1, int n2, int D);
 int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const float* x, float* y,
                                float* logjac, int D, long long N, long long ldx, long long ldy, int accumulate,
                                cudaStream_t stream);

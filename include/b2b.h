@@ -120,6 +120,16 @@ const char* b2b_status_string(int status);
  * Consecutive column-local layers are fused into ONE kernel launch (each column is read once and
  * written once for the whole fused run); COUPLING_AFFINE layers run in their own GEMM kernel, which also
  * absorbs a BATCHNORM layer directly before and/or after it as a per-row affine (needs workspace).
+ * Limits.  Column-local layers need D <= 1024.  A fused launch stages the derived parameters of its layers in
+ * 200 KB of shared memory, in floats at the padded depth Dp = D rounded up to 32, 64, 128, 256, 512 or 1024:
+ * PLANAR 2Dp+4, RADIAL Dp+4, BATCHNORM 4Dp+4, STACKED_EW 3Dp, MVNORMAL_DIAG 2Dp+4, PERMUTE Dp (plus, once per launch
+ * that permutes, 8192 floats of column scratch), RQS (2·KP + 8·K1)·Dp with KP = K1 rounded up
+ * to a power of two -- so an RQS layer takes K1 <= 64 knots for D <= 64, K1 <= 34 for D <= 128, K1 <= 17 for D <= 256,
+ * K1 <= 8 for D <= 512 and K1 <= 4 for D <= 1024 (the default K = 8 bins, K1 = 9, up to D = 256).  A run of column-local
+ * layers that does not fit is split into several launches (the terminal MVNORMAL_DIAG stays in the last one).
+ * COUPLING_AFFINE takes any N, and any D while 264·(n1 + n2) + 4·ceil(D/32) + 2048 <= 204800 bytes (the rows it stages
+ * and a bit per row); up to D = 1024 that is n1 + n2 <= 767.  The whole chain is planned before anything is enqueued: a
+ * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
  * accumulated logjac (transformed_distribution.jl:165-169 when the preceding layers are the inverse
  * chain) and, when sum_out != NULL, *sum_out (device double) receives Σ_n logpdf[n] (fixed summation
@@ -135,7 +145,8 @@ size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_
 /* Workspace of ONE operation (SURVEY §8(b) `b2b_workspace_bytes(op, D, N)`): what b2b_chain_workspace_bytes returns for
  * the one-element chain {*op} with the D x N store and without the batch sum.  The specialised queries below
  * (b2b_coupling_workspace_bytes, b2b_batchnorm_train_workspace_bytes, b2b_*_vjp_workspace_bytes) remain for entry
- * points that are not chain elements. */
+ * points that are not chain elements.  With y == NULL a chain of several launches (a coupling layer, or a split run)
+ * needs a D x N scratch matrix, which is included. */
 size_t b2b_workspace_bytes(const b2b_layer_desc* op, int32_t D, int64_t N);
 
 /* Number of kernel launches the previous b2b_chain_run_f32 call on this thread enqueued. */
@@ -203,7 +214,8 @@ int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const floa
 /* Reverse mode of ONE affine coupling layer (either direction) -- with the eval-mode BatchNorm VJP below it makes a
  * RealNVP flow (BASELINE config 5) trainable on the device.  What the reference's AD computes for coupling.jl:206-228
  * with the law Shift(t)∘Scale(exp.(s)); the pullback of `combine` (ext/BijectorsChainRulesCoreExt.jl:48-62) is the row
- * scatter of the three cotangent blocks.  `layer`: a B2B_COUPLING_AFFINE descriptor (n1, n2 <= 128, any index lists);
+ * scatter of the three cotangent blocks.  `layer`: a B2B_COUPLING_AFFINE descriptor (n1, n2 <= 128, any index lists;
+ * the kernel stages all D rows of the input and the cotangent: D <= 747 at n1 = n2 = 128, else B2B_EUNSUPPORTED);
  * `x`: the batch the layer was applied to (for inverse != 0 the observed y); `ybar` (D x N) / `ljbar` (N, NULL = zeros):
  * cotangents of the layer's two outputs.  Outputs: `xbar` (D x N; may alias `ybar`), `Wbar` (2n1 x n2, column-major like
  * W) and `cbar` (2n1), summed over the N columns (a multi-GPU caller all-reduces them).  Exact fp32 on the CUDA cores,
@@ -248,7 +260,9 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
  * differentiates.  The forward is recomputed once to checkpoint each segment's input, then the segments are
  * differentiated last to first.  Limits are the kernels': planar and radial D <= 128, RQS D <= 256 and K1 <= 64, coupling
- * n1, n2 <= 128, BatchNorm and elementwise runs D <= 1024 (else B2B_EUNSUPPORTED).  N == 0 zeroes the requested parameter
+ * n1, n2 <= 128 and D <= 747 at n1 = n2 = 128 (see b2b_coupling_affine_vjp_f32), BatchNorm and elementwise runs D <= 1024,
+ * and the forward recompute those of b2b_chain_run_f32; an unsupported chain returns B2B_EUNSUPPORTED before anything
+ * is launched.  N == 0 zeroes the requested parameter
  * cotangents.  Launch-only on `stream`, no allocation (CUDA-graph capturable).  workspace: b2b_chain_vjp_workspace_bytes
  * (0 = unsupported chain); b2b_last_launch_count counts every kernel, copy and fill enqueued. */
 size_t b2b_chain_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N);

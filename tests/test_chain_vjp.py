@@ -123,7 +123,7 @@ def check_chain(B, dev_t, olayers, flags, x, ybar, ljbar, mu=None, sigma=None, b
 
 
 # ---- 1. the elementwise-run kernel --------------------------------------------------------------------------------------
-@pytest.mark.parametrize("D,N", [(3, 7), (10, 333), (32, 1000), (128, 515), (200, 129)])
+@pytest.mark.parametrize("D,N", [(3, 7), (10, 333), (32, 1000), (128, 515), (200, 129), (257, 65), (1024, 33)])
 @pytest.mark.parametrize("inverse", [False, True])
 @pytest.mark.parametrize("law", list(LAWS))
 def test_stacked_law_vjp(B, law, inverse, D, N):

@@ -45,6 +45,12 @@ def B():
 f32 = np.float32
 
 
+def rqs_bins(D):
+    """The largest RQS bin count K whose knot tables (K1 = K + 1) fit the fused kernels' shared memory at D (include/b2b.h):
+    the default K = 8 up to D = 256, K1 <= 8 up to D = 512, K1 <= 4 up to D = 1024."""
+    return 8 if D <= 256 else 7 if D <= 512 else 3
+
+
 def make_case(kind, D, rng):
     """(device layer, oracle layer) with float32 parameters."""
     import bijectors_jl_b200 as B
@@ -59,7 +65,7 @@ def make_case(kind, D, rng):
         a, be, z0 = rng.standard_normal(1).astype(f32), rng.standard_normal(1).astype(f32), rng.standard_normal(D).astype(f32)
         return B.RadialLayer(a, be, z0), O.Layer("radial", dict(alpha_raw=a, beta=be, z0=z0))
     if kind == "rqs":
-        K, Bx = 8, 3.0
+        K, Bx = rqs_bins(D), 3.0
         rw, rh, rd = rng.standard_normal((D, K)).astype(f32), rng.standard_normal((D, K)).astype(f32), rng.standard_normal((D, K - 1)).astype(f32)
         lay = B.RationalQuadraticSpline(rw, rh, rd, Bx)
         W, H, Dv = lay.knots()
@@ -77,6 +83,10 @@ def make_case(kind, D, rng):
         mask_first = rng.integers(0, 2) == 0
         idx1 = list(range(1, n1 + 1)) if mask_first else list(range(D - n1 + 1, D + 1))
         idx2 = [i for i in range(1, D + 1) if i not in set(idx1)]
+        if D > 256:  # wide batches: 128-row halves next to each other, the other D - 256 rows pass through (x₃)
+            n1 = 128
+            idx1 = list(range(1, 129)) if mask_first else list(range(D - 127, D + 1))
+            idx2 = list(range(129, 257)) if mask_first else list(range(D - 255, D - 127))
         W = (rng.standard_normal((2 * n1, len(idx2))) * 0.2 / np.sqrt(len(idx2))).astype(f32)
         c = (rng.standard_normal(2 * n1) * 0.1).astype(f32)
         return (B.Coupling(B.AffineConditioner(W, c), B.PartitionMask(D, idx1, idx2)),
@@ -103,7 +113,9 @@ def make_case(kind, D, rng):
 KINDS = ["planar", "planar_randn", "radial", "rqs", "batchnorm", "permute", "coupling", "stacked", "leaky_relu", "bounded"]
 
 
-@pytest.mark.parametrize("D,N", [(128, 1000), (64, 517), (32, 2049), (256, 300), (10, 100), (3, 7), (36, 65), (200, 33)])
+@pytest.mark.parametrize("D,N", [(128, 1000), (64, 517), (32, 2049), (256, 300), (10, 100), (3, 7), (36, 65), (200, 33),
+                                 (257, 4097), (260, 3), (384, 2), (509, 1), (512, 4097), (513, 3), (768, 2), (1000, 4097),
+                                 (1021, 1), (1024, 4097)])
 @pytest.mark.parametrize("kind", KINDS)
 def test_layer_forward_inverse_parity(B, kind, D, N):
     if kind in ("coupling", "stacked") and D < 3:
@@ -159,7 +171,7 @@ def test_layer_forward_inverse_parity(B, kind, D, N):
         assert rel(xih, x) <= rel(xo, x) + gate(xo32, xo), (rel(xih, x), rel(xo, x))
 
 
-@pytest.mark.parametrize("D", [128, 64, 32, 256, 10])
+@pytest.mark.parametrize("D", [128, 64, 32, 256, 10, 384, 1000, 1024])
 def test_fused_chain_matches_layerwise_and_oracle(B, D):
     rng = np.random.default_rng(D)
     N = 1537
@@ -449,7 +461,7 @@ def make_case64(kind, D, rng):
     return lay, olay  # permute: no floating-point parameters
 
 
-@pytest.mark.parametrize("D,N", [(128, 300), (32, 257), (10, 100), (3, 7), (200, 33)])
+@pytest.mark.parametrize("D,N", [(128, 300), (32, 257), (10, 100), (3, 7), (200, 33), (1024, 65), (2048, 33)])
 @pytest.mark.parametrize("kind", F64_KINDS)
 def test_float64_layers_match_the_float64_oracle(B, kind, D, N):
     """Float64 batches with Float64 parameters (b2b_chain_run_f64): the reference is generic in its element type and its
@@ -601,7 +613,7 @@ def test_full_size_properties_config2(B):
     assert float((y0 - y).norm() / y.norm()) <= 2e-6 and float((lj0 - lj).norm() / lj.norm()) <= 2e-6
 
 
-@pytest.mark.parametrize("D", [128, 64, 32, 256, 10, 7])
+@pytest.mark.parametrize("D", [128, 64, 32, 256, 10, 7, 1000, 1024])
 def test_rand_matches_the_oracle_stream(B, D):
     """rand(td, n) with the base samples generated inside the chain kernel (Philox4x32-10 + Box-Muller): the samples
     equal the oracle's restatement of the stream pushed through the oracle's chain (fixed seed = fixed base sample),
@@ -782,7 +794,7 @@ def test_columnwise_sums_over_columns(B):
     assert rel(B.to_numpy(xi), x) <= 1e-4 and abs(float(toti) + ljo.sum()) <= 1e-4 * abs(ljo.sum())
 
 
-@pytest.mark.parametrize("D,N", [(32, 5000), (256, 4097), (10, 333)])
+@pytest.mark.parametrize("D,N", [(32, 5000), (256, 4097), (10, 333), (1024, 2049)])
 def test_batchnorm_training_mode(B, D, N):
     """InvertibleBatchNorm with istraining() == true (normalise.jl:51-60): batch statistics, moving-average update
     with the n/(n-1) correction, output and logjac from the batch statistics."""
