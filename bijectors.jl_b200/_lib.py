@@ -123,6 +123,9 @@ _SIGS = {
     "b2b_chain_workspace_bytes_f64": (c_size_t, [c_int32, c_int]),
     "b2b_chain_run_f64": (c_int, [POINTER(LayerDesc64), c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int64,
                                   c_int64, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
+    "b2b_chain_vjp_workspace_bytes_f64": (c_size_t, [POINTER(LayerDesc64), c_int32, c_int32, c_int64]),
+    "b2b_chain_vjp_f64": (c_int, [POINTER(LayerDesc64), c_int32] + [c_void_p] * 5 +
+                          [c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "b2b_randn_f32": (c_int, [_F32P] * 3 + [c_uint64, c_uint64, c_int64, c_int32, c_int64, c_int64, c_void_p]),
     "b2b_chain_sample_f32": (c_int, [POINTER(LayerDesc), c_int32, _F32P, _F32P, c_uint64, c_uint64, c_int64, _F32P, _F32P,
                                      c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),

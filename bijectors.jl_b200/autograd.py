@@ -19,11 +19,11 @@ from .layers import (AffineConditioner, Coupling, InvertibleBatchNorm, Partition
 _VJP_DIMS = (32, 64, 128)
 
 
-def _colmajor(t: torch.Tensor) -> torch.Tensor:
-    """A (D, N) tensor with strides (1, D) (no copy when it already has them)."""
+def _colmajor(t: torch.Tensor, dtype=torch.float32) -> torch.Tensor:
+    """A (D, N) tensor with strides (1, D) (no copy when it already has them; a copy is made in ``dtype``)."""
     if t.dim() == 2 and t.stride(0) == 1 and (t.shape[1] == 1 or t.stride(1) == t.shape[0]):
         return t
-    out = colmajor_empty(t.shape[0], t.shape[1], t.device)
+    out = colmajor_empty(t.shape[0], t.shape[1], t.device, dtype=dtype)
     out.copy_(t)
     return out
 
@@ -306,7 +306,7 @@ class SplineLayer(torch.nn.Module):
         return _SplineFn.apply(y, *self.knots(), True)
 
 
-# ---- any chain: one b2b_chain_vjp_f32 call per backward ------------------------------------------------------------------
+# ---- any chain: one b2b_chain_vjp_f32 (Float64: b2b_chain_vjp_f64) call per backward -------------------------------------
 def _trainable_tensors(leaf) -> List[torch.Tensor]:
     """The device tensors of a leaf's trainable fields (Functors' trainable set of the reference's layer structs)."""
     lay = leaf.orig if isinstance(leaf, Inverse) else leaf
@@ -327,14 +327,15 @@ def _trainable_tensors(leaf) -> List[torch.Tensor]:
 
 class _ChainFn(torch.autograd.Function):
     """with_logabsdet_jacobian of a whole chain (plus, for logpdf, the terminal MvNormal); backward = ONE
-    b2b_chain_vjp_f32 call whose parameter cotangents are routed to the parameters by device address."""
+    b2b_chain_vjp_f32 call (b2b_chain_vjp_f64 for Float64 batches) whose parameter cotangents are routed to the parameters
+    by device address."""
 
     @staticmethod
     def forward(ctx, x, t, extra, want_y: bool, *params):
-        xc = _colmajor(x.detach())
+        xc = _colmajor(x.detach(), x.dtype)
         D = xc.shape[0]
         y, lj = run_chain(t, xc, want_y=want_y, extra_descs=extra)
-        descs = list(t._descs(False, D, torch.float32)) + list(extra)
+        descs = list(t._descs(False, D, xc.dtype)) + list(extra)
         owner = {p.data_ptr(): k for k, p in enumerate(params) if ctx.needs_input_grad[4 + k]}
         # a parameter can appear in several descriptors (a layer used twice): its cotangent is the sum
         ctx.want = [(l, i, owner[getattr(d, f"p{i}")]) for l, d in enumerate(descs) for i in _trainable_slots(d)
@@ -347,7 +348,7 @@ class _ChainFn(torch.autograd.Function):
     def backward(ctx, *grads):
         (xc,) = ctx.saved_tensors
         ybar, ljbar = grads if ctx.want_y else (None, grads[0])
-        yb = _colmajor(ybar) if ybar is not None else None
+        yb = _colmajor(ybar, xc.dtype) if ybar is not None else None
         lb = ljbar.contiguous() if ljbar is not None else None
         xbar, bars = _chain_vjp_raw(ctx.descs, xc, yb, lb, [(l, i) for l, i, _ in ctx.want])
         out: List = [None] * len(ctx.shapes)
@@ -363,8 +364,9 @@ class Flow(torch.nn.Module):
     fields of every leaf of ``flatten(transform)`` (w/u/b, α_/β/z_0, processed RQS knots, W/c, b/logs) and μ, σ of the
     base when it has them, registered on the leaves' own device storage: an optimiser step is what the next launch reads.
     ``forward(x)`` / ``inverse(y)`` return (result, logjac); ``logpdf(y)`` is logpdf(transformed(base, transform), y) and
-    ``nll(y)`` = −Σ logpdf.  Each is one autograd Function whose backward is one b2b_chain_vjp_f32 call.  A training-mode
-    InvertibleBatchNorm raises (it has no reverse mode here)."""
+    ``nll(y)`` = −Σ logpdf.  Each is one autograd Function whose backward is one b2b_chain_vjp_f32 call.  A flow whose
+    layers (and base) are Float64 takes Float64 batches, and its backward is one b2b_chain_vjp_f64 call; a Float32 /
+    Float64 mix raises TypeError.  A training-mode InvertibleBatchNorm raises (it has no reverse mode here)."""
 
     def __init__(self, transform, base=None):
         super().__init__()
@@ -381,10 +383,10 @@ class Flow(torch.nn.Module):
             tensors += [t for t in (base.mu, base.sigma) if t is not None]
         self.params = torch.nn.ParameterList([torch.nn.Parameter(t) for t in tensors])  # shares the leaves' storage
 
-    def _base(self, D, device):
+    def _base(self, D, device, dtype=torch.float32):
         from .transformed_distribution import MvNormal
 
-        return self.base if self.base is not None else MvNormal(D, device=device)
+        return self.base if self.base is not None else MvNormal(D, device=device, dtype=dtype)
 
     def forward(self, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         return _ChainFn.apply(x, self.transform, (), True, *self.params)
@@ -393,7 +395,7 @@ class Flow(torch.nn.Module):
         return _ChainFn.apply(y, inverse(self.transform), (), True, *self.params)
 
     def logpdf(self, y: torch.Tensor) -> torch.Tensor:
-        term = self._base(y.shape[0], y.device)._terminal_desc()
+        term = self._base(y.shape[0], y.device, y.dtype)._terminal_desc()
         return _ChainFn.apply(y, inverse(self.transform), (term,), False, *self.params)
 
     def nll(self, y: torch.Tensor) -> torch.Tensor:

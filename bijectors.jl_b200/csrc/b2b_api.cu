@@ -39,6 +39,7 @@ extern "C" const char* b2b_status_string(int status) {
 }
 
 extern "C" int b2b_last_launch_count(void) { return g_last_launches; }
+void b2b_set_last_launch_count(int n) { g_last_launches = n; }
 
 extern "C" int b2b_set_kernel_variant(int variant) {
   // low decimal digit: fused chain kernel variant; tens digit: coupling variant (10 = force fp32 CUDA cores)

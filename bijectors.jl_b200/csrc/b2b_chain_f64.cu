@@ -5,7 +5,8 @@
 // plain, layer-by-layer restatement in double precision -- one warp per column, the column staged in shared memory,
 // lanes over rows, row reductions by warp shuffles -- NOT a tuned kernel: Float64 batches are a correctness path, the
 // Float32 kernels are the hot path.  Every layer kind of the Float32 path is
-// covered, including affine coupling (a per-column matrix-vector product) and the terminal MvNormal.
+// covered, including affine coupling (a per-column matrix-vector product) and the terminal MvNormal.  The per-layer
+// arithmetic (f64_layer_forward) lives in b2b_f64_device.cuh, which the reverse mode (b2b_chain_vjp_f64.cu) shares.
 //
 // Reference semantics: planar_layer.jl:65-127,160-185; radial_layer.jl:36-129; rational_quadratic_spline.jl:183-220,
 // 317-357; coupling.jl:206-228; normalise.jl:61-86; permute.jl:152-155; stacked.jl:157-166; transformed_distribution.jl:165-169.
@@ -13,7 +14,7 @@
 
 #include <cstring>
 
-#include "b2b_internal.h"
+#include "b2b_f64_device.cuh"
 
 namespace b2b {
 
@@ -29,167 +30,6 @@ struct F64Params {
   b2b_layer_desc_f64 layers[B2B_MAX_CHAIN];
 };
 
-__device__ __forceinline__ double wsum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ double softplus64(double x) { return x > 0.0 ? x + log1p(exp(-x)) : log1p(exp(x)); }
-
-__device__ __forceinline__ void tanh_sech2_64(double a, double& t, double& s2) {
-  const double e = exp(-2.0 * fabs(a));
-  t = tanh(a);
-  const double r = 1.0 / (1.0 + e);
-  s2 = 4.0 * e * r * r;  // abs2(sech(a)) without cancellation, planar_layer.jl:107
-}
-
-// find_alpha (planar_layer.jl:160-185) in double: bracketed Newton on the monotone f(α) = α + c·tanh(α+b) − t
-__device__ double find_alpha64(double t, double c, double b, double& th, double& s2) {
-  const double delta = 2.0 * fabs(c);
-  double lo = t - delta, hi = t + delta;
-  if (lo == hi) {  // empty bracket, :171-173
-    tanh_sech2_64(lo + b, th, s2);
-    return lo;
-  }
-  tanh_sech2_64(t + b, th, s2);
-  double x = fmin(fmax(t - c * th, lo), hi);
-  for (int it = 0; it < 200; ++it) {
-    tanh_sech2_64(x + b, th, s2);
-    const double f = x + c * th - t;
-    if (f == 0.0) break;
-    if (f < 0.0) lo = x; else hi = x;
-    double xn = x - f / (1.0 + c * s2);
-    if (!(xn > lo && xn < hi)) {
-      xn = 0.5 * (lo + hi);
-      if (!(xn > lo && xn < hi)) break;  // adjacent doubles
-    }
-    if (fabs(xn - x) <= 2.3e-16 * (fabs(t) + delta)) {
-      x = xn;
-      tanh_sech2_64(x + b, th, s2);
-      break;
-    }
-    x = xn;
-  }
-  return x;
-}
-
-__device__ __forceinline__ double ew_apply64(int op, bool inverse, double a, double b, double xv, double& lj) {
-  switch (op) {
-    case B2B_EW_EXP:
-    case B2B_EW_LOG: {
-      const bool is_exp = (op == B2B_EW_EXP) != inverse;
-      if (is_exp) {
-        lj += xv;
-        return exp(xv);
-      }
-      const double lg = log(xv);
-      lj -= lg;
-      return lg;
-    }
-    case B2B_EW_SHIFT: return inverse ? xv - a : a + xv;
-    case B2B_EW_SCALE: {
-      const double la = log(fabs(a));
-      lj += inverse ? -la : la;
-      return inverse ? xv / a : a * xv;
-    }
-    case B2B_EW_LEAKY_RELU: {
-      const double al = inverse ? 1.0 / a : a;
-      if (xv < 0.0) {
-        lj += log(fabs(al));
-        return al * xv;
-      }
-      return xv;
-    }
-    case B2B_EW_LOGIT: {
-      if (!inverse) {
-        const double z = (xv - a) / (b - a);
-        lj -= log((xv - a) * (b - xv) / (b - a));
-        return log(z / (1.0 - z));
-      }
-      const double x = (b - a) / (1.0 + exp(-xv)) + a;
-      lj += log((x - a) * (b - x) / (b - a));
-      return x;
-    }
-    case B2B_EW_TRUNCATED: {
-      const bool lo = !isinf(a), hi = !isinf(b);
-      if (!inverse) {
-        const double x = xv < a ? a : (xv > b ? b : xv);
-        if (lo && hi) {
-          const double z = (x - a) / (b - a);
-          lj -= log((x - a) * (b - x) / (b - a));
-          return log(z / (1.0 - z));
-        }
-        if (lo) {
-          const double lg = log(x - a);
-          lj -= lg;
-          return lg;
-        }
-        if (hi) {
-          const double lg = log(b - x);
-          lj -= lg;
-          return lg;
-        }
-        return x;
-      }
-      double x = xv;
-      if (lo && hi) {
-        const double ay = fabs(xv);
-        lj += log(b - a) - ay - 2.0 * softplus64(-ay);
-        x = (b - a) / (1.0 + exp(-xv)) + a;
-      } else if (lo) {
-        lj += xv;
-        x = exp(xv) + a;
-      } else if (hi) {
-        lj += xv;
-        x = b - exp(xv);
-      }
-      return x < a ? a : (x > b ? b : x);
-    }
-    default: return xv;
-  }
-}
-
-// one RQS element straight from the knot arrays (D x K1, column-major); forward :317-357, inverse :183-220
-__device__ double rqs64(const b2b_layer_desc_f64& d, int D, int i, double v, bool inv, double& lj) {
-  const int K1 = d.n0;
-  const double* Wd = d.p0;
-  const double* Hd = d.p1;
-  const double* Dv = d.p2;
-  const double* S = inv ? Hd : Wd;
-  const double Bs = S[(size_t)(K1 - 1) * D + i];
-  if (v <= -Bs || v >= Bs) return v;
-  int k = 0;  // searchsortedfirst − 1 = number of knots < v
-  while (k < K1 && S[(size_t)k * D + i] < v) ++k;
-  if (k > K1 - 1) k = K1 - 1;
-  const double Wl = Wd[(size_t)(K1 - 1) * D + i], Hl = Hd[(size_t)(K1 - 1) * D + i];
-  const double w_k = k == 0 ? -Wl : Wd[(size_t)(k - 1) * D + i];
-  const double w = Wd[(size_t)k * D + i] - w_k;
-  const double h_k = k == 0 ? -Hl : Hd[(size_t)(k - 1) * D + i];
-  const double dy = Hd[(size_t)k * D + i] - h_k;
-  const double s = dy / w;
-  const double d_k = k == 0 ? 1.0 : Dv[(size_t)(k - 1) * D + i];
-  const double d_k1 = k == K1 - 1 ? 1.0 : Dv[(size_t)k * D + i];
-  const double ds = d_k1 + d_k - 2.0 * s;
-  double xi, res;
-  if (inv) {
-    const double yh = v - h_k;
-    const double a1 = dy * (s - d_k) + yh * ds;
-    const double a2 = dy * d_k - yh * ds;
-    const double a3 = -s * yh;
-    xi = -2.0 * a3 / (a2 + sqrt(a2 * a2 - 4.0 * a1 * a3));
-    res = xi * w + w_k;
-  } else {
-    xi = (v - w_k) / w;
-  }
-  const double omx = 1.0 - xi;
-  const double den = s + ds * xi * omx;
-  const double l = log(s * s * (d_k1 * xi * xi + 2.0 * s * xi * omx + d_k * omx * omx)) - 2.0 * log(den);
-  if (!inv) res = h_k + dy * (s * xi * xi + d_k * xi * omx) / den;
-  lj += inv ? -l : l;
-  return res;
-}
-
 __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_constant__ F64Params P) {
   extern __shared__ double sm64[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, D = P.D;
@@ -200,117 +40,7 @@ __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_
     for (int i = lane; i < D; i += 32) col[i] = P.x[n * P.ldx + i];
     double lj = (P.accumulate && P.logjac) ? P.logjac[n] : 0.0;
     __syncwarp();
-    for (int l = 0; l < P.L; ++l) {
-      const b2b_layer_desc_f64& d = P.layers[l];
-      const bool inv = d.inverse != 0;
-      switch (d.kind) {
-        case B2B_PLANAR: {
-          double s = 0.0, q = 0.0, wz = 0.0;
-          for (int i = lane; i < D; i += 32) {
-            const double w = d.p0[i];
-            s += w * d.p1[i];
-            q += w * w;
-            wz += w * col[i];
-          }
-          s = wsum(s);
-          q = wsum(q);
-          wz = wsum(wz);
-          const double kk = (softplus64(-s) - 1.0) / q;  // get_u_hat, planar_layer.jl:65-70
-          const double c = softplus64(s) - 1.0, b = d.p2[0];
-          double t, s2;
-          if (!inv) {
-            tanh_sech2_64(wz + b, t, s2);
-            lj += log1p(c * s2);
-          } else {
-            find_alpha64(wz, c, b, t, s2);
-            lj -= log1p(c * s2);
-            t = -t;
-          }
-          for (int i = lane; i < D; i += 32) col[i] += (d.p1[i] + kk * d.p0[i]) * t;
-        } break;
-        case B2B_RADIAL: {
-          const double alpha = softplus64(d.p0[0]), apb = softplus64(d.p1[0]), bhat = apb - alpha;
-          double r2 = 0.0;
-          for (int i = lane; i < D; i += 32) {
-            const double dd = col[i] - d.p2[i];
-            r2 += dd * dd;
-          }
-          const double nrm = sqrt(wsum(r2));
-          double r = nrm;
-          if (inv) {
-            const double a = apb - nrm;  // radial_layer.jl:126-127
-            const double sq = sqrt(a * a + 4.0 * alpha * nrm);
-            r = a > 0.0 ? (2.0 * alpha * nrm) / (sq + a) : 0.5 * (sq - a);  // the same root without cancellation
-          }
-          const double hh = 1.0 / (alpha + r);
-          const double ljf = (double)(D - 1) * log1p(bhat * hh) + log1p(bhat * hh - bhat * hh * hh * r);
-          const double g = inv ? (alpha + r) / (apb + r) - 1.0 : bhat * hh;
-          lj += inv ? -ljf : ljf;
-          for (int i = lane; i < D; i += 32) col[i] += g * (col[i] - d.p2[i]);
-        } break;
-        case B2B_RQS: {
-          double p = 0.0;
-          for (int i = lane; i < D; i += 32) col[i] = rqs64(d, D, i, col[i], inv, p);
-          lj += wsum(p);
-        } break;
-        case B2B_BATCHNORM: {
-          double p = 0.0;
-          for (int i = lane; i < D; i += 32) {
-            const double ve = d.p3[i] + d.f0, sc = exp(d.p1[i]);
-            col[i] = inv ? (col[i] - d.p0[i]) / sc * sqrt(ve) + d.p2[i] : sc * (col[i] - d.p2[i]) / sqrt(ve) + d.p0[i];
-            p += d.p1[i] - 0.5 * log(ve);
-          }
-          p = wsum(p);
-          lj += inv ? -p : p;
-        } break;
-        case B2B_STACKED_EW: {
-          double p = 0.0;
-          for (int i = lane; i < D; i += 32)
-            col[i] = ew_apply64(d.i0[i], inv, d.p0 ? d.p0[i] : 0.0, d.p1 ? d.p1[i] : 0.0, col[i], p);
-          lj += wsum(p);
-        } break;
-        case B2B_PERMUTE: {
-          for (int i = lane; i < D; i += 32) tmp[i] = col[i];
-          __syncwarp();
-          for (int i = lane; i < D; i += 32) {
-            if (inv) col[i] = tmp[d.i0[i]];       // Permute(transpose(A)), permute.jl:153
-            else col[d.i0[i]] = tmp[i];           // y[dst[i]] = x[i], :95-97,152
-          }
-        } break;
-        case B2B_COUPLING_AFFINE: {
-          const int n1 = d.n0, n2 = d.n1;
-          double p = 0.0;
-          for (int j = lane; j < n1; j += 32) {
-            double sv = d.p1 ? d.p1[j] : 0.0, tv = d.p1 ? d.p1[n1 + j] : 0.0;
-            for (int k = 0; k < n2; ++k) {
-              const double xk = col[d.i1 ? d.i1[k] : d.n3 + k];
-              sv += d.p0[(size_t)k * (2 * n1) + j] * xk;
-              tv += d.p0[(size_t)k * (2 * n1) + n1 + j] * xk;
-            }
-            const int r = d.i0 ? d.i0[j] : d.n2 + j;
-            tmp[j] = inv ? (col[r] - tv) * exp(-sv) : exp(sv) * col[r] + tv;  // scale.jl:13,16; shift.jl:12,14
-            p += sv;
-          }
-          __syncwarp();  // every lane has read its x₂ rows before x₁ rows are overwritten (disjoint row sets anyway)
-          for (int j = lane; j < n1; j += 32) col[d.i0 ? d.i0[j] : d.n2 + j] = tmp[j];
-          p = wsum(p);
-          lj += inv ? -p : p;
-        } break;
-        case B2B_MVNORMAL_DIAG: {
-          double q = 0.0, ls = 0.0;
-          for (int i = lane; i < D; i += 32) {
-            const double sg = d.p1 ? d.p1[i] : 1.0, z = (col[i] - (d.p0 ? d.p0[i] : 0.0)) / sg;
-            q += z * z;
-            ls += log(sg * sg);
-          }
-          q = wsum(q);
-          ls = wsum(ls);
-          lj += -0.5 * ((double)D * 1.8378770664093453 + ls) - 0.5 * q;
-        } break;
-        default: break;
-      }
-      __syncwarp();
-    }
+    for (int l = 0; l < P.L; ++l) f64_layer_forward(P.layers[l], D, lane, col, tmp, lj);
     if (P.y)
       for (int i = lane; i < D; i += 32) P.y[n * P.ldy + i] = col[i];
     if (lane == 0) {
@@ -333,6 +63,33 @@ __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_
 
 }  // namespace b2b
 
+int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last) {
+  switch (d.kind) {
+    case B2B_PLANAR:
+    case B2B_RADIAL:
+      if (!d.p0 || !d.p1 || !d.p2) return B2B_EINVAL;
+      break;
+    case B2B_RQS:
+      if (!d.p0 || !d.p1 || !d.p2 || d.n0 < 2) return B2B_EINVAL;
+      break;
+    case B2B_COUPLING_AFFINE:
+      if (!d.p0 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
+      break;
+    case B2B_BATCHNORM:
+      if (!d.p0 || !d.p1 || !d.p2 || !d.p3) return B2B_EINVAL;
+      break;
+    case B2B_PERMUTE:
+    case B2B_STACKED_EW:
+      if (!d.i0) return B2B_EINVAL;
+      break;
+    case B2B_MVNORMAL_DIAG:
+      if (!last || d.inverse) return B2B_EINVAL;
+      break;
+    default: return B2B_EINVAL;
+  }
+  return B2B_OK;
+}
+
 extern "C" size_t b2b_chain_workspace_bytes_f64(int32_t L, int want_sum) { return (L > 0 && want_sum) ? 4096 * sizeof(double) : 0; }
 
 extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double* x, double* y, double* logjac,
@@ -350,31 +107,9 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
   F64Params P;
   memset(&P, 0, sizeof(P));
   for (int l = 0; l < L; ++l) {
-    const b2b_layer_desc_f64& d = layers[l];
-    switch (d.kind) {
-      case B2B_PLANAR:
-      case B2B_RADIAL:
-        if (!d.p0 || !d.p1 || !d.p2) return B2B_EINVAL;
-        break;
-      case B2B_RQS:
-        if (!d.p0 || !d.p1 || !d.p2 || d.n0 < 2) return B2B_EINVAL;
-        break;
-      case B2B_COUPLING_AFFINE:
-        if (!d.p0 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-        break;
-      case B2B_BATCHNORM:
-        if (!d.p0 || !d.p1 || !d.p2 || !d.p3) return B2B_EINVAL;
-        break;
-      case B2B_PERMUTE:
-      case B2B_STACKED_EW:
-        if (!d.i0) return B2B_EINVAL;
-        break;
-      case B2B_MVNORMAL_DIAG:
-        if (l != L - 1 || d.inverse) return B2B_EINVAL;
-        break;
-      default: return B2B_EINVAL;
-    }
-    P.layers[l] = d;
+    const int rc = b2b_f64_validate_layer(layers[l], D, l == L - 1);
+    if (rc != B2B_OK) return rc;
+    P.layers[l] = layers[l];
   }
   if (sum_out && !logjac && layers[L - 1].kind != B2B_MVNORMAL_DIAG) return B2B_EINVAL;
   P.x = x;

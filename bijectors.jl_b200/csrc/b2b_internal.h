@@ -119,3 +119,8 @@ bool b2b_coupling_affine_fits(int n1, int n2, int D);
 int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const float* x, float* y,
                                float* logjac, int D, long long N, long long ldx, long long ldy, int accumulate,
                                cudaStream_t stream);
+// Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
+// element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL.
+int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
+// Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
+void b2b_set_last_launch_count(int n);

@@ -249,10 +249,10 @@ HOST_CHUNK_COLS = 1 << 16
 HOST_STREAMS = 3
 
 
-def _desc_array(descs: Sequence[LayerDesc]):
+def _desc_array(descs: Sequence[LayerDesc], desc_t=LayerDesc):
     if len(descs) > _lib.MAX_CHAIN:
         raise B2BError(_lib.B2B_EUNSUPPORTED, f"chain of {len(descs)} layers (max {_lib.MAX_CHAIN})")
-    return (LayerDesc * len(descs))(*descs)
+    return (desc_t * len(descs))(*descs)
 
 
 def run_chain(t, x: torch.Tensor, *, want_y=True, want_logjac=True, y: Optional[torch.Tensor] = None,
@@ -765,7 +765,7 @@ def isclosedform(t) -> bool:
 
 
 # --------------------------------------------------------------------------------------------------
-# reverse mode of any chain: b2b_chain_vjp_f32
+# reverse mode of any chain: b2b_chain_vjp_f32 (Float32 batches) / b2b_chain_vjp_f64 (Float64 batches)
 # --------------------------------------------------------------------------------------------------
 
 # names of the trainable descriptor slots p0..p3 of each kind (the reference's field names)
@@ -798,44 +798,57 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
     return (D,)
 
 
+# per batch dtype: (name, descriptor type, workspace query, entry point)
+_CHAIN_VJP = {
+    torch.float32: ("Float32", LayerDesc, "b2b_chain_vjp_workspace_bytes", "b2b_chain_vjp_f32"),
+    torch.float64: ("Float64", _lib.LayerDesc64, "b2b_chain_vjp_workspace_bytes_f64", "b2b_chain_vjp_f64"),
+}
+
+
 def _chain_vjp_raw(descs, x: torch.Tensor, ybar: Optional[torch.Tensor], ljbar: Optional[torch.Tensor], want):
-    """One b2b_chain_vjp_f32 call.  ``want``: (descriptor index, slot) pairs.  Returns (xbar, {(l, i): cotangent in the
-    storage shape of that parameter})."""
+    """One b2b_chain_vjp_f32 call (b2b_chain_vjp_f64 for a Float64 batch).  ``want``: (descriptor index, slot) pairs.
+    Returns (xbar, {(l, i): cotangent in the storage shape of that parameter}).  The descriptors must be of the batch's
+    element type (a Float32 / Float64 mix raises TypeError), and so must the cotangents."""
     D, N, ldx = _batch_view(x)
-    if not x.is_cuda or x.dtype != torch.float32:
-        raise ValueError("chain_vjp: x must be a Float32 device batch")
+    name, desc_t, query, entry = _CHAIN_VJP[x.dtype]
+    if not x.is_cuda:
+        raise ValueError(f"chain_vjp: x must be a {name} device batch")
+    if not all(isinstance(d, desc_t) for d in descs):
+        raise TypeError(f"{name} batch with layer parameters of another element type: construct the layers with "
+                        f"dtype={x.dtype}")
     ldyb = D
     if ybar is not None:
         Dy, Ny, ldyb = _batch_view(ybar)
-        if (Dy, Ny) != (D, N) or not ybar.is_cuda or ybar.dtype != torch.float32:
-            raise ValueError("chain_vjp: ybar must be a Float32 device batch of x's shape")
-    if ljbar is not None and (ljbar.numel() != N or ljbar.dtype != torch.float32 or not ljbar.is_contiguous()):
-        raise ValueError("ljbar must be a contiguous float32 vector of length N")
-    arr = _desc_array(descs)
+        if (Dy, Ny) != (D, N) or not ybar.is_cuda or ybar.dtype != x.dtype:
+            raise ValueError(f"chain_vjp: ybar must be a {name} device batch of x's shape")
+    if ljbar is not None and (ljbar.numel() != N or ljbar.dtype != x.dtype or not ljbar.is_contiguous()):
+        raise ValueError(f"ljbar must be a contiguous {str(x.dtype)[6:]} vector of length N")
+    arr = _desc_array(descs, desc_t)
     L = len(descs)
     bars = {}
     ptrs = (ctypes.c_void_p * (4 * L))()
     for l, i in want:
-        t = torch.empty(_slot_shape(descs[l], i, D), dtype=torch.float32, device=x.device)
+        t = torch.empty(_slot_shape(descs[l], i, D), dtype=x.dtype, device=x.device)
         bars[(l, i)] = t
         ptrs[4 * l + i] = t.data_ptr()
-    xbar = torch.empty_like(x) if x.dim() == 1 else colmajor_empty(D, N, x.device)
+    xbar = torch.empty_like(x) if x.dim() == 1 else colmajor_empty(D, N, x.device, dtype=x.dtype)
     L_ = lib()
-    ws_bytes = L_.b2b_chain_vjp_workspace_bytes(arr, L, D, N)
+    ws_bytes = getattr(L_, query)(arr, L, D, N)
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device) if ws_bytes else None
-    rc = L_.b2b_chain_vjp_f32(
+    rc = getattr(L_, entry)(
         arr, L, x.data_ptr(), ybar.data_ptr() if ybar is not None else None,
         ljbar.data_ptr() if ljbar is not None else None, xbar.data_ptr(), ctypes.cast(ptrs, ctypes.c_void_p) if want else None,
         D, N, ldx, ldyb, _batch_view(xbar)[2], ws.data_ptr() if ws is not None else None, ws_bytes, _stream())
-    check(rc, "b2b_chain_vjp_f32")
+    check(rc, entry)
     return xbar, bars
 
 
-def _leaf_descs(t, D: int):
-    """(descriptors of ``t`` in application order, number of descriptors of each leaf of flatten(t))."""
+def _leaf_descs(t, D: int, dtype=torch.float32):
+    """(descriptors of ``t`` in application order, number of descriptors of each leaf of flatten(t)), built for batches of
+    ``dtype`` (a leaf whose parameters have another element type raises TypeError)."""
     descs, counts = [], []
     for leaf in flatten(t):
-        ds = list(leaf._descs(False, D, torch.float32))
+        ds = list(leaf._descs(False, D, dtype))
         descs += ds
         counts.append(len(ds))
     return descs, counts
@@ -860,11 +873,12 @@ def chain_vjp(t, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Op
     """Vector-Jacobian product of ``with_logabsdet_jacobian(t, x)`` for ANY chain the forward accepts -- every layer kind,
     either direction, mixed: what the reference's reverse-mode AD computes when a flow is trained
     (docs/src/flows.md:93-100).  ``ybar`` (D×N) / ``ljbar`` (N) are the cotangents of the two outputs (None = zeros).
-    One b2b_chain_vjp_f32 call.  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)`` (application
-    order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives`` (D×K+1),
-    ``W/c``, ``b/logs``, and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
+    One b2b_chain_vjp_f32 call -- b2b_chain_vjp_f64 when ``x`` is a Float64 batch, whose layers and cotangents must then be
+    Float64 too (a mix raises TypeError).  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)``
+    (application order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives``
+    (D×K+1), ``W/c``, ``b/logs``, and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
     D = _batch_view(x)[0]
-    descs, counts = _leaf_descs(t, D)
+    descs, counts = _leaf_descs(t, D, x.dtype)
     if not descs:
         raise ValueError("empty chain")
     want = [(l, i) for l, d in enumerate(descs) for i in _trainable_slots(d)]

@@ -142,8 +142,9 @@ def rand(td, n: int, seed: Optional[int] = None, offset: int = 0, column_offset:
 
 
 def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[torch.Tensor] = None):
-    """Reverse mode of ``logpdf(td, y)``: one b2b_chain_vjp_f32 call through inverse(td.transform) and the terminal
-    MvNormal.  ``lpbar`` (N, None = ones) is the cotangent of the logpdf vector.  Returns ``(ybar, flow_grads, base_grads)``:
+    """Reverse mode of ``logpdf(td, y)``: one b2b_chain_vjp_f32 call (b2b_chain_vjp_f64 for a Float64 ``y``, with Float64
+    layers and base) through inverse(td.transform) and the terminal MvNormal.  ``lpbar`` (N, None = ones in ``y``'s dtype)
+    is the cotangent of the logpdf vector.  Returns ``(ybar, flow_grads, base_grads)``:
     ``flow_grads`` one dict per leaf of ``flatten(td.transform)`` in FLOW order (see chain_vjp for the keys) and
     ``base_grads`` = {"μ", "σ"} for the base parameters that are given; all summed over the columns of this batch."""
     from .interface import _chain_vjp_raw, _leaf_descs, _leaf_grads, _trainable_slots
@@ -152,8 +153,8 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     if D != len(td.dist):
         raise ValueError(f"DimensionMismatch: distribution has {len(td.dist)} dims, input has {D}")
     if lpbar is None:
-        lpbar = torch.ones((N,), dtype=torch.float32, device=y.device)
-    descs, counts = _leaf_descs(inverse(td.transform), D)
+        lpbar = torch.ones((N,), dtype=y.dtype, device=y.device)
+    descs, counts = _leaf_descs(inverse(td.transform), D, y.dtype)
     descs.append(td.dist._terminal_desc())
     want = [(l, i) for l, d in enumerate(descs) for i in _trainable_slots(d)]
     ybar, bars = _chain_vjp_raw(descs, y, None, lpbar, want)

@@ -334,7 +334,8 @@ int b2b_mvnormal_diag_logpdf_f32(const float* x, const float* mu, const float* s
  * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind, both directions, the terminal
  * MvNormal, the deterministic batch sum -- on D x N Float64 batches with Float64 parameters (b2b_layer_desc_f64: the
  * same fields with double pointers).  It is a straightforward double-precision restatement (one warp per column), NOT a
- * tuned kernel: Float64 is a correctness path, Float32 the hot path.  workspace: b2b_chain_workspace_bytes_f64. */
+ * tuned kernel: Float64 is a correctness path, Float32 the hot path.  workspace: b2b_chain_workspace_bytes_f64.
+ * b2b_chain_vjp_f64 is its reverse mode. */
 typedef struct b2b_layer_desc_f64 {
   int32_t kind;
   int32_t inverse;
@@ -351,6 +352,30 @@ size_t b2b_chain_workspace_bytes_f64(int32_t L, int want_sum);
 int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double* x, double* y, double* logjac,
                       double* sum_out, int32_t D, int64_t N, int64_t ldx, int64_t ldy, int accumulate_logjac,
                       void* workspace, size_t workspace_bytes, void* stream);
+/* Reverse mode of b2b_chain_run_f64: the contract of b2b_chain_vjp_f32 with double everywhere.  Any chain
+ * b2b_chain_run_f64 accepts (every kind, either direction, mixed, L <= B2B_MAX_CHAIN, D <= 2048, optionally ending in
+ * the terminal B2B_MVNORMAL_DIAG, whose logjac output is then logpdf).  `xbar` (D x N, required) must not overlap `x` or
+ * `ybar` (B2B_EINVAL); NULL `ybar` / `ljbar` are zeros; `param_bars` (NULL = x̄ only) holds 4*L pointers, entry 4l+i the
+ * cotangent of layers[l].p<i> in its shape and layout, summed over the N columns.  Trainable slots as for Float32: PLANAR
+ * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; BATCHNORM b
+ * logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); any other non-NULL entry
+ * returns B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
+ * parameter cotangents.  One warp per column recomputes the forward with the arithmetic of b2b_chain_run_f64, keeping
+ * each layer's input in a tape, then differentiates the layers last to first; parameter cotangents accumulate in
+ * per-warp slots that a second kernel sums in a fixed order (deterministic, no atomics) and a third turns into the
+ * caller's arrays.  Launch-only on `stream`, no allocation (CUDA-graph capturable); b2b_last_launch_count counts the
+ * kernels and fills enqueued (1, or 3 with parameter cotangents).
+ * Workspace (b2b_chain_vjp_workspace_bytes_f64; 0 exactly when the call refuses the chain) is bounded independently of N:
+ * W warp slots of 8·(T + P) bytes plus 8·P, with T = Lf·D (Lf: layers before the MvNormal) and P the accumulators, per
+ * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, BATCHNORM / MVNORMAL_DIAG 2D doubles (each rounded up
+ * to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
+ * 256 MiB but never below one CTA -- so the bound exceeds 256 MiB only when one CTA's slots do (e.g. wide couplings with
+ * 2n1·n2 in the millions).  The number of warps, and with it the summation order, depends only on the chain, D and N. */
+size_t b2b_chain_vjp_workspace_bytes_f64(const b2b_layer_desc_f64* layers, int32_t L, int32_t D, int64_t N);
+int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, const double* x, const double* ybar,
+                      const double* ljbar, double* xbar, double* const* param_bars, int32_t D, int64_t N,
+                      int64_t ldx, int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes,
+                      void* stream);
 
 /* ---- sampling: rand(rng, td, n) (src/transformed_distribution.jl:212-224) -----------------------------------------
  * Base samples z ~ N(0, I) come from Philox4x32-10 (the counter-based generator of Random123 / cuRAND) + Box-Muller and

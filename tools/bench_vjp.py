@@ -2,7 +2,8 @@
 `python tools/bench_vjp.py chain` times b2b_chain_vjp_f32 instead, as device time of graph-captured calls: (a) the
 elementwise-run kernel alone on Stacked(Logit + exp rows) + Permute + MvNormal, (b) the logpdf gradient of
 inverse(8 x Planar) + MvNormal through logpdf_vjp against planar_chain_vjp with the base density's cotangent in torch, the
-two routes alternated."""
+two routes alternated.  `python tools/bench_vjp.py chain64` times b2b_chain_vjp_f64 on the Float64 8 x Planar chain at D=128,
+N=2^16 (x̄ and every parameter cotangent), also as device time of graph-captured calls."""
 import os
 import subprocess
 import sys
@@ -14,15 +15,50 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bijectors_jl_b200 as B
 
 
-def bench_chain():
-    D, N, L = 128, 1 << 20, 8
-    rng = np.random.default_rng(0)
+def print_card():
     try:
         power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
                                 str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
     except (OSError, subprocess.SubprocessError):
         power = "unknown"
     print(f"card: {torch.cuda.get_device_name()}, power limit: {power}")
+
+
+def graph_replay_ms(fn, reps):
+    """Device time of each of `reps` replays of `fn` captured once into a CUDA graph."""
+    g = B.GraphedCalls(fn)
+    g()
+    torch.cuda.synchronize()
+    out = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        g()
+        e1.record()
+        torch.cuda.synchronize()
+        out.append(e0.elapsed_time(e1))
+    return out
+
+
+def bench_chain64():
+    """b2b_chain_vjp_f64 through 8 x PlanarLayer (Float64), D=128, N=2^16: x̄ and the w̄, ū, b̄ of every layer."""
+    D, N, L = 128, 1 << 16, 8
+    rng = np.random.default_rng(0)
+    print_card()
+    t = torch.float64
+    flow = B.Composed(*[B.PlanarLayer(rng.standard_normal(D) / np.sqrt(D), rng.standard_normal(D) / np.sqrt(D),
+                                      rng.standard_normal(1), dtype=t) for _ in range(L)])
+    x = B.from_numpy(rng.standard_normal((D, N)), dtype=np.float64)
+    yb = B.from_numpy(rng.standard_normal((D, N)), dtype=np.float64)
+    lb = torch.from_numpy(rng.standard_normal(N)).cuda()
+    ts = graph_replay_ms(lambda: B.chain_vjp(flow, x, yb, lb), 20)
+    print(f"b2b_chain_vjp_f64 8 x Planar D={D} N=2^16: median {np.median(ts):.3f} ms, min {min(ts):.3f} ms (20 replays)")
+
+
+def bench_chain():
+    D, N, L = 128, 1 << 20, 8
+    rng = np.random.default_rng(0)
+    print_card()
 
     def device_ms(fn, reps=20):
         """Device time of one call: the call is captured once into a CUDA graph (no host work in the timed window) and
@@ -75,6 +111,9 @@ def bench_chain():
 
 if len(sys.argv) > 1 and sys.argv[1] == "chain":
     bench_chain()
+    sys.exit(0)
+if len(sys.argv) > 1 and sys.argv[1] == "chain64":
+    bench_chain64()
     sys.exit(0)
 
 D, N, L = int(sys.argv[1]) if len(sys.argv) > 1 else 128, 1 << 20, int(sys.argv[2]) if len(sys.argv) > 2 else 8
