@@ -7,7 +7,7 @@ from ._lib import B2BError, LIB_PATH, exported_symbols, lib  # noqa: F401
 from .interface import (  # noqa: F401
     Bijector, Columnwise, Composed, ComposedFunction, GraphedCalls, Inverse, Transform, chain_vjp, colmajor_empty, columnwise, compose, flatten,
     from_numpy,
-    inverse, isclosedform, isinvertible, logabsdetjac, logabsdetjac_, planar_chain_vjp, radial_chain_vjp, coupling_vjp, batchnorm_vjp, rqs_vjp, run_chain, to_numpy, transform, transform_,
+    inverse, isclosedform, isinvertible, logabsdetjac, logabsdetjac_, planar_chain_vjp, radial_chain_vjp, coupling_vjp, batchnorm_vjp, batchnorm_train_vjp, rqs_vjp, run_chain, to_numpy, transform, transform_,
     with_logabsdet_jacobian, with_logabsdet_jacobian_,
 )
 from .layers import (  # noqa: F401

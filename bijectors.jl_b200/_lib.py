@@ -115,6 +115,9 @@ _SIGS = {
     "b2b_batchnorm_train_fwd_f32": (c_int, [_F32P] * 7 + [c_float, c_float, c_int32, c_int64, c_int64, c_int64, c_int, c_void_p,
                                             c_void_p, c_size_t, c_void_p]),
     "b2b_batchnorm_train_workspace_bytes": (c_size_t, [c_int32]),
+    "b2b_batchnorm_train_vjp_workspace_bytes": (c_size_t, [c_int32]),
+    "b2b_batchnorm_train_vjp_f32": (c_int, [_F32P] * 7 + [c_float, c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
     "b2b_permute_rows_f32": (c_int, [_F32P] * 3 + [c_void_p, c_int, c_int32, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "b2b_stacked_elementwise_f32": (c_int, [_F32P] * 3 + [c_void_p, _F32P, _F32P, c_int, c_int32, c_int64, c_int64, c_int64,
                                             c_int, c_void_p]),

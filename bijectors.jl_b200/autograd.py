@@ -6,12 +6,13 @@ from __future__ import annotations
 
 from typing import List, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
 from ._lib import B2BError
-from .interface import (Composed, Inverse, _chain_vjp_raw, _trainable_slots, batchnorm_vjp, colmajor_empty, coupling_vjp, flatten,
-                        inverse, planar_chain_vjp, radial_chain_vjp, rqs_vjp, run_chain)
+from .interface import (Composed, Inverse, _chain_vjp_raw, _trainable_slots, batchnorm_train_vjp, batchnorm_vjp, colmajor_empty,
+                        coupling_vjp, flatten, inverse, planar_chain_vjp, radial_chain_vjp, rqs_vjp, run_chain)
 from .layers import (AffineConditioner, Coupling, InvertibleBatchNorm, PartitionMask, PlanarLayer, RadialLayer,
                      RationalQuadraticSpline)
 
@@ -204,14 +205,63 @@ class _BatchNormFn(torch.autograd.Function):
         return xbar, g["b"], g["logs"], None, None, None, None
 
 
+class _BatchNormTrainFn(torch.autograd.Function):
+    """with_logabsdet_jacobian of ONE training-mode InvertibleBatchNorm (normalise.jl:51-67): the forward runs
+    b2b_batchnorm_train_fwd_f32 once (so the moving statistics move once per step); backward = b2b_batchnorm_train_vjp_f32,
+    which recomputes the batch statistics from the saved x and leaves the moving statistics alone."""
+
+    @staticmethod
+    def forward(ctx, x, b, logs, m, v, eps: float, mtm: float, comm):
+        lay = InvertibleBatchNorm(b=b.detach(), logs=logs.detach(), m=m, v=v, eps=eps, mtm=mtm, device=x.device, training=True)
+        xc = _colmajor(x.detach())
+        y, lj = lay.train_forward(xc, comm)
+        ctx.lay, ctx.comm = lay, comm
+        ctx.save_for_backward(xc)
+        return y, lj
+
+    @staticmethod
+    def backward(ctx, ybar, ljbar):
+        (xc,) = ctx.saved_tensors
+        yb = _colmajor(ybar) if ybar is not None else None
+        xbar, g = batchnorm_train_vjp(ctx.lay, xc, yb, ljbar.contiguous() if ljbar is not None else None, ctx.comm)
+        return xbar, g["b"], g["logs"], None, None, None, None, None
+
+
+class TrainingBatchNorm(torch.nn.Module):
+    """A trainable InvertibleBatchNorm(dims; eps, mtm) in training mode (normalise.jl:26-37,51-67): parameters ``b``,
+    ``logs``; buffers ``m``, ``v`` (the moving statistics, updated once per forward).  ``forward(x)`` returns (y, logjac)
+    computed with the batch statistics -- over all ranks of ``comm`` (a distributed.Communicator) when given --
+    differentiable w.r.t. x, b and logs.  With ``comm``, the b / logs gradients are this rank's share: all-reduce them with
+    the rest of the gradient.  The layer has no inverse in training mode (normalise.jl:75)."""
+
+    def __init__(self, dims: int, comm=None, eps: float = 1e-5, mtm: float = 1e-1, device="cuda"):
+        super().__init__()
+        self.comm, self.eps, self.mtm = comm, float(np.float32(eps)), float(np.float32(mtm))
+        self.b = torch.nn.Parameter(torch.zeros(dims, device=device))
+        self.logs = torch.nn.Parameter(torch.zeros(dims, device=device))
+        self.register_buffer("m", torch.zeros(dims, device=device))
+        self.register_buffer("v", torch.ones(dims, device=device))
+
+    def forward(self, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        return _BatchNormTrainFn.apply(x, self.b, self.logs, self.m, self.v, self.eps, self.mtm, self.comm)
+
+
+_NO_TRAINING_INVERSE = "`with_logabsdet_jacobian(::Inverse{InvertibleBatchNorm})` is only available in test mode."  # normalise.jl:75
+
+
 class RealNVP(torch.nn.Module):
     """A trainable RealNVP flow: `n_blocks` x (affine Coupling with alternating half masks + eval-mode InvertibleBatchNorm),
     the structure of BASELINE config 5.  ``forward(x)`` / ``inverse(y)`` return (result, logjac), differentiable w.r.t.
     the input and the parameters W, c (conditioners) and b, logs (BatchNorm; m, v are statistics); ``nll(y)`` is the
-    training objective of docs/src/flows.md:74-77 with a standard-normal base."""
+    training objective of docs/src/flows.md:74-77 with a standard-normal base.
+    ``batchnorm_training=True`` puts the BatchNorm layers in training mode (istraining() == true, normalise.jl:51-67):
+    ``forward`` then normalises with the batch statistics, updates ``m`` / ``v`` once per call and differentiates through
+    the statistics; ``inverse`` and ``nll`` raise, as the reference asserts at normalise.jl:75."""
 
-    def __init__(self, dims: int, n_blocks: int, device="cuda", generator=None, scale: float = 0.05):
+    def __init__(self, dims: int, n_blocks: int, device="cuda", generator=None, scale: float = 0.05,
+                 batchnorm_training: bool = False):
         super().__init__()
+        self.batchnorm_training = batchnorm_training
         h = dims // 2
         self.dims, self.masks = dims, []
         Ws, cs, bs, ls = [], [], [], []
@@ -229,17 +279,22 @@ class RealNVP(torch.nn.Module):
         self.b, self.logs = torch.nn.ParameterList(bs), torch.nn.ParameterList(ls)
         self.register_buffer("m", torch.zeros(n_blocks, dims, device=device))
         self.register_buffer("v", torch.ones(n_blocks, dims, device=device))
-        self.eps = 1e-5
+        self.eps, self.mtm = 1e-5, float(np.float32(1e-1))
 
     def forward(self, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         lj = None
         for l in range(len(self.W)):
             x, l1 = _CouplingFn.apply(x, self.W[l], self.c[l], self.masks[l], False)
-            x, l2 = _BatchNormFn.apply(x, self.b[l], self.logs[l], self.m[l], self.v[l], self.eps, False)
+            if self.batchnorm_training:
+                x, l2 = _BatchNormTrainFn.apply(x, self.b[l], self.logs[l], self.m[l], self.v[l], self.eps, self.mtm, None)
+            else:
+                x, l2 = _BatchNormFn.apply(x, self.b[l], self.logs[l], self.m[l], self.v[l], self.eps, False)
             lj = l1 + l2 if lj is None else lj + l1 + l2
         return x, lj
 
     def inverse(self, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        if self.batchnorm_training:
+            raise AssertionError(_NO_TRAINING_INVERSE)
         lj = None
         for l in reversed(range(len(self.W))):
             y, l2 = _BatchNormFn.apply(y, self.b[l], self.logs[l], self.m[l], self.v[l], self.eps, True)

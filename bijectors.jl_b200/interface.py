@@ -729,6 +729,46 @@ def batchnorm_vjp(t, x: torch.Tensor, ybar: torch.Tensor, ljbar: Optional[torch.
     return xbar, {"b": bbar, "logs": lbar}
 
 
+def batchnorm_train_vjp(bn, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Optional[torch.Tensor] = None,
+                        comm=None):
+    """Vector-Jacobian product of ``with_logabsdet_jacobian(bn, x)`` for ONE training-mode InvertibleBatchNorm (istraining()
+    == true, normalise.jl:51-67): the batch statistics depend on every column, so x̄ carries the mean and variance terms,
+    and the log-Jacobian's dependence on the batch variance.  ``ybar`` / ``ljbar`` default to zeros.  With ``comm`` (a
+    distributed.Communicator) the batch is sharded over its ranks: x̄ uses the global statistics and sums, while the
+    returned ``{"b": b̄, "logs": l̄ogs}`` are summed over this rank's columns (all-reduce them with the rest of the
+    gradient).  The moving statistics are not touched: b2b_batchnorm_train_vjp_f32."""
+    from .layers import InvertibleBatchNorm
+
+    D, N, ldx = _batch_view(x)
+    if not isinstance(bn, InvertibleBatchNorm):
+        raise B2BError(_lib.B2B_EUNSUPPORTED, "batchnorm_train_vjp: one InvertibleBatchNorm (training mode has no inverse)")
+    if D != bn.b.numel():
+        raise RuntimeError(f"InvertibleBatchNorm expected {bn.b.numel()} channels, got {D}")
+    if not x.is_cuda or x.dim() != 2 or x.dtype != torch.float32:
+        raise ValueError("batchnorm_train_vjp: x must be a Float32 device matrix")
+    ldyb = D
+    if ybar is not None:
+        Dy, Ny, ldyb = _batch_view(ybar)
+        if (Dy, Ny) != (D, N) or not ybar.is_cuda or ybar.dtype != torch.float32:
+            raise ValueError("batchnorm_train_vjp: ybar must be a Float32 device matrix of x's D×N shape")
+    if ljbar is not None and (ljbar.numel() != N or ljbar.dtype != torch.float32 or not ljbar.is_contiguous()):
+        raise ValueError("ljbar must be a contiguous float32 vector of length N")
+    xbar = colmajor_empty(D, N, x.device)
+    bbar = torch.empty((D,), dtype=torch.float32, device=x.device)
+    lbar = torch.empty((D,), dtype=torch.float32, device=x.device)
+    L_ = lib()
+    ws_bytes = L_.b2b_batchnorm_train_vjp_workspace_bytes(D)
+    if ws_bytes == 0:
+        raise B2BError(_lib.B2B_EUNSUPPORTED, "batchnorm_train_vjp: D <= 1024")
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device)
+    handle = comm.handle if (comm is not None and getattr(comm, "handle", None) is not None) else None
+    check(L_.b2b_batchnorm_train_vjp_f32(x.data_ptr(), ybar.data_ptr() if ybar is not None else None,
+                                         ljbar.data_ptr() if ljbar is not None else None, xbar.data_ptr(), bbar.data_ptr(),
+                                         lbar.data_ptr(), bn.logs.data_ptr(), bn.eps, D, N, ldx, ldyb, _batch_view(xbar)[2],
+                                         handle, ws.data_ptr(), ws_bytes, _stream()), "b2b_batchnorm_train_vjp_f32")
+    return xbar, {"b": bbar, "logs": lbar}
+
+
 def rqs_vjp(t, x: torch.Tensor, ybar: torch.Tensor, ljbar: Optional[torch.Tensor] = None):
     """Vector-Jacobian product of ``with_logabsdet_jacobian(t, x)`` for ONE RationalQuadraticSpline ``t`` (or its inverse,
     with ``x`` the observed batch): b2b_rqs_vjp_f32.  Returns ``(xbar, {"widths": W̄, "heights": H̄, "derivatives": D̄})``,

@@ -245,6 +245,23 @@ function batchnorm_train!(bn::InvertibleBatchNorm{<:CuVector{Float32}}, x::CuMat
     return y, logjac
 end
 
+# Its reverse mode: cotangents of x (through the batch statistics, over all ranks when `comm` is given) and of b, logs
+# (summed over this rank's columns).  The moving statistics are not touched.
+function batchnorm_train_vjp(bn::InvertibleBatchNorm{<:CuVector{Float32}}, x::CuMatrix{Float32}, ȳ::CuMatrix{Float32},
+                             l̄::CuVector{Float32}; comm=nothing)
+    D, N = size(x)
+    x̄ = similar(x); b̄ = CUDA.zeros(Float32, D); l̄ogs = CUDA.zeros(Float32, D)
+    nbytes = ccall((:b2b_batchnorm_train_vjp_workspace_bytes, libb2b), Csize_t, (Int32,), D)
+    ws = CuVector{UInt8}(undef, nbytes)
+    GC.@preserve ws check(ccall((:b2b_batchnorm_train_vjp_f32, libb2b), Cint,
+        (CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+         Cfloat, Int32, Int64, Int64, Int64, Int64, Ptr{Cvoid}, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+        pointer(x), pointer(ȳ), pointer(l̄), pointer(x̄), pointer(b̄), pointer(l̄ogs), pointer(bn.logs),
+        Float32(bn.eps), D, N, stride(x, 2), stride(ȳ, 2), stride(x̄, 2),
+        comm === nothing ? C_NULL : comm.handle, pointer(ws), nbytes, stream_handle()))
+    return x̄, b̄, l̄ogs
+end
+
 # Reverse mode: a ChainRulesCore.rrule for device planar chains (what ext/BijectorsChainRulesCoreExt.jl does for the CPU
 # path, incl. the implicit find_alpha rule :42-46).  ȳ, l̄ are the cotangents of (y, logjac).
 function planar_chain_vjp(f, x::CuMatrix{Float32}, ȳ::CuMatrix{Float32}, l̄::CuVector{Float32}; inv::Bool=false)

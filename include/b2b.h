@@ -314,6 +314,26 @@ int b2b_batchnorm_train_fwd_f32(const float* x, float* y, float* logjac, const f
                                 int64_t ldy, int accumulate_logjac, struct b2b_comm* comm, void* workspace,
                                 size_t workspace_bytes, void* stream);
 size_t b2b_batchnorm_train_workspace_bytes(int32_t D);
+/* Reverse mode of the TRAINING-mode InvertibleBatchNorm (normalise.jl:51-67 with istraining() == true): y and logjac
+ * depend on the batch statistics, so the cotangents reach every column through m and v.  With n the number of columns
+ * over all ranks, m, v the batch statistics exactly as b2b_batchnorm_train_fwd_f32 computes them on the same x, device and
+ * communicator (bit-identical), σ² = v + eps, A = exp(logs)/σ and the global sums S1 = Σȳ, S2 = Σȳ(x − m), L̄ = Σl̄:
+ *   x̄ = A ȳ − A S1/n − (x − m)(A S2 + L̄)/(n σ²),   b̄ = S1,   l̄ogs = A S2 + L̄.
+ * `x` (D x N, the batch the forward saw), `xbar` and `logs` are required; `ybar` (D x N) and `ljbar` (N) may be NULL
+ * (zeros).  `xbar` may be exactly `ybar` (same pointer and leading dimension); any other overlap of `xbar` with `x` or
+ * `ybar` returns B2B_EINVAL.  `bbar` and `logsbar` (D each) are both given or both NULL (one alone: B2B_EINVAL).
+ * Sharded batch (comm != NULL): x̄ uses the global statistics and sums -- one all-reduce of 4D+2 doubles -- while `bbar`
+ * and `logsbar` are summed over THIS rank's columns only, like every other parameter cotangent of the library: a
+ * data-parallel caller all-reduces them with the rest of its gradient.  The moving statistics are not touched (they have
+ * no cotangent, and the function takes no pointer to them).  N < 2 (local) returns B2B_EINVAL, D > 1024
+ * B2B_EUNSUPPORTED with nothing launched, as for the forward.  Deterministic (fixed-order fp64 sums, no atomics),
+ * launch-only on `stream`, no allocation (CUDA-graph capturable).
+ * workspace: b2b_batchnorm_train_vjp_workspace_bytes(D) (0 when D < 1 or D > 1024; independent of N). */
+size_t b2b_batchnorm_train_vjp_workspace_bytes(int32_t D);
+int b2b_batchnorm_train_vjp_f32(const float* x, const float* ybar, const float* ljbar, float* xbar, float* bbar,
+                                float* logsbar, const float* logs, float eps, int32_t D, int64_t N, int64_t ldx,
+                                int64_t ldybar, int64_t ldxbar, struct b2b_comm* comm, void* workspace,
+                                size_t workspace_bytes, void* stream);
 /* Permute rows (also serves PartitionMask / Stacked range movement): permute.jl:152-155. Bit-exact. */
 int b2b_permute_rows_f32(const float* x, float* y, float* logjac, const int32_t* dst_of_src,
                          int inverse, int32_t D, int64_t N, int64_t ldx, int64_t ldy,

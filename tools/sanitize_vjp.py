@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Tiny invocation of every kernel family that is not in sanitize_smoke.py, for compute-sanitizer:
    compute-sanitizer --tool memcheck python tools/sanitize_vjp.py
-reverse mode (radial both directions + mixed, coupling fast / generic, BatchNorm, RQS both directions, planar runs),
+reverse mode (radial both directions + mixed, coupling fast / generic, BatchNorm in eval and training mode, RQS both directions, planar runs),
 the in-kernel sampler, Float64 chains, Logit / Truncated blocks, exact-L planar programs, padded spline tables."""
 import os
 import sys
@@ -38,6 +38,7 @@ for D, N in ((64, 777), (32, 1000), (128, 333), (10, 129)):
     bn = B.InvertibleBatchNorm(b=np.zeros(D, f32), logs=np.zeros(D, f32), m=np.zeros(D, f32), v=np.ones(D, f32))
     B.batchnorm_vjp(bn, x, yb, lb)
     B.batchnorm_vjp(B.inverse(bn), x, yb, lb)
+    B.batchnorm_train_vjp(B.InvertibleBatchNorm(D, training=True), x, yb, lb)
     for K in (8, 5, 32):
         sp = B.RationalQuadraticSpline(rng.standard_normal((D, K)).astype(f32), rng.standard_normal((D, K)).astype(f32),
                                        rng.standard_normal((D, K - 1)).astype(f32), 3.0)
