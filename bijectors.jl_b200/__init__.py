@@ -15,7 +15,7 @@ from .layers import (  # noqa: F401
     RationalQuadraticSpline, Scale, Shift, Stacked, TruncatedBijector, coupling, elementwise,
 )
 from .transformed_distribution import (  # noqa: F401
-    MvNormal, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, transformed,
+    MvNormal, PosDefException, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, transformed,
 )
 from . import autograd, distributed  # noqa: F401
 

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libb2b.so")
 B2B_OK = 0
 B2B_EINVAL, B2B_EUNSUPPORTED, B2B_EWORKSPACE, B2B_ENONCCL = -1, -2, -3, -4
 PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG = 1, 2, 3, 4, 5, 6, 7, 8
+MVNORMAL_TRIL = 9
 EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = 0, 1, 2, 3, 4, 5, 6, 7
 MAX_CHAIN = 24
 
@@ -132,6 +133,8 @@ _SIGS = {
     "b2b_randn_f32": (c_int, [_F32P] * 3 + [c_uint64, c_uint64, c_int64, c_int32, c_int64, c_int64, c_void_p]),
     "b2b_chain_sample_f32": (c_int, [POINTER(LayerDesc), c_int32, _F32P, _F32P, c_uint64, c_uint64, c_int64, _F32P, _F32P,
                                      c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "b2b_chain_sample_tril_f32": (c_int, [POINTER(LayerDesc), c_int32, _F32P, _F32P, c_uint64, c_uint64, c_int64, _F32P,
+                                          _F32P, c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "b2b_host_ctx_create": (c_int, [POINTER(c_void_p), c_int32, c_int64, c_int32]),
     "b2b_host_ctx_destroy": (c_int, [c_void_p]),
     "b2b_host_ctx_wait_stream": (c_int, [c_void_p, c_void_p]),

@@ -416,8 +416,8 @@ class _ChainFn(torch.autograd.Function):
 class Flow(torch.nn.Module):
     """A trainable flow made of ANY chain of the supported layers -- `Stacked(ibs) ∘ PlanarLayer(2)`, spline flows with
     permutations, coupling flows with bounded outputs -- over an optional MvNormal base.  Its parameters are the trainable
-    fields of every leaf of ``flatten(transform)`` (w/u/b, α_/β/z_0, processed RQS knots, W/c, b/logs) and μ, σ of the
-    base when it has them, registered on the leaves' own device storage: an optimiser step is what the next launch reads.
+    fields of every leaf of ``flatten(transform)`` (w/u/b, α_/β/z_0, processed RQS knots, W/c, b/logs) and μ, σ or μ, L
+    (``MvNormal(..., scale_tril=L)``; the parameter holds L column-major, i.e. Lᵀ row-major) of the base when it has them, registered on the leaves' own device storage: an optimiser step is what the next launch reads.
     ``forward(x)`` / ``inverse(y)`` return (result, logjac); ``logpdf(y)`` is logpdf(transformed(base, transform), y) and
     ``nll(y)`` = −Σ logpdf.  Each is one autograd Function whose backward is one b2b_chain_vjp_f32 call.  A flow whose
     layers (and base) are Float64 takes Float64 batches, and its backward is one b2b_chain_vjp_f64 call; a Float32 /
@@ -435,7 +435,7 @@ class Flow(torch.nn.Module):
                     seen.add(t.data_ptr())
                     tensors.append(t)
         if isinstance(base, MvNormal):
-            tensors += [t for t in (base.mu, base.sigma) if t is not None]
+            tensors += [t for t in (base.mu, base.sigma, base._tril) if t is not None]
         self.params = torch.nn.ParameterList([torch.nn.Parameter(t) for t in tensors])  # shares the leaves' storage
 
     def _base(self, D, device, dtype=torch.float32):

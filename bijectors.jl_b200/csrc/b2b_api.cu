@@ -84,6 +84,9 @@ static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
     case B2B_MVNORMAL_DIAG:
       if (!last || d.inverse) return B2B_EINVAL;
       break;
+    case B2B_MVNORMAL_TRIL:
+      if (!last || d.inverse || !d.p1) return B2B_EINVAL;
+      break;
     default:
       return B2B_EINVAL;
   }
@@ -170,11 +173,13 @@ extern "C" size_t b2b_coupling_workspace_bytes(int32_t n1, int32_t n2) {
   return b ? align_up(b, 1024) + 1024 : 0;
 }
 
-// A launch of the chain: a run of fusable layers, or one coupling layer (with the BatchNorm neighbours folded into it).
+// A launch of the chain: a run of fusable layers, one coupling layer (with the BatchNorm neighbours folded into it), or
+// the terminal MVNORMAL_TRIL.
 struct Seg {
   int begin, end;
   bool coupling;
   int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
+  bool tril = false;
 };
 
 // Cuts the chain into launches before anything is enqueued: single coupling layers, and maximal runs of fusable layers
@@ -186,6 +191,12 @@ static int plan_segments(const b2b_layer_desc* layers, int32_t L, int32_t D, std
     if (layers[l].kind == B2B_COUPLING_AFFINE) {
       if (!b2b_coupling_affine_fits(layers[l].n0, layers[l].n1, D)) return B2B_EUNSUPPORTED;
       segs.push_back({l, l + 1, true, -1, -1});
+      ++l;
+      continue;
+    }
+    if (layers[l].kind == B2B_MVNORMAL_TRIL) {  // its own launch: the packed factor fills the shared memory
+      if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
+      segs.push_back({l, l + 1, false, -1, -1, true});
       ++l;
       continue;
     }
@@ -209,13 +220,29 @@ int b2b_chain_segment_count(const b2b_layer_desc* layers, int32_t L, int32_t D) 
   return rc != B2B_OK ? rc : (int)segs.size();
 }
 
+int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D) {
+  for (int l = 0; l < L; ++l) {
+    const int rc = validate_layer(layers[l], D, l == L - 1);
+    if (rc != B2B_OK) return rc;
+  }
+  const int n = b2b_chain_segment_count(layers, L, D);
+  return n < 0 ? n : B2B_OK;
+}
+
+static bool tril_terminal(const b2b_layer_desc* layers, int32_t L) {
+  return layers && L >= 1 && layers[L - 1].kind == B2B_MVNORMAL_TRIL;
+}
+
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
                                             int want_y, int want_sum) {
+  if (tril_terminal(layers, L) && D > B2B_TRIL_MAX_D) return 0;  // the call refuses the chain
   size_t bytes = chain_tc_bytes(layers, L, D);
   // a D x N scratch matrix is needed only when y == NULL but the chain has more than one segment
   if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
     bytes += align_up((size_t)D * (size_t)N * sizeof(float), 1024);
   if (want_sum) bytes += 4096 * sizeof(double);
+  // a batch sum without `logjac`: the log-Jacobians of the layers before a TRIL launch go through N floats of workspace
+  if (want_sum && tril_terminal(layers, L) && L > 1) bytes += align_up((size_t)N * sizeof(float), 1024);
   return bytes;
 }
 
@@ -245,7 +272,7 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     if (sum_out) return (int)cudaMemsetAsync(sum_out, 0, sizeof(double), stream);
     return B2B_OK;
   }
-  const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG;
+  const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL;
   if (sum_out && !logjac && !terminal) return B2B_EINVAL;
 
   std::vector<Seg> segs;
@@ -297,6 +324,14 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     ws += need;
     ws_left -= need;
   }
+  if (sum_out && !logjac && L > 1 && tril_terminal(layers, L)) {
+    // the layers before the TRIL launch hand their log-Jacobians to it through N floats of workspace
+    const size_t need = align_up((size_t)N * sizeof(float), 1024);
+    if (ws_left < need) return B2B_EWORKSPACE;
+    logjac = reinterpret_cast<float*>(ws);
+    ws += need;
+    ws_left -= need;
+  }
   double* partials = nullptr;
   if (sum_out) {
     if (segs.back().coupling) return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
@@ -337,6 +372,16 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
         if (rc == B2B_OK) ++g_last_launches;
       }
       if (rc != B2B_OK) return rc;
+    } else if (segs[s].tril) {  // always the last segment
+      rc = b2b_launch_mvnormal_tril(layers[segs[s].begin], cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0,
+                                    sum_out ? partials : nullptr, D, N, stream);
+      if (rc != B2B_OK) return rc;
+      ++g_last_launches;
+      if (sum_out) {
+        rc = b2b_launch_sum_partials(partials, b2b_tril_grid(D, N), sum_out, stream);
+        if (rc != B2B_OK) return rc;
+        ++g_last_launches;
+      }
     } else {
       B2BChainParams p;
       memset(&p, 0, sizeof(p));
@@ -656,7 +701,7 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
 // the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
 namespace {
 
-enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW };
+enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL };
 
 struct VSeg {
   int kind, begin, end;
@@ -694,6 +739,10 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
       case B2B_BATCHNORM:
         if (D > 1024) return B2B_EUNSUPPORTED;
         s.kind = VK_BN;
+        break;
+      case B2B_MVNORMAL_TRIL:  // the terminal, alone
+        if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
+        s.kind = VK_TRIL;
         break;
       default:  // PERMUTE / STACKED_EW (or the terminal MVNORMAL_DIAG alone)
         if (D > 1024) return B2B_EUNSUPPORTED;
@@ -740,6 +789,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case VK_RQS: return b2b_rqs_vjp_workspace_bytes(d.n0, D);
     case VK_COUPLING: return b2b_coupling_affine_vjp_workspace_bytes(d.n0, d.n1);
     case VK_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
+    case VK_TRIL: return b2b_tril_vjp_workspace(D, N);
     default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
   }
 }
@@ -755,7 +805,7 @@ VLayout vjp_layout(const b2b_layer_desc* layers, const std::vector<VSeg>& segs, 
   VLayout v{};
   const size_t S = segs.size(), m = mat_bytes(D, N);
   v.ckpt = (S - 1) * m;
-  v.ncot = (S == 1 && segs[0].kind == VK_EW) ? 0 : 2;
+  v.ncot = (S == 1 && (segs[0].kind == VK_EW || segs[0].kind == VK_TRIL)) ? 0 : 2;
   // the planar kernels read x through TMA: an x they cannot read is copied (into a free checkpoint when there is one)
   v.stage = (S == 1 && segs[0].kind == VK_PLANAR && segs[0].Dk == D) ? m : 0;
   size_t pf = 0;
@@ -779,6 +829,7 @@ size_t slot_len(const b2b_layer_desc& d, int i, int D) {
     case B2B_RADIAL: return i == 2 ? D : 1;
     case B2B_RQS: return (size_t)D * d.n0;
     case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
+    case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }
@@ -828,6 +879,10 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
         case B2B_MVNORMAL_DIAG:
           if (i >= 2) return B2B_EUNSUPPORTED;
           if (!(i == 0 ? d.p0 : d.p1)) return B2B_EINVAL;
+          break;
+        case B2B_MVNORMAL_TRIL:
+          if (i >= 2) return B2B_EUNSUPPORTED;
+          if (i == 0 && !d.p0) return B2B_EINVAL;
           break;
         default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
       }
@@ -1039,6 +1094,11 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       const bool mvn = ls[n - 1].kind == B2B_MVNORMAL_DIAG;
       rc = b2b_launch_ew_vjp(ls, n, in, ldin, cin, ldcin, ljbar, out, ldout, mvn ? bar(sg.end - 1, 0) : nullptr,
                              mvn ? bar(sg.end - 1, 1) : nullptr, D, N, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+    } else if (sg.kind == VK_TRIL) {
+      rc = b2b_launch_tril_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), bar(sg.begin, 1), D, N, kws,
+                               kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
     } else {  // one RQS, coupling or eval-BatchNorm layer: its own entry point (two launches each)

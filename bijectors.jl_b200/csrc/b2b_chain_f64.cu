@@ -1,4 +1,5 @@
-// Float64 evaluation of the same chains (include/b2b.h: b2b_chain_run_f64).
+// Float64 evaluation of the same chains (include/b2b.h: b2b_chain_run_f64), including the full-covariance terminal
+// MVNORMAL_TRIL up to D = 2048 (its factor read through L2).
 //
 // The reference is generic in its element type and its own tests run in Float64 (e.g. the find_alpha residual grid with
 // atol = 1e-14, test/normalising_flows.jl:47-71); this kernel is the device counterpart for those element types.  It is a
@@ -85,6 +86,9 @@ int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last) {
     case B2B_MVNORMAL_DIAG:
       if (!last || d.inverse) return B2B_EINVAL;
       break;
+    case B2B_MVNORMAL_TRIL:
+      if (!last || d.inverse || !d.p1) return B2B_EINVAL;
+      break;
     default: return B2B_EINVAL;
   }
   return B2B_OK;
@@ -111,7 +115,8 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     if (rc != B2B_OK) return rc;
     P.layers[l] = layers[l];
   }
-  if (sum_out && !logjac && layers[L - 1].kind != B2B_MVNORMAL_DIAG) return B2B_EINVAL;
+  if (sum_out && !logjac && layers[L - 1].kind != B2B_MVNORMAL_DIAG && layers[L - 1].kind != B2B_MVNORMAL_TRIL)
+    return B2B_EINVAL;
   P.x = x;
   P.y = y;
   P.logjac = logjac;

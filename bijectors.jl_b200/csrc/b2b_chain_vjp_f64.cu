@@ -410,7 +410,28 @@ __global__ void __launch_bounds__(V64_WARPS * 32) chain_vjp_f64_kernel(const __g
     }
     const double lb = P.ljbar ? P.ljbar[n] : 0.0;
     for (int i = lane; i < D; i += 32) g[i] = P.ybar ? P.ybar[n * P.ldyb + i] : 0.0;
-    if (P.Lf < P.L) {  // terminal MvNormal at y = col: q = (y − μ)/σ, ȳ −= l̄·q/σ, μ̄ += l̄·q/σ, σ̄ += l̄·(q² − 1)/σ
+    if (P.Lf < P.L && P.layers[P.Lf].kind == B2B_MVNORMAL_TRIL) {
+      // full-covariance terminal at y = col: r = L⁻¹(y − μ), s = L⁻ᵀr; ȳ −= l̄·s, μ̄ += l̄·s, L̄(i, j) += l̄·sᵢ·r_j (i ≥ j) and
+      // L̄(i, i) −= l̄/Lᵢᵢ.  Accumulators: μ̄ [D] | L̄ packed by columns (column j holds rows j..D-1).  The lane writing
+      // L̄(i, j) is (i − j) mod 32, the same for every column.
+      const b2b_layer_desc_f64& d = P.layers[P.Lf];
+      double* a = (P.want >> P.Lf) & 1u ? acc + P.off[P.Lf] : nullptr;
+      __syncwarp();
+      f64_tril_solve(d, D, lane, col, t1);
+      f64_tril_back(d, D, lane, t1, t2);
+      for (int i = lane; i < D; i += 32) {
+        const double gs = lb * t2[i];
+        g[i] -= gs;
+        if (a) a[i] += gs;
+      }
+      if (a && lb != 0.0)
+        for (int j = 0; j < D; ++j) {
+          double* Lc = a + D + (size_t)j * D - (size_t)j * (j + 1) / 2;  // L̄(i, j) at Lc[i]
+          const double rj = lb * t1[j];
+          for (int i = j + lane; i < D; i += 32) Lc[i] += t2[i] * rj;
+          if (lane == 0) Lc[j] -= lb / d.p1[(size_t)j * D + j];
+        }
+    } else if (P.Lf < P.L) {  // terminal MvNormal at y = col: q = (y − μ)/σ, ȳ −= l̄·q/σ, μ̄ += l̄·q/σ, σ̄ += l̄·(q² − 1)/σ
       const b2b_layer_desc_f64& d = P.layers[P.Lf];
       double* a = (P.want >> P.Lf) & 1u ? acc + P.off[P.Lf] : nullptr;
       for (int i = lane; i < D; i += 32) {
@@ -509,6 +530,14 @@ __global__ void __launch_bounds__(V64_FIN_THREADS) vjp_f64_finalize_kernel(const
       copy(bars[0], r, D);
       copy(bars[1], r + D, D);
       break;
+    case B2B_MVNORMAL_TRIL:  // L̄ unpacked to D x D column-major, zero above the diagonal
+      copy(bars[0], r, D);
+      if (bars[1])
+        for (size_t k = t; k < (size_t)D * D; k += V64_FIN_THREADS) {
+          const size_t j = k / D, i = k - j * D;
+          bars[1][k] = i >= j ? r[D + j * D - j * (j + 1) / 2 + i] : 0.0;
+        }
+      break;
     default: break;
   }
 }
@@ -523,6 +552,7 @@ long long acc_len(const b2b_layer_desc_f64& d, int D) {
     case B2B_COUPLING_AFFINE: n = 2LL * d.n0 * d.n1 + 2LL * d.n0; break;
     case B2B_BATCHNORM:
     case B2B_MVNORMAL_DIAG: n = 2LL * D; break;
+    case B2B_MVNORMAL_TRIL: n = (long long)D + (long long)D * (D + 1) / 2; break;
     default: break;
   }
   return (n + 31) & ~31LL;
@@ -534,6 +564,7 @@ long long slot_len(const b2b_layer_desc_f64& d, int i, int D) {
     case B2B_RADIAL: return i == 2 ? D : 1;
     case B2B_RQS: return (long long)D * d.n0;
     case B2B_COUPLING_AFFINE: return i == 0 ? 2LL * d.n0 * d.n1 : 2LL * d.n0;
+    case B2B_MVNORMAL_TRIL: return i == 1 ? (long long)D * D : D;
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }
@@ -550,7 +581,7 @@ struct V64Plan {
 // workspace grows with N only up to that bound.
 int v64_plan(const b2b_layer_desc_f64* layers, int L, int D, long long N, V64Plan& p) {
   if (D > 2048) return B2B_EUNSUPPORTED;
-  p.Lf = layers[L - 1].kind == B2B_MVNORMAL_DIAG ? L - 1 : L;
+  p.Lf = (layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL) ? L - 1 : L;
   p.T = ((long long)p.Lf * D + 31) & ~31LL;
   p.P = 0;
   for (int l = 0; l < L; ++l) {
@@ -625,6 +656,10 @@ extern "C" int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, co
         case B2B_MVNORMAL_DIAG:
           if (i >= 2) return B2B_EUNSUPPORTED;
           if (!(i == 0 ? d.p0 : d.p1)) return B2B_EINVAL;
+          break;
+        case B2B_MVNORMAL_TRIL:
+          if (i >= 2) return B2B_EUNSUPPORTED;
+          if (i == 0 && !d.p0) return B2B_EINVAL;
           break;
         default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
       }

@@ -172,6 +172,41 @@ static __device__ double rqs64(const b2b_layer_desc_f64& d, int D, int i, double
   return res;
 }
 
+// r := L⁻¹(col − μ) for the terminal MVNORMAL_TRIL (p0 = μ or NULL, p1 = L column-major, read through L2), by forward
+// substitution: r_j is final once the steps before j have run, then rows i > j subtract L(i, j)·r_j.  Returns, in every
+// lane, −Σ log Lᵢᵢ − ½‖r‖².  `r` may not alias `col`.
+static __device__ double f64_tril_solve(const b2b_layer_desc_f64& d, int D, int lane, const double* col, double* r) {
+  const double* Lm = d.p1;
+  for (int i = lane; i < D; i += 32) r[i] = col[i] - (d.p0 ? d.p0[i] : 0.0);
+  __syncwarp();
+  for (int j = 0; j < D; ++j) {
+    const double rj = r[j] / Lm[(size_t)j * D + j];
+    __syncwarp();  // every lane has read r[j]
+    if (lane == 0) r[j] = rj;
+    for (int i = j + 1 + lane; i < D; i += 32) r[i] = fma(-Lm[(size_t)j * D + i], rj, r[i]);
+    __syncwarp();
+  }
+  double q = 0.0, ls = 0.0;
+  for (int i = lane; i < D; i += 32) {
+    q += r[i] * r[i];
+    ls += log(Lm[(size_t)i * D + i]);
+  }
+  return -wsum(ls) - 0.5 * wsum(q);
+}
+
+// s := L⁻ᵀ r by left-looking back substitution, s_i = (r_i − Σ_{k>i} L(k, i)·s_k)/Lᵢᵢ: column i of L is contiguous, so the
+// dot product is a coalesced read and a warp sum.  `s` may not alias `r`.
+static __device__ void f64_tril_back(const b2b_layer_desc_f64& d, int D, int lane, const double* r, double* s) {
+  const double* Lm = d.p1;
+  for (int i = D - 1; i >= 0; --i) {
+    double p = 0.0;
+    for (int k = i + 1 + lane; k < D; k += 32) p += Lm[(size_t)i * D + k] * s[k];
+    p = wsum(p);
+    if (lane == 0) s[i] = (r[i] - p) / Lm[(size_t)i * D + i];
+    __syncwarp();
+  }
+}
+
 // Applies one layer to the column `col` (D doubles in shared memory; `tmp`: D more, scratch) and adds its log-Jacobian
 // (for MVNORMAL_DIAG: the log-density) to `lj`.  Called by all 32 lanes of a warp; ends with __syncwarp.
 static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f64& d, int D, int lane, double* col,
@@ -281,6 +316,9 @@ static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f6
       ls = wsum(ls);
       lj += -0.5 * ((double)D * 1.8378770664093453 + ls) - 0.5 * q;
     } break;
+    case B2B_MVNORMAL_TRIL:  // the column is left as it is (the terminal's y is its input); r goes to tmp
+      lj += -0.5 * (double)D * 1.8378770664093453 + f64_tril_solve(d, D, lane, col, tmp);
+      break;
     default: break;
   }
   __syncwarp();

@@ -202,9 +202,10 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
     cudaError_t e = cudaMemcpyAsync(c->dx[s], x_host + (size_t)c0 * D, (size_t)n * D * sizeof(float),
                                     cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) return (int)e;
-    const bool want_lj = logjac_host != nullptr || (sum_host && layers[L - 1].kind != B2B_MVNORMAL_DIAG);
+    const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL;
+    const bool want_lj = logjac_host != nullptr || (sum_host && !terminal);
     const int rc = b2b_chain_run_f32(layers, L, c->dx[s], stage_y ? c->dx[s] : nullptr,  // in place
-                                     (want_lj || layers[L - 1].kind == B2B_MVNORMAL_DIAG) ? c->dlj[s] : nullptr,
+                                     (want_lj || terminal) ? c->dlj[s] : nullptr,
                                      sum_host ? c->dsum[s] : nullptr, D, n, D, D, 0, c->dws[s], kWsBytes, st);
     if (rc != B2B_OK) return rc;
     launches += b2b_last_launch_count();

@@ -119,6 +119,21 @@ bool b2b_coupling_affine_fits(int n1, int n2, int D);
 int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const float* x, float* y,
                                float* logjac, int D, long long N, long long ldx, long long ldy, int accumulate,
                                cudaStream_t stream);
+// full-covariance MvNormal terminal (b2b_mvnormal_tril.cu).  Float32 stages the packed lower triangle of L in shared
+// memory: D <= B2B_TRIL_MAX_D.  The logpdf launch reads x (the recovered point), copies it to y when y != NULL and y != x,
+// and writes logpdf (+ logjac when accumulate) to logjac (may be NULL); with partials it writes b2b_tril_grid(D, N) per-CTA
+// batch sums.
+#define B2B_TRIL_MAX_D 256
+int b2b_tril_grid(int D, long long N);
+int b2b_launch_mvnormal_tril(const b2b_layer_desc& d, const float* x, long long ldx, float* y, long long ldy,
+                             float* logjac, int accumulate, double* partials, int D, long long N, cudaStream_t stream);
+// reverse mode: x̄ = ȳ − l̄·s always; μ̄ / L̄ (either may be NULL) need b2b_tril_vjp_workspace(D, N) bytes
+size_t b2b_tril_vjp_workspace(int D, long long N);
+int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
+                        const float* ljbar, float* xbar, long long ldxb, float* mubar, float* Lbar, int D, long long N,
+                        void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
+// B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
+int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL.
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);

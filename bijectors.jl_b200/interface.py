@@ -816,6 +816,7 @@ _SLOT_NAMES = {
     _lib.COUPLING_AFFINE: ("W", "c"),
     _lib.BATCHNORM: ("b", "logs"),
     _lib.MVNORMAL_DIAG: ("μ", "σ"),
+    _lib.MVNORMAL_TRIL: ("μ", "L"),
 }
 
 
@@ -835,6 +836,8 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
         return (d.n0, D)  # column-major D × K+1
     if d.kind == _lib.COUPLING_AFFINE:
         return (d.n1, 2 * d.n0) if i == 0 else (2 * d.n0,)  # W column-major (2n1 × n2)
+    if d.kind == _lib.MVNORMAL_TRIL and i == 1:
+        return (D, D)  # L column-major: element (i, j) at [j, i]
     return (D,)
 
 

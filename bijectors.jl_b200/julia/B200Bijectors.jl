@@ -20,6 +20,8 @@ using Bijectors: PlanarLayer, RadialLayer, RationalQuadraticSpline, Coupling, Pa
 import Bijectors: transform, logabsdetjac, with_logabsdet_jacobian
 import Distributions
 using Distributions: MvNormal
+using PDMats: PDMat, PDiagMat, ScalMat
+using LinearAlgebra: cholesky
 using Functors: fmap
 using SparseArrays: findnz
 using Statistics: mean, var
@@ -35,7 +37,7 @@ struct LayerDesc
     p0::CuPtr{Float32}; p1::CuPtr{Float32}; p2::CuPtr{Float32}; p3::CuPtr{Float32}
     i0::CuPtr{Int32}; i1::CuPtr{Int32}
 end
-const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG = Int32.(1:8)
+const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG, MVNORMAL_TRIL = Int32.(1:9)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
 const NULLI = CuPtr{Int32}(0)
@@ -349,6 +351,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
+    d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))
     return ()
 end
 chain_vjp(f, x::CuMatrix{Float32}, ȳ, l̄; inv::Bool=false) = chain_vjp(descs(f, inv), x, ȳ, l̄)
@@ -366,12 +369,29 @@ function chain_vjp(ds::Vector{LayerDesc}, x::CuMatrix{Float32}, ȳ, l̄)
         D, N, stride(x, 2), ȳ === nothing ? D : stride(ȳ, 2), stride(x̄, 2), pointer(ws), nbytes, stream_handle()))
     return x̄, bars
 end
-# Reverse mode of logpdf(td, y) with cotangent l̄ of the logpdf vector: (ȳ, flow cotangents in flow order, (μ̄, σ̄)).
+# The base distribution as the terminal descriptor, with the device arrays it points to (keep them alive while it is
+# used).  The covariance type decides the op: a diagonal one (PDiagMat, ScalMat) is MVNORMAL_DIAG with σ = sqrt.(var(d)),
+# a dense PDMat (FullNormal) is MVNORMAL_TRIL with its Cholesky factor L.  Any other covariance type has no device op.
+function base_desc(d::MvNormal)
+    μ, Σ = cu(Float32.(mean(d))), d.Σ
+    if Σ isa PDiagMat || Σ isa ScalMat
+        σ = cu(Float32.(sqrt.(var(d))))
+        return LayerDesc(MVNORMAL_DIAG, 0, 0, 0, 0, 0, 0f0, 0f0, pointer(μ), pointer(σ), NULLF, NULLF, NULLI, NULLI), (μ, σ)
+    elseif Σ isa PDMat
+        L = cu(Matrix{Float32}(cholesky(Σ).L))   # column-major, lower triangle
+        return LayerDesc(MVNORMAL_TRIL, 0, 0, 0, 0, 0, 0f0, 0f0, pointer(μ), pointer(L), NULLF, NULLF, NULLI, NULLI), (μ, L)
+    end
+    error("B200Bijectors: no device path for an MvNormal with covariance of type $(typeof(Σ)) " *
+          "(PDiagMat, ScalMat and PDMat are supported)")
+end
+
+# Reverse mode of logpdf(td, y) with cotangent l̄ of the logpdf vector: (ȳ, flow cotangents in flow order, base
+# cotangents: (μ̄, σ̄) for a diagonal covariance, (μ̄, L̄) with L̄ lower triangular for a PDMat).
 function logpdf_vjp(td::TransformedDistribution{<:MvNormal}, y::CuMatrix{Float32}, l̄::CuVector{Float32})
     ds = descs(td.transform, true)
-    μ, σ = cu(Float32.(mean(td.dist))), cu(Float32.(sqrt.(var(td.dist))))
-    push!(ds, LayerDesc(MVNORMAL_DIAG, 0, 0, 0, 0, 0, 0f0, 0f0, pointer(μ), pointer(σ), NULLF, NULLF, NULLI, NULLI))
-    ȳ, bars = GC.@preserve μ σ chain_vjp(ds, y, nothing, l̄)
+    term, keep = base_desc(td.dist)
+    push!(ds, term)
+    ȳ, bars = GC.@preserve keep chain_vjp(ds, y, nothing, l̄)
     return ȳ, reverse(bars[1:end-1]), bars[end]
 end
 
@@ -381,16 +401,25 @@ function device_rand(td::TransformedDistribution{<:MvNormal}, n::Integer; seed::
                      column_offset::Integer=0)
     ds = descs(td.transform, false)
     D = length(td.dist)
-    μ, σ = cu(Float32.(mean(td.dist))), cu(Float32.(sqrt.(var(td.dist))))
+    term, keep = base_desc(td.dist)
     y = CuMatrix{Float32}(undef, D, n)
     ws_bytes = ccall((:b2b_chain_workspace_bytes, libb2b), Csize_t,
                      (Ptr{LayerDesc}, Int32, Int32, Int64, Cint, Cint), ds, length(ds), D, n, true, false)
     ws = CuVector{UInt8}(undef, ws_bytes)
-    GC.@preserve ds μ σ ws check(ccall((:b2b_chain_sample_f32, libb2b), Cint,
-        (Ptr{LayerDesc}, Int32, CuPtr{Float32}, CuPtr{Float32}, UInt64, UInt64, Int64, CuPtr{Float32}, CuPtr{Float32},
-         Int32, Int64, Int64, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
-        ds, length(ds), pointer(μ), pointer(σ), seed, offset, column_offset, pointer(y), NULLF,
-        D, n, stride(y, 2), pointer(ws), ws_bytes, stream_handle()))
+    # y = μ + σ .* z (diagonal) or μ + L z (PDMat), z from the same Philox stream
+    if term.kind == MVNORMAL_TRIL
+        GC.@preserve ds keep ws check(ccall((:b2b_chain_sample_tril_f32, libb2b), Cint,
+            (Ptr{LayerDesc}, Int32, CuPtr{Float32}, CuPtr{Float32}, UInt64, UInt64, Int64, CuPtr{Float32}, CuPtr{Float32},
+             Int32, Int64, Int64, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+            ds, length(ds), term.p0, term.p1, seed, offset, column_offset, pointer(y), NULLF,
+            D, n, stride(y, 2), pointer(ws), ws_bytes, stream_handle()))
+    else
+        GC.@preserve ds keep ws check(ccall((:b2b_chain_sample_f32, libb2b), Cint,
+            (Ptr{LayerDesc}, Int32, CuPtr{Float32}, CuPtr{Float32}, UInt64, UInt64, Int64, CuPtr{Float32}, CuPtr{Float32},
+             Int32, Int64, Int64, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+            ds, length(ds), term.p0, term.p1, seed, offset, column_offset, pointer(y), NULLF,
+            D, n, stride(y, 2), pointer(ws), ws_bytes, stream_handle()))
+    end
     return y
 end
 
@@ -399,9 +428,9 @@ end
 function Distributions.logpdf(td::TransformedDistribution{<:MvNormal}, y::CuMatrix{Float32})
     is_device(td.transform) || return invoke(Distributions.logpdf, Tuple{TransformedDistribution,AbstractMatrix}, td, y)
     ds = descs(td.transform, true)
-    μ, σ = cu(Float32.(mean(td.dist))), cu(Float32.(sqrt.(var(td.dist))))
-    push!(ds, LayerDesc(MVNORMAL_DIAG, 0, 0, 0, 0, 0, 0f0, 0f0, pointer(μ), pointer(σ), NULLF, NULLF, NULLI, NULLI))
-    GC.@preserve μ σ last(run_chain(ds, y; y=nothing))
+    term, keep = base_desc(td.dist)
+    push!(ds, term)
+    GC.@preserve keep last(run_chain(ds, y; y=nothing))
 end
 
 # ---- multi-GPU (one process per GPU): one NCCL sum of the batch log-density (SURVEY §8(e)) ------------

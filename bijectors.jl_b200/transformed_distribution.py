@@ -21,11 +21,26 @@ from .interface import Transform, _batch_view, inverse, run_chain
 from .layers import _desc, _dev_f32
 
 
-class MvNormal:
-    """MvNormal(μ, Diagonal(σ²)) / MvNormal(zeros(D), I) (Distributions + PDMats; third-party arithmetic
-    restated in the kernel: −(D·log2π + Σ log σ²)/2 − Σ((x−μ)/σ)²/2).  `sigma` is the std-dev vector."""
+class PosDefException(ValueError):
+    """A covariance matrix whose Cholesky factorisation fails (LinearAlgebra's PosDefException, raised by PDMats)."""
 
-    def __init__(self, D: int, mu=None, sigma=None, device="cuda", dtype=torch.float32):
+
+class MvNormal:
+    """MvNormal(μ, Diagonal(σ²)) / MvNormal(zeros(D), I) / MvNormal(μ, Σ) (Distributions + PDMats; third-party arithmetic
+    restated in the kernels).
+
+    * ``sigma``: the std-dev vector of a diagonal covariance, −(D·log2π + Σ log σ²)/2 − Σ((x−μ)/σ)²/2 (B2B_MVNORMAL_DIAG).
+    * ``cov``: a dense D × D covariance Σ -- Distributions' FullNormal.  It is factorised once, in float64, into its lower
+      Cholesky factor L (what the PDMat holds); a matrix that is not positive definite raises PosDefException.
+    * ``scale_tril``: that factor L directly (lower triangle read, diagonal > 0), which is what a trainable base needs.
+      −D·log2π/2 − Σ log Lᵢᵢ − ‖L⁻¹(x−μ)‖²/2 (B2B_MVNORMAL_TRIL): Float32 up to D = 256, Float64 up to D = 2048 (no
+      Float64 sampler: ``rand`` raises TypeError).
+
+    At most one of ``sigma``, ``cov`` and ``scale_tril`` may be given."""
+
+    def __init__(self, D: int, mu=None, sigma=None, *, cov=None, scale_tril=None, device="cuda", dtype=torch.float32):
+        if sum(v is not None for v in (sigma, cov, scale_tril)) > 1:
+            raise ValueError("MvNormal: give at most one of sigma, cov and scale_tril")
         self.D = int(D)
         self.dtype = dtype
         self.mu = None if mu is None else _dev_f32(mu, device, dtype)
@@ -34,17 +49,39 @@ class MvNormal:
         for t in (self.mu, self.sigma):
             if t is not None and t.numel() != self.D:
                 raise ValueError("DimensionMismatch: MvNormal parameter length")
+        if cov is not None:
+            c = torch.as_tensor(np.asarray(cov.detach().cpu() if isinstance(cov, torch.Tensor) else cov, np.float64))
+            if c.shape != (self.D, self.D):
+                raise ValueError(f"DimensionMismatch: covariance of shape {tuple(c.shape)} for a {self.D}-dim MvNormal")
+            scale_tril, info = torch.linalg.cholesky_ex(c)
+            if int(info) != 0:
+                raise PosDefException(f"matrix is not positive definite; Cholesky factorization failed (leading minor "
+                                      f"{int(info)})")
+        # L is held column-major -- the layout the library reads -- as the row-major D × D tensor Lᵀ
+        self._tril = None
+        if scale_tril is not None:
+            L = scale_tril.detach() if isinstance(scale_tril, torch.Tensor) else torch.as_tensor(np.asarray(scale_tril))
+            if tuple(L.shape) != (self.D, self.D):
+                raise ValueError(f"DimensionMismatch: scale_tril of shape {tuple(L.shape)} for a {self.D}-dim MvNormal")
+            self._tril = L.to(device=device, dtype=dtype).t().contiguous()
+
+    @property
+    def scale_tril(self) -> Optional[torch.Tensor]:
+        """The lower Cholesky factor L (a view of the device storage), or None for a diagonal covariance."""
+        return None if self._tril is None else self._tril.t()
 
     def __len__(self):
         return self.D
 
     def _terminal_desc(self):
+        if self._tril is not None:
+            return _desc(_lib.MVNORMAL_TRIL, False, p0=self.mu, p1=self._tril)
         return _desc(_lib.MVNORMAL_DIAG, False, p0=self.mu if self.mu is not None else None,
                      p1=self.sigma if self.sigma is not None else None, _f64=self.dtype == torch.float64)
 
     def rand(self, n: int, seed: Optional[int] = None, offset: int = 0, column_offset: int = 0) -> torch.Tensor:
-        """D×n base samples mu + sigma .* z (column-major) from the library's Philox4x32-10 + Box-Muller stream
-        (b2b_randn_f32): a pure function of (seed, offset, global column, row)."""
+        """D×n base samples mu + sigma .* z, or mu + L z (column-major), from the library's Philox4x32-10 + Box-Muller
+        stream (b2b_randn_f32): a pure function of (seed, offset, global column, row)."""
         return _sample(self, (), n, seed, offset, column_offset, want_logjac=False)[0]
 
 
@@ -107,6 +144,8 @@ def _sample(dist: MvNormal, transform, n: int, seed, offset, column_offset, want
 
     import ctypes
 
+    if dist._tril is not None and dist.dtype != torch.float32:
+        raise TypeError("rand: a Float64 full-covariance MvNormal has no device sampler (construct it with dtype=torch.float32)")
     D = dist.D
     if isinstance(transform, tuple):
         descs = list(transform)
@@ -119,6 +158,14 @@ def _sample(dist: MvNormal, transform, n: int, seed, offset, column_offset, want
     lj = torch.empty((n,), dtype=torch.float32, device=y.device) if want_logjac else None
     ws_bytes = lib().b2b_chain_workspace_bytes(arr, L, D, n, 1, 0) if L else 0
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=y.device) if ws_bytes else None
+    if dist._tril is not None:
+        rc = lib().b2b_chain_sample_tril_f32(
+            arr, L, dist.mu.data_ptr() if dist.mu is not None else None, dist._tril.data_ptr(),
+            ctypes.c_uint64(_seed(seed)), ctypes.c_uint64(int(offset)), int(column_offset), y.data_ptr(),
+            lj.data_ptr() if lj is not None else None, D, n, D, ws.data_ptr() if ws is not None else None, ws_bytes,
+            _stream())
+        check(rc, "b2b_chain_sample_tril_f32")
+        return y, lj
     rc = lib().b2b_chain_sample_f32(
         arr, L, dist.mu.data_ptr() if dist.mu is not None else None, dist.sigma.data_ptr() if dist.sigma is not None else None,
         ctypes.c_uint64(_seed(seed)), ctypes.c_uint64(int(offset)), int(column_offset), y.data_ptr(),
@@ -146,8 +193,9 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     layers and base) through inverse(td.transform) and the terminal MvNormal.  ``lpbar`` (N, None = ones in ``y``'s dtype)
     is the cotangent of the logpdf vector.  Returns ``(ybar, flow_grads, base_grads)``:
     ``flow_grads`` one dict per leaf of ``flatten(td.transform)`` in FLOW order (see chain_vjp for the keys) and
-    ``base_grads`` = {"μ", "σ"} for the base parameters that are given; all summed over the columns of this batch."""
-    from .interface import _chain_vjp_raw, _leaf_descs, _leaf_grads, _trainable_slots
+    ``base_grads`` = {"μ", "σ"} (or {"μ", "L"} for a full-covariance base, L̄ lower triangular) for the base parameters
+    that are given; all summed over the columns of this batch."""
+    from .interface import _SLOT_NAMES, _chain_vjp_raw, _leaf_descs, _leaf_grads, _trainable_slots
 
     D, N, _ = _batch_view(y)
     if D != len(td.dist):
@@ -160,5 +208,7 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     ybar, bars = _chain_vjp_raw(descs, y, None, lpbar, want)
     flow = _leaf_grads(descs, counts, bars)[::-1]
     T = len(descs) - 1
-    base = {name: bars[(T, i)] for i, name in enumerate(("μ", "σ")) if (T, i) in bars}
+    base = {name: bars[(T, i)] for i, name in enumerate(_SLOT_NAMES[descs[T].kind]) if (T, i) in bars}
+    if "L" in base:
+        base["L"] = base["L"].t()  # the cotangent's storage is column-major, like L's
     return ybar, flow, base

@@ -62,6 +62,7 @@ extern "C" {
 #define B2B_PERMUTE 6         /* Permute                    src/bijectors/permute.jl                 */
 #define B2B_STACKED_EW 7      /* Stacked of elementwise laws on row ranges  src/bijectors/stacked.jl */
 #define B2B_MVNORMAL_DIAG 8   /* terminal op: logpdf of MvNormal(mu, Diagonal(sigma.^2)) + logjac    */
+#define B2B_MVNORMAL_TRIL 9   /* terminal op: logpdf of MvNormal(mu, L*L') (L lower Cholesky factor) + logjac */
 
 /* elementwise law codes for B2B_STACKED_EW (one code per row) */
 #define B2B_EW_IDENTITY 0
@@ -95,6 +96,13 @@ extern "C" {
  *                    (a = the law's parameter: Shift / Scale / LeakyReLU value, Logit / Truncated lower bound;
  *                     b = second parameter: Logit / Truncated upper bound)
  * MVNORMAL_DIAG      mu[D]|NULL  sigma[D]|NULL -         -        -               -             -     -    -
+ * MVNORMAL_TRIL      mu[D]|NULL  L[D x D]    -           -        -               -             -     -    -
+ *                    (Distributions' FullNormal MvNormal(mu, Σ) with Σ = L Lᵀ: L column-major, required; only its lower
+ *                     triangle is read, the strictly upper entries are ignored.  Lᵢᵢ > 0 is the caller's contract -- what
+ *                     `cholesky` guarantees; nothing on the device checks it, and a non-positive diagonal gives NaN / −Inf.
+ *                     Like MVNORMAL_DIAG it must be the last element with inverse == 0, else B2B_EINVAL.  Float32:
+ *                     D <= 256, Float64 (b2b_layer_desc_f64, L read through L2): D <= 2048; B2B_EUNSUPPORTED beyond.)
+ * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
   int32_t kind;
@@ -134,6 +142,13 @@ const char* b2b_status_string(int status);
  * accumulated logjac (transformed_distribution.jl:165-169 when the preceding layers are the inverse
  * chain) and, when sum_out != NULL, *sum_out (device double) receives Σ_n logpdf[n] (fixed summation
  * order, deterministic).
+ * B2B_MVNORMAL_TRIL as the last element does the same for MvNormal(mu, L Lᵀ).  It runs as its own launch after the
+ * preceding layers (which write the recovered x to y, or to the D x N scratch of the workspace when y == NULL), so it costs
+ * 8·D B/sample more HBM traffic than a terminal fused into the last column-local launch; the launch stages the packed lower
+ * triangle of L in shared memory (Float32 D <= 256, B2B_EUNSUPPORTED beyond, nothing launched) and is bound by the
+ * D(D+1)/2 FP32 FMA per sample of the whitening solve L⁻¹(x − mu).  With layers before it, sum_out needs `logjac`
+ * (without it the log-Jacobians of the preceding layers travel through an N-float slice of the workspace, which
+ * b2b_chain_workspace_bytes includes for a TRIL-terminated chain of several elements when want_sum != 0).
  * workspace: device scratch of at least b2b_chain_workspace_bytes(...) bytes (may be NULL when 0).
  */
 int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const float* x, float* y, float* logjac,
@@ -244,7 +259,7 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
                     float* widths_bar, float* heights_bar, float* derivs_bar, int32_t D, int64_t N, int64_t ldx,
                     int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes, void* stream);
 /* Reverse mode of b2b_chain_run_f32: the vector-Jacobian product through ANY chain it accepts -- layers in application
- * order with their `inverse` flags, optionally ending in the terminal B2B_MVNORMAL_DIAG (then the logjac output is
+ * order with their `inverse` flags, optionally ending in the terminal B2B_MVNORMAL_DIAG / _TRIL (then the logjac output is
  * logpdf).  What the reference's reverse-mode AD computes for `with_logabsdet_jacobian(flow, x)` or
  * `logpdf(transformed(base, flow), y)` (docs/src/flows.md:93-100).
  * Inputs: `x`, the batch the chain was applied to; `ybar` (D x N) the cotangent of the y that b2b_chain_run_f32 writes
@@ -253,12 +268,16 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * 4*L pointers: entry 4l+i receives the cotangent of layers[l].p<i> in the shape and layout of p<i> (NULL entries are not
  * computed), summed over the N columns in a fixed order (deterministic; a multi-GPU caller all-reduces them).
  * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c;
- * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL).  Any other
- * non-NULL entry (BatchNorm m / v, PERMUTE, STACKED_EW) returns B2B_EUNSUPPORTED.
+ * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
+ * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
+ * (BatchNorm m / v, PERMUTE, STACKED_EW, MVNORMAL_TRIL slots 2-3) returns B2B_EUNSUPPORTED.
  * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
  * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling /
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
- * differentiates.  The forward is recomputed once to checkpoint each segment's input, then the segments are
+ * differentiates; a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
+ * launch; with μ̄ / L̄ requested it also stores r = L⁻¹(x − μ) and l̄·L⁻ᵀr (2·D·N floats of workspace), and two more
+ * launches form L̄ = tril(Σ l̄ s rᵀ) over at most 64 column chunks (P·D·(D+1) floats of chunk partials, P = min(ceil(N /
+ * 4096), 64)) and reduce the chunks in order.  The forward is recomputed once to checkpoint each segment's input, then the segments are
  * differentiated last to first.  Limits are the kernels': planar and radial D <= 128, RQS D <= 256 and K1 <= 64, coupling
  * n1, n2 <= 128 and D <= 747 at n1 = n2 = 128 (see b2b_coupling_affine_vjp_f32), BatchNorm and elementwise runs D <= 1024,
  * and the forward recompute those of b2b_chain_run_f32; an unsupported chain returns B2B_EUNSUPPORTED before anything
@@ -374,12 +393,13 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
                       void* workspace, size_t workspace_bytes, void* stream);
 /* Reverse mode of b2b_chain_run_f64: the contract of b2b_chain_vjp_f32 with double everywhere.  Any chain
  * b2b_chain_run_f64 accepts (every kind, either direction, mixed, L <= B2B_MAX_CHAIN, D <= 2048, optionally ending in
- * the terminal B2B_MVNORMAL_DIAG, whose logjac output is then logpdf).  `xbar` (D x N, required) must not overlap `x` or
+ * the terminal B2B_MVNORMAL_DIAG or B2B_MVNORMAL_TRIL, whose logjac output is then logpdf).  `xbar` (D x N, required) must not overlap `x` or
  * `ybar` (B2B_EINVAL); NULL `ybar` / `ljbar` are zeros; `param_bars` (NULL = x̄ only) holds 4*L pointers, entry 4l+i the
  * cotangent of layers[l].p<i> in its shape and layout, summed over the N columns.  Trainable slots as for Float32: PLANAR
  * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; BATCHNORM b
- * logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); any other non-NULL entry
- * returns B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
+ * logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
+ * p0 is NULL) and L (D x D column-major, exactly zero above the diagonal); any other non-NULL entry returns
+ * B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
  * parameter cotangents.  One warp per column recomputes the forward with the arithmetic of b2b_chain_run_f64, keeping
  * each layer's input in a tape, then differentiates the layers last to first; parameter cotangents accumulate in
  * per-warp slots that a second kernel sums in a fixed order (deterministic, no atomics) and a third turns into the
@@ -387,8 +407,8 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * kernels and fills enqueued (1, or 3 with parameter cotangents).
  * Workspace (b2b_chain_vjp_workspace_bytes_f64; 0 exactly when the call refuses the chain) is bounded independently of N:
  * W warp slots of 8·(T + P) bytes plus 8·P, with T = Lf·D (Lf: layers before the MvNormal) and P the accumulators, per
- * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, BATCHNORM / MVNORMAL_DIAG 2D doubles (each rounded up
- * to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
+ * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, BATCHNORM / MVNORMAL_DIAG 2D, MVNORMAL_TRIL
+ * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
  * 256 MiB but never below one CTA -- so the bound exceeds 256 MiB only when one CTA's slots do (e.g. wide couplings with
  * 2n1·n2 in the millions).  The number of warps, and with it the summation order, depends only on the chain, D and N. */
 size_t b2b_chain_vjp_workspace_bytes_f64(const b2b_layer_desc_f64* layers, int32_t L, int32_t D, int64_t N);
@@ -412,6 +432,14 @@ int b2b_randn_f32(float* z, const float* mu, const float* sigma, uint64_t seed, 
 int b2b_chain_sample_f32(const b2b_layer_desc* layers, int32_t L, const float* mu, const float* sigma, uint64_t seed,
                          uint64_t offset, int64_t column_offset, float* y, float* logjac, int32_t D, int64_t N,
                          int64_t ldy, void* workspace, size_t workspace_bytes, void* stream);
+/* rand(td, n) for the base MvNormal(mu, L Lᵀ) (B2B_MVNORMAL_TRIL): y = mu + L z (PDMats' unwhiten), z the SAME stream
+ * b2b_randn_f32 draws for (seed, offset, global column, row) with mu = sigma = NULL, then layers[0..L) applied in place
+ * (two passes; L = 0 returns the base samples and zeroes `logjac` when given).  `scale_tril` (D x D column-major, lower
+ * triangle read) is required; `mu` may be NULL.  D <= 256 (B2B_EUNSUPPORTED beyond, nothing launched); a chain
+ * b2b_chain_run_f32 refuses is refused before anything is launched.  workspace as for b2b_chain_run_f32 on the chain. */
+int b2b_chain_sample_tril_f32(const b2b_layer_desc* layers, int32_t L, const float* mu, const float* scale_tril,
+                              uint64_t seed, uint64_t offset, int64_t column_offset, float* y, float* logjac, int32_t D,
+                              int64_t N, int64_t ldy, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- host-buffer entry point (what a caller holding plain host Arrays uses; the bench's `e2e`) ----
  * Streams the batch through the device in column chunks: H2D copy, chain kernels and D2H copy of
