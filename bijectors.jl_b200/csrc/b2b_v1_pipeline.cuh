@@ -40,10 +40,11 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, uint32_t src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
+// Stores carry an L2 cache policy (`pol`, see l2_evict_first)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, uint32_t src, uint64_t pol) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
-               "r"(c0), "r"(c1), "r"(src)
+               "r"(c0), "r"(c1), "r"(src), "l"(pol)
                : "memory");
 }
 // 3-D forms: the tensor map views a batch as {32 floats, N columns, D/32 row-blocks} so that ONE instruction moves
@@ -54,11 +55,17 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, int c0, int c1, int c2, uint32_t src) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, int c0, int c1, int c2, uint32_t src, uint64_t pol) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2, %3}], [%4], %5;" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
-               "r"(c0), "r"(c1), "r"(c2), "r"(src)
+               "r"(c0), "r"(c1), "r"(c2), "r"(src), "l"(pol)
                : "memory");
+}
+// L2 policy that makes the lines it tags the first candidates for eviction (createpolicy, PTX ISA 7.4)
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -426,12 +433,15 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
       fence_proxy_async();
       __syncwarp();
       if (lane == 0) {
+        // The output tile is written once and not read again by this launch, so it is stored with evict-first L2
+        // priority (8-layer D = 128 chain, N = 2^20, on an H100 at a 400 W limit: 0.394 instead of 0.415 ms)
+        const uint64_t pol = l2_evict_first();
         if (E.tma3d) {
-          tma_store_3d(&map_y, 0, (int)(tile * COLS), 0, smem_u32(my_out));
+          tma_store_3d(&map_y, 0, (int)(tile * COLS), 0, smem_u32(my_out), pol);
         } else {
 #pragma unroll
           for (int q = 0; q < NQ; ++q)
-            tma_store_2d(&map_y, q * 32, (int)(tile * COLS), smem_u32(my_out + q * BOX_BYTES));
+            tma_store_2d(&map_y, q * 32, (int)(tile * COLS), smem_u32(my_out + q * BOX_BYTES), pol);
         }
         tma_commit();
       }
