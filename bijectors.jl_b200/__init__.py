@@ -12,7 +12,7 @@ from .interface import (  # noqa: F401
 )
 from .layers import (  # noqa: F401
     AffineConditioner, Coupling, Elementwise, InvertibleBatchNorm, LeakyReLU, Logit, PartitionMask, Permute, PlanarLayer, RadialLayer,
-    RationalQuadraticSpline, Scale, Shift, Stacked, TruncatedBijector, coupling, elementwise,
+    RationalQuadraticSpline, Scale, Shift, SplineConditioner, Stacked, TruncatedBijector, coupling, elementwise,
 )
 from .transformed_distribution import (  # noqa: F401
     MvNormal, PosDefException, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, transformed,

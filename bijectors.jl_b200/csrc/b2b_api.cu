@@ -87,6 +87,11 @@ static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
     case B2B_MVNORMAL_TRIL:
       if (!last || d.inverse || !d.p1) return B2B_EINVAL;
       break;
+    case B2B_COUPLING_RQS:
+      if (!d.p0 || !d.i0 || !d.i1 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D || d.n2 < 1 || !(d.f0 > 0.f))
+        return B2B_EINVAL;
+      if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
+      break;
     default:
       return B2B_EINVAL;
   }
@@ -173,13 +178,14 @@ extern "C" size_t b2b_coupling_workspace_bytes(int32_t n1, int32_t n2) {
   return b ? align_up(b, 1024) + 1024 : 0;
 }
 
-// A launch of the chain: a run of fusable layers, one coupling layer (with the BatchNorm neighbours folded into it), or
-// the terminal MVNORMAL_TRIL.
+// A launch of the chain: a run of fusable layers, one coupling layer (with the BatchNorm neighbours folded into it), one
+// spline coupling layer, or the terminal MVNORMAL_TRIL.
 struct Seg {
   int begin, end;
   bool coupling;
   int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
   bool tril = false;
+  bool spline = false;
 };
 
 // Cuts the chain into launches before anything is enqueued: single coupling layers, and maximal runs of fusable layers
@@ -191,6 +197,12 @@ static int plan_segments(const b2b_layer_desc* layers, int32_t L, int32_t D, std
     if (layers[l].kind == B2B_COUPLING_AFFINE) {
       if (!b2b_coupling_affine_fits(layers[l].n0, layers[l].n1, D)) return B2B_EUNSUPPORTED;
       segs.push_back({l, l + 1, true, -1, -1});
+      ++l;
+      continue;
+    }
+    if (layers[l].kind == B2B_COUPLING_RQS) {  // its own launch; BatchNorm neighbours keep theirs
+      if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
+      segs.push_back({l, l + 1, false, -1, -1, false, true});
       ++l;
       continue;
     }
@@ -236,6 +248,8 @@ static bool tril_terminal(const b2b_layer_desc* layers, int32_t L) {
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
                                             int want_y, int want_sum) {
   if (tril_terminal(layers, L) && D > B2B_TRIL_MAX_D) return 0;  // the call refuses the chain
+  for (int l = 0; layers && l < L; ++l)
+    if (layers[l].kind == B2B_COUPLING_RQS && !b2b_coupling_rqs_fits(layers[l], D)) return 0;
   size_t bytes = chain_tc_bytes(layers, L, D);
   // a D x N scratch matrix is needed only when y == NULL but the chain has more than one segment
   if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
@@ -334,7 +348,7 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   }
   double* partials = nullptr;
   if (sum_out) {
-    if (segs.back().coupling) return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
+    if (segs.back().coupling || segs.back().spline) return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
     if (ws_left < 4096 * sizeof(double)) return B2B_EWORKSPACE;
     partials = reinterpret_cast<double*>(ws);
   }
@@ -372,6 +386,10 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
         if (rc == B2B_OK) ++g_last_launches;
       }
       if (rc != B2B_OK) return rc;
+    } else if (segs[s].spline) {
+      rc = b2b_launch_coupling_rqs(layers[segs[s].begin], cur, dst, logjac, D, N, cur_ld, dst_ld, lj_started ? 1 : 0, stream);
+      if (rc != B2B_OK) return rc;
+      ++g_last_launches;
     } else if (segs[s].tril) {  // always the last segment
       rc = b2b_launch_mvnormal_tril(layers[segs[s].begin], cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0,
                                     sum_out ? partials : nullptr, D, N, stream);
@@ -701,7 +719,7 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
 // the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
 namespace {
 
-enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL };
+enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL, VK_SPLINE };
 
 struct VSeg {
   int kind, begin, end;
@@ -740,6 +758,10 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
         if (D > 1024) return B2B_EUNSUPPORTED;
         s.kind = VK_BN;
         break;
+      case B2B_COUPLING_RQS:
+        if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
+        s.kind = VK_SPLINE;
+        break;
       case B2B_MVNORMAL_TRIL:  // the terminal, alone
         if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
         s.kind = VK_TRIL;
@@ -776,6 +798,7 @@ size_t seg_param_floats(const b2b_layer_desc* layers, const VSeg& s, int D) {
     case VK_RQS: return 3 * r((size_t)D * d.n0);
     case VK_COUPLING: return r((size_t)2 * d.n0 * d.n1) + r((size_t)2 * d.n0);
     case VK_BN: return 2 * r(D);
+    case VK_SPLINE: return r((size_t)(3 * d.n2 - 1) * d.n0 * d.n1) + r((size_t)(3 * d.n2 - 1) * d.n0);
     default: return 0;
   }
 }
@@ -790,6 +813,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case VK_COUPLING: return b2b_coupling_affine_vjp_workspace_bytes(d.n0, d.n1);
     case VK_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
     case VK_TRIL: return b2b_tril_vjp_workspace(D, N);
+    case VK_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
     default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
   }
 }
@@ -830,6 +854,7 @@ size_t slot_len(const b2b_layer_desc& d, int i, int D) {
     case B2B_RQS: return (size_t)D * d.n0;
     case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
+    case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }
@@ -870,6 +895,7 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
           if (i == 3) return B2B_EUNSUPPORTED;
           break;
         case B2B_COUPLING_AFFINE:
+        case B2B_COUPLING_RQS:
           if (i >= 2) return B2B_EUNSUPPORTED;
           if (i == 1 && !d.p1) return B2B_EINVAL;
           break;
@@ -1094,6 +1120,15 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       const bool mvn = ls[n - 1].kind == B2B_MVNORMAL_DIAG;
       rc = b2b_launch_ew_vjp(ls, n, in, ldin, cin, ldcin, ljbar, out, ldout, mvn ? bar(sg.end - 1, 0) : nullptr,
                              mvn ? bar(sg.end - 1, 1) : nullptr, D, N, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+    } else if (sg.kind == VK_SPLINE) {
+      // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c
+      const b2b_layer_desc& d = ls[0];
+      float* wb = bar(sg.begin, 0) ? bar(sg.begin, 0) : scratch;
+      float* cb = !d.p1 ? nullptr : bar(sg.begin, 1) ? bar(sg.begin, 1)
+                                                       : scratch + ((slot_len(d, 0, D) + 63) & ~(size_t)63);
+      rc = b2b_launch_coupling_rqs_vjp(d, in, ldin, cin, ldcin, ljbar, out, ldout, wb, cb, D, N, kws, kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
     } else if (sg.kind == VK_TRIL) {

@@ -1,0 +1,145 @@
+// Spline coupling layer, B2B_COUPLING_RQS (include/b2b.h): Coupling(x₂ -> RationalQuadraticSpline(…, B), mask)
+// (coupling.jl:206-228 with the normalising constructor rational_quadratic_spline.jl:109-123), forward and inverse, in
+// exact fp32 on the CUDA cores.
+//
+// Mapping.  A CTA owns a tile of CRQ_TN columns, one thread per column.  It stages the tile's x₂ rows in shared memory
+// ([m][column], padded pitch: conflict-free both ways), then walks the n1 transformed rows in order.  For each row i it
+// streams that row's (3K − 1) x n2 block of W through shared memory (W itself is up to 1.5 MB), and every thread forms its
+// column's 3K − 1 raw parameters with an FMA GEMM over x₂, normalises them into K + 1 knots, builds the per-bin constants
+// of rqs_element in a table row of its own, and evaluates the element with rqs_element (b2b_device.cuh), the same element
+// function the fused RQS programs use.  The log-Jacobian is summed over the rows in increasing order by the column's
+// thread, so it is deterministic.  x₂ and x₃ rows are copied bit-exactly (nothing is copied in place).
+#include <cuda_runtime.h>
+
+#include "b2b_coupling_rqs.cuh"
+#include "b2b_device.cuh"
+#include "b2b_internal.h"
+
+namespace b2b {
+
+constexpr int CRQ_TN = 128;
+
+struct CrqParams {
+  const float* x;
+  float* y;
+  float* logjac;
+  const float *W, *c;
+  const int *idx1, *idx2;
+  long long N, ldx, ldy;
+  int D, n1, n2, K, accumulate;
+  float B;
+};
+
+// floats of the per-thread rqs_element table: Sw[KP] | Sh[KP] | 2 float4 per bin
+static __host__ __device__ inline int crq_tab_floats(int K) { return 2 * rqs_kp(K + 1) + 8 * (K + 1); }
+
+template <bool INV>
+__global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_constant__ CrqParams P) {
+  extern __shared__ __align__(16) float crq_sm[];
+  constexpr int TN = CRQ_TN, XP = CRQ_TN + 1;
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, K = P.K, K1 = K + 1, KP = rqs_kp(K1), J = 3 * K - 1;
+  const int JP = crq_jp(K), D = P.D;
+  float* tab = crq_sm;                              // rqs_element table, one row per thread (Dp = TN)
+  float* Ws = tab + crq_tab_floats(K) * TN;         // [n2][JP]
+  float* cs = Ws + n2 * JP;                         // [JP]
+  float* Xs = cs + JP;                              // [n2][XP]
+  float* Pr = Xs + n2 * XP;                         // [J][TN] raw parameters
+  unsigned char* x1row = reinterpret_cast<unsigned char*>(Pr + J * TN);  // [D]: 1 = a transformed row
+  const long long n0 = (long long)blockIdx.x * TN, n = n0 + tid;
+  const int cols = (int)min((long long)TN, P.N - n0);
+  const bool active = tid < cols;
+
+  for (int r = tid; r < D; r += TN) x1row[r] = 0;
+  __syncthreads();
+  for (int i = tid; i < n1; i += TN) x1row[P.idx1[i]] = 1;
+  for (int e = tid; e < n2 * TN; e += TN) {
+    const int c = e / n2, m = e - c * n2;
+    Xs[m * XP + c] = c < cols ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
+  }
+  __syncthreads();
+  if (P.y && (P.y != P.x || P.ldy != P.ldx))  // x₂ and x₃ pass through
+    for (int e = tid; e < cols * D; e += TN) {
+      const int c = e / D, r = e - c * D;
+      if (!x1row[r]) P.y[(n0 + c) * P.ldy + r] = P.x[(n0 + c) * P.ldx + r];
+    }
+
+  float* Sw = tab + tid * KP;
+  float* Sh = tab + TN * KP + tid * KP;
+  float4* cf = reinterpret_cast<float4*>(tab + 2 * TN * KP) + tid * K1 * 2;
+  const float inf = __int_as_float(0x7f800000);
+  float lj = 0.f;
+  for (int i = 0; i < n1; ++i) {
+    __syncthreads();  // the previous row's block of W is no longer read
+    crq_stage_row(P.W, P.c, i, n1, n2, K, Ws, cs, tid, TN);
+    __syncthreads();
+    crq_params(Ws, cs, Xs + tid, XP, n2, K, Pr + tid, TN);
+    crq_knots(Pr + tid, TN, K, P.B, Sw, 1);
+    crq_knots(Pr + K * TN + tid, TN, K, P.B, Sh, 1);
+    for (int k = K1; k < KP; ++k) Sw[k] = Sh[k] = inf;
+    // per-bin constants, as stage_layer(B2B_RQS) computes them from the processed arrays (derivatives: 1, log1pexp, 1)
+    const float Wl = Sw[K], Hl = Sh[K];
+    float dprev = 1.f;
+    for (int k = 0; k < K1; ++k) {
+      const float dcur = (k == 0 || k == K) ? 1.0f : softplus(Pr[(2 * K + k - 1) * TN + tid]);
+      const float w_k = k == 0 ? -Wl : Sw[k - 1], w = Sw[k] - w_k;
+      const float h_k = k == 0 ? -Hl : Sh[k - 1], dy = Sh[k] - h_k;
+      const float d_k = k == 0 ? 1.0f : dprev, d_k1 = dcur;
+      const float sl = dy / w;
+      cf[2 * k + 0] = make_float4(w_k, 1.0f / w, w, h_k);
+      cf[2 * k + 1] = make_float4(dy, sl, d_k, d_k1 + d_k - 2.0f * sl);
+      dprev = dcur;
+    }
+    if (active) {
+      const int row = P.idx1[i];
+      float out, l;
+      rqs_element<INV>(tab, K1, KP, TN, tid, P.x[n * P.ldx + row], out, l);
+      if (P.y) P.y[n * P.ldy + row] = out;
+      lj += l;
+    }
+  }
+  if (active && P.logjac) P.logjac[n] = P.accumulate ? P.logjac[n] + lj : lj;
+}
+
+static size_t crq_smem_bytes(int n2, int K, int D) {
+  const int J = 3 * K - 1, JP = crq_jp(K);
+  const size_t f = (size_t)crq_tab_floats(K) * CRQ_TN + (size_t)n2 * JP + JP + (size_t)n2 * (CRQ_TN + 1) + (size_t)J * CRQ_TN;
+  return (f * sizeof(float) + D + 15) & ~(size_t)15;
+}
+
+}  // namespace b2b
+
+bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D) {
+  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_RQS_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_RQS_MAX_N &&
+         d.n2 >= 2 && d.n2 <= B2B_COUPLING_RQS_MAX_K && D <= B2B_COUPLING_RQS_MAX_D;
+}
+
+int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
+                            long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
+  using namespace b2b;
+  if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (N <= 0) return B2B_OK;
+  CrqParams P;
+  P.x = x;
+  P.y = y;
+  P.logjac = logjac;
+  P.W = d.p0;
+  P.c = d.p1;
+  P.idx1 = d.i0;
+  P.idx2 = d.i1;
+  P.N = N;
+  P.ldx = ldx;
+  P.ldy = ldy;
+  P.D = D;
+  P.n1 = d.n0;
+  P.n2 = d.n1;
+  P.K = d.n2;
+  P.accumulate = accumulate;
+  P.B = d.f0;
+  const size_t smem = crq_smem_bytes(d.n1, d.n2, D);
+  void (*kernel)(const CrqParams) = d.inverse ? coupling_rqs_kernel<true> : coupling_rqs_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return (int)e;
+  const long long tiles = (N + CRQ_TN - 1) / CRQ_TN;
+  kernel<<<(unsigned)tiles, CRQ_TN, smem, stream>>>(P);
+  return (int)cudaGetLastError();
+}

@@ -1,0 +1,255 @@
+// Reverse mode of the spline coupling layer, B2B_COUPLING_RQS, either direction: cotangents of the input and of the
+// conditioner's W and c -- what the reference's reverse-mode AD computes through coupling.jl:206-228 with the law
+// RationalQuadraticSpline(reshape(W·x₂ + c, …)..., B) (rational_quadratic_spline.jl:109-123, :317-357 / :183-220).
+//
+// Per column and transformed row i, the kernel recomputes the raw parameters v (crq_params) and the knots (crq_knots),
+// takes the processed-knot cotangents of the element from rqv_element (b2b_rqs_element.cuh, the RQS VJP's own element
+// function, knot-accurate in both directions) and pulls them back through the normaliser: a reverse cumsum and the
+// softmax pullback for widths and heights (crq_knots_vjp), r̄ = d̄·σ(r) for the derivatives.  With r̄ the (3K − 1)
+// cotangents of row i:  x̄₂ += W_iᵀ r̄,  c̄_i += Σ_n r̄,  W̄_i += Σ_n r̄ x₂ᵀ;  x̄₁ comes from the element, x̄₃ = ȳ₃.
+//
+// Mapping.  A fixed grid of G CTAs (at most one wave, fewer when the W̄ slices would pass 256 MiB) walks the column tiles
+// round-robin, one thread per column, the rows in order as the forward kernel does.  x̄₂ accumulates in shared memory
+// in fp64 (each element sums (3K − 1)·n1 products, which cancel).
+// After each row the CTA forms the (3K − 1) x n2 block Σ_n r̄ x₂ᵀ of its tile and adds it to a private slice of the
+// workspace ([n1][3K − 1][n2] then [n1][3K − 1] for c̄), owned element by element by one thread.  A second kernel sums
+// the G slices in order into W̄ (column-major like W) and c̄.  Deterministic, no atomics, workspace independent of N.
+#include <cuda_runtime.h>
+
+#include "b2b_coupling_rqs.cuh"
+#include "b2b_device.cuh"
+#include "b2b_internal.h"
+#include "b2b_rqs_element.cuh"
+
+namespace b2b {
+
+constexpr int CRV_TN = 64;
+
+struct CrvParams {
+  const float* x;
+  const float* ybar;
+  const float* ljbar;
+  float* xbar;
+  const float *W, *c;
+  const int *idx1, *idx2;
+  float* part;  // [G][slice]
+  long long N, ldx, ldyb, ldxb, slice;
+  int D, n1, n2, K;
+  float B;
+};
+
+template <bool INV>
+__global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __grid_constant__ CrvParams P) {
+  extern __shared__ __align__(16) float crv_sm[];
+  constexpr int TN = CRV_TN, XP = CRV_TN + 1;
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, K = P.K, K1 = K + 1, J = 3 * K - 1, JP = crq_jp(K), D = P.D;
+  float* Ws = crv_sm;               // [n2][JP]
+  float* cs = Ws + n2 * JP;         // [JP]
+  float* KT = cs + JP;              // knots W | H | Dv, [3][K1][TN]
+  float* G = KT + 3 * K1 * TN;      // their cotangents, same layout
+  float* Xs = G + 3 * K1 * TN;      // x₂ [n2][XP]
+  float* Pr = Xs + n2 * XP;         // raw parameters, then their cotangents [J][XP]
+  double* XB = reinterpret_cast<double*>(crv_sm) + ((size_t)(n2 * JP + JP + 6 * K1 * TN + n2 * XP + J * XP) + 1) / 2;
+  // x̄₂ [n2][XP] in fp64: it sums (3K − 1)·n1 products per element
+  unsigned char* kind = reinterpret_cast<unsigned char*>(XB + n2 * XP);  // [D]: 1 = x₁ row, 2 = x₂ row, 0 = x₃ row
+  float* slice = P.part + (size_t)blockIdx.x * P.slice;
+  float* cslice = slice + (size_t)n1 * J * n2;
+
+  for (int r = tid; r < D; r += TN) kind[r] = 0;
+  for (long long e = tid; e < (long long)n1 * J * (n2 + 1); e += TN) slice[e] = 0.f;
+  __syncthreads();
+  for (int i = tid; i < n1; i += TN) kind[P.idx1[i]] = 1;
+  for (int m = tid; m < n2; m += TN) kind[P.idx2[m]] = 2;
+
+  RqvKnots<INV, true> T;
+  T.W = KT + tid;
+  T.H = KT + K1 * TN + tid;
+  T.Dv = KT + 2 * K1 * TN + tid;
+  T.stride = TN;
+  float* dv = KT + 2 * K1 * TN + tid;
+  float* gw = G + tid;
+  float* gh = G + K1 * TN + tid;
+  float* gd = G + 2 * K1 * TN + tid;
+  const long long tiles = (P.N + TN - 1) / TN;
+  for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const long long n0 = t * TN, n = n0 + tid;
+    const int cols = (int)min((long long)TN, P.N - n0);
+    const bool active = tid < cols;
+    __syncthreads();  // the previous tile's x̄₂ has been stored
+    for (int e = tid; e < n2 * TN; e += TN) {
+      const int c = e / n2, m = e - c * n2;
+      const bool ok = c < cols;
+      Xs[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
+      XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
+    }
+    const float lb = active && P.ljbar ? P.ljbar[n] : 0.f;
+    for (int i = 0; i < n1; ++i) {
+      __syncthreads();  // Ws and every column's r̄ of the previous row are no longer read
+      crq_stage_row(P.W, P.c, i, n1, n2, K, Ws, cs, tid, TN);
+      __syncthreads();
+      crq_params(Ws, cs, Xs + tid, XP, n2, K, Pr + tid, XP);
+      crq_knots(Pr + tid, XP, K, P.B, KT + tid, TN);
+      crq_knots(Pr + K * XP + tid, XP, K, P.B, KT + K1 * TN + tid, TN);
+      dv[0] = 1.0f;
+      dv[K * TN] = 1.0f;
+      for (int j = 1; j < K; ++j) dv[j * TN] = softplus(Pr[(2 * K + j - 1) * XP + tid]);
+      for (int k = 0; k < K1; ++k) gw[k * TN] = gh[k * TN] = gd[k * TN] = 0.f;
+      if (active) {
+        const int row = P.idx1[i];
+        const float v = P.x[n * P.ldx + row];
+        const float cb = P.ybar ? P.ybar[n * P.ldyb + row] : 0.f;
+        const float Wl = T.w(K), Hl = T.h(K), Bs = INV ? Hl : Wl;
+        // identity outside the box: evaluated at 0 with zero cotangents, so every knot cotangent is an exact 0
+        const bool in = v > -Bs && v < Bs;
+        const float ve = in ? v : 0.f;
+        int kb = 0;
+        for (int j = 0; j < K; ++j) kb += T.s(j) < ve ? 1 : 0;
+        RqvCot c;
+        const float out = rqv_element<INV, true>(T, K1, kb, Wl, Hl, ve, in ? cb : 0.f, in ? lb : 0.f, c);
+        P.xbar[n * P.ldxb + row] = in ? out : cb;
+        const int ka = kb > 0 ? kb - 1 : K1 - 1;
+        gw[ka * TN] += c.xk;
+        gh[ka * TN] += c.yk;
+        gd[ka * TN] += c.dk;
+        gw[kb * TN] += c.xk1;
+        gh[kb * TN] += c.yk1;
+        gd[kb * TN] += c.dk1;
+      }
+      // pull the knot cotangents back to the raw parameters (zero for columns past the batch)
+      crq_knots_vjp(Pr + tid, XP, K, P.B, gw, TN);
+      crq_knots_vjp(Pr + K * XP + tid, XP, K, P.B, gh, TN);
+      for (int j = 0; j < K - 1; ++j) {
+        float* r = Pr + (2 * K + j) * XP + tid;
+        *r = gd[(j + 1) * TN] / (1.0f + expf(-*r));
+      }
+      for (int m = 0; m < n2; ++m) {
+        float s = 0.f;
+        for (int j = 0; j < J; ++j) s = fmaf(Ws[m * JP + j], Pr[j * XP + tid], s);
+        XB[m * XP + tid] += (double)s;
+      }
+      __syncthreads();
+      // this tile's Σ_n r̄ x₂ᵀ and Σ_n r̄ for row i, added to the CTA's slice (each element always by the same thread)
+      float* sl = slice + (size_t)i * J * n2;
+      for (int e = tid; e < J * n2; e += TN) {
+        const int j = e / n2, m = e - j * n2;
+        const float* pr = Pr + j * XP;
+        const float* xs = Xs + m * XP;
+        float s = 0.f;
+        for (int c = 0; c < cols; ++c) s = fmaf(pr[c], xs[c], s);
+        sl[e] += s;
+      }
+      for (int j = tid; j < J; j += TN) {
+        const float* pr = Pr + j * XP;
+        float s = 0.f;
+        for (int c = 0; c < cols; ++c) s += pr[c];
+        cslice[(size_t)i * J + j] += s;
+      }
+    }
+    __syncthreads();
+    for (int e = tid; e < n2 * TN; e += TN) {
+      const int c = e / n2, m = e - c * n2;
+      if (c < cols) P.xbar[(n0 + c) * P.ldxb + P.idx2[m]] = (float)XB[m * XP + c];
+    }
+    for (int e = tid; e < cols * D; e += TN) {  // x̄₃ = ȳ₃
+      const int c = e / D, r = e - c * D;
+      if (!kind[r]) P.xbar[(n0 + c) * P.ldxb + r] = P.ybar ? P.ybar[(n0 + c) * P.ldyb + r] : 0.f;
+    }
+  }
+}
+
+// W̄ / c̄: the G slices summed in order, element e of the slice layout scattered to W's column-major layout.
+__global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
+                                                                      long long slice, int n1, int n2, int K,
+                                                                      float* __restrict__ Wbar, float* __restrict__ cbar) {
+  const int J = 3 * K - 1;
+  const long long nw = (long long)n1 * J * n2, e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nw + (long long)n1 * J) return;
+  float t = 0.f;
+  for (int g = 0; g < nparts; ++g) t += part[(size_t)g * slice + e];
+  if (e < nw) {
+    const int i = (int)(e / ((long long)J * n2)), rem = (int)(e - (long long)i * J * n2), j = rem / n2, m = rem - j * n2;
+    if (Wbar) Wbar[(size_t)(i + n1 * j) + (size_t)J * n1 * m] = t;
+  } else {
+    const int f = (int)(e - nw), i = f / J, j = f - i * J;
+    if (cbar) cbar[i + n1 * j] = t;
+  }
+}
+
+static size_t crv_smem_bytes(int n2, int K, int D) {
+  const int J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
+  const size_t f = (size_t)n2 * JP + JP + (size_t)6 * K1 * CRV_TN + (size_t)n2 * (CRV_TN + 1) + (size_t)J * (CRV_TN + 1);
+  return (((f + 1) / 2 + (size_t)n2 * (CRV_TN + 1)) * sizeof(double) + D + 15) & ~(size_t)15;
+}
+
+static long long crv_slice_floats(const b2b_layer_desc& d) {
+  const long long f = (long long)d.n0 * (3 * d.n2 - 1) * (d.n1 + 1);
+  return (f + 63) & ~63LL;
+}
+
+static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sms <= 0) sms = 132;
+  int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(d.n1, d.n2, D) + 1024));
+  per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
+  long long g = (long long)sms * per_sm;
+  const long long tiles = (N + CRV_TN - 1) / CRV_TN;
+  if (g > tiles) g = tiles;
+  const long long cap = (256LL << 20) / (crv_slice_floats(d) * (long long)sizeof(float));
+  if (g > cap) g = cap;
+  return g < 1 ? 1 : (int)g;
+}
+
+}  // namespace b2b
+
+size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
+  using namespace b2b;
+  if (!b2b_coupling_rqs_fits(d, D)) return 0;
+  return (size_t)crv_grid(d, D, N) * (size_t)crv_slice_floats(d) * sizeof(float) + 256;
+}
+
+int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
+                                const float* ljbar, float* xbar, long long ldxb, float* Wbar, float* cbar, int D, long long N,
+                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+  using namespace b2b;
+  *launches = 0;
+  if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (N <= 0) return B2B_OK;
+  if (!workspace || workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
+  char* wsb = static_cast<char*>(workspace);
+  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  CrvParams P;
+  P.x = x;
+  P.ybar = ybar;
+  P.ljbar = ljbar;
+  P.xbar = xbar;
+  P.W = d.p0;
+  P.c = d.p1;
+  P.idx1 = d.i0;
+  P.idx2 = d.i1;
+  P.part = reinterpret_cast<float*>(wsb);
+  P.N = N;
+  P.ldx = ldx;
+  P.ldyb = ldyb;
+  P.ldxb = ldxb;
+  P.slice = crv_slice_floats(d);
+  P.D = D;
+  P.n1 = d.n0;
+  P.n2 = d.n1;
+  P.K = d.n2;
+  P.B = d.f0;
+  const int grid = crv_grid(d, D, N);
+  const size_t smem = crv_smem_bytes(d.n1, d.n2, D);
+  void (*kernel)(const CrvParams) = d.inverse ? coupling_rqs_vjp_kernel<true> : coupling_rqs_vjp_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return (int)e;
+  kernel<<<grid, CRV_TN, smem, stream>>>(P);
+  if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  const long long len = (long long)d.n0 * (3 * d.n2 - 1) * (d.n1 + 1);
+  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, stream>>>(P.part, grid, P.slice, d.n0, d.n1, d.n2,
+                                                                                    Wbar, cbar);
+  if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  *launches = 2;
+  return B2B_OK;
+}

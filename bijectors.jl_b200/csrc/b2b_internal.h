@@ -132,10 +132,21 @@ size_t b2b_tril_vjp_workspace(int D, long long N);
 int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
                         const float* ljbar, float* xbar, long long ldxb, float* mubar, float* Lbar, int D, long long N,
                         void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
+// spline coupling (b2b_coupling_rqs.cu, b2b_coupling_rqs_vjp.cu): whether the layer is within the envelope of include/b2b.h
+bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D);
+int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
+                            long long ldx, long long ldy, int accumulate, cudaStream_t stream);
+// reverse mode: x̄ always, W̄ / c̄ when non-NULL; b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the envelope,
+// bounded independently of N); two launches
+size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
+int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
+                                const float* ljbar, float* xbar, long long ldxb, float* Wbar, float* cbar, int D, long long N,
+                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
-// element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL.
+// element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
+// COUPLING_RQS).
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);

@@ -817,6 +817,7 @@ _SLOT_NAMES = {
     _lib.BATCHNORM: ("b", "logs"),
     _lib.MVNORMAL_DIAG: ("μ", "σ"),
     _lib.MVNORMAL_TRIL: ("μ", "L"),
+    _lib.COUPLING_RQS: ("W", "c"),
 }
 
 
@@ -836,6 +837,9 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
         return (d.n0, D)  # column-major D × K+1
     if d.kind == _lib.COUPLING_AFFINE:
         return (d.n1, 2 * d.n0) if i == 0 else (2 * d.n0,)  # W column-major (2n1 × n2)
+    if d.kind == _lib.COUPLING_RQS:
+        J = 3 * d.n2 - 1
+        return (d.n1, J * d.n0) if i == 0 else (J * d.n0,)  # W column-major ((3K−1)n1 × n2)
     if d.kind == _lib.MVNORMAL_TRIL and i == 1:
         return (D, D)  # L column-major: element (i, j) at [j, i]
     return (D,)
@@ -906,7 +910,7 @@ def _leaf_grads(descs, counts, bars) -> List[dict]:
             d = descs[l]
             for i in _trainable_slots(d):
                 t = bars[(l, i)]
-                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind == _lib.RQS or (d.kind == _lib.COUPLING_AFFINE and i == 0)) else t
+                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind == _lib.RQS or (d.kind in (_lib.COUPLING_AFFINE, _lib.COUPLING_RQS) and i == 0)) else t
         grads.append(g)
         k += c
     return grads

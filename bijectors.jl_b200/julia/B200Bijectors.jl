@@ -38,6 +38,7 @@ struct LayerDesc
     i0::CuPtr{Int32}; i1::CuPtr{Int32}
 end
 const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG, MVNORMAL_TRIL = Int32.(1:9)
+const COUPLING_RQS = Int32(11)  # 10 is not a layer kind (include/b2b.h)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
 const NULLI = CuPtr{Int32}(0)
@@ -92,7 +93,30 @@ function desc(cl::Coupling{<:AffineConditioner}, inv::Bool)
     LayerDesc(COUPLING_AFFINE, inv, length(dm.idx1), length(dm.idx2), dm.row1, dm.row2, 0f0, 0f0,
               pointer(cl.θ.W), pointer(cl.θ.c), NULLF, NULLF, pointer(dm.idx1), pointer(dm.idx2))
 end
-desc(cl::Coupling, ::Bool) = error("Coupling: only AffineConditioner laws run on the device path (no CPU fallback)")
+# The neural-spline coupling law (Durkan et al. 2019): θ(x₂) = RationalQuadraticSpline(reshape(v[1:n1K], n1, K),
+# reshape(v[n1K+1:2n1K], n1, K), reshape(v[2n1K+1:end], n1, K−1), B) with v = W*x₂ .+ c -- the reference's own normalising
+# constructor (rational_quadratic_spline.jl:109-123), so the same object also runs on the CPU reference path.  Float32,
+# n1, n2 <= 128, 2 <= K <= 16, D <= 1024 on the device; c === nothing is a zero shift.
+struct SplineConditioner{M<:AbstractMatrix,V}
+    W::M   # ((3K−1)·n1 × n2)
+    c::V   # (3K−1)·n1, or nothing
+    K::Int
+    B::Float32
+end
+function (θ::SplineConditioner)(x₂)
+    v = θ.c === nothing ? θ.W * x₂ : θ.W * x₂ .+ θ.c
+    n1, K = size(θ.W, 1) ÷ (3θ.K - 1), θ.K
+    RationalQuadraticSpline(reshape(v[1:(n1 * K)], n1, K), reshape(v[(n1 * K + 1):(2n1 * K)], n1, K),
+                            reshape(v[(2n1 * K + 1):end], n1, K - 1), θ.B)
+end
+function desc(cl::Coupling{<:SplineConditioner{<:CuMatrix{Float32}}}, inv::Bool)
+    dm = get!(() -> DeviceMask(cl.mask), MASKS, cl.mask)
+    θ = cl.θ
+    LayerDesc(COUPLING_RQS, inv, length(dm.idx1), length(dm.idx2), θ.K, 0, θ.B, 0f0,
+              pointer(θ.W), θ.c === nothing ? NULLF : pointer(θ.c), NULLF, NULLF, pointer(dm.idx1), pointer(dm.idx2))
+end
+desc(cl::Coupling, ::Bool) =
+    error("Coupling: only AffineConditioner and SplineConditioner laws run on the device path (no CPU fallback)")
 
 # Permute(A): y[dst[i]] = x[i] with dst = the row of the single 1 in column i (permute.jl:90-100,152)
 const PERMS = IdDict{Any,CuVector{Int32}}()
@@ -142,7 +166,7 @@ descs(f, inv::Bool) = inv ? [desc(b, true) for b in reverse(flatten(f))] : [desc
 
 const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVector{Float32}},
                           RationalQuadraticSpline{<:CuMatrix{Float32}},InvertibleBatchNorm{<:CuVector{Float32}},
-                          Coupling{<:AffineConditioner},Permute,Stacked}
+                          Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
 is_device(::DeviceLeaf) = true
@@ -349,6 +373,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == RADIAL && return (z(1), z(1), z(D))
     d.kind == RQS && return (z(D, d.n0), z(D, d.n0), z(D, d.n0))
     d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
+    d.kind == COUPLING_RQS && return (z((3d.n2 - 1) * d.n0, d.n1), d.p1 == NULLF ? nothing : z((3d.n2 - 1) * d.n0))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

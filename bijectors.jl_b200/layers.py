@@ -257,17 +257,56 @@ class AffineConditioner:
         return new
 
 
+class SplineConditioner:
+    """The neural-spline coupling law (Durkan et al. 2019) θ(x₂) = RationalQuadraticSpline(reshape(v[1:n1K], n1, K),
+    reshape(v[n1K+1:2n1K], n1, K), reshape(v[2n1K+1:end], n1, K−1), B) with v = W·x₂ + c -- the reference's own
+    constructor (rational_quadratic_spline.jl:109-123) applied to a linear conditioner.  W is ((3K−1)·n1 × n2) in the
+    reference's index order (row i + n1·k of v is row i, bin k of its block); c has (3K−1)·n1 entries (None = no shift,
+    the descriptor's c is NULL).  Float32 only.  Runs as B2B_COUPLING_RQS: n1, n2 <= 128, 2 <= K <= 16, D <= 1024."""
+
+    def __init__(self, W, c=None, *, K: int, B: float, device="cuda", dtype=torch.float32):
+        if dtype != torch.float32:
+            raise TypeError("SplineConditioner: the spline coupling layer runs in Float32 only")
+        K = int(K)
+        if K < 1:
+            raise ValueError("SplineConditioner: K must be >= 1")
+        if not float(B) > 0:
+            raise ValueError("SplineConditioner: B must be > 0")
+        Wn = np.asarray(W.detach().cpu() if isinstance(W, torch.Tensor) else W, dtype=np.float32)
+        J = 3 * K - 1
+        if Wn.ndim != 2 or Wn.shape[0] == 0 or Wn.shape[0] % J:
+            raise ValueError(f"W must be ((3K-1)*n1, n2) = ({J}*n1, n2), got {Wn.shape}")
+        self.K, self.B = K, float(B)
+        self.n1, self.n2 = Wn.shape[0] // J, Wn.shape[1]
+        self.W = _dev_f32(np.ascontiguousarray(Wn.T), device)  # column-major ((3K−1)n1 × n2)
+        self.c = None
+        if c is not None:
+            cn = np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, dtype=np.float32).reshape(-1)
+            if cn.shape != (Wn.shape[0],):
+                raise ValueError(f"c must have (3K-1)*n1 = {Wn.shape[0]} entries, got {cn.shape}")
+            self.c = _dev_f32(cn, device)
+
+    def to(self, device):
+        new = object.__new__(SplineConditioner)
+        new.__dict__.update(self.__dict__)
+        new.W = self.W.to(device)
+        new.c = None if self.c is None else self.c.to(device)
+        return new
+
+
 class Coupling(_ParamLayer):
     """Coupling(θ, mask) (coupling.jl:178-181).  θ is an arbitrary closure in the reference; the device
-    path supports the recognised :class:`AffineConditioner` and raises for anything else (no CPU fallback)."""
+    path supports the recognised :class:`AffineConditioner` and :class:`SplineConditioner` and raises for anything else
+    (no CPU fallback)."""
 
     _fields = ()
 
     def __init__(self, θ, mask, device="cuda"):
         if isinstance(mask, int):  # Coupling(θ, n): first n÷2 rows transformed (:183-186)
             mask = PartitionMask(mask, range(1, mask // 2 + 1))
-        if not isinstance(θ, AffineConditioner):
-            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner laws run on the device path")
+        if not isinstance(θ, (AffineConditioner, SplineConditioner)):
+            raise B2BError(_lib.B2B_EUNSUPPORTED,
+                           "Coupling: only AffineConditioner and SplineConditioner laws run on the device path")
         if θ.n1 != len(mask.indices_1) or θ.n2 != len(mask.indices_2):
             raise ValueError("conditioner shape does not match the PartitionMask")
         self.θ, self.mask = θ, mask
@@ -295,11 +334,18 @@ class Coupling(_ParamLayer):
         if D != self.mask.n:
             raise ValueError(f"DimensionMismatch: Coupling mask has {self.mask.n} dims, input has {D}")
         _check_dtype(self.θ.W, dtype, "Coupling")
+        if isinstance(self.θ, SplineConditioner):
+            return [_desc(_lib.COUPLING_RQS, inverse, p0=self.θ.W, p1=self.θ.c if self.θ.c is not None else 0,
+                          i0=self._idx1, i1=self._idx2, n0=self.θ.n1, n1=self.θ.n2, n2=self.θ.K, n3=0, f0=self.θ.B)]
         return [_desc(_lib.COUPLING_AFFINE, inverse, p0=self.θ.W, p1=self.θ.c, i0=self._idx1, i1=self._idx2,
                       n0=self.θ.n1, n1=self.θ.n2, n2=self._row1, n3=self._row2)]
 
     def __eq__(self, o):
-        return isinstance(o, Coupling) and self.mask == o.mask and torch.equal(self.θ.W, o.θ.W) and torch.equal(self.θ.c, o.θ.c)
+        if not (isinstance(o, Coupling) and type(self.θ) is type(o.θ) and self.mask == o.mask):
+            return False
+        if isinstance(self.θ, SplineConditioner) and ((self.θ.K, self.θ.B) != (o.θ.K, o.θ.B) or (self.θ.c is None) != (o.θ.c is None)):
+            return False
+        return torch.equal(self.θ.W, o.θ.W) and (self.θ.c is None or torch.equal(self.θ.c, o.θ.c))
 
     __hash__ = object.__hash__
 

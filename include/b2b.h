@@ -63,6 +63,14 @@ extern "C" {
 #define B2B_STACKED_EW 7      /* Stacked of elementwise laws on row ranges  src/bijectors/stacked.jl */
 #define B2B_MVNORMAL_DIAG 8   /* terminal op: logpdf of MvNormal(mu, Diagonal(sigma.^2)) + logjac    */
 #define B2B_MVNORMAL_TRIL 9   /* terminal op: logpdf of MvNormal(mu, L*L') (L lower Cholesky factor) + logjac */
+/* 10 is not a layer kind: it stays invalid (B2B_EINVAL) so that callers and tests have one fixed invalid value. */
+#define B2B_COUPLING_RQS 11   /* Coupling, θ = x₂ -> RationalQuadraticSpline(reshape(W·x₂+c), B)  coupling.jl      */
+
+/* Envelope of B2B_COUPLING_RQS (every entry point, forward, inverse and reverse mode): n1, n2 <= 128, 2 <= K <= 16,
+ * D <= 1024.  A layer past it returns B2B_EUNSUPPORTED with nothing launched, and the workspace queries return 0. */
+#define B2B_COUPLING_RQS_MAX_N 128
+#define B2B_COUPLING_RQS_MAX_K 16
+#define B2B_COUPLING_RQS_MAX_D 1024
 
 /* elementwise law codes for B2B_STACKED_EW (one code per row) */
 #define B2B_EW_IDENTITY 0
@@ -102,6 +110,15 @@ extern "C" {
  *                     `cholesky` guarantees; nothing on the device checks it, and a non-positive diagonal gives NaN / −Inf.
  *                     Like MVNORMAL_DIAG it must be the last element with inverse == 0, else B2B_EINVAL.  Float32:
  *                     D <= 256, Float64 (b2b_layer_desc_f64, L read through L2): D <= 2048; B2B_EUNSUPPORTED beyond.)
+ * COUPLING_RQS       W           c|NULL      -           -        idx1[n1]        idx2[n2]      n1    n2   B
+ *                    (n2 of the descriptor = K bins, n3 = 0; W is ((3K−1)·n1 x n2) column-major, c has (3K−1)·n1 entries
+ *                     (NULL = 0); both index lists are required.  Per column, v = W·x₂ + c; transformed row i (0-based) takes
+ *                     raw widths v[i + n1·k] (k < K), raw heights v[n1·K + i + n1·k] (k < K) and raw derivatives
+ *                     v[2·n1·K + i + n1·k] (k < K−1), normalised as rational_quadratic_spline.jl:109-123 does (row softmax,
+ *                     a leading 0, cumsum, 2B·(…) − B; log1pexp derivatives with unit end slopes), then the spline of
+ *                     :317-357 (inverse :183-220) maps x₁; outside [−B, B] an element is the identity with log-Jacobian 0.
+ *                     Float32 only, exact fp32 on the CUDA cores, its own launch (no BatchNorm folding).  Envelope:
+ *                     B2B_COUPLING_RQS_MAX_*; the Float64 entry points return B2B_EUNSUPPORTED for this kind.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -136,7 +153,8 @@ const char* b2b_status_string(int status);
  * K1 <= 8 for D <= 512 and K1 <= 4 for D <= 1024 (the default K = 8 bins, K1 = 9, up to D = 256).  A run of column-local
  * layers that does not fit is split into several launches (the terminal MVNORMAL_DIAG stays in the last one).
  * COUPLING_AFFINE takes any N, and any D while 264·(n1 + n2) + 4·ceil(D/32) + 2048 <= 204800 bytes (the rows it stages
- * and a bit per row); up to D = 1024 that is n1 + n2 <= 767.  The whole chain is planned before anything is enqueued: a
+ * and a bit per row); up to D = 1024 that is n1 + n2 <= 767.  COUPLING_RQS runs in its own launch (any N, the envelope of
+ * B2B_COUPLING_RQS_MAX_*; a batch sum needs the chain to end in a fused launch).  The whole chain is planned before anything is enqueued: a
  * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
  * accumulated logjac (transformed_distribution.jl:165-169 when the preceding layers are the inverse
@@ -267,12 +285,13 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * zeros).  Outputs: `xbar` (D x N, required, must not overlap `x` or `ybar`: B2B_EINVAL) and, when `param_bars` != NULL,
  * 4*L pointers: entry 4l+i receives the cotangent of layers[l].p<i> in the shape and layout of p<i> (NULL entries are not
  * computed), summed over the N columns in a fixed order (deterministic; a multi-GPU caller all-reduces them).
- * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c;
+ * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c (also
+ * COUPLING_RQS, whose W̄ is ((3K−1)·n1 x n2) column-major like W; a c̄ request with c == NULL returns B2B_EINVAL);
  * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
  * (BatchNorm m / v, PERMUTE, STACKED_EW, MVNORMAL_TRIL slots 2-3) returns B2B_EUNSUPPORTED.
  * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
- * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling /
+ * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling / spline coupling /
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
  * differentiates; a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
  * launch; with μ̄ / L̄ requested it also stores r = L⁻¹(x − μ) and l̄·L⁻ᵀr (2·D·N floats of workspace), and two more
@@ -370,7 +389,8 @@ int b2b_mvnormal_diag_logpdf_f32(const float* x, const float* mu, const float* s
 
 /* ---- Float64 batches -------------------------------------------------------------------------------------------------
  * The reference is generic in its element type and its own tests run in Float64 (test/normalising_flows.jl:47-71 checks
- * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind, both directions, the terminal
+ * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind but B2B_COUPLING_RQS (Float32
+ * only: the Float64 entry points and workspace queries refuse it with B2B_EUNSUPPORTED / 0), both directions, the terminal
  * MvNormal, the deterministic batch sum -- on D x N Float64 batches with Float64 parameters (b2b_layer_desc_f64: the
  * same fields with double pointers).  It is a straightforward double-precision restatement (one warp per column), NOT a
  * tuned kernel: Float64 is a correctness path, Float32 the hot path.  workspace: b2b_chain_workspace_bytes_f64.
