@@ -92,6 +92,10 @@ static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
         return B2B_EINVAL;
       if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
       break;
+    case B2B_SCALE_MATRIX:
+      if (!d.p0) return B2B_EINVAL;
+      if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
+      break;
     default:
       return B2B_EINVAL;
   }
@@ -179,13 +183,14 @@ extern "C" size_t b2b_coupling_workspace_bytes(int32_t n1, int32_t n2) {
 }
 
 // A launch of the chain: a run of fusable layers, one coupling layer (with the BatchNorm neighbours folded into it), one
-// spline coupling layer, or the terminal MVNORMAL_TRIL.
+// spline coupling layer, one dense Scale (its factor and map launches), or the terminal MVNORMAL_TRIL.
 struct Seg {
   int begin, end;
   bool coupling;
   int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
   bool tril = false;
   bool spline = false;
+  bool scale = false;
 };
 
 // Cuts the chain into launches before anything is enqueued: single coupling layers, and maximal runs of fusable layers
@@ -203,6 +208,12 @@ static int plan_segments(const b2b_layer_desc* layers, int32_t L, int32_t D, std
     if (layers[l].kind == B2B_COUPLING_RQS) {  // its own launch; BatchNorm neighbours keep theirs
       if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
       segs.push_back({l, l + 1, false, -1, -1, false, true});
+      ++l;
+      continue;
+    }
+    if (layers[l].kind == B2B_SCALE_MATRIX) {  // its own launches: the factor of A, then the map GEMM
+      if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
+      segs.push_back({l, l + 1, false, -1, -1, false, false, true});
       ++l;
       continue;
     }
@@ -245,12 +256,21 @@ static bool tril_terminal(const b2b_layer_desc* layers, int32_t L) {
   return layers && L >= 1 && layers[L - 1].kind == B2B_MVNORMAL_TRIL;
 }
 
+// factor storage of the dense Scale layers (one region: they run one after another); 0 for a chain without one
+static size_t chain_scale_bytes(const b2b_layer_desc* layers, int32_t L, int D) {
+  for (int l = 0; layers && l < L; ++l)
+    if (layers[l].kind == B2B_SCALE_MATRIX) return b2b_scale_matrix_workspace(D);
+  return 0;
+}
+
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
                                             int want_y, int want_sum) {
   if (tril_terminal(layers, L) && D > B2B_TRIL_MAX_D) return 0;  // the call refuses the chain
   for (int l = 0; layers && l < L; ++l)
-    if (layers[l].kind == B2B_COUPLING_RQS && !b2b_coupling_rqs_fits(layers[l], D)) return 0;
-  size_t bytes = chain_tc_bytes(layers, L, D);
+    if ((layers[l].kind == B2B_COUPLING_RQS && !b2b_coupling_rqs_fits(layers[l], D)) ||
+        (layers[l].kind == B2B_SCALE_MATRIX && D > B2B_SCALE_MATRIX_MAX_D))
+      return 0;
+  size_t bytes = chain_scale_bytes(layers, L, D) + chain_tc_bytes(layers, L, D);
   // a D x N scratch matrix is needed only when y == NULL but the chain has more than one segment
   if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
     bytes += align_up((size_t)D * (size_t)N * sizeof(float), 1024);
@@ -297,6 +317,14 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   // workspace carve-up
   char* ws = static_cast<char*>(workspace);
   size_t ws_left = workspace ? workspace_bytes : 0;
+  void* scale_ws = nullptr;
+  const size_t scale_bytes = chain_scale_bytes(layers, L, D);
+  if (scale_bytes) {
+    if (ws_left < scale_bytes) return B2B_EWORKSPACE;
+    scale_ws = ws;
+    ws += scale_bytes;
+    ws_left -= scale_bytes;
+  }
   void* tc_ws = nullptr;
   size_t tc_bytes = 0;
   float* fold_ws = nullptr;
@@ -348,7 +376,8 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   }
   double* partials = nullptr;
   if (sum_out) {
-    if (segs.back().coupling || segs.back().spline) return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
+    if (segs.back().coupling || segs.back().spline || segs.back().scale)
+      return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
     if (ws_left < 4096 * sizeof(double)) return B2B_EWORKSPACE;
     partials = reinterpret_cast<double*>(ws);
   }
@@ -390,6 +419,12 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
       rc = b2b_launch_coupling_rqs(layers[segs[s].begin], cur, dst, logjac, D, N, cur_ld, dst_ld, lj_started ? 1 : 0, stream);
       if (rc != B2B_OK) return rc;
       ++g_last_launches;
+    } else if (segs[s].scale) {
+      int n_launch = 0;
+      rc = b2b_launch_scale_matrix(layers[segs[s].begin], cur, dst, logjac, D, N, cur_ld, dst_ld, lj_started ? 1 : 0,
+                                   scale_ws, scale_bytes, &n_launch, stream);
+      g_last_launches += n_launch;
+      if (rc != B2B_OK) return rc;
     } else if (segs[s].tril) {  // always the last segment
       rc = b2b_launch_mvnormal_tril(layers[segs[s].begin], cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0,
                                     sum_out ? partials : nullptr, D, N, stream);
@@ -719,7 +754,7 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
 // the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
 namespace {
 
-enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL, VK_SPLINE };
+enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL, VK_SPLINE, VK_SCALE };
 
 struct VSeg {
   int kind, begin, end;
@@ -761,6 +796,10 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
       case B2B_COUPLING_RQS:
         if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
         s.kind = VK_SPLINE;
+        break;
+      case B2B_SCALE_MATRIX:
+        if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
+        s.kind = VK_SCALE;
         break;
       case B2B_MVNORMAL_TRIL:  // the terminal, alone
         if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
@@ -814,6 +853,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case VK_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
     case VK_TRIL: return b2b_tril_vjp_workspace(D, N);
     case VK_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
+    case VK_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
     default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
   }
 }
@@ -855,6 +895,7 @@ size_t slot_len(const b2b_layer_desc& d, int i, int D) {
     case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
     case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
+    case B2B_SCALE_MATRIX: return (size_t)D * D;
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }
@@ -909,6 +950,9 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
         case B2B_MVNORMAL_TRIL:
           if (i >= 2) return B2B_EUNSUPPORTED;
           if (i == 0 && !d.p0) return B2B_EINVAL;
+          break;
+        case B2B_SCALE_MATRIX:
+          if (i >= 1) return B2B_EUNSUPPORTED;
           break;
         default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
       }
@@ -970,10 +1014,12 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
     ++launches;                               \
   } while (0)
 
-  // 1. forward recompute: the input of every segment after the first
+  // 1. forward recompute: the input of every segment after the first (a dense Scale keeps its factor in the kernel
+  // workspace, free until the reverse sweep)
   for (int s = 0; s + 1 < S; ++s) {
+    const bool sc = segs[s].kind == VK_SCALE;
     rc = b2b_chain_run_f32(layers + segs[s].begin, segs[s].end - segs[s].begin, s == 0 ? x : ckpt[s], ckpt[s + 1],
-                           nullptr, nullptr, D, N, s == 0 ? ldx : D, D, 0, nullptr, 0, stream);
+                           nullptr, nullptr, D, N, s == 0 ? ldx : D, D, 0, sc ? kws : nullptr, sc ? kws_bytes : 0, stream);
     if (rc != B2B_OK) return rc;
     launches += g_last_launches;
   }
@@ -1129,6 +1175,11 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       float* cb = !d.p1 ? nullptr : bar(sg.begin, 1) ? bar(sg.begin, 1)
                                                        : scratch + ((slot_len(d, 0, D) + 63) & ~(size_t)63);
       rc = b2b_launch_coupling_rqs_vjp(d, in, ldin, cin, ldcin, ljbar, out, ldout, wb, cb, D, N, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+    } else if (sg.kind == VK_SCALE) {
+      rc = b2b_launch_scale_matrix_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), D, N, kws, kws_bytes,
+                                       &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
     } else if (sg.kind == VK_TRIL) {

@@ -90,6 +90,7 @@ int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last) {
       if (!last || d.inverse || !d.p1) return B2B_EINVAL;
       break;
     case B2B_COUPLING_RQS: return B2B_EUNSUPPORTED;  // Float32 only (include/b2b.h)
+    case B2B_SCALE_MATRIX: return B2B_EUNSUPPORTED;  // Float32 only (include/b2b.h)
     default: return B2B_EINVAL;
   }
   return B2B_OK;

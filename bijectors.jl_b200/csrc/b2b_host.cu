@@ -18,13 +18,22 @@ struct b2b_host_ctx {
   std::vector<cudaStream_t> streams;
   std::vector<float*> dx;      // D_max * chunk_cols floats each (y is produced in place)
   std::vector<float*> dlj;     // chunk_cols floats each
-  std::vector<char*> dws;      // workspace for the batch-sum partials
+  std::vector<char*> dws;      // workspace for the batch-sum partials (ws_bytes each)
+  size_t ws_bytes;
   std::vector<double*> dsum;   // one device double per stream
   double* hsum;                // pinned, one slot per chunk (grown on demand)
   long long hsum_cap;
 };
 
 static const size_t kWsBytes = 512 * 1024;  // batch-sum partials + tensor-core W image of a coupling layer
+
+// A chain with a dense Scale also needs its factor storage, before the partials: the staging workspace grows to hold it
+// at D_max, and only such chains are handed the larger size (every other chain sees kWsBytes, as before).
+static size_t ctx_ws_bytes(int D_max) {
+  const int d = D_max < B2B_SCALE_MATRIX_MAX_D ? D_max : B2B_SCALE_MATRIX_MAX_D;
+  const size_t scale = b2b_scale_matrix_workspace(d) + 4096 * sizeof(double) + 1024;
+  return scale > kWsBytes ? scale : kWsBytes;
+}
 
 extern "C" int b2b_host_ctx_create(b2b_host_ctx** out, int32_t D_max, int64_t chunk_cols, int32_t n_streams) {
   if (!out || D_max < 1 || chunk_cols < 1 || n_streams < 1 || n_streams > 16) return B2B_EINVAL;
@@ -34,6 +43,7 @@ extern "C" int b2b_host_ctx_create(b2b_host_ctx** out, int32_t D_max, int64_t ch
   c->n_streams = n_streams;
   c->hsum = nullptr;
   c->hsum_cap = 0;
+  c->ws_bytes = ctx_ws_bytes(D_max);
   cudaError_t e = cudaSuccess;
   for (int s = 0; s < n_streams && e == cudaSuccess; ++s) {
     cudaStream_t st = nullptr;
@@ -43,7 +53,7 @@ extern "C" int b2b_host_ctx_create(b2b_host_ctx** out, int32_t D_max, int64_t ch
     e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaMalloc(&dx, (size_t)D_max * (size_t)chunk_cols * sizeof(float));
     if (e == cudaSuccess) e = cudaMalloc(&dlj, (size_t)chunk_cols * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&ws, kWsBytes);
+    if (e == cudaSuccess) e = cudaMalloc(&ws, c->ws_bytes);
     if (e == cudaSuccess) e = cudaMalloc(&ds, sizeof(double));
     c->streams.push_back(st);
     c->dx.push_back(dx);
@@ -194,6 +204,9 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
   const int nseg = b2b_chain_segment_count(layers, L, D);
   if (nseg < 0) return nseg;
   const bool stage_y = y_host != nullptr || nseg > 1;
+  bool scale = false;
+  for (int l = 0; l < L; ++l) scale = scale || layers[l].kind == B2B_SCALE_MATRIX;
+  const size_t ws_bytes = scale ? c->ws_bytes : kWsBytes;
   for (long long k = 0; k < nchunks; ++k) {
     const int s = (int)(k % c->n_streams);
     cudaStream_t st = c->streams[s];
@@ -206,7 +219,7 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
     const bool want_lj = logjac_host != nullptr || (sum_host && !terminal);
     const int rc = b2b_chain_run_f32(layers, L, c->dx[s], stage_y ? c->dx[s] : nullptr,  // in place
                                      (want_lj || terminal) ? c->dlj[s] : nullptr,
-                                     sum_host ? c->dsum[s] : nullptr, D, n, D, D, 0, c->dws[s], kWsBytes, st);
+                                     sum_host ? c->dsum[s] : nullptr, D, n, D, D, 0, c->dws[s], ws_bytes, st);
     if (rc != B2B_OK) return rc;
     launches += b2b_last_launch_count();
     if (y_host) {

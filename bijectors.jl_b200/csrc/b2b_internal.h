@@ -132,6 +132,24 @@ size_t b2b_tril_vjp_workspace(int D, long long N);
 int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
                         const float* ljbar, float* xbar, long long ldxb, float* mubar, float* Lbar, int D, long long N,
                         void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
+// Σₙ S[:, n] R[:, n]ᵀ over column chunks (b2b_mvnormal_tril.cu): CTA (tile, p) writes its 64 x 64 tile of chunk p's sum
+// to part[p] (D x D, column-major; fp32 FMA within a chunk, which the caller sums over p in a fixed order).  `lower`:
+// only the tiles on and below the diagonal, elements i >= j, and (when mup != NULL) chunk row sums of S to mup[p].
+// b2b_outer_chunk_len(N) columns per chunk, at most 64 chunks.
+long long b2b_outer_chunk_len(long long N);
+int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long long ldr, float* part, float* mup, int D,
+                            long long N, bool lower, cudaStream_t stream);
+// dense Scale(A) (b2b_scale_matrix.cu), D <= B2B_SCALE_MATRIX_MAX_D: factor (one CTA; plus the A⁻¹ solves for the
+// inverse direction) and the map GEMM, in b2b_scale_matrix_workspace(D) bytes; y == NULL writes log-Jacobians only
+size_t b2b_scale_matrix_workspace(int D);
+int b2b_launch_scale_matrix(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
+                            long long ldx, long long ldy, int accumulate, void* workspace, size_t workspace_bytes,
+                            int* launches, cudaStream_t stream);
+// reverse mode: x̄ always, Ā when non-NULL; b2b_scale_matrix_vjp_workspace(D, N) bytes (0 beyond the envelope)
+size_t b2b_scale_matrix_vjp_workspace(int D, long long N);
+int b2b_launch_scale_matrix_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar,
+                                long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* Abar, int D,
+                                long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // spline coupling (b2b_coupling_rqs.cu, b2b_coupling_rqs_vjp.cu): whether the layer is within the envelope of include/b2b.h
 bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D);
 int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
@@ -146,7 +164,7 @@ int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long lo
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
-// COUPLING_RQS).
+// COUPLING_RQS and SCALE_MATRIX).
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);

@@ -330,18 +330,27 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
 }
 
 // ---- L̄ = tril(S Rᵀ) over column chunks: CTA (tile, p) writes the 64 x 64 tile of Σ_{n in chunk p} S[:, n] R[:, n]ᵀ
-// (lower-triangle tiles only) to part[p] (D x D, column-major); diagonal tiles also write the chunk's row sums of S
-// (μ̄) to mup[p].  fp32 FMA within a chunk, fp64 across chunks (finalize_kernel).
+// to part[p] (D x D, column-major): with `lower` the lower-triangle tiles only, whose diagonal tiles also write the
+// chunk's row sums of S (μ̄) to mup[p] when it is given; otherwise every tile (dense Scale's G = Σ ȳ uᵀ).  fp32 FMA within
+// a chunk, fp64 across chunks (finalize_kernel).
 constexpr int kTile = 64, kBK = 16, kChunk = 4096, kMaxChunks = 64;
 
-__global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S, const float* __restrict__ Rm,
-                                                    float* __restrict__ part, float* __restrict__ mup, int D, long long N,
-                                                    long long clen) {
+__global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S, long long lds, const float* __restrict__ Rm,
+                                                    long long ldr, float* __restrict__ part, float* __restrict__ mup, int D,
+                                                    long long N, long long clen, bool lower) {
   __shared__ __align__(16) float As[kBK][kTile];
   __shared__ __align__(16) float Bs[kBK][kTile];
-  int ti = 0, rem = blockIdx.x;  // lower-triangle tile (ti, tj), ti >= tj, in row order
-  while (rem > ti) rem -= ++ti;
-  const int tj = rem;
+  int ti = 0, tj = 0;
+  if (lower) {  // lower-triangle tile (ti, tj), ti >= tj, in row order
+    int rem = blockIdx.x;
+    while (rem > ti) rem -= ++ti;
+    tj = rem;
+  } else {  // every tile, in row order
+    const int T = (D + kTile - 1) / kTile;
+    ti = blockIdx.x / T;
+    tj = blockIdx.x - ti * T;
+  }
+  const bool diag = lower && ti == tj && mup;
   const int p = blockIdx.y, i0 = ti * kTile, j0 = tj * kTile;
   const long long n0 = (long long)p * clen, n1 = n0 + clen < N ? n0 + clen : N;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -353,8 +362,8 @@ __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S,
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int ia = i0 + lr + q, ja = j0 + lr + q;
-      As[lk][lr + q] = (n < n1 && ia < D) ? S[n * D + ia] : 0.f;
-      Bs[lk][lr + q] = (n < n1 && ja < D) ? Rm[n * D + ja] : 0.f;
+      As[lk][lr + q] = (n < n1 && ia < D) ? S[n * lds + ia] : 0.f;
+      Bs[lk][lr + q] = (n < n1 && ja < D) ? Rm[n * ldr + ja] : 0.f;
     }
     __syncthreads();
 #pragma unroll
@@ -367,7 +376,7 @@ __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S,
 #pragma unroll
         for (int v = 0; v < 4; ++v) acc[u][v] = fmaf(av[u], bv[v], acc[u][v]);
     }
-    if (ti == tj && threadIdx.x < kTile) {
+    if (diag && threadIdx.x < kTile) {
 #pragma unroll
       for (int k = 0; k < kBK; ++k) msum += As[k][threadIdx.x];
     }
@@ -379,9 +388,9 @@ __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S,
 #pragma unroll
     for (int v = 0; v < 4; ++v) {
       const int i = i0 + ty * 4 + u, j = j0 + tx * 4 + v;
-      if (i < D && j < D && i >= j) P[(size_t)j * D + i] = acc[u][v];
+      if (i < D && j < D && (i >= j || !lower)) P[(size_t)j * D + i] = acc[u][v];
     }
-  if (ti == tj && threadIdx.x < kTile && i0 + (int)threadIdx.x < D) mup[(size_t)p * D + i0 + threadIdx.x] = msum;
+  if (diag && threadIdx.x < kTile && i0 + (int)threadIdx.x < D) mup[(size_t)p * D + i0 + threadIdx.x] = msum;
 }
 
 // L̄ (D x D column-major, exactly zero above the diagonal) and μ̄ from the chunk partials, in chunk order
@@ -451,6 +460,17 @@ using namespace b2b_tril;
 
 int b2b_tril_grid(int D, long long N) { return grid_for(c_logpdf(rows_per_lane(D)), N); }
 
+long long b2b_outer_chunk_len(long long N) { return chunk_len(N); }
+
+int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long long ldr, float* part, float* mup, int D,
+                            long long N, bool lower, cudaStream_t stream) {
+  const long long clen = chunk_len(N), P = (N + clen - 1) / clen;
+  const int T = (D + kTile - 1) / kTile;
+  outer_kernel<<<dim3(lower ? T * (T + 1) / 2 : T * T, (unsigned)P), 256, 0, stream>>>(S, lds, R, ldr, part, mup, D, N,
+                                                                                        clen, lower);
+  return (int)cudaGetLastError();
+}
+
 int b2b_launch_mvnormal_tril(const b2b_layer_desc& d, const float* x, long long ldx, float* y, long long ldy,
                              float* logjac, int accumulate, double* partials, int D, long long N, cudaStream_t stream) {
   if (D < 1 || D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
@@ -507,9 +527,7 @@ int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, 
   if (rc != B2B_OK) return rc;
   *launches = 1;
   if (!params) return B2B_OK;
-  const int T = (D + kTile - 1) / kTile;
-  outer_kernel<<<dim3(T * (T + 1) / 2, (unsigned)P), 256, 0, stream>>>(Sw, Rw, part, mup, D, N, clen);
-  if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
+  if ((rc = b2b_launch_outer_chunks(Sw, D, Rw, D, part, mup, D, N, true, stream)) != B2B_OK) return rc;
   const long long tot = (long long)D * D + D;
   finalize_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(part, mup, (int)P, ljp, grid, d.p1, Lbar, mubar, D);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;

@@ -818,6 +818,7 @@ _SLOT_NAMES = {
     _lib.MVNORMAL_DIAG: ("μ", "σ"),
     _lib.MVNORMAL_TRIL: ("μ", "L"),
     _lib.COUPLING_RQS: ("W", "c"),
+    _lib.SCALE_MATRIX: ("a",),
 }
 
 
@@ -840,8 +841,8 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
     if d.kind == _lib.COUPLING_RQS:
         J = 3 * d.n2 - 1
         return (d.n1, J * d.n0) if i == 0 else (J * d.n0,)  # W column-major ((3K−1)n1 × n2)
-    if d.kind == _lib.MVNORMAL_TRIL and i == 1:
-        return (D, D)  # L column-major: element (i, j) at [j, i]
+    if (d.kind == _lib.MVNORMAL_TRIL and i == 1) or d.kind == _lib.SCALE_MATRIX:
+        return (D, D)  # L / A column-major: element (i, j) at [j, i]
     return (D,)
 
 
@@ -902,7 +903,8 @@ def _leaf_descs(t, D: int, dtype=torch.float32):
 
 
 def _leaf_grads(descs, counts, bars) -> List[dict]:
-    """One dict per leaf, keyed by the reference's field names; RQS knots as D × K+1 and W as (2n1 × n2)."""
+    """One dict per leaf, keyed by the reference's field names; RQS knots as D × K+1, W as (2n1 × n2) and a dense
+    Scale's ``a`` as D × D in A's own orientation."""
     grads, k = [], 0
     for c in counts:
         g = {}
@@ -910,7 +912,7 @@ def _leaf_grads(descs, counts, bars) -> List[dict]:
             d = descs[l]
             for i in _trainable_slots(d):
                 t = bars[(l, i)]
-                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind == _lib.RQS or (d.kind in (_lib.COUPLING_AFFINE, _lib.COUPLING_RQS) and i == 0)) else t
+                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind in (_lib.RQS, _lib.SCALE_MATRIX) or (d.kind in (_lib.COUPLING_AFFINE, _lib.COUPLING_RQS) and i == 0)) else t
         grads.append(g)
         k += c
     return grads
@@ -923,7 +925,7 @@ def chain_vjp(t, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Op
     One b2b_chain_vjp_f32 call -- b2b_chain_vjp_f64 when ``x`` is a Float64 batch, whose layers and cotangents must then be
     Float64 too (a mix raises TypeError).  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)``
     (application order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives``
-    (D×K+1), ``W/c``, ``b/logs``, and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
+    (D×K+1), ``W/c``, ``b/logs``, ``a`` (D×D, a dense Scale), and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
     D = _batch_view(x)[0]
     descs, counts = _leaf_descs(t, D, x.dtype)
     if not descs:

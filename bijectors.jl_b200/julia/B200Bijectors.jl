@@ -39,6 +39,7 @@ struct LayerDesc
 end
 const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG, MVNORMAL_TRIL = Int32.(1:9)
 const COUPLING_RQS = Int32(11)  # 10 is not a layer kind (include/b2b.h)
+const SCALE_MATRIX = Int32(12)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
 const NULLI = CuPtr{Int32}(0)
@@ -156,6 +157,9 @@ function desc(sb::Stacked, inv::Bool)
     ds = get!(() -> DeviceStacked(sb), STACKS, sb)
     LayerDesc(STACKED_EW, inv, 0, 0, 0, 0, 0f0, 0f0, pointer(ds.a), pointer(ds.b), NULLF, NULLF, pointer(ds.code), NULLI)
 end
+# Scale(A) with a D x D matrix (scale.jl:14,17,35-36): A itself, column-major as CuMatrix stores it; Float32, D <= 256
+desc(b::Scale{<:CuMatrix{Float32}}, inv::Bool) =
+    LayerDesc(SCALE_MATRIX, inv, 0, 0, 0, 0, 0f0, 0f0, pointer(b.a), NULLF, NULLF, NULLF, NULLI, NULLI)
 # a whole-column elementwise law is a one-block Stacked
 const ElementwiseLaw = Union{Shift{<:Real},Scale{<:Real},LeakyReLU{<:Real},Logit{<:Real,<:Real},TruncatedBijector{<:Real,<:Real}}
 
@@ -166,7 +170,8 @@ descs(f, inv::Bool) = inv ? [desc(b, true) for b in reverse(flatten(f))] : [desc
 
 const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVector{Float32}},
                           RationalQuadraticSpline{<:CuMatrix{Float32}},InvertibleBatchNorm{<:CuVector{Float32}},
-                          Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},Permute,Stacked}
+                          Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},
+                          Scale{<:CuMatrix{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
 is_device(::DeviceLeaf) = true
@@ -365,7 +370,7 @@ end
 
 # Reverse mode of ANY device chain (b2b_chain_vjp_f32): `f` (or inverse(f) with inv=true); ȳ, l̄ the cotangents of
 # (y, logjac), `nothing` = zeros.  Returns x̄ and, per descriptor in application order, the cotangents of its trainable
-# fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, BatchNorm b logs, the
+# fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, Scale(A) a, BatchNorm b logs, the
 # terminal MvNormal's μ σ) in the fields' shapes; `nothing` for fields without one.
 function vjp_slots(d::LayerDesc, D::Integer)
     z(dims...) = CUDA.zeros(Float32, dims...)
@@ -374,6 +379,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == RQS && return (z(D, d.n0), z(D, d.n0), z(D, d.n0))
     d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
     d.kind == COUPLING_RQS && return (z((3d.n2 - 1) * d.n0, d.n1), d.p1 == NULLF ? nothing : z((3d.n2 - 1) * d.n0))
+    d.kind == SCALE_MATRIX && return (z(D, D),)
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

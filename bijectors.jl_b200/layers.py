@@ -567,18 +567,61 @@ class Shift(Bijector):
 
 
 class Scale(Bijector):
-    """Scale(a): y = a .* x, logjac = log|a| per element (scale.jl:1-39); scalar `a`."""
+    """Scale(a): y = a .* x, logjac = log|a| per element (scale.jl:1-39) for a scalar `a` (also a Stacked block).
 
-    def __init__(self, a):
-        self.a = float(a)
+    A square matrix `a` gives the dense layer Scale{<:AbstractMatrix} (scale.jl:14,17,35-36): y = A x, inverse A \\ y,
+    logjac = logabsdet(A)[1] per column, with A trainable (B2B_SCALE_MATRIX; Float32 only, D <= 256).  The device tensor
+    `_A` holds A column-major, i.e. Aᵀ row-major (as MvNormal's scale_tril); `.a` returns A in the user's orientation.
+    A singular A is the caller's responsibility: the forward gives logjac = −Inf, the inverse non-finite values."""
+
+    def __init__(self, a, device="cuda", dtype=torch.float32):
+        if (a.dim() if isinstance(a, torch.Tensor) else np.ndim(a)) == 2:
+            if dtype != torch.float32:
+                raise TypeError(f"a dense Scale has Float32 parameters only, got {dtype}")
+            A = a.detach() if isinstance(a, torch.Tensor) else torch.as_tensor(np.asarray(a, dtype=np.float32))
+            if A.shape[0] != A.shape[1]:
+                raise ValueError(f"DimensionMismatch: Scale needs a square matrix, got {tuple(A.shape)}")
+            self._A = A.to(device=device, dtype=torch.float32).t().contiguous()
+            return
+        self._A = None
+        self._a = float(a)
 
     code = _lib.EW_SCALE
 
+    @property
+    def dense(self) -> bool:
+        return self._A is not None
+
+    @property
+    def a(self):
+        return self._A.t() if self.dense else self._a
+
+    @property
+    def device(self):
+        return self._A.device
+
+    def to(self, device):
+        new = object.__new__(Scale)
+        new.__dict__.update(self.__dict__)
+        if self.dense:
+            new._A = self._A.to(device)
+        return new
+
+    def _keepalive(self):
+        return (self._A,) if self.dense else ()
+
     def _descs(self, inverse, D, dtype=torch.float32):
-        return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
+        if not self.dense:
+            return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
+        if D != self._A.shape[0]:
+            raise ValueError(f"DimensionMismatch: Scale has a {self._A.shape[0]} x {self._A.shape[0]} matrix, input has {D} dims")
+        _check_dtype(self._A, dtype, "Scale")
+        return [_desc(_lib.SCALE_MATRIX, inverse, p0=self._A)]
 
     def __eq__(self, o):
-        return isinstance(o, Scale) and o.a == self.a
+        if not isinstance(o, Scale) or self.dense != o.dense:
+            return False
+        return torch.equal(self._A.cpu(), o._A.cpu()) if self.dense else o._a == self._a
 
     __hash__ = object.__hash__
 
@@ -664,6 +707,8 @@ class Stacked(Transform):
         for b in bs:
             if not isinstance(b, (Elementwise, Shift, Scale, LeakyReLU, Logit, TruncatedBijector)) and b is not None:
                 raise B2BError(_lib.B2B_EUNSUPPORTED, f"Stacked block {type(b).__name__}")
+            if isinstance(b, Scale) and b.dense:
+                raise B2BError(_lib.B2B_EUNSUPPORTED, "Stacked block Scale with a matrix (a dense layer acts on whole columns)")
         self.bs, self.ranges_in = bs, ranges
         self.length_in = sum(hi - lo + 1 for lo, hi in ranges)
         self.length_out = self.length_in

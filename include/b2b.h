@@ -72,6 +72,11 @@ extern "C" {
 #define B2B_COUPLING_RQS_MAX_K 16
 #define B2B_COUPLING_RQS_MAX_D 1024
 
+#define B2B_SCALE_MATRIX 12   /* Scale(A), A a trainable D x D matrix: y = A*x, logjac = logabsdet(A)  scale.jl:14,17,35-36 */
+/* Envelope of B2B_SCALE_MATRIX: Float32, D <= 256.  Beyond it every entry point returns B2B_EUNSUPPORTED with nothing
+ * launched and the workspace queries return 0; the Float64 entry points refuse the kind the same way. */
+#define B2B_SCALE_MATRIX_MAX_D 256
+
 /* elementwise law codes for B2B_STACKED_EW (one code per row) */
 #define B2B_EW_IDENTITY 0
 #define B2B_EW_EXP 1   /* elementwise(exp): y=exp(x), logjac += x          exp_log.jl:5-6  */
@@ -119,6 +124,14 @@ extern "C" {
  *                     :317-357 (inverse :183-220) maps x₁; outside [−B, B] an element is the identity with log-Jacobian 0.
  *                     Float32 only, exact fp32 on the CUDA cores, its own launch (no BatchNorm folding).  Envelope:
  *                     B2B_COUPLING_RQS_MAX_*; the Float64 entry points return B2B_EUNSUPPORTED for this kind.)
+ * SCALE_MATRIX       A[D x D]    -           -           -        -               -             -     -    -
+ *                    (A column-major, required.  Per column y = A x with logjac = log|det A|; inverse != 0 gives
+ *                     y = A⁻¹ x with −log|det A|.  The sign of det A does not matter (logabsdet).  log|det A| and A⁻¹ come
+ *                     from an fp64 LU with partial pivoting computed on the device at every call (A may change between
+ *                     calls; nothing synchronises the host); the map is exact fp32 FMA.  An invertible A is the caller's
+ *                     contract, as Lᵢᵢ > 0 is for MVNORMAL_TRIL: for a singular A the forward gives y = A x and −Inf, the
+ *                     inverse non-finite values; nothing on the device checks it.  Float32 only, D <= B2B_SCALE_MATRIX_MAX_D,
+ *                     its own launch; the Float64 entry points return B2B_EUNSUPPORTED for this kind.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -154,7 +167,13 @@ const char* b2b_status_string(int status);
  * layers that does not fit is split into several launches (the terminal MVNORMAL_DIAG stays in the last one).
  * COUPLING_AFFINE takes any N, and any D while 264·(n1 + n2) + 4·ceil(D/32) + 2048 <= 204800 bytes (the rows it stages
  * and a bit per row); up to D = 1024 that is n1 + n2 <= 767.  COUPLING_RQS runs in its own launch (any N, the envelope of
- * B2B_COUPLING_RQS_MAX_*; a batch sum needs the chain to end in a fused launch).  The whole chain is planned before anything is enqueued: a
+ * B2B_COUPLING_RQS_MAX_*; a batch sum needs the chain to end in a fused launch).  SCALE_MATRIX runs in its own launches
+ * (D <= B2B_SCALE_MATRIX_MAX_D, any N): a one-CTA fp64 LU of A, for the inverse direction a second launch forming A⁻¹,
+ * then the per-column GEMM y = M x, which reads each column once and writes it once (y may alias x).  Like COUPLING_RQS,
+ * a batch sum needs the chain to end in a fused launch (a logpdf chain ends in its MvNormal terminal).  The layer needs
+ * workspace for its factor: b2b_chain_workspace_bytes adds 12·D² + 4·D + 8 bytes, each of the four parts rounded up to
+ * 256 bytes, plus 256, for a chain with any SCALE_MATRIX layer (the layers share it; they run one after another).
+ * The whole chain is planned before anything is enqueued: a
  * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
  * accumulated logjac (transformed_distribution.jl:165-169 when the preceding layers are the inverse
@@ -287,11 +306,15 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * computed), summed over the N columns in a fixed order (deterministic; a multi-GPU caller all-reduces them).
  * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c (also
  * COUPLING_RQS, whose W̄ is ((3K−1)·n1 x n2) column-major like W; a c̄ request with c == NULL returns B2B_EINVAL);
+ * SCALE_MATRIX a (Ā, D x D column-major like A: G + (Σ l̄)·A⁻ᵀ, or −A⁻ᵀ G A⁻ᵀ − (Σ l̄)·A⁻ᵀ for the inverse layer, with
+ * G = Σₙ ȳₙ uₙᵀ over the layer's inputs u; slots 1-3 return B2B_EUNSUPPORTED);
  * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
  * (BatchNorm m / v, PERMUTE, STACKED_EW, MVNORMAL_TRIL slots 2-3) returns B2B_EUNSUPPORTED.
  * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
  * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling / spline coupling /
+ * dense Scale (factor, x̄ by the transposed map, G over column chunks, an fp64 finalize; workspace: the factor of
+ * b2b_chain_run_f32 plus P·D² floats, P <= 64 chunks, and 2·D² + 1 doubles) /
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
  * differentiates; a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
  * launch; with μ̄ / L̄ requested it also stores r = L⁻¹(x − μ) and l̄·L⁻ᵀr (2·D·N floats of workspace), and two more

@@ -65,6 +65,17 @@ rf = B.Composed(*[B.RadialLayer(f32([0.2]), f32([0.3]), rng.standard_normal(64).
 B.radial_chain_vjp(rf, B.from_numpy(rng.standard_normal((64, 211)).astype(f32)), B.from_numpy(rng.standard_normal((64, 211)).astype(f32)), torch.randn(211, device="cuda"))
 torch.cuda.synchronize()
 print("radial vjp ok")
+# dense Scale(A): factor, A⁻¹ solves, map GEMM (both operand orders) and the Ā reduction, at every padded depth
+for D, N in [(3, 77), (40, 300), (100, 129), (256, 200)]:
+    A = (np.eye(D) + 0.3 * rng.standard_normal((D, D)) / np.sqrt(D)).astype(f32)
+    sflow = B.Composed(B.Scale(A), B.PlanarLayer(D) if D <= 128 else B.Permute((rng.permutation(D) + 1).tolist()))
+    x = B.from_numpy(rng.standard_normal((D, N)).astype(f32))
+    y, _ = B.with_logabsdet_jacobian(sflow, x)
+    B.with_logabsdet_jacobian(B.inverse(sflow), y)
+    B.chain_vjp(sflow, x, B.from_numpy(rng.standard_normal((D, N)).astype(f32)), torch.randn(N, device="cuda"))
+    B.chain_vjp(B.inverse(sflow), y, B.from_numpy(rng.standard_normal((D, N)).astype(f32)), torch.randn(N, device="cuda"))
+    torch.cuda.synchronize()
+    print(f"scale matrix D={D} ok")
 bn = B.InvertibleBatchNorm(32, training=True)
 bn.train_forward(B.from_numpy(rng.standard_normal((32, 300)).astype(f32)))
 xh = B.from_numpy(rng.standard_normal((64, 1000)).astype(f32), device="cpu", pin_memory=True)
