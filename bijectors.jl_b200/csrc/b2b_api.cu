@@ -5,7 +5,6 @@
 #include <cstdio>
 #include <cstring>
 #include <algorithm>
-#include <utility>
 #include <vector>
 
 #include "b2b_internal.h"
@@ -51,55 +50,44 @@ extern "C" int b2b_set_kernel_variant(int variant) {
   return B2B_OK;
 }
 
-static bool fusable(int kind) {
-  return kind == B2B_PLANAR || kind == B2B_RADIAL || kind == B2B_RQS || kind == B2B_BATCHNORM ||
-         kind == B2B_PERMUTE || kind == B2B_STACKED_EW || kind == B2B_MVNORMAL_DIAG;
+// Float32 envelope of a valid layer at D: B2B_EUNSUPPORTED when its forward kernel does not take it, else B2B_OK.  The
+// fused kinds are also bound by their run's shared-memory budget, which plan_segments checks.
+static int fwd_envelope(const b2b_layer_desc& d, int D) {
+  bool ok = true;
+  switch (d.kind) {
+    case B2B_RQS: ok = d.n0 <= 64; break;
+    case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_fits(d.n0, d.n1, D); break;
+    case B2B_COUPLING_RQS: ok = b2b_coupling_rqs_fits(d, D); break;
+    case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
+    case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
+    default: break;
+  }
+  return ok ? B2B_OK : B2B_EUNSUPPORTED;
 }
 
-static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
+// The same for the kernels of b2b_chain_vjp_f32.
+static int vjp_envelope(const b2b_layer_desc& d, int D) {
+  bool ok;
   switch (d.kind) {
     case B2B_PLANAR:
-      if (!d.p0 || !d.p1 || !d.p2) return B2B_EINVAL;
-      break;
-    case B2B_RADIAL:
-      if (!d.p0 || !d.p1 || !d.p2) return B2B_EINVAL;
-      break;
-    case B2B_RQS:
-      if (!d.p0 || !d.p1 || !d.p2 || d.n0 < 2) return B2B_EINVAL;
-      if (d.n0 > 64) return B2B_EUNSUPPORTED;
-      break;
-    case B2B_COUPLING_AFFINE:
-      if (!d.p0 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D) return B2B_EINVAL;
-      if ((!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-      break;
-    case B2B_BATCHNORM:
-      if (!d.p0 || !d.p1 || !d.p2 || !d.p3) return B2B_EINVAL;
-      break;
-    case B2B_PERMUTE:
-      if (!d.i0) return B2B_EINVAL;
-      break;
-    case B2B_STACKED_EW:
-      if (!d.i0) return B2B_EINVAL;
-      break;
-    case B2B_MVNORMAL_DIAG:
-      if (!last || d.inverse) return B2B_EINVAL;
-      break;
-    case B2B_MVNORMAL_TRIL:
-      if (!last || d.inverse || !d.p1) return B2B_EINVAL;
-      break;
+    case B2B_RADIAL: ok = D <= 128; break;
+    case B2B_RQS: ok = D <= 256 && d.n0 <= 64; break;
+    case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_vjp_fits(d, D); break;
     case B2B_COUPLING_RQS:
-      if (!d.p0 || !d.i0 || !d.i1 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D || d.n2 < 1 || !(d.f0 > 0.f))
-        return B2B_EINVAL;
-      if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
-      break;
     case B2B_SCALE_MATRIX:
-      if (!d.p0) return B2B_EINVAL;
-      if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-      break;
-    default:
-      return B2B_EINVAL;
+    case B2B_MVNORMAL_TRIL: return fwd_envelope(d, D);
+    default: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
   }
-  return B2B_OK;
+  return ok ? B2B_OK : B2B_EUNSUPPORTED;
+}
+
+// The descriptor rules, then the envelope -- but a coupling's kernel limit and the terminal's D are refused only when
+// the chain is planned, after the batch-sum and cotangent-slot checks of the entry points.
+static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
+  const int rc = b2b_check_desc(d, D, last);
+  if (rc != B2B_OK) return rc;
+  const int launch = b2b_kind(d.kind)->launch;
+  return launch == B2B_LC_COUPLING || launch == B2B_LC_TRIL ? B2B_OK : fwd_envelope(d, D);
 }
 
 // number of kernel launches the last launch_fused enqueued (the constant-bank path adds a prep kernel and a copy)
@@ -182,54 +170,39 @@ extern "C" size_t b2b_coupling_workspace_bytes(int32_t n1, int32_t n2) {
   return b ? align_up(b, 1024) + 1024 : 0;
 }
 
-// A launch of the chain: a run of fusable layers, one coupling layer (with the BatchNorm neighbours folded into it), one
-// spline coupling layer, one dense Scale (its factor and map launches), or the terminal MVNORMAL_TRIL.
+// A launch of the chain: a run of fused layers, or one layer of another launch class (a coupling with the BatchNorm
+// neighbours folded into it).
 struct Seg {
   int begin, end;
-  bool coupling;
+  int launch;     // B2BLaunchClass
   int pre, post;  // layer index of a BatchNorm folded into this coupling launch (-1: none)
-  bool tril = false;
-  bool spline = false;
-  bool scale = false;
 };
 
-// Cuts the chain into launches before anything is enqueued: single coupling layers, and maximal runs of fusable layers
-// whose staged parameters fit one fused kernel (a run is ended before the layer that would cross the shared-memory budget,
-// so the terminal MvNormal stays in the last segment).  B2B_EUNSUPPORTED when one layer alone does not fit.
+// Cuts the chain into launches before anything is enqueued: single layers of their own launch class, and maximal runs of
+// fused layers whose staged parameters fit one fused kernel (a run is ended before the layer that would cross the
+// shared-memory budget, so the terminal MvNormal stays in the last segment).  B2B_EUNSUPPORTED when one layer alone does
+// not fit, B2B_EINVAL for a kind include/b2b.h does not define.
 static int plan_segments(const b2b_layer_desc* layers, int32_t L, int32_t D, std::vector<Seg>& segs) {
   segs.clear();
+  auto launch = [&](int l) {
+    const B2BKind* k = b2b_kind(layers[l].kind);
+    return k ? k->launch : -1;
+  };
   for (int l = 0; l < L;) {
-    if (layers[l].kind == B2B_COUPLING_AFFINE) {
-      if (!b2b_coupling_affine_fits(layers[l].n0, layers[l].n1, D)) return B2B_EUNSUPPORTED;
-      segs.push_back({l, l + 1, true, -1, -1});
-      ++l;
-      continue;
-    }
-    if (layers[l].kind == B2B_COUPLING_RQS) {  // its own launch; BatchNorm neighbours keep theirs
-      if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
-      segs.push_back({l, l + 1, false, -1, -1, false, true});
-      ++l;
-      continue;
-    }
-    if (layers[l].kind == B2B_SCALE_MATRIX) {  // its own launches: the factor of A, then the map GEMM
-      if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-      segs.push_back({l, l + 1, false, -1, -1, false, false, true});
-      ++l;
-      continue;
-    }
-    if (layers[l].kind == B2B_MVNORMAL_TRIL) {  // its own launch: the packed factor fills the shared memory
-      if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
-      segs.push_back({l, l + 1, false, -1, -1, true});
+    if (launch(l) < 0) return B2B_EINVAL;
+    if (launch(l) != B2B_LC_FUSED) {
+      if (fwd_envelope(layers[l], D) != B2B_OK) return B2B_EUNSUPPORTED;
+      segs.push_back({l, l + 1, launch(l), -1, -1});
       ++l;
       continue;
     }
     int e = l;
-    while (e < L && fusable(layers[e].kind)) ++e;
+    while (e < L && launch(e) == B2B_LC_FUSED) ++e;
     for (int b = l; b < e;) {
       if (b2b_chain_v0_smem_bytes(layers + b, 1, D) > B2B_V0_SMEM_MAX) return B2B_EUNSUPPORTED;
       int k = b + 1;
       while (k < e && b2b_chain_v0_smem_bytes(layers + b, k + 1 - b, D) <= B2B_V0_SMEM_MAX) ++k;
-      segs.push_back({b, k, false, -1, -1});
+      segs.push_back({b, k, B2B_LC_FUSED, -1, -1});
       b = k;
     }
     l = e;
@@ -258,18 +231,19 @@ static bool tril_terminal(const b2b_layer_desc* layers, int32_t L) {
 
 // factor storage of the dense Scale layers (one region: they run one after another); 0 for a chain without one
 static size_t chain_scale_bytes(const b2b_layer_desc* layers, int32_t L, int D) {
-  for (int l = 0; layers && l < L; ++l)
-    if (layers[l].kind == B2B_SCALE_MATRIX) return b2b_scale_matrix_workspace(D);
-  return 0;
+  return layers && b2b_chain_has_launch(layers, L, B2B_LC_SCALE) ? b2b_scale_matrix_workspace(D) : 0;
 }
 
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
                                             int want_y, int want_sum) {
-  if (tril_terminal(layers, L) && D > B2B_TRIL_MAX_D) return 0;  // the call refuses the chain
-  for (int l = 0; layers && l < L; ++l)
-    if ((layers[l].kind == B2B_COUPLING_RQS && !b2b_coupling_rqs_fits(layers[l], D)) ||
-        (layers[l].kind == B2B_SCALE_MATRIX && D > B2B_SCALE_MATRIX_MAX_D))
+  // 0 for a layer past the envelopes include/b2b.h states (the call refuses the chain); a coupling past its kernel's
+  // limit, or a descriptor the call finds invalid, is still sized
+  for (int l = 0; layers && l < L; ++l) {
+    const B2BKind* k = b2b_kind(layers[l].kind);
+    if (k && (k->launch == B2B_LC_SPLINE || k->launch == B2B_LC_SCALE || (k->launch == B2B_LC_TRIL && l == L - 1)) &&
+        fwd_envelope(layers[l], D) != B2B_OK)
       return 0;
+  }
   size_t bytes = chain_scale_bytes(layers, L, D) + chain_tc_bytes(layers, L, D);
   // a D x N scratch matrix is needed only when y == NULL but the chain has more than one segment
   if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
@@ -302,12 +276,7 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     const int rc = validate_layer(layers[l], D, l == L - 1);
     if (rc != B2B_OK) return rc;
   }
-  if (N == 0) {
-    if (sum_out) return (int)cudaMemsetAsync(sum_out, 0, sizeof(double), stream);
-    return B2B_OK;
-  }
-  const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL;
-  if (sum_out && !logjac && !terminal) return B2B_EINVAL;
+  if (sum_out && !logjac && !b2b_ends_in_terminal(layers, L)) return B2B_EINVAL;
 
   std::vector<Seg> segs;
   {
@@ -345,17 +314,17 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   // fold BatchNorm neighbours (a per-row affine) into the coupling launches: removes their own pass over HBM
   if (fold_ws && g_fold_bn) {
     for (size_t s = 0; s < segs.size(); ++s) {
-      if (!segs[s].coupling) continue;
-      if (s + 1 < segs.size() && !segs[s + 1].coupling && segs[s + 1].end > segs[s + 1].begin &&
+      if (segs[s].launch != B2B_LC_COUPLING) continue;
+      if (s + 1 < segs.size() && segs[s + 1].launch != B2B_LC_COUPLING && segs[s + 1].end > segs[s + 1].begin &&
           layers[segs[s + 1].begin].kind == B2B_BATCHNORM)
         segs[s].post = segs[s + 1].begin++;
-      if (s > 0 && !segs[s - 1].coupling && segs[s - 1].end > segs[s - 1].begin &&
+      if (s > 0 && segs[s - 1].launch != B2B_LC_COUPLING && segs[s - 1].end > segs[s - 1].begin &&
           layers[segs[s - 1].end - 1].kind == B2B_BATCHNORM)
         segs[s].pre = --segs[s - 1].end;
     }
     std::vector<Seg> kept;
     for (const Seg& g : segs)
-      if (g.coupling || g.end > g.begin) kept.push_back(g);
+      if (g.end > g.begin) kept.push_back(g);
     segs.swap(kept);
   }
   float* scratch = nullptr;
@@ -376,8 +345,8 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   }
   double* partials = nullptr;
   if (sum_out) {
-    if (segs.back().coupling || segs.back().spline || segs.back().scale)
-      return B2B_EUNSUPPORTED;  // batch sum needs a fusable last segment
+    if (segs.back().launch != B2B_LC_FUSED && segs.back().launch != B2B_LC_TRIL)
+      return B2B_EUNSUPPORTED;  // the batch sum comes from a fused or the terminal's launch
     if (ws_left < 4096 * sizeof(double)) return B2B_EWORKSPACE;
     partials = reinterpret_cast<double*>(ws);
   }
@@ -390,77 +359,81 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     // destination of this segment: y when given, else scratch for intermediates, nothing for the last
     float* dst = y ? y : (last_seg ? nullptr : scratch);
     const long long dst_ld = y ? ldy : D;
-    int rc;
-    if (segs[s].coupling) {
-      float* cdst = dst;
-      // logjac-only call with a trailing coupling layer still needs no store
-      const float* fold = nullptr;
-      if (segs[s].pre >= 0 || segs[s].post >= 0) {
-        rc = b2b_launch_bn_fold_prep(segs[s].pre >= 0 ? &layers[segs[s].pre] : nullptr,
-                                     segs[s].post >= 0 ? &layers[segs[s].post] : nullptr, D, fold_ws, stream);
+    const b2b_layer_desc& d = layers[segs[s].begin];
+    const int acc = lj_started ? 1 : 0;
+    int rc, n_launch = 0;
+    switch (segs[s].launch) {
+      case B2B_LC_COUPLING: {
+        const float* fold = nullptr;
+        if (segs[s].pre >= 0 || segs[s].post >= 0) {
+          rc = b2b_launch_bn_fold_prep(segs[s].pre >= 0 ? &layers[segs[s].pre] : nullptr,
+                                       segs[s].post >= 0 ? &layers[segs[s].post] : nullptr, D, fold_ws, stream);
+          if (rc != B2B_OK) return rc;
+          ++g_last_launches;
+          fold = fold_ws;
+        }
+        rc = B2B_EUNSUPPORTED;
+        if (tc_ws && g_coupling_variant != 1) {
+          rc = b2b_launch_coupling_affine_tc(d, fold, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, tc_ws, tc_bytes,
+                                             &n_launch, stream);
+          if (rc == B2B_OK) g_last_launches += n_launch;  // W preparation + main kernel (+ fp32 kernel on a ragged tail)
+        }
+        if (rc == B2B_EUNSUPPORTED) {
+          rc = b2b_launch_coupling_affine(d, fold, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
+          if (rc == B2B_OK) ++g_last_launches;
+        }
+        if (rc != B2B_OK) return rc;
+        break;
+      }
+      case B2B_LC_SPLINE:
+        rc = b2b_launch_coupling_rqs(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
         if (rc != B2B_OK) return rc;
         ++g_last_launches;
-        fold = fold_ws;
-      }
-      rc = B2B_EUNSUPPORTED;
-      if (tc_ws && g_coupling_variant != 1) {
-        int n_launch = 0;
-        rc = b2b_launch_coupling_affine_tc(layers[segs[s].begin], fold, cur, cdst, logjac, D, N, cur_ld, dst_ld,
-                                           lj_started ? 1 : 0, tc_ws, tc_bytes, &n_launch, stream);
-        if (rc == B2B_OK) g_last_launches += n_launch;  // W preparation + main kernel (+ fp32 kernel on a ragged tail)
-      }
-      if (rc == B2B_EUNSUPPORTED) {
-        rc = b2b_launch_coupling_affine(layers[segs[s].begin], fold, cur, cdst, logjac, D, N, cur_ld, dst_ld,
-                                        lj_started ? 1 : 0, stream);
-        if (rc == B2B_OK) ++g_last_launches;
-      }
-      if (rc != B2B_OK) return rc;
-    } else if (segs[s].spline) {
-      rc = b2b_launch_coupling_rqs(layers[segs[s].begin], cur, dst, logjac, D, N, cur_ld, dst_ld, lj_started ? 1 : 0, stream);
-      if (rc != B2B_OK) return rc;
-      ++g_last_launches;
-    } else if (segs[s].scale) {
-      int n_launch = 0;
-      rc = b2b_launch_scale_matrix(layers[segs[s].begin], cur, dst, logjac, D, N, cur_ld, dst_ld, lj_started ? 1 : 0,
-                                   scale_ws, scale_bytes, &n_launch, stream);
-      g_last_launches += n_launch;
-      if (rc != B2B_OK) return rc;
-    } else if (segs[s].tril) {  // always the last segment
-      rc = b2b_launch_mvnormal_tril(layers[segs[s].begin], cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0,
-                                    sum_out ? partials : nullptr, D, N, stream);
-      if (rc != B2B_OK) return rc;
-      ++g_last_launches;
-      if (sum_out) {
-        rc = b2b_launch_sum_partials(partials, b2b_tril_grid(D, N), sum_out, stream);
+        break;
+      case B2B_LC_SCALE:
+        rc = b2b_launch_scale_matrix(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, scale_ws, scale_bytes, &n_launch,
+                                     stream);
+        g_last_launches += n_launch;
+        if (rc != B2B_OK) return rc;
+        break;
+      case B2B_LC_TRIL:  // always the last segment
+        rc = b2b_launch_mvnormal_tril(d, cur, cur_ld, dst, dst_ld, logjac, acc, sum_out ? partials : nullptr, D, N, stream);
         if (rc != B2B_OK) return rc;
         ++g_last_launches;
-      }
-    } else {
-      B2BChainParams p;
-      memset(&p, 0, sizeof(p));
-      p.x = cur;
-      p.y = dst;
-      p.logjac = logjac;
-      p.N = N;
-      p.ldx = cur_ld;
-      p.ldy = dst_ld;
-      p.D = D;
-      p.L = segs[s].end - segs[s].begin;
-      p.accumulate = lj_started ? 1 : 0;
-      for (int l = 0; l < p.L; ++l) p.layers[l] = layers[segs[s].begin + l];
-      int grid = 0;
-      if (sum_out && last_seg) {
-        grid = fused_grid(p);
-        if (grid <= 0 || grid > 4096) return B2B_EUNSUPPORTED;
-        p.partials = partials;
-      }
-      rc = launch_fused(p, stream);
-      if (rc != B2B_OK) return rc;
-      g_last_launches += g_fused_launches;
-      if (sum_out && last_seg) {
-        rc = b2b_launch_sum_partials(partials, grid, sum_out, stream);
+        if (sum_out) {
+          rc = b2b_launch_sum_partials(partials, b2b_tril_grid(D, N), sum_out, stream);
+          if (rc != B2B_OK) return rc;
+          ++g_last_launches;
+        }
+        break;
+      case B2B_LC_FUSED: {
+        B2BChainParams p;
+        memset(&p, 0, sizeof(p));
+        p.x = cur;
+        p.y = dst;
+        p.logjac = logjac;
+        p.N = N;
+        p.ldx = cur_ld;
+        p.ldy = dst_ld;
+        p.D = D;
+        p.L = segs[s].end - segs[s].begin;
+        p.accumulate = acc;
+        for (int l = 0; l < p.L; ++l) p.layers[l] = layers[segs[s].begin + l];
+        int grid = 0;
+        if (sum_out && last_seg) {
+          grid = fused_grid(p);
+          if (grid <= 0 || grid > 4096) return B2B_EUNSUPPORTED;
+          p.partials = partials;
+        }
+        rc = launch_fused(p, stream);
         if (rc != B2B_OK) return rc;
-        ++g_last_launches;
+        g_last_launches += g_fused_launches;
+        if (sum_out && last_seg) {
+          rc = b2b_launch_sum_partials(partials, grid, sum_out, stream);
+          if (rc != B2B_OK) return rc;
+          ++g_last_launches;
+        }
+        break;
       }
     }
     if (dst) {
@@ -754,8 +727,6 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
 // the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
 namespace {
 
-enum VKind { VK_PLANAR, VK_RADIAL, VK_RQS, VK_COUPLING, VK_BN, VK_EW, VK_TRIL, VK_SPLINE, VK_SCALE };
-
 struct VSeg {
   int kind, begin, end;
   int Dk;  // rows the segment's kernel runs at: planar runs at D not in {32, 64, 128} are embedded in the next of them
@@ -764,54 +735,21 @@ struct VSeg {
 size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 size_t mat_bytes(int D, long long N) { return al256((size_t)D * (size_t)N * sizeof(float)); }
 
-int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& segs) {
+int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& segs) {  // valid descriptors
   segs.clear();
   for (int l = 0; l < L;) {
-    VSeg s{VK_EW, l, l + 1, D};
+    if (vjp_envelope(layers[l], D) != B2B_OK) return B2B_EUNSUPPORTED;
+    VSeg s{b2b_kind(layers[l].kind)->vjp, l, l + 1, D};
     int& e = s.end;
-    switch (layers[l].kind) {
-      case B2B_PLANAR:
-        if (D > 128) return B2B_EUNSUPPORTED;
-        while (e < L && e - l < 8 && layers[e].kind == B2B_PLANAR && (layers[e].inverse != 0) == (layers[l].inverse != 0)) ++e;
-        s.kind = VK_PLANAR;
-        s.Dk = D <= 32 ? 32 : D <= 64 ? 64 : 128;
-        break;
-      case B2B_RADIAL:
-        if (D > 128) return B2B_EUNSUPPORTED;
-        while (e < L && e - l < 8 && layers[e].kind == B2B_RADIAL) ++e;
-        s.kind = VK_RADIAL;
-        break;
-      case B2B_RQS:
-        if (D > 256 || layers[l].n0 > 64) return B2B_EUNSUPPORTED;
-        s.kind = VK_RQS;
-        break;
-      case B2B_COUPLING_AFFINE:
-        if (!b2b_coupling_affine_vjp_fits(layers[l], D)) return B2B_EUNSUPPORTED;
-        s.kind = VK_COUPLING;
-        break;
-      case B2B_BATCHNORM:
-        if (D > 1024) return B2B_EUNSUPPORTED;
-        s.kind = VK_BN;
-        break;
-      case B2B_COUPLING_RQS:
-        if (!b2b_coupling_rqs_fits(layers[l], D)) return B2B_EUNSUPPORTED;
-        s.kind = VK_SPLINE;
-        break;
-      case B2B_SCALE_MATRIX:
-        if (D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-        s.kind = VK_SCALE;
-        break;
-      case B2B_MVNORMAL_TRIL:  // the terminal, alone
-        if (D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
-        s.kind = VK_TRIL;
-        break;
-      default:  // PERMUTE / STACKED_EW (or the terminal MVNORMAL_DIAG alone)
-        if (D > 1024) return B2B_EUNSUPPORTED;
-        e = l;
-        while (e < L && e - l < 8 && (layers[e].kind == B2B_PERMUTE || layers[e].kind == B2B_STACKED_EW)) ++e;
-        if (e < L && layers[e].kind == B2B_MVNORMAL_DIAG) ++e;
-        if (e == l) return B2B_EINVAL;  // not a layer kind of include/b2b.h
-        s.kind = VK_EW;
+    if (s.kind == B2B_VC_PLANAR) {
+      while (e < L && e - l < 8 && layers[e].kind == B2B_PLANAR && (layers[e].inverse != 0) == (layers[l].inverse != 0)) ++e;
+      s.Dk = D <= 32 ? 32 : D <= 64 ? 64 : 128;
+    } else if (s.kind == B2B_VC_RADIAL) {
+      while (e < L && e - l < 8 && layers[e].kind == B2B_RADIAL) ++e;
+    } else if (s.kind == B2B_VC_EW) {  // PERMUTE / STACKED_EW layers and the terminal MVNORMAL_DIAG after them, or alone
+      e = l;
+      while (e < L && e - l < 8 && (layers[e].kind == B2B_PERMUTE || layers[e].kind == B2B_STACKED_EW)) ++e;
+      if (e < L && layers[e].kind == B2B_MVNORMAL_DIAG) ++e;
     }
     segs.push_back(s);
     l = e;
@@ -832,12 +770,12 @@ size_t seg_param_floats(const b2b_layer_desc* layers, const VSeg& s, int D) {
   auto r = [](size_t f) { return (f + 63) & ~(size_t)63; };
   const b2b_layer_desc& d = layers[s.begin];
   switch (s.kind) {
-    case VK_PLANAR: return 4 * r(n * s.Dk) + r(n);  // w̄, ū, b̄ as the kernel writes them (+ padded w, u)
-    case VK_RADIAL: return 2 * r(n) + r(n * D);
-    case VK_RQS: return 3 * r((size_t)D * d.n0);
-    case VK_COUPLING: return r((size_t)2 * d.n0 * d.n1) + r((size_t)2 * d.n0);
-    case VK_BN: return 2 * r(D);
-    case VK_SPLINE: return r((size_t)(3 * d.n2 - 1) * d.n0 * d.n1) + r((size_t)(3 * d.n2 - 1) * d.n0);
+    case B2B_VC_PLANAR: return 4 * r(n * s.Dk) + r(n);  // w̄, ū, b̄ as the kernel writes them (+ padded w, u)
+    case B2B_VC_RADIAL: return 2 * r(n) + r(n * D);
+    case B2B_VC_RQS: return 3 * r((size_t)D * d.n0);
+    case B2B_VC_COUPLING: return r((size_t)2 * d.n0 * d.n1) + r((size_t)2 * d.n0);
+    case B2B_VC_BN: return 2 * r(D);
+    case B2B_VC_SPLINE: return r((size_t)(3 * d.n2 - 1) * d.n0 * d.n1) + r((size_t)(3 * d.n2 - 1) * d.n0);
     default: return 0;
   }
 }
@@ -846,14 +784,14 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
   const int n = s.end - s.begin;
   const b2b_layer_desc& d = layers[s.begin];
   switch (s.kind) {
-    case VK_PLANAR: return b2b_planar_vjp_workspace(n, s.Dk, N);
-    case VK_RADIAL: return b2b_radial_vjp_workspace(n, D);
-    case VK_RQS: return b2b_rqs_vjp_workspace_bytes(d.n0, D);
-    case VK_COUPLING: return b2b_coupling_affine_vjp_workspace_bytes(d.n0, d.n1);
-    case VK_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
-    case VK_TRIL: return b2b_tril_vjp_workspace(D, N);
-    case VK_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
-    case VK_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
+    case B2B_VC_PLANAR: return b2b_planar_vjp_workspace(n, s.Dk, N);
+    case B2B_VC_RADIAL: return b2b_radial_vjp_workspace(n, D);
+    case B2B_VC_RQS: return b2b_rqs_vjp_workspace_bytes(d.n0, D);
+    case B2B_VC_COUPLING: return b2b_coupling_affine_vjp_workspace_bytes(d.n0, d.n1);
+    case B2B_VC_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
+    case B2B_VC_TRIL: return b2b_tril_vjp_workspace(D, N);
+    case B2B_VC_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
+    case B2B_VC_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
     default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
   }
 }
@@ -869,12 +807,12 @@ VLayout vjp_layout(const b2b_layer_desc* layers, const std::vector<VSeg>& segs, 
   VLayout v{};
   const size_t S = segs.size(), m = mat_bytes(D, N);
   v.ckpt = (S - 1) * m;
-  v.ncot = (S == 1 && (segs[0].kind == VK_EW || segs[0].kind == VK_TRIL)) ? 0 : 2;
+  v.ncot = (S == 1 && (segs[0].kind == B2B_VC_EW || segs[0].kind == B2B_VC_TRIL)) ? 0 : 2;
   // the planar kernels read x through TMA: an x they cannot read is copied (into a free checkpoint when there is one)
-  v.stage = (S == 1 && segs[0].kind == VK_PLANAR && segs[0].Dk == D) ? m : 0;
+  v.stage = (S == 1 && segs[0].kind == B2B_VC_PLANAR && segs[0].Dk == D) ? m : 0;
   size_t pf = 0;
   for (const VSeg& s : segs) {
-    if (s.kind == VK_PLANAR && s.Dk != D) v.Dk_pad = s.Dk;
+    if (s.kind == B2B_VC_PLANAR && s.Dk != D) v.Dk_pad = s.Dk;
     pf = std::max(pf, seg_param_floats(layers, s, D));
     v.kern = std::max(v.kern, al256(seg_kernel_bytes(layers, s, D, N)));
   }
@@ -886,18 +824,25 @@ VLayout vjp_layout(const b2b_layer_desc* layers, const std::vector<VSeg>& segs, 
 
 bool tma_ok(const float* p, long long ld) { return p && (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 4 == 0; }
 
-// elements of parameter slot i of layer d (the cotangent has the parameter's shape)
-size_t slot_len(const b2b_layer_desc& d, int i, int D) {
-  switch (d.kind) {
-    case B2B_PLANAR: return i == 2 ? 1 : D;
-    case B2B_RADIAL: return i == 2 ? D : 1;
-    case B2B_RQS: return (size_t)D * d.n0;
-    case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
-    case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
-    case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
-    case B2B_SCALE_MATRIX: return (size_t)D * D;
-    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
-  }
+// One launch copying the requested cotangents of the run ls[0, n) out of the arrays its kernel wrote: slot i of layer j
+// is at base[i] + j * step[i], and bars[4j + i] (NULL: not requested) receives it.  Nothing is launched when none is.
+int copy_run_bars(const b2b_layer_desc* ls, int n, float* const* bars, const float* const base[3],
+                  const size_t step[3], int D, int* launches, cudaStream_t stream) {
+  const float* src[24];
+  float* dst[24];
+  int len[24], dlen[24], c = 0;
+  for (int j = 0; j < n; ++j)
+    for (int i = 0; i < 3; ++i)
+      if (float* d = bars[4 * j + i]) {
+        src[c] = base[i] + j * step[i];
+        dst[c] = d;
+        len[c] = dlen[c] = (int)b2b_slot_len(ls[j], i, D);
+        ++c;
+      }
+  if (!c) return B2B_OK;
+  const int rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream);
+  if (rc == B2B_OK) ++*launches;
+  return rc;
 }
 
 }  // namespace
@@ -922,69 +867,17 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
     const int rc = validate_layer(layers[l], D, l == L - 1);
     if (rc != B2B_OK) return rc;
   }
-  auto bar = [&](int l, int i) -> float* { return param_bars ? param_bars[4 * l + i] : nullptr; };
-  // trainable slots: PLANAR w u b, RADIAL α_ β z_0, RQS widths heights derivatives, COUPLING W c, BATCHNORM b logs,
-  // MVNORMAL_DIAG μ σ (when given); a cotangent of anything else is not computed
-  for (int l = 0; l < L && param_bars; ++l)
-    for (int i = 0; i < 4; ++i) {
-      if (!bar(l, i)) continue;
-      const b2b_layer_desc& d = layers[l];
-      switch (d.kind) {
-        case B2B_PLANAR:
-        case B2B_RADIAL:
-        case B2B_RQS:
-          if (i == 3) return B2B_EUNSUPPORTED;
-          break;
-        case B2B_COUPLING_AFFINE:
-        case B2B_COUPLING_RQS:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (i == 1 && !d.p1) return B2B_EINVAL;
-          break;
-        case B2B_BATCHNORM:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          break;
-        case B2B_MVNORMAL_DIAG:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (!(i == 0 ? d.p0 : d.p1)) return B2B_EINVAL;
-          break;
-        case B2B_MVNORMAL_TRIL:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (i == 0 && !d.p0) return B2B_EINVAL;
-          break;
-        case B2B_SCALE_MATRIX:
-          if (i >= 1) return B2B_EUNSUPPORTED;
-          break;
-        default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
-      }
-    }
-  std::vector<VSeg> segs;
-  int rc = vjp_segments(layers, L, D, segs);
+  unsigned want;
+  int rc = b2b_vjp_check_slots(layers, L, param_bars, &want);
   if (rc != B2B_OK) return rc;
+  std::vector<VSeg> segs;
+  if ((rc = vjp_segments(layers, L, D, segs)) != B2B_OK) return rc;
+  rc = b2b_vjp_check_batch(layers, L, param_bars, x, ybar, xbar, D, N, ldx, ldybar, ldxbar, stream);
+  if (rc != B2B_OK || N == 0) return rc;
+  float* const none[4 * B2B_MAX_CHAIN] = {};
+  float* const* bars = param_bars ? param_bars : none;
+  auto bar = [&](int l, int i) { return bars[4 * l + i]; };
   int launches = 0;
-  if (N == 0) {  // empty batch: the requested cotangents are zero
-    for (int l = 0; l < L && param_bars; ++l)
-      for (int i = 0; i < 4; ++i)
-        if (bar(l, i)) {
-          const cudaError_t e = cudaMemsetAsync(bar(l, i), 0, slot_len(layers[l], i, D) * sizeof(float), stream);
-          if (e != cudaSuccess) return (int)e;
-          ++launches;
-        }
-    g_last_launches = launches;
-    return B2B_OK;
-  }
-  if (!x || !xbar || ldx < D || ldxbar < D || (ybar && ldybar < D)) return B2B_EINVAL;
-  {  // x̄ is written while x and ȳ are still being read
-    auto range = [&](const void* p, long long ld) {
-      const char* a = static_cast<const char*>(p);
-      return std::make_pair(a, a + ((size_t)(N - 1) * (size_t)ld + (size_t)D) * sizeof(float));
-    };
-    const auto xb = range(xbar, ldxbar), xr = range(x, ldx);
-    if (xb.first < xr.second && xr.first < xb.second) return B2B_EINVAL;
-    if (ybar) {
-      const auto yr = range(ybar, ldybar);
-      if (xb.first < yr.second && yr.first < xb.second) return B2B_EINVAL;
-    }
-  }
   const VLayout lay = vjp_layout(layers, segs, D, N);
   if (!workspace || workspace_bytes < lay.total) return B2B_EWORKSPACE;
   const int S = (int)segs.size();
@@ -1017,7 +910,7 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
   // 1. forward recompute: the input of every segment after the first (a dense Scale keeps its factor in the kernel
   // workspace, free until the reverse sweep)
   for (int s = 0; s + 1 < S; ++s) {
-    const bool sc = segs[s].kind == VK_SCALE;
+    const bool sc = segs[s].kind == B2B_VC_SCALE;
     rc = b2b_chain_run_f32(layers + segs[s].begin, segs[s].end - segs[s].begin, s == 0 ? x : ckpt[s], ckpt[s + 1],
                            nullptr, nullptr, D, N, s == 0 ? ldx : D, D, 0, sc ? kws : nullptr, sc ? kws_bytes : 0, stream);
     if (rc != B2B_OK) return rc;
@@ -1043,13 +936,11 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       return B2B_OK;
     };
     int nl = 0;
-    if (sg.kind == VK_PLANAR) {
+    if (sg.kind == B2B_VC_PLANAR) {
       const int Dk = sg.Dk;
       const size_t r64 = ((size_t)n * Dk + 63) & ~(size_t)63;
       float *wb = nullptr, *ub = nullptr, *bb = nullptr;
-      bool want = false;
-      for (int j = 0; j < n; ++j) want = want || bar(sg.begin + j, 0) || bar(sg.begin + j, 1) || bar(sg.begin + j, 2);
-      if (want) {
+      if (want >> sg.begin & ((1u << n) - 1)) {  // parameter cotangents of this run are requested
         wb = scratch;
         ub = scratch + r64;
         bb = scratch + 2 * r64;
@@ -1116,22 +1007,10 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       if (rc != B2B_OK) return rc;
       launches += nl;
       if (o != out) B2B_VJP_CUDA(cudaMemcpy2DAsync(out, (size_t)ldout * F, o, (size_t)ldo * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-      if (want) {
-        const float* src[24];
-        float* dst[24];
-        int len[24], dlen[24], c = 0;
-        for (int j = 0; j < n; ++j)
-          for (int i = 0; i < 3; ++i)
-            if (float* d = bar(sg.begin + j, i)) {
-              src[c] = i == 0 ? wb + (size_t)j * Dk : i == 1 ? ub + (size_t)j * Dk : bb + j;
-              dst[c] = d;
-              len[c] = dlen[c] = i == 2 ? 1 : D;
-              ++c;
-            }
-        if ((rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream)) != B2B_OK) return rc;
-        ++launches;
-      }
-    } else if (sg.kind == VK_RADIAL) {
+      const float* const base[3] = {wb, ub, bb};
+      const size_t step[3] = {(size_t)Dk, (size_t)Dk, 1};
+      if ((rc = copy_run_bars(ls, n, bars + 4 * sg.begin, base, step, D, &launches, stream)) != B2B_OK) return rc;
+    } else if (sg.kind == B2B_VC_RADIAL) {
       if (!cin && (rc = stage_cot(D)) != B2B_OK) return rc;
       float* ab = scratch;
       float* bb = scratch + 64 * ((n + 63) / 64);
@@ -1147,42 +1026,30 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       rc = b2b_launch_radial_chain_vjp(p, cin, ldcin, ljbar, out, ldout, ab, bb, zb, kws, kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
-      const float* src[24];
-      float* dst[24];
-      int len[24], dlen[24], c = 0;
-      for (int j = 0; j < n; ++j)
-        for (int i = 0; i < 3; ++i)
-          if (float* d = bar(sg.begin + j, i)) {
-            src[c] = i == 0 ? ab + j : i == 1 ? bb + j : zb + (size_t)j * D;
-            dst[c] = d;
-            len[c] = dlen[c] = i == 2 ? D : 1;
-            ++c;
-          }
-      if (c) {
-        if ((rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream)) != B2B_OK) return rc;
-        ++launches;
-      }
-    } else if (sg.kind == VK_EW) {
+      const float* const base[3] = {ab, bb, zb};
+      const size_t step[3] = {1, 1, (size_t)D};
+      if ((rc = copy_run_bars(ls, n, bars + 4 * sg.begin, base, step, D, &launches, stream)) != B2B_OK) return rc;
+    } else if (sg.kind == B2B_VC_EW) {
       const bool mvn = ls[n - 1].kind == B2B_MVNORMAL_DIAG;
       rc = b2b_launch_ew_vjp(ls, n, in, ldin, cin, ldcin, ljbar, out, ldout, mvn ? bar(sg.end - 1, 0) : nullptr,
                              mvn ? bar(sg.end - 1, 1) : nullptr, D, N, kws, kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
-    } else if (sg.kind == VK_SPLINE) {
+    } else if (sg.kind == B2B_VC_SPLINE) {
       // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c
       const b2b_layer_desc& d = ls[0];
       float* wb = bar(sg.begin, 0) ? bar(sg.begin, 0) : scratch;
       float* cb = !d.p1 ? nullptr : bar(sg.begin, 1) ? bar(sg.begin, 1)
-                                                       : scratch + ((slot_len(d, 0, D) + 63) & ~(size_t)63);
+                                                       : scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
       rc = b2b_launch_coupling_rqs_vjp(d, in, ldin, cin, ldcin, ljbar, out, ldout, wb, cb, D, N, kws, kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
-    } else if (sg.kind == VK_SCALE) {
+    } else if (sg.kind == B2B_VC_SCALE) {
       rc = b2b_launch_scale_matrix_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), D, N, kws, kws_bytes,
                                        &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
-    } else if (sg.kind == VK_TRIL) {
+    } else if (sg.kind == B2B_VC_TRIL) {
       rc = b2b_launch_tril_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), bar(sg.begin, 1), D, N, kws,
                                kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
@@ -1194,14 +1061,14 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       size_t off = 0;
       for (int i = 0; i < 3; ++i) {  // cotangents the caller did not ask for go to scratch
         pb[i] = bar(sg.begin, i);
-        if (!pb[i] && (sg.kind == VK_RQS || i < 2)) {
+        if (!pb[i] && (sg.kind == B2B_VC_RQS || i < 2)) {
           pb[i] = scratch + off;
-          off += (slot_len(d, i, D) + 63) & ~(size_t)63;
+          off += (b2b_slot_len(d, i, D) + 63) & ~(size_t)63;
         }
       }
-      if (sg.kind == VK_RQS)
+      if (sg.kind == B2B_VC_RQS)
         rc = b2b_rqs_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], pb[2], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
-      else if (sg.kind == VK_COUPLING)
+      else if (sg.kind == B2B_VC_COUPLING)
         rc = b2b_coupling_affine_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
       else
         rc = b2b_batchnorm_eval_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);

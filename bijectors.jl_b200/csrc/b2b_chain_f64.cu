@@ -65,35 +65,9 @@ __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_
 }  // namespace b2b
 
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last) {
-  switch (d.kind) {
-    case B2B_PLANAR:
-    case B2B_RADIAL:
-      if (!d.p0 || !d.p1 || !d.p2) return B2B_EINVAL;
-      break;
-    case B2B_RQS:
-      if (!d.p0 || !d.p1 || !d.p2 || d.n0 < 2) return B2B_EINVAL;
-      break;
-    case B2B_COUPLING_AFFINE:
-      if (!d.p0 || d.n0 < 1 || d.n1 < 1 || d.n0 + d.n1 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-      break;
-    case B2B_BATCHNORM:
-      if (!d.p0 || !d.p1 || !d.p2 || !d.p3) return B2B_EINVAL;
-      break;
-    case B2B_PERMUTE:
-    case B2B_STACKED_EW:
-      if (!d.i0) return B2B_EINVAL;
-      break;
-    case B2B_MVNORMAL_DIAG:
-      if (!last || d.inverse) return B2B_EINVAL;
-      break;
-    case B2B_MVNORMAL_TRIL:
-      if (!last || d.inverse || !d.p1) return B2B_EINVAL;
-      break;
-    case B2B_COUPLING_RQS: return B2B_EUNSUPPORTED;  // Float32 only (include/b2b.h)
-    case B2B_SCALE_MATRIX: return B2B_EUNSUPPORTED;  // Float32 only (include/b2b.h)
-    default: return B2B_EINVAL;
-  }
-  return B2B_OK;
+  const B2BKind* k = b2b_kind(d.kind);
+  if (k && !k->f64) return B2B_EUNSUPPORTED;  // Float32 only (include/b2b.h)
+  return b2b_check_desc(d, D, last);
 }
 
 extern "C" size_t b2b_chain_workspace_bytes_f64(int32_t L, int want_sum) { return (L > 0 && want_sum) ? 4096 * sizeof(double) : 0; }
@@ -117,8 +91,7 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     if (rc != B2B_OK) return rc;
     P.layers[l] = layers[l];
   }
-  if (sum_out && !logjac && layers[L - 1].kind != B2B_MVNORMAL_DIAG && layers[L - 1].kind != B2B_MVNORMAL_TRIL)
-    return B2B_EINVAL;
+  if (sum_out && !logjac && !b2b_ends_in_terminal(layers, L)) return B2B_EINVAL;
   P.x = x;
   P.y = y;
   P.logjac = logjac;

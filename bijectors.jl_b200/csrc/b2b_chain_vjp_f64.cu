@@ -22,7 +22,6 @@
 
 #include <cstdint>
 #include <cstring>
-#include <utility>
 
 #include "b2b_f64_device.cuh"
 
@@ -558,17 +557,6 @@ long long acc_len(const b2b_layer_desc_f64& d, int D) {
   return (n + 31) & ~31LL;
 }
 
-long long slot_len(const b2b_layer_desc_f64& d, int i, int D) {
-  switch (d.kind) {
-    case B2B_PLANAR: return i == 2 ? 1 : D;
-    case B2B_RADIAL: return i == 2 ? D : 1;
-    case B2B_RQS: return (long long)D * d.n0;
-    case B2B_COUPLING_AFFINE: return i == 0 ? 2LL * d.n0 * d.n1 : 2LL * d.n0;
-    case B2B_MVNORMAL_TRIL: return i == 1 ? (long long)D * D : D;
-    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
-  }
-}
-
 struct V64Plan {
   int Lf, wpc, warps;  // warps: the number the call uses (the workspace holds that many slots)
   long long T, P, stride;
@@ -581,7 +569,7 @@ struct V64Plan {
 // workspace grows with N only up to that bound.
 int v64_plan(const b2b_layer_desc_f64* layers, int L, int D, long long N, V64Plan& p) {
   if (D > 2048) return B2B_EUNSUPPORTED;
-  p.Lf = (layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL) ? L - 1 : L;
+  p.Lf = b2b_ends_in_terminal(layers, L) ? L - 1 : L;
   p.T = ((long long)p.Lf * D + 31) & ~31LL;
   p.P = 0;
   for (int l = 0; l < L; ++l) {
@@ -632,64 +620,11 @@ extern "C" int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, co
   V64Plan plan;
   int rc = v64_plan(layers, L, D, N, plan);
   if (rc != B2B_OK) return rc;
-  auto bar = [&](int l, int i) -> double* { return param_bars ? param_bars[4 * l + i] : nullptr; };
-  // trainable slots as for b2b_chain_vjp_f32: PLANAR w u b, RADIAL α_ β z_0, RQS widths heights derivatives, COUPLING W c,
-  // BATCHNORM b logs, MVNORMAL_DIAG μ σ (when given)
-  unsigned want = 0;
-  for (int l = 0; l < L && param_bars; ++l)
-    for (int i = 0; i < 4; ++i) {
-      if (!bar(l, i)) continue;
-      const b2b_layer_desc_f64& d = layers[l];
-      switch (d.kind) {
-        case B2B_PLANAR:
-        case B2B_RADIAL:
-        case B2B_RQS:
-          if (i == 3) return B2B_EUNSUPPORTED;
-          break;
-        case B2B_COUPLING_AFFINE:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (i == 1 && !d.p1) return B2B_EINVAL;
-          break;
-        case B2B_BATCHNORM:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          break;
-        case B2B_MVNORMAL_DIAG:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (!(i == 0 ? d.p0 : d.p1)) return B2B_EINVAL;
-          break;
-        case B2B_MVNORMAL_TRIL:
-          if (i >= 2) return B2B_EUNSUPPORTED;
-          if (i == 0 && !d.p0) return B2B_EINVAL;
-          break;
-        default: return B2B_EUNSUPPORTED;  // PERMUTE, STACKED_EW
-      }
-      want |= 1u << l;
-    }
+  unsigned want;
+  if ((rc = b2b_vjp_check_slots(layers, L, param_bars, &want)) != B2B_OK) return rc;
+  rc = b2b_vjp_check_batch(layers, L, param_bars, x, ybar, xbar, D, N, ldx, ldybar, ldxbar, stream);
+  if (rc != B2B_OK || N == 0) return rc;
   int launches = 0;
-  if (N == 0) {  // empty batch: the requested cotangents are zero
-    for (int l = 0; l < L && param_bars; ++l)
-      for (int i = 0; i < 4; ++i)
-        if (bar(l, i)) {
-          const cudaError_t e = cudaMemsetAsync(bar(l, i), 0, (size_t)slot_len(layers[l], i, D) * sizeof(double), stream);
-          if (e != cudaSuccess) return (int)e;
-          ++launches;
-        }
-    b2b_set_last_launch_count(launches);
-    return B2B_OK;
-  }
-  if (!x || !xbar || ldx < D || ldxbar < D || (ybar && ldybar < D)) return B2B_EINVAL;
-  {  // x̄ is written while x and ȳ are still being read
-    auto range = [&](const void* p, long long ld) {
-      const char* a = static_cast<const char*>(p);
-      return std::make_pair(a, a + ((size_t)(N - 1) * (size_t)ld + (size_t)D) * sizeof(double));
-    };
-    const auto xb = range(xbar, ldxbar), xr = range(x, ldx);
-    if (xb.first < xr.second && xr.first < xb.second) return B2B_EINVAL;
-    if (ybar) {
-      const auto yr = range(ybar, ldybar);
-      if (xb.first < yr.second && yr.first < xb.second) return B2B_EINVAL;
-    }
-  }
   if (!workspace || workspace_bytes < plan.bytes) return B2B_EWORKSPACE;
   char* ws = static_cast<char*>(workspace);
   ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
@@ -737,7 +672,7 @@ extern "C" int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     for (int l = 0; l < L; ++l) {
       F.off[l] = plan.off[l];
       F.layers[l] = layers[l];
-      for (int i = 0; i < 4; ++i) F.bars[4 * l + i] = bar(l, i);
+      for (int i = 0; i < 4; ++i) F.bars[4 * l + i] = param_bars ? param_bars[4 * l + i] : nullptr;
     }
     vjp_f64_finalize_kernel<<<L, V64_FIN_THREADS, 0, stream>>>(F);
     if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;

@@ -204,9 +204,7 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
   const int nseg = b2b_chain_segment_count(layers, L, D);
   if (nseg < 0) return nseg;
   const bool stage_y = y_host != nullptr || nseg > 1;
-  bool scale = false;
-  for (int l = 0; l < L; ++l) scale = scale || layers[l].kind == B2B_SCALE_MATRIX;
-  const size_t ws_bytes = scale ? c->ws_bytes : kWsBytes;
+  const size_t ws_bytes = b2b_chain_has_launch(layers, L, B2B_LC_SCALE) ? c->ws_bytes : kWsBytes;
   for (long long k = 0; k < nchunks; ++k) {
     const int s = (int)(k % c->n_streams);
     cudaStream_t st = c->streams[s];
@@ -215,7 +213,7 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
     cudaError_t e = cudaMemcpyAsync(c->dx[s], x_host + (size_t)c0 * D, (size_t)n * D * sizeof(float),
                                     cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) return (int)e;
-    const bool terminal = layers[L - 1].kind == B2B_MVNORMAL_DIAG || layers[L - 1].kind == B2B_MVNORMAL_TRIL;
+    const bool terminal = b2b_ends_in_terminal(layers, L);
     const bool want_lj = logjac_host != nullptr || (sum_host && !terminal);
     const int rc = b2b_chain_run_f32(layers, L, c->dx[s], stage_y ? c->dx[s] : nullptr,  // in place
                                      (want_lj || terminal) ? c->dlj[s] : nullptr,

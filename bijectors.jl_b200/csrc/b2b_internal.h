@@ -168,3 +168,148 @@ int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);
+
+// ---- layer kinds ---------------------------------------------------------------------------------------------------
+// What the chain orchestration knows about each kind of include/b2b.h.  A new kind enters the host code as one row of
+// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu, its slot lengths in b2b_slot_len, and its
+// own launch and reverse-mode code in b2b_chain_run_f32 / b2b_chain_vjp_f32.
+
+// Forward launch class: a run of fused column-local layers, or a launch of its own.
+enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL };
+// Reverse-mode segment class of b2b_chain_vjp_f32 (B2B_VC_EW: runs of STACKED_EW / PERMUTE, with MVNORMAL_DIAG).
+enum B2BVjpClass {
+  B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE
+};
+// descriptor pointer fields as bits
+enum { B2B_F_P0 = 1, B2B_F_P1 = 2, B2B_F_P2 = 4, B2B_F_P3 = 8, B2B_F_I0 = 16, B2B_F_I1 = 32 };
+
+struct B2BKind {
+  int kind;
+  int required;   // B2B_F_* fields that must be non-NULL
+  bool terminal;  // must be the chain's last element, with inverse == 0
+  int launch;     // B2BLaunchClass
+  int vjp;        // B2BVjpClass
+  int slots;      // trainable slots: param_bars entries 4l + i for i < slots (p<i>'s cotangent)
+  int optional;   // B2B_F_* bits of the slots that have a cotangent only when their parameter is given
+  bool f64;       // the Float64 entry points accept the kind
+};
+
+// the row of `kind`, NULL for a value include/b2b.h does not define
+inline const B2BKind* b2b_kind(int kind) {
+  // function-local, so that only the host compilation sees the table (at namespace scope the device pass does too)
+  constexpr int P012 = B2B_F_P0 | B2B_F_P1 | B2B_F_P2;
+  static const B2BKind kinds[] = {
+      // kind              required                     terminal launch        vjp              slots optional  f64
+      {B2B_PLANAR,          P012,                        false, B2B_LC_FUSED,    B2B_VC_PLANAR,   3, 0,        true},
+      {B2B_RADIAL,          P012,                        false, B2B_LC_FUSED,    B2B_VC_RADIAL,   3, 0,        true},
+      {B2B_RQS,             P012,                        false, B2B_LC_FUSED,    B2B_VC_RQS,      3, 0,        true},
+      {B2B_COUPLING_AFFINE, B2B_F_P0,                    false, B2B_LC_COUPLING, B2B_VC_COUPLING, 2, B2B_F_P1, true},
+      {B2B_BATCHNORM,       P012 | B2B_F_P3,             false, B2B_LC_FUSED,    B2B_VC_BN,       2, 0,        true},
+      {B2B_PERMUTE,         B2B_F_I0,                    false, B2B_LC_FUSED,    B2B_VC_EW,       0, 0,        true},
+      {B2B_STACKED_EW,      B2B_F_I0,                    false, B2B_LC_FUSED,    B2B_VC_EW,       0, 0,        true},
+      {B2B_MVNORMAL_DIAG,   0,                           true,  B2B_LC_FUSED,    B2B_VC_EW,       2, B2B_F_P0 | B2B_F_P1, true},
+      {B2B_MVNORMAL_TRIL,   B2B_F_P1,                    true,  B2B_LC_TRIL,     B2B_VC_TRIL,     2, B2B_F_P0, true},
+      {B2B_COUPLING_RQS,    B2B_F_P0 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE,   2, B2B_F_P1, false},
+      {B2B_SCALE_MATRIX,    B2B_F_P0,                    false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        false},
+  };
+  for (const B2BKind& k : kinds)
+    if (k.kind == kind) return &k;
+  return nullptr;
+}
+
+inline bool b2b_chain_has_launch(const b2b_layer_desc* layers, int L, int launch) {
+  for (int l = 0; l < L; ++l) {
+    const B2BKind* k = b2b_kind(layers[l].kind);
+    if (k && k->launch == launch) return true;
+  }
+  return false;
+}
+
+// whether the chain ends in its MvNormal terminal (its logjac output is then logpdf)
+template <class Desc>
+bool b2b_ends_in_terminal(const Desc* layers, int L) {
+  const B2BKind* k = b2b_kind(layers[L - 1].kind);
+  return k && k->terminal;
+}
+
+// B2B_EINVAL when `d` breaks the pointer and shape rules of include/b2b.h at D (`last`: the chain's final element),
+// else B2B_OK.  The rules of both precisions; the envelopes are the caller's.
+template <class Desc>
+int b2b_check_desc(const Desc& d, int D, bool last) {
+  const B2BKind* k = b2b_kind(d.kind);
+  if (!k) return B2B_EINVAL;
+  const void* const field[6] = {d.p0, d.p1, d.p2, d.p3, d.i0, d.i1};
+  for (int f = 0; f < 6; ++f)
+    if ((k->required >> f & 1) && !field[f]) return B2B_EINVAL;
+  if (k->terminal && (!last || d.inverse)) return B2B_EINVAL;
+  bool ok = true;
+  switch (d.kind) {
+    case B2B_RQS: ok = d.n0 >= 2; break;
+    case B2B_COUPLING_AFFINE:  // an index list may be NULL when n2 / n3 gives the first row of its contiguous range
+      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && (d.i0 || d.n2 >= 0) && (d.i1 || d.n3 >= 0);
+      break;
+    case B2B_COUPLING_RQS: ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && d.f0 > 0; break;
+    default: break;
+  }
+  return ok ? B2B_OK : B2B_EINVAL;
+}
+
+// elements of trainable slot i of `d` (its cotangent has the parameter's shape)
+template <class Desc>
+size_t b2b_slot_len(const Desc& d, int i, int D) {
+  switch (d.kind) {
+    case B2B_PLANAR: return i == 2 ? 1 : D;
+    case B2B_RADIAL: return i == 2 ? D : 1;
+    case B2B_RQS: return (size_t)D * d.n0;
+    case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
+    case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
+    case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
+    case B2B_SCALE_MATRIX: return (size_t)D * D;
+    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
+  }
+}
+
+// ---- checks shared by b2b_chain_vjp_f32 and b2b_chain_vjp_f64 (valid descriptors; each entry point keeps its order) ----
+// The requested cotangents (non-NULL param_bars entries): B2B_EUNSUPPORTED for a slot the kind does not train,
+// B2B_EINVAL for an optional parameter that is absent.  *want gets bit l for every layer with a request.
+template <class Desc, class T>
+int b2b_vjp_check_slots(const Desc* layers, int L, T* const* param_bars, unsigned* want) {
+  *want = 0;
+  for (int l = 0; l < L && param_bars; ++l)
+    for (int i = 0; i < 4; ++i) {
+      if (!param_bars[4 * l + i]) continue;
+      const B2BKind& k = *b2b_kind(layers[l].kind);
+      const void* const p[4] = {layers[l].p0, layers[l].p1, layers[l].p2, layers[l].p3};
+      if (i >= k.slots) return B2B_EUNSUPPORTED;
+      if ((k.optional >> i & 1) && !p[i]) return B2B_EINVAL;
+      *want |= 1u << l;
+    }
+  return B2B_OK;
+}
+
+// N == 0: zeroes the requested cotangents, which is the whole call.  Otherwise checks the batch arguments: x̄ is written
+// while x and ȳ are still being read, so it must not overlap either.
+template <class Desc, class T>
+int b2b_vjp_check_batch(const Desc* layers, int L, T* const* param_bars, const T* x, const T* ybar, T* xbar, int D,
+                        long long N, long long ldx, long long ldybar, long long ldxbar, cudaStream_t stream) {
+  if (N == 0) {
+    int launches = 0;
+    for (int l = 0; l < L && param_bars; ++l)
+      for (int i = 0; i < 4; ++i)
+        if (T* bar = param_bars[4 * l + i]) {
+          const cudaError_t e = cudaMemsetAsync(bar, 0, b2b_slot_len(layers[l], i, D) * sizeof(T), stream);
+          if (e != cudaSuccess) return (int)e;
+          ++launches;
+        }
+    b2b_set_last_launch_count(launches);
+    return B2B_OK;
+  }
+  if (!x || !xbar || ldx < D || ldxbar < D || (ybar && ldybar < D)) return B2B_EINVAL;
+  const size_t span = ((size_t)(N - 1) * (size_t)ldxbar + (size_t)D) * sizeof(T);
+  auto overlaps = [&](const T* p, long long ld) {
+    const char *a = reinterpret_cast<const char*>(p), *b = reinterpret_cast<const char*>(xbar);
+    return b < a + ((size_t)(N - 1) * (size_t)ld + (size_t)D) * sizeof(T) && a < b + span;
+  };
+  if (overlaps(x, ldx) || (ybar && overlaps(ybar, ldybar))) return B2B_EINVAL;
+  return B2B_OK;
+}

@@ -808,18 +808,20 @@ def isclosedform(t) -> bool:
 # reverse mode of any chain: b2b_chain_vjp_f32 (Float32 batches) / b2b_chain_vjp_f64 (Float64 batches)
 # --------------------------------------------------------------------------------------------------
 
-# names of the trainable descriptor slots p0..p3 of each kind (the reference's field names)
-_SLOT_NAMES = {
-    _lib.PLANAR: ("w", "u", "b"),
-    _lib.RADIAL: ("α_", "β", "z_0"),
-    _lib.RQS: ("widths", "heights", "derivatives"),
-    _lib.COUPLING_AFFINE: ("W", "c"),
-    _lib.BATCHNORM: ("b", "logs"),
-    _lib.MVNORMAL_DIAG: ("μ", "σ"),
-    _lib.MVNORMAL_TRIL: ("μ", "L"),
-    _lib.COUPLING_RQS: ("W", "c"),
-    _lib.SCALE_MATRIX: ("a",),
+# The trainable descriptor slots p0, p1, ... of each kind: (the reference's field names, the shapes of the device tensors
+# the library reads, the slots whose storage is column-major -- the parameter's transpose).
+_SLOTS = {
+    _lib.PLANAR: (("w", "u", "b"), lambda d, D: ((D,), (D,), (1,)), ()),
+    _lib.RADIAL: (("α_", "β", "z_0"), lambda d, D: ((1,), (1,), (D,)), ()),
+    _lib.RQS: (("widths", "heights", "derivatives"), lambda d, D: ((d.n0, D),) * 3, (0, 1, 2)),
+    _lib.COUPLING_AFFINE: (("W", "c"), lambda d, D: ((d.n1, 2 * d.n0), (2 * d.n0,)), (0,)),
+    _lib.BATCHNORM: (("b", "logs"), lambda d, D: ((D,), (D,)), ()),
+    _lib.MVNORMAL_DIAG: (("μ", "σ"), lambda d, D: ((D,), (D,)), ()),
+    _lib.MVNORMAL_TRIL: (("μ", "L"), lambda d, D: ((D,), (D, D)), (1,)),
+    _lib.COUPLING_RQS: (("W", "c"), lambda d, D: ((d.n1, (3 * d.n2 - 1) * d.n0), ((3 * d.n2 - 1) * d.n0,)), (0,)),
+    _lib.SCALE_MATRIX: (("a",), lambda d, D: ((D, D),), (0,)),
 }
+_SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 
 
 def _trainable_slots(d) -> List[int]:
@@ -830,20 +832,13 @@ def _trainable_slots(d) -> List[int]:
 
 def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
     """Shape of the device tensor behind slot i of ``d`` (the storage layout the library reads)."""
-    if d.kind == _lib.PLANAR:
-        return (1,) if i == 2 else (D,)
-    if d.kind == _lib.RADIAL:
-        return (D,) if i == 2 else (1,)
-    if d.kind == _lib.RQS:
-        return (d.n0, D)  # column-major D × K+1
-    if d.kind == _lib.COUPLING_AFFINE:
-        return (d.n1, 2 * d.n0) if i == 0 else (2 * d.n0,)  # W column-major (2n1 × n2)
-    if d.kind == _lib.COUPLING_RQS:
-        J = 3 * d.n2 - 1
-        return (d.n1, J * d.n0) if i == 0 else (J * d.n0,)  # W column-major ((3K−1)n1 × n2)
-    if (d.kind == _lib.MVNORMAL_TRIL and i == 1) or d.kind == _lib.SCALE_MATRIX:
-        return (D, D)  # L / A column-major: element (i, j) at [j, i]
-    return (D,)
+    return _SLOTS[d.kind][1](d, D)[i]
+
+
+def _slot_grads(d, l: int, bars) -> dict:
+    """The cotangents ``bars`` holds for descriptor l (``d``), keyed by field name, each in its parameter's orientation."""
+    names, _, colmajor = _SLOTS.get(d.kind, ((), None, ()))
+    return {name: bars[(l, i)].t() if i in colmajor else bars[(l, i)] for i, name in enumerate(names) if (l, i) in bars}
 
 
 # per batch dtype: (name, descriptor type, workspace query, entry point)
@@ -909,10 +904,7 @@ def _leaf_grads(descs, counts, bars) -> List[dict]:
     for c in counts:
         g = {}
         for l in range(k, k + c):
-            d = descs[l]
-            for i in _trainable_slots(d):
-                t = bars[(l, i)]
-                g[_SLOT_NAMES[d.kind][i]] = t.t() if (d.kind in (_lib.RQS, _lib.SCALE_MATRIX) or (d.kind in (_lib.COUPLING_AFFINE, _lib.COUPLING_RQS) and i == 0)) else t
+            g.update(_slot_grads(descs[l], l, bars))
         grads.append(g)
         k += c
     return grads

@@ -195,7 +195,7 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     ``flow_grads`` one dict per leaf of ``flatten(td.transform)`` in FLOW order (see chain_vjp for the keys) and
     ``base_grads`` = {"μ", "σ"} (or {"μ", "L"} for a full-covariance base, L̄ lower triangular) for the base parameters
     that are given; all summed over the columns of this batch."""
-    from .interface import _SLOT_NAMES, _chain_vjp_raw, _leaf_descs, _leaf_grads, _trainable_slots
+    from .interface import _chain_vjp_raw, _leaf_descs, _leaf_grads, _slot_grads, _trainable_slots
 
     D, N, _ = _batch_view(y)
     if D != len(td.dist):
@@ -208,7 +208,4 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     ybar, bars = _chain_vjp_raw(descs, y, None, lpbar, want)
     flow = _leaf_grads(descs, counts, bars)[::-1]
     T = len(descs) - 1
-    base = {name: bars[(T, i)] for i, name in enumerate(_SLOT_NAMES[descs[T].kind]) if (T, i) in bars}
-    if "L" in base:
-        base["L"] = base["L"].t()  # the cotangent's storage is column-major, like L's
-    return ybar, flow, base
+    return ybar, flow, _slot_grads(descs[T], T, bars)
