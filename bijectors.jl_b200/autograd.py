@@ -372,7 +372,7 @@ def _trainable_tensors(leaf) -> List[torch.Tensor]:
     if isinstance(lay, RationalQuadraticSpline):
         return [lay.widths, lay.heights, lay.derivatives]
     if isinstance(lay, Coupling):
-        return [t for t in (lay.θ.W, lay.θ.c) if t is not None]
+        return [t for t in lay.θ._tensors() if t is not None]
     if isinstance(lay, Scale) and lay.dense:
         return [lay._A]
     if isinstance(lay, InvertibleBatchNorm):

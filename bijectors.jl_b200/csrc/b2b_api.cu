@@ -59,6 +59,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_fits(d.n0, d.n1, D); break;
     case B2B_COUPLING_RQS: ok = b2b_coupling_rqs_fits(d, D); break;
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
+    case B2B_COUPLING_MLP: ok = b2b_coupling_mlp_fits(d, D); break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
     default: break;
   }
@@ -75,6 +76,7 @@ static int vjp_envelope(const b2b_layer_desc& d, int D) {
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_vjp_fits(d, D); break;
     case B2B_COUPLING_RQS:
     case B2B_SCALE_MATRIX:
+    case B2B_COUPLING_MLP:
     case B2B_MVNORMAL_TRIL: return fwd_envelope(d, D);
     default: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
   }
@@ -240,7 +242,7 @@ extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_
   // limit, or a descriptor the call finds invalid, is still sized
   for (int l = 0; layers && l < L; ++l) {
     const B2BKind* k = b2b_kind(layers[l].kind);
-    if (k && (k->launch == B2B_LC_SPLINE || k->launch == B2B_LC_SCALE || (k->launch == B2B_LC_TRIL && l == L - 1)) &&
+    if (k && (k->launch == B2B_LC_SPLINE || k->launch == B2B_LC_SCALE || k->launch == B2B_LC_MLP || (k->launch == B2B_LC_TRIL && l == L - 1)) &&
         fwd_envelope(layers[l], D) != B2B_OK)
       return 0;
   }
@@ -387,6 +389,11 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
       }
       case B2B_LC_SPLINE:
         rc = b2b_launch_coupling_rqs(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
+        if (rc != B2B_OK) return rc;
+        ++g_last_launches;
+        break;
+      case B2B_LC_MLP:
+        rc = b2b_launch_coupling_mlp(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
         if (rc != B2B_OK) return rc;
         ++g_last_launches;
         break;
@@ -791,6 +798,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case B2B_VC_BN: return b2b_batchnorm_eval_vjp_workspace_bytes(D);
     case B2B_VC_TRIL: return b2b_tril_vjp_workspace(D, N);
     case B2B_VC_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
+    case B2B_VC_MLP: return b2b_coupling_mlp_vjp_workspace(d, D, N);
     case B2B_VC_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
     default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
   }
@@ -1042,6 +1050,11 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       float* cb = !d.p1 ? nullptr : bar(sg.begin, 1) ? bar(sg.begin, 1)
                                                        : scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
       rc = b2b_launch_coupling_rqs_vjp(d, in, ldin, cin, ldcin, ljbar, out, ldout, wb, cb, D, N, kws, kws_bytes, &nl, stream);
+      if (rc != B2B_OK) return rc;
+      launches += nl;
+    } else if (sg.kind == B2B_VC_MLP) {  // the four sums come from one kernel: those not asked for are dropped
+      float* const pb[4] = {bar(sg.begin, 0), bar(sg.begin, 1), bar(sg.begin, 2), bar(sg.begin, 3)};
+      rc = b2b_launch_coupling_mlp_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, pb, D, N, kws, kws_bytes, &nl, stream);
       if (rc != B2B_OK) return rc;
       launches += nl;
     } else if (sg.kind == B2B_VC_SCALE) {

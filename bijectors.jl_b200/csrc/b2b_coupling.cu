@@ -18,81 +18,10 @@
 
 #include <cstring>
 
+#include "b2b_coupling_tile.cuh"
 #include "b2b_internal.h"
 
 namespace b2b {
-
-constexpr int CP_TC = 64;       // columns per tile
-constexpr int CP_LD = CP_TC + 1;  // padded row stride of the smem tile
-constexpr int CP_THREADS = 256;
-
-// Conditioner GEMM [s; t] = W·x₂ + c and the affine epilogue on x₁, in place in shared memory, for one 64-column tile;
-// leaves the column sums of s of this warp in red[warp][*].  The two programs stage rows differently: x₂ row k lives at
-// X2 + row2(k)·CP_LD, x₁ row j at X1 + row1(j)·CP_LD.
-template <bool INV, class Row2, class Row1>
-__device__ __forceinline__ void coupling_tile(const float* X2, float* X1, Row2 row2, Row1 row1, const float* __restrict__ W,
-                                              const float* __restrict__ cvec, int n1, int n2, bool wvec, float* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int ldw = 2 * n1;
-  const int cA = lane, cB = lane + 32;
-  float sumA = 0.f, sumB = 0.f;
-  for (int jb = 4 * warp; jb < n1; jb += 4 * (CP_THREADS / 32)) {
-    float sA[4] = {0.f, 0.f, 0.f, 0.f}, sB[4] = {0.f, 0.f, 0.f, 0.f};
-    float tA[4] = {0.f, 0.f, 0.f, 0.f}, tB[4] = {0.f, 0.f, 0.f, 0.f};
-    if (wvec) {
-#pragma unroll 4
-      for (int k = 0; k < n2; ++k) {
-        const int r2 = row2(k);
-        const float xa = X2[r2 * CP_LD + cA], xb = X2[r2 * CP_LD + cB];
-        const float4 ws = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + jb));
-        const float4 wt = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * ldw + n1 + jb));
-        sA[0] = fmaf(ws.x, xa, sA[0]); sB[0] = fmaf(ws.x, xb, sB[0]);
-        sA[1] = fmaf(ws.y, xa, sA[1]); sB[1] = fmaf(ws.y, xb, sB[1]);
-        sA[2] = fmaf(ws.z, xa, sA[2]); sB[2] = fmaf(ws.z, xb, sB[2]);
-        sA[3] = fmaf(ws.w, xa, sA[3]); sB[3] = fmaf(ws.w, xb, sB[3]);
-        tA[0] = fmaf(wt.x, xa, tA[0]); tB[0] = fmaf(wt.x, xb, tB[0]);
-        tA[1] = fmaf(wt.y, xa, tA[1]); tB[1] = fmaf(wt.y, xb, tB[1]);
-        tA[2] = fmaf(wt.z, xa, tA[2]); tB[2] = fmaf(wt.z, xb, tB[2]);
-        tA[3] = fmaf(wt.w, xa, tA[3]); tB[3] = fmaf(wt.w, xb, tB[3]);
-      }
-    } else {
-      for (int k = 0; k < n2; ++k) {
-        const int r2 = row2(k);
-        const float xa = X2[r2 * CP_LD + cA], xb = X2[r2 * CP_LD + cB];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (jb + q < n1) {
-            const float ws = __ldg(W + (size_t)k * ldw + jb + q);
-            const float wt = __ldg(W + (size_t)k * ldw + n1 + jb + q);
-            sA[q] = fmaf(ws, xa, sA[q]); sB[q] = fmaf(ws, xb, sB[q]);
-            tA[q] = fmaf(wt, xa, tA[q]); tB[q] = fmaf(wt, xb, tB[q]);
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int j = jb + q;
-      if (j < n1) {
-        const float cs = cvec ? __ldg(cvec + j) : 0.f, ct = cvec ? __ldg(cvec + n1 + j) : 0.f;
-        const int r1 = row1(j);
-        const float s_a = sA[q] + cs, s_b = sB[q] + cs, t_a = tA[q] + ct, t_b = tB[q] + ct;
-        const float xa = X1[r1 * CP_LD + cA], xb = X1[r1 * CP_LD + cB];
-        if (!INV) {
-          X1[r1 * CP_LD + cA] = fmaf(expf(s_a), xa, t_a);  // exp(s)·x₁ + t  (scale.jl:13, shift.jl:14)
-          X1[r1 * CP_LD + cB] = fmaf(expf(s_b), xb, t_b);
-        } else {
-          X1[r1 * CP_LD + cA] = (xa - t_a) / expf(s_a);  // inv.(a) .* (y₁ + (−t))  (scale.jl:16, shift.jl:12)
-          X1[r1 * CP_LD + cB] = (xb - t_b) / expf(s_b);
-        }
-        sumA += s_a;
-        sumB += s_b;
-      }
-    }
-  }
-  red[warp * CP_TC + cA] = sumA;
-  red[warp * CP_TC + cB] = sumB;
-}
 
 // Layers whose D rows fit shared memory (D <= 777 at n2 = 128) stage the whole tile: every row is read and written
 // coalesced, column by column.

@@ -1,0 +1,183 @@
+// Neural-network coupling layer, B2B_COUPLING_MLP (include/b2b.h): Coupling(θ, mask) (coupling.jl:206-228) with the
+// affine law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) whose parameters come from a one-hidden-layer network,
+//   [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂,   σ = tanh or LeakyReLU(a),
+// forward and inverse, in exact fp32 on the CUDA cores.
+//
+// Mapping.  A CTA owns a tile of 64 columns and stages the n1 + n2 rows it reads, [row][column] with pitch 65, as
+// coupling_affine_rows_kernel does (pass-through rows go global to global and are skipped in place).  Phase 1 forms
+// h = σ(W₁·x₂ + c₁) into a third shared-memory block [H][65] with coupling_gemm_block, eight hidden rows per warp and
+// step.  Phase 2 is coupling_tile of the affine kernel with X2 = h, n2 = H, W = W₂, cvec = c₂: the same GEMM, exp / FMA
+// epilogue and per-warp Σ s.  Every output is a fixed-order fmaf chain over k, then over the hidden units, so it does not
+// depend on N, the tile or the grid.
+#include <cuda_runtime.h>
+
+#include "b2b_coupling_mlp.cuh"
+#include "b2b_coupling_tile.cuh"
+#include "b2b_internal.h"
+
+namespace b2b {
+
+struct CmlpParams {
+  const float* x;
+  float* y;
+  float* logjac;
+  const float *W1, *c1, *W2, *c2;
+  const int *idx1, *idx2;
+  long long N, ldx, ldy;
+  int D, n1, n2, H, act, accumulate;
+  float slope;
+};
+
+template <bool INV>
+__global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __grid_constant__ CmlpParams P) {
+  // x and y may alias (in place): every element is read before it is written, by the same CTA
+  extern __shared__ float smem[];
+  const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H;
+  float* X2 = smem;                                      // [n2][CP_LD]  conditioner input x₂
+  float* X1 = X2 + (size_t)n2 * CP_LD;                   // [n1][CP_LD]  x₁, transformed in place
+  float* Hs = X1 + (size_t)n1 * CP_LD;                   // [H][CP_LD]   hidden layer h
+  float* red = Hs + (size_t)H * CP_LD;                   // [8][CP_TC]
+  int* sidx2 = reinterpret_cast<int*>(red + 8 * CP_TC);  // [n2]
+  int* sidx1 = sidx2 + n2;                               // [n1]
+  unsigned* coupled = reinterpret_cast<unsigned*>(sidx1 + n1);  // [ceil(D/32)] bit r: row r is in idx1 or idx2
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* x = P.x;
+  float* y = P.y;
+  const bool copy_through = y && y != x;  // in place, x₂ and x₃ stay where they are
+  const bool has_x3 = n1 + n2 < D;
+  const int nwords = (D + 31) >> 5;
+  if (has_x3 && copy_through)
+    for (int k = threadIdx.x; k < nwords; k += CP_THREADS) coupled[k] = 0u;
+  for (int k = threadIdx.x; k < n2; k += CP_THREADS) sidx2[k] = P.idx2[k];
+  for (int k = threadIdx.x; k < n1; k += CP_THREADS) sidx1[k] = P.idx1[k];
+  __syncthreads();
+  if (has_x3 && copy_through) {
+    for (int k = threadIdx.x; k < n2; k += CP_THREADS) atomicOr(&coupled[sidx2[k] >> 5], 1u << (sidx2[k] & 31));
+    for (int k = threadIdx.x; k < n1; k += CP_THREADS) atomicOr(&coupled[sidx1[k] >> 5], 1u << (sidx1[k] & 31));
+  }
+  const bool vec1 = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
+  const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
+  const long long tiles = (P.N + CP_TC - 1) / CP_TC;
+  auto same = [](int k) { return k; };
+
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long col0 = tile * CP_TC;
+    __syncthreads();  // previous tile fully written back / index tables visible
+    // ---- load + transpose x₂ and x₁; pass-through rows go straight to y ---------------------------------------
+    for (int c = warp; c < CP_TC; c += CP_THREADS / 32) {
+      const long long col = col0 + c;
+      if (col < P.N) {
+        const float* xc = x + col * P.ldx;
+        for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = __ldcs(xc + sidx2[k]);
+        if (y)  // the log-Jacobian needs x₂ only
+          for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = __ldcs(xc + sidx1[k]);
+        if (has_x3 && copy_through) {
+          float* yc = y + col * P.ldy;
+          for (int r = lane; r < D; r += 32)
+            if (!((coupled[r >> 5] >> (r & 31)) & 1u)) __stcs(yc + r, __ldcs(xc + r));
+        }
+      } else {
+        for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = 0.f;
+        for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = 0.f;
+      }
+    }
+    __syncthreads();
+    // ---- phase 1: h = σ(W₁·x₂ + c₁) ---------------------------------------------------------------------------
+    for (int jb = 8 * warp; jb < H; jb += 8 * (CP_THREADS / 32)) {
+      float va[4][2] = {}, vb[4][2] = {};
+      coupling_gemm_block<2>(X2, CP_LD, same, n2, P.W1 + jb, P.W1 + jb + 4, H, H - jb, H - jb - 4, vec1, va, vb);
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int m = jb + q;
+        if (m < H) {
+          const float c = P.c1 ? __ldg(P.c1 + m) : 0.f;
+          float dh;
+#pragma unroll
+          for (int u = 0; u < 2; ++u)
+            mlp_act(P.act, P.slope, (q < 4 ? va[q & 3][u] : vb[q & 3][u]) + c, Hs[m * CP_LD + lane + 32 * u], dh);
+        }
+      }
+    }
+    __syncthreads();
+    // ---- phase 2: [s; t] = W₂·h + c₂ and the affine law on x₁ ----------------------------------------------------
+    coupling_tile<INV>(Hs, X1, same, same, P.W2, P.c2, n1, H, vec2, red);
+    __syncthreads();
+    // ---- write back x₁ (and x₂ unless it is already in place) ------------------------------------------------------
+    if (y) {
+      for (int c = warp; c < CP_TC; c += CP_THREADS / 32) {
+        const long long col = col0 + c;
+        if (col < P.N) {
+          float* yc = y + col * P.ldy;
+          for (int k = lane; k < n1; k += 32) __stcs(yc + sidx1[k], X1[k * CP_LD + c]);
+          if (copy_through)
+            for (int k = lane; k < n2; k += 32) __stcs(yc + sidx2[k], X2[k * CP_LD + c]);
+        }
+      }
+    }
+    if (P.logjac && threadIdx.x < CP_TC) {
+      const long long col = col0 + threadIdx.x;
+      if (col < P.N) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < CP_THREADS / 32; ++w) s += red[w * CP_TC + threadIdx.x];
+        const float base = P.accumulate ? P.logjac[col] : 0.f;
+        P.logjac[col] = INV ? base - s : base + s;  // Σ log|exp(s)| = Σ s  (scale.jl:31)
+      }
+    }
+  }
+}
+
+// x₂, x₁ and h tiles, the column-sum slab, both index tables and the coupled-row bitmap
+static size_t cmlp_smem_bytes(int n1, int n2, int H, int D) {
+  return ((size_t)(n1 + n2 + H) * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int) +
+         (size_t)((D + 31) / 32) * sizeof(unsigned);
+}
+
+}  // namespace b2b
+
+bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D) {
+  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_MLP_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_MLP_MAX_N && d.n2 >= 1 &&
+         d.n2 <= B2B_COUPLING_MLP_MAX_H && D <= B2B_COUPLING_MLP_MAX_D;
+}
+
+int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
+                            long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
+  using namespace b2b;
+  if (!b2b_coupling_mlp_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (N <= 0) return B2B_OK;
+  CmlpParams P;
+  P.x = x;
+  P.y = y;
+  P.logjac = logjac;
+  P.W1 = d.p0;
+  P.c1 = d.p1;
+  P.W2 = d.p2;
+  P.c2 = d.p3;
+  P.idx1 = d.i0;
+  P.idx2 = d.i1;
+  P.N = N;
+  P.ldx = ldx;
+  P.ldy = ldy;
+  P.D = D;
+  P.n1 = d.n0;
+  P.n2 = d.n1;
+  P.H = d.n2;
+  P.act = d.n3;
+  P.accumulate = accumulate;
+  P.slope = d.f0;
+  const size_t smem = cmlp_smem_bytes(d.n0, d.n1, d.n2, D);
+  void (*kernel)(const CmlpParams) = d.inverse ? coupling_mlp_kernel<true> : coupling_mlp_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return (int)e;
+  int dev = 0, sms = 0, per_sm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CP_THREADS, smem);
+  if (e != cudaSuccess) return (int)e;
+  if (per_sm < 1) per_sm = 1;
+  const long long tiles = (N + CP_TC - 1) / CP_TC;
+  long long grid = (long long)sms * per_sm;
+  if (grid > tiles) grid = tiles;
+  kernel<<<(int)grid, CP_THREADS, smem, stream>>>(P);
+  return (int)cudaGetLastError();
+}

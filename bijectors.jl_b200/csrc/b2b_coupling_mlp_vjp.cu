@@ -1,0 +1,347 @@
+// Reverse mode of the neural-network coupling layer, B2B_COUPLING_MLP, either direction: cotangents of the input and of
+// W₁, c₁, W₂, c₂ -- what the reference's reverse-mode AD computes through coupling.jl:206-228 with the law
+// Shift(t) ∘ Scale(exp.(s)), [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂.  With v = W₁x₂ + c₁, h = σ(v) and the affine law's
+// s̄, t̄, x̄₁ (formed as b2b_coupling_vjp.cu forms them):
+//   h̄ = W₂ᵀ[s̄; t̄]     v̄ = h̄ ⊙ σ′(v)     x̄₂ = ȳ₂ + W₁ᵀ v̄     x̄₃ = ȳ₃
+//   W̄₂ = Σₙ [s̄; t̄] hᵀ   c̄₂ = Σₙ [s̄; t̄]    W̄₁ = Σₙ v̄ x₂ᵀ       c̄₁ = Σₙ v̄
+//
+// Mapping.  A fixed grid of at most one CTA per SM walks groups of 32·S columns round-robin (S = 4, 2 or 1 sub-tiles,
+// the most whose factors fit shared memory: S = 2 at n1 = n2 = 128, H = 256).  Each sub-tile of 32 columns (one per
+// lane) runs the network forward and backward with coupling_gemm_block and its transposed counterpart, leaving the four
+// factors x₂, [s̄; t̄], h and v̄ of its columns in shared memory.  After the group's last sub-tile the CTA forms the
+// four parameter sums of the whole group, a 4 x 4 register block per thread swept over the matrices, and adds them to
+// its private slice of the workspace ([W̄₁ | c̄₁ | W̄₂ | c̄₂], every element always by the same thread): one
+// read-modify-write of the slice per 32·S columns.  A second kernel sums the slices in order, in fp64, into the caller's
+// arrays.  Deterministic, no atomics; the workspace depends on the grid, not on N.
+#include <cuda_runtime.h>
+
+#include "b2b_coupling_mlp.cuh"
+#include "b2b_coupling_tile.cuh"
+#include "b2b_internal.h"
+
+namespace b2b {
+
+constexpr int CMV_THREADS = 256;
+constexpr int CMV_SP = 33;  // pitch of the one-sub-tile scratch block
+
+struct CmvParams {
+  const float* x;
+  const float* ybar;
+  const float* ljbar;
+  float* xbar;
+  const float *W1, *c1, *W2, *c2;
+  const int *idx1, *idx2;
+  float* part;  // [grid][slice], NULL: no parameter cotangents
+  long long N, ldx, ldyb, ldxb, slice;
+  int D, n1, n2, H, act, nsub;
+  float slope;
+};
+
+// acc[q] += Σ_k A[q·nk + k] · B[k·ld + lane] for the `rows` (<= 8) rows at A, each contiguous in k, k increasing
+__device__ __forceinline__ void cmv_gemm_t(const float* B, int ld, int nk, const float* __restrict__ A, int rows, bool vec,
+                                           float (&acc)[8]) {
+  const int lane = threadIdx.x & 31;
+  if (vec && rows >= 8) {
+    for (int k = 0; k < nk; k += 4) {
+      const float b0 = B[k * ld + lane], b1 = B[(k + 1) * ld + lane], b2 = B[(k + 2) * ld + lane], b3 = B[(k + 3) * ld + lane];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 a = __ldg(reinterpret_cast<const float4*>(A + (size_t)q * nk + k));
+        acc[q] = fmaf(a.w, b3, fmaf(a.z, b2, fmaf(a.y, b1, fmaf(a.x, b0, acc[q]))));
+      }
+    }
+  } else {
+    for (int k = 0; k < nk; ++k) {
+      const float b = B[k * ld + lane];
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        if (q < rows) acc[q] = fmaf(__ldg(A + (size_t)q * nk + k), b, acc[q]);
+    }
+  }
+}
+
+// out[i + RA·j] += Σ_c A[i][c]·B[j][c] over the group's `cols` columns (A: RA rows, B: RB rows, pitch ld), and
+// outc[i] += Σ_c A[i][c].  16 x 16 threads, a 4 x 4 block each, swept over 64 x 64 blocks of the matrix.
+__device__ __forceinline__ void cmv_outer(const float* A, int RA, const float* B, int RB, int ld, int cols, float* out,
+                                          float* outc) {
+  const int ti = threadIdx.x & 15, tj = threadIdx.x >> 4;
+  for (int bi = 0; bi < RA; bi += 64)
+    for (int bj = 0; bj < RB; bj += 64) {
+      float acc[4][4] = {};
+      const float *pa[4], *pb[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {  // rows past the matrix read its last row; their sums are dropped below
+        pa[q] = A + (size_t)min(bi + ti + 16 * q, RA - 1) * ld;
+        pb[q] = B + (size_t)min(bj + tj + 16 * q, RB - 1) * ld;
+      }
+      for (int c = 0; c < cols; ++c) {
+        float a[4], b[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          a[q] = pa[q][c];
+          b[q] = pb[q][c];
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+#pragma unroll
+          for (int p = 0; p < 4; ++p) acc[q][p] = fmaf(a[q], b[p], acc[q][p]);
+      }
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const int i = bi + ti + 16 * q, j = bj + tj + 16 * p;
+          if (i < RA && j < RB) out[(size_t)i + (size_t)RA * j] += acc[q][p];
+        }
+    }
+  for (int i = threadIdx.x; i < RA; i += CMV_THREADS) {
+    float s = 0.f;
+    for (int c = 0; c < cols; ++c) s += A[(size_t)i * ld + c];
+    outc[i] += s;
+  }
+}
+
+template <bool INV>
+__global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const __grid_constant__ CmvParams P) {
+  extern __shared__ float cmv_sm[];
+  const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H, TG = 32 * P.nsub, FP = TG + 1, nmax = max(n1, n2);
+  float* X2 = cmv_sm;                   // [n2][FP]   x₂
+  float* ST = X2 + (size_t)n2 * FP;     // [2n1][FP]  ȳ₁, then s̄ | t̄
+  float* Hs = ST + (size_t)2 * n1 * FP; // [H][FP]    h
+  float* Vb = Hs + (size_t)H * FP;      // [H][FP]    σ′(v), then v̄
+  float* Sc = Vb + (size_t)H * FP;      // [max(n1, n2)][33]  one sub-tile: x₁ -> x̄₁, then W₁ᵀ v̄
+  int* sidx1 = reinterpret_cast<int*>(Sc + (size_t)nmax * CMV_SP);  // [n1]
+  int* sidx2 = sidx1 + n1;                                          // [n2]
+  unsigned char* kind = reinterpret_cast<unsigned char*>(sidx2 + n2);  // [D]: 0 = a pass-through row
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float* slice = P.part ? P.part + (size_t)blockIdx.x * P.slice : nullptr;
+  float* sW1 = slice;
+  float* sc1 = sW1 + (size_t)H * n2;
+  float* sW2 = sc1 + H;
+  float* sc2 = sW2 + (size_t)2 * n1 * H;
+
+  for (int r = tid; r < D; r += CMV_THREADS) kind[r] = 0;
+  if (slice)
+    for (long long e = tid; e < P.slice; e += CMV_THREADS) slice[e] = 0.f;
+  __syncthreads();
+  for (int i = tid; i < n1; i += CMV_THREADS) kind[sidx1[i] = P.idx1[i]] = 1;
+  for (int k = tid; k < n2; k += CMV_THREADS) kind[sidx2[k] = P.idx2[k]] = 2;
+  const bool vec1 = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
+  const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
+  const bool vec1t = ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
+  const bool vec2t = ((n1 & 1) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
+  auto same = [](int k) { return k; };
+
+  const long long groups = (P.N + TG - 1) / TG;
+  for (long long g = blockIdx.x; g < groups; g += gridDim.x) {
+    const long long n0 = g * TG;
+    const int gcols = (int)min((long long)TG, P.N - n0);
+    for (int co = 0; co < gcols; co += 32) {
+      __syncthreads();  // index tables visible; Sc and the factors of the previous group are no longer read
+      // ---- stage x₂, x₁, ȳ₁ of the sub-tile; x̄₃ = ȳ₃ goes straight out --------------------------------------------
+      for (int c = warp; c < 32; c += CMV_THREADS / 32) {
+        const long long col = n0 + co + c;
+        const bool ok = col < P.N;
+        const float* xc = P.x + col * P.ldx;
+        const float* yb = P.ybar ? P.ybar + col * P.ldyb : nullptr;
+        for (int k = lane; k < n2; k += 32) X2[k * FP + co + c] = ok ? __ldcs(xc + sidx2[k]) : 0.f;
+        for (int k = lane; k < n1; k += 32) {
+          Sc[k * CMV_SP + c] = ok ? __ldcs(xc + sidx1[k]) : 0.f;
+          ST[k * FP + co + c] = ok && yb ? __ldcs(yb + sidx1[k]) : 0.f;
+        }
+        if (ok && n1 + n2 < D)
+          for (int r = lane; r < D; r += 32)
+            if (!kind[r]) __stcs(P.xbar + col * P.ldxb + r, yb ? __ldcs(yb + r) : 0.f);
+      }
+      __syncthreads();
+      // ---- h = σ(W₁x₂ + c₁) and σ′ -------------------------------------------------------------------------------
+      for (int jb = 8 * warp; jb < H; jb += 8 * (CMV_THREADS / 32)) {
+        float va[4][1] = {}, vb[4][1] = {};
+        coupling_gemm_block<1>(X2 + co, FP, same, n2, P.W1 + jb, P.W1 + jb + 4, H, H - jb, H - jb - 4, vec1, va, vb);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const int m = jb + q;
+          if (m < H)
+            mlp_act(P.act, P.slope, (q < 4 ? va[q & 3][0] : vb[q & 3][0]) + (P.c1 ? __ldg(P.c1 + m) : 0.f),
+                    Hs[m * FP + co + lane], Vb[m * FP + co + lane]);
+        }
+      }
+      __syncthreads();
+      // ---- [s; t] = W₂h + c₂, then x̄₁, s̄, t̄ of the affine law ---------------------------------------------------
+      const long long mycol = n0 + co + lane;
+      const float lb = P.ljbar && mycol < P.N ? P.ljbar[mycol] : 0.f;
+      for (int jb = 4 * warp; jb < n1; jb += 4 * (CMV_THREADS / 32)) {
+        float sv[4][1] = {}, tv[4][1] = {};
+        coupling_gemm_block<1>(Hs + co, FP, same, H, P.W2 + jb, P.W2 + n1 + jb, 2 * n1, n1 - jb, n1 - jb, vec2, sv, tv);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int j = jb + q;
+          if (j < n1) {
+            const float s_ = sv[q][0] + (P.c2 ? __ldg(P.c2 + j) : 0.f), t_ = tv[q][0] + (P.c2 ? __ldg(P.c2 + n1 + j) : 0.f);
+            const float in1 = Sc[j * CMV_SP + lane], cb1 = ST[j * FP + co + lane];
+            float sbar, tbar, out1;
+            if (!INV) {
+              const float e = expf(s_);
+              out1 = e * cb1;                 // x̄₁ = e^s ȳ₁
+              sbar = fmaf(cb1 * e, in1, lb);  // ȳ₁ e^s x₁ + l̄
+              tbar = cb1;
+            } else {
+              const float em = expf(-s_);
+              const float x1 = (in1 - t_) * em;  // the recovered x₁
+              out1 = em * cb1;                   // ȳ₁ = e^−s x̄₁
+              sbar = -fmaf(x1, cb1, lb);         // −x₁ x̄₁ − l̄
+              tbar = -out1;
+            }
+            Sc[j * CMV_SP + lane] = out1;
+            ST[j * FP + co + lane] = sbar;
+            ST[(n1 + j) * FP + co + lane] = tbar;
+          }
+        }
+      }
+      __syncthreads();
+      for (int c = warp; c < 32; c += CMV_THREADS / 32) {
+        const long long col = n0 + co + c;
+        if (col < P.N)
+          for (int k = lane; k < n1; k += 32) __stcs(P.xbar + col * P.ldxb + sidx1[k], Sc[k * CMV_SP + c]);
+      }
+      // ---- v̄ = (W₂ᵀ[s̄; t̄]) ⊙ σ′ ---------------------------------------------------------------------------------
+      for (int mb = 8 * warp; mb < H; mb += 8 * (CMV_THREADS / 32)) {
+        float acc[8] = {};
+        cmv_gemm_t(ST + co, FP, 2 * n1, P.W2 + (size_t)mb * 2 * n1, H - mb, vec2t, acc);
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+          if (mb + q < H) Vb[(mb + q) * FP + co + lane] *= acc[q];
+      }
+      __syncthreads();
+      // ---- x̄₂ = ȳ₂ + W₁ᵀ v̄ ---------------------------------------------------------------------------------------
+      for (int kb = 8 * warp; kb < n2; kb += 8 * (CMV_THREADS / 32)) {
+        float acc[8] = {};
+        cmv_gemm_t(Vb + co, FP, H, P.W1 + (size_t)kb * H, n2 - kb, vec1t, acc);
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+          if (kb + q < n2) Sc[(kb + q) * CMV_SP + lane] = acc[q];
+      }
+      __syncthreads();
+      for (int c = warp; c < 32; c += CMV_THREADS / 32) {
+        const long long col = n0 + co + c;
+        if (col < P.N)
+          for (int k = lane; k < n2; k += 32) {
+            const float yb = P.ybar ? __ldcs(P.ybar + col * P.ldyb + sidx2[k]) : 0.f;
+            __stcs(P.xbar + col * P.ldxb + sidx2[k], yb + Sc[k * CMV_SP + c]);
+          }
+      }
+    }
+    if (slice) {  // the group's parameter sums, added to the CTA's slice
+      __syncthreads();
+      cmv_outer(Vb, H, X2, n2, FP, gcols, sW1, sc1);
+      cmv_outer(ST, 2 * n1, Hs, H, FP, gcols, sW2, sc2);
+    }
+  }
+}
+
+// the `nparts` slices summed in order; element e of the slice layout [W̄₁ | c̄₁ | W̄₂ | c̄₂] goes to its array (NULL: dropped)
+__global__ void __launch_bounds__(256) coupling_mlp_vjp_reduce_kernel(const float* __restrict__ part, int nparts, long long slice,
+                                                                      long long l0, long long l1, long long l2, long long l3,
+                                                                      float* __restrict__ o0, float* __restrict__ o1,
+                                                                      float* __restrict__ o2, float* __restrict__ o3) {
+  long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= l0 + l1 + l2 + l3) return;
+  double t = 0.0;
+  for (int g = 0; g < nparts; ++g) t += (double)part[(size_t)g * slice + e];
+  float* o = o0;
+  if (e >= l0) { e -= l0; o = o1;
+    if (e >= l1) { e -= l1; o = o2;
+      if (e >= l2) { e -= l2; o = o3; } } }
+  if (o) o[e] = (float)t;
+}
+
+static long long cmv_param_floats(const b2b_layer_desc& d) {
+  return (long long)d.n2 * (d.n1 + 1) + (long long)2 * d.n0 * (d.n2 + 1);
+}
+static long long cmv_slice_floats(const b2b_layer_desc& d) { return (cmv_param_floats(d) + 63) & ~63LL; }
+
+static size_t cmv_smem_bytes(const b2b_layer_desc& d, int D, int nsub) {
+  const size_t f = (size_t)(d.n1 + 2 * d.n0 + 2 * d.n2) * (32 * nsub + 1) + (size_t)(d.n0 > d.n1 ? d.n0 : d.n1) * CMV_SP;
+  return (f * sizeof(float) + (size_t)(d.n0 + d.n1) * sizeof(int) + D + 15) & ~(size_t)15;
+}
+
+// sub-tiles per group: the most whose factors fit the 227 KB a CTA may use
+static int cmv_nsub(const b2b_layer_desc& d, int D) {
+  for (int s = 4; s > 1; s >>= 1)
+    if (cmv_smem_bytes(d, D, s) <= 227 * 1024) return s;
+  return 1;
+}
+
+static int cmv_grid(const b2b_layer_desc& d, int D, long long N) {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sms <= 0) sms = 132;
+  long long g = sms;
+  const long long groups = (N + 32 * cmv_nsub(d, D) - 1) / (32 * cmv_nsub(d, D));
+  if (g > groups) g = groups;
+  const long long cap = (256LL << 20) / (cmv_slice_floats(d) * (long long)sizeof(float));
+  if (g > cap) g = cap;
+  return g < 1 ? 1 : (int)g;
+}
+
+}  // namespace b2b
+
+size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
+  using namespace b2b;
+  if (!b2b_coupling_mlp_fits(d, D)) return 0;
+  return (size_t)cmv_grid(d, D, N) * (size_t)cmv_slice_floats(d) * sizeof(float) + 256;
+}
+
+int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
+                                const float* ljbar, float* xbar, long long ldxb, float* const bars[4], int D, long long N,
+                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+  using namespace b2b;
+  *launches = 0;
+  if (!b2b_coupling_mlp_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (N <= 0) return B2B_OK;
+  const bool want = bars[0] || bars[1] || bars[2] || bars[3];
+  if (want && (!workspace || workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
+  char* wsb = static_cast<char*>(workspace);
+  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  CmvParams P;
+  P.x = x;
+  P.ybar = ybar;
+  P.ljbar = ljbar;
+  P.xbar = xbar;
+  P.W1 = d.p0;
+  P.c1 = d.p1;
+  P.W2 = d.p2;
+  P.c2 = d.p3;
+  P.idx1 = d.i0;
+  P.idx2 = d.i1;
+  P.part = want ? reinterpret_cast<float*>(wsb) : nullptr;
+  P.N = N;
+  P.ldx = ldx;
+  P.ldyb = ldyb;
+  P.ldxb = ldxb;
+  P.slice = cmv_slice_floats(d);
+  P.D = D;
+  P.n1 = d.n0;
+  P.n2 = d.n1;
+  P.H = d.n2;
+  P.act = d.n3;
+  P.nsub = cmv_nsub(d, D);
+  P.slope = d.f0;
+  const int grid = cmv_grid(d, D, N);
+  const size_t smem = cmv_smem_bytes(d, D, P.nsub);
+  void (*kernel)(const CmvParams) = d.inverse ? coupling_mlp_vjp_kernel<true> : coupling_mlp_vjp_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return (int)e;
+  kernel<<<grid, CMV_THREADS, smem, stream>>>(P);
+  if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  *launches = 1;
+  if (want) {
+    const long long l0 = (long long)d.n2 * d.n1, l1 = d.n2, l2 = (long long)2 * d.n0 * d.n2, l3 = 2 * d.n0;
+    coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l0 + l1 + l2 + l3 + 255) / 256), 256, 0, stream>>>(
+        P.part, grid, P.slice, l0, l1, l2, l3, bars[0], bars[1], bars[2], bars[3]);
+    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    *launches = 2;
+  }
+  return B2B_OK;
+}

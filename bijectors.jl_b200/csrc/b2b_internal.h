@@ -160,11 +160,23 @@ size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long 
 int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
                                 const float* ljbar, float* xbar, long long ldxb, float* Wbar, float* cbar, int D, long long N,
                                 void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
+// neural-network coupling (b2b_coupling_mlp.cu, b2b_coupling_mlp_vjp.cu): whether the layer is within the envelope of
+// include/b2b.h
+bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D);
+int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
+                            long long ldx, long long ldy, int accumulate, cudaStream_t stream);
+// reverse mode: x̄ always; bars[i] (NULL: not wanted) receives the cotangent of p<i> (W₁ c₁ W₂ c₂).  With any of them
+// b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope, bounded independently of N) and two launches,
+// else one launch and no workspace.
+size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
+int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
+                                const float* ljbar, float* xbar, long long ldxb, float* const bars[4], int D, long long N,
+                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
-// COUPLING_RQS and SCALE_MATRIX).
+// COUPLING_RQS, SCALE_MATRIX and COUPLING_MLP).
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);
@@ -175,10 +187,10 @@ void b2b_set_last_launch_count(int n);
 // own launch and reverse-mode code in b2b_chain_run_f32 / b2b_chain_vjp_f32.
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
-enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL };
+enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };
 // Reverse-mode segment class of b2b_chain_vjp_f32 (B2B_VC_EW: runs of STACKED_EW / PERMUTE, with MVNORMAL_DIAG).
 enum B2BVjpClass {
-  B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE
+  B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE, B2B_VC_MLP
 };
 // descriptor pointer fields as bits
 enum { B2B_F_P0 = 1, B2B_F_P1 = 2, B2B_F_P2 = 4, B2B_F_P3 = 8, B2B_F_I0 = 16, B2B_F_I1 = 32 };
@@ -211,6 +223,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_MVNORMAL_TRIL,   B2B_F_P1,                    true,  B2B_LC_TRIL,     B2B_VC_TRIL,     2, B2B_F_P0, true},
       {B2B_COUPLING_RQS,    B2B_F_P0 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE,   2, B2B_F_P1, false},
       {B2B_SCALE_MATRIX,    B2B_F_P0,                    false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        false},
+      {B2B_COUPLING_MLP,    B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P1 | B2B_F_P3, false},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -249,6 +262,9 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
       ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && (d.i0 || d.n2 >= 0) && (d.i1 || d.n3 >= 0);
       break;
     case B2B_COUPLING_RQS: ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && d.f0 > 0; break;
+    case B2B_COUPLING_MLP:
+      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && (d.n3 == B2B_ACT_TANH || d.n3 == B2B_ACT_LEAKY_RELU);
+      break;
     default: break;
   }
   return ok ? B2B_OK : B2B_EINVAL;
@@ -265,6 +281,10 @@ size_t b2b_slot_len(const Desc& d, int i, int D) {
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
     case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
     case B2B_SCALE_MATRIX: return (size_t)D * D;
+    case B2B_COUPLING_MLP: {  // W₁ (H x n2), c₁ (H), W₂ (2n1 x H), c₂ (2n1)
+      const size_t len[4] = {(size_t)d.n2 * d.n1, (size_t)d.n2, (size_t)2 * d.n0 * d.n2, (size_t)2 * d.n0};
+      return len[i];
+    }
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }

@@ -40,6 +40,8 @@ end
 const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNORMAL_DIAG, MVNORMAL_TRIL = Int32.(1:9)
 const COUPLING_RQS = Int32(11)  # 10 is not a layer kind (include/b2b.h)
 const SCALE_MATRIX = Int32(12)
+const COUPLING_MLP = Int32(13)
+const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
 const NULLI = CuPtr{Int32}(0)
@@ -116,8 +118,33 @@ function desc(cl::Coupling{<:SplineConditioner{<:CuMatrix{Float32}}}, inv::Bool)
     LayerDesc(COUPLING_RQS, inv, length(dm.idx1), length(dm.idx2), θ.K, 0, θ.B, 0f0,
               pointer(θ.W), θ.c === nothing ? NULLF : pointer(θ.c), NULLF, NULLF, pointer(dm.idx1), pointer(dm.idx2))
 end
+# The neural-network coupling law of RealNVP: θ(x₂) = Shift(t) ∘ Scale(exp.(s)), [s; t] = W₂*σ.(W₁*x₂ .+ c₁) .+ c₂ with
+# σ = tanh or LeakyReLU(slope) (x >= 0 ? x : slope*x, leaky_relu.jl:18-29); a callable, so the same object also runs on the
+# CPU reference path.  Float32, n1, n2 <= 128, H <= 256, D <= 1024 on the device; c₁ / c₂ === nothing is a zero shift.
+struct MLPConditioner{M<:AbstractMatrix,V1,V2}
+    W1::M   # (H × n2)
+    c1::V1  # H, or nothing
+    W2::M   # (2n1 × H)
+    c2::V2  # 2n1, or nothing
+    act::Int32      # ACT_TANH or ACT_LEAKY_RELU
+    slope::Float32
+end
+function (θ::MLPConditioner)(x₂)
+    v = θ.c1 === nothing ? θ.W1 * x₂ : θ.W1 * x₂ .+ θ.c1
+    h = θ.act == ACT_TANH ? tanh.(v) : ifelse.(v .>= 0, v, θ.slope .* v)
+    st = θ.c2 === nothing ? θ.W2 * h : θ.W2 * h .+ θ.c2
+    n = length(st) ÷ 2
+    Shift(st[(n + 1):end]) ∘ Scale(exp.(st[1:n]))
+end
+function desc(cl::Coupling{<:MLPConditioner{<:CuMatrix{Float32}}}, inv::Bool)
+    dm = get!(() -> DeviceMask(cl.mask), MASKS, cl.mask)
+    θ = cl.θ
+    ptr(c) = c === nothing ? NULLF : pointer(c)
+    LayerDesc(COUPLING_MLP, inv, length(dm.idx1), length(dm.idx2), size(θ.W1, 1), θ.act, θ.slope, 0f0,
+              pointer(θ.W1), ptr(θ.c1), pointer(θ.W2), ptr(θ.c2), pointer(dm.idx1), pointer(dm.idx2))
+end
 desc(cl::Coupling, ::Bool) =
-    error("Coupling: only AffineConditioner and SplineConditioner laws run on the device path (no CPU fallback)")
+    error("Coupling: only AffineConditioner, SplineConditioner and MLPConditioner laws run on the device path (no CPU fallback)")
 
 # Permute(A): y[dst[i]] = x[i] with dst = the row of the single 1 in column i (permute.jl:90-100,152)
 const PERMS = IdDict{Any,CuVector{Int32}}()
@@ -171,6 +198,7 @@ descs(f, inv::Bool) = inv ? [desc(b, true) for b in reverse(flatten(f))] : [desc
 const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVector{Float32}},
                           RationalQuadraticSpline{<:CuMatrix{Float32}},InvertibleBatchNorm{<:CuVector{Float32}},
                           Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},
+                          Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},
                           Scale{<:CuMatrix{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
@@ -380,6 +408,8 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
     d.kind == COUPLING_RQS && return (z((3d.n2 - 1) * d.n0, d.n1), d.p1 == NULLF ? nothing : z((3d.n2 - 1) * d.n0))
     d.kind == SCALE_MATRIX && return (z(D, D),)
+    d.kind == COUPLING_MLP && return (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(2d.n0, d.n2),
+                                      d.p3 == NULLF ? nothing : z(2d.n0))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

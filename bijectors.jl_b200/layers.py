@@ -256,6 +256,9 @@ class AffineConditioner:
         new.W, new.c = self.W.to(device), self.c.to(device)
         return new
 
+    def _tensors(self):
+        return (self.W, self.c)
+
 
 class SplineConditioner:
     """The neural-spline coupling law (Durkan et al. 2019) θ(x₂) = RationalQuadraticSpline(reshape(v[1:n1K], n1, K),
@@ -293,25 +296,75 @@ class SplineConditioner:
         new.c = None if self.c is None else self.c.to(device)
         return new
 
+    def _tensors(self):
+        return (self.W, self.c)
+
+
+class MLPConditioner:
+    """The neural-network coupling law of RealNVP: θ(x₂) = Shift(t) ∘ Scale(exp.(s)) with
+    [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂, one hidden layer of width H and σ = tanh or LeakyReLU(slope) (slope 0 is ReLU;
+    v >= 0 ? v : slope·v, leaky_relu.jl:18-29).  W1 is (H × n2) and W2 (2·n1 × H) in the reference's index order, rows
+    1..n1 of W2 giving s and the rest t as for :class:`AffineConditioner`; c1 (H) and c2 (2·n1) may be None (no shift,
+    the descriptor's pointer is NULL).  Float32 only.  Runs as B2B_COUPLING_MLP: n1, n2 <= 128, H <= 256, D <= 1024."""
+
+    _ACT = {"tanh": _lib.ACT_TANH, "leaky_relu": _lib.ACT_LEAKY_RELU}
+
+    def __init__(self, W1, c1, W2, c2, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+        if dtype != torch.float32:
+            raise TypeError("MLPConditioner: the neural-network coupling layer runs in Float32 only")
+        if activation not in self._ACT:
+            raise ValueError(f"MLPConditioner: activation must be one of {sorted(self._ACT)}, got {activation!r}")
+
+        def host(v):
+            return np.asarray(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=np.float32)
+
+        W1n, W2n = host(W1), host(W2)
+        if W1n.ndim != 2 or W1n.shape[0] == 0:
+            raise ValueError(f"W1 must be (H, n2), got {W1n.shape}")
+        if W2n.ndim != 2 or W2n.shape[0] == 0 or W2n.shape[0] % 2 or W2n.shape[1] != W1n.shape[0]:
+            raise ValueError(f"W2 must be (2*n1, H) with H = {W1n.shape[0]}, got {W2n.shape}")
+        self.activation, self.slope = activation, float(slope)
+        self.H, self.n2, self.n1 = W1n.shape[0], W1n.shape[1], W2n.shape[0] // 2
+        self.W1 = _dev_f32(np.ascontiguousarray(W1n.T), device)  # column-major (H × n2)
+        self.W2 = _dev_f32(np.ascontiguousarray(W2n.T), device)  # column-major (2n1 × H)
+        self.c1 = self.c2 = None
+        for name, c, n in (("c1", c1, self.H), ("c2", c2, 2 * self.n1)):
+            if c is not None:
+                cn = host(c).reshape(-1)
+                if cn.shape != (n,):
+                    raise ValueError(f"{name} must have {n} entries, got {cn.shape}")
+                setattr(self, name, _dev_f32(cn, device))
+
+    def to(self, device):
+        new = object.__new__(MLPConditioner)
+        new.__dict__.update(self.__dict__)
+        for k in ("W1", "c1", "W2", "c2"):
+            t = getattr(self, k)
+            setattr(new, k, None if t is None else t.to(device))
+        return new
+
+    def _tensors(self):
+        return (self.W1, self.c1, self.W2, self.c2)
+
 
 class Coupling(_ParamLayer):
     """Coupling(θ, mask) (coupling.jl:178-181).  θ is an arbitrary closure in the reference; the device
-    path supports the recognised :class:`AffineConditioner` and :class:`SplineConditioner` and raises for anything else
-    (no CPU fallback)."""
+    path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner` and :class:`MLPConditioner` and
+    raises for anything else (no CPU fallback)."""
 
     _fields = ()
 
     def __init__(self, θ, mask, device="cuda"):
         if isinstance(mask, int):  # Coupling(θ, n): first n÷2 rows transformed (:183-186)
             mask = PartitionMask(mask, range(1, mask // 2 + 1))
-        if not isinstance(θ, (AffineConditioner, SplineConditioner)):
-            raise B2BError(_lib.B2B_EUNSUPPORTED,
-                           "Coupling: only AffineConditioner and SplineConditioner laws run on the device path")
+        if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner)):
+            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner and MLPConditioner "
+                                                  "laws run on the device path")
         if θ.n1 != len(mask.indices_1) or θ.n2 != len(mask.indices_2):
             raise ValueError("conditioner shape does not match the PartitionMask")
         self.θ, self.mask = θ, mask
-        self._idx1 = _dev_i32(np.asarray(mask.indices_1) - 1, θ.W.device)
-        self._idx2 = _dev_i32(np.asarray(mask.indices_2) - 1, θ.W.device)
+        self._idx1 = _dev_i32(np.asarray(mask.indices_1) - 1, self.device)
+        self._idx2 = _dev_i32(np.asarray(mask.indices_2) - 1, self.device)
 
         def first_row(idx):  # 0-based first row when the list is a contiguous increasing range, else -1
             a = np.asarray(idx)
@@ -321,19 +374,24 @@ class Coupling(_ParamLayer):
 
     @property
     def device(self):
-        return self.θ.W.device
+        return self.θ._tensors()[0].device
 
     def to(self, device):
-        """fmap-style movement: the conditioner (W, c) AND the index lists follow."""
+        """fmap-style movement: the conditioner's tensors AND the index lists follow."""
         return Coupling(self.θ.to(device), self.mask)
 
     def _keepalive(self):
-        return (self.θ.W, self.θ.c, self._idx1, self._idx2)
+        return self.θ._tensors() + (self._idx1, self._idx2)
 
     def _descs(self, inverse, D, dtype=torch.float32):
         if D != self.mask.n:
             raise ValueError(f"DimensionMismatch: Coupling mask has {self.mask.n} dims, input has {D}")
-        _check_dtype(self.θ.W, dtype, "Coupling")
+        _check_dtype(self.θ._tensors()[0], dtype, "Coupling")
+        if isinstance(self.θ, MLPConditioner):
+            θ = self.θ
+            return [_desc(_lib.COUPLING_MLP, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
+                          p3=θ.c2 if θ.c2 is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
+                          n3=θ._ACT[θ.activation], f0=θ.slope)]
         if isinstance(self.θ, SplineConditioner):
             return [_desc(_lib.COUPLING_RQS, inverse, p0=self.θ.W, p1=self.θ.c if self.θ.c is not None else 0,
                           i0=self._idx1, i1=self._idx2, n0=self.θ.n1, n1=self.θ.n2, n2=self.θ.K, n3=0, f0=self.θ.B)]
@@ -343,9 +401,12 @@ class Coupling(_ParamLayer):
     def __eq__(self, o):
         if not (isinstance(o, Coupling) and type(self.θ) is type(o.θ) and self.mask == o.mask):
             return False
-        if isinstance(self.θ, SplineConditioner) and ((self.θ.K, self.θ.B) != (o.θ.K, o.θ.B) or (self.θ.c is None) != (o.θ.c is None)):
+        if isinstance(self.θ, SplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
             return False
-        return torch.equal(self.θ.W, o.θ.W) and (self.θ.c is None or torch.equal(self.θ.c, o.θ.c))
+        if isinstance(self.θ, MLPConditioner) and (self.θ.activation, self.θ.slope) != (o.θ.activation, o.θ.slope):
+            return False
+        return all((a is None) == (b is None) and (a is None or torch.equal(a, b))
+                   for a, b in zip(self.θ._tensors(), o.θ._tensors()))
 
     __hash__ = object.__hash__
 
