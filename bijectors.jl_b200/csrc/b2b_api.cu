@@ -40,6 +40,13 @@ extern "C" const char* b2b_status_string(int status) {
 extern "C" int b2b_last_launch_count(void) { return g_last_launches; }
 void b2b_set_last_launch_count(int n) { g_last_launches = n; }
 
+int b2b_sm_count() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? sms : 132;
+}
+
 extern "C" int b2b_set_kernel_variant(int variant) {
   // low decimal digit: fused chain kernel variant; tens digit: coupling variant (10 = force fp32 CUDA cores)
   const int chain = variant % 10, cpl = (variant / 10) % 10, nofold = variant / 100;
@@ -672,17 +679,10 @@ extern "C" int b2b_planar_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
     if (rc != B2B_OK) return rc;
     if ((layers[l].inverse != 0) != (layers[0].inverse != 0)) return B2B_EUNSUPPORTED;  // one direction per call
   }
-  B2BChainParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = x;
-  p.N = N;
-  p.ldx = ldx;
-  p.D = D;
-  p.L = L;
-  for (int l = 0; l < L; ++l) p.layers[l] = layers[l];
+  float* const bars[4 * 8] = {wbar, ubar, bbar};
   int launches = 0;
-  const int rc = b2b_launch_planar_chain_vjp(p, ybar, ldybar, ljbar, xbar, ldxbar, wbar, ubar, bbar, workspace,
-                                             workspace_bytes, &launches, stream);
+  const int rc = b2b_vjp_planar({layers, L, x, ldx, ybar, ldybar, ljbar, xbar, ldxbar, D, N, bars, nullptr, workspace,
+                                 workspace_bytes, &launches, stream});
   if (rc == B2B_OK) g_last_launches = launches;
   return rc;
 }
@@ -711,17 +711,10 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
     const int rc = validate_layer(layers[l], D, false);
     if (rc != B2B_OK) return rc;
   }
-  B2BChainParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = x;
-  p.N = N;
-  p.ldx = ldx;
-  p.D = D;
-  p.L = L;
-  for (int l = 0; l < L; ++l) p.layers[l] = layers[l];
+  float* const bars[4 * 8] = {alpha_bar, beta_bar, z0_bar};
   int launches = 0;
-  const int rc = b2b_launch_radial_chain_vjp(p, ybar, ldybar, ljbar, xbar, ldxbar, alpha_bar, beta_bar, z0_bar,
-                                             workspace, workspace_bytes, &launches, stream);
+  const int rc = b2b_vjp_radial({layers, L, x, ldx, ybar, ldybar, ljbar, xbar, ldxbar, D, N, bars, nullptr, workspace,
+                                 workspace_bytes, &launches, stream});
   if (rc == B2B_OK) g_last_launches = launches;
   return rc;
 }
@@ -832,25 +825,109 @@ VLayout vjp_layout(const b2b_layer_desc* layers, const std::vector<VSeg>& segs, 
 
 bool tma_ok(const float* p, long long ld) { return p && (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 4 == 0; }
 
-// One launch copying the requested cotangents of the run ls[0, n) out of the arrays its kernel wrote: slot i of layer j
-// is at base[i] + j * step[i], and bars[4j + i] (NULL: not requested) receives it.  Nothing is launched when none is.
-int copy_run_bars(const b2b_layer_desc* ls, int n, float* const* bars, const float* const base[3],
-                  const size_t step[3], int D, int* launches, cudaStream_t stream) {
-  const float* src[24];
-  float* dst[24];
-  int len[24], dlen[24], c = 0;
-  for (int j = 0; j < n; ++j)
-    for (int i = 0; i < 3; ++i)
-      if (float* d = bars[4 * j + i]) {
-        src[c] = base[i] + j * step[i];
-        dst[c] = d;
-        len[c] = dlen[c] = (int)b2b_slot_len(ls[j], i, D);
-        ++c;
+// the classes whose kernels read ȳ: a NULL ȳ is staged as zeros for them (the others take NULL as zero)
+bool vjp_needs_ybar(int vc) {
+  return vc == B2B_VC_RADIAL || vc == B2B_VC_RQS || vc == B2B_VC_COUPLING || vc == B2B_VC_BN;
+}
+
+// ȳ := zeros (ȳ == NULL) or a copy of ȳ at ld = D, in `buf`
+int stage_ybar(B2BVjpSeg& a, float* buf) {
+  const size_t F = sizeof(float);
+  const cudaError_t e =
+      a.ybar ? cudaMemcpy2DAsync(buf, (size_t)a.D * F, a.ybar, (size_t)a.ldyb * F, (size_t)a.D * F, a.N, cudaMemcpyDeviceToDevice, a.stream)
+             : cudaMemsetAsync(buf, 0, (size_t)a.D * a.N * F, a.stream);
+  if (e != cudaSuccess) return (int)e;
+  ++*a.launches;
+  a.ybar = buf;
+  a.ldyb = a.D;
+  return B2B_OK;
+}
+
+// A planar run: its kernels read x and ȳ and write x̄ through TMA, at D in {32, 64, 128}.  At another D the run is
+// embedded in the next of them, Dk rows (pad[0..2]; w and u padded with zeros in scratch, after the kernel's w̄, ū, b̄
+// arrays).  Otherwise an operand TMA cannot address is staged: x into `xst`, ȳ into `yst`, x̄ through `xbst`.
+int vjp_planar_run(B2BVjpSeg a, int Dk, float* const pad[3], float* xst, float* yst, float* xbst) {
+  const int n = a.n, D = a.D;
+  const long long N = a.N;
+  const size_t F = sizeof(float);
+  const b2b_layer_desc* const layers = a.layers;
+  float* const* const bars = a.bars;
+  float* const scratch = a.scratch;
+  float* const xbar = a.xbar;
+  const long long ldxb = a.ldxb;
+  cudaError_t e;
+  int rc;
+#define B2B_VJP_CUDA(call)                          \
+  do {                                              \
+    if ((e = (call)) != cudaSuccess) return (int)e; \
+    ++*a.launches;                                  \
+  } while (0)
+  const size_t r64 = ((size_t)n * Dk + 63) & ~(size_t)63;
+  b2b_layer_desc lp[8];
+  float* kbars[4 * 8] = {};
+  if (Dk != D) {
+    // w, u padded with zeros give the same map on the first D rows (wᵀz, wᵀu, ‖w‖² and those rows of û are unchanged)
+    // and leave the zero rows of x at zero.  The kernel writes its w̄, ū, b̄ arrays at Dk; the requested rows go out below.
+    float* wp = scratch + 2 * r64 + 64;
+    float* up = wp + r64;
+    const float* src[16];
+    float* dst[16];
+    int len[16], dlen[16];
+    for (int j = 0; j < n; ++j) {
+      lp[j] = a.layers[j];
+      src[2 * j] = a.layers[j].p0;
+      dst[2 * j] = wp + (size_t)j * Dk;
+      src[2 * j + 1] = a.layers[j].p1;
+      dst[2 * j + 1] = up + (size_t)j * Dk;
+      len[2 * j] = len[2 * j + 1] = D;
+      dlen[2 * j] = dlen[2 * j + 1] = Dk;
+      lp[j].p0 = dst[2 * j];
+      lp[j].p1 = dst[2 * j + 1];
+    }
+    if ((rc = b2b_launch_copy_list(2 * n, src, dst, len, dlen, a.stream)) != B2B_OK) return rc;
+    ++*a.launches;
+    const size_t pitch = (size_t)Dk * F, zrows = (size_t)(Dk - D) * F;
+    B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[0], pitch, a.x, (size_t)a.ldx * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, a.stream));
+    B2B_VJP_CUDA(cudaMemset2DAsync(pad[0] + D, pitch, 0, zrows, N, a.stream));
+    if (a.ybar) {
+      B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[1], pitch, a.ybar, (size_t)a.ldyb * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, a.stream));
+      B2B_VJP_CUDA(cudaMemset2DAsync(pad[1] + D, pitch, 0, zrows, N, a.stream));
+    } else {
+      B2B_VJP_CUDA(cudaMemsetAsync(pad[1], 0, (size_t)Dk * N * F, a.stream));
+    }
+    for (int k = 0; k < 4 * n; ++k)
+      if (bars[k]) {
+        kbars[0] = scratch;
+        kbars[1] = scratch + r64;
+        kbars[2] = scratch + 2 * r64;
       }
-  if (!c) return B2B_OK;
-  const int rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream);
-  if (rc == B2B_OK) ++*launches;
-  return rc;
+    a.layers = lp;
+    a.x = pad[0];
+    a.ybar = pad[1];
+    a.xbar = pad[2];
+    a.ldx = a.ldyb = a.ldxb = a.D = Dk;
+    a.bars = kbars;
+    a.scratch = nullptr;
+  } else {
+    if (!tma_ok(a.x, a.ldx)) {
+      B2B_VJP_CUDA(cudaMemcpy2DAsync(xst, (size_t)D * F, a.x, (size_t)a.ldx * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, a.stream));
+      a.x = xst;
+      a.ldx = D;
+    }
+    if (!tma_ok(a.ybar, a.ldyb) && (rc = stage_ybar(a, yst)) != B2B_OK) return rc;
+    if (!tma_ok(a.xbar, a.ldxb)) {
+      a.xbar = xbst;
+      a.ldxb = D;
+    }
+  }
+  if ((rc = b2b_vjp_planar(a)) != B2B_OK) return rc;
+  if (a.xbar != xbar)
+    B2B_VJP_CUDA(cudaMemcpy2DAsync(xbar, (size_t)ldxb * F, a.xbar, (size_t)a.ldxb * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, a.stream));
+#undef B2B_VJP_CUDA
+  if (Dk == D) return B2B_OK;
+  const float* const base[3] = {scratch, scratch + r64, scratch + 2 * r64};
+  const size_t step[3] = {(size_t)Dk, (size_t)Dk, 1};
+  return b2b_copy_run_bars(layers, n, bars, base, step, D, a.launches, a.stream);
 }
 
 }  // namespace
@@ -884,14 +961,12 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
   if (rc != B2B_OK || N == 0) return rc;
   float* const none[4 * B2B_MAX_CHAIN] = {};
   float* const* bars = param_bars ? param_bars : none;
-  auto bar = [&](int l, int i) { return bars[4 * l + i]; };
   int launches = 0;
   const VLayout lay = vjp_layout(layers, segs, D, N);
   if (!workspace || workspace_bytes < lay.total) return B2B_EWORKSPACE;
   const int S = (int)segs.size();
   const size_t m = mat_bytes(D, N);
-  char* ws = static_cast<char*>(workspace);
-  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
+  char* ws = b2b_align256(workspace);
   std::vector<float*> ckpt(S, nullptr);
   for (int s = 1; s < S; ++s) ckpt[s] = reinterpret_cast<float*>(ws + (size_t)(s - 1) * m);
   ws += lay.ckpt;
@@ -907,14 +982,6 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
   ws += lay.param;
   void* kws = ws;
   const size_t kws_bytes = lay.kern;
-  const size_t F = sizeof(float);
-  cudaError_t e;
-#define B2B_VJP_CUDA(call)                    \
-  do {                                        \
-    if ((e = (call)) != cudaSuccess) return (int)e; \
-    ++launches;                               \
-  } while (0)
-
   // 1. forward recompute: the input of every segment after the first (a dense Scale keeps its factor in the kernel
   // workspace, free until the reverse sweep)
   for (int s = 0; s + 1 < S; ++s) {
@@ -924,172 +991,28 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
     if (rc != B2B_OK) return rc;
     launches += g_last_launches;
   }
-  // 2. reverse sweep
+  // 2. reverse sweep: the cotangent moves between G[0] and G[1]; the one a segment does not write is free while it runs
   for (int s = S - 1; s >= 0; --s) {
     const VSeg& sg = segs[s];
-    const int n = sg.end - sg.begin;
-    const b2b_layer_desc* ls = layers + sg.begin;
-    const float* in = s == 0 ? x : ckpt[s];
-    long long ldin = s == 0 ? ldx : D;
-    const float* cin = s == S - 1 ? ybar : G[(s + 1) & 1];
-    long long ldcin = s == S - 1 ? ldybar : D;
-    float* out = s == 0 ? xbar : G[s & 1];
-    const long long ldout = s == 0 ? ldxbar : D;
-    float* cstage = G[(s + 1) & 1];  // free while this segment runs: holds a zero / realigned ȳ
-    auto stage_cot = [&](int rows) -> int {  // cin := zeros (ȳ == NULL) or a copy at ld = rows
-      if (!cin) B2B_VJP_CUDA(cudaMemsetAsync(cstage, 0, (size_t)D * N * F, stream));
-      else B2B_VJP_CUDA(cudaMemcpy2DAsync(cstage, (size_t)rows * F, cin, (size_t)ldcin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-      cin = cstage;
-      ldcin = rows;
-      return B2B_OK;
-    };
-    int nl = 0;
-    if (sg.kind == B2B_VC_PLANAR) {
-      const int Dk = sg.Dk;
-      const size_t r64 = ((size_t)n * Dk + 63) & ~(size_t)63;
-      float *wb = nullptr, *ub = nullptr, *bb = nullptr;
-      if (want >> sg.begin & ((1u << n) - 1)) {  // parameter cotangents of this run are requested
-        wb = scratch;
-        ub = scratch + r64;
-        bb = scratch + 2 * r64;
-      }
-      B2BChainParams p;
-      memset(&p, 0, sizeof(p));
-      p.N = N;
-      p.D = Dk;
-      p.L = n;
-      for (int j = 0; j < n; ++j) p.layers[j] = ls[j];
-      float* o = out;
-      long long ldo = ldout;
-      if (Dk != D) {
-        // embedded in Dk rows: w, u padded with zeros give the same map on the first D rows (wᵀz, wᵀu, ‖w‖² and those
-        // rows of û are unchanged) and leave the zero rows of x at zero
-        float* wp = scratch + 2 * r64 + 64;
-        float* up = wp + r64;
-        const float* src[16];
-        float* dst[16];
-        int len[16], dlen[16];
-        for (int j = 0; j < n; ++j) {
-          src[2 * j] = ls[j].p0;
-          dst[2 * j] = wp + (size_t)j * Dk;
-          src[2 * j + 1] = ls[j].p1;
-          dst[2 * j + 1] = up + (size_t)j * Dk;
-          len[2 * j] = len[2 * j + 1] = D;
-          dlen[2 * j] = dlen[2 * j + 1] = Dk;
-          p.layers[j].p0 = wp + (size_t)j * Dk;
-          p.layers[j].p1 = up + (size_t)j * Dk;
-        }
-        if ((rc = b2b_launch_copy_list(2 * n, src, dst, len, dlen, stream)) != B2B_OK) return rc;
-        ++launches;
-        const size_t pitch = (size_t)Dk * F, zrows = (size_t)(Dk - D) * F;
-        B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[0], pitch, in, (size_t)ldin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-        B2B_VJP_CUDA(cudaMemset2DAsync(pad[0] + D, pitch, 0, zrows, N, stream));
-        if (cin) {
-          B2B_VJP_CUDA(cudaMemcpy2DAsync(pad[1], pitch, cin, (size_t)ldcin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-          B2B_VJP_CUDA(cudaMemset2DAsync(pad[1] + D, pitch, 0, zrows, N, stream));
-        } else {
-          B2B_VJP_CUDA(cudaMemsetAsync(pad[1], 0, (size_t)Dk * N * F, stream));
-        }
-        in = pad[0];
-        ldin = Dk;
-        cin = pad[1];
-        ldcin = Dk;
-        o = pad[2];
-        ldo = Dk;
-      } else {
-        if (!tma_ok(in, ldin)) {
-          float* st = S >= 2 ? ckpt[1] : stage;  // segment 1's checkpoint is no longer needed
-          B2B_VJP_CUDA(cudaMemcpy2DAsync(st, (size_t)D * F, in, (size_t)ldin * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-          in = st;
-          ldin = D;
-        }
-        if (!tma_ok(cin, ldcin) && (rc = stage_cot(D)) != B2B_OK) return rc;
-        if (!tma_ok(o, ldo)) {
-          o = G[s & 1];
-          ldo = D;
-        }
-      }
-      p.x = in;
-      p.ldx = ldin;
-      rc = b2b_launch_planar_chain_vjp(p, cin, ldcin, ljbar, o, ldo, wb, ub, bb, kws, kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-      if (o != out) B2B_VJP_CUDA(cudaMemcpy2DAsync(out, (size_t)ldout * F, o, (size_t)ldo * F, (size_t)D * F, N, cudaMemcpyDeviceToDevice, stream));
-      const float* const base[3] = {wb, ub, bb};
-      const size_t step[3] = {(size_t)Dk, (size_t)Dk, 1};
-      if ((rc = copy_run_bars(ls, n, bars + 4 * sg.begin, base, step, D, &launches, stream)) != B2B_OK) return rc;
-    } else if (sg.kind == B2B_VC_RADIAL) {
-      if (!cin && (rc = stage_cot(D)) != B2B_OK) return rc;
-      float* ab = scratch;
-      float* bb = scratch + 64 * ((n + 63) / 64);
-      float* zb = bb + 64 * ((n + 63) / 64);
-      B2BChainParams p;
-      memset(&p, 0, sizeof(p));
-      p.x = in;
-      p.ldx = ldin;
-      p.N = N;
-      p.D = D;
-      p.L = n;
-      for (int j = 0; j < n; ++j) p.layers[j] = ls[j];
-      rc = b2b_launch_radial_chain_vjp(p, cin, ldcin, ljbar, out, ldout, ab, bb, zb, kws, kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-      const float* const base[3] = {ab, bb, zb};
-      const size_t step[3] = {1, 1, (size_t)D};
-      if ((rc = copy_run_bars(ls, n, bars + 4 * sg.begin, base, step, D, &launches, stream)) != B2B_OK) return rc;
-    } else if (sg.kind == B2B_VC_EW) {
-      const bool mvn = ls[n - 1].kind == B2B_MVNORMAL_DIAG;
-      rc = b2b_launch_ew_vjp(ls, n, in, ldin, cin, ldcin, ljbar, out, ldout, mvn ? bar(sg.end - 1, 0) : nullptr,
-                             mvn ? bar(sg.end - 1, 1) : nullptr, D, N, kws, kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-    } else if (sg.kind == B2B_VC_SPLINE) {
-      // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c
-      const b2b_layer_desc& d = ls[0];
-      float* wb = bar(sg.begin, 0) ? bar(sg.begin, 0) : scratch;
-      float* cb = !d.p1 ? nullptr : bar(sg.begin, 1) ? bar(sg.begin, 1)
-                                                       : scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
-      rc = b2b_launch_coupling_rqs_vjp(d, in, ldin, cin, ldcin, ljbar, out, ldout, wb, cb, D, N, kws, kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-    } else if (sg.kind == B2B_VC_MLP) {  // the four sums come from one kernel: those not asked for are dropped
-      float* const pb[4] = {bar(sg.begin, 0), bar(sg.begin, 1), bar(sg.begin, 2), bar(sg.begin, 3)};
-      rc = b2b_launch_coupling_mlp_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, pb, D, N, kws, kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-    } else if (sg.kind == B2B_VC_SCALE) {
-      rc = b2b_launch_scale_matrix_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), D, N, kws, kws_bytes,
-                                       &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-    } else if (sg.kind == B2B_VC_TRIL) {
-      rc = b2b_launch_tril_vjp(ls[0], in, ldin, cin, ldcin, ljbar, out, ldout, bar(sg.begin, 0), bar(sg.begin, 1), D, N, kws,
-                               kws_bytes, &nl, stream);
-      if (rc != B2B_OK) return rc;
-      launches += nl;
-    } else {  // one RQS, coupling or eval-BatchNorm layer: its own entry point (two launches each)
-      if (!cin && (rc = stage_cot(D)) != B2B_OK) return rc;
-      const b2b_layer_desc& d = ls[0];
-      float* pb[3];
-      size_t off = 0;
-      for (int i = 0; i < 3; ++i) {  // cotangents the caller did not ask for go to scratch
-        pb[i] = bar(sg.begin, i);
-        if (!pb[i] && (sg.kind == B2B_VC_RQS || i < 2)) {
-          pb[i] = scratch + off;
-          off += (b2b_slot_len(d, i, D) + 63) & ~(size_t)63;
-        }
-      }
-      if (sg.kind == B2B_VC_RQS)
-        rc = b2b_rqs_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], pb[2], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
-      else if (sg.kind == B2B_VC_COUPLING)
-        rc = b2b_coupling_affine_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
-      else
-        rc = b2b_batchnorm_eval_vjp_f32(&d, in, cin, ljbar, out, pb[0], pb[1], D, N, ldin, ldcin, ldout, kws, kws_bytes, stream);
-      if (rc != B2B_OK) return rc;
-      launches += 2;
+    B2BVjpSeg a{layers + sg.begin, sg.end - sg.begin, s == 0 ? x : ckpt[s], s == 0 ? ldx : D,
+                s == S - 1 ? ybar : G[(s + 1) & 1], s == S - 1 ? ldybar : D, ljbar, s == 0 ? xbar : G[s & 1],
+                s == 0 ? ldxbar : D, D, N, bars + 4 * sg.begin, scratch, kws, kws_bytes, &launches, stream};
+    float* const free_cot = G[(s + 1) & 1];
+    if (!a.ybar && vjp_needs_ybar(sg.kind) && (rc = stage_ybar(a, free_cot)) != B2B_OK) return rc;
+    switch (sg.kind) {  // segment 1's checkpoint is no longer needed when a planar run stages its x there
+      case B2B_VC_PLANAR: rc = vjp_planar_run(a, sg.Dk, pad, S >= 2 ? ckpt[1] : stage, free_cot, G[s & 1]); break;
+      case B2B_VC_RADIAL: rc = b2b_vjp_radial(a); break;
+      case B2B_VC_RQS: rc = b2b_vjp_rqs(a); break;
+      case B2B_VC_COUPLING: rc = b2b_vjp_coupling(a); break;
+      case B2B_VC_BN: rc = b2b_vjp_batchnorm(a); break;
+      case B2B_VC_EW: rc = b2b_vjp_ew(a); break;
+      case B2B_VC_TRIL: rc = b2b_vjp_tril(a); break;
+      case B2B_VC_SPLINE: rc = b2b_vjp_spline(a); break;
+      case B2B_VC_SCALE: rc = b2b_vjp_scale(a); break;
+      default: rc = b2b_vjp_mlp(a); break;
     }
+    if (rc != B2B_OK) return rc;
   }
-#undef B2B_VJP_CUDA
   g_last_launches = launches;
   return B2B_OK;
 }

@@ -243,9 +243,7 @@ __global__ void __launch_bounds__(256) bn_vjp_apply_kernel(const float* __restri
 }
 
 static int stats_grid(long long N) {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
   int grid = sms * 4;
   if (grid > 1184) grid = 1184;
   const long long want = (N + 7) / 8;
@@ -271,8 +269,7 @@ extern "C" int b2b_batchnorm_train_fwd_f32(const float* x, float* y, float* logj
   if (D > 1024) return B2B_EUNSUPPORTED;
   if (!workspace || workspace_bytes < b2b_batchnorm_train_workspace_bytes(D)) return B2B_EWORKSPACE;
   const int grid = stats_grid(N);
-  char* ws = static_cast<char*>(workspace);
-  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
+  char* ws = b2b_align256(workspace);
   double* partials = reinterpret_cast<double*>(ws);
   double* acc = partials + (size_t)1184 * 2 * D;
   float* batch_m = reinterpret_cast<float*>(acc + 2 * D + 2);
@@ -332,8 +329,7 @@ extern "C" int b2b_batchnorm_train_vjp_f32(const float* x, const float* ybar, co
   if (D > 1024) return B2B_EUNSUPPORTED;
   if (!workspace || workspace_bytes < b2b_batchnorm_train_vjp_workspace_bytes(D)) return B2B_EWORKSPACE;
   const int grid = stats_grid(N);
-  char* ws = static_cast<char*>(workspace);
-  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
+  char* ws = b2b_align256(workspace);
   double* partials = reinterpret_cast<double*>(ws);
   double* acc = partials + (size_t)1184 * (4 * D + 1);
   double* loc = acc + 4 * D + 2;
@@ -361,9 +357,7 @@ extern "C" int b2b_batchnorm_train_vjp_f32(const float* x, const float* ybar, co
                     (!ybar || ((ldybar % 4 == 0) && (reinterpret_cast<uintptr_t>(ybar) & 15) == 0));
   const int Du = vec2 ? D / 4 : D, rpt = (Du + 255) / 256, Dp = rpt == 1 ? ((Du + 31) & ~31) : 256, nslab = 256 / Dp;
   const int U = rpt == 1 ? 4 : 8 / rpt;
-  int sms = 0, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
   long long grid2 = (long long)sms * 4;
   const long long want = (N + (long long)nslab * U - 1) / ((long long)nslab * U);
   if (grid2 > want) grid2 = want;

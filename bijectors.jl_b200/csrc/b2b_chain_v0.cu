@@ -452,9 +452,8 @@ static int plan_v0(B2BChainParams& p, V0Plan& plan) {
   if (plan.smem > 48 * 1024)
     e = cudaFuncSetAttribute(plan.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
   if (e != cudaSuccess) return (int)e;
-  int dev = 0, sms = 0, per_sm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
+  int per_sm = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, plan.kernel, plan.block, plan.smem);
   if (e != cudaSuccess) return (int)e;
   if (per_sm < 1) per_sm = 1;

@@ -59,26 +59,18 @@ static int plan_v1(B2BChainParams& p, V1Plan& plan) {
   for (int l = 0; l < p.L; ++l) per_row |= p.layers[l].kind == B2B_RQS || p.layers[l].kind == B2B_STACKED_EW;
   // <D, lanes per column, columns per thread, warps>: warps are chosen so that the per-thread register budget
   // (65536 / threads) holds the fragment without spilling: 64 data registers need ~170 (12 warps), 128 need 255
-  // (8 warps), 32 fit in 128 (16 warps).  B2B_V1_CFG selects alternative builds for experiments.
-  static const int cfg = getenv("B2B_V1_CFG") ? atoi(getenv("B2B_V1_CFG")) : 0;
-  int nw, tpc, cpt = 1;
+  // (8 warps), 32 fit in 128 (16 warps).  One column per thread throughout.
+  int nw, tpc;
   if (D == 256) { plan.kernel = chain_v1_kernel<256, 4, 1, 12>; nw = 12; tpc = 4; }
   else if (D == 128) {
-    // default: one thread per column.  Chains with per-row layers
-    // (RQS, Stacked) use two lanes per column.  B2B_V1_CFG=2218 selects the build with two lanes per column and
-    // TWO columns per thread (every parameter load serves two columns: LDS wavefronts -36 %, but more scalar work
-    // per warp), 2112 the 2-lane / 12-warp build.
-    if (cfg == 2218 && !per_row) { plan.kernel = chain_v1_kernel<128, 2, 2, 8>; nw = 8; tpc = 2; cpt = 2; }
-    else if (cfg == 2112 || per_row) { plan.kernel = chain_v1_kernel<128, 2, 1, 12>; nw = 12; tpc = 2; }
+    // one thread per column; chains with per-row layers (RQS, Stacked) use two lanes per column
+    if (per_row) { plan.kernel = chain_v1_kernel<128, 2, 1, 12>; nw = 12; tpc = 2; }
     else { plan.kernel = chain_v1_kernel<128, 1, 1, 8>; nw = 8; tpc = 1; }
   }
-  else if (D == 64) {
-    if (cfg == 1128 && !per_row) { plan.kernel = chain_v1_kernel<64, 1, 2, 8>; nw = 8; tpc = 1; cpt = 2; }
-    else { plan.kernel = chain_v1_kernel<64, 1, 1, 12>; nw = 12; tpc = 1; }
-  }
+  else if (D == 64) { plan.kernel = chain_v1_kernel<64, 1, 1, 12>; nw = 12; tpc = 1; }
   else { plan.kernel = chain_v1_kernel<32, 1, 1, 16>; nw = 16; tpc = 1; }
-  plan.shape = D * 10000 + tpc * 1000 + cpt * 100 + nw;
-  return v1_geometry(D, p.N, nw, (32 / tpc) * cpt, (size_t)off, plan);
+  plan.shape = D * 10000 + tpc * 1000 + 100 + nw;
+  return v1_geometry(D, p.N, nw, 32 / tpc, (size_t)off, plan);
 }
 
 }  // namespace b2b

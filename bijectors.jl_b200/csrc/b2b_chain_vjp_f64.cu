@@ -626,8 +626,7 @@ extern "C" int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, co
   if (rc != B2B_OK || N == 0) return rc;
   int launches = 0;
   if (!workspace || workspace_bytes < plan.bytes) return B2B_EWORKSPACE;
-  char* ws = static_cast<char*>(workspace);
-  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
+  char* ws = b2b_align256(workspace);
   double* slots = reinterpret_cast<double*>(ws);
   double* red = slots + (size_t)plan.warps * plan.stride;
 

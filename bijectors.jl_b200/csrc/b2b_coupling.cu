@@ -267,9 +267,8 @@ int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const
                    : (d.inverse ? coupling_affine_rows_kernel<true> : coupling_affine_rows_kernel<false>);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  int dev = 0, sms = 0, per_sm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
+  int per_sm = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CP_THREADS, smem);
   if (e != cudaSuccess) return (int)e;
   if (per_sm < 1) per_sm = 1;

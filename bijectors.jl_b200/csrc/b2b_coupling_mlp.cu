@@ -169,9 +169,8 @@ int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, f
   void (*kernel)(const CmlpParams) = d.inverse ? coupling_mlp_kernel<true> : coupling_mlp_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  int dev = 0, sms = 0, per_sm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
+  int per_sm = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CP_THREADS, smem);
   if (e != cudaSuccess) return (int)e;
   if (per_sm < 1) per_sm = 1;

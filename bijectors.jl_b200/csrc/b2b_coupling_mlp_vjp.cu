@@ -273,10 +273,7 @@ static int cmv_nsub(const b2b_layer_desc& d, int D) {
 }
 
 static int cmv_grid(const b2b_layer_desc& d, int D, long long N) {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 132;
+  const int sms = b2b_sm_count();
   long long g = sms;
   const long long groups = (N + 32 * cmv_nsub(d, D) - 1) / (32 * cmv_nsub(d, D));
   if (g > groups) g = groups;
@@ -293,22 +290,21 @@ size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long 
   return (size_t)cmv_grid(d, D, N) * (size_t)cmv_slice_floats(d) * sizeof(float) + 256;
 }
 
-int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                                const float* ljbar, float* xbar, long long ldxb, float* const bars[4], int D, long long N,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: those not asked for are dropped
   using namespace b2b;
-  *launches = 0;
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  const long long N = s.N;
+  float* const* bars = s.bars;
   if (!b2b_coupling_mlp_fits(d, D)) return B2B_EUNSUPPORTED;
-  if (N <= 0) return B2B_OK;
   const bool want = bars[0] || bars[1] || bars[2] || bars[3];
-  if (want && (!workspace || workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  if (want && (!s.workspace || s.workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
+  char* wsb = b2b_align256(s.workspace);
   CmvParams P;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
   P.W1 = d.p0;
   P.c1 = d.p1;
   P.W2 = d.p2;
@@ -317,9 +313,9 @@ int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long lo
   P.idx2 = d.i1;
   P.part = want ? reinterpret_cast<float*>(wsb) : nullptr;
   P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldyb;
-  P.ldxb = ldxb;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
   P.slice = cmv_slice_floats(d);
   P.D = D;
   P.n1 = d.n0;
@@ -333,15 +329,15 @@ int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long lo
   void (*kernel)(const CmvParams) = d.inverse ? coupling_mlp_vjp_kernel<true> : coupling_mlp_vjp_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  kernel<<<grid, CMV_THREADS, smem, stream>>>(P);
+  kernel<<<grid, CMV_THREADS, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  *launches = 1;
+  ++*s.launches;
   if (want) {
     const long long l0 = (long long)d.n2 * d.n1, l1 = d.n2, l2 = (long long)2 * d.n0 * d.n2, l3 = 2 * d.n0;
-    coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l0 + l1 + l2 + l3 + 255) / 256), 256, 0, stream>>>(
+    coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l0 + l1 + l2 + l3 + 255) / 256), 256, 0, s.stream>>>(
         P.part, grid, P.slice, l0, l1, l2, l3, bars[0], bars[1], bars[2], bars[3]);
     if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-    *launches = 2;
+    ++*s.launches;
   }
   return B2B_OK;
 }

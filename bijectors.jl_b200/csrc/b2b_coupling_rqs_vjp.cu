@@ -187,10 +187,7 @@ static long long crv_slice_floats(const b2b_layer_desc& d) {
 }
 
 static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 132;
+  const int sms = b2b_sm_count();
   int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(d.n1, d.n2, D) + 1024));
   per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
   long long g = (long long)sms * per_sm;
@@ -209,30 +206,30 @@ size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long 
   return (size_t)crv_grid(d, D, N) * (size_t)crv_slice_floats(d) * sizeof(float) + 256;
 }
 
-int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                                const float* ljbar, float* xbar, long long ldxb, float* Wbar, float* cbar, int D, long long N,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+int b2b_vjp_spline(const B2BVjpSeg& s) {
   using namespace b2b;
-  *launches = 0;
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  const long long N = s.N;
   if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
-  if (N <= 0) return B2B_OK;
-  if (!workspace || workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  if (!s.workspace || s.workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
+  // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c
+  float* const Wbar = s.bars[0] ? s.bars[0] : s.scratch;
+  float* const cbar = !d.p1 ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
   CrvParams P;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
   P.W = d.p0;
   P.c = d.p1;
   P.idx1 = d.i0;
   P.idx2 = d.i1;
-  P.part = reinterpret_cast<float*>(wsb);
+  P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
   P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldyb;
-  P.ldxb = ldxb;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
   P.slice = crv_slice_floats(d);
   P.D = D;
   P.n1 = d.n0;
@@ -244,12 +241,12 @@ int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long lo
   void (*kernel)(const CrvParams) = d.inverse ? coupling_rqs_vjp_kernel<true> : coupling_rqs_vjp_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  kernel<<<grid, CRV_TN, smem, stream>>>(P);
+  kernel<<<grid, CRV_TN, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   const long long len = (long long)d.n0 * (3 * d.n2 - 1) * (d.n1 + 1);
-  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, stream>>>(P.part, grid, P.slice, d.n0, d.n1, d.n2,
-                                                                                    Wbar, cbar);
+  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(P.part, grid, P.slice, d.n0, d.n1,
+                                                                                      d.n2, Wbar, cbar);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  *launches = 2;
+  *s.launches += 2;
   return B2B_OK;
 }

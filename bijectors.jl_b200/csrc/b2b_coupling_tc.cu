@@ -518,9 +518,7 @@ int b2b_launch_coupling_affine_tc(const b2b_layer_desc& d, const float* fold, co
   }
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
   long long grid = sms;
   if (grid > P.tiles) grid = P.tiles;
   if (grid < 1) grid = 1;

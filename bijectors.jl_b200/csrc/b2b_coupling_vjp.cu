@@ -598,13 +598,6 @@ static size_t vjp_smem_bytes(const b2b_layer_desc& d, int D) {
                      : ((size_t)2 * D * CV_LD + (size_t)2 * n1 * CV_LD + CV_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int);
 }
 
-static int sm_count() {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 132;
-}
-
 }  // namespace b2b
 
 bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D) {
@@ -613,50 +606,39 @@ bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D) {
 
 extern "C" size_t b2b_coupling_affine_vjp_workspace_bytes(int32_t n1, int32_t n2) {
   if (n1 < 1 || n1 > 128 || n2 < 1 || n2 > 128) return 0;
-  return (size_t)b2b::sm_count() * ((size_t)2 * n1 * n2 + 2 * n1) * sizeof(float) + 256;
+  return (size_t)b2b_sm_count() * ((size_t)2 * n1 * n2 + 2 * n1) * sizeof(float) + 256;
 }
 
-extern "C" int b2b_coupling_affine_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar,
-                                           float* xbar, float* Wbar, float* cbar, int32_t D, int64_t N, int64_t ldx,
-                                           int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes,
-                                           void* stream_) {
+int b2b_vjp_coupling(const B2BVjpSeg& s) {
   using namespace b2b;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!layer || layer->kind != B2B_COUPLING_AFFINE || D < 1 || N < 0 || !Wbar || !cbar) return B2B_EINVAL;
-  const b2b_layer_desc& d = *layer;
-  const int n1 = d.n0, n2 = d.n1;
-  if (!d.p0 || n1 < 1 || n2 < 1 || n1 + n2 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
-  if (!b2b_coupling_affine_vjp_fits(d, D)) return B2B_EUNSUPPORTED;
-  if (N == 0) {
-    cudaMemsetAsync(Wbar, 0, sizeof(float) * (size_t)2 * n1 * n2, stream);
-    return (int)cudaMemsetAsync(cbar, 0, sizeof(float) * 2 * n1, stream);
-  }
-  if (!x || !ybar || !xbar || ldx < D || ldybar < D || ldxbar < D) return B2B_EINVAL;
-  const size_t need = b2b_coupling_affine_vjp_workspace_bytes(n1, n2);
-  if (!workspace || workspace_bytes < need) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  const b2b_layer_desc& d = s.layers[0];
+  const int n1 = d.n0, n2 = d.n1, D = s.D;
+  if (!s.workspace || s.workspace_bytes < b2b_coupling_affine_vjp_workspace_bytes(n1, n2)) return B2B_EWORKSPACE;
+  const int len0 = 2 * n1 * n2, len = len0 + 2 * n1;
+  // the kernel forms W̄ and c̄: those not asked for go to scratch
+  float* const Wbar = s.bars[0] ? s.bars[0] : s.scratch;
+  float* const cbar = s.bars[1] ? s.bars[1] : s.scratch + ((len0 + 63) & ~63);
   CvParams P;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
   P.W = d.p0;
   P.c = d.p1;
   P.idx1 = d.i0;
   P.idx2 = d.i1;
-  P.part = reinterpret_cast<float*>(wsb);
-  P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldybar;
-  P.ldxb = ldxbar;
+  P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
   P.D = D;
   P.n1 = n1;
   P.n2 = n2;
   P.row1 = d.n2;
   P.row2 = d.n3;
-  const long long tiles = (N + CV_TC - 1) / CV_TC;
-  long long grid = sm_count();
+  const long long tiles = (s.N + CV_TC - 1) / CV_TC;
+  long long grid = b2b_sm_count();
   if (grid > tiles) grid = tiles;
   const bool fast = vjp_fast(d);
   const size_t smem = vjp_smem_bytes(d, D);
@@ -668,24 +650,86 @@ extern "C" int b2b_coupling_affine_vjp_f32(const b2b_layer_desc* layer, const fl
   if (e != cudaSuccess) return (int)e;
   // the smallest carve-out that holds the CTA: the rest of the 256 KB stays L1 (W is re-read through it by every tile)
   cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((smem + 1024) * 100 / (228 * 1024) + 1));
-  kernel<<<(int)grid, CV_THREADS, smem, stream>>>(P);
+  kernel<<<(int)grid, CV_THREADS, smem, s.stream>>>(P);
   e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
-  const int len0 = 2 * n1 * n2, len = len0 + 2 * n1;
-  partial_sum_kernel<<<(len + 255) / 256, 256, 0, stream>>>(P.part, (int)grid, len, Wbar, len0, cbar);
+  partial_sum_kernel<<<(len + 255) / 256, 256, 0, s.stream>>>(P.part, (int)grid, len, Wbar, len0, cbar);
+  *s.launches += 2;
   return (int)cudaGetLastError();
+}
+
+extern "C" int b2b_coupling_affine_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar,
+                                           float* xbar, float* Wbar, float* cbar, int32_t D, int64_t N, int64_t ldx,
+                                           int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes,
+                                           void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!layer || layer->kind != B2B_COUPLING_AFFINE || D < 1 || N < 0 || !Wbar || !cbar) return B2B_EINVAL;
+  const b2b_layer_desc& d = *layer;
+  const int n1 = d.n0, n2 = d.n1;
+  if (!d.p0 || n1 < 1 || n2 < 1 || n1 + n2 > D || (!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
+  if (!b2b_coupling_affine_vjp_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (N == 0) {
+    cudaMemsetAsync(Wbar, 0, sizeof(float) * (size_t)2 * n1 * n2, stream);
+    return (int)cudaMemsetAsync(cbar, 0, sizeof(float) * 2 * n1, stream);
+  }
+  if (!x || !ybar || !xbar || ldx < D || ldybar < D || ldxbar < D) return B2B_EINVAL;
+  float* const bars[4] = {Wbar, cbar, nullptr, nullptr};
+  int launches = 0;
+  return b2b_vjp_coupling({layer, 1, x, ldx, ybar, ldybar, ljbar, xbar, ldxbar, D, N, bars, nullptr, workspace,
+                           workspace_bytes, &launches, stream});
 }
 
 extern "C" size_t b2b_batchnorm_eval_vjp_workspace_bytes(int32_t D) {
   if (D < 1 || D > 1024) return 0;
-  return (size_t)b2b::sm_count() * 4 * (size_t)(2 * D + 1) * sizeof(float) + 256;
+  return (size_t)b2b_sm_count() * 4 * (size_t)(2 * D + 1) * sizeof(float) + 256;
+}
+
+int b2b_vjp_batchnorm(const B2BVjpSeg& s) {
+  using namespace b2b;
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  if (!s.workspace || s.workspace_bytes < b2b_batchnorm_eval_vjp_workspace_bytes(D)) return B2B_EWORKSPACE;
+  // the kernel forms b̄ and log s̄: those not asked for go to scratch
+  float* const bbar = s.bars[0] ? s.bars[0] : s.scratch;
+  float* const logsbar = s.bars[1] ? s.bars[1] : s.scratch + ((D + 63) & ~63);
+  BvParams P;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
+  P.b = d.p0;
+  P.logs = d.p1;
+  P.m = d.p2;
+  P.v = d.p3;
+  P.eps = d.f0;
+  P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
+  P.D = D;
+  P.inverse = d.inverse ? 1 : 0;
+  const int rpt = (D + 255) / 256, Dp = rpt == 1 ? ((D + 31) & ~31) : 256, nslab = 256 / Dp;
+  long long grid = (long long)b2b_sm_count() * 4;
+  const int bu = rpt == 1 ? BV_U : BV_U / 2;
+  const long long want = (s.N + (long long)nslab * bu - 1) / ((long long)nslab * bu);
+  if (grid > want) grid = want;
+  const size_t smem = (size_t)nslab * (2 * D + 1) * sizeof(float);
+  void (*kernel)(const BvParams);
+  if (P.inverse) kernel = rpt == 1 ? bn_eval_vjp_kernel<1, true> : rpt == 2 ? bn_eval_vjp_kernel<2, true> : bn_eval_vjp_kernel<4, true>;
+  else kernel = rpt == 1 ? bn_eval_vjp_kernel<1, false> : rpt == 2 ? bn_eval_vjp_kernel<2, false> : bn_eval_vjp_kernel<4, false>;
+  kernel<<<(int)grid, 256, smem, s.stream>>>(P);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  bn_vjp_finalize_kernel<<<(2 * D + 31) / 32, dim3(32, 8), 0, s.stream>>>(P.part, (int)grid, D, P.inverse, bbar, logsbar);
+  *s.launches += 2;
+  return (int)cudaGetLastError();
 }
 
 extern "C" int b2b_batchnorm_eval_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar,
                                           float* xbar, float* bbar, float* logsbar, int32_t D, int64_t N, int64_t ldx,
                                           int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes,
                                           void* stream_) {
-  using namespace b2b;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!layer || layer->kind != B2B_BATCHNORM || D < 1 || N < 0 || !bbar || !logsbar) return B2B_EINVAL;
   const b2b_layer_desc& d = *layer;
@@ -696,39 +740,8 @@ extern "C" int b2b_batchnorm_eval_vjp_f32(const b2b_layer_desc* layer, const flo
     return (int)cudaMemsetAsync(logsbar, 0, sizeof(float) * D, stream);
   }
   if (!x || !ybar || !xbar || ldx < D || ldybar < D || ldxbar < D) return B2B_EINVAL;
-  const size_t need = b2b_batchnorm_eval_vjp_workspace_bytes(D);
-  if (!workspace || workspace_bytes < need) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
-  BvParams P;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
-  P.b = d.p0;
-  P.logs = d.p1;
-  P.m = d.p2;
-  P.v = d.p3;
-  P.eps = d.f0;
-  P.part = reinterpret_cast<float*>(wsb);
-  P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldybar;
-  P.ldxb = ldxbar;
-  P.D = D;
-  P.inverse = d.inverse ? 1 : 0;
-  const int rpt = (D + 255) / 256, Dp = rpt == 1 ? ((D + 31) & ~31) : 256, nslab = 256 / Dp;
-  long long grid = (long long)sm_count() * 4;
-  const int bu = rpt == 1 ? BV_U : BV_U / 2;
-  const long long want = (N + (long long)nslab * bu - 1) / ((long long)nslab * bu);
-  if (grid > want) grid = want;
-  const size_t smem = (size_t)nslab * (2 * D + 1) * sizeof(float);
-  void (*kernel)(const BvParams);
-  if (P.inverse) kernel = rpt == 1 ? bn_eval_vjp_kernel<1, true> : rpt == 2 ? bn_eval_vjp_kernel<2, true> : bn_eval_vjp_kernel<4, true>;
-  else kernel = rpt == 1 ? bn_eval_vjp_kernel<1, false> : rpt == 2 ? bn_eval_vjp_kernel<2, false> : bn_eval_vjp_kernel<4, false>;
-  kernel<<<(int)grid, 256, smem, stream>>>(P);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return (int)e;
-  bn_vjp_finalize_kernel<<<(2 * D + 31) / 32, dim3(32, 8), 0, stream>>>(P.part, (int)grid, D, P.inverse, bbar, logsbar);
-  return (int)cudaGetLastError();
+  float* const bars[4] = {bbar, logsbar, nullptr, nullptr};
+  int launches = 0;
+  return b2b_vjp_batchnorm({layer, 1, x, ldx, ybar, ldybar, ljbar, xbar, ldxbar, D, N, bars, nullptr, workspace,
+                            workspace_bytes, &launches, stream});
 }

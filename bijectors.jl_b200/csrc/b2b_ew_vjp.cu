@@ -256,19 +256,12 @@ __global__ void __launch_bounds__(128) copy_list_kernel(const __grid_constant__ 
   for (int e = threadIdx.x; e < c.dst_len[k]; e += blockDim.x) c.dst[k][e] = e < c.len[k] ? c.src[k][e] : 0.f;
 }
 
-static int ev_sm_count() {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 132;
-}
-
 static int ev_threads(int D) {
   const int Dp = (D + 31) & ~31;
   return Dp > 256 ? Dp : 256;
 }
 
-static int ev_grid_max() { return ev_sm_count() * 8; }
+static int ev_grid_max() { return b2b_sm_count() * 8; }
 
 }  // namespace b2b
 
@@ -277,10 +270,13 @@ size_t b2b_ew_vjp_workspace(int D, int want_mvn_params) {
   return (size_t)b2b::ev_grid_max() * 2 * (size_t)D * sizeof(float) + 256;
 }
 
-int b2b_launch_ew_vjp(const b2b_layer_desc* layers, int L, const float* x, long long ldx, const float* ybar,
-                      long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* mubar, float* sigmabar,
-                      int D, long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+int b2b_vjp_ew(const B2BVjpSeg& s) {
   using namespace b2b;
+  const b2b_layer_desc* layers = s.layers;
+  const int L = s.n, D = s.D;
+  const bool mvn = L > 0 && layers[L - 1].kind == B2B_MVNORMAL_DIAG;
+  float* const mubar = mvn ? s.bars[4 * (L - 1)] : nullptr;
+  float* const sigmabar = mvn ? s.bars[4 * (L - 1) + 1] : nullptr;
   if (D < 1 || D > 1024 || L < 0) return B2B_EUNSUPPORTED;
   EvParams P;
   memset(&P, 0, sizeof(P));
@@ -300,40 +296,35 @@ int b2b_launch_ew_vjp(const b2b_layer_desc* layers, int L, const float* x, long 
     }
   }
   const bool want = P.mvn && (mubar || sigmabar);
-  if (want && (!workspace || workspace_bytes < b2b_ew_vjp_workspace(D, 1))) return B2B_EWORKSPACE;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
-  P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldyb;
-  P.ldxb = ldxb;
+  if (want && (!s.workspace || s.workspace_bytes < b2b_ew_vjp_workspace(D, 1))) return B2B_EWORKSPACE;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
   P.D = D;
   const int T = ev_threads(D), Dp = (D + 31) & ~31, nslab = T / Dp;
   long long grid = ev_grid_max();
   const int U = T <= 256 ? 4 : 2;  // columns in flight per thread of the instantiation launched below
-  const long long need = (N + (long long)nslab * U - 1) / ((long long)nslab * U);
+  const long long need = (s.N + (long long)nslab * U - 1) / ((long long)nslab * U);
   if (grid > need) grid = need;
   if (grid < 1) grid = 1;
-  if (want) {
-    char* wsb = static_cast<char*>(workspace);
-    wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
-    P.part = reinterpret_cast<float*>(wsb);
-  }
+  if (want) P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
   const size_t smem = ((size_t)P.L * Dp + (size_t)3 * Ls * T) * sizeof(int) + (want ? (size_t)nslab * 2 * D * sizeof(float) : 0);
   void (*kernel)(const EvParams) = T <= 256 ? ew_vjp_kernel<256, 4> : ew_vjp_kernel<1024, 2>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  kernel<<<(int)grid, T, smem, stream>>>(P);
+  kernel<<<(int)grid, T, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  int nl = 1;
+  ++*s.launches;
   if (want) {
-    ew_vjp_finalize_kernel<<<(2 * D + 255) / 256, 256, 0, stream>>>(P.part, (int)grid, D, mubar, sigmabar);
+    ew_vjp_finalize_kernel<<<(2 * D + 255) / 256, 256, 0, s.stream>>>(P.part, (int)grid, D, mubar, sigmabar);
     if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-    ++nl;
+    ++*s.launches;
   }
-  if (launches) *launches = nl;
   return B2B_OK;
 }
 
@@ -353,4 +344,23 @@ int b2b_launch_copy_list(int n, const float* const* src, float* const* dst, cons
   }
   copy_list_kernel<<<dim3(1, n), 128, 0, stream>>>(c);
   return (int)cudaGetLastError();
+}
+
+int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, const float* const base[3],
+                      const size_t step[3], int D, int* launches, cudaStream_t stream) {
+  const float* src[24];
+  float* dst[24];
+  int len[24], dlen[24], c = 0;
+  for (int j = 0; j < n; ++j)
+    for (int i = 0; i < 3; ++i)
+      if (float* d = bars[4 * j + i]) {
+        src[c] = base[i] + j * step[i];
+        dst[c] = d;
+        len[c] = dlen[c] = (int)b2b_slot_len(layers[j], i, D);
+        ++c;
+      }
+  if (!c) return B2B_OK;
+  const int rc = b2b_launch_copy_list(c, src, dst, len, dlen, stream);
+  if (rc == B2B_OK) ++*launches;
+  return rc;
 }

@@ -75,34 +75,23 @@ int b2b_planar_const_grid_size(const B2BChainParams& p);
 int b2b_planar_const_layers(const B2BChainParams& p);
 // reverse mode of a forward radial chain (b2b_radial_vjp.cu)
 size_t b2b_radial_vjp_workspace(int L, int D);
-int b2b_launch_radial_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
-                                float* xbar, long long ldxb, float* alpha_bar, float* beta_bar, float* z0_bar,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // 1..8 radial layers of one direction as a specialised program (b2b_radial_unrolled.cu)
 int b2b_radial_unrolled_applicable(const B2BChainParams& p);
 int b2b_launch_radial_unrolled(const B2BChainParams& p, cudaStream_t stream);
 // a single RQS layer with 9 knots as a specialised program (b2b_rqs_unrolled.cu)
 int b2b_rqs_unrolled_applicable(const B2BChainParams& p);
 int b2b_launch_rqs_unrolled(const B2BChainParams& p, cudaStream_t stream);
-// reverse mode of a forward planar chain (b2b_planar_const.cu)
+// reverse mode of a forward planar chain (b2b_planar_vjp.cu)
 size_t b2b_planar_vjp_workspace(int L, int D, long long N);
-int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
-                                float* xbar, long long ldxb, float* wbar, float* ubar, float* bbar, void* workspace,
-                                size_t workspace_bytes, int* launches, cudaStream_t stream);
 // reverse mode of one affine coupling layer (b2b_coupling_vjp.cu): whether its kernel takes the layer at D (n1, n2 <= 128
 // and the D-row input / cotangent tiles within shared memory: D <= 747 at n1 = n2 = 128)
 bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D);
 // reverse mode of an elementwise run (b2b_ew_vjp.cu): <= 8 STACKED_EW / PERMUTE layers, optionally closed by the terminal
 // MVNORMAL_DIAG.  ybar, ljbar may be NULL (zeros); mubar / sigmabar (D, or NULL) need b2b_ew_vjp_workspace(D, 1) bytes.
 size_t b2b_ew_vjp_workspace(int D, int want_mvn_params);
-int b2b_launch_ew_vjp(const b2b_layer_desc* layers, int L, const float* x, long long ldx, const float* ybar,
-                      long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* mubar, float* sigmabar,
-                      int D, long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // one launch copying up to 24 small device vectors: dst[k][0, len[k]) = src[k][0, len[k]), zero up to dst_len[k]
 int b2b_launch_copy_list(int n, const float* const* src, float* const* dst, const int* len, const int* dst_len,
                          cudaStream_t stream);
-// number of CTAs the v0/v1 launch of `p` will use (size of the partials array)
-int b2b_chain_grid_size(const B2BChainParams& p);
 // deterministic final sum of per-CTA partials into *sum_out
 int b2b_launch_sum_partials(const double* partials, int n, double* sum_out, cudaStream_t stream);
 // affine coupling, tensor-core path (B2B_EUNSUPPORTED when the shape / workspace does not fit)
@@ -127,11 +116,8 @@ int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const
 int b2b_tril_grid(int D, long long N);
 int b2b_launch_mvnormal_tril(const b2b_layer_desc& d, const float* x, long long ldx, float* y, long long ldy,
                              float* logjac, int accumulate, double* partials, int D, long long N, cudaStream_t stream);
-// reverse mode: x̄ = ȳ − l̄·s always; μ̄ / L̄ (either may be NULL) need b2b_tril_vjp_workspace(D, N) bytes
+// reverse mode: μ̄ / L̄ need b2b_tril_vjp_workspace(D, N) bytes
 size_t b2b_tril_vjp_workspace(int D, long long N);
-int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                        const float* ljbar, float* xbar, long long ldxb, float* mubar, float* Lbar, int D, long long N,
-                        void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // Σₙ S[:, n] R[:, n]ᵀ over column chunks (b2b_mvnormal_tril.cu): CTA (tile, p) writes its 64 x 64 tile of chunk p's sum
 // to part[p] (D x D, column-major; fp32 FMA within a chunk, which the caller sums over p in a fixed order).  `lower`:
 // only the tiles on and below the diagonal, elements i >= j, and (when mup != NULL) chunk row sums of S to mup[p].
@@ -145,33 +131,22 @@ size_t b2b_scale_matrix_workspace(int D);
 int b2b_launch_scale_matrix(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, void* workspace, size_t workspace_bytes,
                             int* launches, cudaStream_t stream);
-// reverse mode: x̄ always, Ā when non-NULL; b2b_scale_matrix_vjp_workspace(D, N) bytes (0 beyond the envelope)
+// reverse mode: b2b_scale_matrix_vjp_workspace(D, N) bytes (0 beyond the envelope)
 size_t b2b_scale_matrix_vjp_workspace(int D, long long N);
-int b2b_launch_scale_matrix_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar,
-                                long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* Abar, int D,
-                                long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // spline coupling (b2b_coupling_rqs.cu, b2b_coupling_rqs_vjp.cu): whether the layer is within the envelope of include/b2b.h
 bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D);
 int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, cudaStream_t stream);
-// reverse mode: x̄ always, W̄ / c̄ when non-NULL; b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the envelope,
-// bounded independently of N); two launches
+// reverse mode: b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the envelope, bounded independently of N)
 size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
-int b2b_launch_coupling_rqs_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                                const float* ljbar, float* xbar, long long ldxb, float* Wbar, float* cbar, int D, long long N,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // neural-network coupling (b2b_coupling_mlp.cu, b2b_coupling_mlp_vjp.cu): whether the layer is within the envelope of
 // include/b2b.h
 bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D);
 int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, cudaStream_t stream);
-// reverse mode: x̄ always; bars[i] (NULL: not wanted) receives the cotangent of p<i> (W₁ c₁ W₂ c₂).  With any of them
-// b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope, bounded independently of N) and two launches,
-// else one launch and no workspace.
+// reverse mode: with any parameter cotangent b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope,
+// bounded independently of N) and two launches, else one launch and no workspace
 size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
-int b2b_launch_coupling_mlp_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                                const float* ljbar, float* xbar, long long ldxb, float* const bars[4], int D, long long N,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream);
 // B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
@@ -180,11 +155,64 @@ int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);
+// SMs of the current device, or 132 (an H100 SXM) when the query fails, as in a host-only workspace query
+int b2b_sm_count();
+// `workspace` rounded up to 256 bytes (the workspace sizes include 256 bytes of slack for it)
+inline char* b2b_align256(void* workspace) {
+  char* p = static_cast<char*>(workspace);
+  return p + ((256 - (reinterpret_cast<uintptr_t>(p) & 255)) & 255);
+}
+
+// ---- reverse-mode segment launchers ----------------------------------------------------------------------------------
+// One segment of b2b_chain_vjp_f32: `n` layers of one B2BVjpClass, their input x, the cotangent ȳ of their output, l̄ (N
+// floats, NULL: zero) and x̄ (written).  bars[4j + i] receives the cotangent of slot i of layer j (NULL: not wanted).
+// Every launcher works to the same rules:
+//   - the caller has validated the descriptors against vjp_envelope, N > 0, and ȳ is non-NULL for the classes of
+//     vjp_needs_ybar (b2b_api.cu);
+//   - the launcher checks what its kernels need: alignment, overlap, workspace size;
+//   - a cotangent its kernels always form but nobody asked for goes to `scratch` (seg_param_floats of b2b_api.cu);
+//   - it adds the exact number of launches it enqueued to *launches.
+// Planar and radial runs form their cotangents as whole arrays (w̄, ū n x D, b̄ n; ᾱ, β̄ n, z̄₀ n x D) in scratch and copy
+// the requested slots out in one launch; with scratch == NULL the bars are those arrays themselves (bars[i] is array i).
+struct B2BVjpSeg {
+  const b2b_layer_desc* layers;
+  int n;
+  const float* x;
+  long long ldx;
+  const float* ybar;
+  long long ldyb;
+  const float* ljbar;
+  float* xbar;
+  long long ldxb;
+  int D;
+  long long N;
+  float* const* bars;
+  float* scratch;
+  void* workspace;
+  size_t workspace_bytes;
+  int* launches;
+  cudaStream_t stream;
+};
+int b2b_vjp_planar(const B2BVjpSeg& s);    // b2b_planar_vjp.cu: <= 8 layers of one direction, D in {32, 64, 128}
+int b2b_vjp_radial(const B2BVjpSeg& s);    // b2b_radial_vjp.cu: <= 8 layers
+int b2b_vjp_rqs(const B2BVjpSeg& s);       // b2b_rqs_vjp.cu
+int b2b_vjp_coupling(const B2BVjpSeg& s);  // b2b_coupling_vjp.cu
+int b2b_vjp_batchnorm(const B2BVjpSeg& s); // b2b_coupling_vjp.cu: eval mode
+int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / PERMUTE, optionally closed by MVNORMAL_DIAG
+int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
+int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu
+int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu
+int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu
+// One launch copying slot i of layer j from base[i] + j·step[i] to bars[4j + i], for the requested slots of a run of
+// n <= 8 layers at D (nothing is launched when none is requested).
+int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, const float* const base[3],
+                      const size_t step[3], int D, int* launches, cudaStream_t stream);
 
 // ---- layer kinds ---------------------------------------------------------------------------------------------------
 // What the chain orchestration knows about each kind of include/b2b.h.  A new kind enters the host code as one row of
-// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu, its slot lengths in b2b_slot_len, and its
-// own launch and reverse-mode code in b2b_chain_run_f32 / b2b_chain_vjp_f32.
+// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu, its slot lengths in b2b_slot_len, its own
+// forward launch in b2b_chain_run_f32, and for reverse mode one B2BVjpSeg launcher plus one case of the sweep's switch
+// in b2b_chain_vjp_f32 (and its scratch and workspace sizes in seg_param_floats / seg_kernel_bytes).
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
 enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };

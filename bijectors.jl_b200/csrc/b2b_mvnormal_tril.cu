@@ -496,15 +496,18 @@ size_t b2b_tril_vjp_workspace(int D, long long N) {
          al(sizeof(double) * kMaxGrid);
 }
 
-int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar, long long ldyb,
-                        const float* ljbar, float* xbar, long long ldxb, float* mubar, float* Lbar, int D, long long N,
-                        void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
-  *launches = 0;
+int b2b_vjp_tril(const B2BVjpSeg& s) {
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  const long long N = s.N;
+  float* const mubar = s.bars[0];
+  float* const Lbar = s.bars[1];
+  const cudaStream_t stream = s.stream;
   if (D < 1 || D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
   const bool params = mubar || Lbar;
-  if (params && workspace_bytes < b2b_tril_vjp_workspace(D, N)) return B2B_EWORKSPACE;
+  if (params && s.workspace_bytes < b2b_tril_vjp_workspace(D, N)) return B2B_EWORKSPACE;
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  char* ws = static_cast<char*>(workspace);
+  char* ws = static_cast<char*>(s.workspace);
   float* Rw = params ? reinterpret_cast<float*>(ws) : nullptr;
   float* Sw = params ? reinterpret_cast<float*>(ws + al(sizeof(float) * (size_t)D * N)) : nullptr;
   const long long clen = chunk_len(N), P = (N + clen - 1) / clen;
@@ -517,21 +520,21 @@ int b2b_launch_tril_vjp(const b2b_layer_desc& d, const float* x, long long ldx, 
 #define B2B_TRIL_VJP(RR)                                                                                             \
   case RR:                                                                                                           \
     grid = grid_for(c_two(RR), N);                                                                                   \
-    rc = launch(vjp_kernel<RR, c_two(RR)>, grid, D, stream, x, ldx, ybar, ldyb, ljbar, xbar, ldxb, Rw, Sw, ljp, d.p1, \
-                d.p0, D, N);                                                                                         \
+    rc = launch(vjp_kernel<RR, c_two(RR)>, grid, D, stream, s.x, s.ldx, s.ybar, s.ldyb, s.ljbar, s.xbar, s.ldxb, Rw, Sw, \
+                ljp, d.p1, d.p0, D, N);                                                                              \
     break;
   switch (R) {
     B2B_TRIL_VJP(1) B2B_TRIL_VJP(2) B2B_TRIL_VJP(4) B2B_TRIL_VJP(8) B2B_TRIL_VJP(16)
   }
 #undef B2B_TRIL_VJP
   if (rc != B2B_OK) return rc;
-  *launches = 1;
+  ++*s.launches;
   if (!params) return B2B_OK;
   if ((rc = b2b_launch_outer_chunks(Sw, D, Rw, D, part, mup, D, N, true, stream)) != B2B_OK) return rc;
   const long long tot = (long long)D * D + D;
   finalize_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(part, mup, (int)P, ljp, grid, d.p1, Lbar, mubar, D);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
-  *launches = 3;
+  *s.launches += 2;
   return B2B_OK;
 }
 

@@ -485,7 +485,8 @@ static int launch_vjp_main(int dir, const B2BChainParams& q, const V1Geom& g, co
   return (int)cudaGetLastError();
 }
 
-template <int D, int NW>
+// NW8: the warps of the 8-layer program
+template <int D, int NW, int NW8 = NW>
 static int dispatch_vjp_main(int dir, int L, const B2BChainParams& q, const V1Geom& g, const CUtensorMap& mx,
                              const CUtensorMap& myb, const CUtensorMap& mxb, float* scal, int nreal,
                              cudaStream_t stream) {
@@ -493,7 +494,7 @@ static int dispatch_vjp_main(int dir, int L, const B2BChainParams& q, const V1Ge
     case 1: return launch_vjp_main<D, 1, NW>(dir, q, g, mx, myb, mxb, scal, nreal, stream);
     case 2: return launch_vjp_main<D, 2, NW>(dir, q, g, mx, myb, mxb, scal, nreal, stream);
     case 4: return launch_vjp_main<D, 4, NW>(dir, q, g, mx, myb, mxb, scal, nreal, stream);
-    case 8: return launch_vjp_main<D, 8, NW>(dir, q, g, mx, myb, mxb, scal, nreal, stream);
+    case 8: return launch_vjp_main<D, 8, NW8>(dir, q, g, mx, myb, mxb, scal, nreal, stream);
     default: return B2B_EUNSUPPORTED;
   }
 }
@@ -501,10 +502,9 @@ static int dispatch_vjp_main(int dir, int L, const B2BChainParams& q, const V1Ge
 template <int D, int L>
 static int launch_pgrad_L(const float* x, const float* yb, const float* scal, long long N, long long ldx,
                           long long ldyb, float* partials, cudaStream_t stream) {
-  static const int force_reg = getenv("B2B_PGRAD") && atoi(getenv("B2B_PGRAD")) == 1;
   const bool dense = ldx == D && ldyb == D && !((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(yb) |
                                                  reinterpret_cast<uintptr_t>(scal)) & 15);
-  if (dense && !force_reg) {
+  if (dense) {
     auto kernel = planar_pgrad_bulk_kernel<D, L>;
     const int smem = PGB_STAGES * (2 * PGB_CH * D * 4 + PGB_CH * 3 * L * 4);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -547,31 +547,51 @@ size_t b2b_planar_vjp_workspace(int L, int D, long long N) {
   return b2b::vjp_carve(nullptr, Lp, D, N).bytes;
 }
 
-// p: L (1..8) forward PLANAR layers in p.layers, p.x = x, p.N, p.D, p.ldx.  ybar / xbar: D x N cotangents
-// (xbar may alias ybar), ljbar: N or NULL.  wbar, ubar: L x D, bbar: L (device).  Returns the launch count in *launches.
-int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
-                                float* xbar, long long ldxb, float* wbar, float* ubar, float* bbar, void* workspace,
-                                size_t workspace_bytes, int* launches, cudaStream_t stream) {
+int b2b_vjp_planar(const B2BVjpSeg& s) {
   using namespace b2b;
-  const int n = p.L, D = p.D;
+  const int n = s.n, D = s.D;
   if (n < 1 || n > HP_MAX_L || !(D == 32 || D == 64 || D == 128)) return B2B_EUNSUPPORTED;
-  const int dir = p.layers[0].inverse ? 1 : 0;  // all layers forward, or all inverse (application order)
+  const int dir = s.layers[0].inverse ? 1 : 0;  // all layers forward, or all inverse (application order)
   for (int l = 0; l < n; ++l)
-    if (p.layers[l].kind != B2B_PLANAR || (p.layers[l].inverse ? 1 : 0) != dir) return B2B_EUNSUPPORTED;
+    if (s.layers[l].kind != B2B_PLANAR || (s.layers[l].inverse ? 1 : 0) != dir) return B2B_EUNSUPPORTED;
+  bool want = false;
+  for (int k = 0; k < 4 * n; ++k) want = want || s.bars[k];
+  float *wbar = nullptr, *ubar = nullptr, *bbar = nullptr;
+  const size_t r64 = ((size_t)n * D + 63) & ~(size_t)63;
+  if (want && s.scratch) {
+    wbar = s.scratch;
+    ubar = s.scratch + r64;
+    bbar = s.scratch + 2 * r64;
+  } else if (want) {
+    wbar = s.bars[0];
+    ubar = s.bars[1];
+    bbar = s.bars[2];
+  }
+  B2BChainParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = s.x;
+  p.N = s.N;
+  p.ldx = s.ldx;
+  p.D = D;
+  p.L = n;
+  for (int l = 0; l < n; ++l) p.layers[l] = s.layers[l];
+  const float* ybar = s.ybar;
+  const long long ldyb = s.ldyb;
+  float* xbar = s.xbar;
   int Lp = 1;
   while (Lp < n) Lp <<= 1;
   B2BChainParams q = p;  // main kernel: x -> (fragment 1), ybar -> (fragment 2), xbar out, ljbar read-only
   q.L = 0;
   q.scratch_off = -1;
   q.y = xbar;
-  q.ldy = ldxb;
-  q.logjac = const_cast<float*>(ljbar);
+  q.ldy = s.ldxb;
+  q.logjac = const_cast<float*>(s.ljbar);
   q.accumulate = 3;  // read ljbar, never write it
   q.partials = nullptr;
   if (v1_check_io(q) != 0) return B2B_EUNSUPPORTED;
   if ((ldyb % 4) || (reinterpret_cast<uintptr_t>(ybar) & 15) || !xbar) return B2B_EUNSUPPORTED;
   // the parameter pass re-reads x AND ybar after the main kernel has written xbar: xbar must not overlap either
-  if (wbar && ubar && bbar) {
+  if (want) {
     auto overlaps = [&](const float* a, long long lda, const float* b, long long ldb) {
       const char* a0 = reinterpret_cast<const char*>(a);
       const char* a1 = a0 + ((size_t)(p.N - 1) * (size_t)lda + (size_t)D) * sizeof(float);
@@ -579,47 +599,42 @@ int b2b_launch_planar_chain_vjp(const B2BChainParams& p, const float* ybar, long
       const char* b1 = b0 + ((size_t)(p.N - 1) * (size_t)ldb + (size_t)D) * sizeof(float);
       return a0 < b1 && b0 < a1;
     };
-    if (overlaps(xbar, ldxb, ybar, ldyb) || overlaps(xbar, ldxb, p.x, p.ldx)) return B2B_EINVAL;
+    if (overlaps(xbar, s.ldxb, ybar, ldyb) || overlaps(xbar, s.ldxb, p.x, p.ldx)) return B2B_EINVAL;
   }
-  if (!workspace || workspace_bytes < b2b_planar_vjp_workspace(n, D, p.N)) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
-  const VjpWs ws = vjp_carve(wsb, Lp, D, p.N);
+  if (!s.workspace || s.workspace_bytes < b2b_planar_vjp_workspace(n, D, p.N)) return B2B_EWORKSPACE;
+  const VjpWs ws = vjp_carve(b2b_align256(s.workspace), Lp, D, p.N);
+  const cudaStream_t stream = s.stream;
 
   V1Geom g;
-  static const int vjp_nw = getenv("B2B_VJP_NW") ? atoi(getenv("B2B_VJP_NW")) : 0;
   // D = 128 x 8 layers: two-tensor slots are 32 KB; 7 warps leave room for 3 of them (8 warps: 2)
-  const int nw = (D == 128 && Lp == 8) ? ((vjp_nw == 6 || vjp_nw == 8) ? vjp_nw : 7) : hp_warps(D);
-  int rc = v1_geometry(D, p.N, nw, 32, (size_t)((2 * Lp * D + 2 * Lp + 3) & ~3), g, 2);
+  int rc = v1_geometry(D, p.N, D == 128 && Lp == 8 ? 7 : hp_warps(D), 32, (size_t)((2 * Lp * D + 2 * Lp + 3) & ~3), g, 2);
   if (rc != 0) return rc;
   CUtensorMap mx, mxb, myb;
   if (!make_maps(q, g.cols, &mx, &mxb, &g.extra.tma3d)) return B2B_EUNSUPPORTED;
   if (!make_map(&myb, ybar, D, p.N, ldyb, g.cols, g.extra.tma3d != 0)) return B2B_EUNSUPPORTED;
-  if (D == 128 && Lp == 8 && g.nw == 6) rc = launch_vjp_main<128, 8, 6>(dir, q, g, mx, myb, mxb, ws.scal, n, stream);
-  else if (D == 128 && Lp == 8 && g.nw == 7) rc = launch_vjp_main<128, 8, 7>(dir, q, g, mx, myb, mxb, ws.scal, n, stream);
-  else if (D == 128) rc = dispatch_vjp_main<128, 8>(dir, Lp, q, g, mx, myb, mxb, ws.scal, n, stream);
+  if (D == 128) rc = dispatch_vjp_main<128, 8, 7>(dir, Lp, q, g, mx, myb, mxb, ws.scal, n, stream);
   else if (D == 64) rc = dispatch_vjp_main<64, 12>(dir, Lp, q, g, mx, myb, mxb, ws.scal, n, stream);
   else rc = dispatch_vjp_main<32, 16>(dir, Lp, q, g, mx, myb, mxb, ws.scal, n, stream);
   if (rc != B2B_OK) return rc;
-  cudaError_t e;
-  // parameter gradients: skinny reductions over the ORIGINAL x and ybar.  NOTE: xbar may alias ybar, in which case
-  // ybar has been overwritten -- aliasing is therefore only allowed when the caller does not want parameter gradients.
-  int nl = 1;
-  if (wbar && ubar && bbar) {
-    planar_prep_kernel<<<1, HP_MAX_L * 32, 0, stream>>>(p, n, Lp, ws.packed);  // w | û | c | b for the finalize kernel
-    if (D == 128) rc = launch_pgrad<128>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
-    else if (D == 64) rc = launch_pgrad<64>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
-    else rc = launch_pgrad<32>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
-    if (rc != B2B_OK) return rc;
-    planar_psum_kernel<<<(2 * Lp * D + 7) / 8, 256, 0, stream>>>(ws.pg_partials, VJP_PG_GRID, 2 * Lp * D, ws.A);
-    rc = launch_sstat(Lp, ws.scal, p.N, ws.ss_partials, stream);
-    if (rc != B2B_OK) return rc;
-    const int ns = Lp * Lp + 2 * Lp;
-    planar_psum_kernel<<<(ns + 7) / 8, 256, 0, stream>>>(ws.ss_partials, VJP_SS_GRID, ns, ws.SS);
-    planar_vjp_finalize_kernel<<<n, 256, 0, stream>>>(p, n, Lp, dir, ws.packed, ws.A, ws.SS, wbar, ubar, bbar);
-    if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-    nl += 6;
-  }
-  if (launches) *launches = nl;
-  return B2B_OK;
+  ++*s.launches;
+  if (!want) return B2B_OK;
+  // parameter gradients: skinny reductions over the ORIGINAL x and ybar
+  planar_prep_kernel<<<1, HP_MAX_L * 32, 0, stream>>>(p, n, Lp, ws.packed);  // w | û | c | b for the finalize kernel
+  if (D == 128) rc = launch_pgrad<128>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
+  else if (D == 64) rc = launch_pgrad<64>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
+  else rc = launch_pgrad<32>(Lp, p.x, ybar, ws.scal, p.N, p.ldx, ldyb, ws.pg_partials, stream);
+  if (rc != B2B_OK) return rc;
+  planar_psum_kernel<<<(2 * Lp * D + 7) / 8, 256, 0, stream>>>(ws.pg_partials, VJP_PG_GRID, 2 * Lp * D, ws.A);
+  rc = launch_sstat(Lp, ws.scal, p.N, ws.ss_partials, stream);
+  if (rc != B2B_OK) return rc;
+  const int ns = Lp * Lp + 2 * Lp;
+  planar_psum_kernel<<<(ns + 7) / 8, 256, 0, stream>>>(ws.ss_partials, VJP_SS_GRID, ns, ws.SS);
+  planar_vjp_finalize_kernel<<<n, 256, 0, stream>>>(p, n, Lp, dir, ws.packed, ws.A, ws.SS, wbar, ubar, bbar);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  *s.launches += 6;
+  if (!s.scratch) return B2B_OK;
+  const float* const base[3] = {wbar, ubar, bbar};
+  const size_t step[3] = {(size_t)D, (size_t)D, 1};
+  return b2b_copy_run_bars(s.layers, n, s.bars, base, step, D, s.launches, stream);
 }

@@ -261,23 +261,23 @@ size_t b2b_radial_vjp_workspace(int L, int D) {
   return (size_t)b2b::RV_GRID_MAX * (size_t)(L * D + 2 * L) * sizeof(float) + 256;
 }
 
-// p: L (1..8) forward RADIAL layers, p.x, p.N, p.D (<= 128), p.ldx.  Outputs: xbar (D x N, may alias ybar),
-// alpha_bar / beta_bar (L), z0_bar (L x D).
-int b2b_launch_radial_chain_vjp(const B2BChainParams& p, const float* ybar, long long ldyb, const float* ljbar,
-                                float* xbar, long long ldxb, float* alpha_bar, float* beta_bar, float* z0_bar,
-                                void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
+int b2b_vjp_radial(const B2BVjpSeg& s) {
   using namespace b2b;
-  const int L = p.L, D = p.D;
+  const int L = s.n, D = s.D;
   if (L < 1 || L > 8 || D > 128) return B2B_EUNSUPPORTED;
   for (int l = 0; l < L; ++l)
-    if (p.layers[l].kind != B2B_RADIAL) return B2B_EUNSUPPORTED;
-  if (!workspace || workspace_bytes < b2b_radial_vjp_workspace(L, D)) return B2B_EWORKSPACE;
-  char* ws = static_cast<char*>(workspace);
-  ws += (256 - (reinterpret_cast<uintptr_t>(ws) & 255)) & 255;
-  float* partials = reinterpret_cast<float*>(ws);
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (s.layers[l].kind != B2B_RADIAL) return B2B_EUNSUPPORTED;
+  if (!s.workspace || s.workspace_bytes < b2b_radial_vjp_workspace(L, D)) return B2B_EWORKSPACE;
+  float* partials = reinterpret_cast<float*>(b2b_align256(s.workspace));
+  B2BChainParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = s.x;
+  p.N = s.N;
+  p.ldx = s.ldx;
+  p.D = D;
+  p.L = L;
+  for (int l = 0; l < L; ++l) p.layers[l] = s.layers[l];
+  const int sms = b2b_sm_count();
   int grid = sms * 4;
   if (grid > RV_GRID_MAX) grid = RV_GRID_MAX;
   const int tpc = D <= 32 ? 4 : D <= 64 ? 8 : 16;
@@ -288,11 +288,20 @@ int b2b_launch_radial_chain_vjp(const B2BChainParams& p, const float* ybar, long
   for (int l = 0; l < L; ++l) fwd = fwd && !p.layers[l].inverse;
   const bool exact = D == 8 * tpc;
   int rc;
-  if (tpc == 4) rc = dispatch_radial_vjp<4>(exact, fwd, L, grid, p, ybar, ldyb, ljbar, xbar, ldxb, partials, stream);
-  else if (tpc == 8) rc = dispatch_radial_vjp<8>(exact, fwd, L, grid, p, ybar, ldyb, ljbar, xbar, ldxb, partials, stream);
-  else rc = dispatch_radial_vjp<16>(exact, fwd, L, grid, p, ybar, ldyb, ljbar, xbar, ldxb, partials, stream);
+  if (tpc == 4) rc = dispatch_radial_vjp<4>(exact, fwd, L, grid, p, s.ybar, s.ldyb, s.ljbar, s.xbar, s.ldxb, partials, s.stream);
+  else if (tpc == 8) rc = dispatch_radial_vjp<8>(exact, fwd, L, grid, p, s.ybar, s.ldyb, s.ljbar, s.xbar, s.ldxb, partials, s.stream);
+  else rc = dispatch_radial_vjp<16>(exact, fwd, L, grid, p, s.ybar, s.ldyb, s.ljbar, s.xbar, s.ldxb, partials, s.stream);
   if (rc != B2B_OK) return rc;
-  radial_vjp_finalize_kernel<<<1 + (L * D + 7) / 8, 256, 0, stream>>>(p, L, partials, grid, alpha_bar, beta_bar, z0_bar);
-  if (launches) *launches = 2;
-  return (int)cudaGetLastError();
+  // ᾱ, β̄ (L) and z̄₀ (L x D), each array 64-float aligned in scratch
+  const size_t r = 64 * (size_t)((L + 63) / 64);
+  float* const ab = s.scratch ? s.scratch : s.bars[0];
+  float* const bb = s.scratch ? s.scratch + r : s.bars[1];
+  float* const zb = s.scratch ? s.scratch + 2 * r : s.bars[2];
+  radial_vjp_finalize_kernel<<<1 + (L * D + 7) / 8, 256, 0, s.stream>>>(p, L, partials, grid, ab, bb, zb);
+  if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
+  *s.launches += 2;
+  if (!s.scratch) return B2B_OK;
+  const float* const base[3] = {ab, bb, zb};
+  const size_t step[3] = {1, 1, (size_t)D};
+  return b2b_copy_run_bars(s.layers, L, s.bars, base, step, D, s.launches, s.stream);
 }

@@ -169,10 +169,7 @@ static RqvShape rqv_shape(int K1, int D) {
   const size_t acc = (size_t)3 * K1 * RQV_THREADS * sizeof(float), tab = (size_t)3 * K1 * Dp * sizeof(float);
   s.stab = acc + tab <= RQV_SMEM_MAX;
   s.smem = acc + (s.stab ? tab : 0);
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 132;
+  const int sms = b2b_sm_count();
   int per_sm = (int)((size_t)(227 * 1024) / (s.smem + 1024));
   if (per_sm > 3) per_sm = 3;  // 80 registers x 256 threads: three CTAs per SM
   if (per_sm < 1) per_sm = 1;
@@ -187,45 +184,34 @@ extern "C" size_t b2b_rqs_vjp_workspace_bytes(int32_t K1, int32_t D) {
   return (size_t)b2b::rqv_shape(K1, D).grid_max * 3 * (size_t)K1 * D * sizeof(float) + 256;
 }
 
-extern "C" int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar, float* xbar,
-                               float* widths_bar, float* heights_bar, float* derivs_bar, int32_t D, int64_t N, int64_t ldx,
-                               int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes, void* stream_) {
+int b2b_vjp_rqs(const B2BVjpSeg& s) {
   using namespace b2b;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!layer || layer->kind != B2B_RQS || D < 1 || N < 0 || !widths_bar || !heights_bar || !derivs_bar) return B2B_EINVAL;
-  const b2b_layer_desc& d = *layer;
-  const int K1 = d.n0;
-  if (!d.p0 || !d.p1 || !d.p2 || K1 < 2) return B2B_EINVAL;
-  if (K1 > 64 || D > 256) return B2B_EUNSUPPORTED;
+  const b2b_layer_desc& d = s.layers[0];
+  const int K1 = d.n0, D = s.D;
   const size_t per = (size_t)K1 * D;
-  if (N == 0) {
-    cudaMemsetAsync(widths_bar, 0, per * sizeof(float), stream);
-    cudaMemsetAsync(heights_bar, 0, per * sizeof(float), stream);
-    return (int)cudaMemsetAsync(derivs_bar, 0, per * sizeof(float), stream);
-  }
-  if (!x || !ybar || !xbar || ldx < D || ldybar < D || ldxbar < D) return B2B_EINVAL;
-  if (!workspace || workspace_bytes < b2b_rqs_vjp_workspace_bytes(K1, D)) return B2B_EWORKSPACE;
-  char* wsb = static_cast<char*>(workspace);
-  wsb += (256 - (reinterpret_cast<uintptr_t>(wsb) & 255)) & 255;
+  if (!s.workspace || s.workspace_bytes < b2b_rqs_vjp_workspace_bytes(K1, D)) return B2B_EWORKSPACE;
+  float* bar[3];
+  for (int i = 0; i < 3; ++i)  // the kernel forms all three: those not asked for go to scratch
+    bar[i] = s.bars[i] ? s.bars[i] : s.scratch + i * ((per + 63) & ~(size_t)63);
   RqvParams P;
-  P.x = x;
-  P.ybar = ybar;
-  P.ljbar = ljbar;
-  P.xbar = xbar;
+  P.x = s.x;
+  P.ybar = s.ybar;
+  P.ljbar = s.ljbar;
+  P.xbar = s.xbar;
   P.W = d.p0;
   P.H = d.p1;
   P.Dv = d.p2;
-  P.part = reinterpret_cast<float*>(wsb);
-  P.N = N;
-  P.ldx = ldx;
-  P.ldyb = ldybar;
-  P.ldxb = ldxbar;
+  P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldyb = s.ldyb;
+  P.ldxb = s.ldxb;
   P.D = D;
   P.K1 = K1;
   const RqvShape sh = rqv_shape(K1, D);
   const int Dp = (D + 31) & ~31, nslab = RQV_THREADS / Dp;
   int grid = sh.grid_max;
-  const long long want = (N + (long long)nslab * RQV_U - 1) / ((long long)nslab * RQV_U);
+  const long long want = (s.N + (long long)nslab * RQV_U - 1) / ((long long)nslab * RQV_U);
   if (grid > want) grid = (int)want;
   void (*kernel)(const RqvParams) = nullptr;
 #define B2B_RQV_EXACT(KK, DD)                                                                        \
@@ -239,11 +225,33 @@ extern "C" int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, cons
                        : (sh.stab ? rqs_vjp_kernel<false, true, 0, 0> : rqs_vjp_kernel<false, false, 0, 0>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
   if (e != cudaSuccess) return (int)e;
-  kernel<<<grid, RQV_THREADS, sh.smem, stream>>>(P);
+  kernel<<<grid, RQV_THREADS, sh.smem, s.stream>>>(P);
   e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   const int len = (int)(3 * per);
-  rqs_vjp_reduce_kernel<<<(len + 31) / 32, dim3(32, 8), 0, stream>>>(P.part, grid, len, (int)per, widths_bar, heights_bar,
-                                                                     derivs_bar);
+  rqs_vjp_reduce_kernel<<<(len + 31) / 32, dim3(32, 8), 0, s.stream>>>(P.part, grid, len, (int)per, bar[0], bar[1], bar[2]);
+  *s.launches += 2;
   return (int)cudaGetLastError();
+}
+
+extern "C" int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* ybar, const float* ljbar, float* xbar,
+                               float* widths_bar, float* heights_bar, float* derivs_bar, int32_t D, int64_t N, int64_t ldx,
+                               int64_t ldybar, int64_t ldxbar, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!layer || layer->kind != B2B_RQS || D < 1 || N < 0 || !widths_bar || !heights_bar || !derivs_bar) return B2B_EINVAL;
+  const b2b_layer_desc& d = *layer;
+  const int K1 = d.n0;
+  if (!d.p0 || !d.p1 || !d.p2 || K1 < 2) return B2B_EINVAL;
+  if (K1 > 64 || D > 256) return B2B_EUNSUPPORTED;
+  const size_t per = (size_t)K1 * D;
+  if (N == 0) {
+    cudaMemsetAsync(widths_bar, 0, per * sizeof(float), stream);
+    cudaMemsetAsync(heights_bar, 0, per * sizeof(float), stream);
+    return (int)cudaMemsetAsync(derivs_bar, 0, per * sizeof(float), stream);
+  }
+  if (!x || !ybar || !xbar || ldx < D || ldybar < D || ldxbar < D) return B2B_EINVAL;
+  float* const bars[4] = {widths_bar, heights_bar, derivs_bar, nullptr};
+  int launches = 0;
+  return b2b_vjp_rqs({layer, 1, x, ldx, ybar, ldybar, ljbar, xbar, ldxbar, D, N, bars, nullptr, workspace, workspace_bytes,
+                      &launches, stream});
 }

@@ -123,7 +123,6 @@ extern "C" int b2b_chain_sample_f32(const b2b_layer_desc* layers, int32_t L, con
           case 1282112: return launch_sample<128, 2, 1, 12>(p, g, my, gen, stream);
           case 641112: return launch_sample<64, 1, 1, 12>(p, g, my, gen, stream);
           case 321116: return launch_sample<32, 1, 1, 16>(p, g, my, gen, stream);
-          default: break;  // experimental shapes (B2B_V1_CFG): two passes below
         }
       }
     }

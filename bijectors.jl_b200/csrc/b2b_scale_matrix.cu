@@ -51,8 +51,7 @@ size_t factor_bytes(int D) {
 }
 
 Factor carve(void* ws, int D) {
-  char* p = static_cast<char*>(ws);
-  p += (256 - (reinterpret_cast<uintptr_t>(p) & 255)) & 255;
+  char* p = b2b_align256(ws);
   Factor f;
   f.lu = reinterpret_cast<double*>(p);
   p += al256(sizeof(double) * (size_t)D * D);
@@ -501,12 +500,18 @@ size_t b2b_scale_matrix_vjp_workspace(int D, long long N) {
          al256(sizeof(double));
 }
 
-int b2b_launch_scale_matrix_vjp(const b2b_layer_desc& d, const float* x, long long ldx, const float* ybar,
-                                long long ldyb, const float* ljbar, float* xbar, long long ldxb, float* Abar, int D,
-                                long long N, void* workspace, size_t workspace_bytes, int* launches, cudaStream_t stream) {
-  *launches = 0;
+int b2b_vjp_scale(const B2BVjpSeg& s) {
+  const b2b_layer_desc& d = s.layers[0];
+  const float *x = s.x, *ybar = s.ybar, *ljbar = s.ljbar;
+  const long long ldx = s.ldx, ldyb = s.ldyb, ldxb = s.ldxb, N = s.N;
+  float* const xbar = s.xbar;
+  float* const Abar = s.bars[0];
+  void* const workspace = s.workspace;
+  const int D = s.D;
+  int* const launches = s.launches;
+  const cudaStream_t stream = s.stream;
   if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-  if (!workspace || workspace_bytes < b2b_scale_matrix_vjp_workspace(D, N)) return B2B_EWORKSPACE;
+  if (!workspace || s.workspace_bytes < b2b_scale_matrix_vjp_workspace(D, N)) return B2B_EWORKSPACE;
   const Factor f = carve(workspace, D);
   const bool inv = d.inverse != 0;
   char* ws = static_cast<char*>(workspace) + factor_bytes(D);

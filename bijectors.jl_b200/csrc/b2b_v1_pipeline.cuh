@@ -512,10 +512,9 @@ static inline bool make_map(CUtensorMap* m, const float* base, int D, long long 
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// Both maps of a launch; 3-D when the driver accepts them (B2B_V1_TMA=2 forces the 2-D form)
+// Both maps of a launch; 3-D when the driver accepts them, else 2-D
 static inline bool make_maps(const B2BChainParams& q, int cols, CUtensorMap* mx, CUtensorMap* my, int* tma3d) {
-  static const int force2d = getenv("B2B_V1_TMA") && atoi(getenv("B2B_V1_TMA")) == 2;
-  for (int three_d = force2d ? 0 : 1; three_d >= 0; --three_d) {
+  for (int three_d = 1; three_d >= 0; --three_d) {
     if (three_d && q.D == 32) continue;  // one row-block: the 2-D form already is one instruction
     bool ok = make_map(mx, q.x, q.D, q.N, q.ldx, cols, three_d != 0);
     if (ok && q.y) ok = make_map(my, q.y, q.D, q.N, q.ldy, cols, three_d != 0);
@@ -562,9 +561,7 @@ static inline int v1_geometry(int D, long long N, int nw, int cols, size_t param
   g.extra.bar_off = g.extra.param_off + (int)((param_bytes + 15) & ~(size_t)15);
   g.extra.tiles = (N + cols - 1) / cols;
   g.smem = (size_t)g.extra.bar_off + 16 * sizeof(uint64_t) + 1024;  // +1024: base alignment slack
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = b2b_sm_count();
   long long grid = sms;
   const long long want = (g.extra.tiles + nw - 1) / nw;
   if (grid > want) grid = want;

@@ -23,7 +23,7 @@ from bijectors_jl_b200 import _lib  # noqa: E402
 P = 0x10000  # a fake device address
 NS = (1000, 1 << 20)
 DS = (1, 32, 36, 128, 129, 256, 257, 747, 748, 1024, 1025, 2048, 2049)
-VALID_KINDS = {1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 12}
+VALID_KINDS = {1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 12, 13}
 
 
 def planar(inv=0):
@@ -82,6 +82,12 @@ def scale(inv=0):
     return dict(kind=_lib.SCALE_MATRIX, inverse=inv, p0=P)
 
 
+def mlp(n1, n2, H, inv=0, act=None):
+    act = _lib.ACT_TANH if act is None else act
+    return dict(kind=_lib.COUPLING_MLP, inverse=inv, p0=P, p1=P, p2=P, p3=P, i0=P, i1=P, n0=n1, n1=n2, n2=H, n3=act,
+                f0=0.01)
+
+
 def cases():
     """(name, chain, D): every chain the sweep queries, each under a unique name."""
     out = []
@@ -114,6 +120,12 @@ def cases():
                       (16, 16, 16)):
         for inv in (0, 1):
             add(f"srqs{n1}x{n2}K{K}{'-inv' if inv else ''}", [srqs(n1, n2, K, inv)], (36, 256, 257, 1024, 1025))
+    for n1, n2, H in ((1, 1, 1), (32, 32, 64), (128, 128, 256), (129, 64, 64), (64, 129, 64), (64, 64, 257),
+                      (16, 16, 0)):
+        for inv in (0, 1):
+            add(f"mlp{n1}x{n2}H{H}{'-inv' if inv else ''}", [mlp(n1, n2, H, inv)], (36, 256, 257, 1024, 1025))
+    add("mlp-leaky", [mlp(32, 32, 64, act=_lib.ACT_LEAKY_RELU)], (64, 1024))
+    add("mlp-act9", [mlp(32, 32, 64, act=9)], (64,))
     # BatchNorm neighbours folded into coupling launches
     add("bn-cpl-bn", [bn(), cpl(32, 32), bn()], (64, 256, 1024))
     add("bn-cpl", [bn(), cpl(32, 32)], (64, 1024))
@@ -130,6 +142,8 @@ def cases():
     add("srqs-scale-diag", [srqs(32, 32), scale(1), ew(), diag()], (64, 256, 257))
     add("mixed-all", [planar(), radial(1), rqs(), bn(), perm(), ew(1), cpl(16, 16), srqs(16, 16), scale(), tril()],
         (32, 64, 128, 256))
+    add("planar-bn-mlp-diag", [planar(), bn(), mlp(32, 32, 64), bn(1), diag()], (64, 128, 1024, 1025))
+    add("mlp-inv-planar-tril", [mlp(64, 64, 128, 1), planar(1), tril()], (128, 256, 257))
     add("ew9-diag", [ew()] * 9 + [diag()], (32, 1024, 1025))
     add("planar9-radial9", [planar()] * 9 + [radial()] * 9, (32, 100, 128))
     add("planar-dirs", [planar(), planar(1), planar(), planar()], (32, 100))
@@ -152,7 +166,8 @@ def cases():
     # each required pointer set to NULL in turn (an optional one too)
     for name, d in (("planar", planar()), ("radial", radial()), ("rqs", rqs()), ("cpl", cpl(16, 16)),
                     ("cpl-lists", cpl(16, 16, lists=True)), ("bn", bn()), ("perm", perm()), ("ew", ew()),
-                    ("diag", diag()), ("tril", tril()), ("srqs", srqs(16, 16)), ("scale", scale())):
+                    ("diag", diag()), ("tril", tril()), ("srqs", srqs(16, 16)), ("scale", scale()),
+                    ("mlp", mlp(16, 16, 32))):
         for f in ("p0", "p1", "p2", "p3", "i0", "i1"):
             if f in d:
                 e = dict(d)
