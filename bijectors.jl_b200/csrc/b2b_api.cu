@@ -234,8 +234,11 @@ int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D) {
   return n < 0 ? n : B2B_OK;
 }
 
-static bool tril_terminal(const b2b_layer_desc* layers, int32_t L) {
-  return layers && L >= 1 && layers[L - 1].kind == B2B_MVNORMAL_TRIL;
+// A batch sum without `logjac` over a terminal-ended chain of several launches: the launches before the last hand their
+// log-Jacobians to it through N floats of workspace (`nsegs`: the plan's launch count before BatchNorm folding, which
+// never changes whether a terminal-ended chain has more than one)
+static bool sum_needs_logjac_ws(const b2b_layer_desc* layers, int32_t L, int nsegs) {
+  return layers && L >= 1 && b2b_ends_in_terminal(layers, L) && nsegs > 1;
 }
 
 // factor storage of the dense Scale layers (one region: they run one after another); 0 for a chain without one
@@ -258,8 +261,8 @@ extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_
   if (!want_y && b2b_chain_segment_count(layers, L, D) > 1)
     bytes += align_up((size_t)D * (size_t)N * sizeof(float), 1024);
   if (want_sum) bytes += 4096 * sizeof(double);
-  // a batch sum without `logjac`: the log-Jacobians of the layers before a TRIL launch go through N floats of workspace
-  if (want_sum && tril_terminal(layers, L) && L > 1) bytes += align_up((size_t)N * sizeof(float), 1024);
+  if (want_sum && sum_needs_logjac_ws(layers, L, b2b_chain_segment_count(layers, L, D)))
+    bytes += align_up((size_t)N * sizeof(float), 1024);
   return bytes;
 }
 
@@ -292,6 +295,7 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     const int rc = plan_segments(layers, L, D, segs);
     if (rc != B2B_OK) return rc;
   }
+  const bool lj_ws = sum_out && !logjac && sum_needs_logjac_ws(layers, L, (int)segs.size());
   // workspace carve-up
   char* ws = static_cast<char*>(workspace);
   size_t ws_left = workspace ? workspace_bytes : 0;
@@ -320,12 +324,14 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
       ws_left -= want;
     }
   }
-  // fold BatchNorm neighbours (a per-row affine) into the coupling launches: removes their own pass over HBM
+  // fold BatchNorm neighbours (a per-row affine) into the coupling launches: removes their own pass over HBM.  With a
+  // batch sum, the chain's last fused launch is never emptied: the sum comes from it.
   if (fold_ws && g_fold_bn) {
     for (size_t s = 0; s < segs.size(); ++s) {
       if (segs[s].launch != B2B_LC_COUPLING) continue;
+      const bool keeps_sum = sum_out && s + 2 == segs.size() && segs[s + 1].end - segs[s + 1].begin == 1;
       if (s + 1 < segs.size() && segs[s + 1].launch != B2B_LC_COUPLING && segs[s + 1].end > segs[s + 1].begin &&
-          layers[segs[s + 1].begin].kind == B2B_BATCHNORM)
+          layers[segs[s + 1].begin].kind == B2B_BATCHNORM && !keeps_sum)
         segs[s].post = segs[s + 1].begin++;
       if (s > 0 && segs[s - 1].launch != B2B_LC_COUPLING && segs[s - 1].end > segs[s - 1].begin &&
           layers[segs[s - 1].end - 1].kind == B2B_BATCHNORM)
@@ -344,8 +350,8 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     ws += need;
     ws_left -= need;
   }
-  if (sum_out && !logjac && L > 1 && tril_terminal(layers, L)) {
-    // the layers before the TRIL launch hand their log-Jacobians to it through N floats of workspace
+  if (lj_ws) {
+    // the launches before the last hand their log-Jacobians to it through N floats of workspace
     const size_t need = align_up((size_t)N * sizeof(float), 1024);
     if (ws_left < need) return B2B_EWORKSPACE;
     logjac = reinterpret_cast<float*>(ws);
@@ -362,7 +368,8 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
 
   const float* cur = x;
   long long cur_ld = ldx;
-  bool lj_started = accumulate_logjac != 0;
+  // accumulate_logjac adds onto the caller's logjac; the workspace slice is written by the first launch
+  bool lj_started = accumulate_logjac != 0 && !lj_ws;
   for (size_t s = 0; s < segs.size(); ++s) {
     const bool last_seg = s + 1 == segs.size();
     // destination of this segment: y when given, else scratch for intermediates, nothing for the last

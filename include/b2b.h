@@ -203,9 +203,12 @@ const char* b2b_status_string(int status);
  * preceding layers (which write the recovered x to y, or to the D x N scratch of the workspace when y == NULL), so it costs
  * 8·D B/sample more HBM traffic than a terminal fused into the last column-local launch; the launch stages the packed lower
  * triangle of L in shared memory (Float32 D <= 256, B2B_EUNSUPPORTED beyond, nothing launched) and is bound by the
- * D(D+1)/2 FP32 FMA per sample of the whitening solve L⁻¹(x − mu).  With layers before it, sum_out needs `logjac`
- * (without it the log-Jacobians of the preceding layers travel through an N-float slice of the workspace, which
- * b2b_chain_workspace_bytes includes for a TRIL-terminated chain of several elements when want_sum != 0).
+ * D(D+1)/2 FP32 FMA per sample of the whitening solve L⁻¹(x − mu).
+ * A batch sum without `logjac` (sum_out != NULL, logjac == NULL) needs the chain to end in either terminal.  When such a
+ * chain takes more than one launch, the log-Jacobians of the launches before the last travel through an N-float slice of
+ * the workspace, which b2b_chain_workspace_bytes includes when want_sum != 0 (align_up(4·N, 1024) bytes); the first
+ * launch writes that slice, so accumulate_logjac has no effect, as everywhere `logjac` is NULL.
+ * With a batch sum, a BatchNorm that is the chain's last launch on its own is not folded into the coupling before it.
  * workspace: device scratch of at least b2b_chain_workspace_bytes(...) bytes (may be NULL when 0).
  */
 int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const float* x, float* y, float* logjac,

@@ -1,10 +1,12 @@
 """Float64 restatements of the reverse mode of the elementwise layers (Stacked laws, Permute), of the terminal MvNormal and
-of whole mixed chains -- the references of b2b_chain_vjp_f32.  They compose the per-kind VJPs of oracle/oracle_np.py and
-are themselves checked against central finite differences (tests/test_oracle_chain_vjp.py)."""
+of whole mixed chains of every layer kind, closed by either terminal -- the references of b2b_chain_vjp_f32.  They
+compose the per-kind VJPs of oracle/oracle_np.py and of the spline / MLP coupling and dense Scale references, and are
+themselves checked against central finite differences (tests/test_oracle_chain_vjp.py)."""
 from __future__ import annotations
 
 import numpy as np
 
+import mvnormal_tril_oracle as T
 from oracle import oracle_np as O
 
 EW = O.EW
@@ -88,9 +90,13 @@ def mvnormal_diag_logpdf_vjp(mu, sigma, x, lpbar):
     return -g, g.sum(axis=1), (lb * (q * q - 1) / sigma[:, None]).sum(axis=1)
 
 
-def _layer_vjp(lay: O.Layer, inv: bool, x, ybar, ljbar):
-    """(x̄, parameter cotangents as a dict keyed like the device grads) of one oracle layer applied to x."""
-    p, k = lay.params, lay.kind
+def _layer_vjp(lay, inv: bool, x, ybar, ljbar):
+    """(x̄, parameter cotangents as a dict keyed like the device grads) of one oracle layer applied to x: an O.Layer, or a
+    SplineLayer / MLPLayer / ScaleLayer, whose own .vjp evaluates in x's dtype."""
+    k = lay.kind
+    if k in ("coupling_rqs", "coupling_mlp", "scale_matrix"):
+        return lay.vjp(x, ybar, ljbar, inverse=inv)
+    p = lay.params
     if k == "planar":
         fn = O.planar_inverse_chain_vjp if inv else O.planar_chain_vjp
         xb, g = fn([(p["w"], p["u"], p["b"])], x, ybar, ljbar)
@@ -114,11 +120,14 @@ def _layer_vjp(lay: O.Layer, inv: bool, x, ybar, ljbar):
     raise ValueError(k)
 
 
-def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, terminal=False, dtype=np.float64):
+def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, terminal=False, dtype=np.float64,
+              scale_tril=None):
     """Reverse mode of a chain applied in the given order (layer l inverted when inverse_flags[l]), optionally closed by
-    the terminal MvNormal(μ, σ) (then the log-Jacobian output is logpdf).  ybar (D, N) or None (zeros), ljbar (N,).
+    a terminal MvNormal (then the log-Jacobian output is logpdf): MvNormal(μ, Diagonal(σ²)) when ``terminal``, or
+    MvNormal(μ, L Lᵀ) when ``scale_tril`` = L is given.  ybar (D, N) or None (zeros), ljbar (N,) or None (zeros).
     Evaluated in `dtype` (float32 gives the reference's own float32 error for the parity gate).
-    Returns (x̄, [grads dict per layer], {"μ": …, "σ": …} or {})."""
+    Returns (x̄, [grads dict per layer], the base's cotangents: {"μ": …, "σ": …} / {"μ": …, "L": …}, μ̄ and σ̄ only for
+    a given μ / σ; {} without a terminal)."""
     x = np.asarray(x, dtype)
     N = x.shape[1]
     lb = np.zeros(N, dtype) if ljbar is None else np.asarray(ljbar, dtype)
@@ -128,8 +137,15 @@ def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, termin
         cur = (lay.inverse if inv else lay.forward)(cur)[0]
     g = np.zeros_like(cur) if ybar is None else np.asarray(ybar, dtype)
     base = {}
-    if terminal:
-        gx, gm, gs = mvnormal_diag_logpdf_vjp(mu, sigma, cur, lb)
+    if scale_tril is not None:
+        gx, gm, gL = T.logpdf_vjp(scale_tril, mu, cur, lb, dtype)
+        g = g + gx
+        if mu is not None:
+            base["μ"] = gm
+        base["L"] = gL
+    elif terminal:
+        mu_, sigma_ = (None if v is None else np.asarray(v, dtype) for v in (mu, sigma))
+        gx, gm, gs = mvnormal_diag_logpdf_vjp(mu_, sigma_, cur, lb)
         g = g + gx
         if mu is not None:
             base["μ"] = gm
@@ -141,12 +157,15 @@ def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, termin
     return g, grads, base
 
 
-def chain_logjac(layers, inverse_flags, x, mu=None, sigma=None, terminal=False):
-    """(y, logjac or logpdf) of the same chain in float64 (for finite differences)."""
-    cur, lj = np.asarray(x, np.float64), 0.0
+def chain_logjac(layers, inverse_flags, x, mu=None, sigma=None, terminal=False, dtype=np.float64, scale_tril=None):
+    """(y, logjac or logpdf) of the same chain, in `dtype` (float64 for finite differences and references, float32 for
+    the reference's own error); the terminal as in chain_vjp."""
+    cur, lj = np.asarray(x, dtype), 0.0
     for lay, inv in zip(layers, inverse_flags):
         cur, l = (lay.inverse if inv else lay.forward)(cur)
         lj = lj + l
-    if terminal:
-        lj = lj + O.mvnormal_diag_logpdf(mu, sigma, cur)
-    return cur, lj
+    if scale_tril is not None:
+        lj = lj + T.logpdf(scale_tril, mu, cur, dtype)
+    elif terminal:
+        lj = lj + O.mvnormal_diag_logpdf(*(None if v is None else np.asarray(v, dtype) for v in (mu, sigma)), cur)
+    return cur, np.asarray(lj, dtype)

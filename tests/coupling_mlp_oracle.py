@@ -91,4 +91,5 @@ class MLPLayer:
         return inverse(*self.args, y, y.dtype)
 
     def vjp(self, x, ybar, ljbar, inverse=False):
-        return vjp(*self.args, x, ybar, ljbar, inverse)
+        x = np.asarray(x)
+        return vjp(*self.args, x, ybar, ljbar, inverse, x.dtype)

@@ -6,13 +6,12 @@
     x̄ = ȳ − l̄·s,   μ̄ = Σₙ l̄ₙ sₙ,   L̄ = tril(Σₙ l̄ₙ sₙ rₙᵀ) − (Σₙ l̄ₙ)·diag(1/Lᵢᵢ)
 
 Every function takes a ``dtype``: float32 evaluates the same formulas in float32 (LAPACK's strtrs), which gives the
-reference's own float32 error for the parity gates.  Chains before the terminal use tests/chain_vjp_oracle.py."""
+reference's own float32 error for the parity gates.  Whole chains closed by this terminal are chain_vjp_oracle's
+chain_logjac / chain_vjp with ``scale_tril``."""
 import math
 
 import numpy as np
 from scipy.linalg import solve_triangular
-
-import chain_vjp_oracle as V
 
 
 def _prep(L, mu, x, dtype):
@@ -47,33 +46,6 @@ def sample(L, mu, z):
     L = np.tril(np.asarray(L, np.float64))
     y = L @ np.asarray(z, np.float64)
     return y if mu is None else y + np.asarray(mu, np.float64)[:, None]
-
-
-def chain_logpdf(layers, flags, x, L, mu, dtype=np.float64):
-    """The chain (layer l inverted when flags[l]) closed by the terminal MvNormal(μ, L Lᵀ): logpdf + logjac."""
-    cur, lj = np.asarray(x, dtype), 0.0
-    for lay, inv in zip(layers, flags):
-        cur, l = (lay.inverse if inv else lay.forward)(cur)
-        lj = lj + l
-    return logpdf(L, mu, cur, dtype) + lj
-
-
-def chain_vjp(layers, flags, x, ybar, ljbar, L, mu, dtype=np.float64):
-    """Reverse mode of chain_logpdf: (x̄, [grads dict per layer], {"μ": …, "L": …}); ``ybar`` is the cotangent of the
-    recovered point the terminal sees (None = zeros), μ̄ only when ``mu`` is given."""
-    x = np.asarray(x, dtype)
-    lb = np.asarray(ljbar, dtype)
-    inputs, cur = [], x
-    for lay, inv in zip(layers, flags):
-        inputs.append(cur)
-        cur = (lay.inverse if inv else lay.forward)(cur)[0]
-    gx, gm, gL = logpdf_vjp(L, mu, cur, lb, dtype)
-    g = gx if ybar is None else np.asarray(ybar, dtype) + gx
-    base = {"L": gL} if mu is None else {"μ": gm, "L": gL}
-    grads = [None] * len(layers)
-    for l in reversed(range(len(layers))):
-        g, grads[l] = V._layer_vjp(layers[l], flags[l], inputs[l], g, lb)
-    return g, grads, base
 
 
 def random_tril(rng, D, cond=1.0, dtype=np.float64):

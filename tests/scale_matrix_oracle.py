@@ -25,19 +25,21 @@ def inverse(A, y, dtype=np.float64):
     return np.linalg.solve(A, y), np.full(N, -logabsdet(A), dtype)
 
 
-def vjp(A, x, ybar, ljbar, inverse=False):
+def vjp(A, x, ybar, ljbar, inverse=False, dtype=np.float64):
     """(x̄, Ā) of with_logabsdet_jacobian(Scale(A), x) (inverse=False) or of Inverse(Scale(A)) (inverse=True) at x (D, N);
-    ybar (D, N) / ljbar (N,) may be None (zeros)."""
-    A = np.asarray(A, np.float64)
-    x = np.asarray(x, np.float64)
+    ybar (D, N) / ljbar (N,) may be None (zeros).  Float64 by default; float32 restates the same formulas in float32 (the
+    parity gates' own-error term)."""
+    dt = np.dtype(dtype)
+    A = np.asarray(A, dt)
+    x = np.asarray(x, dt)
     D, N = x.shape
-    yb = np.zeros((D, N)) if ybar is None else np.asarray(ybar, np.float64)
-    s = 0.0 if ljbar is None else float(np.sum(np.asarray(ljbar, np.float64)))
+    yb = np.zeros((D, N), dt) if ybar is None else np.asarray(ybar, dt)
+    s = dt.type(0) if ljbar is None else np.sum(np.asarray(ljbar, dt), dtype=dt)
     Bm = np.linalg.inv(A).T
     G = yb @ x.T
     if not inverse:
-        return A.T @ yb, G + s * Bm
-    return Bm @ yb, -Bm @ G @ Bm - s * Bm
+        return A.T @ yb, (G + s * Bm).astype(dt)
+    return (Bm @ yb).astype(dt), (-Bm @ G @ Bm - s * Bm).astype(dt)
 
 
 class ScaleLayer:
@@ -55,7 +57,8 @@ class ScaleLayer:
         return inverse(self.A, y, y.dtype)
 
     def vjp(self, x, ybar, ljbar, inverse=False):
-        xb, Ab = vjp(self.A, x, ybar, ljbar, inverse)
+        x = np.asarray(x)
+        xb, Ab = vjp(self.A, x, ybar, ljbar, inverse, x.dtype)
         return xb, dict(a=Ab)
 
 

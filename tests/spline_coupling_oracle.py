@@ -139,5 +139,6 @@ class SplineLayer:
         return inverse(self.idx1, self.idx2, self.Wm, self.c, self.K, self.B, y, y.dtype)
 
     def vjp(self, x, ybar, ljbar, inverse=False):
-        xb, Wb, cb = vjp(self.idx1, self.idx2, self.Wm, self.c, self.K, self.B, x, ybar, ljbar, inverse)
+        x = np.asarray(x)
+        xb, Wb, cb = vjp(self.idx1, self.idx2, self.Wm, self.c, self.K, self.B, x, ybar, ljbar, inverse, x.dtype)
         return xb, dict(W=Wb, c=cb)

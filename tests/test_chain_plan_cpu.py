@@ -145,6 +145,12 @@ def cases():
     add("planar-bn-mlp-diag", [planar(), bn(), mlp(32, 32, 64), bn(1), diag()], (64, 128, 1024, 1025))
     add("mlp-inv-planar-tril", [mlp(64, 64, 128, 1), planar(1), tril()], (128, 256, 257))
     add("ew9-diag", [ew()] * 9 + [diag()], (32, 1024, 1025))
+    # a batch sum without logjac over a DIAG-terminated chain of several launches (N floats of log-Jacobian workspace)
+    add("cpl-diag", [cpl(32, 32), diag()], (64, 256, 1024))
+    add("mlp-ew-diag", [mlp(32, 32, 64), ew(), diag()], (64, 256, 1024))
+    add("bn-cpl-bn-diag", [bn(), cpl(32, 32), bn(), diag()], (64, 256))
+    add("srqs-diag", [srqs(32, 32), diag()], (64, 256))
+    add("scale-diag", [scale(1), diag()], (64, 256))
     add("planar9-radial9", [planar()] * 9 + [radial()] * 9, (32, 100, 128))
     add("planar-dirs", [planar(), planar(1), planar(), planar()], (32, 100))
     # runs split at the fused kernels' shared-memory budget

@@ -278,21 +278,11 @@ def test_logpdf_and_vjp(B, base):
     # reverse mode: ȳ and the four cotangents of both MLP layers
     lb = rng.standard_normal(N)
     ybar, fgrads, _ = B.logpdf_vjp(td, yd, torch.from_numpy(lb.astype(f32)).cuda())
-    inputs, cur = [], y.astype(np.float64)
-    for lay in inv_layers:
-        inputs.append(cur)
-        cur = lay.inverse(cur)[0]
+    flags = [True] * len(inv_layers)
     if base == "diag":
-        g = V.mvnormal_diag_logpdf_vjp(mu.astype(np.float64), sigma.astype(np.float64), cur, lb)[0]
+        g, grads, _ = V.chain_vjp(inv_layers, flags, y, None, lb, mu, sigma, terminal=True)
     else:
-        g = T.logpdf_vjp(L, mu, cur, lb)[0]
-    grads = [None] * len(inv_layers)
-    for l in reversed(range(len(inv_layers))):
-        lay = inv_layers[l]
-        if isinstance(lay, M.MLPLayer):
-            g, grads[l] = lay.vjp(inputs[l], g, lb, inverse=True)
-        else:
-            g, grads[l] = V._layer_vjp(lay, True, inputs[l], g, lb)
+        g, grads, _ = V.chain_vjp(inv_layers, flags, y, None, lb, mu, scale_tril=L)
     assert rel(B.to_numpy(ybar), g) < 1e-4
     flow_grads = grads[::-1]  # flow order
     for k in (0, 3):

@@ -7,6 +7,7 @@ import math
 import numpy as np
 import pytest
 
+import chain_vjp_oracle as V
 import mvnormal_tril_oracle as T
 from oracle import oracle_np as O
 
@@ -124,7 +125,8 @@ def test_logpdf_after_inverse_chain(B, kind, D, N):
     flow, ol, flags = chain(B, kind, D, rng)
     td = B.transformed(base(B, L, mu), flow)
     lp = B.to_numpy(B.logpdf(td, B.from_numpy(y)))
-    gate(lp, T.chain_logpdf(ol, flags, y, L, mu), T.chain_logpdf(ol, flags, y.astype(f32), L, mu, np.float32), kind)
+    gate(lp, V.chain_logjac(ol, flags, y, mu, scale_tril=L)[1],
+         V.chain_logjac(ol, flags, y.astype(f32), mu, dtype=np.float32, scale_tril=L)[1], kind)
     s, lp2 = B.logpdf_sum(td, B.from_numpy(y))
     assert abs(float(s) - float(lp2.double().sum())) <= 1e-9 * max(1.0, abs(float(s)))
 
@@ -190,8 +192,8 @@ def check_vjp(B, td, ol, flags, y, lb, L, mu):
     import torch
 
     yb, flow_g, base_g = B.logpdf_vjp(td, B.from_numpy(y), torch.from_numpy(lb.astype(f32)).cuda())
-    o64 = T.chain_vjp(ol, flags, y, None, lb, L, mu)
-    o32 = T.chain_vjp(ol, flags, y.astype(f32), None, lb, L, mu, np.float32)
+    o64 = V.chain_vjp(ol, flags, y, None, lb, mu, scale_tril=L)
+    o32 = V.chain_vjp(ol, flags, y.astype(f32), None, lb, mu, dtype=np.float32, scale_tril=L)
     gate(B.to_numpy(yb), o64[0], o32[0], "x̄")
     assert set(base_g) == set(o64[2])
     for k in base_g:
@@ -279,8 +281,8 @@ def test_flow_routes_mu_and_L(B):
     assert bse.mu.data_ptr() in ptrs and bse._tril.data_ptr() in ptrs
     F.nll(B.from_numpy(y)).backward()
     lb = np.full(N, -1.0)
-    o64 = T.chain_vjp(ol, flags, y, None, lb, L, mu)
-    o32 = T.chain_vjp(ol, flags, y.astype(f32), None, lb, L, mu, np.float32)
+    o64 = V.chain_vjp(ol, flags, y, None, lb, mu, scale_tril=L)
+    o32 = V.chain_vjp(ol, flags, y.astype(f32), None, lb, mu, dtype=np.float32, scale_tril=L)
     gate(ptrs[bse.mu.data_ptr()].grad.cpu().numpy(), o64[2]["μ"], o32[2]["μ"], "μ")
     gate(ptrs[bse._tril.data_ptr()].grad.t().cpu().numpy(), o64[2]["L"], o32[2]["L"], "L")
 
@@ -478,7 +480,7 @@ def test_batch_sum_without_logjac_after_layers(B):
     rc = lib.b2b_chain_run_f32(arr, len(descs), yd.data_ptr(), None, None, s.data_ptr(), D, N, D, D, 0, ws.data_ptr(), ws_b,
                                stream())
     assert rc == 0
-    ref = float(T.chain_logpdf(ol, flags, y, L, mu).sum())
+    ref = float(V.chain_logjac(ol, flags, y, mu, scale_tril=L)[1].sum())
     s_lj, _ = B.logpdf_sum(B.transformed(bse, flow), yd)
     assert float(s) == float(s_lj)
     assert abs(float(s) - ref) <= 1e-5 * abs(ref)
@@ -514,10 +516,10 @@ def test_float64_run_and_vjp(B, D):
     yd = B.from_numpy(y, dtype=np.float64)
     lp = B.logpdf(td, yd)
     assert lp.dtype == torch.float64
-    assert rel(lp.cpu().numpy(), T.chain_logpdf(ol, flags, y, L, mu)) <= TOL64
+    assert rel(lp.cpu().numpy(), V.chain_logjac(ol, flags, y, mu, scale_tril=L)[1]) <= TOL64
     lb = rng.standard_normal(N)
     yb, flow_g, base_g = B.logpdf_vjp(td, yd, torch.from_numpy(lb).cuda())
-    o = T.chain_vjp(ol, flags, y, None, lb, L, mu)
+    o = V.chain_vjp(ol, flags, y, None, lb, mu, scale_tril=L)
     assert rel(B.to_numpy(yb), o[0]) <= TOL64
     assert rel(base_g["μ"].cpu().numpy(), o[2]["μ"]) <= TOL64
     Lb = base_g["L"].cpu().numpy()

@@ -240,9 +240,8 @@ def test_logpdf_and_chain_vjp(B, base):
     yd = B.from_numpy(y)
     lp = B.to_numpy(B.logpdf(td, yd))
     inv_layers = ora[::-1]
-    cur, lj, inputs = y.astype(np.float64), 0.0, []
+    cur, lj = y.astype(np.float64), 0.0
     for lay in inv_layers:
-        inputs.append(cur)
         cur, l = lay.inverse(cur)
         lj = lj + l
     if base == "diag":
@@ -255,17 +254,11 @@ def test_logpdf_and_chain_vjp(B, base):
     assert abs(float(s) - lp64.sum()) <= 1e-5 * abs(lp64.sum())
     lb = rng.standard_normal(N)
     ybar, fgrads, _ = B.logpdf_vjp(td, yd, torch.from_numpy(lb.astype(f32)).cuda())
+    flags = [True] * len(inv_layers)
     if base == "diag":
-        g = V.mvnormal_diag_logpdf_vjp(mu.astype(np.float64), sigma.astype(np.float64), cur, lb)[0]
+        g, grads, _ = V.chain_vjp(inv_layers, flags, y, None, lb, mu, sigma, terminal=True)
     else:
-        g = T.logpdf_vjp(L, mu, cur, lb)[0]
-    grads = [None] * len(inv_layers)
-    for l in reversed(range(len(inv_layers))):
-        lay = inv_layers[l]
-        if isinstance(lay, (S.ScaleLayer, SC.SplineLayer)):
-            g, grads[l] = lay.vjp(inputs[l], g, lb, inverse=True)
-        else:
-            g, grads[l] = V._layer_vjp(lay, True, inputs[l], g, lb)
+        g, grads, _ = V.chain_vjp(inv_layers, flags, y, None, lb, mu, scale_tril=L)
     assert rel(B.to_numpy(ybar), g) < 1e-3
     flow_grads = grads[::-1]
     for k in (3, 7):
