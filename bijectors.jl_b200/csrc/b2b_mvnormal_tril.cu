@@ -331,9 +331,11 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
 
 // ---- L̄ = tril(S Rᵀ) over column chunks: CTA (tile, p) writes the 64 x 64 tile of Σ_{n in chunk p} S[:, n] R[:, n]ᵀ
 // to part[p] (D x D, column-major): with `lower` the lower-triangle tiles only, whose diagonal tiles also write the
-// chunk's row sums of S (μ̄) to mup[p] when it is given; otherwise every tile (dense Scale's G = Σ ȳ uᵀ).  fp32 FMA within
-// a chunk, fp64 across chunks (finalize_kernel).
-constexpr int kTile = 64, kBK = 16, kChunk = 4096, kMaxChunks = 64;
+// chunk's row sums of S (μ̄) to mup[p] when it is given; otherwise every tile (dense Scale's G = Σ ȳ uᵀ).  fp32 FMA over
+// blocks of kFlush stages (16 384 columns), fp64 across the blocks of a chunk and across chunks (finalize_kernel): a chunk
+// holds up to N / kMaxChunks columns (65 536 at N = 2²²), and one fp32 sum over all of them loses ~1e-5 relative.  Up to
+// N = 2²⁰ a chunk is one block.
+constexpr int kTile = 64, kBK = 16, kChunk = 4096, kMaxChunks = 64, kFlush = 1024;
 
 __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S, long long lds, const float* __restrict__ Rm,
                                                     long long ldr, float* __restrict__ part, float* __restrict__ mup, int D,
@@ -355,32 +357,42 @@ __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S,
   const long long n0 = (long long)p * clen, n1 = n0 + clen < N ? n0 + clen : N;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int lk = threadIdx.x >> 4, lr = (threadIdx.x & 15) * 4;  // loader: column lk of the stage, rows lr..lr+3
-  float acc[4][4] = {};
-  float msum = 0.f;
-  for (long long nb = n0; nb < n1; nb += kBK) {
-    const long long n = nb + lk;
+  double accd[4][4] = {};
+  double msumd = 0.0;
+  for (long long nf = n0; nf < n1; nf += (long long)kFlush * kBK) {
+    const long long nf1 = nf + (long long)kFlush * kBK < n1 ? nf + (long long)kFlush * kBK : n1;
+    float acc[4][4] = {};
+    float msum = 0.f;
+    for (long long nb = nf; nb < nf1; nb += kBK) {
+      const long long n = nb + lk;
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int ia = i0 + lr + q, ja = j0 + lr + q;
-      As[lk][lr + q] = (n < n1 && ia < D) ? S[n * lds + ia] : 0.f;
-      Bs[lk][lr + q] = (n < n1 && ja < D) ? Rm[n * ldr + ja] : 0.f;
+      for (int q = 0; q < 4; ++q) {
+        const int ia = i0 + lr + q, ja = j0 + lr + q;
+        As[lk][lr + q] = (n < nf1 && ia < D) ? S[n * lds + ia] : 0.f;
+        Bs[lk][lr + q] = (n < nf1 && ja < D) ? Rm[n * ldr + ja] : 0.f;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < kBK; ++k) {
+        const float4 a = *reinterpret_cast<const float4*>(&As[k][ty * 4]);
+        const float4 b = *reinterpret_cast<const float4*>(&Bs[k][tx * 4]);
+        const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+#pragma unroll
+          for (int v = 0; v < 4; ++v) acc[u][v] = fmaf(av[u], bv[v], acc[u][v]);
+      }
+      if (diag && threadIdx.x < kTile) {
+#pragma unroll
+        for (int k = 0; k < kBK; ++k) msum += As[k][threadIdx.x];
+      }
+      __syncthreads();
     }
-    __syncthreads();
 #pragma unroll
-    for (int k = 0; k < kBK; ++k) {
-      const float4 a = *reinterpret_cast<const float4*>(&As[k][ty * 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&Bs[k][tx * 4]);
-      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+    for (int u = 0; u < 4; ++u)
 #pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) acc[u][v] = fmaf(av[u], bv[v], acc[u][v]);
-    }
-    if (diag && threadIdx.x < kTile) {
-#pragma unroll
-      for (int k = 0; k < kBK; ++k) msum += As[k][threadIdx.x];
-    }
-    __syncthreads();
+      for (int v = 0; v < 4; ++v) accd[u][v] += (double)acc[u][v];
+    msumd += (double)msum;
   }
   float* P = part + (size_t)p * D * D;
 #pragma unroll
@@ -388,9 +400,9 @@ __global__ void __launch_bounds__(256) outer_kernel(const float* __restrict__ S,
 #pragma unroll
     for (int v = 0; v < 4; ++v) {
       const int i = i0 + ty * 4 + u, j = j0 + tx * 4 + v;
-      if (i < D && j < D && (i >= j || !lower)) P[(size_t)j * D + i] = acc[u][v];
+      if (i < D && j < D && (i >= j || !lower)) P[(size_t)j * D + i] = (float)accd[u][v];
     }
-  if (diag && threadIdx.x < kTile && i0 + (int)threadIdx.x < D) mup[(size_t)p * D + i0 + threadIdx.x] = msum;
+  if (diag && threadIdx.x < kTile && i0 + (int)threadIdx.x < D) mup[(size_t)p * D + i0 + threadIdx.x] = (float)msumd;
 }
 
 // L̄ (D x D column-major, exactly zero above the diagonal) and μ̄ from the chunk partials, in chunk order

@@ -111,7 +111,7 @@ def find_alpha_partials(alpha, wt_u_hat, b):
     return x, -np.tanh(alpha + b) * x, x - 1.0
 
 
-def planar_chain_vjp(params, x, ybar, ljbar):
+def planar_chain_vjp(params, x, ybar, ljbar, b_terms=None):
     """Vector-Jacobian product of a ∘-chain of PlanarLayers (forward direction) -- what reverse-mode AD of
     with_logabsdet_jacobian (src/bijectors/planar_layer.jl:73-80,102-110 through get_u_hat :65-70) yields; the
     reference trains flows this way (docs/src/flows.md:93-100).
@@ -119,7 +119,7 @@ def planar_chain_vjp(params, x, ybar, ljbar):
     params: list of (w, u, b); x (D, N); ybar (D, N) cotangent of the transformed batch; ljbar (N,) cotangent of the
     accumulated logjac.  Returns (xbar (D, N), [(wbar, ubar, bbar), ...]).  Written layer by layer with stored
     activations (the plain restatement); the device kernels use the algebraically equal reorganisation described
-    in DESIGN.md."""
+    in DESIGN.md.  A list ``b_terms`` receives, per layer, the N column terms whose sum is b̄."""
     dt = x.dtype
     zs, cache = [x], []
     for (w, u, b) in params:
@@ -144,6 +144,8 @@ def planar_chain_vjp(params, x, ybar, ljbar):
         c_bar = np.sum(ljbar * s2 / den)                 # ∂ log1p(c·s2)/∂c
         w_bar = z @ g                                    # direct dependence a = wᵀz + b
         b_bar = np.sum(g)
+        if b_terms is not None:
+            b_terms.insert(0, g)
         yb = yb + w[:, None] * g[None, :]
         # through get_u_hat: û = u + k(s, q)·w, k = (log1pexp(−s) − 1)/q, s = wᵀu, q = wᵀw; c = log1pexp(s) − 1
         s_ = dt.type(np.dot(w, u))
@@ -174,7 +176,7 @@ def _get_u_hat_pullback(w, u, uhat_bar, c_bar, dt):
     return w_bar, u_bar
 
 
-def planar_inverse_chain_vjp(params, y, xbar, ljbar):
+def planar_inverse_chain_vjp(params, y, xbar, ljbar, b_terms=None):
     """Vector-Jacobian product of with_logabsdet_jacobian(inverse(f_L ∘ … ∘ f_1), y) -- the computation under
     ``logpdf(transformed(d, flow), y)`` that the reference's training example differentiates
     (docs/src/flows.md:66-100).  Inverse layers are applied in the order L, L−1, …, 1 (planar_layer.jl:112-127); α comes
@@ -182,7 +184,8 @@ def planar_inverse_chain_vjp(params, y, xbar, ljbar):
     (ext/BijectorsChainRulesCoreExt.jl:42-46, restated in find_alpha_partials).
 
     params: [(w, u, b)] in FORWARD order; y (D, N); xbar (D, N) cotangent of the recovered x; ljbar (N,) cotangent of the
-    accumulated (inverse) logjac.  Returns (ybar, [(wbar, ubar, bbar), ...]) in forward order."""
+    accumulated (inverse) logjac.  Returns (ybar, [(wbar, ubar, bbar), ...]) in forward order.  A list ``b_terms``
+    receives, per layer in forward order, the N column terms whose sum is b̄."""
     dt = y.dtype
     L = len(params)
     us, cache = [y], []
@@ -213,6 +216,8 @@ def planar_inverse_chain_vjp(params, y, xbar, ljbar):
         t_bar = a_bar * pt
         c_bar = np.sum(a_bar * pc) + c_bar_direct
         b_bar = np.sum(a_bar * (1 + pb))                    # a = α + b: direct + through α
+        if b_terms is not None:
+            b_terms.append(a_bar * (1 + pb))  # k = L−1 … 0 runs over l = 0 … L−1
         w_bar = inp @ t_bar
         zb = zb + w[:, None] * t_bar[None, :]
         gw, gu = _get_u_hat_pullback(w, u, uhat_bar, c_bar, dt)

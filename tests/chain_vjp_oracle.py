@@ -90,16 +90,17 @@ def mvnormal_diag_logpdf_vjp(mu, sigma, x, lpbar):
     return -g, g.sum(axis=1), (lb * (q * q - 1) / sigma[:, None]).sum(axis=1)
 
 
-def _layer_vjp(lay, inv: bool, x, ybar, ljbar):
+def _layer_vjp(lay, inv: bool, x, ybar, ljbar, b_terms=None):
     """(x̄, parameter cotangents as a dict keyed like the device grads) of one oracle layer applied to x: an O.Layer, or a
-    SplineLayer / MLPLayer / ScaleLayer, whose own .vjp evaluates in x's dtype."""
+    SplineLayer / MLPLayer / ScaleLayer, whose own .vjp evaluates in x's dtype.  A planar layer appends the N column
+    terms of its b̄ to the list ``b_terms`` when one is given."""
     k = lay.kind
     if k in ("coupling_rqs", "coupling_mlp", "scale_matrix"):
         return lay.vjp(x, ybar, ljbar, inverse=inv)
     p = lay.params
     if k == "planar":
         fn = O.planar_inverse_chain_vjp if inv else O.planar_chain_vjp
-        xb, g = fn([(p["w"], p["u"], p["b"])], x, ybar, ljbar)
+        xb, g = fn([(p["w"], p["u"], p["b"])], x, ybar, ljbar, b_terms=b_terms)
         return xb, dict(w=g[0][0], u=g[0][1], b=g[0][2])
     if k == "radial":
         xb, g = O.radial_chain_vjp_dir([(p["alpha_raw"], p["beta"], p["z0"])], [inv], x, ybar, ljbar)
@@ -121,13 +122,14 @@ def _layer_vjp(lay, inv: bool, x, ybar, ljbar):
 
 
 def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, terminal=False, dtype=np.float64,
-              scale_tril=None):
+              scale_tril=None, b_terms=None):
     """Reverse mode of a chain applied in the given order (layer l inverted when inverse_flags[l]), optionally closed by
     a terminal MvNormal (then the log-Jacobian output is logpdf): MvNormal(μ, Diagonal(σ²)) when ``terminal``, or
     MvNormal(μ, L Lᵀ) when ``scale_tril`` = L is given.  ybar (D, N) or None (zeros), ljbar (N,) or None (zeros).
     Evaluated in `dtype` (float32 gives the reference's own float32 error for the parity gate).
     Returns (x̄, [grads dict per layer], the base's cotangents: {"μ": …, "σ": …} / {"μ": …, "L": …}, μ̄ and σ̄ only for
-    a given μ / σ; {} without a terminal)."""
+    a given μ / σ; {} without a terminal).  A dict ``b_terms`` receives {l: the N column terms of b̄} for every planar
+    layer l, whose sum is that layer's b̄."""
     x = np.asarray(x, dtype)
     N = x.shape[1]
     lb = np.zeros(N, dtype) if ljbar is None else np.asarray(ljbar, dtype)
@@ -153,7 +155,10 @@ def chain_vjp(layers, inverse_flags, x, ybar, ljbar, mu=None, sigma=None, termin
             base["σ"] = gs
     grads = [None] * len(layers)
     for l in reversed(range(len(layers))):
-        g, grads[l] = _layer_vjp(layers[l], inverse_flags[l], inputs[l], g, lb)
+        terms = [] if b_terms is not None and layers[l].kind == "planar" else None
+        g, grads[l] = _layer_vjp(layers[l], inverse_flags[l], inputs[l], g, lb, terms)
+        if terms:
+            b_terms[l] = terms[0]
     return g, grads, base
 
 
