@@ -67,6 +67,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_COUPLING_RQS: ok = b2b_coupling_rqs_fits(d, D); break;
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
     case B2B_COUPLING_MLP: ok = b2b_coupling_mlp_fits(d, D); break;
+    case B2B_COUPLING_MLP_RQS: ok = b2b_coupling_mlp_rqs_fits(d, D); break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
     default: break;
   }
@@ -84,6 +85,7 @@ static int vjp_envelope(const b2b_layer_desc& d, int D) {
     case B2B_COUPLING_RQS:
     case B2B_SCALE_MATRIX:
     case B2B_COUPLING_MLP:
+    case B2B_COUPLING_MLP_RQS:
     case B2B_MVNORMAL_TRIL: return fwd_envelope(d, D);
     default: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
   }
@@ -782,7 +784,7 @@ size_t seg_param_floats(const b2b_layer_desc* layers, const VSeg& s, int D) {
     case B2B_VC_RQS: return 3 * r((size_t)D * d.n0);
     case B2B_VC_COUPLING: return r((size_t)2 * d.n0 * d.n1) + r((size_t)2 * d.n0);
     case B2B_VC_BN: return 2 * r(D);
-    case B2B_VC_SPLINE: return r((size_t)(3 * d.n2 - 1) * d.n0 * d.n1) + r((size_t)(3 * d.n2 - 1) * d.n0);
+    case B2B_VC_SPLINE: return r(b2b_slot_len(d, 0, D)) + r(b2b_slot_len(d, 1, D));  // W̄ / c̄ sent to scratch
     default: return 0;
   }
 }

@@ -9,8 +9,14 @@
 // of rqs_element in a table row of its own, and evaluates the element with rqs_element (b2b_device.cuh), the same element
 // function the fused RQS programs use.  The log-Jacobian is summed over the rows in increasing order by the column's
 // thread, so it is deterministic.  x₂ and x₃ rows are copied bit-exactly (nothing is copied in place).
+//
+// The neural spline coupling, B2B_COUPLING_MLP_RQS, is the instantiation MLP = true: v = W₂·σ.(W₁·x₂ + c₁) + c₂.  The
+// tile's x₂ is staged where the rqs_element table and W's row block will be (neither is written before the row loop),
+// spilling past them only when they are smaller than x₂ (small K); each thread forms h = σ(W₁·x₂ + c₁) of its own column
+// into the [H][XP] block the row loop reads, and the row loop runs unchanged with (x₂, n2, W, c) := (h, H, W₂, c₂).
 #include <cuda_runtime.h>
 
+#include "b2b_coupling_mlp.cuh"
 #include "b2b_coupling_rqs.cuh"
 #include "b2b_device.cuh"
 #include "b2b_internal.h"
@@ -23,27 +29,39 @@ struct CrqParams {
   const float* x;
   float* y;
   float* logjac;
-  const float *W, *c;
+  const float *W, *c;  // MLP: W₂, c₂
   const int *idx1, *idx2;
   long long N, ldx, ldy;
   int D, n1, n2, K, accumulate;
   float B;
+  const float *W1, *c1;  // MLP only
+  int H, act;
+  float slope;
 };
 
 // floats of the per-thread rqs_element table: Sw[KP] | Sh[KP] | 2 float4 per bin
 static __host__ __device__ inline int crq_tab_floats(int K) { return 2 * rqs_kp(K + 1) + 8 * (K + 1); }
 
-template <bool INV>
+// float offset of the conditioning block Xs: after the table, W's row block and c; with the network (n2x = n2 rows of x₂
+// staged from offset 0) at least past x₂
+static __host__ __device__ inline int crq_xs_off(int nc, int K, int n2x) {
+  const int off = crq_tab_floats(K) * CRQ_TN + nc * crq_jp(K) + crq_jp(K);
+  return off > n2x * (CRQ_TN + 1) ? off : n2x * (CRQ_TN + 1);
+}
+
+template <bool INV, bool MLP>
 __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_constant__ CrqParams P) {
   extern __shared__ __align__(16) float crq_sm[];
   constexpr int TN = CRQ_TN, XP = CRQ_TN + 1;
-  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, K = P.K, K1 = K + 1, KP = rqs_kp(K1), J = 3 * K - 1;
-  const int JP = crq_jp(K), D = P.D;
+  // nc: rows of the conditioning block the row loop reads (x₂, or the hidden layer h)
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = MLP ? P.H : n2, K = P.K, K1 = K + 1, KP = rqs_kp(K1);
+  const int J = 3 * K - 1, JP = crq_jp(K), D = P.D;
   float* tab = crq_sm;                              // rqs_element table, one row per thread (Dp = TN)
-  float* Ws = tab + crq_tab_floats(K) * TN;         // [n2][JP]
-  float* cs = Ws + n2 * JP;                         // [JP]
-  float* Xs = cs + JP;                              // [n2][XP]
-  float* Pr = Xs + n2 * XP;                         // [J][TN] raw parameters
+  float* Ws = tab + crq_tab_floats(K) * TN;         // [nc][JP]
+  float* cs = Ws + nc * JP;                         // [JP]
+  float* Xs = MLP ? crq_sm + crq_xs_off(nc, K, n2) : cs + JP;  // [nc][XP]
+  float* X2 = MLP ? crq_sm : Xs;                    // [n2][XP] x₂
+  float* Pr = Xs + nc * XP;                         // [J][TN] raw parameters
   unsigned char* x1row = reinterpret_cast<unsigned char*>(Pr + J * TN);  // [D]: 1 = a transformed row
   const long long n0 = (long long)blockIdx.x * TN, n = n0 + tid;
   const int cols = (int)min((long long)TN, P.N - n0);
@@ -54,9 +72,15 @@ __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_const
   for (int i = tid; i < n1; i += TN) x1row[P.idx1[i]] = 1;
   for (int e = tid; e < n2 * TN; e += TN) {
     const int c = e / n2, m = e - c * n2;
-    Xs[m * XP + c] = c < cols ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
+    X2[m * XP + c] = c < cols ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
   }
   __syncthreads();
+  if (MLP) {  // h = σ(W₁·x₂ + c₁) of this thread's column
+    for (int m = 0; m < P.H; ++m) {
+      float dh;
+      mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, P.H, n2, X2 + tid, XP, m), Xs[m * XP + tid], dh);
+    }
+  }
   if (P.y && (P.y != P.x || P.ldy != P.ldx))  // x₂ and x₃ pass through
     for (int e = tid; e < cols * D; e += TN) {
       const int c = e / D, r = e - c * D;
@@ -70,9 +94,9 @@ __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_const
   float lj = 0.f;
   for (int i = 0; i < n1; ++i) {
     __syncthreads();  // the previous row's block of W is no longer read
-    crq_stage_row(P.W, P.c, i, n1, n2, K, Ws, cs, tid, TN);
+    crq_stage_row(P.W, P.c, i, n1, nc, K, Ws, cs, tid, TN);
     __syncthreads();
-    crq_params(Ws, cs, Xs + tid, XP, n2, K, Pr + tid, TN);
+    crq_params(Ws, cs, Xs + tid, XP, nc, K, Pr + tid, TN);
     crq_knots(Pr + tid, TN, K, P.B, Sw, 1);
     crq_knots(Pr + K * TN + tid, TN, K, P.B, Sh, 1);
     for (int k = K1; k < KP; ++k) Sw[k] = Sh[k] = inf;
@@ -100,9 +124,9 @@ __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_const
   if (active && P.logjac) P.logjac[n] = P.accumulate ? P.logjac[n] + lj : lj;
 }
 
-static size_t crq_smem_bytes(int n2, int K, int D) {
-  const int J = 3 * K - 1, JP = crq_jp(K);
-  const size_t f = (size_t)crq_tab_floats(K) * CRQ_TN + (size_t)n2 * JP + JP + (size_t)n2 * (CRQ_TN + 1) + (size_t)J * CRQ_TN;
+// nc conditioning rows; with the network, n2x = n2 rows of x₂ staged before the row loop
+static size_t crq_smem_bytes(int nc, int K, int D, int n2x) {
+  const size_t f = (size_t)crq_xs_off(nc, K, n2x) + (size_t)nc * (CRQ_TN + 1) + (size_t)(3 * K - 1) * CRQ_TN;
   return (f * sizeof(float) + D + 15) & ~(size_t)15;
 }
 
@@ -113,17 +137,27 @@ bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D) {
          d.n2 >= 2 && d.n2 <= B2B_COUPLING_RQS_MAX_K && D <= B2B_COUPLING_RQS_MAX_D;
 }
 
+bool b2b_coupling_mlp_rqs_fits(const b2b_layer_desc& d, int D) {
+  const int K = d.n3 >> 8;
+  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_MLP_RQS_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_MLP_RQS_MAX_N &&
+         d.n2 >= 1 && d.n2 <= B2B_COUPLING_MLP_RQS_MAX_H && K >= 2 && K <= B2B_COUPLING_MLP_RQS_MAX_K &&
+         D <= B2B_COUPLING_MLP_RQS_MAX_D;
+}
+
 int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
   using namespace b2b;
-  if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
+  const bool mlp = d.kind == B2B_COUPLING_MLP_RQS;
+  if (!(mlp ? b2b_coupling_mlp_rqs_fits(d, D) : b2b_coupling_rqs_fits(d, D))) return B2B_EUNSUPPORTED;
   if (N <= 0) return B2B_OK;
-  CrqParams P;
+  CrqParams P = {};
   P.x = x;
   P.y = y;
   P.logjac = logjac;
-  P.W = d.p0;
-  P.c = d.p1;
+  P.W = mlp ? d.p2 : d.p0;
+  P.c = mlp ? d.p3 : d.p1;
+  P.W1 = d.p0;
+  P.c1 = d.p1;
   P.idx1 = d.i0;
   P.idx2 = d.i1;
   P.N = N;
@@ -132,11 +166,15 @@ int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, f
   P.D = D;
   P.n1 = d.n0;
   P.n2 = d.n1;
-  P.K = d.n2;
+  P.K = mlp ? d.n3 >> 8 : d.n2;
+  P.H = d.n2;
+  P.act = d.n3 & 255;
   P.accumulate = accumulate;
-  P.B = d.f0;
-  const size_t smem = crq_smem_bytes(d.n1, d.n2, D);
-  void (*kernel)(const CrqParams) = d.inverse ? coupling_rqs_kernel<true> : coupling_rqs_kernel<false>;
+  P.B = mlp ? d.f1 : d.f0;
+  P.slope = d.f0;
+  const size_t smem = mlp ? crq_smem_bytes(P.H, P.K, D, P.n2) : crq_smem_bytes(P.n2, P.K, D, 0);
+  void (*kernel)(const CrqParams) = mlp ? (d.inverse ? coupling_rqs_kernel<true, true> : coupling_rqs_kernel<false, true>)
+                                        : (d.inverse ? coupling_rqs_kernel<true, false> : coupling_rqs_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   const long long tiles = (N + CRQ_TN - 1) / CRQ_TN;

@@ -52,6 +52,16 @@ __device__ __forceinline__ void crq_params(const float* Ws, const float* cs, con
   }
 }
 
+// The neural spline coupling's hidden pre-activation W₁·x₂ + c₁ of unit m for one column (x₂ at xcol[k·xs]): from c₁
+// (NULL: 0), FMAs over k in increasing order, so the forward and reverse-mode kernels form bit-identical values.  W₁ is
+// H x n2 column-major.
+__device__ __forceinline__ float crq_hidden_pre(const float* __restrict__ W1, const float* __restrict__ c1, int H, int n2,
+                                                const float* xcol, int xs, int m) {
+  float a = c1 ? __ldg(c1 + m) : 0.f;
+  for (int k = 0; k < n2; ++k) a = fmaf(__ldg(W1 + (size_t)k * H + m), xcol[k * xs], a);
+  return a;
+}
+
 // K + 1 knots from K raw values (stride as): out[k·os] = 2B·cumsum([0; softmax(a)])[k] − B, the max-subtracted softmax of
 // oracle_np.softmax_rows and a sequential cumsum, each product and difference rounded as the float32 restatement does.
 __device__ __forceinline__ void crq_knots(const float* a, int as, int K, float B, float* out, int os) {

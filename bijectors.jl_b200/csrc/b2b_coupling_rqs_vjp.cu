@@ -14,8 +14,14 @@
 // After each row the CTA forms the (3K − 1) x n2 block Σ_n r̄ x₂ᵀ of its tile and adds it to a private slice of the
 // workspace ([n1][3K − 1][n2] then [n1][3K − 1] for c̄), owned element by element by one thread.  A second kernel sums
 // the G slices in order into W̄ (column-major like W) and c̄.  Deterministic, no atomics, workspace independent of N.
+//
+// The neural spline coupling, B2B_COUPLING_MLP_RQS, is the instantiation MLP = true.  Each thread forms h = σ(W₁·x₂ + c₁)
+// of its column from a staged x₂ tile, and the row loop runs on h with W₂ and c₂, so its fp64 accumulator holds h̄.
+// After the loop each thread recomputes W₁x₂ + c₁ for σ′, turns h̄ into v̄ = h̄ ⊙ σ′ and forms x̄₂ = ȳ₂ + W₁ᵀv̄ in a fixed
+// order; the CTA adds Σ v̄ x₂ᵀ and Σ v̄ to its slice, laid out [W̄₂ | c̄₂ | W̄₁ ([H][n2]) | c̄₁ ([H])].
 #include <cuda_runtime.h>
 
+#include "b2b_coupling_mlp.cuh"
 #include "b2b_coupling_rqs.cuh"
 #include "b2b_device.cuh"
 #include "b2b_internal.h"
@@ -30,33 +36,42 @@ struct CrvParams {
   const float* ybar;
   const float* ljbar;
   float* xbar;
-  const float *W, *c;
+  const float *W, *c;  // MLP: W₂, c₂
   const int *idx1, *idx2;
   float* part;  // [G][slice]
   long long N, ldx, ldyb, ldxb, slice;
   int D, n1, n2, K;
   float B;
+  const float *W1, *c1;  // MLP only
+  int H, act;
+  float slope;
 };
 
-template <bool INV>
+template <bool INV, bool MLP>
 __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __grid_constant__ CrvParams P) {
   extern __shared__ __align__(16) float crv_sm[];
   constexpr int TN = CRV_TN, XP = CRV_TN + 1;
-  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, K = P.K, K1 = K + 1, J = 3 * K - 1, JP = crq_jp(K), D = P.D;
-  float* Ws = crv_sm;               // [n2][JP]
-  float* cs = Ws + n2 * JP;         // [JP]
+  // nc: rows of the conditioning block the row loop reads (x₂, or the hidden layer h)
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = MLP ? P.H : n2, K = P.K, K1 = K + 1, J = 3 * K - 1;
+  const int JP = crq_jp(K), D = P.D;
+  float* Ws = crv_sm;               // [nc][JP]
+  float* cs = Ws + nc * JP;         // [JP]
   float* KT = cs + JP;              // knots W | H | Dv, [3][K1][TN]
   float* G = KT + 3 * K1 * TN;      // their cotangents, same layout
-  float* Xs = G + 3 * K1 * TN;      // x₂ [n2][XP]
-  float* Pr = Xs + n2 * XP;         // raw parameters, then their cotangents [J][XP]
-  double* XB = reinterpret_cast<double*>(crv_sm) + ((size_t)(n2 * JP + JP + 6 * K1 * TN + n2 * XP + J * XP) + 1) / 2;
-  // x̄₂ [n2][XP] in fp64: it sums (3K − 1)·n1 products per element
-  unsigned char* kind = reinterpret_cast<unsigned char*>(XB + n2 * XP);  // [D]: 1 = x₁ row, 2 = x₂ row, 0 = x₃ row
+  float* Xs = G + 3 * K1 * TN;      // x₂ (MLP: h) [nc][XP]
+  float* Pr = Xs + nc * XP;         // raw parameters, then their cotangents [J][XP]
+  double* XB = reinterpret_cast<double*>(crv_sm) + ((size_t)(nc * JP + JP + 6 * K1 * TN + nc * XP + J * XP) + 1) / 2;
+  // x̄₂ (MLP: h̄) [nc][XP] in fp64: it sums (3K − 1)·n1 products per element
+  float* X2 = reinterpret_cast<float*>(XB + nc * XP);  // MLP: x₂ [n2][XP]
+  // [D]: 1 = x₁ row, 2 = x₂ row, 0 = x₃ row
+  unsigned char* kind = reinterpret_cast<unsigned char*>(MLP ? reinterpret_cast<void*>(X2 + n2 * XP) : XB + n2 * XP);
   float* slice = P.part + (size_t)blockIdx.x * P.slice;
-  float* cslice = slice + (size_t)n1 * J * n2;
+  float* cslice = slice + (size_t)n1 * J * nc;
+  float* w1slice = cslice + (size_t)n1 * J;  // MLP: [H][n2], then c̄₁ [H]
+  const long long slen = MLP ? (long long)n1 * J * (nc + 1) + (long long)nc * (n2 + 1) : (long long)n1 * J * (n2 + 1);
 
   for (int r = tid; r < D; r += TN) kind[r] = 0;
-  for (long long e = tid; e < (long long)n1 * J * (n2 + 1); e += TN) slice[e] = 0.f;
+  for (long long e = tid; e < slen; e += TN) slice[e] = 0.f;
   __syncthreads();
   for (int i = tid; i < n1; i += TN) kind[P.idx1[i]] = 1;
   for (int m = tid; m < n2; m += TN) kind[P.idx2[m]] = 2;
@@ -79,15 +94,23 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
     for (int e = tid; e < n2 * TN; e += TN) {
       const int c = e / n2, m = e - c * n2;
       const bool ok = c < cols;
-      Xs[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
-      XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
+      (MLP ? X2 : Xs)[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
+      if (!MLP) XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
+    }
+    if (MLP) {  // h of this thread's column (as the forward kernel forms it); h̄ starts at 0
+      __syncthreads();
+      for (int m = 0; m < nc; ++m) {
+        float dh;
+        mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, nc, n2, X2 + tid, XP, m), Xs[m * XP + tid], dh);
+        XB[m * XP + tid] = 0.0;
+      }
     }
     const float lb = active && P.ljbar ? P.ljbar[n] : 0.f;
     for (int i = 0; i < n1; ++i) {
       __syncthreads();  // Ws and every column's r̄ of the previous row are no longer read
-      crq_stage_row(P.W, P.c, i, n1, n2, K, Ws, cs, tid, TN);
+      crq_stage_row(P.W, P.c, i, n1, nc, K, Ws, cs, tid, TN);
       __syncthreads();
-      crq_params(Ws, cs, Xs + tid, XP, n2, K, Pr + tid, XP);
+      crq_params(Ws, cs, Xs + tid, XP, nc, K, Pr + tid, XP);
       crq_knots(Pr + tid, XP, K, P.B, KT + tid, TN);
       crq_knots(Pr + K * XP + tid, XP, K, P.B, KT + K1 * TN + tid, TN);
       dv[0] = 1.0f;
@@ -122,16 +145,16 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
         float* r = Pr + (2 * K + j) * XP + tid;
         *r = gd[(j + 1) * TN] / (1.0f + expf(-*r));
       }
-      for (int m = 0; m < n2; ++m) {
+      for (int m = 0; m < nc; ++m) {
         float s = 0.f;
         for (int j = 0; j < J; ++j) s = fmaf(Ws[m * JP + j], Pr[j * XP + tid], s);
         XB[m * XP + tid] += (double)s;
       }
       __syncthreads();
       // this tile's Σ_n r̄ x₂ᵀ and Σ_n r̄ for row i, added to the CTA's slice (each element always by the same thread)
-      float* sl = slice + (size_t)i * J * n2;
-      for (int e = tid; e < J * n2; e += TN) {
-        const int j = e / n2, m = e - j * n2;
+      float* sl = slice + (size_t)i * J * nc;
+      for (int e = tid; e < J * nc; e += TN) {
+        const int j = e / nc, m = e - j * nc;
         const float* pr = Pr + j * XP;
         const float* xs = Xs + m * XP;
         float s = 0.f;
@@ -146,9 +169,43 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
       }
     }
     __syncthreads();
+    if (MLP) {
+      // v̄ = h̄ ⊙ σ′(W₁x₂ + c₁) of this thread's column into Xs (h is no longer read)
+      for (int m = 0; m < nc; ++m) {
+        float h, dh;
+        mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, nc, n2, X2 + tid, XP, m), h, dh);
+        Xs[m * XP + tid] = (float)XB[m * XP + tid] * dh;
+      }
+      __syncthreads();
+      // this tile's Σ_n v̄ x₂ᵀ and Σ_n v̄, added to the CTA's slice (each element always by the same thread)
+      for (int e = tid; e < nc * n2; e += TN) {
+        const int m = e / n2, k = e - m * n2;
+        const float* vb = Xs + m * XP;
+        const float* xs = X2 + k * XP;
+        float s = 0.f;
+        for (int c = 0; c < cols; ++c) s = fmaf(vb[c], xs[c], s);
+        w1slice[e] += s;
+      }
+      for (int m = tid; m < nc; m += TN) {
+        const float* vb = Xs + m * XP;
+        float s = 0.f;
+        for (int c = 0; c < cols; ++c) s += vb[c];
+        w1slice[(size_t)nc * n2 + m] += s;
+      }
+      __syncthreads();
+      // W₁ᵀv̄ of this thread's column into X2 (x₂ is no longer read), the sum over the hidden units in increasing order
+      for (int k = 0; k < n2; ++k) {
+        float s = 0.f;
+        for (int m = 0; m < nc; ++m) s = fmaf(__ldg(P.W1 + (size_t)k * nc + m), Xs[m * XP + tid], s);
+        X2[k * XP + tid] = s;
+      }
+      __syncthreads();
+    }
     for (int e = tid; e < n2 * TN; e += TN) {
       const int c = e / n2, m = e - c * n2;
-      if (c < cols) P.xbar[(n0 + c) * P.ldxb + P.idx2[m]] = (float)XB[m * XP + c];
+      if (c < cols)  // MLP: x̄₂ = ȳ₂ + W₁ᵀv̄
+        P.xbar[(n0 + c) * P.ldxb + P.idx2[m]] =
+            MLP ? (P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.f) + X2[m * XP + c] : (float)XB[m * XP + c];
     }
     for (int e = tid; e < cols * D; e += TN) {  // x̄₃ = ȳ₃
       const int c = e / D, r = e - c * D;
@@ -157,38 +214,63 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
   }
 }
 
-// W̄ / c̄: the G slices summed in order, element e of the slice layout scattered to W's column-major layout.
+// W̄ / c̄: the G slices summed in order, element e of the slice layout scattered to W's column-major layout.  nc: the
+// conditioning rows (n2, or H); with the network also W̄₁ (nh x nx, the slice's [nh][nx]) and c̄₁ (nh), else nh = 0.
 __global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
-                                                                      long long slice, int n1, int n2, int K,
-                                                                      float* __restrict__ Wbar, float* __restrict__ cbar) {
+                                                                      long long slice, int n1, int nc, int K,
+                                                                      float* __restrict__ Wbar, float* __restrict__ cbar,
+                                                                      int nh, int nx, float* __restrict__ W1bar,
+                                                                      float* __restrict__ c1bar) {
   const int J = 3 * K - 1;
-  const long long nw = (long long)n1 * J * n2, e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= nw + (long long)n1 * J) return;
+  const long long nw = (long long)n1 * J * nc, nwc = nw + (long long)n1 * J, nw1 = nwc + (long long)nh * nx;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nw1 + nh) return;
   float t = 0.f;
   for (int g = 0; g < nparts; ++g) t += part[(size_t)g * slice + e];
   if (e < nw) {
-    const int i = (int)(e / ((long long)J * n2)), rem = (int)(e - (long long)i * J * n2), j = rem / n2, m = rem - j * n2;
+    const int i = (int)(e / ((long long)J * nc)), rem = (int)(e - (long long)i * J * nc), j = rem / nc, m = rem - j * nc;
     if (Wbar) Wbar[(size_t)(i + n1 * j) + (size_t)J * n1 * m] = t;
-  } else {
+  } else if (e < nwc) {
     const int f = (int)(e - nw), i = f / J, j = f - i * J;
     if (cbar) cbar[i + n1 * j] = t;
+  } else if (e < nw1) {
+    const int f = (int)(e - nwc), m = f / nx, k = f - m * nx;
+    if (W1bar) W1bar[m + (size_t)nh * k] = t;
+  } else if (c1bar) {
+    c1bar[e - nw1] = t;
   }
 }
 
-static size_t crv_smem_bytes(int n2, int K, int D) {
-  const int J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
-  const size_t f = (size_t)n2 * JP + JP + (size_t)6 * K1 * CRV_TN + (size_t)n2 * (CRV_TN + 1) + (size_t)J * (CRV_TN + 1);
-  return (((f + 1) / 2 + (size_t)n2 * (CRV_TN + 1)) * sizeof(double) + D + 15) & ~(size_t)15;
+// the shape of a spline coupling layer as the kernels see it: nc conditioning rows (n2, or the H hidden units), and for
+// the network nh = H hidden units over nx = n2 rows of x₂ (both 0 without it)
+struct CrvShape {
+  int n1, nc, K, nh, nx;
+};
+static CrvShape crv_shape(const b2b_layer_desc& d) {
+  if (d.kind == B2B_COUPLING_MLP_RQS) return {d.n0, d.n2, d.n3 >> 8, d.n2, d.n1};
+  return {d.n0, d.n1, d.n2, 0, 0};
+}
+
+static size_t crv_smem_bytes(const CrvShape& sh, int D) {
+  const int nc = sh.nc, K = sh.K, J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
+  const size_t f = (size_t)nc * JP + JP + (size_t)6 * K1 * CRV_TN + (size_t)nc * (CRV_TN + 1) + (size_t)J * (CRV_TN + 1);
+  return (((f + 1) / 2 + (size_t)nc * (CRV_TN + 1)) * sizeof(double) + (size_t)sh.nx * (CRV_TN + 1) * sizeof(float) + D +
+          15) & ~(size_t)15;
+}
+
+// floats of the slice's sums: W̄ / c̄ of the spline's conditioner, then W̄₁ / c̄₁ of the network
+static long long crv_sum_floats(const CrvShape& sh) {
+  return (long long)sh.n1 * (3 * sh.K - 1) * (sh.nc + 1) + (long long)sh.nh * (sh.nx + 1);
 }
 
 static long long crv_slice_floats(const b2b_layer_desc& d) {
-  const long long f = (long long)d.n0 * (3 * d.n2 - 1) * (d.n1 + 1);
+  const long long f = crv_sum_floats(crv_shape(d));
   return (f + 63) & ~63LL;
 }
 
 static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
   const int sms = b2b_sm_count();
-  int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(d.n1, d.n2, D) + 1024));
+  int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(crv_shape(d), D) + 1024));
   per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
   long long g = (long long)sms * per_sm;
   const long long tiles = (N + CRV_TN - 1) / CRV_TN;
@@ -198,11 +280,15 @@ static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
   return g < 1 ? 1 : (int)g;
 }
 
+static bool crv_fits(const b2b_layer_desc& d, int D) {
+  return d.kind == B2B_COUPLING_MLP_RQS ? b2b_coupling_mlp_rqs_fits(d, D) : b2b_coupling_rqs_fits(d, D);
+}
+
 }  // namespace b2b
 
 size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
   using namespace b2b;
-  if (!b2b_coupling_rqs_fits(d, D)) return 0;
+  if (!crv_fits(d, D)) return 0;
   return (size_t)crv_grid(d, D, N) * (size_t)crv_slice_floats(d) * sizeof(float) + 256;
 }
 
@@ -211,18 +297,24 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   const b2b_layer_desc& d = s.layers[0];
   const int D = s.D;
   const long long N = s.N;
-  if (!b2b_coupling_rqs_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (!crv_fits(d, D)) return B2B_EUNSUPPORTED;
   if (!s.workspace || s.workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
-  // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c
-  float* const Wbar = s.bars[0] ? s.bars[0] : s.scratch;
-  float* const cbar = !d.p1 ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
-  CrvParams P;
+  const bool mlp = d.kind == B2B_COUPLING_MLP_RQS;
+  const CrvShape sh = crv_shape(d);
+  // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c.  The network's four sums are
+  // written only where they are asked for.
+  float* const Wbar = mlp ? s.bars[2] : s.bars[0] ? s.bars[0] : s.scratch;
+  float* const cbar = mlp ? (d.p3 ? s.bars[3] : nullptr)
+                          : !d.p1 ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
+  CrvParams P = {};
   P.x = s.x;
   P.ybar = s.ybar;
   P.ljbar = s.ljbar;
   P.xbar = s.xbar;
-  P.W = d.p0;
-  P.c = d.p1;
+  P.W = mlp ? d.p2 : d.p0;
+  P.c = mlp ? d.p3 : d.p1;
+  P.W1 = d.p0;
+  P.c1 = d.p1;
   P.idx1 = d.i0;
   P.idx2 = d.i1;
   P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
@@ -234,18 +326,24 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   P.D = D;
   P.n1 = d.n0;
   P.n2 = d.n1;
-  P.K = d.n2;
-  P.B = d.f0;
+  P.K = sh.K;
+  P.H = sh.nh;
+  P.act = d.n3 & 255;
+  P.B = mlp ? d.f1 : d.f0;
+  P.slope = d.f0;
   const int grid = crv_grid(d, D, N);
-  const size_t smem = crv_smem_bytes(d.n1, d.n2, D);
-  void (*kernel)(const CrvParams) = d.inverse ? coupling_rqs_vjp_kernel<true> : coupling_rqs_vjp_kernel<false>;
+  const size_t smem = crv_smem_bytes(sh, D);
+  void (*kernel)(const CrvParams) =
+      mlp ? (d.inverse ? coupling_rqs_vjp_kernel<true, true> : coupling_rqs_vjp_kernel<false, true>)
+          : (d.inverse ? coupling_rqs_vjp_kernel<true, false> : coupling_rqs_vjp_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CRV_TN, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  const long long len = (long long)d.n0 * (3 * d.n2 - 1) * (d.n1 + 1);
-  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(P.part, grid, P.slice, d.n0, d.n1,
-                                                                                      d.n2, Wbar, cbar);
+  const long long len = crv_sum_floats(sh);
+  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
+      P.part, grid, P.slice, sh.n1, sh.nc, sh.K, Wbar, cbar, sh.nh, sh.nx, mlp ? s.bars[0] : nullptr,
+      mlp && d.p1 ? s.bars[1] : nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   *s.launches += 2;
   return B2B_OK;

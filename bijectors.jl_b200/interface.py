@@ -821,6 +821,9 @@ _SLOTS = {
     _lib.COUPLING_RQS: (("W", "c"), lambda d, D: ((d.n1, (3 * d.n2 - 1) * d.n0), ((3 * d.n2 - 1) * d.n0,)), (0,)),
     _lib.SCALE_MATRIX: (("a",), lambda d, D: ((D, D),), (0,)),
     _lib.COUPLING_MLP: (("W1", "c1", "W2", "c2"), lambda d, D: ((d.n1, d.n2), (d.n2,), (d.n2, 2 * d.n0), (2 * d.n0,)), (0, 2)),
+    _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"),
+                            lambda d, D: ((d.n1, d.n2), (d.n2,), (d.n2, (3 * (d.n3 >> 8) - 1) * d.n0), ((3 * (d.n3 >> 8) - 1) * d.n0,)),
+                            (0, 2)),
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 

@@ -41,6 +41,7 @@ const PLANAR, RADIAL, RQS, COUPLING_AFFINE, BATCHNORM, PERMUTE, STACKED_EW, MVNO
 const COUPLING_RQS = Int32(11)  # 10 is not a layer kind (include/b2b.h)
 const SCALE_MATRIX = Int32(12)
 const COUPLING_MLP = Int32(13)
+const COUPLING_MLP_RQS = Int32(14)
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -143,8 +144,35 @@ function desc(cl::Coupling{<:MLPConditioner{<:CuMatrix{Float32}}}, inv::Bool)
     LayerDesc(COUPLING_MLP, inv, length(dm.idx1), length(dm.idx2), size(θ.W1, 1), θ.act, θ.slope, 0f0,
               pointer(θ.W1), ptr(θ.c1), pointer(θ.W2), ptr(θ.c2), pointer(dm.idx1), pointer(dm.idx2))
 end
+# The neural spline flow's coupling law (Durkan et al. 2019): the RationalQuadraticSpline of SplineConditioner whose raw
+# knots v = W₂*σ.(W₁*x₂ .+ c₁) .+ c₂ come from the hidden layer of MLPConditioner; a callable returning the reference's
+# own spline, so the same object also runs on the CPU reference path.  Float32, n1, n2 <= 128, H <= 128, 2 <= K <= 16,
+# D <= 1024 on the device; c₁ / c₂ === nothing is a zero shift.
+struct MLPSplineConditioner{M<:AbstractMatrix,V1,V2}
+    W1::M   # (H × n2)
+    c1::V1  # H, or nothing
+    W2::M   # ((3K−1)·n1 × H)
+    c2::V2  # (3K−1)·n1, or nothing
+    K::Int
+    B::Float32
+    act::Int32      # ACT_TANH or ACT_LEAKY_RELU
+    slope::Float32
+end
+function (θ::MLPSplineConditioner)(x₂)
+    u = θ.c1 === nothing ? θ.W1 * x₂ : θ.W1 * x₂ .+ θ.c1
+    h = θ.act == ACT_TANH ? tanh.(u) : ifelse.(u .>= 0, u, θ.slope .* u)
+    SplineConditioner(θ.W2, θ.c2, θ.K, θ.B)(h)
+end
+function desc(cl::Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}}, inv::Bool)
+    dm = get!(() -> DeviceMask(cl.mask), MASKS, cl.mask)
+    θ = cl.θ
+    ptr(c) = c === nothing ? NULLF : pointer(c)
+    LayerDesc(COUPLING_MLP_RQS, inv, length(dm.idx1), length(dm.idx2), size(θ.W1, 1), θ.act | (Int32(θ.K) << 8),
+              θ.slope, θ.B, pointer(θ.W1), ptr(θ.c1), pointer(θ.W2), ptr(θ.c2), pointer(dm.idx1), pointer(dm.idx2))
+end
 desc(cl::Coupling, ::Bool) =
-    error("Coupling: only AffineConditioner, SplineConditioner and MLPConditioner laws run on the device path (no CPU fallback)")
+    error("Coupling: only AffineConditioner, SplineConditioner, MLPConditioner and MLPSplineConditioner laws run on the " *
+          "device path (no CPU fallback)")
 
 # Permute(A): y[dst[i]] = x[i] with dst = the row of the single 1 in column i (permute.jl:90-100,152)
 const PERMS = IdDict{Any,CuVector{Int32}}()
@@ -198,7 +226,7 @@ descs(f, inv::Bool) = inv ? [desc(b, true) for b in reverse(flatten(f))] : [desc
 const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVector{Float32}},
                           RationalQuadraticSpline{<:CuMatrix{Float32}},InvertibleBatchNorm{<:CuVector{Float32}},
                           Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},
-                          Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},
+                          Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
                           Scale{<:CuMatrix{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
@@ -410,6 +438,9 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == SCALE_MATRIX && return (z(D, D),)
     d.kind == COUPLING_MLP && return (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(2d.n0, d.n2),
                                       d.p3 == NULLF ? nothing : z(2d.n0))
+    d.kind == COUPLING_MLP_RQS && return (J = (3(d.n3 >> 8) - 1) * d.n0;
+                                          (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(J, d.n2),
+                                           d.p3 == NULLF ? nothing : z(J)))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

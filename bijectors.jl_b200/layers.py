@@ -260,6 +260,35 @@ class AffineConditioner:
         return (self.W, self.c)
 
 
+def _host32(v):
+    return np.asarray(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=np.float32)
+
+
+def _spline_law(who, Wn, K, B, cols):
+    """(K, B, n1) of a spline conditioner whose last layer Wn has (3K−1)·n1 rows and ``cols`` columns."""
+    K = int(K)
+    if K < 1:
+        raise ValueError(f"{who}: K must be >= 1")
+    if not float(B) > 0:
+        raise ValueError(f"{who}: B must be > 0")
+    J = 3 * K - 1
+    if Wn.ndim != 2 or Wn.shape[0] == 0 or Wn.shape[0] % J:
+        raise ValueError(f"{who}: W must be ((3K-1)*n1, {cols}) = ({J}*n1, {cols}), got {Wn.shape}")
+    return K, float(B), Wn.shape[0] // J
+
+
+def _bias(c, name, n, device):
+    if c is None:
+        return None
+    cn = _host32(c).reshape(-1)
+    if cn.shape != (n,):
+        raise ValueError(f"{name} must have {n} entries, got {cn.shape}")
+    return _dev_f32(cn, device)
+
+
+_ACT = {"tanh": _lib.ACT_TANH, "leaky_relu": _lib.ACT_LEAKY_RELU}
+
+
 class SplineConditioner:
     """The neural-spline coupling law (Durkan et al. 2019) θ(x₂) = RationalQuadraticSpline(reshape(v[1:n1K], n1, K),
     reshape(v[n1K+1:2n1K], n1, K), reshape(v[2n1K+1:end], n1, K−1), B) with v = W·x₂ + c -- the reference's own
@@ -270,24 +299,11 @@ class SplineConditioner:
     def __init__(self, W, c=None, *, K: int, B: float, device="cuda", dtype=torch.float32):
         if dtype != torch.float32:
             raise TypeError("SplineConditioner: the spline coupling layer runs in Float32 only")
-        K = int(K)
-        if K < 1:
-            raise ValueError("SplineConditioner: K must be >= 1")
-        if not float(B) > 0:
-            raise ValueError("SplineConditioner: B must be > 0")
-        Wn = np.asarray(W.detach().cpu() if isinstance(W, torch.Tensor) else W, dtype=np.float32)
-        J = 3 * K - 1
-        if Wn.ndim != 2 or Wn.shape[0] == 0 or Wn.shape[0] % J:
-            raise ValueError(f"W must be ((3K-1)*n1, n2) = ({J}*n1, n2), got {Wn.shape}")
-        self.K, self.B = K, float(B)
-        self.n1, self.n2 = Wn.shape[0] // J, Wn.shape[1]
+        Wn = _host32(W)
+        self.K, self.B, self.n1 = _spline_law("SplineConditioner", Wn, K, B, "n2")
+        self.n2 = Wn.shape[1]
         self.W = _dev_f32(np.ascontiguousarray(Wn.T), device)  # column-major ((3K−1)n1 × n2)
-        self.c = None
-        if c is not None:
-            cn = np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, dtype=np.float32).reshape(-1)
-            if cn.shape != (Wn.shape[0],):
-                raise ValueError(f"c must have (3K-1)*n1 = {Wn.shape[0]} entries, got {cn.shape}")
-            self.c = _dev_f32(cn, device)
+        self.c = _bias(c, "c", Wn.shape[0], device)
 
     def to(self, device):
         new = object.__new__(SplineConditioner)
@@ -300,43 +316,27 @@ class SplineConditioner:
         return (self.W, self.c)
 
 
-class MLPConditioner:
-    """The neural-network coupling law of RealNVP: θ(x₂) = Shift(t) ∘ Scale(exp.(s)) with
-    [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂, one hidden layer of width H and σ = tanh or LeakyReLU(slope) (slope 0 is ReLU;
-    v >= 0 ? v : slope·v, leaky_relu.jl:18-29).  W1 is (H × n2) and W2 (2·n1 × H) in the reference's index order, rows
-    1..n1 of W2 giving s and the rest t as for :class:`AffineConditioner`; c1 (H) and c2 (2·n1) may be None (no shift,
-    the descriptor's pointer is NULL).  Float32 only.  Runs as B2B_COUPLING_MLP: n1, n2 <= 128, H <= 256, D <= 1024."""
+class _NetworkConditioner:
+    """A conditioner whose parameters come from a hidden layer h = σ.(W₁·x₂ + c₁) and a last layer W₂·h + c₂."""
 
-    _ACT = {"tanh": _lib.ACT_TANH, "leaky_relu": _lib.ACT_LEAKY_RELU}
+    _ACT = _ACT
 
-    def __init__(self, W1, c1, W2, c2, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+    def _hidden_layer(self, who, W1, c1, activation, slope, dtype, device):
+        """Checks the hidden layer and sets activation, slope, H, n2, W1 (column-major) and c1 (None: NULL pointer)."""
         if dtype != torch.float32:
-            raise TypeError("MLPConditioner: the neural-network coupling layer runs in Float32 only")
-        if activation not in self._ACT:
-            raise ValueError(f"MLPConditioner: activation must be one of {sorted(self._ACT)}, got {activation!r}")
-
-        def host(v):
-            return np.asarray(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=np.float32)
-
-        W1n, W2n = host(W1), host(W2)
+            raise TypeError(f"{who}: the network coupling layers run in Float32 only")
+        if activation not in _ACT:
+            raise ValueError(f"{who}: activation must be one of {sorted(_ACT)}, got {activation!r}")
+        W1n = _host32(W1)
         if W1n.ndim != 2 or W1n.shape[0] == 0:
             raise ValueError(f"W1 must be (H, n2), got {W1n.shape}")
-        if W2n.ndim != 2 or W2n.shape[0] == 0 or W2n.shape[0] % 2 or W2n.shape[1] != W1n.shape[0]:
-            raise ValueError(f"W2 must be (2*n1, H) with H = {W1n.shape[0]}, got {W2n.shape}")
         self.activation, self.slope = activation, float(slope)
-        self.H, self.n2, self.n1 = W1n.shape[0], W1n.shape[1], W2n.shape[0] // 2
+        self.H, self.n2 = W1n.shape
         self.W1 = _dev_f32(np.ascontiguousarray(W1n.T), device)  # column-major (H × n2)
-        self.W2 = _dev_f32(np.ascontiguousarray(W2n.T), device)  # column-major (2n1 × H)
-        self.c1 = self.c2 = None
-        for name, c, n in (("c1", c1, self.H), ("c2", c2, 2 * self.n1)):
-            if c is not None:
-                cn = host(c).reshape(-1)
-                if cn.shape != (n,):
-                    raise ValueError(f"{name} must have {n} entries, got {cn.shape}")
-                setattr(self, name, _dev_f32(cn, device))
+        self.c1 = _bias(c1, "c1", self.H, device)
 
     def to(self, device):
-        new = object.__new__(MLPConditioner)
+        new = object.__new__(type(self))
         new.__dict__.update(self.__dict__)
         for k in ("W1", "c1", "W2", "c2"):
             t = getattr(self, k)
@@ -347,19 +347,54 @@ class MLPConditioner:
         return (self.W1, self.c1, self.W2, self.c2)
 
 
+class MLPConditioner(_NetworkConditioner):
+    """The neural-network coupling law of RealNVP: θ(x₂) = Shift(t) ∘ Scale(exp.(s)) with
+    [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂, one hidden layer of width H and σ = tanh or LeakyReLU(slope) (slope 0 is ReLU;
+    v >= 0 ? v : slope·v, leaky_relu.jl:18-29).  W1 is (H × n2) and W2 (2·n1 × H) in the reference's index order, rows
+    1..n1 of W2 giving s and the rest t as for :class:`AffineConditioner`; c1 (H) and c2 (2·n1) may be None (no shift,
+    the descriptor's pointer is NULL).  Float32 only.  Runs as B2B_COUPLING_MLP: n1, n2 <= 128, H <= 256, D <= 1024."""
+
+    def __init__(self, W1, c1, W2, c2, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+        self._hidden_layer("MLPConditioner", W1, c1, activation, slope, dtype, device)
+        W2n = _host32(W2)
+        if W2n.ndim != 2 or W2n.shape[0] == 0 or W2n.shape[0] % 2 or W2n.shape[1] != self.H:
+            raise ValueError(f"W2 must be (2*n1, H) with H = {self.H}, got {W2n.shape}")
+        self.n1 = W2n.shape[0] // 2
+        self.W2 = _dev_f32(np.ascontiguousarray(W2n.T), device)  # column-major (2n1 × H)
+        self.c2 = _bias(c2, "c2", 2 * self.n1, device)
+
+
+class MLPSplineConditioner(_NetworkConditioner):
+    """The neural spline flow's coupling law (Durkan et al. 2019): θ(x₂) = RationalQuadraticSpline(…, B) as for
+    :class:`SplineConditioner`, with the raw knots v = W₂·σ.(W₁·x₂ + c₁) + c₂ from one hidden layer of width H as for
+    :class:`MLPConditioner`.  W1 is (H × n2) and W2 ((3K−1)·n1 × H) in the reference's index order; c1 (H) and c2
+    ((3K−1)·n1) may be None.  Float32 only.  Runs as B2B_COUPLING_MLP_RQS: n1, n2 <= 128, H <= 128, 2 <= K <= 16,
+    D <= 1024."""
+
+    def __init__(self, W1, c1, W2, c2, *, K: int, B: float, activation="tanh", slope=0.0, device="cuda",
+                 dtype=torch.float32):
+        self._hidden_layer("MLPSplineConditioner", W1, c1, activation, slope, dtype, device)
+        W2n = _host32(W2)
+        self.K, self.B, self.n1 = _spline_law("MLPSplineConditioner", W2n, K, B, "H")
+        if W2n.shape[1] != self.H:
+            raise ValueError(f"W2 must be ((3K-1)*n1, H) with H = {self.H}, got {W2n.shape}")
+        self.W2 = _dev_f32(np.ascontiguousarray(W2n.T), device)  # column-major ((3K−1)n1 × H)
+        self.c2 = _bias(c2, "c2", W2n.shape[0], device)
+
+
 class Coupling(_ParamLayer):
     """Coupling(θ, mask) (coupling.jl:178-181).  θ is an arbitrary closure in the reference; the device
-    path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner` and :class:`MLPConditioner` and
-    raises for anything else (no CPU fallback)."""
+    path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner`, :class:`MLPConditioner` and
+    :class:`MLPSplineConditioner` and raises for anything else (no CPU fallback)."""
 
     _fields = ()
 
     def __init__(self, θ, mask, device="cuda"):
         if isinstance(mask, int):  # Coupling(θ, n): first n÷2 rows transformed (:183-186)
             mask = PartitionMask(mask, range(1, mask // 2 + 1))
-        if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner)):
-            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner and MLPConditioner "
-                                                  "laws run on the device path")
+        if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner)):
+            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner, MLPConditioner "
+                                                  "and MLPSplineConditioner laws run on the device path")
         if θ.n1 != len(mask.indices_1) or θ.n2 != len(mask.indices_2):
             raise ValueError("conditioner shape does not match the PartitionMask")
         self.θ, self.mask = θ, mask
@@ -392,6 +427,11 @@ class Coupling(_ParamLayer):
             return [_desc(_lib.COUPLING_MLP, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
                           p3=θ.c2 if θ.c2 is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
                           n3=θ._ACT[θ.activation], f0=θ.slope)]
+        if isinstance(self.θ, MLPSplineConditioner):
+            θ = self.θ
+            return [_desc(_lib.COUPLING_MLP_RQS, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
+                          p3=θ.c2 if θ.c2 is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
+                          n3=θ._ACT[θ.activation] | (θ.K << 8), f0=θ.slope, f1=θ.B)]
         if isinstance(self.θ, SplineConditioner):
             return [_desc(_lib.COUPLING_RQS, inverse, p0=self.θ.W, p1=self.θ.c if self.θ.c is not None else 0,
                           i0=self._idx1, i1=self._idx2, n0=self.θ.n1, n1=self.θ.n2, n2=self.θ.K, n3=0, f0=self.θ.B)]
@@ -403,7 +443,10 @@ class Coupling(_ParamLayer):
             return False
         if isinstance(self.θ, SplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
             return False
-        if isinstance(self.θ, MLPConditioner) and (self.θ.activation, self.θ.slope) != (o.θ.activation, o.θ.slope):
+        if isinstance(self.θ, MLPSplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
+            return False
+        if isinstance(self.θ, (MLPConditioner, MLPSplineConditioner)) and \
+                (self.θ.activation, self.θ.slope) != (o.θ.activation, o.θ.slope):
             return False
         return all((a is None) == (b is None) and (a is None or torch.equal(a, b))
                    for a, b in zip(self.θ._tensors(), o.θ._tensors()))

@@ -83,7 +83,15 @@ extern "C" {
 #define B2B_COUPLING_MLP_MAX_N 128
 #define B2B_COUPLING_MLP_MAX_H 256
 #define B2B_COUPLING_MLP_MAX_D 1024
-/* hidden-layer activation σ of B2B_COUPLING_MLP (descriptor field n3) */
+#define B2B_COUPLING_MLP_RQS 14 /* Coupling, θ = x₂ -> RationalQuadraticSpline(reshape(W₂·σ.(W₁·x₂+c₁)+c₂), B)  coupling.jl */
+/* Envelope of B2B_COUPLING_MLP_RQS (every entry point, forward, inverse and reverse mode): n1, n2 <= 128, 1 <= H <= 128,
+ * 2 <= K <= 16, D <= 1024.  A layer past it returns B2B_EUNSUPPORTED with nothing launched, and the workspace queries
+ * return 0; the Float64 entry points refuse the kind the same way. */
+#define B2B_COUPLING_MLP_RQS_MAX_N 128
+#define B2B_COUPLING_MLP_RQS_MAX_H 128
+#define B2B_COUPLING_MLP_RQS_MAX_K 16
+#define B2B_COUPLING_MLP_RQS_MAX_D 1024
+/* hidden-layer activation σ of B2B_COUPLING_MLP and B2B_COUPLING_MLP_RQS (descriptor field n3) */
 #define B2B_ACT_TANH 0
 #define B2B_ACT_LEAKY_RELU 1 /* v >= 0 ? v : a*v with a = f0 (a = 0: ReLU), the convention of B2B_EW_LEAKY_RELU */
 
@@ -150,6 +158,16 @@ extern "C" {
  *                     COUPLING_AFFINE, whose law, log-Jacobian ±Σ s and inverse (the network evaluated on y₂ = x₂) the
  *                     layer shares.  Float32 only, exact fp32 FMA on the CUDA cores, its own launch (no BatchNorm
  *                     folding).  Envelope: B2B_COUPLING_MLP_MAX_*; the Float64 entry points return B2B_EUNSUPPORTED.)
+ * COUPLING_MLP_RQS   W₁[H x n2]  c₁[H]|NULL  W₂[J x H]   c₂[J]|NULL idx1[n1]      idx2[n2]      n1    n2   a
+ *                    (J = (3K−1)·n1; n2 of the descriptor = H hidden units, n3 = σ | (K << 8) with σ = B2B_ACT_TANH or
+ *                     B2B_ACT_LEAKY_RELU (slope a = f0) and K bins, f1 = B > 0.  W₁ and W₂ are column-major and required,
+ *                     c₁ / c₂ may be NULL (= 0); both index lists are required.  Per column h = σ.(W₁·x₂ + c₁) and
+ *                     v = W₂·h + c₂; transformed row i takes its raw widths, heights and derivatives from v as COUPLING_RQS
+ *                     does (v[i + n1·k], v[n1·K + i + n1·k], v[2·n1·K + i + n1·k]), with that layer's normalisation, spline,
+ *                     inverse (the network evaluated on y₂ = x₂) and identity outside [−B, B].  n1, n2, H >= 1,
+ *                     n1 + n2 <= D, K >= 1, a known σ and B > 0, else B2B_EINVAL.  Float32 only, exact fp32 on the CUDA
+ *                     cores, its own launch.  Envelope: B2B_COUPLING_MLP_RQS_MAX_*; the Float64 entry points return
+ *                     B2B_EUNSUPPORTED.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -193,6 +211,8 @@ const char* b2b_status_string(int status);
  * 256 bytes, plus 256, for a chain with any SCALE_MATRIX layer (the layers share it; they run one after another).
  * COUPLING_MLP runs in its own launch (any N, any ld >= D, scattered index lists, y may alias x; the envelope of
  * B2B_COUPLING_MLP_MAX_*; no workspace); like COUPLING_RQS, a batch sum needs the chain to end in a fused launch.
+ * COUPLING_MLP_RQS runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x; the
+ * envelope of B2B_COUPLING_MLP_RQS_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
  * The whole chain is planned before anything is enqueued: a
  * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
@@ -329,7 +349,8 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * computed), summed over the N columns in a fixed order (deterministic; a multi-GPU caller all-reduces them).
  * Trainable slots: PLANAR w u b; RADIAL α_ β z_0 (raw); RQS widths heights derivatives (processed); COUPLING W c (also
  * COUPLING_RQS, whose W̄ is ((3K−1)·n1 x n2) column-major like W; a c̄ request with c == NULL returns B2B_EINVAL);
- * COUPLING_MLP W₁ c₁ W₂ c₂ (column-major like the parameters; a c̄₁ / c̄₂ request whose c is NULL returns B2B_EINVAL);
+ * COUPLING_MLP and COUPLING_MLP_RQS W₁ c₁ W₂ c₂ (column-major like the parameters; a c̄₁ / c̄₂ request whose c is NULL
+ * returns B2B_EINVAL);
  * SCALE_MATRIX a (Ā, D x D column-major like A: G + (Σ l̄)·A⁻ᵀ, or −A⁻ᵀ G A⁻ᵀ − (Σ l̄)·A⁻ᵀ for the inverse layer, with
  * G = Σₙ ȳₙ uₙᵀ over the layer's inputs u; slots 1-3 return B2B_EUNSUPPORTED);
  * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
@@ -436,8 +457,8 @@ int b2b_mvnormal_diag_logpdf_f32(const float* x, const float* mu, const float* s
 
 /* ---- Float64 batches -------------------------------------------------------------------------------------------------
  * The reference is generic in its element type and its own tests run in Float64 (test/normalising_flows.jl:47-71 checks
- * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind but B2B_COUPLING_RQS and
- * B2B_COUPLING_MLP (Float32 only: the Float64 entry points and workspace queries refuse them with B2B_EUNSUPPORTED / 0),
+ * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind but B2B_COUPLING_RQS,
+ * B2B_COUPLING_MLP and B2B_COUPLING_MLP_RQS (Float32 only: the Float64 entry points and workspace queries refuse them with B2B_EUNSUPPORTED / 0),
  * both directions, the terminal
  * MvNormal, the deterministic batch sum -- on D x N Float64 batches with Float64 parameters (b2b_layer_desc_f64: the
  * same fields with double pointers).  It is a straightforward double-precision restatement (one warp per column), NOT a
