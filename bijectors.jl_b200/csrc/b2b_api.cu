@@ -68,6 +68,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
     case B2B_COUPLING_MLP: ok = b2b_coupling_mlp_fits(d, D); break;
     case B2B_COUPLING_MLP_RQS: ok = b2b_coupling_mlp_rqs_fits(d, D); break;
+    case B2B_COUPLING_DEEP_MLP: ok = b2b_coupling_deep_mlp_fits(d, D); break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
     default: break;
   }
@@ -86,6 +87,7 @@ static int vjp_envelope(const b2b_layer_desc& d, int D) {
     case B2B_SCALE_MATRIX:
     case B2B_COUPLING_MLP:
     case B2B_COUPLING_MLP_RQS:
+    case B2B_COUPLING_DEEP_MLP:
     case B2B_MVNORMAL_TRIL: return fwd_envelope(d, D);
     default: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
   }

@@ -9,6 +9,11 @@
 // step.  Phase 2 is coupling_tile of the affine kernel with X2 = h, n2 = H, W = W₂, cvec = c₂: the same GEMM, exp / FMA
 // epilogue and per-warp Σ s.  Every output is a fixed-order fmaf chain over k, then over the hidden units, so it does not
 // depend on N, the tile or the grid.
+//
+// The deep network of B2B_COUPLING_DEEP_MLP (DEEP = true) runs phase 1 M times, h_l = σ(W_l·h_{l−1} + c_l) with
+// h_0 = x₂ and W_1 = W_in; phase 2 runs on h_M with W_out and c_out.  Odd layers go to the h block, even layers to the
+// x₂ block (max(n2, H) rows), whose x₂ was stored to y₂ when it was loaded: at n1 = n2 = H = 128 the kernel then needs
+// the shared memory of the one-hidden-layer kernel, and two CTAs still fit an SM.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -26,16 +31,42 @@ struct CmlpParams {
   long long N, ldx, ldy;
   int D, n1, n2, H, act, accumulate;
   float slope;
+  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
+  int depth;        // DEEP: M hidden layers
 };
 
-template <bool INV>
+// dst = σ(W·src + c) for one tile: W is H x nk column-major, src [nk][CP_LD], dst [H][CP_LD], c NULL = 0.  Eight
+// hidden rows per warp and step.
+__device__ __forceinline__ void cmlp_hidden(const float* src, int nk, const float* __restrict__ W,
+                                            const float* __restrict__ c, bool vec, int H, int act, float slope,
+                                            float* dst) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto same = [](int k) { return k; };
+  for (int jb = 8 * warp; jb < H; jb += 8 * (CP_THREADS / 32)) {
+    float va[4][2] = {}, vb[4][2] = {};
+    coupling_gemm_block<2>(src, CP_LD, same, nk, W + jb, W + jb + 4, H, H - jb, H - jb - 4, vec, va, vb);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int m = jb + q;
+      if (m < H) {
+        const float cm = c ? __ldg(c + m) : 0.f;
+        float dh;
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          mlp_act(act, slope, (q < 4 ? va[q & 3][u] : vb[q & 3][u]) + cm, dst[m * CP_LD + lane + 32 * u], dh);
+      }
+    }
+  }
+}
+
+template <bool INV, bool DEEP>
 __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __grid_constant__ CmlpParams P) {
   // x and y may alias (in place): every element is read before it is written, by the same CTA
   extern __shared__ float smem[];
   const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H;
-  float* X2 = smem;                                      // [n2][CP_LD]  conditioner input x₂
-  float* X1 = X2 + (size_t)n2 * CP_LD;                   // [n1][CP_LD]  x₁, transformed in place
-  float* Hs = X1 + (size_t)n1 * CP_LD;                   // [H][CP_LD]   hidden layer h
+  float* X2 = smem;                                      // [n2][CP_LD]  x₂ (DEEP: max(n2, H) rows, h_l of even l)
+  float* X1 = X2 + (size_t)(DEEP ? max(n2, H) : n2) * CP_LD;  // [n1][CP_LD]  x₁, transformed in place
+  float* Hs = X1 + (size_t)n1 * CP_LD;                   // [H][CP_LD]   hidden layer h (DEEP: h_l of odd l)
   float* red = Hs + (size_t)H * CP_LD;                   // [8][CP_TC]
   int* sidx2 = reinterpret_cast<int*>(red + 8 * CP_TC);  // [n2]
   int* sidx1 = sidx2 + n2;                               // [n1]
@@ -57,6 +88,7 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
   }
   const bool vec1 = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
   const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
+  const bool vech = DEEP && ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
   const long long tiles = (P.N + CP_TC - 1) / CP_TC;
   auto same = [](int k) { return k; };
 
@@ -69,6 +101,10 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
       if (col < P.N) {
         const float* xc = x + col * P.ldx;
         for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = __ldcs(xc + sidx2[k]);
+        if constexpr (DEEP) {  // the x₂ block will hold h_2 and h_4: y₂ = x₂ goes out now
+          if (copy_through)
+            for (int k = lane; k < n2; k += 32) __stcs(y + col * P.ldy + sidx2[k], X2[k * CP_LD + c]);
+        }
         if (y)  // the log-Jacobian needs x₂ only
           for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = __ldcs(xc + sidx1[k]);
         if (has_x3 && copy_through) {
@@ -99,8 +135,18 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
       }
     }
     __syncthreads();
+    const float* hM = Hs;
+    if constexpr (DEEP) {  // h_l = σ(W_l·h_{l−1} + c_l), l = 2..M
+      for (int l = 2; l <= P.depth; ++l) {
+        float* dst = (l & 1) ? Hs : X2;
+        cmlp_hidden(hM, H, P.Wh + (size_t)(l - 2) * H * H, P.c1 ? P.c1 + (size_t)(l - 1) * H : nullptr, vech, H,
+                    P.act, P.slope, dst);
+        __syncthreads();
+        hM = dst;
+      }
+    }
     // ---- phase 2: [s; t] = W₂·h + c₂ and the affine law on x₁ ----------------------------------------------------
-    coupling_tile<INV>(Hs, X1, same, same, P.W2, P.c2, n1, H, vec2, red);
+    coupling_tile<INV>(hM, X1, same, same, P.W2, P.c2, n1, H, vec2, red);
     __syncthreads();
     // ---- write back x₁ (and x₂ unless it is already in place) ------------------------------------------------------
     if (y) {
@@ -109,7 +155,7 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
         if (col < P.N) {
           float* yc = y + col * P.ldy;
           for (int k = lane; k < n1; k += 32) __stcs(yc + sidx1[k], X1[k * CP_LD + c]);
-          if (copy_through)
+          if (!DEEP && copy_through)
             for (int k = lane; k < n2; k += 32) __stcs(yc + sidx2[k], X2[k * CP_LD + c]);
         }
       }
@@ -127,9 +173,10 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
   }
 }
 
-// x₂, x₁ and h tiles, the column-sum slab, both index tables and the coupled-row bitmap
-static size_t cmlp_smem_bytes(int n1, int n2, int H, int D) {
-  return ((size_t)(n1 + n2 + H) * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int) +
+// x₂ (DEEP: max(n2, H) rows), x₁ and h tiles, the column-sum slab, both index tables and the coupled-row bitmap
+static size_t cmlp_smem_bytes(int n1, int n2, int H, int D, bool deep) {
+  const int r2 = deep && H > n2 ? H : n2;
+  return ((size_t)(n1 + r2 + H) * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int) +
          (size_t)((D + 31) / 32) * sizeof(unsigned);
 }
 
@@ -140,19 +187,24 @@ bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D) {
          d.n2 <= B2B_COUPLING_MLP_MAX_H && D <= B2B_COUPLING_MLP_MAX_D;
 }
 
+bool b2b_coupling_deep_mlp_fits(const b2b_layer_desc& d, int D) {
+  const int M = d.n3 >> 8;
+  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_DEEP_MLP_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_DEEP_MLP_MAX_N &&
+         d.n2 >= 1 && d.n2 <= B2B_COUPLING_DEEP_MLP_MAX_H && M >= 2 && M <= B2B_COUPLING_DEEP_MLP_MAX_DEPTH &&
+         D <= B2B_COUPLING_DEEP_MLP_MAX_D;
+}
+
+// COUPLING_MLP and COUPLING_DEEP_MLP
 int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
   using namespace b2b;
-  if (!b2b_coupling_mlp_fits(d, D)) return B2B_EUNSUPPORTED;
+  const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
+  if (!(deep ? b2b_coupling_deep_mlp_fits(d, D) : b2b_coupling_mlp_fits(d, D))) return B2B_EUNSUPPORTED;
   if (N <= 0) return B2B_OK;
   CmlpParams P;
   P.x = x;
   P.y = y;
   P.logjac = logjac;
-  P.W1 = d.p0;
-  P.c1 = d.p1;
-  P.W2 = d.p2;
-  P.c2 = d.p3;
   P.idx1 = d.i0;
   P.idx2 = d.i1;
   P.N = N;
@@ -162,11 +214,28 @@ int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, f
   P.n1 = d.n0;
   P.n2 = d.n1;
   P.H = d.n2;
-  P.act = d.n3;
   P.accumulate = accumulate;
   P.slope = d.f0;
-  const size_t smem = cmlp_smem_bytes(d.n0, d.n1, d.n2, D);
-  void (*kernel)(const CmlpParams) = d.inverse ? coupling_mlp_kernel<true> : coupling_mlp_kernel<false>;
+  if (deep) {  // p0 = W_in, p1 = W_hid, p2 = W_out, p3 = [c_1 | … | c_M | c_out] or NULL; n3 = σ | M << 8
+    P.W1 = d.p0;
+    P.Wh = d.p1;
+    P.W2 = d.p2;
+    P.depth = d.n3 >> 8;
+    P.c1 = d.p3;
+    P.c2 = d.p3 ? d.p3 + (size_t)P.depth * d.n2 : nullptr;
+    P.act = d.n3 & 255;
+  } else {
+    P.W1 = d.p0;
+    P.c1 = d.p1;
+    P.W2 = d.p2;
+    P.c2 = d.p3;
+    P.Wh = nullptr;
+    P.depth = 1;
+    P.act = d.n3;
+  }
+  const size_t smem = cmlp_smem_bytes(d.n0, d.n1, d.n2, D, deep);
+  void (*kernel)(const CmlpParams) = deep ? (d.inverse ? coupling_mlp_kernel<true, true> : coupling_mlp_kernel<false, true>)
+                                          : (d.inverse ? coupling_mlp_kernel<true, false> : coupling_mlp_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   const int sms = b2b_sm_count();

@@ -13,6 +13,12 @@
 // its private slice of the workspace ([W̄₁ | c̄₁ | W̄₂ | c̄₂], every element always by the same thread): one
 // read-modify-write of the slice per 32·S columns.  A second kernel sums the slices in order, in fp64, into the caller's
 // arrays.  Deterministic, no atomics; the workspace depends on the grid, not on N.
+//
+// The deep network of B2B_COUPLING_DEEP_MLP (DEEP = true, M hidden layers, h_0 = x₂, W_1 = W_in) keeps h_l and σ′_l of
+// every layer of the group in shared memory and runs back through them:
+//   v̄_M = (W_outᵀ[s̄; t̄]) ⊙ σ′_M     v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}     x̄₂ = ȳ₂ + W_inᵀ v̄_1
+//   W̄_out = Σₙ [s̄; t̄] h_Mᵀ   W̄_l = Σₙ v̄_l h_{l−1}ᵀ   c̄ = [Σₙ v̄_1 | … | Σₙ v̄_M | Σₙ [s̄; t̄]]
+// with the slice laid out [W̄_in | W̄_hid | W̄_out | c̄], the order of the descriptor's p0 .. p3.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -35,6 +41,8 @@ struct CmvParams {
   long long N, ldx, ldyb, ldxb, slice;
   int D, n1, n2, H, act, nsub;
   float slope;
+  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
+  int depth;        // DEEP: M hidden layers
 };
 
 // acc[q] += Σ_k A[q·nk + k] · B[k·ld + lane] for the `rows` (<= 8) rows at A, each contiguous in k, k increasing
@@ -101,24 +109,66 @@ __device__ __forceinline__ void cmv_outer(const float* A, int RA, const float* B
   }
 }
 
-template <bool INV>
+// One sub-tile's hidden layer: h = σ(W·src + c) and σ′ into hs / dv ([H][ld], column `lane`), W H x nk column-major
+__device__ __forceinline__ void cmv_hidden(const float* src, int ld, int nk, const float* __restrict__ W,
+                                           const float* __restrict__ c, bool vec, int H, int act, float slope, float* hs,
+                                           float* dv) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto same = [](int k) { return k; };
+  for (int jb = 8 * warp; jb < H; jb += 8 * (CMV_THREADS / 32)) {
+    float va[4][1] = {}, vb[4][1] = {};
+    coupling_gemm_block<1>(src, ld, same, nk, W + jb, W + jb + 4, H, H - jb, H - jb - 4, vec, va, vb);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int m = jb + q;
+      if (m < H)
+        mlp_act(act, slope, (q < 4 ? va[q & 3][0] : vb[q & 3][0]) + (c ? __ldg(c + m) : 0.f), hs[m * ld + lane],
+                dv[m * ld + lane]);
+    }
+  }
+}
+
+// v̄ = (Wᵀ g) ⊙ σ′ in place over the σ′ block v ([H][ld]), W ng x H column-major, g [ng][ld]
+__device__ __forceinline__ void cmv_back(const float* g, int ld, int ng, const float* __restrict__ W, bool vec, int H,
+                                         float* v) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int mb = 8 * warp; mb < H; mb += 8 * (CMV_THREADS / 32)) {
+    float acc[8] = {};
+    cmv_gemm_t(g, ld, ng, W + (size_t)mb * ng, H - mb, vec, acc);
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      if (mb + q < H) v[(mb + q) * ld + lane] *= acc[q];
+  }
+}
+
+template <bool INV, bool DEEP>
 __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const __grid_constant__ CmvParams P) {
   extern __shared__ float cmv_sm[];
   const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H, TG = 32 * P.nsub, FP = TG + 1, nmax = max(n1, n2);
+  const int M = DEEP ? P.depth : 1;
+  const size_t HB = (size_t)H * FP;     // one hidden block
   float* X2 = cmv_sm;                   // [n2][FP]   x₂
   float* ST = X2 + (size_t)n2 * FP;     // [2n1][FP]  ȳ₁, then s̄ | t̄
-  float* Hs = ST + (size_t)2 * n1 * FP; // [H][FP]    h
-  float* Vb = Hs + (size_t)H * FP;      // [H][FP]    σ′(v), then v̄
-  float* Sc = Vb + (size_t)H * FP;      // [max(n1, n2)][33]  one sub-tile: x₁ -> x̄₁, then W₁ᵀ v̄
+  float* Hs = ST + (size_t)2 * n1 * FP; // [M][H][FP] h_l
+  float* Vb = Hs + M * HB;              // [M][H][FP] σ′(v_l), then v̄_l
+  float* Sc = Vb + M * HB;              // [max(n1, n2)][33]  one sub-tile: x₁ -> x̄₁, then W₁ᵀ v̄
+  const float* hM = Hs + (M - 1) * HB;  // h_M, the input of W_out
   int* sidx1 = reinterpret_cast<int*>(Sc + (size_t)nmax * CMV_SP);  // [n1]
   int* sidx2 = sidx1 + n1;                                          // [n2]
   unsigned char* kind = reinterpret_cast<unsigned char*>(sidx2 + n2);  // [D]: 0 = a pass-through row
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float* slice = P.part ? P.part + (size_t)blockIdx.x * P.slice : nullptr;
-  float* sW1 = slice;
-  float* sc1 = sW1 + (size_t)H * n2;
-  float* sW2 = sc1 + H;
-  float* sc2 = sW2 + (size_t)2 * n1 * H;
+  float *sW1 = slice, *sWh = nullptr, *sc1, *sW2, *sc2;
+  if constexpr (DEEP) {  // [W̄_in | W̄_hid | W̄_out | c̄_1 … c̄_M c̄_out]
+    sWh = sW1 + (size_t)H * n2;
+    sW2 = sWh + (size_t)(M - 1) * H * H;
+    sc1 = sW2 + (size_t)2 * n1 * H;
+    sc2 = sc1 + (size_t)M * H;
+  } else {  // [W̄₁ | c̄₁ | W̄₂ | c̄₂]
+    sc1 = sW1 + (size_t)H * n2;
+    sW2 = sc1 + H;
+    sc2 = sW2 + (size_t)2 * n1 * H;
+  }
 
   for (int r = tid; r < D; r += CMV_THREADS) kind[r] = 0;
   if (slice)
@@ -130,6 +180,8 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
   const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
   const bool vec1t = ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
   const bool vec2t = ((n1 & 1) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
+  const bool vech = DEEP && ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
+  const bool vecht = DEEP && ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
   auto same = [](int k) { return k; };
 
   const long long groups = (P.N + TG - 1) / TG;
@@ -167,12 +219,19 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
         }
       }
       __syncthreads();
+      if constexpr (DEEP) {  // h_l = σ(W_l h_{l−1} + c_l), l = 2..M
+        for (int l = 1; l < M; ++l) {
+          cmv_hidden(Hs + (l - 1) * HB + co, FP, H, P.Wh + (size_t)(l - 1) * H * H, P.c1 ? P.c1 + (size_t)l * H : nullptr,
+                     vech, H, P.act, P.slope, Hs + l * HB + co, Vb + l * HB + co);
+          __syncthreads();
+        }
+      }
       // ---- [s; t] = W₂h + c₂, then x̄₁, s̄, t̄ of the affine law ---------------------------------------------------
       const long long mycol = n0 + co + lane;
       const float lb = P.ljbar && mycol < P.N ? P.ljbar[mycol] : 0.f;
       for (int jb = 4 * warp; jb < n1; jb += 4 * (CMV_THREADS / 32)) {
         float sv[4][1] = {}, tv[4][1] = {};
-        coupling_gemm_block<1>(Hs + co, FP, same, H, P.W2 + jb, P.W2 + n1 + jb, 2 * n1, n1 - jb, n1 - jb, vec2, sv, tv);
+        coupling_gemm_block<1>(hM + co, FP, same, H, P.W2 + jb, P.W2 + n1 + jb, 2 * n1, n1 - jb, n1 - jb, vec2, sv, tv);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int j = jb + q;
@@ -205,14 +264,21 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
           for (int k = lane; k < n1; k += 32) __stcs(P.xbar + col * P.ldxb + sidx1[k], Sc[k * CMV_SP + c]);
       }
       // ---- v̄ = (W₂ᵀ[s̄; t̄]) ⊙ σ′ ---------------------------------------------------------------------------------
+      float* VbM = Vb + (M - 1) * HB;  // v̄_M
       for (int mb = 8 * warp; mb < H; mb += 8 * (CMV_THREADS / 32)) {
         float acc[8] = {};
         cmv_gemm_t(ST + co, FP, 2 * n1, P.W2 + (size_t)mb * 2 * n1, H - mb, vec2t, acc);
 #pragma unroll
         for (int q = 0; q < 8; ++q)
-          if (mb + q < H) Vb[(mb + q) * FP + co + lane] *= acc[q];
+          if (mb + q < H) VbM[(mb + q) * FP + co + lane] *= acc[q];
       }
       __syncthreads();
+      if constexpr (DEEP) {  // v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}, l = M..2
+        for (int l = M - 1; l >= 1; --l) {
+          cmv_back(Vb + l * HB + co, FP, H, P.Wh + (size_t)(l - 1) * H * H, vecht, H, Vb + (l - 1) * HB + co);
+          __syncthreads();
+        }
+      }
       // ---- x̄₂ = ȳ₂ + W₁ᵀ v̄ ---------------------------------------------------------------------------------------
       for (int kb = 8 * warp; kb < n2; kb += 8 * (CMV_THREADS / 32)) {
         float acc[8] = {};
@@ -234,12 +300,16 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
     if (slice) {  // the group's parameter sums, added to the CTA's slice
       __syncthreads();
       cmv_outer(Vb, H, X2, n2, FP, gcols, sW1, sc1);
-      cmv_outer(ST, 2 * n1, Hs, H, FP, gcols, sW2, sc2);
+      if constexpr (DEEP)
+        for (int l = 1; l < M; ++l)
+          cmv_outer(Vb + l * HB, H, Hs + (l - 1) * HB, H, FP, gcols, sWh + (size_t)(l - 1) * H * H, sc1 + (size_t)l * H);
+      cmv_outer(ST, 2 * n1, hM, H, FP, gcols, sW2, sc2);
     }
   }
 }
 
-// the `nparts` slices summed in order; element e of the slice layout [W̄₁ | c̄₁ | W̄₂ | c̄₂] goes to its array (NULL: dropped)
+// the `nparts` slices summed in order; element e of the slice layout ([W̄₁ | c̄₁ | W̄₂ | c̄₂], DEEP:
+// [W̄_in | W̄_hid | W̄_out | c̄]) goes to its array (NULL: dropped)
 __global__ void __launch_bounds__(256) coupling_mlp_vjp_reduce_kernel(const float* __restrict__ part, int nparts, long long slice,
                                                                       long long l0, long long l1, long long l2, long long l3,
                                                                       float* __restrict__ o0, float* __restrict__ o1,
@@ -256,12 +326,18 @@ __global__ void __launch_bounds__(256) coupling_mlp_vjp_reduce_kernel(const floa
 }
 
 static long long cmv_param_floats(const b2b_layer_desc& d) {
-  return (long long)d.n2 * (d.n1 + 1) + (long long)2 * d.n0 * (d.n2 + 1);
+  long long n = 0;
+  for (int i = 0; i < 4; ++i) n += (long long)b2b_slot_len(d, i, 0);
+  return n;
 }
 static long long cmv_slice_floats(const b2b_layer_desc& d) { return (cmv_param_floats(d) + 63) & ~63LL; }
 
+// hidden layers whose factors the kernel keeps
+static int cmv_depth(const b2b_layer_desc& d) { return d.kind == B2B_COUPLING_DEEP_MLP ? d.n3 >> 8 : 1; }
+
 static size_t cmv_smem_bytes(const b2b_layer_desc& d, int D, int nsub) {
-  const size_t f = (size_t)(d.n1 + 2 * d.n0 + 2 * d.n2) * (32 * nsub + 1) + (size_t)(d.n0 > d.n1 ? d.n0 : d.n1) * CMV_SP;
+  const size_t f = (size_t)(d.n1 + 2 * d.n0 + 2 * cmv_depth(d) * d.n2) * (32 * nsub + 1) +
+                   (size_t)(d.n0 > d.n1 ? d.n0 : d.n1) * CMV_SP;
   return (f * sizeof(float) + (size_t)(d.n0 + d.n1) * sizeof(int) + D + 15) & ~(size_t)15;
 }
 
@@ -282,11 +358,15 @@ static int cmv_grid(const b2b_layer_desc& d, int D, long long N) {
   return g < 1 ? 1 : (int)g;
 }
 
+static bool cmv_fits(const b2b_layer_desc& d, int D) {
+  return d.kind == B2B_COUPLING_DEEP_MLP ? b2b_coupling_deep_mlp_fits(d, D) : b2b_coupling_mlp_fits(d, D);
+}
+
 }  // namespace b2b
 
 size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
   using namespace b2b;
-  if (!b2b_coupling_mlp_fits(d, D)) return 0;
+  if (!cmv_fits(d, D)) return 0;
   return (size_t)cmv_grid(d, D, N) * (size_t)cmv_slice_floats(d) * sizeof(float) + 256;
 }
 
@@ -296,7 +376,8 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   const int D = s.D;
   const long long N = s.N;
   float* const* bars = s.bars;
-  if (!b2b_coupling_mlp_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (!cmv_fits(d, D)) return B2B_EUNSUPPORTED;
+  const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
   const bool want = bars[0] || bars[1] || bars[2] || bars[3];
   if (want && (!s.workspace || s.workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
   char* wsb = b2b_align256(s.workspace);
@@ -305,10 +386,23 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.ybar = s.ybar;
   P.ljbar = s.ljbar;
   P.xbar = s.xbar;
-  P.W1 = d.p0;
-  P.c1 = d.p1;
-  P.W2 = d.p2;
-  P.c2 = d.p3;
+  if (deep) {  // p0 = W_in, p1 = W_hid, p2 = W_out, p3 = [c_1 | … | c_M | c_out] or NULL; n3 = σ | M << 8
+    P.W1 = d.p0;
+    P.Wh = d.p1;
+    P.W2 = d.p2;
+    P.depth = d.n3 >> 8;
+    P.c1 = d.p3;
+    P.c2 = d.p3 ? d.p3 + (size_t)P.depth * d.n2 : nullptr;
+    P.act = d.n3 & 255;
+  } else {
+    P.W1 = d.p0;
+    P.c1 = d.p1;
+    P.W2 = d.p2;
+    P.c2 = d.p3;
+    P.Wh = nullptr;
+    P.depth = 1;
+    P.act = d.n3;
+  }
   P.idx1 = d.i0;
   P.idx2 = d.i1;
   P.part = want ? reinterpret_cast<float*>(wsb) : nullptr;
@@ -321,21 +415,24 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.n1 = d.n0;
   P.n2 = d.n1;
   P.H = d.n2;
-  P.act = d.n3;
   P.nsub = cmv_nsub(d, D);
   P.slope = d.f0;
   const int grid = cmv_grid(d, D, N);
   const size_t smem = cmv_smem_bytes(d, D, P.nsub);
-  void (*kernel)(const CmvParams) = d.inverse ? coupling_mlp_vjp_kernel<true> : coupling_mlp_vjp_kernel<false>;
+  void (*kernel)(const CmvParams) = deep ? (d.inverse ? coupling_mlp_vjp_kernel<true, true> : coupling_mlp_vjp_kernel<false, true>)
+                                         : (d.inverse ? coupling_mlp_vjp_kernel<true, false> : coupling_mlp_vjp_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CMV_THREADS, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   ++*s.launches;
   if (want) {
-    const long long l0 = (long long)d.n2 * d.n1, l1 = d.n2, l2 = (long long)2 * d.n0 * d.n2, l3 = 2 * d.n0;
-    coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l0 + l1 + l2 + l3 + 255) / 256), 256, 0, s.stream>>>(
-        P.part, grid, P.slice, l0, l1, l2, l3, bars[0], bars[1], bars[2], bars[3]);
+    // the slice holds the four slots in the order of p0 .. p3
+    long long l[4];
+    for (int i = 0; i < 4; ++i) l[i] = (long long)b2b_slot_len(d, i, D);
+    float* o[4] = {bars[0], bars[1], bars[2], bars[3]};
+    coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l[0] + l[1] + l[2] + l[3] + 255) / 256), 256, 0, s.stream>>>(
+        P.part, grid, P.slice, l[0], l[1], l[2], l[3], o[0], o[1], o[2], o[3]);
     if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
     ++*s.launches;
   }

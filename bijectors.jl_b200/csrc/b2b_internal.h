@@ -144,6 +144,8 @@ size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long 
 // neural-network coupling (b2b_coupling_mlp.cu, b2b_coupling_mlp_vjp.cu): whether the layer is within the envelope of
 // include/b2b.h
 bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D);
+// the deep-network coupling (B2B_COUPLING_DEEP_MLP) runs on the same kernels and launchers
+bool b2b_coupling_deep_mlp_fits(const b2b_layer_desc& d, int D);
 int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
                             long long ldx, long long ldy, int accumulate, cudaStream_t stream);
 // reverse mode: with any parameter cotangent b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope,
@@ -153,7 +155,7 @@ size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long 
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
-// COUPLING_RQS, SCALE_MATRIX, COUPLING_MLP and COUPLING_MLP_RQS).
+// COUPLING_RQS, SCALE_MATRIX, COUPLING_MLP, COUPLING_MLP_RQS and COUPLING_DEEP_MLP).
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);
@@ -204,7 +206,7 @@ int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / P
 int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
 int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS and COUPLING_MLP_RQS
 int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu
-int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu
+int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
 // One launch copying slot i of layer j from base[i] + j·step[i] to bars[4j + i], for the requested slots of a run of
 // n <= 8 layers at D (nothing is launched when none is requested).
 int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, const float* const base[3],
@@ -255,6 +257,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_SCALE_MATRIX,    B2B_F_P0,                    false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        false},
       {B2B_COUPLING_MLP,    B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P1 | B2B_F_P3, false},
       {B2B_COUPLING_MLP_RQS, B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P1 | B2B_F_P3, false},
+      {B2B_COUPLING_DEEP_MLP, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P3, false},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -302,6 +305,12 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
            (act == B2B_ACT_TANH || act == B2B_ACT_LEAKY_RELU) && d.f1 > 0;
       break;
     }
+    case B2B_COUPLING_DEEP_MLP: {  // n3 = σ | M << 8
+      const int act = d.n3 & 255, M = d.n3 >> 8;
+      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && M >= 2 &&
+           (act == B2B_ACT_TANH || act == B2B_ACT_LEAKY_RELU);
+      break;
+    }
     default: break;
   }
   return ok ? B2B_OK : B2B_EINVAL;
@@ -325,6 +334,11 @@ size_t b2b_slot_len(const Desc& d, int i, int D) {
     case B2B_COUPLING_MLP_RQS: {  // W₁ (H x n2), c₁ (H), W₂ ((3K−1)n1 x H), c₂ ((3K−1)n1)
       const size_t J = (size_t)(3 * (d.n3 >> 8) - 1) * d.n0;
       const size_t len[4] = {(size_t)d.n2 * d.n1, (size_t)d.n2, J * d.n2, J};
+      return len[i];
+    }
+    case B2B_COUPLING_DEEP_MLP: {  // W_in (H x n2), W_hid ((M−1) x H x H), W_out (2n1 x H), c (M·H + 2n1)
+      const size_t H = d.n2, M = d.n3 >> 8;
+      const size_t len[4] = {H * d.n1, (M - 1) * H * H, (size_t)2 * d.n0 * H, M * H + (size_t)2 * d.n0};
       return len[i];
     }
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ

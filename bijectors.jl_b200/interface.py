@@ -824,6 +824,10 @@ _SLOTS = {
     _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"),
                             lambda d, D: ((d.n1, d.n2), (d.n2,), (d.n2, (3 * (d.n3 >> 8) - 1) * d.n0), ((3 * (d.n3 >> 8) - 1) * d.n0,)),
                             (0, 2)),
+    _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"),
+                             lambda d, D: ((d.n1, d.n2), ((d.n3 >> 8) - 1, d.n2, d.n2), (d.n2, 2 * d.n0),
+                                           ((d.n3 >> 8) * d.n2 + 2 * d.n0,)),
+                             (0, 1, 2)),
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 
@@ -842,7 +846,8 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
 def _slot_grads(d, l: int, bars) -> dict:
     """The cotangents ``bars`` holds for descriptor l (``d``), keyed by field name, each in its parameter's orientation."""
     names, _, colmajor = _SLOTS.get(d.kind, ((), None, ()))
-    return {name: bars[(l, i)].t() if i in colmajor else bars[(l, i)] for i, name in enumerate(names) if (l, i) in bars}
+    return {name: bars[(l, i)].transpose(-1, -2) if i in colmajor else bars[(l, i)]
+            for i, name in enumerate(names) if (l, i) in bars}
 
 
 # per batch dtype: (name, descriptor type, workspace query, entry point)

@@ -42,6 +42,7 @@ const COUPLING_RQS = Int32(11)  # 10 is not a layer kind (include/b2b.h)
 const SCALE_MATRIX = Int32(12)
 const COUPLING_MLP = Int32(13)
 const COUPLING_MLP_RQS = Int32(14)
+const COUPLING_DEEP_MLP = Int32(15)
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -170,9 +171,42 @@ function desc(cl::Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}}, inv::Bo
     LayerDesc(COUPLING_MLP_RQS, inv, length(dm.idx1), length(dm.idx2), size(θ.W1, 1), θ.act | (Int32(θ.K) << 8),
               θ.slope, θ.B, pointer(θ.W1), ptr(θ.c1), pointer(θ.W2), ptr(θ.c2), pointer(dm.idx1), pointer(dm.idx2))
 end
+# The RealNVP law of MLPConditioner with M >= 2 hidden layers, a Flux Chain(Dense(n2, H, σ), Dense(H, H, σ), …,
+# Dense(H, 2n1)): h_1 = σ.(W_in*x₂ .+ c_1), h_l = σ.(W_hid[:, :, l−1]*h_{l−1} .+ c_l), [s; t] = W_out*h_M .+ c_out.  W_hid
+# is H × H × (M−1), whose memory order is the packed layout of the descriptor; c packs [c_1; …; c_M; c_out] or is
+# `nothing` (no biases at all).  A callable, so the same object also runs on the CPU reference path.  Float32,
+# n1, n2 <= 128, H <= 128, M <= 4, D <= 1024 on the device.
+struct DeepMLPConditioner{M<:AbstractMatrix,A<:AbstractArray,V}
+    W_in::M   # (H × n2)
+    W_hid::A  # (H × H × (M−1))
+    W_out::M  # (2n1 × H)
+    c::V      # M·H + 2n1, or nothing
+    act::Int32      # ACT_TANH or ACT_LEAKY_RELU
+    slope::Float32
+end
+function (θ::DeepMLPConditioner)(x₂)
+    H, M = size(θ.W_in, 1), size(θ.W_hid, 3) + 1
+    σ(v) = θ.act == ACT_TANH ? tanh.(v) : ifelse.(v .>= 0, v, θ.slope .* v)
+    bias(l) = θ.c === nothing ? false : θ.c[((l - 1) * H + 1):(l * H)]
+    h = σ(θ.W_in * x₂ .+ bias(1))
+    for l in 2:M
+        h = σ(θ.W_hid[:, :, l - 1] * h .+ bias(l))
+    end
+    st = θ.c === nothing ? θ.W_out * h : θ.W_out * h .+ θ.c[(M * H + 1):end]
+    n = length(st) ÷ 2
+    Shift(st[(n + 1):end]) ∘ Scale(exp.(st[1:n]))
+end
+function desc(cl::Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}}, inv::Bool)
+    dm = get!(() -> DeviceMask(cl.mask), MASKS, cl.mask)
+    θ = cl.θ
+    M = size(θ.W_hid, 3) + 1
+    LayerDesc(COUPLING_DEEP_MLP, inv, length(dm.idx1), length(dm.idx2), size(θ.W_in, 1), θ.act | (Int32(M) << 8),
+              θ.slope, 0f0, pointer(θ.W_in), pointer(θ.W_hid), pointer(θ.W_out), θ.c === nothing ? NULLF : pointer(θ.c),
+              pointer(dm.idx1), pointer(dm.idx2))
+end
 desc(cl::Coupling, ::Bool) =
-    error("Coupling: only AffineConditioner, SplineConditioner, MLPConditioner and MLPSplineConditioner laws run on the " *
-          "device path (no CPU fallback)")
+    error("Coupling: only AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner and " *
+          "DeepMLPConditioner laws run on the device path (no CPU fallback)")
 
 # Permute(A): y[dst[i]] = x[i] with dst = the row of the single 1 in column i (permute.jl:90-100,152)
 const PERMS = IdDict{Any,CuVector{Int32}}()
@@ -227,6 +261,7 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           RationalQuadraticSpline{<:CuMatrix{Float32}},InvertibleBatchNorm{<:CuVector{Float32}},
                           Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
+                          Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
                           Scale{<:CuMatrix{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
@@ -441,6 +476,9 @@ function vjp_slots(d::LayerDesc, D::Integer)
     d.kind == COUPLING_MLP_RQS && return (J = (3(d.n3 >> 8) - 1) * d.n0;
                                           (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(J, d.n2),
                                            d.p3 == NULLF ? nothing : z(J)))
+    d.kind == COUPLING_DEEP_MLP && return (M = d.n3 >> 8;
+                                           (z(d.n2, d.n1), z(d.n2, d.n2, M - 1), z(2d.n0, d.n2),
+                                            d.p3 == NULLF ? nothing : z(M * d.n2 + 2d.n0)))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

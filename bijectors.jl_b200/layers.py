@@ -320,31 +320,40 @@ class _NetworkConditioner:
     """A conditioner whose parameters come from a hidden layer h = σ.(W₁·x₂ + c₁) and a last layer W₂·h + c₂."""
 
     _ACT = _ACT
+    _fields = ("W1", "c1", "W2", "c2")  # the device tensors, in the order of the descriptor's p0 .. p3
 
-    def _hidden_layer(self, who, W1, c1, activation, slope, dtype, device):
-        """Checks the hidden layer and sets activation, slope, H, n2, W1 (column-major) and c1 (None: NULL pointer)."""
+    def _network(self, who, activation, slope, dtype):
+        """Checks the element type and the activation and sets activation and slope."""
         if dtype != torch.float32:
             raise TypeError(f"{who}: the network coupling layers run in Float32 only")
         if activation not in _ACT:
             raise ValueError(f"{who}: activation must be one of {sorted(_ACT)}, got {activation!r}")
-        W1n = _host32(W1)
-        if W1n.ndim != 2 or W1n.shape[0] == 0:
-            raise ValueError(f"W1 must be (H, n2), got {W1n.shape}")
         self.activation, self.slope = activation, float(slope)
-        self.H, self.n2 = W1n.shape
-        self.W1 = _dev_f32(np.ascontiguousarray(W1n.T), device)  # column-major (H × n2)
+
+    def _first_layer(self, name, W):
+        """Checks the input layer (H × n2), sets H and n2 and returns it column-major on the host."""
+        Wn = _host32(W)
+        if Wn.ndim != 2 or Wn.shape[0] == 0:
+            raise ValueError(f"{name} must be (H, n2), got {Wn.shape}")
+        self.H, self.n2 = Wn.shape
+        return np.ascontiguousarray(Wn.T)
+
+    def _hidden_layer(self, who, W1, c1, activation, slope, dtype, device):
+        """Checks the hidden layer and sets activation, slope, H, n2, W1 (column-major) and c1 (None: NULL pointer)."""
+        self._network(who, activation, slope, dtype)
+        self.W1 = _dev_f32(self._first_layer("W1", W1), device)  # column-major (H × n2)
         self.c1 = _bias(c1, "c1", self.H, device)
 
     def to(self, device):
         new = object.__new__(type(self))
         new.__dict__.update(self.__dict__)
-        for k in ("W1", "c1", "W2", "c2"):
+        for k in self._fields:
             t = getattr(self, k)
             setattr(new, k, None if t is None else t.to(device))
         return new
 
     def _tensors(self):
-        return (self.W1, self.c1, self.W2, self.c2)
+        return tuple(getattr(self, k) for k in self._fields)
 
 
 class MLPConditioner(_NetworkConditioner):
@@ -382,19 +391,80 @@ class MLPSplineConditioner(_NetworkConditioner):
         self.c2 = _bias(c2, "c2", W2n.shape[0], device)
 
 
+class DeepMLPConditioner(_NetworkConditioner):
+    """The RealNVP coupling law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) of :class:`MLPConditioner` with a deeper network, a
+    Flux ``Chain(Dense(n2, H, σ), Dense(H, H, σ), …, Dense(H, 2n1))``: h_1 = σ.(W_in·x₂ + c_1), h_l = σ.(W_l·h_{l−1} + c_l)
+    for l = 2..M, [s; t] = W_out·h_M + c_out.  ``weights = [W_in (H × n2), W_2 … W_M (H × H), W_out (2·n1 × H)]`` in the
+    reference's index order, M >= 2 hidden layers, rows 1..n1 of W_out giving s.  ``biases`` is None (no biases at all,
+    the descriptor's pointer is NULL) or all M + 1 vectors ``[c_1 … c_M (H each), c_out (2·n1)]``, so that training never
+    adds a bias the network did not have.  Float32 only.  Runs as B2B_COUPLING_DEEP_MLP: n1, n2 <= 128, H <= 128,
+    M <= 4, D <= 1024.  Device tensors: W_in, W_hid (M−1, H, H: each matrix column-major, back to back), W_out and c
+    (every bias packed); ``weights`` / ``biases`` give per-layer views in the reference's orientation."""
+
+    _fields = ("W_in", "W_hid", "W_out", "c")
+
+    def __init__(self, weights, biases=None, *, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+        self._network("DeepMLPConditioner", activation, slope, dtype)
+        weights = list(weights)
+        if len(weights) < 3:
+            raise ValueError(f"DeepMLPConditioner: weights must be [W_in, W_2, …, W_M, W_out] with M >= 2 hidden layers "
+                             f"(one hidden layer is MLPConditioner), got {len(weights)} matrices")
+        self.M = len(weights) - 1
+        W_in = self._first_layer("W_in", weights[0])
+        H = self.H
+        hid = [_host32(W) for W in weights[1:-1]]
+        for l, W in enumerate(hid, start=2):
+            if W.shape != (H, H):
+                raise ValueError(f"W_{l} must be (H, H) with H = {H}, got {W.shape}")
+        W_out = _host32(weights[-1])
+        if W_out.ndim != 2 or W_out.shape[0] == 0 or W_out.shape[0] % 2 or W_out.shape[1] != H:
+            raise ValueError(f"W_out must be (2*n1, H) with H = {H}, got {W_out.shape}")
+        self.n1 = W_out.shape[0] // 2
+        self.W_in = _dev_f32(W_in, device)  # column-major (H × n2)
+        self.W_hid = _dev_f32(np.ascontiguousarray(np.stack([W.T for W in hid])), device)  # [l − 2] = W_l column-major
+        self.W_out = _dev_f32(np.ascontiguousarray(W_out.T), device)  # column-major (2n1 × H)
+        self.c = None
+        if biases is not None:
+            biases = list(biases)
+            if len(biases) != self.M + 1:
+                raise ValueError(f"biases must be None or all {self.M + 1} vectors [c_1, …, c_{self.M}, c_out], "
+                                 f"got {len(biases)}")
+            names = [f"c_{l}" for l in range(1, self.M + 1)] + ["c_out"]
+            sizes = [H] * self.M + [2 * self.n1]
+            parts = [_host32(b).reshape(-1) for b in biases]
+            for name, n, b in zip(names, sizes, parts):
+                if b.shape != (n,):
+                    raise ValueError(f"{name} must have {n} entries, got {b.shape}")
+            self.c = _dev_f32(np.concatenate(parts), device)
+
+    @property
+    def weights(self):
+        """[W_in, W_2, …, W_M, W_out] as views of the device tensors, in the reference's orientation."""
+        return [self.W_in.t()] + [W.t() for W in self.W_hid] + [self.W_out.t()]
+
+    @property
+    def biases(self):
+        """[c_1, …, c_M, c_out] as views of the packed bias, or None."""
+        if self.c is None:
+            return None
+        H, M = self.H, self.M
+        return [self.c[l * H:(l + 1) * H] for l in range(M)] + [self.c[M * H:]]
+
+
 class Coupling(_ParamLayer):
     """Coupling(θ, mask) (coupling.jl:178-181).  θ is an arbitrary closure in the reference; the device
-    path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner`, :class:`MLPConditioner` and
-    :class:`MLPSplineConditioner` and raises for anything else (no CPU fallback)."""
+    path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner`, :class:`MLPConditioner`,
+    :class:`MLPSplineConditioner` and :class:`DeepMLPConditioner` and raises for anything else (no CPU fallback)."""
 
     _fields = ()
 
     def __init__(self, θ, mask, device="cuda"):
         if isinstance(mask, int):  # Coupling(θ, n): first n÷2 rows transformed (:183-186)
             mask = PartitionMask(mask, range(1, mask // 2 + 1))
-        if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner)):
-            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner, MLPConditioner "
-                                                  "and MLPSplineConditioner laws run on the device path")
+        if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner,
+                              DeepMLPConditioner)):
+            raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner, MLPConditioner, "
+                                                  "MLPSplineConditioner and DeepMLPConditioner laws run on the device path")
         if θ.n1 != len(mask.indices_1) or θ.n2 != len(mask.indices_2):
             raise ValueError("conditioner shape does not match the PartitionMask")
         self.θ, self.mask = θ, mask
@@ -427,6 +497,11 @@ class Coupling(_ParamLayer):
             return [_desc(_lib.COUPLING_MLP, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
                           p3=θ.c2 if θ.c2 is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
                           n3=θ._ACT[θ.activation], f0=θ.slope)]
+        if isinstance(self.θ, DeepMLPConditioner):
+            θ = self.θ
+            return [_desc(_lib.COUPLING_DEEP_MLP, inverse, p0=θ.W_in, p1=θ.W_hid, p2=θ.W_out,
+                          p3=θ.c if θ.c is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
+                          n3=θ._ACT[θ.activation] | (θ.M << 8), f0=θ.slope)]
         if isinstance(self.θ, MLPSplineConditioner):
             θ = self.θ
             return [_desc(_lib.COUPLING_MLP_RQS, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
@@ -445,7 +520,9 @@ class Coupling(_ParamLayer):
             return False
         if isinstance(self.θ, MLPSplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
             return False
-        if isinstance(self.θ, (MLPConditioner, MLPSplineConditioner)) and \
+        if isinstance(self.θ, DeepMLPConditioner) and self.θ.M != o.θ.M:
+            return False
+        if isinstance(self.θ, (MLPConditioner, MLPSplineConditioner, DeepMLPConditioner)) and \
                 (self.θ.activation, self.θ.slope) != (o.θ.activation, o.θ.slope):
             return False
         return all((a is None) == (b is None) and (a is None or torch.equal(a, b))
