@@ -57,6 +57,26 @@ extern "C" int b2b_set_kernel_variant(int variant) {
   return B2B_OK;
 }
 
+// one row of limits per kind of b2b_coupling
+bool b2b_coupling_fits(const b2b_layer_desc& d, int D) {
+  struct Limits { int kind, n, h_lo, h_hi, k_lo, k_hi, m_lo, m_hi, d; };
+  static const Limits rows[] = {  // kind, n1 and n2, H, K, M, D
+      {B2B_COUPLING_RQS, B2B_COUPLING_RQS_MAX_N, 0, 0, 2, B2B_COUPLING_RQS_MAX_K, 0, 0, B2B_COUPLING_RQS_MAX_D},
+      {B2B_COUPLING_MLP, B2B_COUPLING_MLP_MAX_N, 1, B2B_COUPLING_MLP_MAX_H, 0, 0, 1, 1, B2B_COUPLING_MLP_MAX_D},
+      {B2B_COUPLING_MLP_RQS, B2B_COUPLING_MLP_RQS_MAX_N, 1, B2B_COUPLING_MLP_RQS_MAX_H, 2, B2B_COUPLING_MLP_RQS_MAX_K,
+       1, 1, B2B_COUPLING_MLP_RQS_MAX_D},
+      {B2B_COUPLING_DEEP_MLP, B2B_COUPLING_DEEP_MLP_MAX_N, 1, B2B_COUPLING_DEEP_MLP_MAX_H, 0, 0,
+       2, B2B_COUPLING_DEEP_MLP_MAX_DEPTH, B2B_COUPLING_DEEP_MLP_MAX_D},
+  };
+  const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
+  auto in = [](int v, int lo, int hi) { return v >= lo && v <= hi; };
+  for (const Limits& r : rows)
+    if (r.kind == d.kind)
+      return in(c.n1, 1, r.n) && in(c.n2, 1, r.n) && in(c.H, r.h_lo, r.h_hi) && in(c.K, r.k_lo, r.k_hi) &&
+             in(c.M, r.m_lo, r.m_hi) && D <= r.d;
+  return false;
+}
+
 // Float32 envelope of a valid layer at D: B2B_EUNSUPPORTED when its forward kernel does not take it, else B2B_OK.  The
 // fused kinds are also bound by their run's shared-memory budget, which plan_segments checks.
 static int fwd_envelope(const b2b_layer_desc& d, int D) {
@@ -64,13 +84,9 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
   switch (d.kind) {
     case B2B_RQS: ok = d.n0 <= 64; break;
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_fits(d.n0, d.n1, D); break;
-    case B2B_COUPLING_RQS: ok = b2b_coupling_rqs_fits(d, D); break;
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
-    case B2B_COUPLING_MLP: ok = b2b_coupling_mlp_fits(d, D); break;
-    case B2B_COUPLING_MLP_RQS: ok = b2b_coupling_mlp_rqs_fits(d, D); break;
-    case B2B_COUPLING_DEEP_MLP: ok = b2b_coupling_deep_mlp_fits(d, D); break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
-    default: break;
+    default: ok = !b2b_is_coupling(d.kind) || b2b_coupling_fits(d, D); break;  // the other couplings' table
   }
   return ok ? B2B_OK : B2B_EUNSUPPORTED;
 }
@@ -83,13 +99,11 @@ static int vjp_envelope(const b2b_layer_desc& d, int D) {
     case B2B_RADIAL: ok = D <= 128; break;
     case B2B_RQS: ok = D <= 256 && d.n0 <= 64; break;
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_vjp_fits(d, D); break;
-    case B2B_COUPLING_RQS:
-    case B2B_SCALE_MATRIX:
-    case B2B_COUPLING_MLP:
-    case B2B_COUPLING_MLP_RQS:
-    case B2B_COUPLING_DEEP_MLP:
-    case B2B_MVNORMAL_TRIL: return fwd_envelope(d, D);
-    default: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
+    case B2B_BATCHNORM:
+    case B2B_PERMUTE:
+    case B2B_STACKED_EW:
+    case B2B_MVNORMAL_DIAG: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
+    default: return fwd_envelope(d, D);
   }
   return ok ? B2B_OK : B2B_EUNSUPPORTED;
 }
@@ -103,19 +117,12 @@ static int validate_layer(const b2b_layer_desc& d, int D, bool last) {
   return launch == B2B_LC_COUPLING || launch == B2B_LC_TRIL ? B2B_OK : fwd_envelope(d, D);
 }
 
-// number of kernel launches the last launch_fused enqueued (the constant-bank path adds a prep kernel and a copy)
-static thread_local int g_fused_launches = 1;
-
 static int launch_fused(B2BChainParams& p, cudaStream_t stream) {
   int rc = B2B_EUNSUPPORTED;
-  g_fused_launches = 1;
   // segments made of <= 8 PlanarLayers: the fused planar chain kernel (variant 3 forces, 1 / 2 disable)
   if (g_variant == 0 || g_variant == 3) {
     rc = b2b_launch_planar_chain_const(p, stream);
-    if (rc == B2B_OK) {
-      g_fused_launches = 1;
-      return rc;
-    }
+    if (rc == B2B_OK) return rc;
     if (g_variant == 3 || rc != B2B_EUNSUPPORTED) return rc;
   }
   if (g_variant == 0 && b2b_radial_unrolled_applicable(p)) {  // inverse radial chains: specialised program
@@ -148,6 +155,62 @@ static int fused_grid(const B2BChainParams& p) {
     if (g > 0) return g;
   }
   return b2b_chain_grid_size_v0(p);
+}
+
+// A run of fused column-local layers: one launch of the kernel launch_fused picks (with a batch sum, a second adding its
+// per-CTA partials)
+static int fwd_fused(const B2BFwdSeg& s) {
+  B2BChainParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = s.x;
+  p.y = s.y;
+  p.logjac = s.logjac;
+  p.N = s.N;
+  p.ldx = s.ldx;
+  p.ldy = s.ldy;
+  p.D = s.D;
+  p.L = s.n;
+  p.accumulate = s.accumulate;
+  for (int l = 0; l < p.L; ++l) p.layers[l] = s.layers[l];
+  int grid = 0;
+  if (s.partials) {
+    grid = fused_grid(p);
+    if (grid <= 0 || grid > 4096) return B2B_EUNSUPPORTED;
+    p.partials = s.partials;
+  }
+  int rc = launch_fused(p, s.stream);
+  if (rc != B2B_OK) return rc;
+  ++*s.launches;
+  if (!s.partials) return B2B_OK;
+  if ((rc = b2b_launch_sum_partials(s.partials, grid, s.sum_out, s.stream)) != B2B_OK) return rc;
+  ++*s.launches;
+  return B2B_OK;
+}
+
+// An affine coupling, with the BatchNorm neighbours folded into it: the fold table's preparation, then the tensor-core
+// kernel when the layer and the workspace fit it (and b2b_set_kernel_variant does not rule it out), else the exact-fp32
+// kernel
+static int fwd_coupling(const B2BFwdSeg& s) {
+  const b2b_layer_desc& d = s.layers[0];
+  const float* fold = nullptr;
+  int rc;
+  if (s.pre || s.post) {
+    if ((rc = b2b_launch_bn_fold_prep(s.pre, s.post, s.D, s.fold, s.stream)) != B2B_OK) return rc;
+    ++*s.launches;
+    fold = s.fold;
+  }
+  rc = B2B_EUNSUPPORTED;
+  if (s.workspace && g_coupling_variant != 1) {
+    int n = 0;  // W preparation + main kernel (+ fp32 kernel on a ragged tail)
+    rc = b2b_launch_coupling_affine_tc(d, fold, s.x, s.y, s.logjac, s.D, s.N, s.ldx, s.ldy, s.accumulate, s.workspace,
+                                       s.workspace_bytes, &n, s.stream);
+    if (rc == B2B_OK) *s.launches += n;
+  }
+  if (rc == B2B_EUNSUPPORTED) {
+    rc = b2b_launch_coupling_affine(d, fold, s.x, s.y, s.logjac, s.D, s.N, s.ldx, s.ldy, s.accumulate, s.stream);
+    if (rc == B2B_OK) ++*s.launches;
+  }
+  return rc;
 }
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -375,92 +438,26 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
   // accumulate_logjac adds onto the caller's logjac; the workspace slice is written by the first launch
   bool lj_started = accumulate_logjac != 0 && !lj_ws;
   for (size_t s = 0; s < segs.size(); ++s) {
+    const Seg& g = segs[s];
     const bool last_seg = s + 1 == segs.size();
     // destination of this segment: y when given, else scratch for intermediates, nothing for the last
     float* dst = y ? y : (last_seg ? nullptr : scratch);
     const long long dst_ld = y ? ldy : D;
-    const b2b_layer_desc& d = layers[segs[s].begin];
-    const int acc = lj_started ? 1 : 0;
-    int rc, n_launch = 0;
-    switch (segs[s].launch) {
-      case B2B_LC_COUPLING: {
-        const float* fold = nullptr;
-        if (segs[s].pre >= 0 || segs[s].post >= 0) {
-          rc = b2b_launch_bn_fold_prep(segs[s].pre >= 0 ? &layers[segs[s].pre] : nullptr,
-                                       segs[s].post >= 0 ? &layers[segs[s].post] : nullptr, D, fold_ws, stream);
-          if (rc != B2B_OK) return rc;
-          ++g_last_launches;
-          fold = fold_ws;
-        }
-        rc = B2B_EUNSUPPORTED;
-        if (tc_ws && g_coupling_variant != 1) {
-          rc = b2b_launch_coupling_affine_tc(d, fold, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, tc_ws, tc_bytes,
-                                             &n_launch, stream);
-          if (rc == B2B_OK) g_last_launches += n_launch;  // W preparation + main kernel (+ fp32 kernel on a ragged tail)
-        }
-        if (rc == B2B_EUNSUPPORTED) {
-          rc = b2b_launch_coupling_affine(d, fold, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
-          if (rc == B2B_OK) ++g_last_launches;
-        }
-        if (rc != B2B_OK) return rc;
-        break;
-      }
-      case B2B_LC_SPLINE:
-        rc = b2b_launch_coupling_rqs(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
-        if (rc != B2B_OK) return rc;
-        ++g_last_launches;
-        break;
-      case B2B_LC_MLP:
-        rc = b2b_launch_coupling_mlp(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, stream);
-        if (rc != B2B_OK) return rc;
-        ++g_last_launches;
-        break;
-      case B2B_LC_SCALE:
-        rc = b2b_launch_scale_matrix(d, cur, dst, logjac, D, N, cur_ld, dst_ld, acc, scale_ws, scale_bytes, &n_launch,
-                                     stream);
-        g_last_launches += n_launch;
-        if (rc != B2B_OK) return rc;
-        break;
-      case B2B_LC_TRIL:  // always the last segment
-        rc = b2b_launch_mvnormal_tril(d, cur, cur_ld, dst, dst_ld, logjac, acc, sum_out ? partials : nullptr, D, N, stream);
-        if (rc != B2B_OK) return rc;
-        ++g_last_launches;
-        if (sum_out) {
-          rc = b2b_launch_sum_partials(partials, b2b_tril_grid(D, N), sum_out, stream);
-          if (rc != B2B_OK) return rc;
-          ++g_last_launches;
-        }
-        break;
-      case B2B_LC_FUSED: {
-        B2BChainParams p;
-        memset(&p, 0, sizeof(p));
-        p.x = cur;
-        p.y = dst;
-        p.logjac = logjac;
-        p.N = N;
-        p.ldx = cur_ld;
-        p.ldy = dst_ld;
-        p.D = D;
-        p.L = segs[s].end - segs[s].begin;
-        p.accumulate = acc;
-        for (int l = 0; l < p.L; ++l) p.layers[l] = layers[segs[s].begin + l];
-        int grid = 0;
-        if (sum_out && last_seg) {
-          grid = fused_grid(p);
-          if (grid <= 0 || grid > 4096) return B2B_EUNSUPPORTED;
-          p.partials = partials;
-        }
-        rc = launch_fused(p, stream);
-        if (rc != B2B_OK) return rc;
-        g_last_launches += g_fused_launches;
-        if (sum_out && last_seg) {
-          rc = b2b_launch_sum_partials(partials, grid, sum_out, stream);
-          if (rc != B2B_OK) return rc;
-          ++g_last_launches;
-        }
-        break;
-      }
+    const bool cpl = g.launch == B2B_LC_COUPLING, sc = g.launch == B2B_LC_SCALE;  // the classes with a workspace slice
+    const B2BFwdSeg a{layers + g.begin, g.end - g.begin, cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0, D, N,
+                      g.pre >= 0 ? &layers[g.pre] : nullptr, g.post >= 0 ? &layers[g.post] : nullptr, fold_ws,
+                      last_seg ? partials : nullptr, sum_out, cpl ? tc_ws : sc ? scale_ws : nullptr,
+                      cpl ? tc_bytes : sc ? scale_bytes : 0, &g_last_launches, stream};
+    int rc;
+    switch (g.launch) {
+      case B2B_LC_COUPLING: rc = fwd_coupling(a); break;
+      case B2B_LC_SPLINE: rc = b2b_fwd_spline(a); break;
+      case B2B_LC_MLP: rc = b2b_fwd_mlp(a); break;
+      case B2B_LC_SCALE: rc = b2b_fwd_scale(a); break;
+      case B2B_LC_TRIL: rc = b2b_fwd_tril(a); break;  // always the last segment
+      default: rc = fwd_fused(a); break;
     }
+    if (rc != B2B_OK) return rc;
     if (dst) {
       cur = dst;
       cur_ld = dst_ld;

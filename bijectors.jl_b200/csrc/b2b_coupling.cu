@@ -256,9 +256,7 @@ int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const
                                int D, long long N, long long ldx, long long ldy, int accumulate,
                                cudaStream_t stream) {
   using namespace b2b;
-  const int n1 = d.n0, n2 = d.n1;
-  if (n1 < 1 || n2 < 1 || n1 + n2 > D || !d.p0) return B2B_EINVAL;
-  if ((!d.i0 && d.n2 < 0) || (!d.i1 && d.n3 < 0)) return B2B_EINVAL;
+  const int n1 = d.n0, n2 = d.n1;  // a valid descriptor (b2b_check_desc)
   if (!b2b_coupling_affine_fits(n1, n2, D)) return B2B_EUNSUPPORTED;
   const size_t smem_full = ((size_t)D * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)n2 * sizeof(int);
   const bool full = smem_full <= 200 * 1024;

@@ -182,58 +182,36 @@ static size_t cmlp_smem_bytes(int n1, int n2, int H, int D, bool deep) {
 
 }  // namespace b2b
 
-bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D) {
-  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_MLP_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_MLP_MAX_N && d.n2 >= 1 &&
-         d.n2 <= B2B_COUPLING_MLP_MAX_H && D <= B2B_COUPLING_MLP_MAX_D;
-}
-
-bool b2b_coupling_deep_mlp_fits(const b2b_layer_desc& d, int D) {
-  const int M = d.n3 >> 8;
-  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_DEEP_MLP_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_DEEP_MLP_MAX_N &&
-         d.n2 >= 1 && d.n2 <= B2B_COUPLING_DEEP_MLP_MAX_H && M >= 2 && M <= B2B_COUPLING_DEEP_MLP_MAX_DEPTH &&
-         D <= B2B_COUPLING_DEEP_MLP_MAX_D;
-}
-
-// COUPLING_MLP and COUPLING_DEEP_MLP
-int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
+int b2b_fwd_mlp(const B2BFwdSeg& s) {
   using namespace b2b;
-  const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
-  if (!(deep ? b2b_coupling_deep_mlp_fits(d, D) : b2b_coupling_mlp_fits(d, D))) return B2B_EUNSUPPORTED;
-  if (N <= 0) return B2B_OK;
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
+  const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
+  const bool deep = c.M > 1;
   CmlpParams P;
-  P.x = x;
-  P.y = y;
-  P.logjac = logjac;
-  P.idx1 = d.i0;
-  P.idx2 = d.i1;
-  P.N = N;
-  P.ldx = ldx;
-  P.ldy = ldy;
+  P.x = s.x;
+  P.y = s.y;
+  P.logjac = s.logjac;
+  P.W1 = c.W_in;
+  P.c1 = c.c_in;
+  P.Wh = c.W_hid;
+  P.W2 = c.W_out;
+  P.c2 = c.c_out;
+  P.idx1 = c.idx1;
+  P.idx2 = c.idx2;
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldy = s.ldy;
   P.D = D;
-  P.n1 = d.n0;
-  P.n2 = d.n1;
-  P.H = d.n2;
-  P.accumulate = accumulate;
-  P.slope = d.f0;
-  if (deep) {  // p0 = W_in, p1 = W_hid, p2 = W_out, p3 = [c_1 | … | c_M | c_out] or NULL; n3 = σ | M << 8
-    P.W1 = d.p0;
-    P.Wh = d.p1;
-    P.W2 = d.p2;
-    P.depth = d.n3 >> 8;
-    P.c1 = d.p3;
-    P.c2 = d.p3 ? d.p3 + (size_t)P.depth * d.n2 : nullptr;
-    P.act = d.n3 & 255;
-  } else {
-    P.W1 = d.p0;
-    P.c1 = d.p1;
-    P.W2 = d.p2;
-    P.c2 = d.p3;
-    P.Wh = nullptr;
-    P.depth = 1;
-    P.act = d.n3;
-  }
-  const size_t smem = cmlp_smem_bytes(d.n0, d.n1, d.n2, D, deep);
+  P.n1 = c.n1;
+  P.n2 = c.n2;
+  P.H = c.H;
+  P.act = c.act;
+  P.accumulate = s.accumulate;
+  P.slope = c.slope;
+  P.depth = c.M;
+  const size_t smem = cmlp_smem_bytes(c.n1, c.n2, c.H, D, deep);
   void (*kernel)(const CmlpParams) = deep ? (d.inverse ? coupling_mlp_kernel<true, true> : coupling_mlp_kernel<false, true>)
                                           : (d.inverse ? coupling_mlp_kernel<true, false> : coupling_mlp_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -243,9 +221,11 @@ int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, f
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CP_THREADS, smem);
   if (e != cudaSuccess) return (int)e;
   if (per_sm < 1) per_sm = 1;
-  const long long tiles = (N + CP_TC - 1) / CP_TC;
+  const long long tiles = (s.N + CP_TC - 1) / CP_TC;
   long long grid = (long long)sms * per_sm;
   if (grid > tiles) grid = tiles;
-  kernel<<<(int)grid, CP_THREADS, smem, stream>>>(P);
-  return (int)cudaGetLastError();
+  kernel<<<(int)grid, CP_THREADS, smem, s.stream>>>(P);
+  if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  ++*s.launches;
+  return B2B_OK;
 }

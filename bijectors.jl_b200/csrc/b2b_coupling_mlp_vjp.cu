@@ -332,13 +332,11 @@ static long long cmv_param_floats(const b2b_layer_desc& d) {
 }
 static long long cmv_slice_floats(const b2b_layer_desc& d) { return (cmv_param_floats(d) + 63) & ~63LL; }
 
-// hidden layers whose factors the kernel keeps
-static int cmv_depth(const b2b_layer_desc& d) { return d.kind == B2B_COUPLING_DEEP_MLP ? d.n3 >> 8 : 1; }
-
+// the kernel keeps the factors of every hidden layer
 static size_t cmv_smem_bytes(const b2b_layer_desc& d, int D, int nsub) {
-  const size_t f = (size_t)(d.n1 + 2 * d.n0 + 2 * cmv_depth(d) * d.n2) * (32 * nsub + 1) +
-                   (size_t)(d.n0 > d.n1 ? d.n0 : d.n1) * CMV_SP;
-  return (f * sizeof(float) + (size_t)(d.n0 + d.n1) * sizeof(int) + D + 15) & ~(size_t)15;
+  const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
+  const size_t f = (size_t)(c.n2 + 2 * c.n1 + 2 * c.M * c.H) * (32 * nsub + 1) + (size_t)(c.n1 > c.n2 ? c.n1 : c.n2) * CMV_SP;
+  return (f * sizeof(float) + (size_t)(c.n1 + c.n2) * sizeof(int) + D + 15) & ~(size_t)15;
 }
 
 // sub-tiles per group: the most whose factors fit the 227 KB a CTA may use
@@ -358,15 +356,11 @@ static int cmv_grid(const b2b_layer_desc& d, int D, long long N) {
   return g < 1 ? 1 : (int)g;
 }
 
-static bool cmv_fits(const b2b_layer_desc& d, int D) {
-  return d.kind == B2B_COUPLING_DEEP_MLP ? b2b_coupling_deep_mlp_fits(d, D) : b2b_coupling_mlp_fits(d, D);
-}
-
 }  // namespace b2b
 
 size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
   using namespace b2b;
-  if (!cmv_fits(d, D)) return 0;
+  if (!b2b_coupling_fits(d, D)) return 0;
   return (size_t)cmv_grid(d, D, N) * (size_t)cmv_slice_floats(d) * sizeof(float) + 256;
 }
 
@@ -376,8 +370,9 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   const int D = s.D;
   const long long N = s.N;
   float* const* bars = s.bars;
-  if (!cmv_fits(d, D)) return B2B_EUNSUPPORTED;
-  const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
+  if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
+  const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
+  const bool deep = c.M > 1;
   const bool want = bars[0] || bars[1] || bars[2] || bars[3];
   if (want && (!s.workspace || s.workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
   char* wsb = b2b_align256(s.workspace);
@@ -386,25 +381,15 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.ybar = s.ybar;
   P.ljbar = s.ljbar;
   P.xbar = s.xbar;
-  if (deep) {  // p0 = W_in, p1 = W_hid, p2 = W_out, p3 = [c_1 | … | c_M | c_out] or NULL; n3 = σ | M << 8
-    P.W1 = d.p0;
-    P.Wh = d.p1;
-    P.W2 = d.p2;
-    P.depth = d.n3 >> 8;
-    P.c1 = d.p3;
-    P.c2 = d.p3 ? d.p3 + (size_t)P.depth * d.n2 : nullptr;
-    P.act = d.n3 & 255;
-  } else {
-    P.W1 = d.p0;
-    P.c1 = d.p1;
-    P.W2 = d.p2;
-    P.c2 = d.p3;
-    P.Wh = nullptr;
-    P.depth = 1;
-    P.act = d.n3;
-  }
-  P.idx1 = d.i0;
-  P.idx2 = d.i1;
+  P.W1 = c.W_in;
+  P.c1 = c.c_in;
+  P.Wh = c.W_hid;
+  P.W2 = c.W_out;
+  P.c2 = c.c_out;
+  P.depth = c.M;
+  P.act = c.act;
+  P.idx1 = c.idx1;
+  P.idx2 = c.idx2;
   P.part = want ? reinterpret_cast<float*>(wsb) : nullptr;
   P.N = N;
   P.ldx = s.ldx;
@@ -412,11 +397,11 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.ldxb = s.ldxb;
   P.slice = cmv_slice_floats(d);
   P.D = D;
-  P.n1 = d.n0;
-  P.n2 = d.n1;
-  P.H = d.n2;
+  P.n1 = c.n1;
+  P.n2 = c.n2;
+  P.H = c.H;
   P.nsub = cmv_nsub(d, D);
-  P.slope = d.f0;
+  P.slope = c.slope;
   const int grid = cmv_grid(d, D, N);
   const size_t smem = cmv_smem_bytes(d, D, P.nsub);
   void (*kernel)(const CmvParams) = deep ? (d.inverse ? coupling_mlp_vjp_kernel<true, true> : coupling_mlp_vjp_kernel<false, true>)

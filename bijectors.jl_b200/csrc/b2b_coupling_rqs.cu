@@ -132,52 +132,41 @@ static size_t crq_smem_bytes(int nc, int K, int D, int n2x) {
 
 }  // namespace b2b
 
-bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D) {
-  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_RQS_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_RQS_MAX_N &&
-         d.n2 >= 2 && d.n2 <= B2B_COUPLING_RQS_MAX_K && D <= B2B_COUPLING_RQS_MAX_D;
-}
-
-bool b2b_coupling_mlp_rqs_fits(const b2b_layer_desc& d, int D) {
-  const int K = d.n3 >> 8;
-  return d.n0 >= 1 && d.n0 <= B2B_COUPLING_MLP_RQS_MAX_N && d.n1 >= 1 && d.n1 <= B2B_COUPLING_MLP_RQS_MAX_N &&
-         d.n2 >= 1 && d.n2 <= B2B_COUPLING_MLP_RQS_MAX_H && K >= 2 && K <= B2B_COUPLING_MLP_RQS_MAX_K &&
-         D <= B2B_COUPLING_MLP_RQS_MAX_D;
-}
-
-int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, cudaStream_t stream) {
+int b2b_fwd_spline(const B2BFwdSeg& s) {
   using namespace b2b;
-  const bool mlp = d.kind == B2B_COUPLING_MLP_RQS;
-  if (!(mlp ? b2b_coupling_mlp_rqs_fits(d, D) : b2b_coupling_rqs_fits(d, D))) return B2B_EUNSUPPORTED;
-  if (N <= 0) return B2B_OK;
+  const b2b_layer_desc& d = s.layers[0];
+  if (!b2b_coupling_fits(d, s.D)) return B2B_EUNSUPPORTED;
+  const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
   CrqParams P = {};
-  P.x = x;
-  P.y = y;
-  P.logjac = logjac;
-  P.W = mlp ? d.p2 : d.p0;
-  P.c = mlp ? d.p3 : d.p1;
-  P.W1 = d.p0;
-  P.c1 = d.p1;
-  P.idx1 = d.i0;
-  P.idx2 = d.i1;
-  P.N = N;
-  P.ldx = ldx;
-  P.ldy = ldy;
-  P.D = D;
-  P.n1 = d.n0;
-  P.n2 = d.n1;
-  P.K = mlp ? d.n3 >> 8 : d.n2;
-  P.H = d.n2;
-  P.act = d.n3 & 255;
-  P.accumulate = accumulate;
-  P.B = mlp ? d.f1 : d.f0;
-  P.slope = d.f0;
-  const size_t smem = mlp ? crq_smem_bytes(P.H, P.K, D, P.n2) : crq_smem_bytes(P.n2, P.K, D, 0);
-  void (*kernel)(const CrqParams) = mlp ? (d.inverse ? coupling_rqs_kernel<true, true> : coupling_rqs_kernel<false, true>)
-                                        : (d.inverse ? coupling_rqs_kernel<true, false> : coupling_rqs_kernel<false, false>);
+  P.x = s.x;
+  P.y = s.y;
+  P.logjac = s.logjac;
+  P.W = c.W_out;
+  P.c = c.c_out;
+  P.W1 = c.W_in;
+  P.c1 = c.c_in;
+  P.idx1 = c.idx1;
+  P.idx2 = c.idx2;
+  P.N = s.N;
+  P.ldx = s.ldx;
+  P.ldy = s.ldy;
+  P.D = s.D;
+  P.n1 = c.n1;
+  P.n2 = c.n2;
+  P.K = c.K;
+  P.H = c.H;
+  P.act = c.act;
+  P.accumulate = s.accumulate;
+  P.B = c.B;
+  P.slope = c.slope;
+  const size_t smem = c.net ? crq_smem_bytes(c.H, c.K, s.D, c.n2) : crq_smem_bytes(c.n2, c.K, s.D, 0);
+  void (*kernel)(const CrqParams) = c.net ? (d.inverse ? coupling_rqs_kernel<true, true> : coupling_rqs_kernel<false, true>)
+                                          : (d.inverse ? coupling_rqs_kernel<true, false> : coupling_rqs_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  const long long tiles = (N + CRQ_TN - 1) / CRQ_TN;
-  kernel<<<(unsigned)tiles, CRQ_TN, smem, stream>>>(P);
-  return (int)cudaGetLastError();
+  const long long tiles = (s.N + CRQ_TN - 1) / CRQ_TN;
+  kernel<<<(unsigned)tiles, CRQ_TN, smem, s.stream>>>(P);
+  if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  ++*s.launches;
+  return B2B_OK;
 }

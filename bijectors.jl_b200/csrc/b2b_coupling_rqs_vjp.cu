@@ -241,36 +241,28 @@ __global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const floa
   }
 }
 
-// the shape of a spline coupling layer as the kernels see it: nc conditioning rows (n2, or the H hidden units), and for
-// the network nh = H hidden units over nx = n2 rows of x₂ (both 0 without it)
-struct CrvShape {
-  int n1, nc, K, nh, nx;
-};
-static CrvShape crv_shape(const b2b_layer_desc& d) {
-  if (d.kind == B2B_COUPLING_MLP_RQS) return {d.n0, d.n2, d.n3 >> 8, d.n2, d.n1};
-  return {d.n0, d.n1, d.n2, 0, 0};
-}
+using Cpl = B2BCoupling<b2b_layer_desc>;
+// the kernels' nc conditioning rows (x₂, or the network's H hidden units) and nx rows of x₂ under the network (0: none)
+static int crv_nc(const Cpl& c) { return c.net ? c.H : c.n2; }
+static int crv_nx(const Cpl& c) { return c.net ? c.n2 : 0; }
 
-static size_t crv_smem_bytes(const CrvShape& sh, int D) {
-  const int nc = sh.nc, K = sh.K, J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
+static size_t crv_smem_bytes(const Cpl& c, int D) {
+  const int nc = crv_nc(c), K = c.K, J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
   const size_t f = (size_t)nc * JP + JP + (size_t)6 * K1 * CRV_TN + (size_t)nc * (CRV_TN + 1) + (size_t)J * (CRV_TN + 1);
-  return (((f + 1) / 2 + (size_t)nc * (CRV_TN + 1)) * sizeof(double) + (size_t)sh.nx * (CRV_TN + 1) * sizeof(float) + D +
-          15) & ~(size_t)15;
+  return (((f + 1) / 2 + (size_t)nc * (CRV_TN + 1)) * sizeof(double) + (size_t)crv_nx(c) * (CRV_TN + 1) * sizeof(float) +
+          D + 15) & ~(size_t)15;
 }
 
 // floats of the slice's sums: W̄ / c̄ of the spline's conditioner, then W̄₁ / c̄₁ of the network
-static long long crv_sum_floats(const CrvShape& sh) {
-  return (long long)sh.n1 * (3 * sh.K - 1) * (sh.nc + 1) + (long long)sh.nh * (sh.nx + 1);
+static long long crv_sum_floats(const Cpl& c) {
+  return (long long)c.n1 * (3 * c.K - 1) * (crv_nc(c) + 1) + (long long)c.H * (crv_nx(c) + 1);
 }
 
-static long long crv_slice_floats(const b2b_layer_desc& d) {
-  const long long f = crv_sum_floats(crv_shape(d));
-  return (f + 63) & ~63LL;
-}
+static long long crv_slice_floats(const b2b_layer_desc& d) { return (crv_sum_floats(b2b_coupling(d)) + 63) & ~63LL; }
 
 static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
   const int sms = b2b_sm_count();
-  int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(crv_shape(d), D) + 1024));
+  int per_sm = (int)((size_t)(227 * 1024) / (crv_smem_bytes(b2b_coupling(d), D) + 1024));
   per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
   long long g = (long long)sms * per_sm;
   const long long tiles = (N + CRV_TN - 1) / CRV_TN;
@@ -280,15 +272,11 @@ static int crv_grid(const b2b_layer_desc& d, int D, long long N) {
   return g < 1 ? 1 : (int)g;
 }
 
-static bool crv_fits(const b2b_layer_desc& d, int D) {
-  return d.kind == B2B_COUPLING_MLP_RQS ? b2b_coupling_mlp_rqs_fits(d, D) : b2b_coupling_rqs_fits(d, D);
-}
-
 }  // namespace b2b
 
 size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N) {
   using namespace b2b;
-  if (!crv_fits(d, D)) return 0;
+  if (!b2b_coupling_fits(d, D)) return 0;
   return (size_t)crv_grid(d, D, N) * (size_t)crv_slice_floats(d) * sizeof(float) + 256;
 }
 
@@ -297,26 +285,26 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   const b2b_layer_desc& d = s.layers[0];
   const int D = s.D;
   const long long N = s.N;
-  if (!crv_fits(d, D)) return B2B_EUNSUPPORTED;
+  if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
   if (!s.workspace || s.workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
-  const bool mlp = d.kind == B2B_COUPLING_MLP_RQS;
-  const CrvShape sh = crv_shape(d);
+  const Cpl c = b2b_coupling(d);
+  const bool mlp = c.net;
   // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c.  The network's four sums are
   // written only where they are asked for.
   float* const Wbar = mlp ? s.bars[2] : s.bars[0] ? s.bars[0] : s.scratch;
-  float* const cbar = mlp ? (d.p3 ? s.bars[3] : nullptr)
-                          : !d.p1 ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
+  float* const cbar = mlp ? (c.c_out ? s.bars[3] : nullptr)
+                          : !c.c_out ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
   CrvParams P = {};
   P.x = s.x;
   P.ybar = s.ybar;
   P.ljbar = s.ljbar;
   P.xbar = s.xbar;
-  P.W = mlp ? d.p2 : d.p0;
-  P.c = mlp ? d.p3 : d.p1;
-  P.W1 = d.p0;
-  P.c1 = d.p1;
-  P.idx1 = d.i0;
-  P.idx2 = d.i1;
+  P.W = c.W_out;
+  P.c = c.c_out;
+  P.W1 = c.W_in;
+  P.c1 = c.c_in;
+  P.idx1 = c.idx1;
+  P.idx2 = c.idx2;
   P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
   P.N = N;
   P.ldx = s.ldx;
@@ -324,15 +312,15 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   P.ldxb = s.ldxb;
   P.slice = crv_slice_floats(d);
   P.D = D;
-  P.n1 = d.n0;
-  P.n2 = d.n1;
-  P.K = sh.K;
-  P.H = sh.nh;
-  P.act = d.n3 & 255;
-  P.B = mlp ? d.f1 : d.f0;
-  P.slope = d.f0;
+  P.n1 = c.n1;
+  P.n2 = c.n2;
+  P.K = c.K;
+  P.H = c.H;
+  P.act = c.act;
+  P.B = c.B;
+  P.slope = c.slope;
   const int grid = crv_grid(d, D, N);
-  const size_t smem = crv_smem_bytes(sh, D);
+  const size_t smem = crv_smem_bytes(c, D);
   void (*kernel)(const CrvParams) =
       mlp ? (d.inverse ? coupling_rqs_vjp_kernel<true, true> : coupling_rqs_vjp_kernel<false, true>)
           : (d.inverse ? coupling_rqs_vjp_kernel<true, false> : coupling_rqs_vjp_kernel<false, false>);
@@ -340,10 +328,10 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CRV_TN, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  const long long len = crv_sum_floats(sh);
+  const long long len = crv_sum_floats(c);
   coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
-      P.part, grid, P.slice, sh.n1, sh.nc, sh.K, Wbar, cbar, sh.nh, sh.nx, mlp ? s.bars[0] : nullptr,
-      mlp && d.p1 ? s.bars[1] : nullptr);
+      P.part, grid, P.slice, c.n1, crv_nc(c), c.K, Wbar, cbar, c.H, crv_nx(c), mlp ? s.bars[0] : nullptr,
+      c.c_in ? s.bars[1] : nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   *s.launches += 2;
   return B2B_OK;

@@ -109,13 +109,8 @@ int b2b_launch_coupling_affine(const b2b_layer_desc& d, const float* fold, const
                                float* logjac, int D, long long N, long long ldx, long long ldy, int accumulate,
                                cudaStream_t stream);
 // full-covariance MvNormal terminal (b2b_mvnormal_tril.cu).  Float32 stages the packed lower triangle of L in shared
-// memory: D <= B2B_TRIL_MAX_D.  The logpdf launch reads x (the recovered point), copies it to y when y != NULL and y != x,
-// and writes logpdf (+ logjac when accumulate) to logjac (may be NULL); with partials it writes b2b_tril_grid(D, N) per-CTA
-// batch sums.
+// memory: D <= B2B_TRIL_MAX_D.
 #define B2B_TRIL_MAX_D 256
-int b2b_tril_grid(int D, long long N);
-int b2b_launch_mvnormal_tril(const b2b_layer_desc& d, const float* x, long long ldx, float* y, long long ldy,
-                             float* logjac, int accumulate, double* partials, int D, long long N, cudaStream_t stream);
 // reverse mode: μ̄ / L̄ need b2b_tril_vjp_workspace(D, N) bytes
 size_t b2b_tril_vjp_workspace(int D, long long N);
 // Σₙ S[:, n] R[:, n]ᵀ over column chunks (b2b_mvnormal_tril.cu): CTA (tile, p) writes its 64 x 64 tile of chunk p's sum
@@ -125,31 +120,16 @@ size_t b2b_tril_vjp_workspace(int D, long long N);
 long long b2b_outer_chunk_len(long long N);
 int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long long ldr, float* part, float* mup, int D,
                             long long N, bool lower, cudaStream_t stream);
-// dense Scale(A) (b2b_scale_matrix.cu), D <= B2B_SCALE_MATRIX_MAX_D: factor (one CTA; plus the A⁻¹ solves for the
-// inverse direction) and the map GEMM, in b2b_scale_matrix_workspace(D) bytes; y == NULL writes log-Jacobians only
+// dense Scale(A) (b2b_scale_matrix.cu), D <= B2B_SCALE_MATRIX_MAX_D: the factor storage of its forward launches
 size_t b2b_scale_matrix_workspace(int D);
-int b2b_launch_scale_matrix(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, void* workspace, size_t workspace_bytes,
-                            int* launches, cudaStream_t stream);
 // reverse mode: b2b_scale_matrix_vjp_workspace(D, N) bytes (0 beyond the envelope)
 size_t b2b_scale_matrix_vjp_workspace(int D, long long N);
-// spline coupling (b2b_coupling_rqs.cu, b2b_coupling_rqs_vjp.cu): whether the layer is within the envelope of include/b2b.h
-bool b2b_coupling_rqs_fits(const b2b_layer_desc& d, int D);
-int b2b_launch_coupling_rqs(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, cudaStream_t stream);
-// the neural spline coupling (B2B_COUPLING_MLP_RQS) runs on the same kernels and launchers
-bool b2b_coupling_mlp_rqs_fits(const b2b_layer_desc& d, int D);
-// reverse mode: b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the envelope, bounded independently of N)
+// spline coupling, reverse mode (b2b_coupling_rqs_vjp.cu): b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the
+// envelope, bounded independently of N)
 size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
-// neural-network coupling (b2b_coupling_mlp.cu, b2b_coupling_mlp_vjp.cu): whether the layer is within the envelope of
-// include/b2b.h
-bool b2b_coupling_mlp_fits(const b2b_layer_desc& d, int D);
-// the deep-network coupling (B2B_COUPLING_DEEP_MLP) runs on the same kernels and launchers
-bool b2b_coupling_deep_mlp_fits(const b2b_layer_desc& d, int D);
-int b2b_launch_coupling_mlp(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, cudaStream_t stream);
-// reverse mode: with any parameter cotangent b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope,
-// bounded independently of N) and two launches, else one launch and no workspace
+// neural-network coupling, reverse mode (b2b_coupling_mlp_vjp.cu): with any parameter cotangent
+// b2b_coupling_mlp_vjp_workspace(d, D, N) bytes (0 outside the envelope, bounded independently of N) and two launches,
+// else one launch and no workspace
 size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
 // B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
@@ -166,6 +146,37 @@ inline char* b2b_align256(void* workspace) {
   char* p = static_cast<char*>(workspace);
   return p + ((256 - (reinterpret_cast<uintptr_t>(p) & 255)) & 255);
 }
+
+// ---- forward segment launchers ---------------------------------------------------------------------------------------
+// One launch segment of b2b_chain_run_f32: `n` layers of one B2BLaunchClass from x to y (NULL: not stored), adding their
+// log-Jacobians to logjac (may be NULL).  The rules of the reverse-mode launchers below hold: the caller has validated
+// the descriptors, the launcher checks what its kernels need, and it adds the launches it enqueued to *launches.
+// pre / post: BatchNorm layers folded into a coupling launch through the table `fold`; partials (NULL: no batch sum):
+// per-CTA sums of the fused or TRIL launch, added into *sum_out; workspace: the class's slice (W image, Scale factor).
+struct B2BFwdSeg {
+  const b2b_layer_desc* layers;
+  int n;
+  const float* x;
+  long long ldx;
+  float* y;
+  long long ldy;
+  float* logjac;
+  int accumulate;
+  int D;
+  long long N;
+  const b2b_layer_desc *pre, *post;
+  float* fold;
+  double* partials;
+  double* sum_out;
+  void* workspace;
+  size_t workspace_bytes;
+  int* launches;
+  cudaStream_t stream;
+};
+int b2b_fwd_spline(const B2BFwdSeg& s);  // b2b_coupling_rqs.cu: COUPLING_RQS and COUPLING_MLP_RQS
+int b2b_fwd_mlp(const B2BFwdSeg& s);     // b2b_coupling_mlp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
+int b2b_fwd_scale(const B2BFwdSeg& s);   // b2b_scale_matrix.cu: y == NULL writes log-Jacobians only
+int b2b_fwd_tril(const B2BFwdSeg& s);    // b2b_mvnormal_tril.cu: copies x to y (when y != x), writes logpdf to logjac
 
 // ---- reverse-mode segment launchers ----------------------------------------------------------------------------------
 // One segment of b2b_chain_vjp_f32: `n` layers of one B2BVjpClass, their input x, the cotangent ȳ of their output, l̄ (N
@@ -214,9 +225,10 @@ int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, c
 
 // ---- layer kinds ---------------------------------------------------------------------------------------------------
 // What the chain orchestration knows about each kind of include/b2b.h.  A new kind enters the host code as one row of
-// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu, its slot lengths in b2b_slot_len, its own
-// forward launch in b2b_chain_run_f32, and for reverse mode one B2BVjpSeg launcher plus one case of the sweep's switch
-// in b2b_chain_vjp_f32 (and its scratch and workspace sizes in seg_param_floats / seg_kernel_bytes).
+// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu (a coupling: its packing in b2b_coupling and
+// a row of b2b_coupling_fits), its slot lengths in b2b_slot_len, one B2BFwdSeg launcher plus one case of the forward
+// switch in b2b_chain_run_f32, and for reverse mode one B2BVjpSeg launcher plus one case of the sweep's switch in
+// b2b_chain_vjp_f32 (and its scratch and workspace sizes in seg_param_floats / seg_kernel_bytes).
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
 enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };
@@ -272,6 +284,67 @@ inline bool b2b_chain_has_launch(const b2b_layer_desc* layers, int L, int launch
   return false;
 }
 
+// ---- coupling descriptors ------------------------------------------------------------------------------------------
+// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP descriptor decoded: the one place that knows how include/b2b.h
+// packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or b2b_layer_desc_f64.
+template <class Desc>
+struct B2BCoupling {
+  using Ptr = decltype(Desc::p0);
+  int n1, n2;        // rows of x₁ (transformed) and of x₂ (conditioning)
+  int H, M, K;       // hidden units and hidden layers (0, 0: a linear conditioner); spline bins (0: the affine law)
+  bool net, spline;  // the conditioner is a network (H, M, act, slope apply); the law is the spline (K, B apply)
+  int act;
+  decltype(Desc::f0) slope, B;
+  Ptr W_in, c_in;    // the network's first layer (c_1 .. c_M packed for the deep network)
+  Ptr W_hid;         // W_2 .. W_M of the deep network, back to back
+  Ptr W_out, c_out;  // the last layer: W and c of a linear conditioner
+  const int32_t *idx1, *idx2;
+  int row1, row2;    // affine law: first rows of idx1 / idx2 when they are contiguous ranges (< 0: use the list)
+};
+
+inline bool b2b_is_coupling(int kind) {
+  return kind == B2B_COUPLING_AFFINE || kind == B2B_COUPLING_RQS || kind == B2B_COUPLING_MLP ||
+         kind == B2B_COUPLING_MLP_RQS || kind == B2B_COUPLING_DEEP_MLP;
+}
+
+template <class Desc>
+B2BCoupling<Desc> b2b_coupling(const Desc& d) {
+  const int k = d.kind;
+  const bool deep = k == B2B_COUPLING_DEEP_MLP;
+  B2BCoupling<Desc> c{};
+  c.n1 = d.n0;
+  c.n2 = d.n1;
+  c.net = k == B2B_COUPLING_MLP || k == B2B_COUPLING_MLP_RQS || deep;
+  c.spline = k == B2B_COUPLING_RQS || k == B2B_COUPLING_MLP_RQS;
+  c.K = k == B2B_COUPLING_RQS ? d.n2 : k == B2B_COUPLING_MLP_RQS ? d.n3 >> 8 : 0;  // MLP_RQS: n3 = σ | K << 8
+  c.M = deep ? d.n3 >> 8 : c.net ? 1 : 0;                                          // DEEP_MLP: n3 = σ | M << 8
+  c.B = k == B2B_COUPLING_RQS ? d.f0 : k == B2B_COUPLING_MLP_RQS ? d.f1 : 0;
+  c.idx1 = d.i0;
+  c.idx2 = d.i1;
+  c.row1 = k == B2B_COUPLING_AFFINE ? d.n2 : -1;
+  c.row2 = k == B2B_COUPLING_AFFINE ? d.n3 : -1;
+  if (!c.net) {
+    c.W_out = d.p0;
+    c.c_out = d.p1;
+    return c;
+  }
+  c.H = d.n2;
+  c.act = k == B2B_COUPLING_MLP ? d.n3 : d.n3 & 255;
+  c.slope = d.f0;
+  c.W_in = d.p0;
+  c.W_out = d.p2;
+  // DEEP_MLP: p1 = W_hid, p3 = [c_1 | … | c_M | c_out] (or NULL)
+  c.W_hid = deep ? d.p1 : nullptr;
+  c.c_in = deep ? d.p3 : d.p1;
+  c.c_out = !deep ? d.p3 : d.p3 ? d.p3 + (size_t)c.M * c.H : nullptr;
+  return c;
+}
+
+// Float32 kernel envelope of a COUPLING_RQS / _MLP / _MLP_RQS / _DEEP_MLP layer at D: the B2B_COUPLING_*_MAX_* limits
+// of include/b2b.h (the affine coupling's limits are shared-memory budgets, b2b_coupling_affine_fits).  Defined in
+// b2b_api.cu: inline here, it changes the SASS nvcc 12.9 emits for the neural-spline reverse-mode kernels.
+bool b2b_coupling_fits(const b2b_layer_desc& d, int D);
+
 // whether the chain ends in its MvNormal terminal (its logjac output is then logpdf)
 template <class Desc>
 bool b2b_ends_in_terminal(const Desc* layers, int L) {
@@ -289,58 +362,37 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
   for (int f = 0; f < 6; ++f)
     if ((k->required >> f & 1) && !field[f]) return B2B_EINVAL;
   if (k->terminal && (!last || d.inverse)) return B2B_EINVAL;
-  bool ok = true;
-  switch (d.kind) {
-    case B2B_RQS: ok = d.n0 >= 2; break;
-    case B2B_COUPLING_AFFINE:  // an index list may be NULL when n2 / n3 gives the first row of its contiguous range
-      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && (d.i0 || d.n2 >= 0) && (d.i1 || d.n3 >= 0);
-      break;
-    case B2B_COUPLING_RQS: ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && d.f0 > 0; break;
-    case B2B_COUPLING_MLP:
-      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && (d.n3 == B2B_ACT_TANH || d.n3 == B2B_ACT_LEAKY_RELU);
-      break;
-    case B2B_COUPLING_MLP_RQS: {  // n3 = σ | K << 8
-      const int act = d.n3 & 255, K = d.n3 >> 8;
-      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && K >= 1 &&
-           (act == B2B_ACT_TANH || act == B2B_ACT_LEAKY_RELU) && d.f1 > 0;
-      break;
-    }
-    case B2B_COUPLING_DEEP_MLP: {  // n3 = σ | M << 8
-      const int act = d.n3 & 255, M = d.n3 >> 8;
-      ok = d.n0 >= 1 && d.n1 >= 1 && d.n0 + d.n1 <= D && d.n2 >= 1 && M >= 2 &&
-           (act == B2B_ACT_TANH || act == B2B_ACT_LEAKY_RELU);
-      break;
-    }
-    default: break;
-  }
+  if (d.kind == B2B_RQS) return d.n0 >= 2 ? B2B_OK : B2B_EINVAL;
+  if (!b2b_is_coupling(d.kind)) return B2B_OK;
+  const B2BCoupling<Desc> c = b2b_coupling(d);
+  bool ok = c.n1 >= 1 && c.n2 >= 1 && c.n1 + c.n2 <= D;
+  if (c.net) ok = ok && c.H >= 1 && (c.act == B2B_ACT_TANH || c.act == B2B_ACT_LEAKY_RELU);
+  if (c.spline) ok = ok && c.K >= 1 && c.B > 0;
+  if (d.kind == B2B_COUPLING_DEEP_MLP) ok = ok && c.M >= 2;
+  // an index list may be NULL when n2 / n3 gives the first row of its contiguous range
+  if (d.kind == B2B_COUPLING_AFFINE) ok = ok && (c.idx1 || c.row1 >= 0) && (c.idx2 || c.row2 >= 0);
   return ok ? B2B_OK : B2B_EINVAL;
 }
 
 // elements of trainable slot i of `d` (its cotangent has the parameter's shape)
 template <class Desc>
 size_t b2b_slot_len(const Desc& d, int i, int D) {
+  if (b2b_is_coupling(d.kind)) {
+    const B2BCoupling<Desc> c = b2b_coupling(d);
+    const size_t J = c.spline ? (size_t)(3 * c.K - 1) * c.n1 : (size_t)2 * c.n1;  // rows of W_out
+    if (!c.net) return i == 0 ? J * c.n2 : J;                                      // W, c
+    const size_t H = c.H, M = c.M;
+    const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
+    // W_in (H x n2), c_in (H) or the deep network's W_hid ((M−1) x H x H), W_out (J x H), c_out (J) or every bias
+    const size_t len[4] = {H * c.n2, deep ? (M - 1) * H * H : H, J * H, deep ? M * H + J : J};
+    return len[i];
+  }
   switch (d.kind) {
     case B2B_PLANAR: return i == 2 ? 1 : D;
     case B2B_RADIAL: return i == 2 ? D : 1;
     case B2B_RQS: return (size_t)D * d.n0;
-    case B2B_COUPLING_AFFINE: return i == 0 ? (size_t)2 * d.n0 * d.n1 : (size_t)2 * d.n0;
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
-    case B2B_COUPLING_RQS: return (size_t)(3 * d.n2 - 1) * d.n0 * (i == 0 ? d.n1 : 1);
     case B2B_SCALE_MATRIX: return (size_t)D * D;
-    case B2B_COUPLING_MLP: {  // W₁ (H x n2), c₁ (H), W₂ (2n1 x H), c₂ (2n1)
-      const size_t len[4] = {(size_t)d.n2 * d.n1, (size_t)d.n2, (size_t)2 * d.n0 * d.n2, (size_t)2 * d.n0};
-      return len[i];
-    }
-    case B2B_COUPLING_MLP_RQS: {  // W₁ (H x n2), c₁ (H), W₂ ((3K−1)n1 x H), c₂ ((3K−1)n1)
-      const size_t J = (size_t)(3 * (d.n3 >> 8) - 1) * d.n0;
-      const size_t len[4] = {(size_t)d.n2 * d.n1, (size_t)d.n2, J * d.n2, J};
-      return len[i];
-    }
-    case B2B_COUPLING_DEEP_MLP: {  // W_in (H x n2), W_hid ((M−1) x H x H), W_out (2n1 x H), c (M·H + 2n1)
-      const size_t H = d.n2, M = d.n3 >> 8;
-      const size_t len[4] = {H * d.n1, (M - 1) * H * H, (size_t)2 * d.n0 * H, M * H + (size_t)2 * d.n0};
-      return len[i];
-    }
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
   }
 }

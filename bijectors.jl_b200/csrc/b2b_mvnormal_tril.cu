@@ -470,8 +470,6 @@ long long chunk_len(long long N) {
 
 using namespace b2b_tril;
 
-int b2b_tril_grid(int D, long long N) { return grid_for(c_logpdf(rows_per_lane(D)), N); }
-
 long long b2b_outer_chunk_len(long long N) { return chunk_len(N); }
 
 int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long long ldr, float* part, float* mup, int D,
@@ -483,20 +481,31 @@ int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long 
   return (int)cudaGetLastError();
 }
 
-int b2b_launch_mvnormal_tril(const b2b_layer_desc& d, const float* x, long long ldx, float* y, long long ldy,
-                             float* logjac, int accumulate, double* partials, int D, long long N, cudaStream_t stream) {
+// logjac := logpdf of x, the recovered point (+ logjac when accumulate); with partials, their per-CTA sums as well
+int b2b_fwd_tril(const B2BFwdSeg& s) {
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
+  const long long N = s.N;
   if (D < 1 || D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
-  if (y == x) y = nullptr;  // in place: nothing to copy
+  float* const y = s.y == s.x ? nullptr : s.y;  // in place: nothing to copy
   const int R = rows_per_lane(D);
-#define B2B_TRIL_LP(RR)                                                                                           \
-  case RR:                                                                                                        \
-    return launch(logpdf_kernel<RR, c_logpdf(RR)>, grid_for(c_logpdf(RR), N), D, stream, x, ldx, y, ldy, logjac, \
-                  accumulate, partials, d.p1, d.p0, D, N);
+  const int grid = grid_for(c_logpdf(R), N);
+  int rc = B2B_EUNSUPPORTED;
+#define B2B_TRIL_LP(RR)                                                                                                \
+  case RR:                                                                                                             \
+    rc = launch(logpdf_kernel<RR, c_logpdf(RR)>, grid, D, s.stream, s.x, s.ldx, y, s.ldy, s.logjac, s.accumulate,     \
+                s.partials, d.p1, d.p0, D, N);                                                                         \
+    break;
   switch (R) {
     B2B_TRIL_LP(1) B2B_TRIL_LP(2) B2B_TRIL_LP(4) B2B_TRIL_LP(8) B2B_TRIL_LP(16)
   }
 #undef B2B_TRIL_LP
-  return B2B_EUNSUPPORTED;
+  if (rc != B2B_OK) return rc;
+  ++*s.launches;
+  if (!s.partials) return B2B_OK;
+  if ((rc = b2b_launch_sum_partials(s.partials, grid, s.sum_out, s.stream)) != B2B_OK) return rc;
+  ++*s.launches;
+  return B2B_OK;
 }
 
 // workspace: [r | l̄·s] (2 x D x N floats) [chunk partials of L̄ (P x D x D) and μ̄ (P x D)] [per-CTA Σ l̄ (kMaxGrid doubles)]

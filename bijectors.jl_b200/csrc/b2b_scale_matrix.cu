@@ -467,28 +467,28 @@ size_t b2b_scale_matrix_workspace(int D) {
   return D >= 1 && D <= B2B_SCALE_MATRIX_MAX_D ? factor_bytes(D) : 0;
 }
 
-int b2b_launch_scale_matrix(const b2b_layer_desc& d, const float* x, float* y, float* logjac, int D, long long N,
-                            long long ldx, long long ldy, int accumulate, void* workspace, size_t workspace_bytes,
-                            int* launches, cudaStream_t stream) {
-  *launches = 0;
+int b2b_fwd_scale(const B2BFwdSeg& s) {
+  const b2b_layer_desc& d = s.layers[0];
+  const int D = s.D;
   if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-  if (!workspace || workspace_bytes < factor_bytes(D)) return B2B_EWORKSPACE;
-  const Factor f = carve(workspace, D);
+  if (!s.workspace || s.workspace_bytes < factor_bytes(D)) return B2B_EWORKSPACE;
+  const Factor f = carve(s.workspace, D);
   const bool inv = d.inverse != 0;
-  int rc = launch_factor(d, f, D, inv && y, launches, stream);
+  int rc = launch_factor(d, f, D, inv && s.y, s.launches, s.stream);
   if (rc != B2B_OK) return rc;
   const float sign = inv ? -1.f : 1.f;
-  if (!y) {  // log-Jacobians only
-    if (!logjac) return B2B_OK;
-    long long g = (N + 255) / 256;
-    logjac_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, stream>>>(logjac, accumulate, f.logdet, sign, N);
+  if (!s.y) {  // log-Jacobians only
+    if (!s.logjac) return B2B_OK;
+    long long g = (s.N + 255) / 256;
+    logjac_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, s.stream>>>(s.logjac, s.accumulate, f.logdet, sign, s.N);
     if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
-    ++*launches;
+    ++*s.launches;
     return B2B_OK;
   }
-  rc = launch_map<false>(inv ? f.minv : d.p0, x, ldx, y, ldy, logjac, accumulate, f.logdet, sign, D, N, stream);
+  rc = launch_map<false>(inv ? f.minv : d.p0, s.x, s.ldx, s.y, s.ldy, s.logjac, s.accumulate, f.logdet, sign, D, s.N,
+                         s.stream);
   if (rc != B2B_OK) return rc;
-  ++*launches;
+  ++*s.launches;
   return B2B_OK;
 }
 

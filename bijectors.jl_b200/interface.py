@@ -808,26 +808,34 @@ def isclosedform(t) -> bool:
 # reverse mode of any chain: b2b_chain_vjp_f32 (Float32 batches) / b2b_chain_vjp_f64 (Float64 batches)
 # --------------------------------------------------------------------------------------------------
 
+def _coupling_slots(d, D):
+    """Shapes of a coupling descriptor's slots.  H hidden units, K spline bins and M hidden layers (0 where the kind has
+    none) are decoded here only: n2 is K or H, and n3 packs σ | K << 8 or σ | M << 8 (include/b2b.h)."""
+    H, K, M = {_lib.COUPLING_RQS: (0, d.n2, 0), _lib.COUPLING_MLP: (d.n2, 0, 1), _lib.COUPLING_MLP_RQS: (d.n2, d.n3 >> 8, 1),
+               _lib.COUPLING_DEEP_MLP: (d.n2, 0, d.n3 >> 8)}.get(d.kind, (0, 0, 0))
+    J = (3 * K - 1) * d.n0 if K else 2 * d.n0  # rows of the last layer
+    if not H:
+        return (d.n1, J), (J,)
+    if d.kind == _lib.COUPLING_DEEP_MLP:
+        return (d.n1, H), (M - 1, H, H), (H, J), (M * H + J,)
+    return (d.n1, H), (H,), (H, J), (J,)
+
+
 # The trainable descriptor slots p0, p1, ... of each kind: (the reference's field names, the shapes of the device tensors
 # the library reads, the slots whose storage is column-major -- the parameter's transpose).
 _SLOTS = {
     _lib.PLANAR: (("w", "u", "b"), lambda d, D: ((D,), (D,), (1,)), ()),
     _lib.RADIAL: (("α_", "β", "z_0"), lambda d, D: ((1,), (1,), (D,)), ()),
     _lib.RQS: (("widths", "heights", "derivatives"), lambda d, D: ((d.n0, D),) * 3, (0, 1, 2)),
-    _lib.COUPLING_AFFINE: (("W", "c"), lambda d, D: ((d.n1, 2 * d.n0), (2 * d.n0,)), (0,)),
+    _lib.COUPLING_AFFINE: (("W", "c"), _coupling_slots, (0,)),
     _lib.BATCHNORM: (("b", "logs"), lambda d, D: ((D,), (D,)), ()),
     _lib.MVNORMAL_DIAG: (("μ", "σ"), lambda d, D: ((D,), (D,)), ()),
     _lib.MVNORMAL_TRIL: (("μ", "L"), lambda d, D: ((D,), (D, D)), (1,)),
-    _lib.COUPLING_RQS: (("W", "c"), lambda d, D: ((d.n1, (3 * d.n2 - 1) * d.n0), ((3 * d.n2 - 1) * d.n0,)), (0,)),
+    _lib.COUPLING_RQS: (("W", "c"), _coupling_slots, (0,)),
     _lib.SCALE_MATRIX: (("a",), lambda d, D: ((D, D),), (0,)),
-    _lib.COUPLING_MLP: (("W1", "c1", "W2", "c2"), lambda d, D: ((d.n1, d.n2), (d.n2,), (d.n2, 2 * d.n0), (2 * d.n0,)), (0, 2)),
-    _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"),
-                            lambda d, D: ((d.n1, d.n2), (d.n2,), (d.n2, (3 * (d.n3 >> 8) - 1) * d.n0), ((3 * (d.n3 >> 8) - 1) * d.n0,)),
-                            (0, 2)),
-    _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"),
-                             lambda d, D: ((d.n1, d.n2), ((d.n3 >> 8) - 1, d.n2, d.n2), (d.n2, 2 * d.n0),
-                                           ((d.n3 >> 8) * d.n2 + 2 * d.n0,)),
-                             (0, 1, 2)),
+    _lib.COUPLING_MLP: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
+    _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
+    _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 

@@ -463,22 +463,25 @@ end
 # (y, logjac), `nothing` = zeros.  Returns x̄ and, per descriptor in application order, the cotangents of its trainable
 # fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, Scale(A) a, BatchNorm b logs, the
 # terminal MvNormal's μ σ) in the fields' shapes; `nothing` for fields without one.
+# Hidden units H, spline bins K and hidden layers M of a coupling descriptor (0 where the kind has none), decoded here only:
+# n2 is K or H, and n3 packs σ | K << 8 or σ | M << 8 (include/b2b.h).
+coupling_hkm(d::LayerDesc) =
+    d.kind == COUPLING_RQS ? (0, Int(d.n2), 0) : d.kind == COUPLING_MLP ? (Int(d.n2), 0, 1) :
+    d.kind == COUPLING_MLP_RQS ? (Int(d.n2), Int(d.n3 >> 8), 1) :
+    d.kind == COUPLING_DEEP_MLP ? (Int(d.n2), 0, Int(d.n3 >> 8)) : (0, 0, 0)
 function vjp_slots(d::LayerDesc, D::Integer)
     z(dims...) = CUDA.zeros(Float32, dims...)
     d.kind == PLANAR && return (z(D), z(D), z(1))
     d.kind == RADIAL && return (z(1), z(1), z(D))
     d.kind == RQS && return (z(D, d.n0), z(D, d.n0), z(D, d.n0))
-    d.kind == COUPLING_AFFINE && return (z(2d.n0, d.n1), d.p1 == NULLF ? nothing : z(2d.n0))
-    d.kind == COUPLING_RQS && return (z((3d.n2 - 1) * d.n0, d.n1), d.p1 == NULLF ? nothing : z((3d.n2 - 1) * d.n0))
+    if d.kind in (COUPLING_AFFINE, COUPLING_RQS, COUPLING_MLP, COUPLING_MLP_RQS, COUPLING_DEEP_MLP)
+        H, K, M = coupling_hkm(d)
+        J = K > 0 ? (3K - 1) * d.n0 : 2d.n0  # rows of the last layer
+        H == 0 && return (z(J, d.n1), d.p1 == NULLF ? nothing : z(J))
+        d.kind == COUPLING_DEEP_MLP && return (z(H, d.n1), z(H, H, M - 1), z(J, H), d.p3 == NULLF ? nothing : z(M * H + J))
+        return (z(H, d.n1), d.p1 == NULLF ? nothing : z(H), z(J, H), d.p3 == NULLF ? nothing : z(J))
+    end
     d.kind == SCALE_MATRIX && return (z(D, D),)
-    d.kind == COUPLING_MLP && return (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(2d.n0, d.n2),
-                                      d.p3 == NULLF ? nothing : z(2d.n0))
-    d.kind == COUPLING_MLP_RQS && return (J = (3(d.n3 >> 8) - 1) * d.n0;
-                                          (z(d.n2, d.n1), d.p1 == NULLF ? nothing : z(d.n2), z(J, d.n2),
-                                           d.p3 == NULLF ? nothing : z(J)))
-    d.kind == COUPLING_DEEP_MLP && return (M = d.n3 >> 8;
-                                           (z(d.n2, d.n1), z(d.n2, d.n2, M - 1), z(2d.n0, d.n2),
-                                            d.p3 == NULLF ? nothing : z(M * d.n2 + 2d.n0)))
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))

@@ -1,5 +1,5 @@
 """Chain planning pinned on the host: workspace sizes, status codes and launch counts of the chain entry points for a sweep
-of descriptor chains, against tests/golden/chain_plan.json.  No GPU needed: the workspace queries are pure host functions,
+of descriptor chains, against tests/golden/chain_plan.json (and, for the neural spline and deep network couplings, chain_plan_couplings.json).  No GPU needed: the workspace queries are pure host functions,
 and so is b2b_chain_vjp_f32 / _f64 at N = 0 without parameter cotangents (it validates, plans and returns before any CUDA
 call).  The descriptors carry a fake non-NULL address for every parameter; nothing is ever read through it.
 
@@ -15,6 +15,7 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "chain_plan.json")
+GOLDEN_COUPLINGS = os.path.join(ROOT, "tests", "golden", "chain_plan_couplings.json")
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
@@ -23,7 +24,7 @@ from bijectors_jl_b200 import _lib  # noqa: E402
 P = 0x10000  # a fake device address
 NS = (1000, 1 << 20)
 DS = (1, 32, 36, 128, 129, 256, 257, 747, 748, 1024, 1025, 2048, 2049)
-VALID_KINDS = {1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 12, 13}
+VALID_KINDS = {1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 12, 13, 14, 15}
 
 
 def planar(inv=0):
@@ -86,6 +87,18 @@ def mlp(n1, n2, H, inv=0, act=None):
     act = _lib.ACT_TANH if act is None else act
     return dict(kind=_lib.COUPLING_MLP, inverse=inv, p0=P, p1=P, p2=P, p3=P, i0=P, i1=P, n0=n1, n1=n2, n2=H, n3=act,
                 f0=0.01)
+
+
+def nrqs(n1, n2, H, K=8, inv=0, act=None, B=3.0):
+    act = _lib.ACT_TANH if act is None else act
+    return dict(kind=_lib.COUPLING_MLP_RQS, inverse=inv, p0=P, p1=P, p2=P, p3=P, i0=P, i1=P, n0=n1, n1=n2, n2=H,
+                n3=act | K << 8, f0=0.01, f1=B)
+
+
+def deep(n1, n2, H, M=2, inv=0, act=None):
+    act = _lib.ACT_TANH if act is None else act
+    return dict(kind=_lib.COUPLING_DEEP_MLP, inverse=inv, p0=P, p1=P, p2=P, p3=P, i0=P, i1=P, n0=n1, n1=n2, n2=H,
+                n3=act | M << 8, f0=0.01)
 
 
 def cases():
@@ -184,6 +197,45 @@ def cases():
     return out
 
 
+def coupling_cases():
+    """(name, chain, D) for the neural spline (B2B_COUPLING_MLP_RQS) and deep network (B2B_COUPLING_DEEP_MLP) couplings:
+    both sides of every limit, the descriptor rules, both directions, and chains mixing them with other kinds."""
+    out = []
+
+    def add(name, chain, Ds):
+        for D in Ds:
+            out.append((f"{name}@{D}", chain, D))
+
+    # n1, n2, H, K or M and D each on both sides of their limits.  K = 1 is a valid descriptor past the envelope
+    # (B2B_EUNSUPPORTED), M = 1 and H = 0 are invalid descriptors (B2B_EINVAL).
+    for kind, f, depths in (("nrqs", lambda n1, n2, H, k, inv=0: nrqs(n1, n2, H, k, inv), (16, 17, 1, 0)),
+                            ("deep", lambda n1, n2, H, k, inv=0: deep(n1, n2, H, k, inv), (4, 5, 1, 0))):
+        top, past, low, zero = depths
+        for n1, n2, H, k in ((1, 1, 1, 2), (128, 128, 128, top), (129, 64, 64, 2), (64, 129, 64, 2), (64, 64, 129, 2),
+                             (64, 64, 0, 2), (64, 64, 64, past), (64, 64, 64, low), (64, 64, 64, zero)):
+            add(f"{kind}{n1}x{n2}H{H}k{k}", [f(n1, n2, H, k)], (36, 1024, 1025))
+        add(f"{kind}-inv", [f(32, 32, 64, 3, 1)], (64, 1024, 1025))
+        base = f(16, 16, 32, 2)
+        for field in ("p0", "p1", "p2", "p3", "i0", "i1"):
+            e = dict(base)
+            del e[field]
+            add(f"null-{kind}-{field}", [e], (64,))
+            add(f"planar-then-null-{kind}-{field}", [planar(), e], (64,))
+        add(f"{kind}-then-null-planar", [base, dict(planar(), p1=0)], (64,))
+        # with planar, BatchNorm and both terminals
+        add(f"planar-bn-{kind}-bn-diag", [planar(), bn(), f(32, 32, 64, 3), bn(1), diag()], (64, 1025))
+        add(f"{kind}-inv-planar-tril", [f(64, 64, 128, 4, 1), planar(1), tril()], (128, 257))
+        add(f"{kind}-ew-diag", [f(32, 32, 64, 2), ew(), diag()], (64, 1024))
+    add("nrqs-leaky", [nrqs(32, 32, 64, act=_lib.ACT_LEAKY_RELU)], (64,))
+    add("nrqs-act9", [nrqs(32, 32, 64, act=9)], (64,))
+    add("nrqs-B0", [nrqs(32, 32, 64, B=0.0)], (64,))
+    add("nrqs-Bneg", [nrqs(32, 32, 64, B=-1.0)], (64,))
+    add("deep-leaky", [deep(32, 32, 64, act=_lib.ACT_LEAKY_RELU)], (64,))
+    add("deep-act9", [deep(32, 32, 64, act=9)], (64,))
+    add("nrqs-deep-mlp-srqs", [nrqs(16, 16, 32), deep(16, 16, 32, 2, 1), mlp(16, 16, 32), srqs(16, 16)], (32, 64))
+    return out
+
+
 def _arr(chain, t):
     ds = []
     for spec in chain:
@@ -220,23 +272,35 @@ def _load(path):
     return handle
 
 
+def all_cases():
+    return cases() + coupling_cases()
+
+
 def record(path=_lib.LIB_PATH):
     L_ = _load(path)
-    data = {name: measure(L_, chain, D) for name, chain, D in cases()}
-    with open(GOLDEN, "w") as f:
-        json.dump(data, f, separators=(",", ":"), sort_keys=True)
-        f.write("\n")
-    print(f"{len(data)} chains -> {GOLDEN}")
+    for golden, sweep in ((GOLDEN, cases), (GOLDEN_COUPLINGS, coupling_cases)):
+        data = {name: measure(L_, chain, D) for name, chain, D in sweep()}
+        with open(golden, "w") as f:
+            if golden == GOLDEN:
+                json.dump(data, f, separators=(",", ":"), sort_keys=True)
+            else:  # one chain per line
+                f.write("{\n" + ",\n".join(f"{json.dumps(k)}:{json.dumps(data[k], separators=(',', ':'))}"
+                                             for k in sorted(data)) + "\n}")
+            f.write("\n")
+        print(f"{len(data)} chains -> {golden}")
 
 
 @pytest.fixture(scope="module")
 def expected():
-    with open(GOLDEN) as f:
-        return json.load(f)
+    out = {}
+    for golden in (GOLDEN, GOLDEN_COUPLINGS):
+        with open(golden) as f:
+            out.update(json.load(f))
+    return out
 
 
 def test_sweep_covers_the_fixture(expected):
-    names = [name for name, _, _ in cases()]
+    names = [name for name, _, _ in all_cases()]
     assert len(names) == len(set(names))
     assert set(names) == set(expected)
 
@@ -244,7 +308,7 @@ def test_sweep_covers_the_fixture(expected):
 def test_chain_plan_matches_fixture(expected):
     L_ = _lib.lib()
     bad = []
-    for name, chain, D in cases():
+    for name, chain, D in all_cases():
         got = measure(L_, chain, D)
         if got != expected[name]:
             bad.append((name, got, expected[name]))
@@ -255,7 +319,7 @@ def test_invalid_kind_needs_no_intermediate():
     """A chain with a kind include/b2b.h does not define has no launch plan: the workspace query returns at once, sizing
     no D x N intermediate whether or not y is wanted."""
     L_ = _lib.lib()
-    for name, chain, D in cases():
+    for name, chain, D in all_cases():
         if all(s["kind"] in VALID_KINDS for s in chain):
             continue
         a = _arr(chain, _lib.LayerDesc)
