@@ -11,7 +11,7 @@ from .interface import (  # noqa: F401
     with_logabsdet_jacobian, with_logabsdet_jacobian_,
 )
 from .layers import (  # noqa: F401
-    AffineConditioner, Coupling, Elementwise, InvertibleBatchNorm, LeakyReLU, Logit, MLPConditioner, MLPSplineConditioner, DeepMLPConditioner, PartitionMask, Permute, PlanarLayer, RadialLayer,
+    AffineConditioner, Coupling, Elementwise, InvertibleBatchNorm, LeakyReLU, Logit, MLPConditioner, MLPSplineConditioner, DeepMLPConditioner, DeepMLPSplineConditioner, PartitionMask, Permute, PlanarLayer, RadialLayer,
     RationalQuadraticSpline, Scale, Shift, SplineConditioner, Stacked, TruncatedBijector, coupling, elementwise,
 )
 from .transformed_distribution import (  # noqa: F401

@@ -67,6 +67,8 @@ bool b2b_coupling_fits(const b2b_layer_desc& d, int D) {
        1, 1, B2B_COUPLING_MLP_RQS_MAX_D},
       {B2B_COUPLING_DEEP_MLP, B2B_COUPLING_DEEP_MLP_MAX_N, 1, B2B_COUPLING_DEEP_MLP_MAX_H, 0, 0,
        2, B2B_COUPLING_DEEP_MLP_MAX_DEPTH, B2B_COUPLING_DEEP_MLP_MAX_D},
+      {B2B_COUPLING_DEEP_MLP_RQS, B2B_COUPLING_DEEP_MLP_RQS_MAX_N, 1, B2B_COUPLING_DEEP_MLP_RQS_MAX_H, 2,
+       B2B_COUPLING_DEEP_MLP_RQS_MAX_K, 2, B2B_COUPLING_DEEP_MLP_RQS_MAX_DEPTH, B2B_COUPLING_DEEP_MLP_RQS_MAX_D},
   };
   const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
   auto in = [](int v, int lo, int hi) { return v >= lo && v <= hi; };

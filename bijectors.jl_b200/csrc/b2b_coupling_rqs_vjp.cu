@@ -19,6 +19,15 @@
 // of its column from a staged x₂ tile, and the row loop runs on h with W₂ and c₂, so its fp64 accumulator holds h̄.
 // After the loop each thread recomputes W₁x₂ + c₁ for σ′, turns h̄ into v̄ = h̄ ⊙ σ′ and forms x̄₂ = ȳ₂ + W₁ᵀv̄ in a fixed
 // order; the CTA adds Σ v̄ x₂ᵀ and Σ v̄ to its slice, laid out [W̄₂ | c̄₂ | W̄₁ ([H][n2]) | c̄₁ ([H])].
+//
+// The deep neural spline coupling, B2B_COUPLING_DEEP_MLP_RQS, is the instantiation DEEP = true (with MLP = true).  Each
+// thread forms h_1 .. h_M of its column before the row loop, alternating between Xs and one more [H][XP] block E.  After
+// the loop the fp64 accumulator holds h̄_M, and the kernel walks back l = M .. 2: each thread recomputes h_{l−1} of its
+// column from x₂ (again through Xs and E: the hidden layers cost (M − 1)·H² FMAs per column against (3K − 1)·n1·H for
+// the row loop, so recomputing them is cheap and keeps the workspace independent of N), forms v̄_l = h̄_l ⊙ σ′_l in the
+// other block and h̄_{l−1} = W_lᵀv̄_l into the accumulator, and the CTA adds Σ v̄_l h_{l−1}ᵀ and Σ v̄_l to its slice.
+// Layer 1 is kind 14's hidden layer above.  The slice appends [W̄_2 … W̄_M ([H][H] each) | c̄_2 … c̄_M ([H] each)] to kind
+// 14's layout, and coupling_rqs_deep_vjp_reduce_kernel sums the slices into the layouts of p0 .. p3.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -42,12 +51,31 @@ struct CrvParams {
   long long N, ldx, ldyb, ldxb, slice;
   int D, n1, n2, K;
   float B;
-  const float *W1, *c1;  // MLP only
+  const float *W1, *c1;  // MLP only (DEEP: c1 = [c_1 | … | c_M], or NULL)
   int H, act;
   float slope;
+  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
+  int M;            // DEEP: hidden layers
 };
 
-template <bool INV, bool MLP>
+// DEEP: layer l (1-based) of the network on this thread's column, from `in` (n_in rows) to `out` ([H] rows), stride XP
+template <int XP>
+__device__ __forceinline__ void crv_layer(const CrvParams& P, int l, const float* in, int n_in, float* out, int tid) {
+  const int H = P.H;
+  const float* W = l == 1 ? P.W1 : P.Wh + (size_t)(l - 2) * H * H;
+  const float* c = P.c1 ? P.c1 + (size_t)(l - 1) * H : nullptr;
+  for (int m = 0; m < H; ++m) {
+    float dh;
+    mlp_act(P.act, P.slope, crq_hidden_pre(W, c, H, n_in, in + tid, XP, m), out[m * XP + tid], dh);
+  }
+}
+
+// DEEP: the second [H][XP] block E, after the D row kinds
+__device__ __forceinline__ float* crv_deep_block(unsigned char* kind, int D) {
+  return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kind + D) + 15) & ~(uintptr_t)15);
+}
+
+template <bool INV, bool MLP, bool DEEP>
 __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __grid_constant__ CrvParams P) {
   extern __shared__ __align__(16) float crv_sm[];
   constexpr int TN = CRV_TN, XP = CRV_TN + 1;
@@ -72,6 +100,8 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
 
   for (int r = tid; r < D; r += TN) kind[r] = 0;
   for (long long e = tid; e < slen; e += TN) slice[e] = 0.f;
+  if constexpr (DEEP)  // W̄_2 .. W̄_M and c̄_2 .. c̄_M follow kind 14's sums
+    for (long long e = tid; e < (long long)(P.M - 1) * nc * (nc + 1); e += TN) slice[slen + e] = 0.f;
   __syncthreads();
   for (int i = tid; i < n1; i += TN) kind[P.idx1[i]] = 1;
   for (int m = tid; m < n2; m += TN) kind[P.idx2[m]] = 2;
@@ -97,7 +127,17 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
       (MLP ? X2 : Xs)[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
       if (!MLP) XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
     }
-    if (MLP) {  // h of this thread's column (as the forward kernel forms it); h̄ starts at 0
+    if constexpr (DEEP) {  // h_1 .. h_M of this thread's column (as the forward kernel forms them), h_M in Xs
+      __syncthreads();
+      float* const E = crv_deep_block(kind, D);
+      const float* in = X2;
+      for (int l = 1; l <= P.M; ++l) {
+        float* out = (P.M - l) % 2 == 0 ? Xs : E;
+        crv_layer<XP>(P, l, in, l == 1 ? n2 : nc, out, tid);
+        in = out;
+      }
+      for (int m = 0; m < nc; ++m) XB[m * XP + tid] = 0.0;  // h̄_M starts at 0
+    } else if (MLP) {  // h of this thread's column (as the forward kernel forms it); h̄ starts at 0
       __syncthreads();
       for (int m = 0; m < nc; ++m) {
         float dh;
@@ -169,6 +209,52 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
       }
     }
     __syncthreads();
+    if constexpr (DEEP) {
+      float* const E = crv_deep_block(kind, D);
+      float* const whslice = w1slice + (size_t)nc * (n2 + 1);  // W̄_2 .. W̄_M ([H][H] each), then c̄_2 .. c̄_M
+      for (int l = P.M; l >= 2; --l) {
+        // h_{l−1} of this thread's column, recomputed from x₂ through E and Xs (the previous step's reads are done)
+        const float* hin = X2;
+        for (int j = 1; j < l; ++j) {
+          float* out = (l - 1 - j) % 2 == 0 ? Xs : E;
+          crv_layer<XP>(P, j, hin, j == 1 ? n2 : nc, out, tid);
+          hin = out;
+        }
+        // v̄_l = h̄_l ⊙ σ′(W_l·h_{l−1} + c_l) into E, then h̄_{l−1} = W_lᵀv̄_l (the sum over the units in increasing
+        // order) into the accumulator: both this thread's column only
+        const float* Wl = P.Wh + (size_t)(l - 2) * nc * nc;
+        const float* cl = P.c1 ? P.c1 + (size_t)(l - 1) * nc : nullptr;
+        for (int m = 0; m < nc; ++m) {
+          float h, dh;
+          mlp_act(P.act, P.slope, crq_hidden_pre(Wl, cl, nc, nc, hin + tid, XP, m), h, dh);
+          E[m * XP + tid] = (float)XB[m * XP + tid] * dh;
+        }
+        for (int k = 0; k < nc; ++k) {
+          float s = 0.f;
+          for (int m = 0; m < nc; ++m) s = fmaf(__ldg(Wl + (size_t)k * nc + m), E[m * XP + tid], s);
+          XB[k * XP + tid] = (double)s;
+        }
+        __syncthreads();
+        // this tile's Σ_n v̄_l h_{l−1}ᵀ and Σ_n v̄_l, added to the CTA's slice (each element always by the same thread)
+        float* wsl = whslice + (size_t)(l - 2) * nc * nc;
+        for (int e = tid; e < nc * nc; e += TN) {
+          const int m = e / nc, k = e - m * nc;
+          const float* vb = E + m * XP;
+          const float* hs = hin + k * XP;
+          float s = 0.f;
+          for (int c = 0; c < cols; ++c) s = fmaf(vb[c], hs[c], s);
+          wsl[e] += s;
+        }
+        float* csl = whslice + (size_t)(P.M - 1) * nc * nc + (size_t)(l - 2) * nc;
+        for (int m = tid; m < nc; m += TN) {
+          const float* vb = E + m * XP;
+          float s = 0.f;
+          for (int c = 0; c < cols; ++c) s += vb[c];
+          csl[m] += s;
+        }
+        __syncthreads();
+      }
+    }
     if (MLP) {
       // v̄ = h̄ ⊙ σ′(W₁x₂ + c₁) of this thread's column into Xs (h is no longer read)
       for (int m = 0; m < nc; ++m) {
@@ -214,6 +300,40 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
   }
 }
 
+// The deep network's four sums, the G slices summed in order in fp64: W̄_out (J x H, J = (3K − 1)·n1) and c̄_out, W̄_in
+// (H x n2) and c̄_1, then W̄_2 .. W̄_M and c̄_2 .. c̄_M, each to the layout of its parameter (p0 = W_in, p1 = W_hid, p2 =
+// W_out, p3 = [c_1 | … | c_M | c_out]; NULL: not wanted).
+__global__ void __launch_bounds__(256) coupling_rqs_deep_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
+                                                                           long long slice, int n1, int H, int n2, int K,
+                                                                           int M, float* __restrict__ Winbar,
+                                                                           float* __restrict__ Whbar,
+                                                                           float* __restrict__ Woutbar,
+                                                                           float* __restrict__ cbar) {
+  const long long J = (long long)(3 * K - 1) * n1, hh = (long long)H * H;
+  const long long nw = J * H, nwc = nw + J, nw1 = nwc + (long long)H * n2, nc1 = nw1 + H, nwh = nc1 + (M - 1) * hh;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nwh + (long long)(M - 1) * H) return;
+  double t = 0.0;
+  for (int g = 0; g < nparts; ++g) t += part[(size_t)g * slice + e];
+  if (e < nw) {  // [i][j][m] -> W_out row i + n1·j, column m
+    const long long i = e / ((3 * K - 1) * (long long)H), rem = e - i * (3 * K - 1) * H, j = rem / H, m = rem - j * H;
+    if (Woutbar) Woutbar[(size_t)(i + n1 * j) + (size_t)J * m] = (float)t;
+  } else if (e < nwc) {  // [i][j] -> c_out[i + n1·j]
+    const long long f = e - nw, i = f / (3 * K - 1), j = f - i * (3 * K - 1);
+    if (cbar) cbar[(size_t)M * H + (size_t)(i + n1 * j)] = (float)t;
+  } else if (e < nw1) {  // [m][k] -> W_in row m, column k
+    const long long f = e - nwc, m = f / n2, k = f - m * n2;
+    if (Winbar) Winbar[(size_t)(m + H * k)] = (float)t;
+  } else if (e < nc1) {
+    if (cbar) cbar[e - nw1] = (float)t;
+  } else if (e < nwh) {  // [l − 2][m][k] -> W_l row m, column k
+    const long long f = e - nc1, l = f / hh, m = (f - l * hh) / H, k = f - l * hh - m * H;
+    if (Whbar) Whbar[(size_t)(l * hh + m + H * k)] = (float)t;
+  } else if (cbar) {  // c̄_2 .. c̄_M
+    cbar[(size_t)H + (size_t)(e - nwh)] = (float)t;
+  }
+}
+
 // W̄ / c̄: the G slices summed in order, element e of the slice layout scattered to W's column-major layout.  nc: the
 // conditioning rows (n2, or H); with the network also W̄₁ (nh x nx, the slice's [nh][nx]) and c̄₁ (nh), else nh = 0.
 __global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
@@ -246,16 +366,22 @@ using Cpl = B2BCoupling<b2b_layer_desc>;
 static int crv_nc(const Cpl& c) { return c.net ? c.H : c.n2; }
 static int crv_nx(const Cpl& c) { return c.net ? c.n2 : 0; }
 
+// the deep network's hidden-to-hidden layers W_2 .. W_M (0: none)
+static int crv_nl(const Cpl& c) { return c.M > 1 ? c.M - 1 : 0; }
+
 static size_t crv_smem_bytes(const Cpl& c, int D) {
   const int nc = crv_nc(c), K = c.K, J = 3 * K - 1, JP = crq_jp(K), K1 = K + 1;
   const size_t f = (size_t)nc * JP + JP + (size_t)6 * K1 * CRV_TN + (size_t)nc * (CRV_TN + 1) + (size_t)J * (CRV_TN + 1);
-  return (((f + 1) / 2 + (size_t)nc * (CRV_TN + 1)) * sizeof(double) + (size_t)crv_nx(c) * (CRV_TN + 1) * sizeof(float) +
-          D + 15) & ~(size_t)15;
+  const size_t e = crv_nl(c) ? (size_t)c.H * (CRV_TN + 1) * sizeof(float) : 0;  // the deep network's block E
+  return ((((f + 1) / 2 + (size_t)nc * (CRV_TN + 1)) * sizeof(double) + (size_t)crv_nx(c) * (CRV_TN + 1) * sizeof(float) +
+           D + 15) & ~(size_t)15) + e;
 }
 
-// floats of the slice's sums: W̄ / c̄ of the spline's conditioner, then W̄₁ / c̄₁ of the network
+// floats of the slice's sums: W̄ / c̄ of the spline's conditioner, then W̄₁ / c̄₁ of the network, then W̄_2 .. W̄_M and
+// c̄_2 .. c̄_M of the deep network
 static long long crv_sum_floats(const Cpl& c) {
-  return (long long)c.n1 * (3 * c.K - 1) * (crv_nc(c) + 1) + (long long)c.H * (crv_nx(c) + 1);
+  return (long long)c.n1 * (3 * c.K - 1) * (crv_nc(c) + 1) + (long long)c.H * (crv_nx(c) + 1) +
+         (long long)crv_nl(c) * c.H * (c.H + 1);
 }
 
 static long long crv_slice_floats(const b2b_layer_desc& d) { return (crv_sum_floats(b2b_coupling(d)) + 63) & ~63LL; }
@@ -319,19 +445,27 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   P.act = c.act;
   P.B = c.B;
   P.slope = c.slope;
+  P.Wh = c.W_hid;
+  P.M = c.M;
+  const bool deep = crv_nl(c) > 0;
   const int grid = crv_grid(d, D, N);
   const size_t smem = crv_smem_bytes(c, D);
   void (*kernel)(const CrvParams) =
-      mlp ? (d.inverse ? coupling_rqs_vjp_kernel<true, true> : coupling_rqs_vjp_kernel<false, true>)
-          : (d.inverse ? coupling_rqs_vjp_kernel<true, false> : coupling_rqs_vjp_kernel<false, false>);
+      !deep ? (mlp ? (d.inverse ? coupling_rqs_vjp_kernel<true, true, false> : coupling_rqs_vjp_kernel<false, true, false>)
+                   : (d.inverse ? coupling_rqs_vjp_kernel<true, false, false> : coupling_rqs_vjp_kernel<false, false, false>))
+            : (d.inverse ? coupling_rqs_vjp_kernel<true, true, true> : coupling_rqs_vjp_kernel<false, true, true>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CRV_TN, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   const long long len = crv_sum_floats(c);
-  coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
-      P.part, grid, P.slice, c.n1, crv_nc(c), c.K, Wbar, cbar, c.H, crv_nx(c), mlp ? s.bars[0] : nullptr,
-      c.c_in ? s.bars[1] : nullptr);
+  if (!deep)
+    coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
+        P.part, grid, P.slice, c.n1, crv_nc(c), c.K, Wbar, cbar, c.H, crv_nx(c), mlp ? s.bars[0] : nullptr,
+        c.c_in ? s.bars[1] : nullptr);
+  else  // c̄ packs every bias: there is one only when the layer has biases
+    coupling_rqs_deep_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
+        P.part, grid, P.slice, c.n1, c.H, c.n2, c.K, c.M, s.bars[0], s.bars[1], s.bars[2], c.c_in ? s.bars[3] : nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   *s.launches += 2;
   return B2B_OK;

@@ -135,7 +135,7 @@ size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long 
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
-// COUPLING_RQS, SCALE_MATRIX, COUPLING_MLP, COUPLING_MLP_RQS and COUPLING_DEEP_MLP).
+// COUPLING_RQS, SCALE_MATRIX, COUPLING_MLP, COUPLING_MLP_RQS, COUPLING_DEEP_MLP and COUPLING_DEEP_MLP_RQS).
 int b2b_f64_validate_layer(const b2b_layer_desc_f64& d, int D, bool last);
 // Sets what b2b_last_launch_count reports for the calling thread (entry points outside b2b_api.cu).
 void b2b_set_last_launch_count(int n);
@@ -173,7 +173,7 @@ struct B2BFwdSeg {
   int* launches;
   cudaStream_t stream;
 };
-int b2b_fwd_spline(const B2BFwdSeg& s);  // b2b_coupling_rqs.cu: COUPLING_RQS and COUPLING_MLP_RQS
+int b2b_fwd_spline(const B2BFwdSeg& s);  // b2b_coupling_rqs.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
 int b2b_fwd_mlp(const B2BFwdSeg& s);     // b2b_coupling_mlp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
 int b2b_fwd_scale(const B2BFwdSeg& s);   // b2b_scale_matrix.cu: y == NULL writes log-Jacobians only
 int b2b_fwd_tril(const B2BFwdSeg& s);    // b2b_mvnormal_tril.cu: copies x to y (when y != x), writes logpdf to logjac
@@ -215,7 +215,7 @@ int b2b_vjp_coupling(const B2BVjpSeg& s);  // b2b_coupling_vjp.cu
 int b2b_vjp_batchnorm(const B2BVjpSeg& s); // b2b_coupling_vjp.cu: eval mode
 int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / PERMUTE, optionally closed by MVNORMAL_DIAG
 int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
-int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS and COUPLING_MLP_RQS
+int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
 int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu
 int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
 // One launch copying slot i of layer j from base[i] + j·step[i] to bars[4j + i], for the requested slots of a run of
@@ -270,6 +270,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_COUPLING_MLP,    B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P1 | B2B_F_P3, false},
       {B2B_COUPLING_MLP_RQS, B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P1 | B2B_F_P3, false},
       {B2B_COUPLING_DEEP_MLP, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P3, false},
+      {B2B_COUPLING_DEEP_MLP_RQS, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P3, false},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -285,7 +286,7 @@ inline bool b2b_chain_has_launch(const b2b_layer_desc* layers, int L, int launch
 }
 
 // ---- coupling descriptors ------------------------------------------------------------------------------------------
-// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP descriptor decoded: the one place that knows how include/b2b.h
+// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS descriptor decoded: the one place that knows how include/b2b.h
 // packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or b2b_layer_desc_f64.
 template <class Desc>
 struct B2BCoupling {
@@ -304,21 +305,22 @@ struct B2BCoupling {
 
 inline bool b2b_is_coupling(int kind) {
   return kind == B2B_COUPLING_AFFINE || kind == B2B_COUPLING_RQS || kind == B2B_COUPLING_MLP ||
-         kind == B2B_COUPLING_MLP_RQS || kind == B2B_COUPLING_DEEP_MLP;
+         kind == B2B_COUPLING_MLP_RQS || kind == B2B_COUPLING_DEEP_MLP || kind == B2B_COUPLING_DEEP_MLP_RQS;
 }
 
 template <class Desc>
 B2BCoupling<Desc> b2b_coupling(const Desc& d) {
   const int k = d.kind;
-  const bool deep = k == B2B_COUPLING_DEEP_MLP;
+  const bool deep_rqs = k == B2B_COUPLING_DEEP_MLP_RQS, deep = k == B2B_COUPLING_DEEP_MLP || deep_rqs;
   B2BCoupling<Desc> c{};
   c.n1 = d.n0;
   c.n2 = d.n1;
   c.net = k == B2B_COUPLING_MLP || k == B2B_COUPLING_MLP_RQS || deep;
-  c.spline = k == B2B_COUPLING_RQS || k == B2B_COUPLING_MLP_RQS;
-  c.K = k == B2B_COUPLING_RQS ? d.n2 : k == B2B_COUPLING_MLP_RQS ? d.n3 >> 8 : 0;  // MLP_RQS: n3 = σ | K << 8
-  c.M = deep ? d.n3 >> 8 : c.net ? 1 : 0;                                          // DEEP_MLP: n3 = σ | M << 8
-  c.B = k == B2B_COUPLING_RQS ? d.f0 : k == B2B_COUPLING_MLP_RQS ? d.f1 : 0;
+  c.spline = k == B2B_COUPLING_RQS || k == B2B_COUPLING_MLP_RQS || deep_rqs;
+  // MLP_RQS: n3 = σ | K << 8; DEEP_MLP: n3 = σ | M << 8; DEEP_MLP_RQS: n3 = σ | K << 8 | M << 16
+  c.K = k == B2B_COUPLING_RQS ? d.n2 : k == B2B_COUPLING_MLP_RQS ? d.n3 >> 8 : deep_rqs ? (d.n3 >> 8) & 255 : 0;
+  c.M = deep_rqs ? d.n3 >> 16 : deep ? d.n3 >> 8 : c.net ? 1 : 0;
+  c.B = k == B2B_COUPLING_RQS ? d.f0 : k == B2B_COUPLING_MLP_RQS || deep_rqs ? d.f1 : 0;
   c.idx1 = d.i0;
   c.idx2 = d.i1;
   c.row1 = k == B2B_COUPLING_AFFINE ? d.n2 : -1;
@@ -333,14 +335,14 @@ B2BCoupling<Desc> b2b_coupling(const Desc& d) {
   c.slope = d.f0;
   c.W_in = d.p0;
   c.W_out = d.p2;
-  // DEEP_MLP: p1 = W_hid, p3 = [c_1 | … | c_M | c_out] (or NULL)
+  // DEEP_MLP, DEEP_MLP_RQS: p1 = W_hid, p3 = [c_1 | … | c_M | c_out] (or NULL)
   c.W_hid = deep ? d.p1 : nullptr;
   c.c_in = deep ? d.p3 : d.p1;
   c.c_out = !deep ? d.p3 : d.p3 ? d.p3 + (size_t)c.M * c.H : nullptr;
   return c;
 }
 
-// Float32 kernel envelope of a COUPLING_RQS / _MLP / _MLP_RQS / _DEEP_MLP layer at D: the B2B_COUPLING_*_MAX_* limits
+// Float32 kernel envelope of a COUPLING_RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS layer at D: the B2B_COUPLING_*_MAX_* limits
 // of include/b2b.h (the affine coupling's limits are shared-memory budgets, b2b_coupling_affine_fits).  Defined in
 // b2b_api.cu: inline here, it changes the SASS nvcc 12.9 emits for the neural-spline reverse-mode kernels.
 bool b2b_coupling_fits(const b2b_layer_desc& d, int D);
@@ -368,7 +370,7 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
   bool ok = c.n1 >= 1 && c.n2 >= 1 && c.n1 + c.n2 <= D;
   if (c.net) ok = ok && c.H >= 1 && (c.act == B2B_ACT_TANH || c.act == B2B_ACT_LEAKY_RELU);
   if (c.spline) ok = ok && c.K >= 1 && c.B > 0;
-  if (d.kind == B2B_COUPLING_DEEP_MLP) ok = ok && c.M >= 2;
+  if (d.kind == B2B_COUPLING_DEEP_MLP || d.kind == B2B_COUPLING_DEEP_MLP_RQS) ok = ok && c.M >= 2;
   // an index list may be NULL when n2 / n3 gives the first row of its contiguous range
   if (d.kind == B2B_COUPLING_AFFINE) ok = ok && (c.idx1 || c.row1 >= 0) && (c.idx2 || c.row2 >= 0);
   return ok ? B2B_OK : B2B_EINVAL;
@@ -382,7 +384,7 @@ size_t b2b_slot_len(const Desc& d, int i, int D) {
     const size_t J = c.spline ? (size_t)(3 * c.K - 1) * c.n1 : (size_t)2 * c.n1;  // rows of W_out
     if (!c.net) return i == 0 ? J * c.n2 : J;                                      // W, c
     const size_t H = c.H, M = c.M;
-    const bool deep = d.kind == B2B_COUPLING_DEEP_MLP;
+    const bool deep = d.kind == B2B_COUPLING_DEEP_MLP || d.kind == B2B_COUPLING_DEEP_MLP_RQS;
     // W_in (H x n2), c_in (H) or the deep network's W_hid ((M−1) x H x H), W_out (J x H), c_out (J) or every bias
     const size_t len[4] = {H * c.n2, deep ? (M - 1) * H * H : H, J * H, deep ? M * H + J : J};
     return len[i];

@@ -810,13 +810,15 @@ def isclosedform(t) -> bool:
 
 def _coupling_slots(d, D):
     """Shapes of a coupling descriptor's slots.  H hidden units, K spline bins and M hidden layers (0 where the kind has
-    none) are decoded here only: n2 is K or H, and n3 packs σ | K << 8 or σ | M << 8 (include/b2b.h)."""
+    none) are decoded here only: n2 is K or H, and n3 packs σ | K << 8, σ | M << 8 or σ | K << 8 | M << 16
+    (include/b2b.h)."""
     H, K, M = {_lib.COUPLING_RQS: (0, d.n2, 0), _lib.COUPLING_MLP: (d.n2, 0, 1), _lib.COUPLING_MLP_RQS: (d.n2, d.n3 >> 8, 1),
-               _lib.COUPLING_DEEP_MLP: (d.n2, 0, d.n3 >> 8)}.get(d.kind, (0, 0, 0))
+               _lib.COUPLING_DEEP_MLP: (d.n2, 0, d.n3 >> 8),
+               _lib.COUPLING_DEEP_MLP_RQS: (d.n2, (d.n3 >> 8) & 255, d.n3 >> 16)}.get(d.kind, (0, 0, 0))
     J = (3 * K - 1) * d.n0 if K else 2 * d.n0  # rows of the last layer
     if not H:
         return (d.n1, J), (J,)
-    if d.kind == _lib.COUPLING_DEEP_MLP:
+    if d.kind in (_lib.COUPLING_DEEP_MLP, _lib.COUPLING_DEEP_MLP_RQS):
         return (d.n1, H), (M - 1, H, H), (H, J), (M * H + J,)
     return (d.n1, H), (H,), (H, J), (J,)
 
@@ -836,6 +838,7 @@ _SLOTS = {
     _lib.COUPLING_MLP: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
+    _lib.COUPLING_DEEP_MLP_RQS: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 

@@ -43,6 +43,7 @@ const SCALE_MATRIX = Int32(12)
 const COUPLING_MLP = Int32(13)
 const COUPLING_MLP_RQS = Int32(14)
 const COUPLING_DEEP_MLP = Int32(15)
+const COUPLING_DEEP_MLP_RQS = Int32(16)
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -204,9 +205,42 @@ function desc(cl::Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}}, inv::Bool
               θ.slope, 0f0, pointer(θ.W_in), pointer(θ.W_hid), pointer(θ.W_out), θ.c === nothing ? NULLF : pointer(θ.c),
               pointer(dm.idx1), pointer(dm.idx2))
 end
+# The neural spline flow's law with the deep network of DeepMLPConditioner: the RationalQuadraticSpline of
+# SplineConditioner whose raw knots v = W_out*h_M .+ c_out come from M >= 2 hidden layers.  W_hid is H × H × (M−1) and c
+# packs [c_1; …; c_M; c_out] or is `nothing`, as for DeepMLPConditioner.  A callable returning the reference's own spline,
+# so the same object also runs on the CPU reference path.  Float32, n1, n2 <= 128, H <= 128, 2 <= K <= 16, M <= 4,
+# D <= 1024 on the device.
+struct DeepMLPSplineConditioner{M<:AbstractMatrix,A<:AbstractArray,V}
+    W_in::M   # (H × n2)
+    W_hid::A  # (H × H × (M−1))
+    W_out::M  # ((3K−1)·n1 × H)
+    c::V      # M·H + (3K−1)·n1, or nothing
+    K::Int
+    B::Float32
+    act::Int32      # ACT_TANH or ACT_LEAKY_RELU
+    slope::Float32
+end
+function (θ::DeepMLPSplineConditioner)(x₂)
+    H, M = size(θ.W_in, 1), size(θ.W_hid, 3) + 1
+    σ(v) = θ.act == ACT_TANH ? tanh.(v) : ifelse.(v .>= 0, v, θ.slope .* v)
+    bias(l) = θ.c === nothing ? false : θ.c[((l - 1) * H + 1):(l * H)]
+    h = σ(θ.W_in * x₂ .+ bias(1))
+    for l in 2:M
+        h = σ(θ.W_hid[:, :, l - 1] * h .+ bias(l))
+    end
+    SplineConditioner(θ.W_out, θ.c === nothing ? nothing : θ.c[(M * H + 1):end], θ.K, θ.B)(h)
+end
+function desc(cl::Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}}, inv::Bool)
+    dm = get!(() -> DeviceMask(cl.mask), MASKS, cl.mask)
+    θ = cl.θ
+    M = size(θ.W_hid, 3) + 1
+    LayerDesc(COUPLING_DEEP_MLP_RQS, inv, length(dm.idx1), length(dm.idx2), size(θ.W_in, 1),
+              θ.act | (Int32(θ.K) << 8) | (Int32(M) << 16), θ.slope, θ.B, pointer(θ.W_in), pointer(θ.W_hid),
+              pointer(θ.W_out), θ.c === nothing ? NULLF : pointer(θ.c), pointer(dm.idx1), pointer(dm.idx2))
+end
 desc(cl::Coupling, ::Bool) =
-    error("Coupling: only AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner and " *
-          "DeepMLPConditioner laws run on the device path (no CPU fallback)")
+    error("Coupling: only AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner, " *
+          "DeepMLPConditioner and DeepMLPSplineConditioner laws run on the device path (no CPU fallback)")
 
 # Permute(A): y[dst[i]] = x[i] with dst = the row of the single 1 in column i (permute.jl:90-100,152)
 const PERMS = IdDict{Any,CuVector{Int32}}()
@@ -262,6 +296,7 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           Coupling{<:AffineConditioner},Coupling{<:SplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
+                          Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}},
                           Scale{<:CuMatrix{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
@@ -464,21 +499,23 @@ end
 # fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, Scale(A) a, BatchNorm b logs, the
 # terminal MvNormal's μ σ) in the fields' shapes; `nothing` for fields without one.
 # Hidden units H, spline bins K and hidden layers M of a coupling descriptor (0 where the kind has none), decoded here only:
-# n2 is K or H, and n3 packs σ | K << 8 or σ | M << 8 (include/b2b.h).
+# n2 is K or H, and n3 packs σ | K << 8, σ | M << 8 or σ | K << 8 | M << 16 (include/b2b.h).
 coupling_hkm(d::LayerDesc) =
     d.kind == COUPLING_RQS ? (0, Int(d.n2), 0) : d.kind == COUPLING_MLP ? (Int(d.n2), 0, 1) :
     d.kind == COUPLING_MLP_RQS ? (Int(d.n2), Int(d.n3 >> 8), 1) :
-    d.kind == COUPLING_DEEP_MLP ? (Int(d.n2), 0, Int(d.n3 >> 8)) : (0, 0, 0)
+    d.kind == COUPLING_DEEP_MLP ? (Int(d.n2), 0, Int(d.n3 >> 8)) :
+    d.kind == COUPLING_DEEP_MLP_RQS ? (Int(d.n2), Int((d.n3 >> 8) & 255), Int(d.n3 >> 16)) : (0, 0, 0)
 function vjp_slots(d::LayerDesc, D::Integer)
     z(dims...) = CUDA.zeros(Float32, dims...)
     d.kind == PLANAR && return (z(D), z(D), z(1))
     d.kind == RADIAL && return (z(1), z(1), z(D))
     d.kind == RQS && return (z(D, d.n0), z(D, d.n0), z(D, d.n0))
-    if d.kind in (COUPLING_AFFINE, COUPLING_RQS, COUPLING_MLP, COUPLING_MLP_RQS, COUPLING_DEEP_MLP)
+    if d.kind in (COUPLING_AFFINE, COUPLING_RQS, COUPLING_MLP, COUPLING_MLP_RQS, COUPLING_DEEP_MLP, COUPLING_DEEP_MLP_RQS)
         H, K, M = coupling_hkm(d)
         J = K > 0 ? (3K - 1) * d.n0 : 2d.n0  # rows of the last layer
         H == 0 && return (z(J, d.n1), d.p1 == NULLF ? nothing : z(J))
-        d.kind == COUPLING_DEEP_MLP && return (z(H, d.n1), z(H, H, M - 1), z(J, H), d.p3 == NULLF ? nothing : z(M * H + J))
+        d.kind in (COUPLING_DEEP_MLP, COUPLING_DEEP_MLP_RQS) &&
+            return (z(H, d.n1), z(H, H, M - 1), z(J, H), d.p3 == NULLF ? nothing : z(M * H + J))
         return (z(H, d.n1), d.p1 == NULLF ? nothing : z(H), z(J, H), d.p3 == NULLF ? nothing : z(J))
     end
     d.kind == SCALE_MATRIX && return (z(D, D),)

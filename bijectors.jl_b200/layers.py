@@ -391,24 +391,23 @@ class MLPSplineConditioner(_NetworkConditioner):
         self.c2 = _bias(c2, "c2", W2n.shape[0], device)
 
 
-class DeepMLPConditioner(_NetworkConditioner):
-    """The RealNVP coupling law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) of :class:`MLPConditioner` with a deeper network, a
-    Flux ``Chain(Dense(n2, H, σ), Dense(H, H, σ), …, Dense(H, 2n1))``: h_1 = σ.(W_in·x₂ + c_1), h_l = σ.(W_l·h_{l−1} + c_l)
-    for l = 2..M, [s; t] = W_out·h_M + c_out.  ``weights = [W_in (H × n2), W_2 … W_M (H × H), W_out (2·n1 × H)]`` in the
-    reference's index order, M >= 2 hidden layers, rows 1..n1 of W_out giving s.  ``biases`` is None (no biases at all,
-    the descriptor's pointer is NULL) or all M + 1 vectors ``[c_1 … c_M (H each), c_out (2·n1)]``, so that training never
-    adds a bias the network did not have.  Float32 only.  Runs as B2B_COUPLING_DEEP_MLP: n1, n2 <= 128, H <= 128,
-    M <= 4, D <= 1024.  Device tensors: W_in, W_hid (M−1, H, H: each matrix column-major, back to back), W_out and c
-    (every bias packed); ``weights`` / ``biases`` give per-layer views in the reference's orientation."""
+class _DeepNetworkConditioner(_NetworkConditioner):
+    """A conditioner whose parameters come from M >= 2 hidden layers h_1 = σ.(W_in·x₂ + c_1),
+    h_l = σ.(W_l·h_{l−1} + c_l) (l = 2..M) and a last layer W_out·h_M + c_out.  Device tensors: W_in, W_hid (M−1, H, H:
+    each matrix column-major, back to back), W_out and c (every bias packed); ``weights`` / ``biases`` give per-layer
+    views in the reference's orientation."""
 
     _fields = ("W_in", "W_hid", "W_out", "c")
+    _shallow = ""  # the one-hidden-layer conditioner of the same law
 
-    def __init__(self, weights, biases=None, *, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
-        self._network("DeepMLPConditioner", activation, slope, dtype)
+    def _deep_network(self, who, weights, biases, activation, slope, dtype, device, last_layer):
+        """Checks the layers and sets activation, slope, M, H, n2, W_in, W_hid, W_out and c; ``last_layer(W_out)``
+        checks the law's last layer (rows × H) and sets n1."""
+        self._network(who, activation, slope, dtype)
         weights = list(weights)
         if len(weights) < 3:
-            raise ValueError(f"DeepMLPConditioner: weights must be [W_in, W_2, …, W_M, W_out] with M >= 2 hidden layers "
-                             f"(one hidden layer is MLPConditioner), got {len(weights)} matrices")
+            raise ValueError(f"{who}: weights must be [W_in, W_2, …, W_M, W_out] with M >= 2 hidden layers "
+                             f"(one hidden layer is {self._shallow}), got {len(weights)} matrices")
         self.M = len(weights) - 1
         W_in = self._first_layer("W_in", weights[0])
         H = self.H
@@ -417,12 +416,10 @@ class DeepMLPConditioner(_NetworkConditioner):
             if W.shape != (H, H):
                 raise ValueError(f"W_{l} must be (H, H) with H = {H}, got {W.shape}")
         W_out = _host32(weights[-1])
-        if W_out.ndim != 2 or W_out.shape[0] == 0 or W_out.shape[0] % 2 or W_out.shape[1] != H:
-            raise ValueError(f"W_out must be (2*n1, H) with H = {H}, got {W_out.shape}")
-        self.n1 = W_out.shape[0] // 2
+        last_layer(W_out)
         self.W_in = _dev_f32(W_in, device)  # column-major (H × n2)
         self.W_hid = _dev_f32(np.ascontiguousarray(np.stack([W.T for W in hid])), device)  # [l − 2] = W_l column-major
-        self.W_out = _dev_f32(np.ascontiguousarray(W_out.T), device)  # column-major (2n1 × H)
+        self.W_out = _dev_f32(np.ascontiguousarray(W_out.T), device)  # column-major (rows × H)
         self.c = None
         if biases is not None:
             biases = list(biases)
@@ -430,7 +427,7 @@ class DeepMLPConditioner(_NetworkConditioner):
                 raise ValueError(f"biases must be None or all {self.M + 1} vectors [c_1, …, c_{self.M}, c_out], "
                                  f"got {len(biases)}")
             names = [f"c_{l}" for l in range(1, self.M + 1)] + ["c_out"]
-            sizes = [H] * self.M + [2 * self.n1]
+            sizes = [H] * self.M + [W_out.shape[0]]
             parts = [_host32(b).reshape(-1) for b in biases]
             for name, n, b in zip(names, sizes, parts):
                 if b.shape != (n,):
@@ -451,10 +448,53 @@ class DeepMLPConditioner(_NetworkConditioner):
         return [self.c[l * H:(l + 1) * H] for l in range(M)] + [self.c[M * H:]]
 
 
+class DeepMLPConditioner(_DeepNetworkConditioner):
+    """The RealNVP coupling law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) of :class:`MLPConditioner` with a deeper network, a
+    Flux ``Chain(Dense(n2, H, σ), Dense(H, H, σ), …, Dense(H, 2n1))``: h_1 = σ.(W_in·x₂ + c_1), h_l = σ.(W_l·h_{l−1} + c_l)
+    for l = 2..M, [s; t] = W_out·h_M + c_out.  ``weights = [W_in (H × n2), W_2 … W_M (H × H), W_out (2·n1 × H)]`` in the
+    reference's index order, M >= 2 hidden layers, rows 1..n1 of W_out giving s.  ``biases`` is None (no biases at all,
+    the descriptor's pointer is NULL) or all M + 1 vectors ``[c_1 … c_M (H each), c_out (2·n1)]``, so that training never
+    adds a bias the network did not have.  Float32 only.  Runs as B2B_COUPLING_DEEP_MLP: n1, n2 <= 128, H <= 128,
+    M <= 4, D <= 1024.  Device tensors: W_in, W_hid (M−1, H, H: each matrix column-major, back to back), W_out and c
+    (every bias packed); ``weights`` / ``biases`` give per-layer views in the reference's orientation."""
+
+    _shallow = "MLPConditioner"
+
+    def __init__(self, weights, biases=None, *, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+        self._deep_network("DeepMLPConditioner", weights, biases, activation, slope, dtype, device, self._affine_out)
+
+    def _affine_out(self, W_out):
+        if W_out.ndim != 2 or W_out.shape[0] == 0 or W_out.shape[0] % 2 or W_out.shape[1] != self.H:
+            raise ValueError(f"W_out must be (2*n1, H) with H = {self.H}, got {W_out.shape}")
+        self.n1 = W_out.shape[0] // 2
+
+
+class DeepMLPSplineConditioner(_DeepNetworkConditioner):
+    """The neural spline flow's coupling law (Durkan et al. 2019) with a deep network: θ(x₂) =
+    RationalQuadraticSpline(…, B) as for :class:`SplineConditioner`, with the raw knots v = W_out·h_M + c_out from the M
+    hidden layers of :class:`DeepMLPConditioner`, a Flux ``Chain(Dense(n2, H, σ), Dense(H, H, σ), …,
+    Dense(H, (3K−1)·n1))``.  ``weights = [W_in (H × n2), W_2 … W_M (H × H), W_out ((3K−1)·n1 × H)]`` in the reference's
+    index order, M >= 2 hidden layers; ``biases`` is None or all M + 1 vectors ``[c_1 … c_M (H each),
+    c_out ((3K−1)·n1)]``.  Float32 only.  Runs as B2B_COUPLING_DEEP_MLP_RQS: n1, n2 <= 128, H <= 128, 2 <= K <= 16,
+    M <= 4, D <= 1024.  Device tensors and views as for :class:`DeepMLPConditioner`."""
+
+    _shallow = "MLPSplineConditioner"
+
+    def __init__(self, weights, biases=None, *, K: int, B: float, activation="tanh", slope=0.0, device="cuda",
+                 dtype=torch.float32):
+        def spline_out(W_out):
+            self.K, self.B, self.n1 = _spline_law("DeepMLPSplineConditioner", W_out, K, B, "H")
+            if W_out.shape[1] != self.H:
+                raise ValueError(f"W_out must be ((3K-1)*n1, H) with H = {self.H}, got {W_out.shape}")
+
+        self._deep_network("DeepMLPSplineConditioner", weights, biases, activation, slope, dtype, device, spline_out)
+
+
 class Coupling(_ParamLayer):
     """Coupling(θ, mask) (coupling.jl:178-181).  θ is an arbitrary closure in the reference; the device
     path supports the recognised :class:`AffineConditioner`, :class:`SplineConditioner`, :class:`MLPConditioner`,
-    :class:`MLPSplineConditioner` and :class:`DeepMLPConditioner` and raises for anything else (no CPU fallback)."""
+    :class:`MLPSplineConditioner`, :class:`DeepMLPConditioner` and :class:`DeepMLPSplineConditioner` and raises for
+    anything else (no CPU fallback)."""
 
     _fields = ()
 
@@ -462,9 +502,10 @@ class Coupling(_ParamLayer):
         if isinstance(mask, int):  # Coupling(θ, n): first n÷2 rows transformed (:183-186)
             mask = PartitionMask(mask, range(1, mask // 2 + 1))
         if not isinstance(θ, (AffineConditioner, SplineConditioner, MLPConditioner, MLPSplineConditioner,
-                              DeepMLPConditioner)):
+                              DeepMLPConditioner, DeepMLPSplineConditioner)):
             raise B2BError(_lib.B2B_EUNSUPPORTED, "Coupling: only AffineConditioner, SplineConditioner, MLPConditioner, "
-                                                  "MLPSplineConditioner and DeepMLPConditioner laws run on the device path")
+                                                  "MLPSplineConditioner, DeepMLPConditioner and DeepMLPSplineConditioner "
+                                                  "laws run on the device path")
         if θ.n1 != len(mask.indices_1) or θ.n2 != len(mask.indices_2):
             raise ValueError("conditioner shape does not match the PartitionMask")
         self.θ, self.mask = θ, mask
@@ -502,6 +543,11 @@ class Coupling(_ParamLayer):
             return [_desc(_lib.COUPLING_DEEP_MLP, inverse, p0=θ.W_in, p1=θ.W_hid, p2=θ.W_out,
                           p3=θ.c if θ.c is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
                           n3=θ._ACT[θ.activation] | (θ.M << 8), f0=θ.slope)]
+        if isinstance(self.θ, DeepMLPSplineConditioner):
+            θ = self.θ
+            return [_desc(_lib.COUPLING_DEEP_MLP_RQS, inverse, p0=θ.W_in, p1=θ.W_hid, p2=θ.W_out,
+                          p3=θ.c if θ.c is not None else 0, i0=self._idx1, i1=self._idx2, n0=θ.n1, n1=θ.n2, n2=θ.H,
+                          n3=θ._ACT[θ.activation] | (θ.K << 8) | (θ.M << 16), f0=θ.slope, f1=θ.B)]
         if isinstance(self.θ, MLPSplineConditioner):
             θ = self.θ
             return [_desc(_lib.COUPLING_MLP_RQS, inverse, p0=θ.W1, p1=θ.c1 if θ.c1 is not None else 0, p2=θ.W2,
@@ -518,11 +564,11 @@ class Coupling(_ParamLayer):
             return False
         if isinstance(self.θ, SplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
             return False
-        if isinstance(self.θ, MLPSplineConditioner) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
+        if isinstance(self.θ, (MLPSplineConditioner, DeepMLPSplineConditioner)) and (self.θ.K, self.θ.B) != (o.θ.K, o.θ.B):
             return False
-        if isinstance(self.θ, DeepMLPConditioner) and self.θ.M != o.θ.M:
+        if isinstance(self.θ, _DeepNetworkConditioner) and self.θ.M != o.θ.M:
             return False
-        if isinstance(self.θ, (MLPConditioner, MLPSplineConditioner, DeepMLPConditioner)) and \
+        if isinstance(self.θ, _NetworkConditioner) and \
                 (self.θ.activation, self.θ.slope) != (o.θ.activation, o.θ.slope):
             return False
         return all((a is None) == (b is None) and (a is None or torch.equal(a, b))

@@ -99,7 +99,17 @@ extern "C" {
 #define B2B_COUPLING_DEEP_MLP_MAX_H 128
 #define B2B_COUPLING_DEEP_MLP_MAX_DEPTH 4
 #define B2B_COUPLING_DEEP_MLP_MAX_D 1024
-/* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS and B2B_COUPLING_DEEP_MLP (descriptor field n3) */
+#define B2B_COUPLING_DEEP_MLP_RQS 16 /* Coupling, θ = x₂ -> RationalQuadraticSpline(…, B), raw knots from an MLP with M hidden layers   coupling.jl */
+/* Envelope of B2B_COUPLING_DEEP_MLP_RQS (every entry point, forward, inverse and reverse mode): n1, n2 <= 128,
+ * 1 <= H <= 128, 2 <= K <= 16, 2 <= M <= 4 hidden layers, D <= 1024.  A layer past it returns B2B_EUNSUPPORTED with
+ * nothing launched, and the workspace queries return 0; the Float64 entry points refuse the kind the same way. */
+#define B2B_COUPLING_DEEP_MLP_RQS_MAX_N 128
+#define B2B_COUPLING_DEEP_MLP_RQS_MAX_H 128
+#define B2B_COUPLING_DEEP_MLP_RQS_MAX_K 16
+#define B2B_COUPLING_DEEP_MLP_RQS_MAX_DEPTH 4
+#define B2B_COUPLING_DEEP_MLP_RQS_MAX_D 1024
+/* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and
+ * B2B_COUPLING_DEEP_MLP_RQS (descriptor field n3) */
 #define B2B_ACT_TANH 0
 #define B2B_ACT_LEAKY_RELU 1 /* v >= 0 ? v : a*v with a = f0 (a = 0: ReLU), the convention of B2B_EW_LEAKY_RELU */
 
@@ -187,6 +197,18 @@ extern "C" {
  *                     y₂ = x₂) as for COUPLING_MLP.  n1, n2, H >= 1, n1 + n2 <= D, M >= 2 and a known σ, else B2B_EINVAL.
  *                     Float32 only, exact fp32 FMA on the CUDA cores, its own launch.  Envelope:
  *                     B2B_COUPLING_DEEP_MLP_MAX_*; the Float64 entry points return B2B_EUNSUPPORTED.)
+ * COUPLING_DEEP_MLP_RQS W_in[H x n2] W_hid  W_out[J x H] c|NULL    idx1[n1]        idx2[n2]      n1    n2   a
+ *                    (J = (3K−1)·n1; n2 of the descriptor = H hidden units, n3 = σ | (K << 8) | (M << 16) with
+ *                     σ = B2B_ACT_TANH or B2B_ACT_LEAKY_RELU (slope a = f0), K bins and M >= 2 hidden layers, f1 = B > 0.
+ *                     W_hid holds W_2 .. W_M, each H x H, back to back (W_l at offset (l − 2)·H²); c packs every bias,
+ *                     [c_1 (H) | … | c_M (H) | c_out (J)], or is NULL for none.  All matrices are column-major; W_in,
+ *                     W_hid, W_out and both index lists are required.  Per column h_1 = σ.(W_in·x₂ + c_1),
+ *                     h_l = σ.(W_l·h_{l−1} + c_l) for l = 2..M and v = W_out·h_M + c_out; transformed row i takes its raw
+ *                     widths, heights and derivatives from v, with the normalisation, spline, inverse (the network
+ *                     evaluated on y₂ = x₂) and identity outside [−B, B] of COUPLING_RQS and COUPLING_MLP_RQS.
+ *                     n1, n2, H >= 1, n1 + n2 <= D, K >= 1, M >= 2, a known σ and B > 0, else B2B_EINVAL.  Float32 only,
+ *                     exact fp32 on the CUDA cores, its own launch.  Envelope: B2B_COUPLING_DEEP_MLP_RQS_MAX_*; the
+ *                     Float64 entry points return B2B_EUNSUPPORTED.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -234,6 +256,8 @@ const char* b2b_status_string(int status);
  * envelope of B2B_COUPLING_MLP_RQS_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
  * COUPLING_DEEP_MLP runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x; the
  * envelope of B2B_COUPLING_DEEP_MLP_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
+ * COUPLING_DEEP_MLP_RQS runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x;
+ * the envelope of B2B_COUPLING_DEEP_MLP_RQS_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
  * The whole chain is planned before anything is enqueued: a
  * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
@@ -372,7 +396,8 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * COUPLING_RQS, whose W̄ is ((3K−1)·n1 x n2) column-major like W; a c̄ request with c == NULL returns B2B_EINVAL);
  * COUPLING_MLP and COUPLING_MLP_RQS W₁ c₁ W₂ c₂ (column-major like the parameters; a c̄₁ / c̄₂ request whose c is NULL
  * returns B2B_EINVAL); COUPLING_DEEP_MLP W_in W_hid W_out c (in the layouts of p0 .. p3: W̄_hid packs the M − 1 matrices
- * like W_hid, c̄ every bias like c; a c̄ request with c == NULL returns B2B_EINVAL);
+ * like W_hid, c̄ every bias like c; a c̄ request with c == NULL returns B2B_EINVAL); COUPLING_DEEP_MLP_RQS W_in W_hid
+ * W_out c the same way (W̄_out ((3K−1)·n1 x H) column-major like W_out);
  * SCALE_MATRIX a (Ā, D x D column-major like A: G + (Σ l̄)·A⁻ᵀ, or −A⁻ᵀ G A⁻ᵀ − (Σ l̄)·A⁻ᵀ for the inverse layer, with
  * G = Σₙ ȳₙ uₙᵀ over the layer's inputs u; slots 1-3 return B2B_EUNSUPPORTED);
  * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
@@ -480,7 +505,8 @@ int b2b_mvnormal_diag_logpdf_f32(const float* x, const float* mu, const float* s
 /* ---- Float64 batches -------------------------------------------------------------------------------------------------
  * The reference is generic in its element type and its own tests run in Float64 (test/normalising_flows.jl:47-71 checks
  * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind but B2B_COUPLING_RQS,
- * B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS and B2B_COUPLING_DEEP_MLP (Float32 only: the Float64 entry points and workspace
+ * B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and B2B_COUPLING_DEEP_MLP_RQS (Float32 only: the Float64
+ * entry points and workspace
  * queries refuse them with B2B_EUNSUPPORTED / 0),
  * both directions, the terminal
  * MvNormal, the deterministic batch sum -- on D x N Float64 batches with Float64 parameters (b2b_layer_desc_f64: the
