@@ -15,7 +15,8 @@ from .layers import (  # noqa: F401
     RationalQuadraticSpline, Scale, Shift, SplineConditioner, Stacked, TruncatedBijector, coupling, elementwise,
 )
 from .transformed_distribution import (  # noqa: F401
-    MvNormal, PosDefException, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, transformed,
+    MvNormal, PosDefException, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, rand_logpdf, rand_vjp,
+    transformed,
 )
 from . import autograd, distributed  # noqa: F401
 

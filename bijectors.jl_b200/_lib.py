@@ -148,6 +148,12 @@ _SIGS = {
                                      c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "b2b_chain_sample_tril_f32": (c_int, [POINTER(LayerDesc), c_int32, _F32P, _F32P, c_uint64, c_uint64, c_int64, _F32P,
                                           _F32P, c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "b2b_chain_sample_logq_workspace_bytes": (c_size_t, [POINTER(LayerDesc), c_int32, POINTER(LayerDesc), c_int32, c_int64]),
+    "b2b_chain_sample_logq_f32": (c_int, [POINTER(LayerDesc), c_int32, POINTER(LayerDesc), c_uint64, c_uint64, c_int64,
+                                          _F32P, _F32P, c_int32, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "b2b_chain_sample_vjp_workspace_bytes": (c_size_t, [POINTER(LayerDesc), c_int32, POINTER(LayerDesc), c_int32, c_int64]),
+    "b2b_chain_sample_vjp_f32": (c_int, [POINTER(LayerDesc), c_int32, POINTER(LayerDesc), c_uint64, c_uint64, c_int64,
+                                         _F32P, c_int64, _F32P, c_void_p, c_int32, c_int64, c_void_p, c_size_t, c_void_p]),
     "b2b_host_ctx_create": (c_int, [POINTER(c_void_p), c_int32, c_int64, c_int32]),
     "b2b_host_ctx_destroy": (c_int, [c_void_p]),
     "b2b_host_ctx_wait_stream": (c_int, [c_void_p, c_void_p]),

@@ -415,6 +415,40 @@ class _ChainFn(torch.autograd.Function):
         return (xbar, None, None, None, *out)
 
 
+class _RSampleFn(torch.autograd.Function):
+    """rand_logpdf of a transformed base, differentiable in the flow's and the base's parameters with the draw z held
+    fixed; backward = ONE b2b_chain_sample_vjp_f32 call whose cotangents are routed to the parameters by device address.
+    The seed of the forward is kept for the backward."""
+
+    @staticmethod
+    def forward(ctx, td, n: int, seed: int, offset: int, column_offset: int, *params):
+        from .transformed_distribution import _rsample_setup, rand_logpdf
+
+        y, lq = rand_logpdf(td, n, seed, offset, column_offset)
+        dist, descs, _, base, dev = _rsample_setup(td, n, "rsample")
+        full = list(descs) + [base]
+        owner = {p.data_ptr(): k for k, p in enumerate(params) if ctx.needs_input_grad[5 + k]}
+        ctx.want = [(l, i, owner[getattr(d, f"p{i}")]) for l, d in enumerate(full) for i in _trainable_slots(d)
+                    if getattr(d, f"p{i}") in owner]
+        ctx.descs, ctx.base, ctx.D, ctx.n, ctx.dev = descs, base, dist.D, int(n), dev
+        ctx.seed, ctx.offset, ctx.column_offset, ctx.shapes = seed, offset, column_offset, [p.shape for p in params]
+        return y, lq
+
+    @staticmethod
+    def backward(ctx, ybar, lqbar):
+        from .transformed_distribution import _rand_vjp_raw
+
+        yb = _colmajor(ybar) if ybar is not None else None
+        lb = lqbar.contiguous() if lqbar is not None else None
+        bars = _rand_vjp_raw(ctx.descs, ctx.base, ctx.D, ctx.n, ctx.dev, yb, lb, ctx.seed, ctx.offset,
+                             ctx.column_offset, [(l, i) for l, i, _ in ctx.want])
+        out: List = [None] * len(ctx.shapes)
+        for l, i, k in ctx.want:
+            g = bars[(l, i)].reshape(ctx.shapes[k])
+            out[k] = g if out[k] is None else out[k] + g
+        return (None, None, None, None, None, *out)
+
+
 class Flow(torch.nn.Module):
     """A trainable flow made of ANY chain of the supported layers -- `Stacked(ibs) ∘ PlanarLayer(2)`, spline flows with
     permutations, coupling flows with bounded outputs -- over an optional MvNormal base.  Its parameters are the trainable
@@ -457,3 +491,15 @@ class Flow(torch.nn.Module):
 
     def nll(self, y: torch.Tensor) -> torch.Tensor:
         return -self.logpdf(y).sum()
+
+    def rsample(self, n: int, seed=None, offset: int = 0, column_offset: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``(y, logq)`` = rand_logpdf(transformed(base, transform), n, ...): n samples of the flow and their log-density,
+        differentiable in ``params`` -- the flow's and the base's μ, σ or L -- with the base draw held fixed (the
+        reparameterisation gradient of an ELBO, docs/src/advi.md).  The backward is one b2b_chain_sample_vjp_f32 call
+        with the forward's seed (``seed=None`` draws one, once).  Float32 only; the flow needs an MvNormal base."""
+        from .transformed_distribution import MvNormal, _seed, transformed
+
+        if not isinstance(self.base, MvNormal):
+            raise ValueError("Flow.rsample: the flow has no base distribution; construct it with Flow(transform, MvNormal(D, ...))")
+        td = transformed(self.base, self.transform)
+        return _RSampleFn.apply(td, int(n), _seed(seed), int(offset), int(column_offset), *self.params)

@@ -942,14 +942,28 @@ int vjp_planar_run(B2BVjpSeg a, int Dk, float* const pad[3], float* xst, float* 
 
 }  // namespace
 
-extern "C" size_t b2b_chain_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N) {
-  if (!layers || L < 1 || L > B2B_MAX_CHAIN || D < 1 || N < 0) return 0;
-  for (int l = 0; l < L; ++l)
-    if (validate_layer(layers[l], D, l == L - 1) != B2B_OK) return 0;
+// The chain checks of the reverse mode that need no batch: descriptors, then segments.  b2b_chain_vjp_f32 makes the same
+// checks with the slot requests between them, so that its status for a bad request keeps its precedence.
+static int vjp_chain_check(const b2b_layer_desc* layers, int32_t L, int32_t D, std::vector<VSeg>& segs) {
+  if (!layers || L < 1 || L > B2B_MAX_CHAIN || D < 1) return B2B_EINVAL;
+  for (int l = 0; l < L; ++l) {
+    const int rc = validate_layer(layers[l], D, l == L - 1);
+    if (rc != B2B_OK) return rc;
+  }
+  return vjp_segments(layers, L, D, segs);
+}
+
+int b2b_chain_vjp_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D) {
   std::vector<VSeg> segs;
-  if (vjp_segments(layers, L, D, segs) != B2B_OK) return 0;
+  return vjp_chain_check(layers, L, D, segs);
+}
+
+extern "C" size_t b2b_chain_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N) {
+  std::vector<VSeg> segs;
+  if (N < 0 || vjp_chain_check(layers, L, D, segs) != B2B_OK) return 0;
   return vjp_layout(layers, segs, D, N).total;
 }
+
 
 extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const float* x, const float* ybar,
                                  const float* ljbar, float* xbar, float* const* param_bars, int32_t D, int64_t N,

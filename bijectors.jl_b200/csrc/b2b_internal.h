@@ -133,6 +133,23 @@ size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long 
 size_t b2b_coupling_mlp_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
 // B2B_OK when b2b_chain_run_f32 accepts `layers` at D (every descriptor valid, every segment planned), else its status
 int b2b_chain_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
+// The one-launch form of rand (b2b_sample.cu), shared by b2b_chain_sample_f32 and b2b_chain_sample_logq_f32 (logq: `out`
+// receives log q instead of ℓ): *launched = false, with nothing enqueued, when the chain does not fuse.
+int b2b_launch_sample_fused(const b2b_layer_desc* layers, int L, const float* mu, const float* sigma, uint64_t seed,
+                            uint64_t offset, int64_t column_offset, float* y, float* out, int D, long long N,
+                            long long ldy, bool logq, bool* launched, cudaStream_t stream);
+// B2B_OK when b2b_chain_vjp_f32 accepts `layers` at D (L >= 1), else the status it returns before launching anything
+int b2b_chain_vjp_check_f32(const b2b_layer_desc* layers, int32_t L, int32_t D);
+// The TRIL base of the reparameterised sampler (b2b_mvnormal_tril.cu, D <= B2B_TRIL_MAX_D).  b2b_tril_sample: y = μ + L z
+// with z the b2b_randn_f32 stream, and with logq != NULL logq[n] = qsign·(−½·D·log2π − Σ log Lᵢᵢ − ½‖zₙ‖²), one launch.
+// b2b_tril_base_vjp: μ̄ = Σ x̄ₙ and L̄ = tril(Σ x̄ₙ zₙᵀ) − (*qsum)·diag(1/Lᵢᵢ) (qsum NULL: 0) over the chunked GEMM and
+// its ordered reduce, two launches; workspace b2b_tril_base_vjp_workspace(D, N) bytes.
+int b2b_tril_sample(const float* Lg, const float* mu, uint64_t seed, uint64_t offset, long long col0, float* y,
+                    long long ldy, float* logq, float qsign, int D, long long N, cudaStream_t stream);
+size_t b2b_tril_base_vjp_workspace(int D, long long N);
+int b2b_tril_base_vjp(const float* xbar, long long ldxb, const float* z, const double* qsum, const float* Lg,
+                      float* mubar, float* Lbar, int D, long long N, void* workspace, int* launches,
+                      cudaStream_t stream);
 // Float64 chains (b2b_chain_f64.cu): B2B_OK when b2b_chain_run_f64 accepts descriptor `d` at D (`last`: the chain's final
 // element, the only place a MVNORMAL_DIAG may stand), else B2B_EINVAL (B2B_EUNSUPPORTED for the Float32-only
 // COUPLING_RQS, SCALE_MATRIX, COUPLING_MLP, COUPLING_MLP_RQS, COUPLING_DEEP_MLP and COUPLING_DEEP_MLP_RQS).

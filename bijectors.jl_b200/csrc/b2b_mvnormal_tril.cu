@@ -261,13 +261,14 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
   if (ljp) cta_partial(acc, sm.red, ljp);
 }
 
-// y = μ + L z with z the Philox stream of b2b_randn_f32 (rows 4k..4k+3 of global column n from one counter)
-template <int R, int C>
-__global__ void __launch_bounds__(kWarps * 32, 1)
-    sample_kernel(float* __restrict__ y, long long ldy, const b2b::V1Gen gen, const float* __restrict__ Lg,
-                  const float* __restrict__ mu, int D, long long N) {
+// y = μ + L z with z the Philox stream of b2b_randn_f32 (rows 4k..4k+3 of global column n from one counter).
+// LOGQ: also logq[n] = qsign·(c0 − ½‖zₙ‖²), the base log-density of the sample from the z it holds in registers.
+template <int R, int C, bool LOGQ>
+__device__ __forceinline__ void sample_body(float* __restrict__ y, long long ldy, const b2b::V1Gen& gen,
+                                            const float* __restrict__ Lg, const float* __restrict__ mu, int D, long long N,
+                                            float* __restrict__ logq, float qsign) {
   const Smem sm = carve(D);
-  stage(Lg, mu, D, sm.L, sm.rinv, sm.mu, sm.c0);
+  const float c0 = stage(Lg, mu, D, sm.L, sm.rinv, sm.mu, sm.c0);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = lane & (kLPG - 1), g0 = lane & kLPG;
   const long long chunks = (N + 2 * C - 1) / (2 * C);
   for (long long ch = (long long)blockIdx.x * kWarps + warp; ch < chunks; ch += (long long)gridDim.x * kWarps) {
@@ -316,6 +317,17 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
         }
       }
     }
+    if constexpr (LOGQ) {
+#pragma unroll
+      for (int c = 0; c < C; ++c) {
+        float q = 0.f;
+#pragma unroll
+        for (int k = 0; k < R; ++k) q = fmaf(z[k][c], z[k][c], q);
+        q = group_sum(q);
+        const long long n = col0 + c;
+        if (t == c && n < N) logq[n] = qsign * fmaf(-0.5f, q, c0);
+      }
+    }
 #pragma unroll
     for (int c = 0; c < C; ++c) {
       const long long n = col0 + c;
@@ -327,6 +339,20 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
       }
     }
   }
+}
+
+template <int R, int C>
+__global__ void __launch_bounds__(kWarps * 32, 1)
+    sample_kernel(float* __restrict__ y, long long ldy, const b2b::V1Gen gen, const float* __restrict__ Lg,
+                  const float* __restrict__ mu, int D, long long N) {
+  sample_body<R, C, false>(y, ldy, gen, Lg, mu, D, N, nullptr, 0.f);
+}
+
+template <int R, int C>
+__global__ void __launch_bounds__(kWarps * 32, 1)
+    sample_logq_kernel(float* __restrict__ y, long long ldy, const b2b::V1Gen gen, const float* __restrict__ Lg,
+                       const float* __restrict__ mu, int D, long long N, float* __restrict__ logq, float qsign) {
+  sample_body<R, C, true>(y, ldy, gen, Lg, mu, D, N, logq, qsign);
 }
 
 // ---- L̄ = tril(S Rᵀ) over column chunks: CTA (tile, p) writes the 64 x 64 tile of Σ_{n in chunk p} S[:, n] R[:, n]ᵀ
@@ -599,5 +625,47 @@ extern "C" int b2b_chain_sample_tril_f32(const b2b_layer_desc* layers, int32_t L
     launches += b2b_last_launch_count();
   }
   b2b_set_last_launch_count(launches);
+  return B2B_OK;
+}
+
+// ---- the TRIL base of the reparameterised sampler (b2b_rsample.cu) ----------------------------------------------------
+int b2b_tril_sample(const float* Lg, const float* mu, uint64_t seed, uint64_t offset, long long col0, float* y,
+                    long long ldy, float* logq, float qsign, int D, long long N, cudaStream_t stream) {
+  if (D < 1 || D > B2B_TRIL_MAX_D) return B2B_EUNSUPPORTED;
+  const b2b::V1Gen gen{seed, offset, col0, nullptr, nullptr};
+  const int R = rows_per_lane(D);
+  int rc = B2B_EUNSUPPORTED;
+#define B2B_TRIL_SMPQ(RR)                                                                                          \
+  case RR:                                                                                                         \
+    rc = logq ? launch(sample_logq_kernel<RR, c_two(RR)>, grid_for(c_two(RR), N), D, stream, y, ldy, gen, Lg, mu, D, \
+                       N, logq, qsign)                                                                             \
+              : launch(sample_kernel<RR, c_two(RR)>, grid_for(c_two(RR), N), D, stream, y, ldy, gen, Lg, mu, D, N); \
+    break;
+  switch (R) {
+    B2B_TRIL_SMPQ(1) B2B_TRIL_SMPQ(2) B2B_TRIL_SMPQ(4) B2B_TRIL_SMPQ(8) B2B_TRIL_SMPQ(16)
+  }
+#undef B2B_TRIL_SMPQ
+  return rc;
+}
+
+size_t b2b_tril_base_vjp_workspace(int D, long long N) {
+  if (D < 1 || D > B2B_TRIL_MAX_D || N < 1) return 0;
+  const long long clen = chunk_len(N), P = (N + clen - 1) / clen;
+  return (sizeof(float) * (size_t)P * D * (D + 1) + 255) & ~(size_t)255;
+}
+
+int b2b_tril_base_vjp(const float* xbar, long long ldxb, const float* z, const double* qsum, const float* Lg,
+                      float* mubar, float* Lbar, int D, long long N, void* workspace, int* launches,
+                      cudaStream_t stream) {
+  const long long clen = chunk_len(N), P = (N + clen - 1) / clen;
+  float* part = static_cast<float*>(workspace);
+  float* mup = mubar ? part + (size_t)P * D * D : nullptr;
+  int rc = b2b_launch_outer_chunks(xbar, ldxb, z, D, part, mup, D, N, true, stream);
+  if (rc != B2B_OK) return rc;
+  const long long tot = (long long)D * D + D;
+  finalize_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(part, mup, (int)P, qsum, qsum ? 1 : 0, Lg, Lbar,
+                                                                     mubar, D);
+  if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
+  *launches += 2;
   return B2B_OK;
 }

@@ -6,6 +6,7 @@
 //   b2b_randn_f32        : the generator alone (any D, any ld) -- also the first pass of chains the fused kernel
 //                          does not cover (coupling layers, Permute, D not in {32, 64, 128, 256})
 //   b2b_chain_sample_f32 : generator + chain
+//   b2b_launch_sample_fused : the one-launch form, shared with b2b_chain_sample_logq_f32 (b2b_rsample.cu)
 // The stream is a pure function of (seed, offset, global column, row): see V1Gen.
 #include "b2b_chain_v1_prog.cuh"
 
@@ -50,9 +51,18 @@ __global__ void __launch_bounds__(NW * 32, 1)
   v1_run<D, TPC, CPT, NW, InterpProg<D, TPC, CPT>, 1, true>(P, E, map_y, map_y, prog, nullptr, &G);
 }
 
+// LOGQ (b2b_chain_sample_logq_f32): the N-vector output is log q(y) instead of ℓ(x), see v1_run
 template <int D, int TPC, int CPT, int NW>
+__global__ void __launch_bounds__(NW * 32, 1)
+    chain_sample_logq_kernel(const __grid_constant__ B2BChainParams P, const __grid_constant__ V1Extra E,
+                             const __grid_constant__ CUtensorMap map_y, const __grid_constant__ V1Gen G) {
+  const InterpProg<D, TPC, CPT> prog{P};
+  v1_run<D, TPC, CPT, NW, InterpProg<D, TPC, CPT>, 1, true, true>(P, E, map_y, map_y, prog, nullptr, &G);
+}
+
+template <bool LOGQ, int D, int TPC, int CPT, int NW>
 static int launch_sample(const B2BChainParams& q, const V1Geom& g, const CUtensorMap& my, const V1Gen& gen, cudaStream_t stream) {
-  auto kernel = chain_sample_kernel<D, TPC, CPT, NW>;
+  auto kernel = LOGQ ? chain_sample_logq_kernel<D, TPC, CPT, NW> : chain_sample_kernel<D, TPC, CPT, NW>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<g.grid, NW * 32, g.smem, stream>>>(q, g.extra, my, gen);
@@ -79,11 +89,55 @@ extern "C" int b2b_randn_f32(float* z, const float* mu, const float* sigma, uint
   return (int)cudaGetLastError();
 }
 
+// The one-launch form of a sampling call: the chain is column-local, D is one the thread-per-column pipeline covers and the
+// base vectors are 16-byte aligned.  Both entry points take this decision here, so a chain fuses for
+// b2b_chain_sample_logq_f32 exactly when it fuses for b2b_chain_sample_f32, with the same geometry and therefore the
+// same y.  *launched = false (nothing enqueued) when the chain does not fuse.
+int b2b_launch_sample_fused(const b2b_layer_desc* layers, int L, const float* mu, const float* sigma, uint64_t seed,
+                            uint64_t offset, int64_t column_offset, float* y, float* out, int D, long long N,
+                            long long ldy, bool logq, bool* launched, cudaStream_t stream) {
+  using namespace b2b;
+  *launched = false;
+  bool fused = L > 0 && (D % 4 == 0) && (!mu || (reinterpret_cast<uintptr_t>(mu) & 15) == 0) &&
+               (!sigma || (reinterpret_cast<uintptr_t>(sigma) & 15) == 0);
+  for (int l = 0; l < L && fused; ++l) fused = fusable_kind(layers[l].kind);
+  if (!fused) return B2B_OK;
+  B2BChainParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = y;  // geometry / alignment checks only: the sampling kernel never reads x
+  p.y = y;
+  p.logjac = out;
+  p.N = N;
+  p.ldx = ldy;
+  p.ldy = ldy;
+  p.D = D;
+  p.L = L;
+  for (int l = 0; l < L; ++l) p.layers[l] = layers[l];
+  V1Geom g;
+  int shape = 0;
+  if (b2b_v1_plan(p, g, &shape) != 0) return B2B_OK;
+  CUtensorMap mx, my;
+  if (!make_maps(p, g.cols, &mx, &my, &g.extra.tma3d)) return B2B_OK;
+  const V1Gen gen{seed, offset, column_offset, mu, sigma};
+  *launched = true;
+#define B2B_SAMPLE_SHAPE(S, DD, TPC, CPT, NW) \
+  case S: return logq ? launch_sample<true, DD, TPC, CPT, NW>(p, g, my, gen, stream) : launch_sample<false, DD, TPC, CPT, NW>(p, g, my, gen, stream);
+  switch (shape) {
+    B2B_SAMPLE_SHAPE(2564112, 256, 4, 1, 12)
+    B2B_SAMPLE_SHAPE(1281108, 128, 1, 1, 8)
+    B2B_SAMPLE_SHAPE(1282112, 128, 2, 1, 12)
+    B2B_SAMPLE_SHAPE(641112, 64, 1, 1, 12)
+    B2B_SAMPLE_SHAPE(321116, 32, 1, 1, 16)
+  }
+#undef B2B_SAMPLE_SHAPE
+  *launched = false;
+  return B2B_OK;
+}
+
 extern "C" int b2b_chain_sample_f32(const b2b_layer_desc* layers, int32_t L, const float* mu, const float* sigma,
                                     uint64_t seed, uint64_t offset, int64_t column_offset, float* y, float* logjac,
                                     int32_t D, int64_t N, int64_t ldy, void* workspace, size_t workspace_bytes,
                                     void* stream_) {
-  using namespace b2b;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (L < 0 || L > B2B_MAX_CHAIN || (L > 0 && !layers) || D < 1 || N < 0 || ldy < D) return B2B_EINVAL;
   if (N == 0) return B2B_OK;
@@ -96,39 +150,11 @@ extern "C" int b2b_chain_sample_f32(const b2b_layer_desc* layers, int32_t L, con
     return b2b_randn_f32(y, mu, sigma, seed, offset, column_offset, D, N, ldy, stream_);
   }
   // fused: one launch when the whole chain is column-local and the thread-per-column pipeline covers D
-  bool fused = (D % 4 == 0) && (!mu || (reinterpret_cast<uintptr_t>(mu) & 15) == 0) &&
-               (!sigma || (reinterpret_cast<uintptr_t>(sigma) & 15) == 0);
-  for (int l = 0; l < L && fused; ++l) fused = fusable_kind(layers[l].kind);
-  if (fused) {
-    B2BChainParams p;
-    memset(&p, 0, sizeof(p));
-    p.x = y;  // geometry / alignment checks only: the sampling kernel never reads x
-    p.y = y;
-    p.logjac = logjac;
-    p.N = N;
-    p.ldx = ldy;
-    p.ldy = ldy;
-    p.D = D;
-    p.L = L;
-    for (int l = 0; l < L; ++l) p.layers[l] = layers[l];
-    V1Geom g;
-    int shape = 0;
-    if (b2b_v1_plan(p, g, &shape) == 0) {
-      CUtensorMap mx, my;
-      if (make_maps(p, g.cols, &mx, &my, &g.extra.tma3d)) {
-        V1Gen gen{seed, offset, column_offset, mu, sigma};
-        switch (shape) {
-          case 2564112: return launch_sample<256, 4, 1, 12>(p, g, my, gen, stream);
-          case 1281108: return launch_sample<128, 1, 1, 8>(p, g, my, gen, stream);
-          case 1282112: return launch_sample<128, 2, 1, 12>(p, g, my, gen, stream);
-          case 641112: return launch_sample<64, 1, 1, 12>(p, g, my, gen, stream);
-          case 321116: return launch_sample<32, 1, 1, 16>(p, g, my, gen, stream);
-        }
-      }
-    }
-  }
+  bool launched = false;
+  int rc = b2b_launch_sample_fused(layers, L, mu, sigma, seed, offset, column_offset, y, logjac, D, N, ldy, false,
+                                   &launched, stream);
+  if (launched) return rc;
   // two passes: base samples into y, then the chain in place
-  int rc = b2b_randn_f32(y, mu, sigma, seed, offset, column_offset, D, N, ldy, stream_);
-  if (rc != B2B_OK) return rc;
+  if ((rc = b2b_randn_f32(y, mu, sigma, seed, offset, column_offset, D, N, ldy, stream_)) != B2B_OK) return rc;
   return b2b_chain_run_f32(layers, L, y, y, logjac, nullptr, D, N, ldy, ldy, 0, workspace, workspace_bytes, stream_);
 }

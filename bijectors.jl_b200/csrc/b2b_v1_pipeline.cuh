@@ -278,7 +278,10 @@ struct V1NoState {};
 
 // GEN = true (sampling, rand(td, n)): there is no input batch -- every thread GENERATES the fragment of its column
 // (philox_normal4), the input ring is unused and the kernel's only HBM traffic is the D x N store: 4·(D+1) B/sample.
-template <int D, int TPC, int CPT, int NW, class Prog, int NIN = 1, bool GEN = false>
+// LOGQ = true (with GEN): the N-vector output is the samples' log-density log q(y) = base(z) − ℓ(x) instead of ℓ(x).
+// ‖z‖² is accumulated while z is generated and summed over the TPC lanes of the column; lj starts at −base(z), the
+// program adds ℓ(x), and −lj is stored.  The traffic stays 4·(D+1) B/sample.
+template <int D, int TPC, int CPT, int NW, class Prog, int NIN = 1, bool GEN = false, bool LOGQ = false>
 __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E, const CUtensorMap& map_x,
                                        const CUtensorMap& map_y, const Prog& prog,
                                        const CUtensorMap* map_x2 = nullptr, const V1Gen* gen = nullptr) {
@@ -346,6 +349,19 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
   const int line = t * 128 + ctx.h * C::NQT * BOX_BYTES;  // this thread's first line inside its first box
   double dsum = 0.0;
   bool store_pending = false;
+  // LOGQ: −½·D·log 2π − Σᵢ log σᵢ, the base density's constant (every lane of a column holds the same value: the
+  // butterfly adds the same pairs in every lane)
+  float qc = 0.f;
+  if constexpr (LOGQ) {
+    float ls = 0.f;
+    if (gen->sigma) {
+      B2B_FOR_SLOTS {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) ls += logf(__ldg(gen->sigma + ctx.row(ql, r, e)));
+      }
+    }
+    qc = -0.5f * (D * 1.8378770664093453f) - part_sum<TPC>(ls);
+  }
 
   for (long long j = warp; j < my_tiles; j += NW) {
     const int buf = (int)(j % E.n_in);
@@ -358,6 +374,7 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
     }
 
     float2 x[CPT][C::EPT / 2];
+    float zz[CPT];  // LOGQ: this thread's part of ‖z‖² per column
     auto load_fragment = [&](const unsigned char* src) {
       B2B_FOR_COLS {
         B2B_FOR_SLOTS {
@@ -371,9 +388,12 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
     if constexpr (GEN) {
       B2B_FOR_COLS {
         const long long n = gen->col0 + col + cc * LPC;
+        if constexpr (LOGQ) zz[cc] = 0.f;
         B2B_FOR_SLOTS {
           const int row0 = ctx.row(ql, r, 0);
           float4 z = philox_normal4(*gen, n, row0 >> 2);
+          if constexpr (LOGQ)
+            zz[cc] = fmaf(z.w, z.w, fmaf(z.z, z.z, fmaf(z.y, z.y, fmaf(z.x, z.x, zz[cc]))));
           if (gen->sigma) {
             const float4 sg = __ldg(reinterpret_cast<const float4*>(gen->sigma + row0));
             z = make_float4(z.x * sg.x, z.y * sg.y, z.z * sg.z, z.w * sg.w);
@@ -412,7 +432,8 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
     float lj[CPT];
     B2B_FOR_COLS {
       const long long cl = col + cc * LPC;
-      lj[cc] = (P.accumulate && P.logjac && cl < P.N) ? P.logjac[cl] : 0.0f;
+      if constexpr (LOGQ) lj[cc] = fmaf(0.5f, part_sum<TPC>(zz[cc]), -qc);
+      else lj[cc] = (P.accumulate && P.logjac && cl < P.N) ? P.logjac[cl] : 0.0f;
     }
     if constexpr (NIN == 2) prog.apply(x, ctx, params, lj, st, col);
     else prog.apply(x, ctx, params, lj);
@@ -451,7 +472,7 @@ __device__ __forceinline__ void v1_run(const B2BChainParams& P, const V1Extra& E
       B2B_FOR_COLS {
         const long long cl = col + cc * LPC;
         if (cl < P.N) {
-          if (P.logjac && !(P.accumulate & 2)) P.logjac[cl] = lj[cc];  // accumulate bit 1: logjac is read-only
+          if (P.logjac && !(P.accumulate & 2)) P.logjac[cl] = LOGQ ? -lj[cc] : lj[cc];  // accumulate bit 1: logjac is read-only
           dsum += (double)lj[cc];
         }
       }

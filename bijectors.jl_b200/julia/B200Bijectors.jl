@@ -21,10 +21,12 @@ import Bijectors: transform, logabsdetjac, with_logabsdet_jacobian
 import Distributions
 using Distributions: MvNormal
 using PDMats: PDMat, PDiagMat, ScalMat
-using LinearAlgebra: cholesky
+using LinearAlgebra: LowerTriangular, cholesky, diagind
 using Functors: fmap
 using SparseArrays: findnz
 using Statistics: mean, var
+import ChainRulesCore
+using ChainRulesCore: NoTangent
 
 const libb2b = get(ENV, "LIBB2B", "libb2b.so")
 
@@ -591,6 +593,101 @@ function device_rand(td::TransformedDistribution{<:MvNormal}, n::Integer; seed::
             D, n, stride(y, 2), pointer(ws), ws_bytes, stream_handle()))
     end
     return y
+end
+
+# Reparameterised sampling (variational inference, docs/src/advi.md; the reference keeps non-in-place rand for
+# "differentiating sampling wrt. params of `td.dist` or params of `Bijector`", src/transformed_distribution.jl:210-213).
+# rand_logpdf: the samples device_rand draws (bit for bit) and their log-density log q(y) in the same pass.
+function rand_logpdf(td::TransformedDistribution{<:MvNormal}, n::Integer; seed::UInt64=rand(UInt64),
+                     offset::UInt64=UInt64(0), column_offset::Integer=0)
+    ds = descs(td.transform, false)
+    D, L = length(td.dist), length(ds)
+    base, keep = base_desc(td.dist)
+    bd = [base]
+    y = CuMatrix{Float32}(undef, D, n)
+    lq = CuVector{Float32}(undef, n)
+    nbytes = ccall((:b2b_chain_sample_logq_workspace_bytes, libb2b), Csize_t,
+                   (Ptr{LayerDesc}, Int32, Ptr{LayerDesc}, Int32, Int64), ds, L, bd, D, n)
+    nbytes == 0 && error("B200Bijectors: rand_logpdf: the device path refuses this flow and base")
+    ws = CuVector{UInt8}(undef, nbytes)
+    GC.@preserve ds bd keep ws check(ccall((:b2b_chain_sample_logq_f32, libb2b), Cint,
+        (Ptr{LayerDesc}, Int32, Ptr{LayerDesc}, UInt64, UInt64, Int64, CuPtr{Float32}, CuPtr{Float32}, Int32, Int64, Int64,
+         CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+        ds, L, bd, seed, offset, column_offset, pointer(y), pointer(lq), D, n, stride(y, 2), pointer(ws), nbytes,
+        stream_handle()))
+    return y, lq
+end
+
+# Reverse mode of rand_logpdf with the draw held fixed: ȳ, q̄ the cotangents of (y, log q), `nothing` = zeros.  Returns
+# the flow's cotangents per descriptor in application order (the fields of chain_vjp) and the base's (μ̄, σ̄) or
+# (μ̄, L̄), L̄ lower triangular; all summed over the n columns.
+function rand_vjp(td::TransformedDistribution{<:MvNormal}, n::Integer, ȳ, q̄; seed::UInt64,
+                  offset::UInt64=UInt64(0), column_offset::Integer=0)
+    ds = descs(td.transform, false)
+    D, L = length(td.dist), length(ds)
+    base, keep = base_desc(td.dist)
+    bd = [base]
+    bars = [vjp_slots(d, D) for d in vcat(ds, bd)]
+    ptrs = Ptr{Cvoid}[i <= length(b) && b[i] !== nothing ? Ptr{Cvoid}(UInt(pointer(b[i]))) : C_NULL for b in bars for i in 1:4]
+    nbytes = ccall((:b2b_chain_sample_vjp_workspace_bytes, libb2b), Csize_t,
+                   (Ptr{LayerDesc}, Int32, Ptr{LayerDesc}, Int32, Int64), ds, L, bd, D, n)
+    nbytes == 0 && error("B200Bijectors: rand_vjp: the device path refuses this flow and base")
+    ws = CuVector{UInt8}(undef, nbytes)
+    GC.@preserve ds bd keep bars ptrs ws ȳ q̄ check(ccall((:b2b_chain_sample_vjp_f32, libb2b), Cint,
+        (Ptr{LayerDesc}, Int32, Ptr{LayerDesc}, UInt64, UInt64, Int64, CuPtr{Float32}, Int64, CuPtr{Float32},
+         Ptr{Ptr{Cvoid}}, Int32, Int64, CuPtr{Cvoid}, Csize_t, Ptr{Cvoid}),
+        ds, L, bd, seed, offset, column_offset, ȳ === nothing ? NULLF : pointer(ȳ), ȳ === nothing ? D : stride(ȳ, 2),
+        q̄ === nothing ? NULLF : pointer(q̄), ptrs, D, n, pointer(ws), nbytes, stream_handle()))
+    return bars[1:end-1], bars[end]
+end
+
+# Structural tangents of what rand_vjp returns.  The transform: flatten() lists the leaves inner-most first, one
+# descriptor each, so a ComposedFunction takes its inner part's cotangents first.  A leaf's trainable fields are the first
+# fields of its struct in slot order (PlanarLayer w u b, RadialLayer α_ β z_0, RationalQuadraticSpline widths heights
+# derivatives, InvertibleBatchNorm b logs, Scale a), a Coupling's those of its conditioner θ, and Inverse wraps `orig`.
+function transform_tangent(f, bars, k::Base.RefValue{Int})
+    f isa ComposedFunction || return leaf_tangent(f, bars[k[] += 1])
+    inner = transform_tangent(f.inner, bars, k)
+    return ChainRulesCore.Tangent{typeof(f)}(outer=transform_tangent(f.outer, bars, k), inner=inner)
+end
+function leaf_tangent(b, bar)
+    all(t -> t === nothing, bar) && return NoTangent()
+    b isa Inverse && return ChainRulesCore.Tangent{typeof(b)}(orig=leaf_tangent(b.orig, bar))
+    b isa Coupling && return ChainRulesCore.Tangent{typeof(b)}(θ=leaf_tangent(b.θ, bar))
+    names = fieldnames(typeof(b))
+    return ChainRulesCore.Tangent{typeof(b)}(; (names[i] => bar[i] for i in eachindex(bar) if bar[i] !== nothing)...)
+end
+# The base: μ̄, and the covariance's tangent from σ̄ or L̄ (Σ = diag(σ²): Σ̄ᵢᵢ = σ̄ᵢ/(2σᵢ); Σ = L Lᵀ: Σ̄ = sym(L⁻ᵀ Φ(Lᵀ L̄) L⁻¹)/2,
+# Φ the lower triangle with its diagonal halved).
+function base_tangent(d::MvNormal, (μ̄, p̄))
+    Σ = d.Σ
+    if Σ isa PDMat
+        L = Matrix(cholesky(Σ).L)
+        P = LowerTriangular(L' * Array(p̄))
+        P[diagind(P)] ./= 2
+        S = L' \ (Matrix(P) / L)
+        Σ̄ = ChainRulesCore.Tangent{typeof(Σ)}(mat=(S + S') / 2)
+    else
+        g = Array(p̄) ./ (2 .* sqrt.(var(d)))
+        Σ̄ = Σ isa ScalMat ? ChainRulesCore.Tangent{typeof(Σ)}(value=sum(g)) : ChainRulesCore.Tangent{typeof(Σ)}(diag=g)
+    end
+    return ChainRulesCore.Tangent{typeof(d)}(μ=Array(μ̄), Σ=Σ̄)
+end
+
+# The ELBO's gradient through the sampler: the pullback of rand_logpdf is one b2b_chain_sample_vjp_f32 call with the
+# forward's seed; the tangent of td is structural in its transform and its MvNormal.
+function ChainRulesCore.rrule(::typeof(rand_logpdf), td::TransformedDistribution{<:MvNormal}, n::Integer;
+                              seed::UInt64=rand(UInt64), offset::UInt64=UInt64(0), column_offset::Integer=0)
+    y, lq = rand_logpdf(td, n; seed=seed, offset=offset, column_offset=column_offset)
+    function rand_logpdf_pullback((ȳ, q̄))
+        ȳd = ȳ isa ChainRulesCore.AbstractZero ? nothing : CuMatrix{Float32}(ȳ)
+        q̄d = q̄ isa ChainRulesCore.AbstractZero ? nothing : CuVector{Float32}(q̄)
+        flow, base = rand_vjp(td, n, ȳd, q̄d; seed=seed, offset=offset, column_offset=column_offset)
+        t̄ = ChainRulesCore.Tangent{typeof(td)}(dist=base_tangent(td.dist, base),
+                                               transform=transform_tangent(td.transform, flow, Ref(0)))
+        return NoTangent(), t̄, NoTangent()
+    end
+    return (y, lq), rand_logpdf_pullback
 end
 
 # logpdf(td::MvTransformed, y::Matrix) (src/transformed_distribution.jl:165-169): inverse chain + base

@@ -4,6 +4,7 @@
   logpdf(td, y::Matrix) = logpdf(td.dist, x) + logjac with
       (x, logjac) = with_logabsdet_jacobian(inverse(td.transform), y)          :165-169
   rand(td, n): base samples pushed through the forward chain                   :212-224
+  rand_logpdf / rand_vjp: the reparameterised sampler of variational inference   :210-213 (docs/src/advi.md)
 
 The inverse chain, the base MvNormal log-density and (optionally) the batch sum run as ONE fused chain
 launch per fusable segment: the terminal B2B_MVNORMAL_DIAG op consumes the recovered x in registers, so no
@@ -209,3 +210,100 @@ def logpdf_vjp(td: TransformedDistribution, y: torch.Tensor, lpbar: Optional[tor
     flow = _leaf_grads(descs, counts, bars)[::-1]
     T = len(descs) - 1
     return ybar, flow, _slot_grads(descs[T], T, bars)
+
+
+def _rsample_setup(td, n: int, where: str):
+    """(base MvNormal, descriptors of the forward chain, per-leaf descriptor counts, base descriptor, device) of the
+    reparameterised sampler, after the argument checks that need no device: Float32 only (TypeError otherwise)."""
+    from .interface import _leaf_descs
+
+    dist, t = (td, None) if isinstance(td, MvNormal) else (td.dist, td.transform)
+    if not isinstance(dist, MvNormal):
+        raise TypeError(f"{where}: the base must be an MvNormal, got {type(dist).__name__}")
+    if dist.dtype != torch.float32:
+        raise TypeError(f"{where}: the sampler is Float32 only (construct the base with dtype=torch.float32)")
+    if int(n) < 0:
+        raise ValueError(f"{where}: n must be >= 0")
+    descs, counts = _leaf_descs(t, dist.D, torch.float32) if t is not None else ([], [])
+    dev = dist.device if not isinstance(dist.device, str) or dist.device != "cuda" else torch.device("cuda", torch.cuda.current_device())
+    return dist, descs, counts, dist._terminal_desc(), dev
+
+
+def rand_logpdf(td, n: int, seed: Optional[int] = None, offset: int = 0, column_offset: int = 0):
+    """``(y, logq)``: the samples ``rand(td, n, seed, offset, column_offset)`` draws -- bit for bit -- and their
+    log-density log q(y) = logpdf(td, y), formed in the same pass from the base draw z and the forward log-Jacobian
+    (b2b_chain_sample_logq_f32): log q = −½‖z‖² − Σ log σᵢ (or log Lᵢᵢ) − ½·D·log2π − ℓ(x).  No inverse chain runs,
+    so it costs what ``rand(with_logjac=True)`` costs.  Float32 flows and bases only (TypeError otherwise)."""
+    import ctypes
+
+    from ._lib import check, lib
+    from .interface import _desc_array, _stream, colmajor_empty
+
+    dist, descs, _, base, dev = _rsample_setup(td, n, "rand_logpdf")
+    D, L = dist.D, len(descs)
+    arr = _desc_array(descs) if L else None
+    bdesc = _desc_array([base])
+    y = colmajor_empty(D, n, dev)
+    lq = torch.empty((n,), dtype=torch.float32, device=y.device)
+    ws_bytes = lib().b2b_chain_sample_logq_workspace_bytes(arr, L, bdesc, D, n)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=y.device) if ws_bytes else None
+    rc = lib().b2b_chain_sample_logq_f32(arr, L, bdesc, ctypes.c_uint64(_seed(seed)), ctypes.c_uint64(int(offset)),
+                                         int(column_offset), y.data_ptr(), lq.data_ptr(), D, n, D,
+                                         ws.data_ptr() if ws is not None else None, ws_bytes, _stream())
+    check(rc, "b2b_chain_sample_logq_f32")
+    return y, lq
+
+
+def _rand_vjp_raw(descs, base, D: int, n: int, dev, ybar, lqbar, seed: int, offset: int, column_offset: int, want):
+    """One b2b_chain_sample_vjp_f32 call.  ``descs`` + [``base``] index the cotangents; ``want``: (descriptor index, slot)
+    pairs.  Returns {(l, i): cotangent in the storage shape of that parameter}."""
+    import ctypes
+
+    from ._lib import check, lib
+    from .interface import _batch_view, _desc_array, _slot_shape, _stream
+
+    L = len(descs)
+    ldyb = D
+    if ybar is not None:
+        Dy, Ny, ldyb = _batch_view(ybar)
+        if (Dy, Ny) != (D, n) or not ybar.is_cuda or ybar.dtype != torch.float32:
+            raise ValueError("rand_vjp: ybar must be a Float32 device batch of the samples' shape")
+    if lqbar is not None and (lqbar.numel() != n or lqbar.dtype != torch.float32 or not lqbar.is_contiguous()):
+        raise ValueError("rand_vjp: lqbar must be a contiguous float32 vector of length n")
+    arr = _desc_array(descs) if L else None
+    bdesc = _desc_array([base])
+    full = list(descs) + [base]
+    bars = {}
+    ptrs = (ctypes.c_void_p * (4 * (L + 1)))()
+    for l, i in want:
+        t = torch.empty(_slot_shape(full[l], i, D), dtype=torch.float32, device=dev)
+        bars[(l, i)] = t
+        ptrs[4 * l + i] = t.data_ptr()
+    L_ = lib()
+    ws_bytes = L_.b2b_chain_sample_vjp_workspace_bytes(arr, L, bdesc, D, n)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
+    rc = L_.b2b_chain_sample_vjp_f32(arr, L, bdesc, ctypes.c_uint64(seed), ctypes.c_uint64(int(offset)),
+                                     int(column_offset), ybar.data_ptr() if ybar is not None else None, ldyb,
+                                     lqbar.data_ptr() if lqbar is not None else None, ptrs, D, n,
+                                     ws.data_ptr() if ws is not None else None, ws_bytes, _stream())
+    check(rc, "b2b_chain_sample_vjp_f32")
+    return bars
+
+
+def rand_vjp(td, n: int, ybar: Optional[torch.Tensor] = None, lqbar: Optional[torch.Tensor] = None,
+             seed: Optional[int] = None, offset: int = 0, column_offset: int = 0):
+    """Reverse mode of ``rand_logpdf(td, n, seed, offset, column_offset)`` with the base draw z held fixed -- the
+    reparameterisation gradient of an ELBO: one b2b_chain_sample_vjp_f32 call.  ``ybar`` (D×n) and ``lqbar`` (n) are the
+    cotangents of the samples and of log q (None = zeros); pass the ``seed`` the forward used.  Returns ``(flow_grads,
+    base_grads)`` with the shapes and leaf order of ``logpdf_vjp``: one dict per leaf of ``flatten(td.transform)`` and
+    {"μ", "σ"} (or {"μ", "L"}, L̄ lower triangular) for the base parameters that are given, summed over the n columns."""
+    from .interface import _leaf_grads, _slot_grads, _trainable_slots
+
+    if seed is None:
+        raise ValueError("rand_vjp: pass the seed the samples were drawn with")
+    dist, descs, counts, base, dev = _rsample_setup(td, n, "rand_vjp")
+    full = list(descs) + [base]
+    want = [(l, i) for l, d in enumerate(full) for i in _trainable_slots(d)]
+    bars = _rand_vjp_raw(descs, base, dist.D, int(n), dev, ybar, lqbar, _seed(seed), offset, column_offset, want)
+    T = len(descs)
+    return _leaf_grads(descs, counts, bars), _slot_grads(base, T, bars)

@@ -578,6 +578,41 @@ int b2b_chain_sample_f32(const b2b_layer_desc* layers, int32_t L, const float* m
 int b2b_chain_sample_tril_f32(const b2b_layer_desc* layers, int32_t L, const float* mu, const float* scale_tril,
                               uint64_t seed, uint64_t offset, int64_t column_offset, float* y, float* logjac, int32_t D,
                               int64_t N, int64_t ldy, void* workspace, size_t workspace_bytes, void* stream);
+/* ---- reparameterised sampling: rand(td, n) with log q, and its reverse mode (variational inference, the ELBO) ------
+ * `base` is a descriptor of kind B2B_MVNORMAL_DIAG (p0 = mu or NULL, p1 = sigma or NULL) or B2B_MVNORMAL_TRIL (p0 = mu or
+ * NULL, p1 = L, D x D column-major, lower triangle read), inverse == 0.  With z the stream of b2b_randn_f32 for (seed,
+ * offset, global column, row), x = mu + sigma .* z or mu + L z, y = T(x) through layers[0..L) in the forward direction and
+ * ℓ(x) its log|det J|, the samples' log-density is
+ *   log q(y) = −½‖z‖² − Σᵢ log sigmaᵢ (or log Lᵢᵢ) − ½·D·log2π − ℓ(x).
+ * b2b_chain_sample_logq_f32 writes y bit-identical to b2b_chain_sample_f32 / b2b_chain_sample_tril_f32 for the same
+ * arguments, and log q (N floats) to `logq`.  A chain b2b_chain_sample_f32 runs as one launch stays one launch (‖z‖² is
+ * summed while z is generated, the store is still 4·(D+1) B/sample); a two-pass chain adds one pass over the N floats of
+ * logq (the diagonal base regenerates z per column; the TRIL sample launch emits the base term itself).
+ * b2b_chain_sample_vjp_f32 is its reverse mode with z held fixed (the reparameterisation gradient): `ybar` (D x N,
+ * leading dimension ldybar) and `lqbar` (N) are the cotangents of y and log q, NULL = zeros.  `param_bars` is NULL or
+ * 4·(L+1) pointers: entries 0 .. 4L−1 as in b2b_chain_vjp_f32 (same slots, layouts and rules), entries 4L .. 4L+3 the base's:
+ * μ̄ and σ̄ (DIAG; a request whose parameter is NULL returns B2B_EINVAL) or μ̄ (B2B_EINVAL when p0 is NULL) and L̄ (D x D
+ * column-major, exactly zero above the diagonal); slots 4L+2, 4L+3 return B2B_EUNSUPPORTED.
+ *   x̄ = b2b_chain_vjp_f32 at x with ybar and l̄ = −lqbar,   μ̄ = Σₙ x̄ₙ,
+ *   σ̄ = Σₙ x̄ₙ ⊙ zₙ − (Σₙ q̄ₙ)/σ,   L̄ = tril(Σₙ x̄ₙ zₙᵀ) − (Σₙ q̄ₙ)·diag(1/Lᵢᵢ).
+ * x (and for TRIL z) is regenerated into the workspace; every cotangent is summed over this call's N columns in a fixed
+ * order (deterministic, no atomics): column shards pass their first global column as column_offset and all-reduce the
+ * cotangents like any other.  N == 0 zeroes the requested cotangents.
+ * Refusals, before anything is launched: a chain b2b_chain_vjp_f32 refuses (its status), a chain holding an MvNormal
+ * terminal or a base of another kind (B2B_EINVAL), a TRIL base with D > 256 (B2B_EUNSUPPORTED).  Float32 only.
+ * Launch-only on `stream`, no allocation (CUDA-graph capturable); both set b2b_last_launch_count.  The workspace queries
+ * return 0 exactly when their call refuses the input, and depend on nothing else. */
+size_t b2b_chain_sample_logq_workspace_bytes(const b2b_layer_desc* layers, int32_t L, const b2b_layer_desc* base,
+                                             int32_t D, int64_t N);
+int b2b_chain_sample_logq_f32(const b2b_layer_desc* layers, int32_t L, const b2b_layer_desc* base, uint64_t seed,
+                              uint64_t offset, int64_t column_offset, float* y, float* logq, int32_t D, int64_t N,
+                              int64_t ldy, void* workspace, size_t workspace_bytes, void* stream);
+size_t b2b_chain_sample_vjp_workspace_bytes(const b2b_layer_desc* layers, int32_t L, const b2b_layer_desc* base,
+                                            int32_t D, int64_t N);
+int b2b_chain_sample_vjp_f32(const b2b_layer_desc* layers, int32_t L, const b2b_layer_desc* base, uint64_t seed,
+                             uint64_t offset, int64_t column_offset, const float* ybar, int64_t ldybar,
+                             const float* lqbar, float* const* param_bars, int32_t D, int64_t N, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 /* ---- host-buffer entry point (what a caller holding plain host Arrays uses; the bench's `e2e`) ----
  * Streams the batch through the device in column chunks: H2D copy, chain kernels and D2H copy of
