@@ -1,19 +1,17 @@
-// Neural-network coupling layer, B2B_COUPLING_MLP (include/b2b.h): Coupling(θ, mask) (coupling.jl:206-228) with the
-// affine law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) whose parameters come from a one-hidden-layer network,
-//   [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂,   σ = tanh or LeakyReLU(a),
+// Neural-network coupling layers, B2B_COUPLING_MLP and B2B_COUPLING_DEEP_MLP (include/b2b.h): Coupling(θ, mask)
+// (coupling.jl:206-228) with the affine law θ(x₂) = Shift(t) ∘ Scale(exp.(s)) whose parameters come from a network of
+// M hidden layers (M = 1 for B2B_COUPLING_MLP),
+//   h_0 = x₂,   h_l = σ.(W_l·h_{l−1} + c_l) (W_1 = W_in),   [s; t] = W_out·h_M + c_out,   σ = tanh or LeakyReLU(a),
 // forward and inverse, in exact fp32 on the CUDA cores.
 //
 // Mapping.  A CTA owns a tile of 64 columns and stages the n1 + n2 rows it reads, [row][column] with pitch 65, as
 // coupling_affine_rows_kernel does (pass-through rows go global to global and are skipped in place).  Phase 1 forms
-// h = σ(W₁·x₂ + c₁) into a third shared-memory block [H][65] with coupling_gemm_block, eight hidden rows per warp and
-// step.  Phase 2 is coupling_tile of the affine kernel with X2 = h, n2 = H, W = W₂, cvec = c₂: the same GEMM, exp / FMA
-// epilogue and per-warp Σ s.  Every output is a fixed-order fmaf chain over k, then over the hidden units, so it does not
-// depend on N, the tile or the grid.
-//
-// The deep network of B2B_COUPLING_DEEP_MLP (DEEP = true) runs phase 1 M times, h_l = σ(W_l·h_{l−1} + c_l) with
-// h_0 = x₂ and W_1 = W_in; phase 2 runs on h_M with W_out and c_out.  Odd layers go to the h block, even layers to the
-// x₂ block (max(n2, H) rows), whose x₂ was stored to y₂ when it was loaded: at n1 = n2 = H = 128 the kernel then needs
-// the shared memory of the one-hidden-layer kernel, and two CTAs still fit an SM.
+// h_1 .. h_M with cmlp_hidden (coupling_gemm_block, eight hidden rows per warp and step): odd layers go to a third
+// shared-memory block [H][65], even layers back to the x₂ block, which holds max(n2, H) rows when M >= 2 (x₂ has then
+// been stored to y₂ as it was loaded).  At n1 = n2 = H = 128 any depth then needs the shared memory of M = 1, and two
+// CTAs still fit an SM.  Phase 2 is coupling_tile of the affine kernel with X2 = h_M, n2 = H, W = W_out, cvec = c_out: the same
+// GEMM, exp / FMA epilogue and per-warp Σ s.  Every output is a fixed-order fmaf chain over k, then over the hidden
+// units, so it does not depend on N, the tile or the grid.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -26,13 +24,13 @@ struct CmlpParams {
   const float* x;
   float* y;
   float* logjac;
-  const float *W1, *c1, *W2, *c2;
+  const float *W1, *c1, *W2, *c2;  // W_in, [c_1 | … | c_M] (or NULL), W_out, c_out
   const int *idx1, *idx2;
   long long N, ldx, ldy;
   int D, n1, n2, H, act, accumulate;
   float slope;
-  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
-  int depth;        // DEEP: M hidden layers
+  const float* Wh;  // W_2 .. W_M, each H x H column-major, back to back
+  int depth;        // M hidden layers
 };
 
 // dst = σ(W·src + c) for one tile: W is H x nk column-major, src [nk][CP_LD], dst [H][CP_LD], c NULL = 0.  Eight
@@ -59,14 +57,14 @@ __device__ __forceinline__ void cmlp_hidden(const float* src, int nk, const floa
   }
 }
 
-template <bool INV, bool DEEP>
+template <bool INV>
 __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __grid_constant__ CmlpParams P) {
   // x and y may alias (in place): every element is read before it is written, by the same CTA
   extern __shared__ float smem[];
   const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H;
-  float* X2 = smem;                                      // [n2][CP_LD]  x₂ (DEEP: max(n2, H) rows, h_l of even l)
-  float* X1 = X2 + (size_t)(DEEP ? max(n2, H) : n2) * CP_LD;  // [n1][CP_LD]  x₁, transformed in place
-  float* Hs = X1 + (size_t)n1 * CP_LD;                   // [H][CP_LD]   hidden layer h (DEEP: h_l of odd l)
+  float* X2 = smem;                                      // [n2][CP_LD]  x₂ (M >= 2: max(n2, H) rows, h_l of even l)
+  float* X1 = X2 + (size_t)(P.depth > 1 ? max(n2, H) : n2) * CP_LD;  // [n1][CP_LD]  x₁, transformed in place
+  float* Hs = X1 + (size_t)n1 * CP_LD;                   // [H][CP_LD]   h_l of odd l
   float* red = Hs + (size_t)H * CP_LD;                   // [8][CP_TC]
   int* sidx2 = reinterpret_cast<int*>(red + 8 * CP_TC);  // [n2]
   int* sidx1 = sidx2 + n2;                               // [n1]
@@ -75,6 +73,9 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
   const float* x = P.x;
   float* y = P.y;
   const bool copy_through = y && y != x;  // in place, x₂ and x₃ stay where they are
+  // y₂ = x₂ goes out with y₁ at M = 1 (measured faster at H = 128), and as x₂ is loaded at M >= 2, where the x₂ block
+  // will hold h_2
+  const bool y2_early = copy_through && P.depth > 1, y2_late = copy_through && P.depth == 1;
   const bool has_x3 = n1 + n2 < D;
   const int nwords = (D + 31) >> 5;
   if (has_x3 && copy_through)
@@ -88,7 +89,7 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
   }
   const bool vec1 = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
   const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
-  const bool vech = DEEP && ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
+  const bool vech = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
   const long long tiles = (P.N + CP_TC - 1) / CP_TC;
   auto same = [](int k) { return k; };
 
@@ -101,10 +102,8 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
       if (col < P.N) {
         const float* xc = x + col * P.ldx;
         for (int k = lane; k < n2; k += 32) X2[k * CP_LD + c] = __ldcs(xc + sidx2[k]);
-        if constexpr (DEEP) {  // the x₂ block will hold h_2 and h_4: y₂ = x₂ goes out now
-          if (copy_through)
-            for (int k = lane; k < n2; k += 32) __stcs(y + col * P.ldy + sidx2[k], X2[k * CP_LD + c]);
-        }
+        if (y2_early)
+          for (int k = lane; k < n2; k += 32) __stcs(y + col * P.ldy + sidx2[k], X2[k * CP_LD + c]);
         if (y)  // the log-Jacobian needs x₂ only
           for (int k = lane; k < n1; k += 32) X1[k * CP_LD + c] = __ldcs(xc + sidx1[k]);
         if (has_x3 && copy_through) {
@@ -118,44 +117,29 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
       }
     }
     __syncthreads();
-    // ---- phase 1: h = σ(W₁·x₂ + c₁) ---------------------------------------------------------------------------
-    for (int jb = 8 * warp; jb < H; jb += 8 * (CP_THREADS / 32)) {
-      float va[4][2] = {}, vb[4][2] = {};
-      coupling_gemm_block<2>(X2, CP_LD, same, n2, P.W1 + jb, P.W1 + jb + 4, H, H - jb, H - jb - 4, vec1, va, vb);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int m = jb + q;
-        if (m < H) {
-          const float c = P.c1 ? __ldg(P.c1 + m) : 0.f;
-          float dh;
-#pragma unroll
-          for (int u = 0; u < 2; ++u)
-            mlp_act(P.act, P.slope, (q < 4 ? va[q & 3][u] : vb[q & 3][u]) + c, Hs[m * CP_LD + lane + 32 * u], dh);
-        }
-      }
+    // ---- phase 1: h_l = σ(W_l·h_{l−1} + c_l), l = 1..M ----------------------------------------------------------
+    const float* hM = X2;  // h_{l−1}, read with W (nk columns)
+    const float* W = P.W1;
+    int nk = n2;
+    for (int l = 1; l <= P.depth; ++l) {
+      float* dst = (l & 1) ? Hs : X2;
+      cmlp_hidden(hM, nk, W, P.c1 ? P.c1 + (size_t)(l - 1) * H : nullptr, l == 1 ? vec1 : vech, H, P.act, P.slope, dst);
+      __syncthreads();
+      hM = dst;
+      W = P.Wh + (size_t)(l - 1) * H * H;
+      nk = H;
     }
-    __syncthreads();
-    const float* hM = Hs;
-    if constexpr (DEEP) {  // h_l = σ(W_l·h_{l−1} + c_l), l = 2..M
-      for (int l = 2; l <= P.depth; ++l) {
-        float* dst = (l & 1) ? Hs : X2;
-        cmlp_hidden(hM, H, P.Wh + (size_t)(l - 2) * H * H, P.c1 ? P.c1 + (size_t)(l - 1) * H : nullptr, vech, H,
-                    P.act, P.slope, dst);
-        __syncthreads();
-        hM = dst;
-      }
-    }
-    // ---- phase 2: [s; t] = W₂·h + c₂ and the affine law on x₁ ----------------------------------------------------
+    // ---- phase 2: [s; t] = W_out·h_M + c_out and the affine law on x₁ --------------------------------------------
     coupling_tile<INV>(hM, X1, same, same, P.W2, P.c2, n1, H, vec2, red);
     __syncthreads();
-    // ---- write back x₁ (and x₂ unless it is already in place) ------------------------------------------------------
+    // ---- write back x₁ (and x₂ at M = 1) ---------------------------------------------------------------------------
     if (y) {
       for (int c = warp; c < CP_TC; c += CP_THREADS / 32) {
         const long long col = col0 + c;
         if (col < P.N) {
           float* yc = y + col * P.ldy;
           for (int k = lane; k < n1; k += 32) __stcs(yc + sidx1[k], X1[k * CP_LD + c]);
-          if (!DEEP && copy_through)
+          if (y2_late)
             for (int k = lane; k < n2; k += 32) __stcs(yc + sidx2[k], X2[k * CP_LD + c]);
         }
       }
@@ -173,7 +157,7 @@ __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __gri
   }
 }
 
-// x₂ (DEEP: max(n2, H) rows), x₁ and h tiles, the column-sum slab, both index tables and the coupled-row bitmap
+// x₂ (M >= 2: max(n2, H) rows), x₁ and h tiles, the column-sum slab, both index tables and the coupled-row bitmap
 static size_t cmlp_smem_bytes(int n1, int n2, int H, int D, bool deep) {
   const int r2 = deep && H > n2 ? H : n2;
   return ((size_t)(n1 + r2 + H) * CP_LD + 8 * CP_TC) * sizeof(float) + (size_t)(n1 + n2) * sizeof(int) +
@@ -188,7 +172,6 @@ int b2b_fwd_mlp(const B2BFwdSeg& s) {
   const int D = s.D;
   if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
   const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
-  const bool deep = c.M > 1;
   CmlpParams P;
   P.x = s.x;
   P.y = s.y;
@@ -211,9 +194,8 @@ int b2b_fwd_mlp(const B2BFwdSeg& s) {
   P.accumulate = s.accumulate;
   P.slope = c.slope;
   P.depth = c.M;
-  const size_t smem = cmlp_smem_bytes(c.n1, c.n2, c.H, D, deep);
-  void (*kernel)(const CmlpParams) = deep ? (d.inverse ? coupling_mlp_kernel<true, true> : coupling_mlp_kernel<false, true>)
-                                          : (d.inverse ? coupling_mlp_kernel<true, false> : coupling_mlp_kernel<false, false>);
+  const size_t smem = cmlp_smem_bytes(c.n1, c.n2, c.H, D, c.M > 1);
+  void (*kernel)(const CmlpParams) = d.inverse ? coupling_mlp_kernel<true> : coupling_mlp_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   const int sms = b2b_sm_count();

@@ -1,24 +1,20 @@
-// Reverse mode of the neural-network coupling layer, B2B_COUPLING_MLP, either direction: cotangents of the input and of
-// W₁, c₁, W₂, c₂ -- what the reference's reverse-mode AD computes through coupling.jl:206-228 with the law
-// Shift(t) ∘ Scale(exp.(s)), [s; t] = W₂·σ.(W₁·x₂ + c₁) + c₂.  With v = W₁x₂ + c₁, h = σ(v) and the affine law's
-// s̄, t̄, x̄₁ (formed as b2b_coupling_vjp.cu forms them):
-//   h̄ = W₂ᵀ[s̄; t̄]     v̄ = h̄ ⊙ σ′(v)     x̄₂ = ȳ₂ + W₁ᵀ v̄     x̄₃ = ȳ₃
-//   W̄₂ = Σₙ [s̄; t̄] hᵀ   c̄₂ = Σₙ [s̄; t̄]    W̄₁ = Σₙ v̄ x₂ᵀ       c̄₁ = Σₙ v̄
+// Reverse mode of the neural-network coupling layers, B2B_COUPLING_MLP and B2B_COUPLING_DEEP_MLP, either direction:
+// cotangents of the input and of every weight and bias -- what the reference's reverse-mode AD computes through
+// coupling.jl:206-228 with the law Shift(t) ∘ Scale(exp.(s)) and the network of b2b_coupling_mlp.cu, M hidden layers
+// (M = 1 for B2B_COUPLING_MLP), h_0 = x₂, W_1 = W_in.  With h_l = σ(v_l) and the affine law's s̄, t̄, x̄₁ (formed as
+// b2b_coupling_vjp.cu forms them):
+//   v̄_M = (W_outᵀ[s̄; t̄]) ⊙ σ′_M     v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}     x̄₂ = ȳ₂ + W_inᵀ v̄_1     x̄₃ = ȳ₃
+//   W̄_out = Σₙ [s̄; t̄] h_Mᵀ   c̄_out = Σₙ [s̄; t̄]   W̄_l = Σₙ v̄_l h_{l−1}ᵀ   c̄_l = Σₙ v̄_l
 //
 // Mapping.  A fixed grid of at most one CTA per SM walks groups of 32·S columns round-robin (S = 4, 2 or 1 sub-tiles,
-// the most whose factors fit shared memory: S = 2 at n1 = n2 = 128, H = 256).  Each sub-tile of 32 columns (one per
-// lane) runs the network forward and backward with coupling_gemm_block and its transposed counterpart, leaving the four
-// factors x₂, [s̄; t̄], h and v̄ of its columns in shared memory.  After the group's last sub-tile the CTA forms the
-// four parameter sums of the whole group, a 4 x 4 register block per thread swept over the matrices, and adds them to
-// its private slice of the workspace ([W̄₁ | c̄₁ | W̄₂ | c̄₂], every element always by the same thread): one
-// read-modify-write of the slice per 32·S columns.  A second kernel sums the slices in order, in fp64, into the caller's
-// arrays.  Deterministic, no atomics; the workspace depends on the grid, not on N.
-//
-// The deep network of B2B_COUPLING_DEEP_MLP (DEEP = true, M hidden layers, h_0 = x₂, W_1 = W_in) keeps h_l and σ′_l of
-// every layer of the group in shared memory and runs back through them:
-//   v̄_M = (W_outᵀ[s̄; t̄]) ⊙ σ′_M     v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}     x̄₂ = ȳ₂ + W_inᵀ v̄_1
-//   W̄_out = Σₙ [s̄; t̄] h_Mᵀ   W̄_l = Σₙ v̄_l h_{l−1}ᵀ   c̄ = [Σₙ v̄_1 | … | Σₙ v̄_M | Σₙ [s̄; t̄]]
-// with the slice laid out [W̄_in | W̄_hid | W̄_out | c̄], the order of the descriptor's p0 .. p3.
+// the most whose factors fit shared memory: S = 2 at n1 = n2 = 128, H = 256, M = 1).  Each sub-tile of 32 columns (one
+// per lane) runs the network forward and backward with coupling_gemm_block and its transposed counterpart, leaving x₂,
+// [s̄; t̄] and h_l, v̄_l of every layer of its columns in shared memory.  After the group's last sub-tile the CTA forms the
+// parameter sums of the whole group, a 4 x 4 register block per thread swept over the matrices, and adds them to its
+// private slice of the workspace (the descriptor's four slots back to back, each role at the offset the host gives it;
+// every element always by the same thread): one read-modify-write of the slice per 32·S columns.  A second kernel sums
+// the slices in order, in fp64, into the caller's arrays.  Deterministic, no atomics; the workspace depends on the
+// grid, not on N.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -35,14 +31,15 @@ struct CmvParams {
   const float* ybar;
   const float* ljbar;
   float* xbar;
-  const float *W1, *c1, *W2, *c2;
+  const float *W1, *c1, *W2, *c2;  // W_in, [c_1 | … | c_M] (or NULL), W_out, c_out
   const int *idx1, *idx2;
   float* part;  // [grid][slice], NULL: no parameter cotangents
   long long N, ldx, ldyb, ldxb, slice;
+  long long soff[B2B_NROLES];  // offset of each B2BRole's sums in the slice
   int D, n1, n2, H, act, nsub;
   float slope;
-  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
-  int depth;        // DEEP: M hidden layers
+  const float* Wh;  // W_2 .. W_M, each H x H column-major, back to back
+  int depth;        // M hidden layers
 };
 
 // acc[q] += Σ_k A[q·nk + k] · B[k·ld + lane] for the `rows` (<= 8) rows at A, each contiguous in k, k increasing
@@ -141,11 +138,11 @@ __device__ __forceinline__ void cmv_back(const float* g, int ld, int ng, const f
   }
 }
 
-template <bool INV, bool DEEP>
+template <bool INV>
 __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const __grid_constant__ CmvParams P) {
   extern __shared__ float cmv_sm[];
   const int D = P.D, n1 = P.n1, n2 = P.n2, H = P.H, TG = 32 * P.nsub, FP = TG + 1, nmax = max(n1, n2);
-  const int M = DEEP ? P.depth : 1;
+  const int M = P.depth;
   const size_t HB = (size_t)H * FP;     // one hidden block
   float* X2 = cmv_sm;                   // [n2][FP]   x₂
   float* ST = X2 + (size_t)n2 * FP;     // [2n1][FP]  ȳ₁, then s̄ | t̄
@@ -158,17 +155,6 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
   unsigned char* kind = reinterpret_cast<unsigned char*>(sidx2 + n2);  // [D]: 0 = a pass-through row
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float* slice = P.part ? P.part + (size_t)blockIdx.x * P.slice : nullptr;
-  float *sW1 = slice, *sWh = nullptr, *sc1, *sW2, *sc2;
-  if constexpr (DEEP) {  // [W̄_in | W̄_hid | W̄_out | c̄_1 … c̄_M c̄_out]
-    sWh = sW1 + (size_t)H * n2;
-    sW2 = sWh + (size_t)(M - 1) * H * H;
-    sc1 = sW2 + (size_t)2 * n1 * H;
-    sc2 = sc1 + (size_t)M * H;
-  } else {  // [W̄₁ | c̄₁ | W̄₂ | c̄₂]
-    sc1 = sW1 + (size_t)H * n2;
-    sW2 = sc1 + H;
-    sc2 = sW2 + (size_t)2 * n1 * H;
-  }
 
   for (int r = tid; r < D; r += CMV_THREADS) kind[r] = 0;
   if (slice)
@@ -180,8 +166,8 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
   const bool vec2 = ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
   const bool vec1t = ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.W1) & 15) == 0);
   const bool vec2t = ((n1 & 1) == 0) && ((reinterpret_cast<uintptr_t>(P.W2) & 15) == 0);
-  const bool vech = DEEP && ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
-  const bool vecht = DEEP && ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
+  const bool vech = ((H & 7) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
+  const bool vecht = ((H & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.Wh) & 15) == 0);
   auto same = [](int k) { return k; };
 
   const long long groups = (P.N + TG - 1) / TG;
@@ -206,27 +192,14 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
             if (!kind[r]) __stcs(P.xbar + col * P.ldxb + r, yb ? __ldcs(yb + r) : 0.f);
       }
       __syncthreads();
-      // ---- h = σ(W₁x₂ + c₁) and σ′ -------------------------------------------------------------------------------
-      for (int jb = 8 * warp; jb < H; jb += 8 * (CMV_THREADS / 32)) {
-        float va[4][1] = {}, vb[4][1] = {};
-        coupling_gemm_block<1>(X2 + co, FP, same, n2, P.W1 + jb, P.W1 + jb + 4, H, H - jb, H - jb - 4, vec1, va, vb);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int m = jb + q;
-          if (m < H)
-            mlp_act(P.act, P.slope, (q < 4 ? va[q & 3][0] : vb[q & 3][0]) + (P.c1 ? __ldg(P.c1 + m) : 0.f),
-                    Hs[m * FP + co + lane], Vb[m * FP + co + lane]);
-        }
+      // ---- h_l = σ(W_l h_{l−1} + c_l) and σ′_l, l = 1..M ---------------------------------------------------------
+      for (int l = 1; l <= M; ++l) {
+        cmv_hidden(l == 1 ? X2 + co : Hs + (l - 2) * HB + co, FP, l == 1 ? n2 : H,
+                   l == 1 ? P.W1 : P.Wh + (size_t)(l - 2) * H * H, P.c1 ? P.c1 + (size_t)(l - 1) * H : nullptr,
+                   l == 1 ? vec1 : vech, H, P.act, P.slope, Hs + (l - 1) * HB + co, Vb + (l - 1) * HB + co);
+        __syncthreads();
       }
-      __syncthreads();
-      if constexpr (DEEP) {  // h_l = σ(W_l h_{l−1} + c_l), l = 2..M
-        for (int l = 1; l < M; ++l) {
-          cmv_hidden(Hs + (l - 1) * HB + co, FP, H, P.Wh + (size_t)(l - 1) * H * H, P.c1 ? P.c1 + (size_t)l * H : nullptr,
-                     vech, H, P.act, P.slope, Hs + l * HB + co, Vb + l * HB + co);
-          __syncthreads();
-        }
-      }
-      // ---- [s; t] = W₂h + c₂, then x̄₁, s̄, t̄ of the affine law ---------------------------------------------------
+      // ---- [s; t] = W_out h_M + c_out, then x̄₁, s̄, t̄ of the affine law --------------------------------------------
       const long long mycol = n0 + co + lane;
       const float lb = P.ljbar && mycol < P.N ? P.ljbar[mycol] : 0.f;
       for (int jb = 4 * warp; jb < n1; jb += 4 * (CMV_THREADS / 32)) {
@@ -263,23 +236,14 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
         if (col < P.N)
           for (int k = lane; k < n1; k += 32) __stcs(P.xbar + col * P.ldxb + sidx1[k], Sc[k * CMV_SP + c]);
       }
-      // ---- v̄ = (W₂ᵀ[s̄; t̄]) ⊙ σ′ ---------------------------------------------------------------------------------
-      float* VbM = Vb + (M - 1) * HB;  // v̄_M
-      for (int mb = 8 * warp; mb < H; mb += 8 * (CMV_THREADS / 32)) {
-        float acc[8] = {};
-        cmv_gemm_t(ST + co, FP, 2 * n1, P.W2 + (size_t)mb * 2 * n1, H - mb, vec2t, acc);
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          if (mb + q < H) VbM[(mb + q) * FP + co + lane] *= acc[q];
-      }
+      // ---- v̄_M = (W_outᵀ[s̄; t̄]) ⊙ σ′_M, then v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}, l = M..2 ---------------------------
+      cmv_back(ST + co, FP, 2 * n1, P.W2, vec2t, H, Vb + (M - 1) * HB + co);
       __syncthreads();
-      if constexpr (DEEP) {  // v̄_{l−1} = (W_lᵀ v̄_l) ⊙ σ′_{l−1}, l = M..2
-        for (int l = M - 1; l >= 1; --l) {
-          cmv_back(Vb + l * HB + co, FP, H, P.Wh + (size_t)(l - 1) * H * H, vecht, H, Vb + (l - 1) * HB + co);
-          __syncthreads();
-        }
+      for (int l = M - 1; l >= 1; --l) {
+        cmv_back(Vb + l * HB + co, FP, H, P.Wh + (size_t)(l - 1) * H * H, vecht, H, Vb + (l - 1) * HB + co);
+        __syncthreads();
       }
-      // ---- x̄₂ = ȳ₂ + W₁ᵀ v̄ ---------------------------------------------------------------------------------------
+      // ---- x̄₂ = ȳ₂ + W_inᵀ v̄_1 ------------------------------------------------------------------------------------
       for (int kb = 8 * warp; kb < n2; kb += 8 * (CMV_THREADS / 32)) {
         float acc[8] = {};
         cmv_gemm_t(Vb + co, FP, H, P.W1 + (size_t)kb * H, n2 - kb, vec1t, acc);
@@ -299,17 +263,18 @@ __global__ void __launch_bounds__(CMV_THREADS, 1) coupling_mlp_vjp_kernel(const 
     }
     if (slice) {  // the group's parameter sums, added to the CTA's slice
       __syncthreads();
-      cmv_outer(Vb, H, X2, n2, FP, gcols, sW1, sc1);
-      if constexpr (DEEP)
-        for (int l = 1; l < M; ++l)
-          cmv_outer(Vb + l * HB, H, Hs + (l - 1) * HB, H, FP, gcols, sWh + (size_t)(l - 1) * H * H, sc1 + (size_t)l * H);
-      cmv_outer(ST, 2 * n1, hM, H, FP, gcols, sW2, sc2);
+      float* const sc = slice + P.soff[B2B_C_IN];  // c̄_1 .. c̄_M
+      cmv_outer(Vb, H, X2, n2, FP, gcols, slice + P.soff[B2B_W_IN], sc);
+      for (int l = 1; l < M; ++l)
+        cmv_outer(Vb + l * HB, H, Hs + (l - 1) * HB, H, FP, gcols, slice + P.soff[B2B_W_HID] + (size_t)(l - 1) * H * H,
+                  sc + (size_t)l * H);
+      cmv_outer(ST, 2 * n1, hM, H, FP, gcols, slice + P.soff[B2B_W_OUT], slice + P.soff[B2B_C_OUT]);
     }
   }
 }
 
-// the `nparts` slices summed in order; element e of the slice layout ([W̄₁ | c̄₁ | W̄₂ | c̄₂], DEEP:
-// [W̄_in | W̄_hid | W̄_out | c̄]) goes to its array (NULL: dropped)
+// the `nparts` slices summed in order; element e of the slice layout (the four slots back to back, of lengths l0 .. l3)
+// goes to its array (NULL: dropped)
 __global__ void __launch_bounds__(256) coupling_mlp_vjp_reduce_kernel(const float* __restrict__ part, int nparts, long long slice,
                                                                       long long l0, long long l1, long long l2, long long l3,
                                                                       float* __restrict__ o0, float* __restrict__ o1,
@@ -372,7 +337,6 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   float* const* bars = s.bars;
   if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
   const B2BCoupling<b2b_layer_desc> c = b2b_coupling(d);
-  const bool deep = c.M > 1;
   const bool want = bars[0] || bars[1] || bars[2] || bars[3];
   if (want && (!s.workspace || s.workspace_bytes < b2b_coupling_mlp_vjp_workspace(d, D, N))) return B2B_EWORKSPACE;
   char* wsb = b2b_align256(s.workspace);
@@ -396,6 +360,12 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.ldyb = s.ldyb;
   P.ldxb = s.ldxb;
   P.slice = cmv_slice_floats(d);
+  long long l[4], so[4] = {};  // the slots' lengths and offsets in the slice
+  for (int i = 0; i < 4; ++i) {
+    l[i] = (long long)b2b_slot_len(d, i, D);
+    if (i) so[i] = so[i - 1] + l[i - 1];
+  }
+  for (int r = 0; r < B2B_NROLES; ++r) P.soff[r] = c.slot[r] < 0 ? 0 : so[c.slot[r]] + (long long)c.off[r];
   P.D = D;
   P.n1 = c.n1;
   P.n2 = c.n2;
@@ -404,17 +374,13 @@ int b2b_vjp_mlp(const B2BVjpSeg& s) {  // the four sums come from one kernel: th
   P.slope = c.slope;
   const int grid = cmv_grid(d, D, N);
   const size_t smem = cmv_smem_bytes(d, D, P.nsub);
-  void (*kernel)(const CmvParams) = deep ? (d.inverse ? coupling_mlp_vjp_kernel<true, true> : coupling_mlp_vjp_kernel<false, true>)
-                                         : (d.inverse ? coupling_mlp_vjp_kernel<true, false> : coupling_mlp_vjp_kernel<false, false>);
+  void (*kernel)(const CmvParams) = d.inverse ? coupling_mlp_vjp_kernel<true> : coupling_mlp_vjp_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CMV_THREADS, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   ++*s.launches;
   if (want) {
-    // the slice holds the four slots in the order of p0 .. p3
-    long long l[4];
-    for (int i = 0; i < 4; ++i) l[i] = (long long)b2b_slot_len(d, i, D);
     float* o[4] = {bars[0], bars[1], bars[2], bars[3]};
     coupling_mlp_vjp_reduce_kernel<<<(unsigned)((l[0] + l[1] + l[2] + l[3] + 255) / 256), 256, 0, s.stream>>>(
         P.part, grid, P.slice, l[0], l[1], l[2], l[3], o[0], o[1], o[2], o[3]);

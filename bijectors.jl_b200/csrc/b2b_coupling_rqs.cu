@@ -10,16 +10,14 @@
 // function the fused RQS programs use.  The log-Jacobian is summed over the rows in increasing order by the column's
 // thread, so it is deterministic.  x₂ and x₃ rows are copied bit-exactly (nothing is copied in place).
 //
-// The neural spline coupling, B2B_COUPLING_MLP_RQS, is the instantiation MLP = true: v = W₂·σ.(W₁·x₂ + c₁) + c₂.  The
-// tile's x₂ is staged where the rqs_element table and W's row block will be (neither is written before the row loop),
-// spilling past them only when they are smaller than x₂ (small K); each thread forms h = σ(W₁·x₂ + c₁) of its own column
-// into the [H][XP] block the row loop reads, and the row loop runs unchanged with (x₂, n2, W, c) := (h, H, W₂, c₂).
-//
-// The deep neural spline coupling, B2B_COUPLING_DEEP_MLP_RQS, is the instantiation DEEP = true (with MLP = true): M
-// hidden layers h_l = σ(W_l·h_{l−1} + c_l) before the row loop, which runs unchanged on (h_M, H, W_out, c_out).  Each
-// thread forms the layers of its own column, alternating between the [H][XP] h block and the table region (both sized
-// for max(n2, H) rows, so the shared memory is kind 14's with n2 := max(n2, H)).  x₂ is staged in the h block when M is
-// even and in the table region when M is odd, so that h_M lands in the h block; layer 1 is kind 14's hidden layer.
+// The neural spline couplings, B2B_COUPLING_MLP_RQS and B2B_COUPLING_DEEP_MLP_RQS, are the instantiation NET = true:
+// v = W_out·h_M + c_out with M hidden layers h_l = σ(W_l·h_{l−1} + c_l), h_0 = x₂, W_1 = W_in (M = 1 for
+// B2B_COUPLING_MLP_RQS).  Each thread forms the layers of its own column before the row loop, which runs unchanged
+// with (x₂, n2, W, c) := (h_M, H, W_out, c_out).  The layers alternate between the [H][XP] h block the row loop reads
+// and the table region, where the rqs_element table and W's row block will be (neither is written before the row loop;
+// x₂ spills past them only when they are smaller than x₂, at small K).  x₂ is staged in the table region when M is odd
+// and in the h block when M is even, so that h_M lands in the h block.  For M >= 2 both blocks hold max(n2, H) rows,
+// so the shared memory is that of M = 1 with n2 := max(n2, H).
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -35,16 +33,16 @@ struct CrqParams {
   const float* x;
   float* y;
   float* logjac;
-  const float *W, *c;  // MLP: W₂, c₂
+  const float *W, *c;  // NET: W_out, c_out
   const int *idx1, *idx2;
   long long N, ldx, ldy;
   int D, n1, n2, K, accumulate;
   float B;
-  const float *W1, *c1;  // MLP only (DEEP: c1 = [c_1 | … | c_M], or NULL)
+  const float *W1, *c1;  // NET only: W_in, [c_1 | … | c_M] (or NULL)
   int H, act;
   float slope;
-  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
-  int M;            // DEEP: hidden layers
+  const float* Wh;  // NET: W_2 .. W_M, each H x H column-major, back to back
+  int M;            // NET: hidden layers
 };
 
 // floats of the per-thread rqs_element table: Sw[KP] | Sh[KP] | 2 float4 per bin
@@ -57,19 +55,20 @@ static __host__ __device__ inline int crq_xs_off(int nc, int K, int n2x) {
   return off > n2x * (CRQ_TN + 1) ? off : n2x * (CRQ_TN + 1);
 }
 
-template <bool INV, bool MLP, bool DEEP>
+template <bool INV, bool NET>
 __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_constant__ CrqParams P) {
   extern __shared__ __align__(16) float crq_sm[];
   constexpr int TN = CRQ_TN, XP = CRQ_TN + 1;
   // nc: rows of the conditioning block the row loop reads (x₂, or the hidden layer h)
-  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = MLP ? P.H : n2, K = P.K, K1 = K + 1, KP = rqs_kp(K1);
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = NET ? P.H : n2, K = P.K, K1 = K + 1, KP = rqs_kp(K1);
   const int J = 3 * K - 1, JP = crq_jp(K), D = P.D;
   float* tab = crq_sm;                              // rqs_element table, one row per thread (Dp = TN)
   float* Ws = tab + crq_tab_floats(K) * TN;         // [nc][JP]
   float* cs = Ws + nc * JP;                         // [JP]
-  const int nxs = DEEP ? max(n2, nc) : nc;         // rows of the Xs block (DEEP: h_l and x₂ alternate there)
-  float* Xs = MLP ? crq_sm + crq_xs_off(nc, K, DEEP ? nxs : n2) : cs + JP;  // [nc][XP]
-  float* X2 = MLP && !(DEEP && P.M % 2 == 0) ? crq_sm : Xs;  // [n2][XP] x₂
+  const bool deep = NET && P.M > 1;                // h_l and x₂ alternate between Xs and the table region
+  const int nxs = deep ? max(n2, nc) : nc;          // rows of the Xs block
+  float* Xs = NET ? crq_sm + crq_xs_off(nc, K, deep ? nxs : n2) : cs + JP;  // [nc][XP]
+  float* X2 = NET && P.M % 2 == 1 ? crq_sm : Xs;   // [n2][XP] x₂
   float* Pr = Xs + nxs * XP;                        // [J][TN] raw parameters
   unsigned char* x1row = reinterpret_cast<unsigned char*>(Pr + J * TN);  // [D]: 1 = a transformed row
   const long long n0 = (long long)blockIdx.x * TN, n = n0 + tid;
@@ -84,7 +83,7 @@ __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_const
     X2[m * XP + c] = c < cols ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
   }
   __syncthreads();
-  if (DEEP) {  // h_1 .. h_M of this thread's column, alternating between the two blocks and ending in Xs
+  if (NET) {  // h_1 .. h_M of this thread's column, alternating between the two blocks and ending in Xs
     const int H = P.H;
     float* in = X2;
     for (int l = 1; l <= P.M; ++l) {
@@ -96,11 +95,6 @@ __global__ void __launch_bounds__(CRQ_TN) coupling_rqs_kernel(const __grid_const
         mlp_act(P.act, P.slope, crq_hidden_pre(W, c, H, l == 1 ? n2 : H, in + tid, XP, m), out[m * XP + tid], dh);
       }
       in = out;
-    }
-  } else if (MLP) {  // h = σ(W₁·x₂ + c₁) of this thread's column
-    for (int m = 0; m < P.H; ++m) {
-      float dh;
-      mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, P.H, n2, X2 + tid, XP, m), Xs[m * XP + tid], dh);
     }
   }
   if (P.y && (P.y != P.x || P.ldy != P.ldx))  // x₂ and x₃ pass through
@@ -183,15 +177,12 @@ int b2b_fwd_spline(const B2BFwdSeg& s) {
   P.slope = c.slope;
   P.Wh = c.W_hid;
   P.M = c.M;
-  const bool deep = c.M > 1;
-  const int nd = deep ? (c.n2 > c.H ? c.n2 : c.H) : 0;  // DEEP: max(n2, H)
-  const size_t smem = deep    ? crq_smem_bytes(c.H, c.K, s.D, nd, nd)
+  const int nd = c.n2 > c.H ? c.n2 : c.H;  // M >= 2: max(n2, H)
+  const size_t smem = c.M > 1 ? crq_smem_bytes(c.H, c.K, s.D, nd, nd)
                       : c.net ? crq_smem_bytes(c.H, c.K, s.D, c.n2, c.H)
                               : crq_smem_bytes(c.n2, c.K, s.D, 0, c.n2);
-  void (*kernel)(const CrqParams) =
-      deep    ? (d.inverse ? coupling_rqs_kernel<true, true, true> : coupling_rqs_kernel<false, true, true>)
-      : c.net ? (d.inverse ? coupling_rqs_kernel<true, true, false> : coupling_rqs_kernel<false, true, false>)
-              : (d.inverse ? coupling_rqs_kernel<true, false, false> : coupling_rqs_kernel<false, false, false>);
+  void (*kernel)(const CrqParams) = c.net ? (d.inverse ? coupling_rqs_kernel<true, true> : coupling_rqs_kernel<false, true>)
+                                          : (d.inverse ? coupling_rqs_kernel<true, false> : coupling_rqs_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   const long long tiles = (s.N + CRQ_TN - 1) / CRQ_TN;

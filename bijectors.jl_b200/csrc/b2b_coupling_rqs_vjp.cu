@@ -15,19 +15,17 @@
 // workspace ([n1][3K − 1][n2] then [n1][3K − 1] for c̄), owned element by element by one thread.  A second kernel sums
 // the G slices in order into W̄ (column-major like W) and c̄.  Deterministic, no atomics, workspace independent of N.
 //
-// The neural spline coupling, B2B_COUPLING_MLP_RQS, is the instantiation MLP = true.  Each thread forms h = σ(W₁·x₂ + c₁)
-// of its column from a staged x₂ tile, and the row loop runs on h with W₂ and c₂, so its fp64 accumulator holds h̄.
-// After the loop each thread recomputes W₁x₂ + c₁ for σ′, turns h̄ into v̄ = h̄ ⊙ σ′ and forms x̄₂ = ȳ₂ + W₁ᵀv̄ in a fixed
-// order; the CTA adds Σ v̄ x₂ᵀ and Σ v̄ to its slice, laid out [W̄₂ | c̄₂ | W̄₁ ([H][n2]) | c̄₁ ([H])].
-//
-// The deep neural spline coupling, B2B_COUPLING_DEEP_MLP_RQS, is the instantiation DEEP = true (with MLP = true).  Each
-// thread forms h_1 .. h_M of its column before the row loop, alternating between Xs and one more [H][XP] block E.  After
-// the loop the fp64 accumulator holds h̄_M, and the kernel walks back l = M .. 2: each thread recomputes h_{l−1} of its
-// column from x₂ (again through Xs and E: the hidden layers cost (M − 1)·H² FMAs per column against (3K − 1)·n1·H for
-// the row loop, so recomputing them is cheap and keeps the workspace independent of N), forms v̄_l = h̄_l ⊙ σ′_l in the
-// other block and h̄_{l−1} = W_lᵀv̄_l into the accumulator, and the CTA adds Σ v̄_l h_{l−1}ᵀ and Σ v̄_l to its slice.
-// Layer 1 is kind 14's hidden layer above.  The slice appends [W̄_2 … W̄_M ([H][H] each) | c̄_2 … c̄_M ([H] each)] to kind
-// 14's layout, and coupling_rqs_deep_vjp_reduce_kernel sums the slices into the layouts of p0 .. p3.
+// The neural spline couplings, B2B_COUPLING_MLP_RQS and B2B_COUPLING_DEEP_MLP_RQS, are the instantiation NET = true,
+// with the network of b2b_coupling_rqs.cu (M hidden layers, M = 1 for B2B_COUPLING_MLP_RQS).  Each thread forms
+// h_1 .. h_M of its column from a staged x₂ tile before the row loop, alternating between Xs and one more [H][XP] block
+// E so that h_M lands in Xs, and the row loop runs on h_M with W_out and c_out, so its fp64 accumulator holds h̄_M.  The
+// kernel then walks back l = M .. 2: each thread recomputes h_{l−1} of its column from x₂ (again through Xs and E: the
+// hidden layers cost (M − 1)·H² FMAs per column against (3K − 1)·n1·H for the row loop, so recomputing them is cheap and
+// keeps the workspace independent of N), forms v̄_l = h̄_l ⊙ σ′_l in the other block and h̄_{l−1} = W_lᵀv̄_l into the
+// accumulator, and the CTA adds Σ v̄_l h_{l−1}ᵀ and Σ v̄_l to its slice.  Last, each thread recomputes W_in·x₂ + c_1 for
+// σ′_1, turns h̄_1 into v̄_1 and forms x̄₂ = ȳ₂ + W_inᵀv̄_1 in a fixed order, and the CTA adds Σ v̄_1 x₂ᵀ and Σ v̄_1.  The
+// slice is laid out [W̄_out | c̄_out | W̄_in ([H][n2]) | c̄_1 ([H]) | W̄_2 … W̄_M ([H][H] each) | c̄_2 … c̄_M ([H] each)],
+// and coupling_rqs_vjp_reduce_kernel sums the slices into the arrays of each parameter role.
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
@@ -45,20 +43,20 @@ struct CrvParams {
   const float* ybar;
   const float* ljbar;
   float* xbar;
-  const float *W, *c;  // MLP: W₂, c₂
+  const float *W, *c;  // NET: W_out, c_out
   const int *idx1, *idx2;
   float* part;  // [G][slice]
   long long N, ldx, ldyb, ldxb, slice;
   int D, n1, n2, K;
   float B;
-  const float *W1, *c1;  // MLP only (DEEP: c1 = [c_1 | … | c_M], or NULL)
+  const float *W1, *c1;  // NET only: W_in, [c_1 | … | c_M] (or NULL)
   int H, act;
   float slope;
-  const float* Wh;  // DEEP: W_2 .. W_M, each H x H column-major, back to back
-  int M;            // DEEP: hidden layers
+  const float* Wh;  // NET: W_2 .. W_M, each H x H column-major, back to back
+  int M;            // NET: hidden layers
 };
 
-// DEEP: layer l (1-based) of the network on this thread's column, from `in` (n_in rows) to `out` ([H] rows), stride XP
+// NET: layer l (1-based) of the network on this thread's column, from `in` (n_in rows) to `out` ([H] rows), stride XP
 template <int XP>
 __device__ __forceinline__ void crv_layer(const CrvParams& P, int l, const float* in, int n_in, float* out, int tid) {
   const int H = P.H;
@@ -70,38 +68,38 @@ __device__ __forceinline__ void crv_layer(const CrvParams& P, int l, const float
   }
 }
 
-// DEEP: the second [H][XP] block E, after the D row kinds
+// NET: the second [H][XP] block E, after the D row kinds.  The launcher allocates it for M >= 2 only; at M = 1 the
+// pointer lies past the allocation and is never dereferenced (see the forward walk).
 __device__ __forceinline__ float* crv_deep_block(unsigned char* kind, int D) {
   return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kind + D) + 15) & ~(uintptr_t)15);
 }
 
-template <bool INV, bool MLP, bool DEEP>
+template <bool INV, bool NET>
 __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __grid_constant__ CrvParams P) {
   extern __shared__ __align__(16) float crv_sm[];
   constexpr int TN = CRV_TN, XP = CRV_TN + 1;
   // nc: rows of the conditioning block the row loop reads (x₂, or the hidden layer h)
-  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = MLP ? P.H : n2, K = P.K, K1 = K + 1, J = 3 * K - 1;
+  const int tid = threadIdx.x, n1 = P.n1, n2 = P.n2, nc = NET ? P.H : n2, K = P.K, K1 = K + 1, J = 3 * K - 1;
   const int JP = crq_jp(K), D = P.D;
   float* Ws = crv_sm;               // [nc][JP]
   float* cs = Ws + nc * JP;         // [JP]
   float* KT = cs + JP;              // knots W | H | Dv, [3][K1][TN]
   float* G = KT + 3 * K1 * TN;      // their cotangents, same layout
-  float* Xs = G + 3 * K1 * TN;      // x₂ (MLP: h) [nc][XP]
+  float* Xs = G + 3 * K1 * TN;      // x₂ (NET: h) [nc][XP]
   float* Pr = Xs + nc * XP;         // raw parameters, then their cotangents [J][XP]
   double* XB = reinterpret_cast<double*>(crv_sm) + ((size_t)(nc * JP + JP + 6 * K1 * TN + nc * XP + J * XP) + 1) / 2;
-  // x̄₂ (MLP: h̄) [nc][XP] in fp64: it sums (3K − 1)·n1 products per element
-  float* X2 = reinterpret_cast<float*>(XB + nc * XP);  // MLP: x₂ [n2][XP]
+  // x̄₂ (NET: h̄) [nc][XP] in fp64: it sums (3K − 1)·n1 products per element
+  float* X2 = reinterpret_cast<float*>(XB + nc * XP);  // NET: x₂ [n2][XP]
   // [D]: 1 = x₁ row, 2 = x₂ row, 0 = x₃ row
-  unsigned char* kind = reinterpret_cast<unsigned char*>(MLP ? reinterpret_cast<void*>(X2 + n2 * XP) : XB + n2 * XP);
+  unsigned char* kind = reinterpret_cast<unsigned char*>(NET ? reinterpret_cast<void*>(X2 + n2 * XP) : XB + n2 * XP);
   float* slice = P.part + (size_t)blockIdx.x * P.slice;
   float* cslice = slice + (size_t)n1 * J * nc;
-  float* w1slice = cslice + (size_t)n1 * J;  // MLP: [H][n2], then c̄₁ [H]
-  const long long slen = MLP ? (long long)n1 * J * (nc + 1) + (long long)nc * (n2 + 1) : (long long)n1 * J * (n2 + 1);
+  float* w1slice = cslice + (size_t)n1 * J;  // NET: W̄_in [H][n2], c̄_1 [H], W̄_2 .. W̄_M, c̄_2 .. c̄_M
+  const long long slen = NET ? (long long)n1 * J * (nc + 1) + (long long)nc * (n2 + 1) + (long long)(P.M - 1) * nc * (nc + 1)
+                             : (long long)n1 * J * (n2 + 1);
 
   for (int r = tid; r < D; r += TN) kind[r] = 0;
   for (long long e = tid; e < slen; e += TN) slice[e] = 0.f;
-  if constexpr (DEEP)  // W̄_2 .. W̄_M and c̄_2 .. c̄_M follow kind 14's sums
-    for (long long e = tid; e < (long long)(P.M - 1) * nc * (nc + 1); e += TN) slice[slen + e] = 0.f;
   __syncthreads();
   for (int i = tid; i < n1; i += TN) kind[P.idx1[i]] = 1;
   for (int m = tid; m < n2; m += TN) kind[P.idx2[m]] = 2;
@@ -124,26 +122,21 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
     for (int e = tid; e < n2 * TN; e += TN) {
       const int c = e / n2, m = e - c * n2;
       const bool ok = c < cols;
-      (MLP ? X2 : Xs)[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
-      if (!MLP) XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
+      (NET ? X2 : Xs)[m * XP + c] = ok ? P.x[(n0 + c) * P.ldx + P.idx2[m]] : 0.f;
+      if (!NET) XB[m * XP + c] = ok && P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.0;
     }
-    if constexpr (DEEP) {  // h_1 .. h_M of this thread's column (as the forward kernel forms them), h_M in Xs
+    if constexpr (NET) {  // h_1 .. h_M of this thread's column (as the forward kernel forms them), h_M in Xs
       __syncthreads();
       float* const E = crv_deep_block(kind, D);
       const float* in = X2;
+      // layer l goes to Xs when M − l is even: at M = 1 the only layer lands in Xs and E is untouched, as it is by the
+      // walk back l = M .. 2 below, which is then empty
       for (int l = 1; l <= P.M; ++l) {
         float* out = (P.M - l) % 2 == 0 ? Xs : E;
         crv_layer<XP>(P, l, in, l == 1 ? n2 : nc, out, tid);
         in = out;
       }
       for (int m = 0; m < nc; ++m) XB[m * XP + tid] = 0.0;  // h̄_M starts at 0
-    } else if (MLP) {  // h of this thread's column (as the forward kernel forms it); h̄ starts at 0
-      __syncthreads();
-      for (int m = 0; m < nc; ++m) {
-        float dh;
-        mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, nc, n2, X2 + tid, XP, m), Xs[m * XP + tid], dh);
-        XB[m * XP + tid] = 0.0;
-      }
     }
     const float lb = active && P.ljbar ? P.ljbar[n] : 0.f;
     for (int i = 0; i < n1; ++i) {
@@ -209,7 +202,7 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
       }
     }
     __syncthreads();
-    if constexpr (DEEP) {
+    if constexpr (NET) {
       float* const E = crv_deep_block(kind, D);
       float* const whslice = w1slice + (size_t)nc * (n2 + 1);  // W̄_2 .. W̄_M ([H][H] each), then c̄_2 .. c̄_M
       for (int l = P.M; l >= 2; --l) {
@@ -255,15 +248,15 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
         __syncthreads();
       }
     }
-    if (MLP) {
-      // v̄ = h̄ ⊙ σ′(W₁x₂ + c₁) of this thread's column into Xs (h is no longer read)
+    if (NET) {
+      // v̄_1 = h̄_1 ⊙ σ′(W_in·x₂ + c_1) of this thread's column into Xs (h_1 is no longer read)
       for (int m = 0; m < nc; ++m) {
         float h, dh;
         mlp_act(P.act, P.slope, crq_hidden_pre(P.W1, P.c1, nc, n2, X2 + tid, XP, m), h, dh);
         Xs[m * XP + tid] = (float)XB[m * XP + tid] * dh;
       }
       __syncthreads();
-      // this tile's Σ_n v̄ x₂ᵀ and Σ_n v̄, added to the CTA's slice (each element always by the same thread)
+      // this tile's Σ_n v̄_1 x₂ᵀ and Σ_n v̄_1, added to the CTA's slice (each element always by the same thread)
       for (int e = tid; e < nc * n2; e += TN) {
         const int m = e / n2, k = e - m * n2;
         const float* vb = Xs + m * XP;
@@ -279,7 +272,7 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
         w1slice[(size_t)nc * n2 + m] += s;
       }
       __syncthreads();
-      // W₁ᵀv̄ of this thread's column into X2 (x₂ is no longer read), the sum over the hidden units in increasing order
+      // W_inᵀv̄_1 of this thread's column into X2 (x₂ is no longer read), the sum over the hidden units in increasing order
       for (int k = 0; k < n2; ++k) {
         float s = 0.f;
         for (int m = 0; m < nc; ++m) s = fmaf(__ldg(P.W1 + (size_t)k * nc + m), Xs[m * XP + tid], s);
@@ -289,9 +282,9 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
     }
     for (int e = tid; e < n2 * TN; e += TN) {
       const int c = e / n2, m = e - c * n2;
-      if (c < cols)  // MLP: x̄₂ = ȳ₂ + W₁ᵀv̄
+      if (c < cols)  // NET: x̄₂ = ȳ₂ + W_inᵀv̄_1
         P.xbar[(n0 + c) * P.ldxb + P.idx2[m]] =
-            MLP ? (P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.f) + X2[m * XP + c] : (float)XB[m * XP + c];
+            NET ? (P.ybar ? P.ybar[(n0 + c) * P.ldyb + P.idx2[m]] : 0.f) + X2[m * XP + c] : (float)XB[m * XP + c];
     }
     for (int e = tid; e < cols * D; e += TN) {  // x̄₃ = ȳ₃
       const int c = e / D, r = e - c * D;
@@ -300,64 +293,38 @@ __global__ void __launch_bounds__(CRV_TN, 1) coupling_rqs_vjp_kernel(const __gri
   }
 }
 
-// The deep network's four sums, the G slices summed in order in fp64: W̄_out (J x H, J = (3K − 1)·n1) and c̄_out, W̄_in
-// (H x n2) and c̄_1, then W̄_2 .. W̄_M and c̄_2 .. c̄_M, each to the layout of its parameter (p0 = W_in, p1 = W_hid, p2 =
-// W_out, p3 = [c_1 | … | c_M | c_out]; NULL: not wanted).
-__global__ void __launch_bounds__(256) coupling_rqs_deep_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
-                                                                           long long slice, int n1, int H, int n2, int K,
-                                                                           int M, float* __restrict__ Winbar,
-                                                                           float* __restrict__ Whbar,
-                                                                           float* __restrict__ Woutbar,
-                                                                           float* __restrict__ cbar) {
+// The G slices summed in order (in T: float, or double for the deep network) and scattered from the slice layout
+// [W̄_out | c̄_out | W̄_in | c̄_1 | W̄_2 .. W̄_M | c̄_2 .. c̄_M] to the arrays of the parameter roles (NULL: not wanted).  nc:
+// the conditioning rows (n2, or H); H, nl: the network's hidden units and hidden-to-hidden layers (0, 0: none).  W_out is
+// J x nc column-major (J = (3K − 1)·n1), W_in H x n2, W_hid nl H x H blocks, cin = [c_1 | … | c_M].
+template <class T>
+__global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
+                                                                      long long slice, int n1, int nc, int K, int H,
+                                                                      int n2, int nl, float* __restrict__ Wout,
+                                                                      float* __restrict__ cout, float* __restrict__ Win,
+                                                                      float* __restrict__ cin, float* __restrict__ Whid) {
   const long long J = (long long)(3 * K - 1) * n1, hh = (long long)H * H;
-  const long long nw = J * H, nwc = nw + J, nw1 = nwc + (long long)H * n2, nc1 = nw1 + H, nwh = nc1 + (M - 1) * hh;
+  const long long nw = J * nc, nwc = nw + J, nw1 = nwc + (long long)H * n2, nc1 = nw1 + H, nwh = nc1 + nl * hh;
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= nwh + (long long)(M - 1) * H) return;
-  double t = 0.0;
+  if (e >= nwh + (long long)nl * H) return;
+  T t = 0;
   for (int g = 0; g < nparts; ++g) t += part[(size_t)g * slice + e];
   if (e < nw) {  // [i][j][m] -> W_out row i + n1·j, column m
-    const long long i = e / ((3 * K - 1) * (long long)H), rem = e - i * (3 * K - 1) * H, j = rem / H, m = rem - j * H;
-    if (Woutbar) Woutbar[(size_t)(i + n1 * j) + (size_t)J * m] = (float)t;
+    const long long i = e / ((3 * K - 1) * (long long)nc), rem = e - i * (3 * K - 1) * nc, j = rem / nc, m = rem - j * nc;
+    if (Wout) Wout[(size_t)(i + n1 * j) + (size_t)J * m] = (float)t;
   } else if (e < nwc) {  // [i][j] -> c_out[i + n1·j]
     const long long f = e - nw, i = f / (3 * K - 1), j = f - i * (3 * K - 1);
-    if (cbar) cbar[(size_t)M * H + (size_t)(i + n1 * j)] = (float)t;
+    if (cout) cout[(size_t)(i + n1 * j)] = (float)t;
   } else if (e < nw1) {  // [m][k] -> W_in row m, column k
     const long long f = e - nwc, m = f / n2, k = f - m * n2;
-    if (Winbar) Winbar[(size_t)(m + H * k)] = (float)t;
+    if (Win) Win[(size_t)(m + H * k)] = (float)t;
   } else if (e < nc1) {
-    if (cbar) cbar[e - nw1] = (float)t;
+    if (cin) cin[e - nw1] = (float)t;
   } else if (e < nwh) {  // [l − 2][m][k] -> W_l row m, column k
     const long long f = e - nc1, l = f / hh, m = (f - l * hh) / H, k = f - l * hh - m * H;
-    if (Whbar) Whbar[(size_t)(l * hh + m + H * k)] = (float)t;
-  } else if (cbar) {  // c̄_2 .. c̄_M
-    cbar[(size_t)H + (size_t)(e - nwh)] = (float)t;
-  }
-}
-
-// W̄ / c̄: the G slices summed in order, element e of the slice layout scattered to W's column-major layout.  nc: the
-// conditioning rows (n2, or H); with the network also W̄₁ (nh x nx, the slice's [nh][nx]) and c̄₁ (nh), else nh = 0.
-__global__ void __launch_bounds__(256) coupling_rqs_vjp_reduce_kernel(const float* __restrict__ part, int nparts,
-                                                                      long long slice, int n1, int nc, int K,
-                                                                      float* __restrict__ Wbar, float* __restrict__ cbar,
-                                                                      int nh, int nx, float* __restrict__ W1bar,
-                                                                      float* __restrict__ c1bar) {
-  const int J = 3 * K - 1;
-  const long long nw = (long long)n1 * J * nc, nwc = nw + (long long)n1 * J, nw1 = nwc + (long long)nh * nx;
-  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= nw1 + nh) return;
-  float t = 0.f;
-  for (int g = 0; g < nparts; ++g) t += part[(size_t)g * slice + e];
-  if (e < nw) {
-    const int i = (int)(e / ((long long)J * nc)), rem = (int)(e - (long long)i * J * nc), j = rem / nc, m = rem - j * nc;
-    if (Wbar) Wbar[(size_t)(i + n1 * j) + (size_t)J * n1 * m] = t;
-  } else if (e < nwc) {
-    const int f = (int)(e - nw), i = f / J, j = f - i * J;
-    if (cbar) cbar[i + n1 * j] = t;
-  } else if (e < nw1) {
-    const int f = (int)(e - nwc), m = f / nx, k = f - m * nx;
-    if (W1bar) W1bar[m + (size_t)nh * k] = t;
-  } else if (c1bar) {
-    c1bar[e - nw1] = t;
+    if (Whid) Whid[(size_t)(l * hh + m + H * k)] = (float)t;
+  } else if (cin) {  // c̄_2 .. c̄_M
+    cin[(size_t)H + (size_t)(e - nwh)] = (float)t;
   }
 }
 
@@ -414,12 +381,11 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   if (!b2b_coupling_fits(d, D)) return B2B_EUNSUPPORTED;
   if (!s.workspace || s.workspace_bytes < b2b_coupling_rqs_vjp_workspace(d, D, N)) return B2B_EWORKSPACE;
   const Cpl c = b2b_coupling(d);
-  const bool mlp = c.net;
-  // W̄ always goes somewhere (the kernel forms it anyway); c̄ only when the layer has a c.  The network's four sums are
-  // written only where they are asked for.
-  float* const Wbar = mlp ? s.bars[2] : s.bars[0] ? s.bars[0] : s.scratch;
-  float* const cbar = mlp ? (c.c_out ? s.bars[3] : nullptr)
-                          : !c.c_out ? nullptr : s.bars[1] ? s.bars[1] : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
+  // The network's sums are written only where they are asked for.  Without the network, W̄ always goes somewhere (the
+  // kernel forms it anyway), and c̄ when the layer has a c.
+  float* const Wbar = c.net || s.bars[0] ? c.role(s.bars, B2B_W_OUT) : s.scratch;
+  float* const cbar = c.net || !c.c_out || s.bars[1] ? c.role(s.bars, B2B_C_OUT)
+                                                     : s.scratch + ((b2b_slot_len(d, 0, D) + 63) & ~(size_t)63);
   CrvParams P = {};
   P.x = s.x;
   P.ybar = s.ybar;
@@ -447,25 +413,18 @@ int b2b_vjp_spline(const B2BVjpSeg& s) {
   P.slope = c.slope;
   P.Wh = c.W_hid;
   P.M = c.M;
-  const bool deep = crv_nl(c) > 0;
   const int grid = crv_grid(d, D, N);
   const size_t smem = crv_smem_bytes(c, D);
-  void (*kernel)(const CrvParams) =
-      !deep ? (mlp ? (d.inverse ? coupling_rqs_vjp_kernel<true, true, false> : coupling_rqs_vjp_kernel<false, true, false>)
-                   : (d.inverse ? coupling_rqs_vjp_kernel<true, false, false> : coupling_rqs_vjp_kernel<false, false, false>))
-            : (d.inverse ? coupling_rqs_vjp_kernel<true, true, true> : coupling_rqs_vjp_kernel<false, true, true>);
+  void (*kernel)(const CrvParams) = c.net ? (d.inverse ? coupling_rqs_vjp_kernel<true, true> : coupling_rqs_vjp_kernel<false, true>)
+                                          : (d.inverse ? coupling_rqs_vjp_kernel<true, false> : coupling_rqs_vjp_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<grid, CRV_TN, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
-  const long long len = crv_sum_floats(c);
-  if (!deep)
-    coupling_rqs_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
-        P.part, grid, P.slice, c.n1, crv_nc(c), c.K, Wbar, cbar, c.H, crv_nx(c), mlp ? s.bars[0] : nullptr,
-        c.c_in ? s.bars[1] : nullptr);
-  else  // c̄ packs every bias: there is one only when the layer has biases
-    coupling_rqs_deep_vjp_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, s.stream>>>(
-        P.part, grid, P.slice, c.n1, c.H, c.n2, c.K, c.M, s.bars[0], s.bars[1], s.bars[2], c.c_in ? s.bars[3] : nullptr);
+  const unsigned blocks = (unsigned)((crv_sum_floats(c) + 255) / 256);
+  (crv_nl(c) ? coupling_rqs_vjp_reduce_kernel<double> : coupling_rqs_vjp_reduce_kernel<float>)<<<blocks, 256, 0, s.stream>>>(
+      P.part, grid, P.slice, c.n1, crv_nc(c), c.K, c.H, c.n2, crv_nl(c), Wbar, cbar, c.role(s.bars, B2B_W_IN),
+      c.role(s.bars, B2B_C_IN), c.role(s.bars, B2B_W_HID));
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   *s.launches += 2;
   return B2B_OK;

@@ -242,10 +242,11 @@ int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, c
 
 // ---- layer kinds ---------------------------------------------------------------------------------------------------
 // What the chain orchestration knows about each kind of include/b2b.h.  A new kind enters the host code as one row of
-// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu (a coupling: its packing in b2b_coupling and
-// a row of b2b_coupling_fits), its slot lengths in b2b_slot_len, one B2BFwdSeg launcher plus one case of the forward
-// switch in b2b_chain_run_f32, and for reverse mode one B2BVjpSeg launcher plus one case of the sweep's switch in
-// b2b_chain_vjp_f32 (and its scratch and workspace sizes in seg_param_floats / seg_kernel_bytes).
+// the table in b2b_kind, its limits in the envelope functions of b2b_api.cu, its slot lengths in b2b_slot_len, one
+// B2BFwdSeg launcher plus one case of the forward switch in b2b_chain_run_f32, and for reverse mode one B2BVjpSeg
+// launcher plus one case of the sweep's switch in b2b_chain_vjp_f32 (and its scratch and workspace sizes in
+// seg_param_floats / seg_kernel_bytes).  A coupling instead gives its shape fields and the slot of each parameter role
+// in b2b_coupling, which b2b_slot_len and the coupling launchers read, and a row of b2b_coupling_fits.
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
 enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };
@@ -303,8 +304,14 @@ inline bool b2b_chain_has_launch(const b2b_layer_desc* layers, int L, int launch
 }
 
 // ---- coupling descriptors ------------------------------------------------------------------------------------------
-// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS descriptor decoded: the one place that knows how include/b2b.h
-// packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or b2b_layer_desc_f64.
+// Parameter roles of a coupling's conditioner: the network's first layer (W_in, and c_in = [c_1 | … | c_M], every hidden
+// layer's bias), its hidden-to-hidden layers (W_hid = W_2 … W_M back to back) and the last layer (W_out, c_out: all a
+// linear conditioner has).  Each kind keeps each role in one descriptor slot p0 .. p3, the roles of a slot back to back
+// in this order, so the slot table of b2b_coupling fixes every role's offset and every slot's length.
+enum B2BRole { B2B_W_IN, B2B_C_IN, B2B_W_HID, B2B_W_OUT, B2B_C_OUT, B2B_NROLES };
+
+// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS descriptor decoded: the one place that knows how
+// include/b2b.h packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or b2b_layer_desc_f64.
 template <class Desc>
 struct B2BCoupling {
   using Ptr = decltype(Desc::p0);
@@ -313,11 +320,17 @@ struct B2BCoupling {
   bool net, spline;  // the conditioner is a network (H, M, act, slope apply); the law is the spline (K, B apply)
   int act;
   decltype(Desc::f0) slope, B;
-  Ptr W_in, c_in;    // the network's first layer (c_1 .. c_M packed for the deep network)
-  Ptr W_hid;         // W_2 .. W_M of the deep network, back to back
-  Ptr W_out, c_out;  // the last layer: W and c of a linear conditioner
+  int slot[B2B_NROLES];                     // descriptor slot of each role (-1: the kind has none)
+  size_t off[B2B_NROLES], len[B2B_NROLES];  // its offset in the slot and its elements
+  Ptr W_in, c_in, W_hid, W_out, c_out;      // the roles in the descriptor (NULL: absent)
   const int32_t *idx1, *idx2;
   int row1, row2;    // affine law: first rows of idx1 / idx2 when they are contiguous ranges (< 0: use the list)
+
+  // role r within the arrays p[0..3] of the four slots (NULL when the kind has no role r or its slot's array is NULL)
+  template <class T>
+  T* role(T* const* p, int r) const {
+    return slot[r] < 0 || !p[slot[r]] ? nullptr : p[slot[r]] + off[r];
+  }
 };
 
 inline bool b2b_is_coupling(int kind) {
@@ -342,20 +355,31 @@ B2BCoupling<Desc> b2b_coupling(const Desc& d) {
   c.idx2 = d.i1;
   c.row1 = k == B2B_COUPLING_AFFINE ? d.n2 : -1;
   c.row2 = k == B2B_COUPLING_AFFINE ? d.n3 : -1;
-  if (!c.net) {
-    c.W_out = d.p0;
-    c.c_out = d.p1;
-    return c;
+  if (c.net) {
+    c.H = d.n2;
+    c.act = k == B2B_COUPLING_MLP ? d.n3 : d.n3 & 255;
+    c.slope = d.f0;
   }
-  c.H = d.n2;
-  c.act = k == B2B_COUPLING_MLP ? d.n3 : d.n3 & 255;
-  c.slope = d.f0;
-  c.W_in = d.p0;
-  c.W_out = d.p2;
-  // DEEP_MLP, DEEP_MLP_RQS: p1 = W_hid, p3 = [c_1 | … | c_M | c_out] (or NULL)
-  c.W_hid = deep ? d.p1 : nullptr;
-  c.c_in = deep ? d.p3 : d.p1;
-  c.c_out = !deep ? d.p3 : d.p3 ? d.p3 + (size_t)c.M * c.H : nullptr;
+  // the slot of each role: W_in, c_in, W_hid, W_out, c_out
+  static constexpr int linear[B2B_NROLES] = {-1, -1, -1, 0, 1};  // AFFINE, RQS: p0 = W, p1 = c
+  static constexpr int one[B2B_NROLES] = {0, 1, -1, 2, 3};       // MLP, MLP_RQS: p0 = W₁, p1 = c₁, p2 = W₂, p3 = c₂
+  static constexpr int many[B2B_NROLES] = {0, 3, 1, 2, 3};       // DEEP_*: p3 = [c_1 | … | c_M | c_out]
+  const int* slot = deep ? many : c.net ? one : linear;
+  const size_t J = c.spline ? (size_t)(3 * c.K - 1) * c.n1 : (size_t)2 * c.n1;  // rows of W_out
+  const size_t H = c.H, M = c.M;
+  const size_t len[B2B_NROLES] = {H * c.n2, M * H, M > 1 ? (M - 1) * H * H : 0, J * (c.net ? H : c.n2), J};
+  const typename B2BCoupling<Desc>::Ptr p[4] = {d.p0, d.p1, d.p2, d.p3};
+  for (int r = 0; r < B2B_NROLES; ++r) {
+    c.slot[r] = slot[r];
+    c.len[r] = len[r];
+    for (int q = 0; q < r; ++q)
+      if (slot[q] == slot[r]) c.off[r] += len[q];
+  }
+  c.W_in = c.role(p, B2B_W_IN);
+  c.c_in = c.role(p, B2B_C_IN);
+  c.W_hid = c.role(p, B2B_W_HID);
+  c.W_out = c.role(p, B2B_W_OUT);
+  c.c_out = c.role(p, B2B_C_OUT);
   return c;
 }
 
@@ -396,15 +420,12 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
 // elements of trainable slot i of `d` (its cotangent has the parameter's shape)
 template <class Desc>
 size_t b2b_slot_len(const Desc& d, int i, int D) {
-  if (b2b_is_coupling(d.kind)) {
+  if (b2b_is_coupling(d.kind)) {  // the sum of the slot's roles
     const B2BCoupling<Desc> c = b2b_coupling(d);
-    const size_t J = c.spline ? (size_t)(3 * c.K - 1) * c.n1 : (size_t)2 * c.n1;  // rows of W_out
-    if (!c.net) return i == 0 ? J * c.n2 : J;                                      // W, c
-    const size_t H = c.H, M = c.M;
-    const bool deep = d.kind == B2B_COUPLING_DEEP_MLP || d.kind == B2B_COUPLING_DEEP_MLP_RQS;
-    // W_in (H x n2), c_in (H) or the deep network's W_hid ((M−1) x H x H), W_out (J x H), c_out (J) or every bias
-    const size_t len[4] = {H * c.n2, deep ? (M - 1) * H * H : H, J * H, deep ? M * H + J : J};
-    return len[i];
+    size_t n = 0;
+    for (int r = 0; r < B2B_NROLES; ++r)
+      if (c.slot[r] == i) n += c.len[r];
+    return n;
   }
   switch (d.kind) {
     case B2B_PLANAR: return i == 2 ? 1 : D;

@@ -190,6 +190,26 @@ def test_slope_one_equals_the_affine_coupling(B, inv):
 
 
 @pytest.mark.parametrize("inv", [False, True])
+def test_exact_reduction_to_the_one_hidden_layer_kind(B, inv):
+    """M = 2 with W_2 = I, c_2 = 0 and ReLU (LeakyReLU slope 0): h_2 = relu(h_1) = h_1, so the layer is
+    B2B_COUPLING_MLP on the same W_in, c_1, W_out, c_out -- bit for bit, since layer 1 and the affine law are that
+    kind's own code and each h_2 is an fmaf chain of exact products."""
+    rng = np.random.default_rng(17 + inv)
+    D, N, H = 40, 3001, 24
+    idx1, idx2, weights, biases = spec(rng, D, 16, 20, H, 2, scattered=True)
+    weights[1] = np.eye(H, dtype=f32)
+    biases[1] = np.zeros(H, f32)
+    assert np.abs(biases[2]).min() > 0  # c_out nonzero: no sum of the output layer starts at a signed zero
+    x = rng.standard_normal((D, N)).astype(f32)
+    deep = layer(B, D, idx1, idx2, weights, biases, "leaky_relu", 0.0)
+    mlp = B.Coupling(B.MLPConditioner(weights[0], biases[0], weights[2], biases[2], activation="leaky_relu", slope=0.0),
+                     B.PartitionMask(D, idx1, idx2))
+    run = lambda l: [B.to_numpy(a) for a in B.with_logabsdet_jacobian(B.inverse(l) if inv else l, B.from_numpy(x))]  # noqa: E731
+    (yd, ld), (ym, lm) = run(deep), run(mlp)
+    assert yd.tobytes() == ym.tobytes() and ld.tobytes() == lm.tobytes()
+
+
+@pytest.mark.parametrize("inv", [False, True])
 @pytest.mark.parametrize("act,slope", ACTS)
 @pytest.mark.parametrize("M", [2, 3, 4])
 @pytest.mark.parametrize("D,n1,n2,H,N,with_c,cots", [
