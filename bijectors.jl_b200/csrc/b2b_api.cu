@@ -104,6 +104,7 @@ static int vjp_envelope(const b2b_layer_desc& d, int D) {
     case B2B_BATCHNORM:
     case B2B_PERMUTE:
     case B2B_STACKED_EW:
+    case B2B_ELEMENTWISE_VEC:
     case B2B_MVNORMAL_DIAG: ok = D <= 1024; break;  // BatchNorm and the elementwise-run kernel
     default: return fwd_envelope(d, D);
   }
@@ -732,7 +733,7 @@ extern "C" int b2b_radial_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L,
 // ---- reverse mode of any chain ------------------------------------------------------------------------------------------
 // The chain is cut into VJP segments, each differentiated by an existing per-kind kernel or by the elementwise-run kernel:
 // planar runs of one direction (<= 8), radial runs (<= 8, mixed directions), single RQS / coupling / eval-BatchNorm layers,
-// and runs of <= 8 STACKED_EW / PERMUTE layers optionally closed by the terminal MVNORMAL_DIAG.  The forward is recomputed
+// and runs of <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE layers optionally closed by the terminal MVNORMAL_DIAG.  The forward is recomputed
 // once, segment by segment, storing each segment's input (at ld = D); then the segments are differentiated last to first,
 // the cotangent moving between two D x N buffers.  Every segment sees the same l̄ (the log-Jacobians add up).
 namespace {
@@ -756,9 +757,9 @@ int vjp_segments(const b2b_layer_desc* layers, int L, int D, std::vector<VSeg>& 
       s.Dk = D <= 32 ? 32 : D <= 64 ? 64 : 128;
     } else if (s.kind == B2B_VC_RADIAL) {
       while (e < L && e - l < 8 && layers[e].kind == B2B_RADIAL) ++e;
-    } else if (s.kind == B2B_VC_EW) {  // PERMUTE / STACKED_EW layers and the terminal MVNORMAL_DIAG after them, or alone
-      e = l;
-      while (e < L && e - l < 8 && (layers[e].kind == B2B_PERMUTE || layers[e].kind == B2B_STACKED_EW)) ++e;
+    } else if (s.kind == B2B_VC_EW) {  // PERMUTE / STACKED_EW / ELEMENTWISE_VEC layers and the terminal MVNORMAL_DIAG after
+      e = l;                           // them, or alone
+      while (e < L && e - l < 8 && layers[e].kind != B2B_MVNORMAL_DIAG && b2b_kind(layers[e].kind)->vjp == B2B_VC_EW) ++e;
       if (e < L && layers[e].kind == B2B_MVNORMAL_DIAG) ++e;
     }
     segs.push_back(s);
@@ -803,7 +804,11 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case B2B_VC_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
     case B2B_VC_MLP: return b2b_coupling_mlp_vjp_workspace(d, D, N);
     case B2B_VC_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
-    default: return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG);
+    default: {
+      int vec = 0;
+      for (int l = s.begin; l < s.end; ++l) vec += layers[l].kind == B2B_ELEMENTWISE_VEC;
+      return b2b_ew_vjp_workspace(D, layers[s.end - 1].kind == B2B_MVNORMAL_DIAG, vec);
+    }
   }
 }
 

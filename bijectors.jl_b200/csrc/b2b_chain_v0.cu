@@ -259,6 +259,7 @@ __global__ void __launch_bounds__(256) chain_v0_kernel(const __grid_constant__ B
           }
           lj += reduce_cols<G, C>(p, j);  // sum over dimensions, :304-309
         } break;
+        case B2B_ELEMENTWISE_VEC:  // staged as the STACKED_EW table
         case B2B_STACKED_EW: {
           // stacked.jl:157-166,242-252 with elementwise blocks (exp_log.jl, shift.jl, scale.jl)
           const int* code = reinterpret_cast<const int*>(sp);

@@ -56,7 +56,8 @@ static int plan_v1(B2BChainParams& p, V1Plan& plan) {
   }
   p.scratch_off = -1;
   bool per_row = false;  // RQS / Stacked are unrolled per row: only built for <= 64 rows per thread
-  for (int l = 0; l < p.L; ++l) per_row |= p.layers[l].kind == B2B_RQS || p.layers[l].kind == B2B_STACKED_EW;
+  for (int l = 0; l < p.L; ++l)
+    per_row |= p.layers[l].kind == B2B_RQS || p.layers[l].kind == B2B_STACKED_EW || p.layers[l].kind == B2B_ELEMENTWISE_VEC;
   // <D, lanes per column, columns per thread, warps>: warps are chosen so that the per-thread register budget
   // (65536 / threads) holds the fragment without spilling: 64 data registers need ~170 (12 warps), 128 need 255
   // (8 warps), 32 fit in 128 (16 warps).  One column per thread throughout.

@@ -143,6 +143,7 @@ struct InterpProg {
         case B2B_RQS:
           if constexpr (C::EPT * CPT <= 64) rqs_apply<D, TPC, CPT>(x, ctx, sp, d.n0, d.inverse != 0, lj);
           break;
+        case B2B_ELEMENTWISE_VEC:  // staged as the STACKED_EW table
         case B2B_STACKED_EW:
           if constexpr (C::EPT * CPT <= 64) stacked_apply<D, TPC, CPT>(x, ctx, sp, d.inverse != 0, lj);
           break;

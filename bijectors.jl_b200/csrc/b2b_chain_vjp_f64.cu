@@ -373,6 +373,24 @@ __device__ __forceinline__ void layer_vjp(const b2b_layer_desc_f64& d, int D, in
         g[i] = g[i] * f + lb * dl;
       }
     } break;
+    case B2B_ELEMENTWISE_VEC: {  // accumulators: ā [D]; ∂y/∂a, ∂ℓ/∂a as in b2b_ew_vjp.cu:ew_vec_dparam
+      for (int i = lane; i < D; i += 32) {
+        const double a = d.p0[i], x = col[i];
+        double f, dl;
+        law_deriv64(d.n0, inv, a, 0.0, x, f, dl);
+        if (acc) {
+          double dy = 0.0, da = 0.0;
+          if (d.n0 == B2B_EW_SHIFT) {
+            dy = inv ? -1.0 : 1.0;
+          } else if (d.n0 == B2B_EW_SCALE || x < 0.0) {
+            dy = inv ? -x / (a * a) : x;
+            da = inv ? -1.0 / a : 1.0 / a;
+          }
+          acc[i] += g[i] * dy + lb * da;
+        }
+        g[i] = g[i] * f + lb * dl;
+      }
+    } break;
     case B2B_PERMUTE: {
       for (int i = lane; i < D; i += 32) t1[i] = g[i];
       __syncwarp();
@@ -520,6 +538,7 @@ __global__ void __launch_bounds__(V64_FIN_THREADS) vjp_f64_finalize_kernel(const
     case B2B_RQS:
       for (int i = 0; i < 3; ++i) copy(bars[i], r + (size_t)i * D * d.n0, (size_t)D * d.n0);
       break;
+    case B2B_ELEMENTWISE_VEC: copy(bars[0], r, D); break;
     case B2B_COUPLING_AFFINE:
       copy(bars[0], r, (size_t)2 * d.n0 * d.n1);
       copy(bars[1], r + (size_t)2 * d.n0 * d.n1, (size_t)2 * d.n0);
@@ -547,6 +566,7 @@ long long acc_len(const b2b_layer_desc_f64& d, int D) {
   switch (d.kind) {
     case B2B_PLANAR: n = 2LL * D + 2; break;
     case B2B_RADIAL: n = (long long)D + 2; break;
+    case B2B_ELEMENTWISE_VEC: n = D; break;
     case B2B_RQS: n = 3LL * D * d.n0; break;
     case B2B_COUPLING_AFFINE: n = 2LL * d.n0 * d.n1 + 2LL * d.n0; break;
     case B2B_BATCHNORM:

@@ -319,7 +319,7 @@ __device__ __forceinline__ float ew_apply(int op, bool inverse, float a, float b
 //   BATCHNORM : A[Dp] | C[Dp] | iA[Dp] | iC[Dp] | {Σ(logs − log(v+eps)/2)}   y = A·x + C, x = iA·y + iC
 //   RQS       : Sw[Dp][KP] | Sh[Dp][KP] | per-(row,bin) constants float4 x 2 [Dp][K1]  ((2·KP + 8·K1)·Dp floats)
 //   PERMUTE   : src_of_dst[Dp] (int)
-//   STACKED_EW: code[Dp] (int) | a[Dp] | b[Dp]
+//   STACKED_EW: code[Dp] (int) | a[Dp] | b[Dp]   (ELEMENTWISE_VEC: the same table, code = n0 and b = 0 on every row)
 //   MVNORMAL  : mu[Dp] | 1/sigma[Dp] | {−(D·log2π + Σ log σ²)/2}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -462,6 +462,14 @@ __device__ inline void stage_layer(const b2b_layer_desc& d, float* sm, int D, in
         sc[i] = i < D ? d.i0[i] : B2B_EW_IDENTITY;
         sm[Dp + i] = (i < D && d.p0) ? d.p0[i] : 0.f;
         sm[2 * Dp + i] = (i < D && d.p1) ? d.p1[i] : 0.f;
+      }
+    } break;
+    case B2B_ELEMENTWISE_VEC: {
+      int* sc = reinterpret_cast<int*>(sm);
+      for (int i = lane; i < Dp; i += 32) {
+        sc[i] = i < D ? d.n0 : B2B_EW_IDENTITY;
+        sm[Dp + i] = i < D ? d.p0[i] : 0.f;
+        sm[2 * Dp + i] = 0.f;
       }
     } break;
     case B2B_MVNORMAL_DIAG: {

@@ -12,6 +12,13 @@
 // layer loop stays rolled and the kernel is a pure stream over x, ȳ and x̄.  μ̄ and σ̄ of row r_K belong to exactly one
 // thread per slab (the path is a permutation); slabs are summed in shared memory and CTAs by a fixed-order finalize,
 // so the result is bitwise deterministic.
+//
+// ELEMENTWISE_VEC layers run as the STACKED_EW layer they equal: code[r] = the law (a row of the constant table
+// ew_vec_codes), a = p0, b = 0 -- so x̄ is the same stream with the same bits.  Their ā needs the cotangent ḡ_k at each
+// such layer's output, which the forward-only sweep does not have: when ā is requested, the SLOTS instantiation also runs
+// the run backwards per column, recomputing each layer's input from x (O(Ls²) law evaluations for Ls laws, no tape):
+//   ā_k[r_k] += ḡ_k·∂y/∂a + l̄·∂ℓ/∂a,   ḡ_{k−1} = ḡ_k·f′_k + l̄·∂log|f′_k|/∂x
+// Row r_k at layer k belongs to one thread per slab, so ā goes through the same slab / CTA / finalize path as μ̄ and σ̄.
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -33,7 +40,25 @@ struct EvParams {
   long long N, ldx, ldyb, ldxb;
   int D, L, mvn;
   b2b_layer_desc layers[EV_MAXL];
+  // SLOTS instantiation only (the fields after `layers` leave the other instantiations' parameter offsets as they were)
+  int width;            // floats per CTA in `part`: [μ̄ | σ̄] (2D, when the run ends in the MvNormal) | ā of each vec layer (D)
+  int mw;               // 2D or 0: where the ā blocks start
+  int vlo;              // first Stacked layer with an ā block
+  int vslot[EV_MAXL];   // per Stacked layer: its ā block, -1 for none
 };
+
+// The law column of an ELEMENTWISE_VEC layer seen as STACKED_EW: ew_vec_codes.c[law − B2B_EW_SHIFT][r] = law.
+static_assert(B2B_EW_SCALE == B2B_EW_SHIFT + 1 && B2B_EW_LEAKY_RELU == B2B_EW_SHIFT + 2, "law codes");
+struct EwVecCodes {
+  int32_t c[3][1024];
+};
+constexpr EwVecCodes ew_vec_codes_init() {
+  EwVecCodes t{};
+  for (int k = 0; k < 3; ++k)
+    for (int r = 0; r < 1024; ++r) t.c[k][r] = B2B_EW_SHIFT + k;
+  return t;
+}
+__device__ const EwVecCodes ew_vec_codes = ew_vec_codes_init();
 
 // One law of ew_apply at input xv: returns the value (the formulas of ew_apply) together with f′ and ∂log|f′|/∂x, the
 // derivatives of exactly those formulas.  Value and derivatives share their transcendentals; reciprocals are the
@@ -118,6 +143,20 @@ __device__ __forceinline__ float ew_step(int op, bool inverse, float a, float b,
       return xo < a ? a : (xo > b ? b : xo);
     }
     default: return xv;  // IDENTITY
+  }
+}
+
+// ∂y/∂a and ∂ℓ/∂a of an ELEMENTWISE_VEC law at input xv (the row's a; the laws of ew_step):
+//   Shift 1, 0 (inverse −1, 0); Scale xv, 1/a (inverse −xv/a², −1/a); LeakyReLU those of Scale where xv < 0, else 0, 0
+__device__ __forceinline__ void ew_vec_dparam(int op, bool inverse, float a, float xv, float& dy, float& dl) {
+  dy = 0.0f;
+  dl = 0.0f;
+  if (op == B2B_EW_SHIFT) {
+    dy = inverse ? -1.0f : 1.0f;
+  } else if (op == B2B_EW_SCALE || xv < 0.f) {
+    const float ra = 1.0f / a;
+    dy = inverse ? -(xv * ra) * ra : xv;
+    dl = inverse ? -ra : ra;
   }
 }
 
@@ -229,17 +268,168 @@ __global__ void __launch_bounds__(TMAX) ew_vjp_kernel(const __grid_constant__ Ev
   }
 }
 
-// out[e] = Σ_cta part[cta][e] in a fixed order: μ̄ = out[0, D), σ̄ = out[D, 2D)
-__global__ void __launch_bounds__(256) ew_vjp_finalize_kernel(const float* __restrict__ part, int nparts, int D,
-                                                              float* __restrict__ mubar, float* __restrict__ sigmabar) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= 2 * D) return;
+
+// ew_vjp_kernel with the ā of the run's ELEMENTWISE_VEC layers, for any D <= 1024 (T = max(256, Dp) threads, two columns
+// in flight).  A kernel of its own so that the x̄-only instantiations above keep their code.  Shared memory as above,
+// with acc [V][T] (the thread's ā sums of the V vec layers) before red [nslab][P.width] (μ̄ | σ̄ | ā).  x̄, μ̄ and σ̄
+// are computed exactly as above.
+__global__ void __launch_bounds__(1024) ew_vjp_slots_kernel(const __grid_constant__ EvParams P) {
+  constexpr int U = 2;
+  extern __shared__ __align__(16) int esm[];
+  const int D = P.D, L = P.L, Dp = (D + 31) & ~31, T = blockDim.x, nslab = T / Dp, tid = threadIdx.x, W = P.width;
+  int Ls = 0;
+  for (int l = 0; l < L; ++l) Ls += P.layers[l].kind == B2B_STACKED_EW;
+  int* nxt = esm;
+  int* law = nxt + L * Dp;
+  float* pa = reinterpret_cast<float*>(law + Ls * T);
+  float* pb = pa + Ls * T;
+  float* acc = pb + Ls * T;
+  float* red = acc + (W - P.mw) / D * T;
+  for (int l = 0; l < L; ++l) {
+    const b2b_layer_desc& d = P.layers[l];
+    if (d.kind != B2B_PERMUTE) continue;
+    for (int i = tid; i < D; i += T) {
+      const int j = d.i0[i];
+      if (d.inverse) nxt[l * Dp + j] = i;
+      else nxt[l * Dp + i] = j;
+    }
+  }
+  __syncthreads();
+  const int slab = tid / Dp, r0 = tid - slab * Dp;
+  const bool active = slab < nslab && r0 < D;
+  int rK = r0;
+  if (active) {
+    int s = 0;
+    for (int l = 0; l < L; ++l) {
+      const b2b_layer_desc& d = P.layers[l];
+      if (d.kind == B2B_PERMUTE) {
+        rK = nxt[l * Dp + rK];
+      } else {
+        law[s * T + tid] = d.i0[rK] | (d.inverse ? 256 : 0);
+        pa[s * T + tid] = d.p0 ? d.p0[rK] : 0.f;
+        pb[s * T + tid] = d.p1 ? d.p1[rK] : 0.f;
+        if (P.vslot[s] >= 0) acc[P.vslot[s] * T + tid] = 0.f;
+        ++s;
+      }
+    }
+  }
+  float mu = 0.f, is = 1.f;
+  if (P.mvn && active) {
+    mu = P.mu ? P.mu[rK] : 0.f;
+    is = P.sigma ? 1.0f / P.sigma[rK] : 1.0f;
+  }
+  float gmu = 0.f, gsg = 0.f;
+  const long long per = (P.N + gridDim.x - 1) / gridDim.x;
+  const long long c0 = (long long)blockIdx.x * per, c1 = (c0 + per < P.N) ? c0 + per : P.N;
+  if (active) {
+    for (long long n0 = c0 + slab; n0 < c1; n0 += (long long)U * nslab) {
+      float v[U], g[U], lb[U], Pp[U], Q[U], x0[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const long long n = n0 + (long long)u * nslab;
+        const bool ok = n < c1;
+        v[u] = x0[u] = ok ? __ldcs(P.x + n * P.ldx + r0) : 0.f;
+        g[u] = (ok && P.ybar) ? __ldcs(P.ybar + n * P.ldyb + rK) : 0.f;
+        lb[u] = (ok && P.ljbar) ? __ldcs(P.ljbar + n) : 0.f;
+        Pp[u] = 1.0f;
+        Q[u] = 0.0f;
+      }
+#pragma unroll 1
+      for (int s = 0; s < Ls; ++s) {
+        const int c = law[s * T + tid];
+        const int op = c & 255;
+        const bool inv = c >> 8;
+        const float a = pa[s * T + tid], b = pb[s * T + tid];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          float f1, dl;
+          v[u] = ew_step(op, inv, a, b, v[u], f1, dl);
+          Q[u] = fmaf(Pp[u], dl, Q[u]);
+          Pp[u] *= f1;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const long long n = n0 + (long long)u * nslab;
+        if (n >= c1) continue;
+        float gk = g[u];
+        if (P.mvn) {
+          const float q = (v[u] - mu) * is;
+          const float w = lb[u] * q * is;
+          gk -= w;
+          gmu += w;
+          gsg = fmaf(lb[u] * is, fmaf(q, q, -1.0f), gsg);
+        }
+        __stcs(P.xbar + n * P.ldxb + r0, fmaf(gk, Pp[u], lb[u] * Q[u]));
+        // the backward sweep from the run's output down to the first vec layer, each layer's input recomputed from x
+#pragma unroll 1
+        for (int k = Ls - 1; k >= P.vlo; --k) {
+          float xin = x0[u], f1, dl;
+#pragma unroll 1
+          for (int s = 0; s < k; ++s) {
+            const int c = law[s * T + tid];
+            xin = ew_step(c & 255, c >> 8, pa[s * T + tid], pb[s * T + tid], xin, f1, dl);
+          }
+          const int c = law[k * T + tid];
+          const int op = c & 255;
+          const bool inv = c >> 8;
+          const float a = pa[k * T + tid];
+          ew_step(op, inv, a, pb[k * T + tid], xin, f1, dl);
+          const int j = P.vslot[k];
+          if (j >= 0) {
+            float dy, da;
+            ew_vec_dparam(op, inv, a, xin, dy, da);
+            acc[j * T + tid] = fmaf(gk, dy, fmaf(lb[u], da, acc[j * T + tid]));
+          }
+          gk = fmaf(gk, f1, lb[u] * dl);
+        }
+      }
+    }
+  }
+  if (active) {
+    if (P.mvn) {
+      red[slab * W + rK] = gmu;
+      red[slab * W + D + rK] = gsg;
+    }
+    int r = r0, s = 0;  // the thread's row at each Stacked layer, walked again
+    for (int l = 0; l < L; ++l) {
+      if (P.layers[l].kind == B2B_PERMUTE) {
+        r = nxt[l * Dp + r];
+        continue;
+      }
+      if (P.vslot[s] >= 0) red[slab * W + P.mw + P.vslot[s] * D + r] = acc[P.vslot[s] * T + tid];
+      ++s;
+    }
+  }
+  __syncthreads();
+  for (int e = tid; e < W; e += T) {
+    float t = 0.f;
+    for (int w = 0; w < nslab; ++w) t += red[w * W + e];
+    P.part[(size_t)blockIdx.x * W + e] = t;
+  }
+}
+
+// The per-CTA partials summed in a fixed order: out[e] = Σ_cta part[cta][e], e < width, then μ̄ = out[0, D),
+// σ̄ = out[D, 2D) (mw = 2D), ā of vec layer j = out[mw + jD, mw + (j+1)D)
+struct EvFin {
+  const float* part;
+  int nparts, D, width, mw;
+  float* mubar;
+  float* sigmabar;
+  float* abar[EV_MAXL];
+};
+
+__global__ void __launch_bounds__(256) ew_vjp_finalize_kernel(const __grid_constant__ EvFin F) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x, D = F.D;
+  if (e >= F.width) return;
   float t = 0.f;
-  for (int p = 0; p < nparts; ++p) t += part[(size_t)p * 2 * D + e];
-  if (e < D) {
-    if (mubar) mubar[e] = t;
-  } else if (sigmabar) {
-    sigmabar[e - D] = t;
+  for (int p = 0; p < F.nparts; ++p) t += F.part[(size_t)p * F.width + e];
+  if (e >= F.mw) {
+    if (float* a = F.abar[(e - F.mw) / D]) a[(e - F.mw) % D] = t;
+  } else if (e < D) {
+    if (F.mubar) F.mubar[e] = t;
+  } else if (F.sigmabar) {
+    F.sigmabar[e - D] = t;
   }
 }
 
@@ -265,9 +455,10 @@ static int ev_grid_max() { return b2b_sm_count() * 8; }
 
 }  // namespace b2b
 
-size_t b2b_ew_vjp_workspace(int D, int want_mvn_params) {
-  if (!want_mvn_params) return 0;
-  return (size_t)b2b::ev_grid_max() * 2 * (size_t)D * sizeof(float) + 256;
+size_t b2b_ew_vjp_workspace(int D, int want_mvn_params, int vec_layers) {
+  const size_t width = (want_mvn_params ? 2 * (size_t)D : 0) + (size_t)vec_layers * D;
+  if (!width) return 0;
+  return (size_t)b2b::ev_grid_max() * width * sizeof(float) + 256;
 }
 
 int b2b_vjp_ew(const B2BVjpSeg& s) {
@@ -280,23 +471,43 @@ int b2b_vjp_ew(const B2BVjpSeg& s) {
   if (D < 1 || D > 1024 || L < 0) return B2B_EUNSUPPORTED;
   EvParams P;
   memset(&P, 0, sizeof(P));
-  int Ls = 0;
+  float* abar[EV_MAXL] = {};
+  const int32_t* codes = nullptr;
+  int Ls = 0, V = 0;
+  bool want_a = false;
   for (int l = 0; l < L; ++l) {
     const b2b_layer_desc& d = layers[l];
     if (d.kind == B2B_MVNORMAL_DIAG && l == L - 1) {
       P.mvn = 1;
       P.mu = d.p0;
       P.sigma = d.p1;
-    } else if (d.kind == B2B_STACKED_EW || d.kind == B2B_PERMUTE) {
+    } else if (d.kind == B2B_STACKED_EW || d.kind == B2B_PERMUTE || d.kind == B2B_ELEMENTWISE_VEC) {
       if (P.L == EV_MAXL) return B2B_EUNSUPPORTED;
-      Ls += d.kind == B2B_STACKED_EW;
-      P.layers[P.L++] = d;
+      b2b_layer_desc& e = P.layers[P.L++] = d;
+      if (d.kind == B2B_PERMUTE) continue;
+      P.vslot[Ls] = -1;
+      if (d.kind == B2B_ELEMENTWISE_VEC) {  // the STACKED_EW layer it equals
+        if (!codes) {
+          const EwVecCodes* t;
+          cudaError_t err = cudaGetSymbolAddress((void**)&t, ew_vec_codes);
+          if (err != cudaSuccess) return (int)err;
+          codes = &t->c[0][0];
+        }
+        e.kind = B2B_STACKED_EW;
+        e.i0 = codes + (size_t)(d.n0 - B2B_EW_SHIFT) * 1024;
+        e.p1 = nullptr;
+        abar[V] = s.bars[4 * l];
+        want_a |= abar[V] != nullptr;
+        if (V == 0) P.vlo = Ls;
+        P.vslot[Ls] = V++;
+      }
+      ++Ls;
     } else {
       return B2B_EUNSUPPORTED;
     }
   }
-  const bool want = P.mvn && (mubar || sigmabar);
-  if (want && (!s.workspace || s.workspace_bytes < b2b_ew_vjp_workspace(D, 1))) return B2B_EWORKSPACE;
+  const bool want = (P.mvn && (mubar || sigmabar)) || want_a;
+  if (want && (!s.workspace || s.workspace_bytes < b2b_ew_vjp_workspace(D, P.mvn, V))) return B2B_EWORKSPACE;
   P.x = s.x;
   P.ybar = s.ybar;
   P.ljbar = s.ljbar;
@@ -306,22 +517,38 @@ int b2b_vjp_ew(const B2BVjpSeg& s) {
   P.ldyb = s.ldyb;
   P.ldxb = s.ldxb;
   P.D = D;
+  P.mw = P.mvn ? 2 * D : 0;
+  P.width = want_a ? P.mw + V * D : 2 * D;
   const int T = ev_threads(D), Dp = (D + 31) & ~31, nslab = T / Dp;
   long long grid = ev_grid_max();
-  const int U = T <= 256 ? 4 : 2;  // columns in flight per thread of the instantiation launched below
+  const int U = want_a || T > 256 ? 2 : 4;  // columns in flight per thread of the instantiation launched below
   const long long need = (s.N + (long long)nslab * U - 1) / ((long long)nslab * U);
   if (grid > need) grid = need;
   if (grid < 1) grid = 1;
   if (want) P.part = reinterpret_cast<float*>(b2b_align256(s.workspace));
-  const size_t smem = ((size_t)P.L * Dp + (size_t)3 * Ls * T) * sizeof(int) + (want ? (size_t)nslab * 2 * D * sizeof(float) : 0);
+  size_t smem = ((size_t)P.L * Dp + (size_t)3 * Ls * T) * sizeof(int) + (want ? (size_t)nslab * P.width * sizeof(float) : 0);
   void (*kernel)(const EvParams) = T <= 256 ? ew_vjp_kernel<256, 4> : ew_vjp_kernel<1024, 2>;
+  if (want_a) {
+    kernel = ew_vjp_slots_kernel;
+    smem += (size_t)V * T * sizeof(float);
+  }
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<(int)grid, T, smem, s.stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   ++*s.launches;
   if (want) {
-    ew_vjp_finalize_kernel<<<(2 * D + 255) / 256, 256, 0, s.stream>>>(P.part, (int)grid, D, mubar, sigmabar);
+    EvFin F;
+    memset(&F, 0, sizeof(F));
+    F.part = P.part;
+    F.nparts = (int)grid;
+    F.D = D;
+    F.width = P.width;
+    F.mw = want_a ? P.mw : 2 * D;
+    F.mubar = mubar;
+    F.sigmabar = sigmabar;
+    for (int j = 0; j < V; ++j) F.abar[j] = abar[j];
+    ew_vjp_finalize_kernel<<<(F.width + 255) / 256, 256, 0, s.stream>>>(F);
     if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
     ++*s.launches;
   }

@@ -272,10 +272,12 @@ static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f6
       p = wsum(p);
       lj += inv ? -p : p;
     } break;
+    case B2B_ELEMENTWISE_VEC:  // the law n0 on every row, a = p0 (b unused)
     case B2B_STACKED_EW: {
+      const bool vec = d.kind == B2B_ELEMENTWISE_VEC;
       double p = 0.0;
       for (int i = lane; i < D; i += 32)
-        col[i] = ew_apply64(d.i0[i], inv, d.p0 ? d.p0[i] : 0.0, d.p1 ? d.p1[i] : 0.0, col[i], p);
+        col[i] = ew_apply64(vec ? d.n0 : d.i0[i], inv, d.p0 ? d.p0[i] : 0.0, d.p1 && !vec ? d.p1[i] : 0.0, col[i], p);
       lj += wsum(p);
     } break;
     case B2B_PERMUTE: {

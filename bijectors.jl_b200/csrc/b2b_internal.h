@@ -44,7 +44,8 @@ static inline int b2b_layer_smem_floats(const b2b_layer_desc& d, int Dp) {
       return (2 * kp + 8 * d.n0) * Dp;
     }
     case B2B_PERMUTE: return Dp;
-    case B2B_STACKED_EW: return 3 * Dp;
+    case B2B_STACKED_EW:
+    case B2B_ELEMENTWISE_VEC: return 3 * Dp;  // staged as the STACKED_EW table
     case B2B_MVNORMAL_DIAG: return 2 * Dp + 4;
     default: return 0;
   }
@@ -86,9 +87,10 @@ size_t b2b_planar_vjp_workspace(int L, int D, long long N);
 // reverse mode of one affine coupling layer (b2b_coupling_vjp.cu): whether its kernel takes the layer at D (n1, n2 <= 128
 // and the D-row input / cotangent tiles within shared memory: D <= 747 at n1 = n2 = 128)
 bool b2b_coupling_affine_vjp_fits(const b2b_layer_desc& d, int D);
-// reverse mode of an elementwise run (b2b_ew_vjp.cu): <= 8 STACKED_EW / PERMUTE layers, optionally closed by the terminal
-// MVNORMAL_DIAG.  ybar, ljbar may be NULL (zeros); mubar / sigmabar (D, or NULL) need b2b_ew_vjp_workspace(D, 1) bytes.
-size_t b2b_ew_vjp_workspace(int D, int want_mvn_params);
+// reverse mode of an elementwise run (b2b_ew_vjp.cu): <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE layers, optionally closed
+// by the terminal MVNORMAL_DIAG.  ybar, ljbar may be NULL (zeros); mubar / sigmabar (D, or NULL) and the ā of the run's
+// `vec_layers` ELEMENTWISE_VEC layers need b2b_ew_vjp_workspace(D, 1, vec_layers) bytes (0 for a run with neither).
+size_t b2b_ew_vjp_workspace(int D, int want_mvn_params, int vec_layers);
 // one launch copying up to 24 small device vectors: dst[k][0, len[k]) = src[k][0, len[k]), zero up to dst_len[k]
 int b2b_launch_copy_list(int n, const float* const* src, float* const* dst, const int* len, const int* dst_len,
                          cudaStream_t stream);
@@ -230,7 +232,7 @@ int b2b_vjp_radial(const B2BVjpSeg& s);    // b2b_radial_vjp.cu: <= 8 layers
 int b2b_vjp_rqs(const B2BVjpSeg& s);       // b2b_rqs_vjp.cu
 int b2b_vjp_coupling(const B2BVjpSeg& s);  // b2b_coupling_vjp.cu
 int b2b_vjp_batchnorm(const B2BVjpSeg& s); // b2b_coupling_vjp.cu: eval mode
-int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / PERMUTE, optionally closed by MVNORMAL_DIAG
+int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE, optionally closed by MVNORMAL_DIAG
 int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
 int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
 int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu
@@ -250,7 +252,8 @@ int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, c
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
 enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };
-// Reverse-mode segment class of b2b_chain_vjp_f32 (B2B_VC_EW: runs of STACKED_EW / PERMUTE, with MVNORMAL_DIAG).
+// Reverse-mode segment class of b2b_chain_vjp_f32 (B2B_VC_EW: runs of STACKED_EW / ELEMENTWISE_VEC / PERMUTE, with
+// MVNORMAL_DIAG).
 enum B2BVjpClass {
   B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE, B2B_VC_MLP
 };
@@ -289,6 +292,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_COUPLING_MLP_RQS, B2B_F_P0 | B2B_F_P2 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P1 | B2B_F_P3, false},
       {B2B_COUPLING_DEEP_MLP, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_MLP, B2B_VC_MLP, 4, B2B_F_P3, false},
       {B2B_COUPLING_DEEP_MLP_RQS, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P3, false},
+      {B2B_ELEMENTWISE_VEC, B2B_F_P0,                    false, B2B_LC_FUSED,    B2B_VC_EW,       1, 0,        true},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -406,6 +410,8 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
     if ((k->required >> f & 1) && !field[f]) return B2B_EINVAL;
   if (k->terminal && (!last || d.inverse)) return B2B_EINVAL;
   if (d.kind == B2B_RQS) return d.n0 >= 2 ? B2B_OK : B2B_EINVAL;
+  if (d.kind == B2B_ELEMENTWISE_VEC)
+    return d.n0 == B2B_EW_SHIFT || d.n0 == B2B_EW_SCALE || d.n0 == B2B_EW_LEAKY_RELU ? B2B_OK : B2B_EINVAL;
   if (!b2b_is_coupling(d.kind)) return B2B_OK;
   const B2BCoupling<Desc> c = b2b_coupling(d);
   bool ok = c.n1 >= 1 && c.n2 >= 1 && c.n1 + c.n2 <= D;
@@ -433,7 +439,7 @@ size_t b2b_slot_len(const Desc& d, int i, int D) {
     case B2B_RQS: return (size_t)D * d.n0;
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
     case B2B_SCALE_MATRIX: return (size_t)D * D;
-    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ
+    default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ, ELEMENTWISE_VEC a
   }
 }
 

@@ -72,7 +72,8 @@ static int launch_sample(const B2BChainParams& q, const V1Geom& g, const CUtenso
 }  // namespace b2b
 
 static bool fusable_kind(int kind) {
-  return kind == B2B_PLANAR || kind == B2B_RADIAL || kind == B2B_RQS || kind == B2B_BATCHNORM || kind == B2B_STACKED_EW;
+  return kind == B2B_PLANAR || kind == B2B_RADIAL || kind == B2B_RQS || kind == B2B_BATCHNORM || kind == B2B_STACKED_EW ||
+         kind == B2B_ELEMENTWISE_VEC;
 }
 
 extern "C" int b2b_randn_f32(float* z, const float* mu, const float* sigma, uint64_t seed, uint64_t offset,

@@ -839,13 +839,21 @@ _SLOTS = {
     _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
     _lib.COUPLING_DEEP_MLP_RQS: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
+    _lib.ELEMENTWISE_VEC: (("a",), lambda d, D: ((D,),), ()),  # named α for the LeakyReLU law (_slot_names)
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
 
 
+def _slot_names(d) -> Tuple[str, ...]:
+    """The field names of ``d``'s slots: a vector LeakyReLU's slope is ``α`` (leaky_relu.jl), Shift's and Scale's ``a``."""
+    if d.kind == _lib.ELEMENTWISE_VEC and d.n0 == _lib.EW_LEAKY_RELU:
+        return ("α",)
+    return _SLOT_NAMES.get(d.kind, ())
+
+
 def _trainable_slots(d) -> List[int]:
     """Slots of descriptor ``d`` that have a cotangent (absent optional parameters have none)."""
-    names = _SLOT_NAMES.get(d.kind, ())
+    names = _slot_names(d)
     return [i for i in range(len(names)) if getattr(d, f"p{i}")]
 
 
@@ -856,7 +864,8 @@ def _slot_shape(d, i: int, D: int) -> Tuple[int, ...]:
 
 def _slot_grads(d, l: int, bars) -> dict:
     """The cotangents ``bars`` holds for descriptor l (``d``), keyed by field name, each in its parameter's orientation."""
-    names, _, colmajor = _SLOTS.get(d.kind, ((), None, ()))
+    colmajor = _SLOTS.get(d.kind, ((), None, ()))[2]
+    names = _slot_names(d)
     return {name: bars[(l, i)].transpose(-1, -2) if i in colmajor else bars[(l, i)]
             for i, name in enumerate(names) if (l, i) in bars}
 
@@ -937,7 +946,8 @@ def chain_vjp(t, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Op
     One b2b_chain_vjp_f32 call -- b2b_chain_vjp_f64 when ``x`` is a Float64 batch, whose layers and cotangents must then be
     Float64 too (a mix raises TypeError).  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)``
     (application order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives``
-    (D×K+1), ``W/c``, ``b/logs``, ``a`` (D×D, a dense Scale), and ``{}`` for Permute and Stacked -- summed over the columns of this batch."""
+    (D×K+1), ``W/c``, ``b/logs``, ``a`` (D×D, a dense Scale; D, a vector Shift / Scale), ``α`` (D, a vector LeakyReLU), and ``{}`` for Permute, Stacked and
+    the scalar elementwise layers -- summed over the columns of this batch."""
     D = _batch_view(x)[0]
     descs, counts = _leaf_descs(t, D, x.dtype)
     if not descs:

@@ -46,6 +46,7 @@ const COUPLING_MLP = Int32(13)
 const COUPLING_MLP_RQS = Int32(14)
 const COUPLING_DEEP_MLP = Int32(15)
 const COUPLING_DEEP_MLP_RQS = Int32(16)
+const ELEMENTWISE_VEC = Int32(17)
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -285,6 +286,27 @@ end
 # Scale(A) with a D x D matrix (scale.jl:14,17,35-36): A itself, column-major as CuMatrix stores it; Float32, D <= 256
 desc(b::Scale{<:CuMatrix{Float32}}, inv::Bool) =
     LayerDesc(SCALE_MATRIX, inv, 0, 0, 0, 0, 0f0, 0f0, pointer(b.a), NULLF, NULLF, NULLF, NULLI, NULLI)
+# Shift / Scale / LeakyReLU with a vector field (shift.jl, scale.jl:16,31-32, leaky_relu.jl:25-29): the law on every row with
+# the row's own, trainable parameter, n0 = the law.  Float32 vectors give the descriptor of b2b_chain_run_f32 /
+# b2b_chain_vjp_f32; Float64 ones the b2b_layer_desc_f64 of b2b_chain_run_f64 / b2b_chain_vjp_f64 (include/b2b.h).
+struct LayerDesc64
+    kind::Int32; inverse::Int32
+    n0::Int32; n1::Int32; n2::Int32; n3::Int32
+    f0::Float64; f1::Float64
+    p0::CuPtr{Float64}; p1::CuPtr{Float64}; p2::CuPtr{Float64}; p3::CuPtr{Float64}
+    i0::CuPtr{Int32}; i1::CuPtr{Int32}
+end
+const NULLD = CuPtr{Float64}(0)
+const VectorLaw{A} = Union{Shift{<:A},Scale{<:A},LeakyReLU{<:A}}
+vec_param(b::Union{Shift,Scale}) = b.a
+vec_param(b::LeakyReLU) = b.α
+vec_code(::Shift) = EW_SHIFT
+vec_code(::Scale) = EW_SCALE
+vec_code(::LeakyReLU) = EW_LEAKY_RELU
+desc(b::VectorLaw{CuVector{Float32}}, inv::Bool) =
+    LayerDesc(ELEMENTWISE_VEC, inv, vec_code(b), 0, 0, 0, 0f0, 0f0, pointer(vec_param(b)), NULLF, NULLF, NULLF, NULLI, NULLI)
+desc(b::VectorLaw{CuVector{Float64}}, inv::Bool) =
+    LayerDesc64(ELEMENTWISE_VEC, inv, vec_code(b), 0, 0, 0, 0.0, 0.0, pointer(vec_param(b)), NULLD, NULLD, NULLD, NULLI, NULLI)
 # a whole-column elementwise law is a one-block Stacked
 const ElementwiseLaw = Union{Shift{<:Real},Scale{<:Real},LeakyReLU{<:Real},Logit{<:Real,<:Real},TruncatedBijector{<:Real,<:Real}}
 
@@ -299,7 +321,7 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}},
-                          Scale{<:CuMatrix{Float32}},Permute,Stacked}
+                          Scale{<:CuMatrix{Float32}},VectorLaw{CuVector{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
 is_device(::DeviceLeaf) = true
@@ -498,7 +520,8 @@ end
 
 # Reverse mode of ANY device chain (b2b_chain_vjp_f32): `f` (or inverse(f) with inv=true); ȳ, l̄ the cotangents of
 # (y, logjac), `nothing` = zeros.  Returns x̄ and, per descriptor in application order, the cotangents of its trainable
-# fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, Scale(A) a, BatchNorm b logs, the
+# fields (PlanarLayer w u b, RadialLayer α_ β z_0, RQS widths heights derivatives, Coupling W c, Scale(A) a, vector Shift /
+# Scale a and LeakyReLU α, BatchNorm b logs, the
 # terminal MvNormal's μ σ) in the fields' shapes; `nothing` for fields without one.
 # Hidden units H, spline bins K and hidden layers M of a coupling descriptor (0 where the kind has none), decoded here only:
 # n2 is K or H, and n3 packs σ | K << 8, σ | M << 8 or σ | K << 8 | M << 16 (include/b2b.h).
@@ -521,6 +544,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
         return (z(H, d.n1), d.p1 == NULLF ? nothing : z(H), z(J, H), d.p3 == NULLF ? nothing : z(J))
     end
     d.kind == SCALE_MATRIX && return (z(D, D),)
+    d.kind == ELEMENTWISE_VEC && return (z(D),)  # Shift / Scale a, LeakyReLU α
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
     d.kind == MVNORMAL_TRIL && return (d.p0 == NULLF ? nothing : z(D), z(D, D))
@@ -644,7 +668,7 @@ end
 # Structural tangents of what rand_vjp returns.  The transform: flatten() lists the leaves inner-most first, one
 # descriptor each, so a ComposedFunction takes its inner part's cotangents first.  A leaf's trainable fields are the first
 # fields of its struct in slot order (PlanarLayer w u b, RadialLayer α_ β z_0, RationalQuadraticSpline widths heights
-# derivatives, InvertibleBatchNorm b logs, Scale a), a Coupling's those of its conditioner θ, and Inverse wraps `orig`.
+# derivatives, InvertibleBatchNorm b logs, Scale a, vector Shift a and LeakyReLU α), a Coupling's those of its conditioner θ, and Inverse wraps `orig`.
 function transform_tangent(f, bars, k::Base.RefValue{Int})
     f isa ComposedFunction || return leaf_tangent(f, bars[k[] += 1])
     inner = transform_tangent(f.inner, bars, k)

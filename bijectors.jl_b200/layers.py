@@ -773,33 +773,86 @@ def _as_stacked(b, D, dtype=torch.float32):
     return cache[key]
 
 
-class Shift(Bijector):
-    """Shift(a): y = a .+ x, logjac 0 (shift.jl:4-24); scalar `a` inside Stacked blocks."""
+class _ElementwiseLaw(Bijector):
+    """Shift / Scale / LeakyReLU with a scalar parameter -- the law's row of a Stacked table (B2B_STACKED_EW), constant --
+    or with a vector a[D]: the law on every row with the row's own parameter a[r], one B2B_ELEMENTWISE_VEC descriptor
+    whose `a` is trainable (shift.jl, scale.jl:16,31-32, leaky_relu.jl:25-29; Optimisers.jl trains array leaves).  The
+    vector lives in the device tensor ``_a`` of the `dtype` given, Float32 (the hot path) or Float64; a 1-D tensor or
+    array builds it, a Python scalar or 0-d value the scalar form.  The vector form is not a Stacked block, and its
+    inverse is Inverse(layer) on the same tensor, so that reverse mode reaches it."""
 
-    def __init__(self, a):
-        self.a = float(a)
+    code: int
 
-    code = _lib.EW_SHIFT
+    def _init_law(self, a, device, dtype):
+        if (a.dim() if isinstance(a, torch.Tensor) else np.ndim(a)) == 1:
+            self._a, self._s = _dev_f32(a, device, dtype), None
+        else:
+            self._a, self._s = None, float(a)
+
+    @property
+    def vector(self) -> bool:
+        return self._a is not None
+
+    @property
+    def a(self):
+        return self._a if self.vector else self._s
+
+    @property
+    def device(self):
+        return self._a.device
+
+    def to(self, device):
+        if not self.vector:
+            return self
+        new = object.__new__(type(self))
+        new.__dict__.update(self.__dict__)
+        new._a = self._a.to(device)
+        return new
+
+    def _keepalive(self):
+        return (self._a,) if self.vector else ()
 
     def _inverse(self):
-        return Shift(-self.a)  # shift.jl:12
+        return Inverse(self) if self.vector else self._scalar_inverse()
 
     def _descs(self, inverse, D, dtype=torch.float32):
-        return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
+        if not self.vector:
+            return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
+        if D != self._a.numel():
+            raise ValueError(f"DimensionMismatch: {type(self).__name__} has {self._a.numel()} dims, input has {D}")
+        _check_dtype(self._a, dtype, type(self).__name__)
+        return [_desc(_lib.ELEMENTWISE_VEC, inverse, n0=self.code, p0=self._a)]
 
     def __eq__(self, o):
-        return isinstance(o, Shift) and o.a == self.a
+        if type(o) is not type(self) or o.vector != self.vector:
+            return False
+        return torch.equal(self._a.cpu(), o._a.cpu()) if self.vector else o._s == self._s
 
     __hash__ = object.__hash__
 
 
-class Scale(Bijector):
-    """Scale(a): y = a .* x, logjac = log|a| per element (scale.jl:1-39) for a scalar `a` (also a Stacked block).
+class Shift(_ElementwiseLaw):
+    """Shift(a): y = a .+ x, logjac 0 (shift.jl:4-24); a scalar `a` (also a Stacked block) or a trainable vector a[D]."""
+
+    code = _lib.EW_SHIFT
+
+    def __init__(self, a, device="cuda", dtype=torch.float32):
+        self._init_law(a, device, dtype)
+
+    def _scalar_inverse(self):
+        return Shift(-self.a)  # shift.jl:12
+
+
+class Scale(_ElementwiseLaw):
+    """Scale(a): y = a .* x, logjac = log|a| per element (scale.jl:1-39) for a scalar `a` (also a Stacked block) or a
+    trainable vector a[D] (scale.jl:16,31-32).
 
     A square matrix `a` gives the dense layer Scale{<:AbstractMatrix} (scale.jl:14,17,35-36): y = A x, inverse A \\ y,
     logjac = logabsdet(A)[1] per column, with A trainable (B2B_SCALE_MATRIX; Float32 only, D <= 256).  The device tensor
     `_A` holds A column-major, i.e. Aᵀ row-major (as MvNormal's scale_tril); `.a` returns A in the user's orientation.
     A singular A is the caller's responsibility: the forward gives logjac = −Inf, the inverse non-finite values."""
+
+    code = _lib.EW_SCALE
 
     def __init__(self, a, device="cuda", dtype=torch.float32):
         if (a.dim() if isinstance(a, torch.Tensor) else np.ndim(a)) == 2:
@@ -809,11 +862,10 @@ class Scale(Bijector):
             if A.shape[0] != A.shape[1]:
                 raise ValueError(f"DimensionMismatch: Scale needs a square matrix, got {tuple(A.shape)}")
             self._A = A.to(device=device, dtype=torch.float32).t().contiguous()
+            self._a = self._s = None
             return
         self._A = None
-        self._a = float(a)
-
-    code = _lib.EW_SCALE
+        self._init_law(a, device, dtype)
 
     @property
     def dense(self) -> bool:
@@ -821,25 +873,30 @@ class Scale(Bijector):
 
     @property
     def a(self):
-        return self._A.t() if self.dense else self._a
+        return self._A.t() if self.dense else _ElementwiseLaw.a.fget(self)
 
     @property
     def device(self):
-        return self._A.device
+        return self._A.device if self.dense else self._a.device
 
     def to(self, device):
         new = object.__new__(Scale)
         new.__dict__.update(self.__dict__)
         if self.dense:
             new._A = self._A.to(device)
+        elif self.vector:
+            new._a = self._a.to(device)
         return new
 
     def _keepalive(self):
-        return (self._A,) if self.dense else ()
+        return (self._A,) if self.dense else _ElementwiseLaw._keepalive(self)
+
+    def _inverse(self):
+        return Inverse(self)  # the scalar form included, as before: the inverse flag on the same table
 
     def _descs(self, inverse, D, dtype=torch.float32):
         if not self.dense:
-            return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
+            return _ElementwiseLaw._descs(self, inverse, D, dtype)
         if D != self._A.shape[0]:
             raise ValueError(f"DimensionMismatch: Scale has a {self._A.shape[0]} x {self._A.shape[0]} matrix, input has {D} dims")
         _check_dtype(self._A, dtype, "Scale")
@@ -848,33 +905,26 @@ class Scale(Bijector):
     def __eq__(self, o):
         if not isinstance(o, Scale) or self.dense != o.dense:
             return False
-        return torch.equal(self._A.cpu(), o._A.cpu()) if self.dense else o._a == self._a
+        return torch.equal(self._A.cpu(), o._A.cpu()) if self.dense else _ElementwiseLaw.__eq__(self, o)
 
     __hash__ = object.__hash__
 
 
-class LeakyReLU(Bijector):
-    """LeakyReLU(α): x ↦ x if x ≥ 0 else αx, α > 0 (leaky_relu.jl:9-29); inverse = LeakyReLU(1/α) (:16).
-    Batched logjac is per column (the reference sums over the whole array)."""
-
-    def __init__(self, α):
-        self.a = float(α)
-        if not self.a > 0:
-            raise ValueError("LeakyReLU needs α > 0")
+class LeakyReLU(_ElementwiseLaw):
+    """LeakyReLU(α): x ↦ x if x ≥ 0 else αx, α > 0 (leaky_relu.jl:9-29); inverse = LeakyReLU(1/α) (:16) for a scalar α,
+    Inverse(layer) for a trainable vector α[D] (:25-29).  α > 0 is checked here; values reached by training are not
+    checked on the device.  Batched logjac is per column (the reference sums over the whole array)."""
 
     code = _lib.EW_LEAKY_RELU
     α = property(lambda s: s.a)
 
-    def _inverse(self):
+    def __init__(self, α, device="cuda", dtype=torch.float32):
+        self._init_law(α, device, dtype)
+        if not (bool((self._a > 0).all()) if self.vector else self._s > 0):
+            raise ValueError("LeakyReLU needs α > 0")
+
+    def _scalar_inverse(self):
         return LeakyReLU(1.0 / self.a)
-
-    def _descs(self, inverse, D, dtype=torch.float32):
-        return _as_stacked(self, D, dtype)._descs(inverse, D, dtype)
-
-    def __eq__(self, o):
-        return isinstance(o, LeakyReLU) and o.a == self.a
-
-    __hash__ = object.__hash__
 
 
 class Logit(Bijector):
@@ -936,6 +986,8 @@ class Stacked(Transform):
                 raise B2BError(_lib.B2B_EUNSUPPORTED, f"Stacked block {type(b).__name__}")
             if isinstance(b, Scale) and b.dense:
                 raise B2BError(_lib.B2B_EUNSUPPORTED, "Stacked block Scale with a matrix (a dense layer acts on whole columns)")
+            if isinstance(b, _ElementwiseLaw) and b.vector:
+                raise B2BError(_lib.B2B_EUNSUPPORTED, f"Stacked block {type(b).__name__} with a vector (one law on whole columns)")
         self.bs, self.ranges_in = bs, ranges
         self.length_in = sum(hi - lo + 1 for lo, hi in ranges)
         self.length_out = self.length_in

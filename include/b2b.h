@@ -108,6 +108,7 @@ extern "C" {
 #define B2B_COUPLING_DEEP_MLP_RQS_MAX_K 16
 #define B2B_COUPLING_DEEP_MLP_RQS_MAX_DEPTH 4
 #define B2B_COUPLING_DEEP_MLP_RQS_MAX_D 1024
+#define B2B_ELEMENTWISE_VEC 17 /* Shift(a) / Scale(a) / LeakyReLU(a) with a trainable vector a[D]   shift.jl, scale.jl:16,31-32, leaky_relu.jl:25-29 */
 /* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and
  * B2B_COUPLING_DEEP_MLP_RQS (descriptor field n3) */
 #define B2B_ACT_TANH 0
@@ -209,6 +210,13 @@ extern "C" {
  *                     n1, n2, H >= 1, n1 + n2 <= D, K >= 1, M >= 2, a known σ and B > 0, else B2B_EINVAL.  Float32 only,
  *                     exact fp32 on the CUDA cores, its own launch.  Envelope: B2B_COUPLING_DEEP_MLP_RQS_MAX_*; the
  *                     Float64 entry points return B2B_EUNSUPPORTED.)
+ * ELEMENTWISE_VEC    a[D]        -           -           -        -               -             law   -    -
+ *                    (one law on every row, n0 = B2B_EW_SHIFT, B2B_EW_SCALE or B2B_EW_LEAKY_RELU (any other value returns
+ *                     B2B_EINVAL), with the row's own parameter a = p0[r] (required): the map and log-Jacobian of that law of
+ *                     STACKED_EW, and inverse != 0 its inverse on the same a.  A STACKED_EW layer with code[r] = n0 and the
+ *                     same a gives the same bits.  It fuses into column-local launches like STACKED_EW (same 3Dp staging,
+ *                     D <= 1024), runs in both precisions, and trains a: slot 0 of b2b_chain_vjp_f32 / _f64.  a > 0 for
+ *                     LeakyReLU is the caller's contract; nothing on the device checks it.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -237,7 +245,7 @@ const char* b2b_status_string(int status);
  * absorbs a BATCHNORM layer directly before and/or after it as a per-row affine (needs workspace).
  * Limits.  Column-local layers need D <= 1024.  A fused launch stages the derived parameters of its layers in
  * 200 KB of shared memory, in floats at the padded depth Dp = D rounded up to 32, 64, 128, 256, 512 or 1024:
- * PLANAR 2Dp+4, RADIAL Dp+4, BATCHNORM 4Dp+4, STACKED_EW 3Dp, MVNORMAL_DIAG 2Dp+4, PERMUTE Dp (plus, once per launch
+ * PLANAR 2Dp+4, RADIAL Dp+4, BATCHNORM 4Dp+4, STACKED_EW and ELEMENTWISE_VEC 3Dp, MVNORMAL_DIAG 2Dp+4, PERMUTE Dp (plus, once per launch
  * that permutes, 8192 floats of column scratch), RQS (2·KP + 8·K1)·Dp with KP = K1 rounded up
  * to a power of two -- so an RQS layer takes K1 <= 64 knots for D <= 64, K1 <= 34 for D <= 128, K1 <= 17 for D <= 256,
  * K1 <= 8 for D <= 512 and K1 <= 4 for D <= 1024 (the default K = 8 bins, K1 = 9, up to D = 256).  A run of column-local
@@ -400,15 +408,17 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * W_out c the same way (W̄_out ((3K−1)·n1 x H) column-major like W_out);
  * SCALE_MATRIX a (Ā, D x D column-major like A: G + (Σ l̄)·A⁻ᵀ, or −A⁻ᵀ G A⁻ᵀ − (Σ l̄)·A⁻ᵀ for the inverse layer, with
  * G = Σₙ ȳₙ uₙᵀ over the layer's inputs u; slots 1-3 return B2B_EUNSUPPORTED);
- * BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
+ * ELEMENTWISE_VEC a (ā[D], Σₙ of ḡ·∂y/∂a + l̄·∂ℓ/∂a at the layer's output cotangent ḡ; slots 1-3 return
+ * B2B_EUNSUPPORTED); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
  * (BatchNorm m / v, PERMUTE, STACKED_EW, MVNORMAL_TRIL slots 2-3) returns B2B_EUNSUPPORTED.
  * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
  * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling / spline coupling /
  * dense Scale (factor, x̄ by the transposed map, G over column chunks, an fp64 finalize; workspace: the factor of
  * b2b_chain_run_f32 plus P·D² floats, P <= 64 chunks, and 2·D² + 1 doubles) /
- * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / PERMUTE layers (with the terminal MvNormal), which one kernel
- * differentiates; a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
+ * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE layers (with the terminal MvNormal),
+ * which one kernel differentiates (with ā requested, a second instantiation that also sweeps the run backwards, plus
+ * G·V·D floats of per-CTA partials for the V ELEMENTWISE_VEC layers of the run, G <= 8 per SM); a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
  * launch; with μ̄ / L̄ requested it also stores r = L⁻¹(x − μ) and l̄·L⁻ᵀr (2·D·N floats of workspace), and two more
  * launches form L̄ = tril(Σ l̄ s rᵀ) over at most 64 column chunks (P·D·(D+1) floats of chunk partials, P = min(ceil(N /
  * 4096), 64)) and reduce the chunks in order.  The forward is recomputed once to checkpoint each segment's input, then the segments are
@@ -534,8 +544,8 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * the terminal B2B_MVNORMAL_DIAG or B2B_MVNORMAL_TRIL, whose logjac output is then logpdf).  `xbar` (D x N, required) must not overlap `x` or
  * `ybar` (B2B_EINVAL); NULL `ybar` / `ljbar` are zeros; `param_bars` (NULL = x̄ only) holds 4*L pointers, entry 4l+i the
  * cotangent of layers[l].p<i> in its shape and layout, summed over the N columns.  Trainable slots as for Float32: PLANAR
- * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; BATCHNORM b
- * logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
+ * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; ELEMENTWISE_VEC
+ * a; BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
  * p0 is NULL) and L (D x D column-major, exactly zero above the diagonal); any other non-NULL entry returns
  * B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
  * parameter cotangents.  One warp per column recomputes the forward with the arithmetic of b2b_chain_run_f64, keeping
@@ -545,7 +555,7 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * kernels and fills enqueued (1, or 3 with parameter cotangents).
  * Workspace (b2b_chain_vjp_workspace_bytes_f64; 0 exactly when the call refuses the chain) is bounded independently of N:
  * W warp slots of 8·(T + P) bytes plus 8·P, with T = Lf·D (Lf: layers before the MvNormal) and P the accumulators, per
- * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, BATCHNORM / MVNORMAL_DIAG 2D, MVNORMAL_TRIL
+ * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, ELEMENTWISE_VEC D, BATCHNORM / MVNORMAL_DIAG 2D, MVNORMAL_TRIL
  * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
  * 256 MiB but never below one CTA -- so the bound exceeds 256 MiB only when one CTA's slots do (e.g. wide couplings with
  * 2n1·n2 in the millions).  The number of warps, and with it the summation order, depends only on the chain, D and N. */
