@@ -373,7 +373,7 @@ def _trainable_tensors(leaf) -> List[torch.Tensor]:
         return [lay.widths, lay.heights, lay.derivatives]
     if isinstance(lay, Coupling):
         return [t for t in lay.θ._tensors() if t is not None]
-    if isinstance(lay, Scale) and lay.dense:
+    if isinstance(lay, Scale) and lay._A is not None:  # dense or triangular matrix
         return [lay._A]
     if isinstance(lay, _ElementwiseLaw) and lay.vector:  # Shift / Scale / LeakyReLU with a vector parameter
         return [lay._a]

@@ -87,6 +87,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_RQS: ok = d.n0 <= 64; break;
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_fits(d.n0, d.n1, D); break;
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
+    case B2B_SCALE_TRIANGULAR: ok = D <= B2B_SCALE_TRIANGULAR_MAX_D; break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
     default: ok = !b2b_is_coupling(d.kind) || b2b_coupling_fits(d, D); break;  // the other couplings' table
   }
@@ -311,9 +312,18 @@ static bool sum_needs_logjac_ws(const b2b_layer_desc* layers, int32_t L, int nse
   return layers && L >= 1 && b2b_ends_in_terminal(layers, L) && nsegs > 1;
 }
 
-// factor storage of the dense Scale layers (one region: they run one after another); 0 for a chain without one
+// factor storage of the dense and triangular Scale layers (one region of the largest: they run one after another); 0 for a
+// chain without one
 static size_t chain_scale_bytes(const b2b_layer_desc* layers, int32_t L, int D) {
-  return layers && b2b_chain_has_launch(layers, L, B2B_LC_SCALE) ? b2b_scale_matrix_workspace(D) : 0;
+  size_t bytes = 0;
+  for (int l = 0; layers && l < L; ++l) {
+    const B2BKind* k = b2b_kind(layers[l].kind);
+    if (k && k->launch == B2B_LC_SCALE) {
+      const size_t b = b2b_scale_workspace(layers[l].kind, D);
+      if (b > bytes) bytes = b;
+    }
+  }
+  return bytes;
 }
 
 extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_t L, int32_t D, int64_t N,
@@ -803,7 +813,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case B2B_VC_TRIL: return b2b_tril_vjp_workspace(D, N);
     case B2B_VC_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
     case B2B_VC_MLP: return b2b_coupling_mlp_vjp_workspace(d, D, N);
-    case B2B_VC_SCALE: return b2b_scale_matrix_vjp_workspace(D, N);  // also holds the factor of the forward recompute
+    case B2B_VC_SCALE: return b2b_scale_vjp_workspace(d.kind, D, N);  // also holds the factor of the forward recompute
     default: {
       int vec = 0;
       for (int l = s.begin; l < s.end; ++l) vec += layers[l].kind == B2B_ELEMENTWISE_VEC;

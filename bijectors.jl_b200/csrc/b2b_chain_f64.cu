@@ -31,6 +31,8 @@ struct F64Params {
   b2b_layer_desc_f64 layers[B2B_MAX_CHAIN];
 };
 
+// TRI: the chain holds a SCALE_TRIANGULAR layer (f64_layer_forward<TRI>)
+template <bool TRI>
 __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_constant__ F64Params P) {
   extern __shared__ double sm64[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, D = P.D;
@@ -41,7 +43,7 @@ __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_
     for (int i = lane; i < D; i += 32) col[i] = P.x[n * P.ldx + i];
     double lj = (P.accumulate && P.logjac) ? P.logjac[n] : 0.0;
     __syncwarp();
-    for (int l = 0; l < P.L; ++l) f64_layer_forward(P.layers[l], D, lane, col, tmp, lj);
+    for (int l = 0; l < P.L; ++l) f64_layer_forward<TRI>(P.layers[l], D, lane, col, tmp, lj);
     if (P.y)
       for (int i = lane; i < D; i += 32) P.y[n * P.ldy + i] = col[i];
     if (lane == 0) {
@@ -108,9 +110,12 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     P.partials = static_cast<double*>(workspace);
   }
   const size_t smem = (size_t)F64_WARPS * 2 * D * sizeof(double);
-  cudaError_t e = cudaFuncSetAttribute(chain_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  bool tri = false;
+  for (int l = 0; l < L; ++l) tri = tri || layers[l].kind == B2B_SCALE_TRIANGULAR;
+  const auto kernel = tri ? chain_f64_kernel<true> : chain_f64_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  chain_f64_kernel<<<(int)grid, F64_WARPS * 32, smem, stream>>>(P);
+  kernel<<<(int)grid, F64_WARPS * 32, smem, stream>>>(P);
   e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   if (sum_out) return b2b_launch_sum_partials(P.partials, (int)grid, sum_out, stream);

@@ -391,6 +391,46 @@ __device__ __forceinline__ void layer_vjp(const b2b_layer_desc_f64& d, int D, in
         g[i] = g[i] * f + lb * dl;
       }
     } break;
+    case B2B_SCALE_TRIANGULAR: {  // accumulators: T̄ on 𝒫 packed by columns (column j: rows j..D-1 lower, 0..j upper)
+      const double* Tm = d.p0;
+      const bool up = d.n0 != 0, unit = d.n1 != 0;
+      const double* u = col;  // forward: T̄ += ȳ xᵀ on 𝒫 (+ l̄/Tᵢᵢ);  inverse: T̄ −= x̄ yᵀ on 𝒫 (+ l̄/Tᵢᵢ), y = T⁻¹x in t2
+      if (!inv) {
+        for (int k = 0; k < D; ++k) {  // x̄_k = Σᵢ T(i, k)·ȳᵢ over column k of T: a coalesced read and a warp sum
+          double p = 0.0;
+          for (int i = (up ? 0 : k + 1) + lane; i < (up ? k : D); i += 32) p += Tm[(size_t)k * D + i] * g[i];
+          p = wsum(p);
+          if (lane == 0) t1[k] = p + (unit ? g[k] : Tm[(size_t)k * D + k] * g[k]);
+        }
+      } else {
+        for (int i = lane; i < D; i += 32) t2[i] = col[i];
+        __syncwarp();
+        f64_tri_solve(d, D, lane, t2);
+        for (int ii = 0; ii < D; ++ii) {  // Tᵀ x̄ = ȳ: x̄ᵢ = (ȳᵢ − Σ_k T(k, i)·x̄_k)/Tᵢᵢ over the finished k of column i
+          const int i = up ? ii : D - 1 - ii;
+          double p = 0.0;
+          for (int k = (up ? 0 : i + 1) + lane; k < (up ? i : D); k += 32) p += Tm[(size_t)i * D + k] * t1[k];
+          p = wsum(p);
+          if (lane == 0) t1[i] = (g[i] - p) / (unit ? 1.0 : Tm[(size_t)i * D + i]);
+          __syncwarp();
+        }
+        u = t2;
+      }
+      __syncwarp();
+      if (acc) {
+        const double* gl = inv ? t1 : g;  // the outer product's left factor: ȳ, or −x̄ for the inverse layer
+        const double sg = inv ? -1.0 : 1.0;
+        for (int j = 0; j < D; ++j) {
+          double* Ac = acc + (up ? (size_t)j * (j + 1) / 2 : (size_t)j * D - (size_t)j * (j + 1) / 2);  // T̄(i, j) at Ac[i]
+          const double uj = sg * u[j];
+          const int i0 = up ? 0 : (unit ? j + 1 : j), i1 = up ? (unit ? j : j + 1) : D;
+          for (int i = i0 + lane; i < i1; i += 32) Ac[i] += gl[i] * uj;
+          if (!unit && lane == 0) Ac[j] += sg * lb / Tm[(size_t)j * D + j];
+        }
+      }
+      __syncwarp();  // the outer product reads g with a lane mapping that shifts with j: every lane is done with it
+      for (int i = lane; i < D; i += 32) g[i] = t1[i];
+    } break;
     case B2B_PERMUTE: {
       for (int i = lane; i < D; i += 32) t1[i] = g[i];
       __syncwarp();
@@ -556,6 +596,14 @@ __global__ void __launch_bounds__(V64_FIN_THREADS) vjp_f64_finalize_kernel(const
           bars[1][k] = i >= j ? r[D + j * D - j * (j + 1) / 2 + i] : 0.0;
         }
       break;
+    case B2B_SCALE_TRIANGULAR:  // T̄ unpacked to D x D column-major, zero outside 𝒫
+      if (bars[0])
+        for (size_t k = t; k < (size_t)D * D; k += V64_FIN_THREADS) {
+          const size_t j = k / D, i = k - j * D;
+          const bool in = d.n0 ? (d.n1 ? i < j : i <= j) : (d.n1 ? i > j : i >= j);
+          bars[0][k] = in ? r[(d.n0 ? j * (j + 1) / 2 : j * D - j * (j + 1) / 2) + i] : 0.0;
+        }
+      break;
     default: break;
   }
 }
@@ -572,6 +620,7 @@ long long acc_len(const b2b_layer_desc_f64& d, int D) {
     case B2B_BATCHNORM:
     case B2B_MVNORMAL_DIAG: n = 2LL * D; break;
     case B2B_MVNORMAL_TRIL: n = (long long)D + (long long)D * (D + 1) / 2; break;
+    case B2B_SCALE_TRIANGULAR: n = (long long)D * (D + 1) / 2; break;
     default: break;
   }
   return (n + 31) & ~31LL;

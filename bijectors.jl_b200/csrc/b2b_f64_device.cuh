@@ -207,8 +207,59 @@ static __device__ void f64_tril_back(const b2b_layer_desc_f64& d, int D, int lan
   }
 }
 
+// v := T⁻¹ v in place for SCALE_TRIANGULAR (p0 = T column-major, read through L2; n0: upper, n1: unit diagonal): forward
+// substitution for a lower T, back substitution for an upper one, v_j final once the steps before it have run, then the
+// rest of column j of T is subtracted.  Reads only the triangle (not the diagonal of a unit T).
+static __device__ void f64_tri_solve(const b2b_layer_desc_f64& d, int D, int lane, double* v) {
+  const double* Tm = d.p0;
+  const bool up = d.n0 != 0, unit = d.n1 != 0;
+  for (int jj = 0; jj < D; ++jj) {
+    const int j = up ? D - 1 - jj : jj;
+    const double vj = unit ? v[j] : v[j] / Tm[(size_t)j * D + j];
+    __syncwarp();  // every lane has read v[j]
+    if (lane == 0) v[j] = vj;
+    for (int i = (up ? 0 : j + 1) + lane; i < (up ? j : D); i += 32) v[i] = fma(-Tm[(size_t)j * D + i], vj, v[i]);
+    __syncwarp();
+  }
+}
+
+// Σᵢ log|Tᵢᵢ| of SCALE_TRIANGULAR in every lane (0 for a unit diagonal)
+static __device__ __forceinline__ double f64_tri_logdet(const b2b_layer_desc_f64& d, int D, int lane) {
+  double p = 0.0;
+  for (int i = lane; i < D && !d.n1; i += 32) p += log(fabs(d.p0[(size_t)i * D + i]));
+  return wsum(p);
+}
+
+// y = T x (rows owned by lanes, k increasing; `tmp` holds x) or T⁻¹ x (substitution in place) for SCALE_TRIANGULAR;
+// returns its log-Jacobian in every lane.
+static __device__ double f64_tri_forward(const b2b_layer_desc_f64& d, int D, int lane, double* col,
+                                                      double* tmp) {
+  const double lp = f64_tri_logdet(d, D, lane);
+  if (d.inverse) {
+    f64_tri_solve(d, D, lane, col);
+    return -lp;
+  }
+  const bool up = d.n0 != 0, unit = d.n1 != 0;
+  for (int i = lane; i < D; i += 32) {
+    tmp[i] = col[i];
+    col[i] = unit ? col[i] : 0.0;
+  }
+  __syncwarp();
+  for (int k = 0; k < D; ++k) {
+    const double xk = tmp[k];
+    const double* Tk = d.p0 + (size_t)k * D;
+    for (int i = lane; i < D; i += 32)
+      if (up ? (i < k || (i == k && !unit)) : (i > k || (i == k && !unit))) col[i] = fma(Tk[i], xk, col[i]);
+  }
+  __syncwarp();
+  return lp;
+}
+
 // Applies one layer to the column `col` (D doubles in shared memory; `tmp`: D more, scratch) and adds its log-Jacobian
-// (for MVNORMAL_DIAG: the log-density) to `lj`.  Called by all 32 lanes of a warp; ends with __syncwarp.
+// (for MVNORMAL_DIAG: the log-density) to `lj`.  Called by all 32 lanes of a warp; ends with __syncwarp.  TRI = false
+// leaves SCALE_TRIANGULAR out: compiled in, that case costs the Float64 forward kernel registers (80 instead of 96, and a
+// spill), so b2b_chain_run_f64 uses that instantiation only for chains that hold the layer.
+template <bool TRI = true>
 static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f64& d, int D, int lane, double* col,
                                                          double* tmp, double& lj) {
   const bool inv = d.inverse != 0;
@@ -318,6 +369,9 @@ static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f6
       ls = wsum(ls);
       lj += -0.5 * ((double)D * 1.8378770664093453 + ls) - 0.5 * q;
     } break;
+    case B2B_SCALE_TRIANGULAR:
+      if constexpr (TRI) lj += f64_tri_forward(d, D, lane, col, tmp);
+      break;
     case B2B_MVNORMAL_TRIL:  // the column is left as it is (the terminal's y is its input); r goes to tmp
       lj += -0.5 * (double)D * 1.8378770664093453 + f64_tril_solve(d, D, lane, col, tmp);
       break;

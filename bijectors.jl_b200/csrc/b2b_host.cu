@@ -27,11 +27,12 @@ struct b2b_host_ctx {
 
 static const size_t kWsBytes = 512 * 1024;  // batch-sum partials + tensor-core W image of a coupling layer
 
-// A chain with a dense Scale also needs its factor storage, before the partials: the staging workspace grows to hold it
-// at D_max, and only such chains are handed the larger size (every other chain sees kWsBytes, as before).
+// A chain with a dense or triangular Scale also needs its factor storage, before the partials: the staging workspace grows
+// to hold the dense one's (the larger) at D_max, and only such chains are handed the larger size (every other chain sees
+// kWsBytes, as before).
 static size_t ctx_ws_bytes(int D_max) {
   const int d = D_max < B2B_SCALE_MATRIX_MAX_D ? D_max : B2B_SCALE_MATRIX_MAX_D;
-  const size_t scale = b2b_scale_matrix_workspace(d) + 4096 * sizeof(double) + 1024;
+  const size_t scale = b2b_scale_workspace(B2B_SCALE_MATRIX, d) + 4096 * sizeof(double) + 1024;
   return scale > kWsBytes ? scale : kWsBytes;
 }
 

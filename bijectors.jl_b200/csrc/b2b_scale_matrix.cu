@@ -19,6 +19,17 @@
 // Reverse mode: x̄ by map_kernel with the transposed operand; G by the chunked outer-product kernel of the full-covariance
 // base (all tiles), its chunks and Σ l̄ summed in a fixed order in fp64, and the two D x D products of the inverse layer
 // in fp64.  No atomics; every launch is graph-capturable.
+//
+// Triangular layer, B2B_SCALE_TRIANGULAR: Scale(T) with T lower or upper triangular, stored or unit diagonal.  The same
+// launches with the structure made explicit, selected by the descriptor's kind in scale_prep:
+//   tri_prep_kernel (parallel over columns, no serial step) writes M = T or T⁻¹ in fp32, zero outside the triangle and 1
+//     on a unit diagonal, reading only the triangle of T; T⁻¹ column by column, a warp per kInvC columns with lanes over
+//     rows, one fp64 substitution against identity columns.  An extra CTA sums log|Tᵢᵢ| in row order.
+//   map_kernel<DP, BN, TRANS, TRI>: each warp owns contiguous row blocks -- one from the top and one from the bottom of
+//     the tile, so the warps' work is balanced -- and skips the k-blocks that are zero for every row of a block.
+//   reverse mode: T̄ = 𝒫(Ā) with 𝒫 the parameter's triangle (strict for the unit forms).  G is needed on 𝒫 only for the
+//     forward layer (the outer-product kernel's lower tiles; for an upper T with the operands swapped, giving Gᵀ), in full
+//     for the inverse layer; the finalize kernels take 𝒫 as an output mask ("full" for the dense layer).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -60,6 +71,22 @@ Factor carve(void* ws, int D) {
   f.perm = reinterpret_cast<int*>(p);
   p += al256(sizeof(int) * (size_t)D);
   f.logdet = reinterpret_cast<double*>(p);
+  return f;
+}
+
+// triangular storage: [M = T or T⁻¹ (D x D fp32, column-major)][log|det T| (fp64)]
+struct TriFactor {
+  float* m;
+  double* logdet;
+};
+
+size_t tri_bytes(int D) { return al256(sizeof(float) * (size_t)D * D) + al256(sizeof(double)) + 256; }
+
+TriFactor carve_tri(void* ws, int D) {
+  char* p = b2b_align256(ws);
+  TriFactor f;
+  f.m = reinterpret_cast<float*>(p);
+  f.logdet = reinterpret_cast<double*>(p + al256(sizeof(float) * (size_t)D * D));
   return f;
 }
 
@@ -258,6 +285,110 @@ __global__ void __launch_bounds__(kInvWarps * 32)
   }
 }
 
+// M = T (inv == 0) or T⁻¹ of a triangular T (lower: upper == 0), fp32, zero outside the triangle; only the triangle of T
+// is read, and not its diagonal when unit != 0.  T⁻¹ column j: the substitution of T z = e_j in fp64 (right-looking: z_k is
+// final once steps before k ran, then the rows beyond k take −T(i, k)·z_k), rows owned by lanes.  The last CTA writes
+// log|det T| = Σ log|Tᵢᵢ| in row order (0 for unit).
+template <int R>
+__global__ void __launch_bounds__(kInvWarps * 32)
+    tri_prep_kernel(const float* __restrict__ T, int D, int upper, int unit, int inv, float* __restrict__ M,
+                    double* __restrict__ logdet) {
+  const int lane = threadIdx.x & 31;
+  if (blockIdx.x == gridDim.x - 1) {
+    __shared__ double lg[32 * R];
+    if (threadIdx.x >= 32) return;
+    for (int i = lane; i < D; i += 32) lg[i] = unit ? 0.0 : log(fabs((double)T[(size_t)i * D + i]));
+    __syncwarp();
+    if (lane == 0) {
+      double s = 0.0;
+      for (int i = 0; i < D; ++i) s += lg[i];
+      *logdet = s;
+    }
+    return;
+  }
+  const int col0 = (blockIdx.x * kInvWarps + (threadIdx.x >> 5)) * kInvC;
+  if (col0 >= D) return;
+  auto in_tri = [&](int i, int j) { return upper ? i <= j : i >= j; };
+  double z[R][kInvC];
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int i = lane + 32 * r;
+#pragma unroll
+    for (int c = 0; c < kInvC; ++c) {
+      const int j = col0 + c;
+      double v = 0.0;
+      if (i < D && j < D && in_tri(i, j)) {
+        if (i == j) v = (unit || inv) ? 1.0 : (double)T[(size_t)j * D + i];
+        else if (!inv) v = (double)T[(size_t)j * D + i];
+      }
+      z[r][c] = v;
+    }
+  }
+  if (inv && !upper) {  // forward substitution from the warp's first column down
+#pragma unroll
+    for (int kb = 0; kb < R; ++kb) {
+      for (int jj = 0; jj < 32; ++jj) {
+        const int k = kb * 32 + jj;
+        if (k >= D) break;
+        if (k < col0) continue;
+        const float* Tk = T + (size_t)k * D;
+        const double tkk = unit ? 1.0 : (double)Tk[k];
+        double v[kInvC];
+#pragma unroll
+        for (int c = 0; c < kInvC; ++c) {
+          v[c] = __shfl_sync(kFull, z[kb][c], jj) / tkk;
+          if (lane == jj) z[kb][c] = v[c];
+        }
+#pragma unroll
+        for (int r = kb; r < R; ++r) {
+          const int i = lane + 32 * r;
+          if (i > k && i < D) {
+            const double l = (double)Tk[i];
+#pragma unroll
+            for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-l, v[c], z[r][c]);
+          }
+        }
+      }
+    }
+  } else if (inv) {  // back substitution from the warp's last column up
+    const int klast = col0 + kInvC - 1;
+#pragma unroll
+    for (int kb = R - 1; kb >= 0; --kb) {
+      for (int jj = 31; jj >= 0; --jj) {
+        const int k = kb * 32 + jj;
+        if (k >= D || k > klast) continue;
+        const float* Tk = T + (size_t)k * D;
+        const double tkk = unit ? 1.0 : (double)Tk[k];
+        double v[kInvC];
+#pragma unroll
+        for (int c = 0; c < kInvC; ++c) {
+          v[c] = __shfl_sync(kFull, z[kb][c], jj) / tkk;
+          if (lane == jj) z[kb][c] = v[c];
+        }
+#pragma unroll
+        for (int r = 0; r <= kb; ++r) {
+          const int i = lane + 32 * r;
+          if (i < k) {
+            const double u = (double)Tk[i];
+#pragma unroll
+            for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-u, v[c], z[r][c]);
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < kInvC; ++c) {
+    const int j = col0 + c;
+    if (j >= D) break;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int i = lane + 32 * r;
+      if (i < D) M[(size_t)j * D + i] = (float)z[r][c];
+    }
+  }
+}
+
 template <int DP, int BN>
 __host__ __device__ constexpr int map_threads() {
   return (DP / 8) * (BN / 8);
@@ -267,8 +398,38 @@ constexpr size_t map_smem() {
   return sizeof(float) * ((size_t)DP * (BN + 4) + 2 * (size_t)kBK * DP);
 }
 
-// Y = op(M) X with op(M) = M (TRANS = false) or Mᵀ; logjac[n] = lj (+ logjac[n]) when logjac != NULL
-template <int DP, int BN, bool TRANS>
+// acc[u][v] += a[u]·b[v] over one k-block for the rows u in [U0, U1) of a thread of the triangular map: rows u < 4 from
+// the low block (first row r0), u >= 4 from the high block (r1)
+template <int U0, int U1, int DP, int BN>
+__device__ __forceinline__ void map_block(float (&acc)[8][8], const float* Mb, const float* Xb, int r0, int r1, int tx) {
+  constexpr int XS = BN + 4;
+#pragma unroll
+  for (int kk = 0; kk < kBK; ++kk) {
+    float a[8];
+    if (U0 == 0) {
+      const float4 a0 = *reinterpret_cast<const float4*>(Mb + kk * DP + r0);
+      a[0] = a0.x, a[1] = a0.y, a[2] = a0.z, a[3] = a0.w;
+    }
+    if (U1 == 8) {
+      const float4 a1 = *reinterpret_cast<const float4*>(Mb + kk * DP + r1);
+      a[4] = a1.x, a[5] = a1.y, a[6] = a1.z, a[7] = a1.w;
+    }
+    const float4 b0 = *reinterpret_cast<const float4*>(Xb + kk * XS + tx * 4);
+    const float4 b1 = *reinterpret_cast<const float4*>(Xb + kk * XS + BN / 2 + tx * 4);
+    const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+    for (int u = U0; u < U1; ++u)
+#pragma unroll
+      for (int v = 0; v < 8; ++v) acc[u][v] = fmaf(a[u], b[v], acc[u][v]);
+  }
+}
+
+// Y = op(M) X with op(M) = M (TRANS = false) or Mᵀ; logjac[n] = lj (+ logjac[n]) when logjac != NULL.  TRI = 0: dense M;
+// TRI = 1 / 2: op(M) is lower / upper triangular, and row i reads k <= i / k >= i only.  Then warp w owns the low row
+// block [w·H, (w+1)·H) and the high block [DP − (w+1)·H, DP − w·H), H = DP / (2·warps), so every warp has the same share
+// of the triangle, and a block is skipped on the k-blocks that are zero for all its rows.  A skipped k-block would only
+// add ±0 products to each chain, so the results are those of the dense map on the same M.
+template <int DP, int BN, bool TRANS, int TRI = 0>
 __global__ void __launch_bounds__(map_threads<DP, BN>(), 1)
     map_kernel(const float* __restrict__ M, const float* x, long long ldx, float* y, long long ldy, float* logjac,
                int accumulate, const double* __restrict__ logdet, float lj_sign, int D, long long N) {
@@ -276,7 +437,10 @@ __global__ void __launch_bounds__(map_threads<DP, BN>(), 1)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* Xs = reinterpret_cast<float*>(smem_raw);  // Xs[k * XS + n]
   float* Ms = Xs + (size_t)DP * XS;                // Ms[buf][kk * DP + i] = op(M)(i, k0 + kk)
-  const int tid = threadIdx.x, ty = tid % (DP / 8), tx = tid / (DP / 8);
+  constexpr int H = DP / (2 * (T / 32));  // rows of a warp's block (TRI)
+  static_assert(TRI == 0 || H == 4 * (32 / (BN / 8)), "a warp's row block is its thread groups' 4 rows each");
+  const int tid = threadIdx.x, ty = TRI ? tid % 32 / (BN / 8) : tid % (DP / 8), tx = TRI ? tid % (BN / 8) : tid / (DP / 8);
+  const int lo_base = TRI ? tid / 32 * H : 0, hi_base = TRI ? DP - (tid / 32 + 1) * H : 0;  // the warp's row blocks
   const long long n0 = (long long)blockIdx.x * BN;
   const int Kp = (D + kBK - 1) / kBK * kBK, KB = Kp / kBK;
   float pre[PER];
@@ -324,18 +488,28 @@ __global__ void __launch_bounds__(map_threads<DP, BN>(), 1)
     if (kb + 1 < KB) fetch(kb + 1);
     const float* Mb = Ms + (kb & 1) * kBK * DP;
     const float* Xb = Xs + (size_t)kb * kBK * XS;
+    if constexpr (TRI == 0) {
 #pragma unroll
-    for (int kk = 0; kk < kBK; ++kk) {
-      const float4 a0 = *reinterpret_cast<const float4*>(Mb + kk * DP + ty * 4);
-      const float4 a1 = *reinterpret_cast<const float4*>(Mb + kk * DP + DP / 2 + ty * 4);
-      const float4 b0 = *reinterpret_cast<const float4*>(Xb + kk * XS + tx * 4);
-      const float4 b1 = *reinterpret_cast<const float4*>(Xb + kk * XS + BN / 2 + tx * 4);
-      const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-      const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+      for (int kk = 0; kk < kBK; ++kk) {
+        const float4 a0 = *reinterpret_cast<const float4*>(Mb + kk * DP + ty * 4);
+        const float4 a1 = *reinterpret_cast<const float4*>(Mb + kk * DP + DP / 2 + ty * 4);
+        const float4 b0 = *reinterpret_cast<const float4*>(Xb + kk * XS + tx * 4);
+        const float4 b1 = *reinterpret_cast<const float4*>(Xb + kk * XS + BN / 2 + tx * 4);
+        const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
-      for (int u = 0; u < 8; ++u)
+        for (int u = 0; u < 8; ++u)
 #pragma unroll
-        for (int v = 0; v < 8; ++v) acc[u][v] = fmaf(a[u], b[v], acc[u][v]);
+          for (int v = 0; v < 8; ++v) acc[u][v] = fmaf(a[u], b[v], acc[u][v]);
+      }
+    } else {  // warp-uniform: whether each row block meets a non-zero of this k-block
+      const int k0 = kb * kBK, k1 = k0 + kBK - 1;
+      const bool lo = lo_base < D && (TRI == 1 ? k0 <= lo_base + H - 1 : k1 >= lo_base);
+      const bool hi = hi_base < D && (TRI == 1 ? k0 <= hi_base + H - 1 : k1 >= hi_base);
+      const int r0 = lo_base + ty * 4, r1 = hi_base + ty * 4;
+      if (lo && hi) map_block<0, 8, DP, BN>(acc, Mb, Xb, r0, r1, tx);
+      else if (lo) map_block<0, 4, DP, BN>(acc, Mb, Xb, r0, r1, tx);
+      else if (hi) map_block<4, 8, DP, BN>(acc, Mb, Xb, r0, r1, tx);
     }
     if (kb + 1 < KB) stash((kb + 1) & 1);
     __syncthreads();
@@ -346,7 +520,7 @@ __global__ void __launch_bounds__(map_threads<DP, BN>(), 1)
     if (col >= N) continue;
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
-      const int i = u < 4 ? ty * 4 + u : DP / 2 + ty * 4 + u - 4;
+      const int i = TRI ? (u < 4 ? lo_base : hi_base) + ty * 4 + (u & 3) : (u < 4 ? ty * 4 + u : DP / 2 + ty * 4 + u - 4);
       if (i < D) y[col * ldy + i] = acc[u][v];
     }
   }
@@ -382,39 +556,67 @@ __global__ void __launch_bounds__(1024) ljsum_kernel(const float* __restrict__ l
   if (threadIdx.x == 0) *out = red[0];
 }
 
+// Output masks of the finalize kernels: kMaskFull (the dense layer) or kMaskTri | upper·kMaskUpper | unit·kMaskStrict, the
+// triangle 𝒫 of a triangular T's parameters (strict for a unit diagonal).
+constexpr int kMaskFull = 0, kMaskTri = 1, kMaskUpper = 2, kMaskStrict = 4;
+
+__device__ __forceinline__ bool in_mask(int mask, int i, int j) {
+  if (mask == kMaskFull) return true;
+  if (mask & kMaskUpper) return (mask & kMaskStrict) ? i < j : i <= j;
+  return (mask & kMaskStrict) ? i > j : i >= j;
+}
+
 // forward layer: Ā = Σ_p part[p] + s·B;  inverse layer: Gd = Σ_p part[p] (fp64).  B(i, j) = A⁻¹(j, i) = minv[i·D + j].
+// Triangular forward layer (mask != kMaskFull): T̄ = 𝒫(Σ_p part[p] + s·B), 0 elsewhere, with minv = T, so B's diagonal is
+// 1/Tᵢᵢ and 𝒫 keeps nothing else of it; for an upper T the chunks hold Gᵀ and are read transposed.
 __global__ void __launch_bounds__(256) gsum_kernel(const float* __restrict__ part, int P, const double* __restrict__ ljs,
-                                                   const float* __restrict__ minv, int D, float* __restrict__ Abar,
+                                                   const float* __restrict__ minv, int D, int mask, float* __restrict__ Abar,
                                                    double* __restrict__ Gd) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x, DD = (long long)D * D;
   if (idx >= DD) return;
+  const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
+  if (!Gd && !in_mask(mask, i, j)) {
+    Abar[idx] = 0.f;
+    return;
+  }
+  const long long src = (!Gd && (mask & kMaskUpper)) ? (long long)i * D + j : idx;
   double a = 0.0;
-  for (int p = 0; p < P; ++p) a += (double)part[(size_t)p * DD + idx];
+  for (int p = 0; p < P; ++p) a += (double)part[(size_t)p * DD + src];
   if (Gd) {
     Gd[idx] = a;
     return;
   }
-  const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
-  Abar[idx] = (float)(a + *ljs * (double)minv[(size_t)i * D + j]);
+  if (mask == kMaskFull) Abar[idx] = (float)(a + *ljs * (double)minv[(size_t)i * D + j]);
+  else Abar[idx] = (float)(i == j && !(mask & kMaskStrict) ? a + *ljs / (double)minv[(size_t)i * D + i] : a);
 }
 
-// T = Gd · B (fp64, column-major)
+// T = Gd · B (fp64, column-major).  With a triangular mask only the triangle the final product reads (𝒫 with its diagonal),
+// zeros elsewhere.
 __global__ void __launch_bounds__(256) prod_gb_kernel(const double* __restrict__ Gd, const float* __restrict__ minv, int D,
-                                                      double* __restrict__ Tm) {
+                                                      int mask, double* __restrict__ Tm) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)D * D) return;
   const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
+  if (!in_mask(mask & ~kMaskStrict, i, j)) {
+    Tm[idx] = 0.0;
+    return;
+  }
   double a = 0.0;
   for (int k = 0; k < D; ++k) a = fma(Gd[(size_t)k * D + i], (double)minv[(size_t)k * D + j], a);
   Tm[idx] = a;
 }
 
-// inverse layer: Ā = −B · T − s·B
+// inverse layer: Ā = −B · T − s·B, on the mask (0 elsewhere)
 __global__ void __launch_bounds__(256) final_inv_kernel(const double* __restrict__ Tm, const float* __restrict__ minv,
-                                                        const double* __restrict__ ljs, int D, float* __restrict__ Abar) {
+                                                        const double* __restrict__ ljs, int D, int mask,
+                                                        float* __restrict__ Abar) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)D * D) return;
   const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
+  if (!in_mask(mask, i, j)) {
+    Abar[idx] = 0.f;
+    return;
+  }
   double a = 0.0;
   for (int k = 0; k < D; ++k) a = fma((double)minv[(size_t)i * D + k], Tm[(size_t)j * D + k], a);
   Abar[idx] = (float)(-a - *ljs * (double)minv[(size_t)i * D + j]);
@@ -438,11 +640,25 @@ int launch_factor(const b2b_layer_desc& d, const Factor& f, int D, bool want_inv
   return B2B_OK;
 }
 
-template <int DP, int BN, bool TRANS>
+// M = T or T⁻¹ and log|det T| of a triangular layer, one launch
+int launch_tri_prep(const b2b_layer_desc& d, const TriFactor& f, int D, int* launches, cudaStream_t stream) {
+  const int grid = (D + kInvWarps * kInvC - 1) / (kInvWarps * kInvC) + 1;  // + the log|det T| CTA
+  const int up = d.n0, unit = d.n1, inv = d.inverse != 0;
+  if (D <= 32) tri_prep_kernel<1><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, D, up, unit, inv, f.m, f.logdet);
+  else if (D <= 64) tri_prep_kernel<2><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, D, up, unit, inv, f.m, f.logdet);
+  else if (D <= 128) tri_prep_kernel<4><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, D, up, unit, inv, f.m, f.logdet);
+  else tri_prep_kernel<8><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, D, up, unit, inv, f.m, f.logdet);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  ++*launches;
+  return B2B_OK;
+}
+
+template <int DP, int BN, bool TRANS, int TRI>
 int launch_map_t(const float* M, const float* x, long long ldx, float* y, long long ldy, float* logjac, int accumulate,
                  const double* logdet, float sign, int D, long long N, cudaStream_t stream) {
   constexpr size_t smem = map_smem<DP, BN>();
-  auto k = map_kernel<DP, BN, TRANS>;
+  auto k = map_kernel<DP, BN, TRANS, TRI>;
   cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   const long long grid = (N + BN - 1) / BN;
@@ -450,53 +666,86 @@ int launch_map_t(const float* M, const float* x, long long ldx, float* y, long l
   return (int)cudaGetLastError();
 }
 
+template <bool TRANS, int TRI>
+int launch_map_d(const float* M, const float* x, long long ldx, float* y, long long ldy, float* logjac, int accumulate,
+                 const double* logdet, float sign, int D, long long N, cudaStream_t stream) {
+  if (D <= 32) return launch_map_t<32, 128, TRANS, TRI>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+  if (D <= 64) return launch_map_t<64, 128, TRANS, TRI>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+  if (D <= 128) return launch_map_t<128, 128, TRANS, TRI>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+  return launch_map_t<256, 64, TRANS, TRI>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+}
+
+// Y = op(M) X with op(M) = M or (TRANS) Mᵀ, where M is dense (tri = 0) or lower / upper triangular (tri = 1 / 2)
 template <bool TRANS>
-int launch_map(const float* M, const float* x, long long ldx, float* y, long long ldy, float* logjac, int accumulate,
-               const double* logdet, float sign, int D, long long N, cudaStream_t stream) {
-  if (D <= 32) return launch_map_t<32, 128, TRANS>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
-  if (D <= 64) return launch_map_t<64, 128, TRANS>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
-  if (D <= 128) return launch_map_t<128, 128, TRANS>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
-  return launch_map_t<256, 64, TRANS>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+int launch_map(int tri, const float* M, const float* x, long long ldx, float* y, long long ldy, float* logjac,
+               int accumulate, const double* logdet, float sign, int D, long long N, cudaStream_t stream) {
+  if (tri == 0) return launch_map_d<TRANS, 0>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+  if ((tri == 1) != TRANS) return launch_map_d<TRANS, 1>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+  return launch_map_d<TRANS, 2>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
+}
+
+// What the launches after the prep need, for either kind: the map operand M (A, A⁻¹, T or T⁻¹), the B = M⁻ᵀ source of the
+// finalize kernels, log|det|, the structure of M for the map and the output mask of the cotangent.
+struct ScaleOp {
+  const float* M;
+  const float* minv;
+  double* logdet;
+  int tri;   // 0 dense, 1 lower, 2 upper
+  int mask;  // kMaskFull or the triangle 𝒫
+};
+
+size_t prep_bytes(int kind, int D) { return kind == B2B_SCALE_TRIANGULAR ? tri_bytes(D) : factor_bytes(D); }
+
+// The prep launches of the layer `d` (the descriptor's kind decides them here, and nowhere else): the dense layer's LU, and
+// A⁻¹ when `want_inverse`; the triangular layer's M (always: its map must not read the entries outside the triangle).
+int scale_prep(const b2b_layer_desc& d, void* ws, int D, bool want_inverse, ScaleOp* op, int* launches,
+               cudaStream_t stream) {
+  const bool inv = d.inverse != 0;
+  if (d.kind == B2B_SCALE_TRIANGULAR) {
+    const TriFactor f = carve_tri(ws, D);
+    *op = ScaleOp{f.m, f.m, f.logdet, d.n0 ? 2 : 1, kMaskTri | (d.n0 ? kMaskUpper : 0) | (d.n1 ? kMaskStrict : 0)};
+    return launch_tri_prep(d, f, D, launches, stream);
+  }
+  const Factor f = carve(ws, D);
+  *op = ScaleOp{inv ? f.minv : d.p0, f.minv, f.logdet, 0, kMaskFull};
+  return launch_factor(d, f, D, want_inverse, launches, stream);
 }
 
 }  // namespace b2b_scale
 
 using namespace b2b_scale;
 
-size_t b2b_scale_matrix_workspace(int D) {
-  return D >= 1 && D <= B2B_SCALE_MATRIX_MAX_D ? factor_bytes(D) : 0;
-}
+size_t b2b_scale_workspace(int kind, int D) { return D >= 1 && D <= B2B_SCALE_MATRIX_MAX_D ? prep_bytes(kind, D) : 0; }
 
 int b2b_fwd_scale(const B2BFwdSeg& s) {
   const b2b_layer_desc& d = s.layers[0];
   const int D = s.D;
-  if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-  if (!s.workspace || s.workspace_bytes < factor_bytes(D)) return B2B_EWORKSPACE;
-  const Factor f = carve(s.workspace, D);
+  if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;  // = B2B_SCALE_TRIANGULAR_MAX_D
+  if (!s.workspace || s.workspace_bytes < prep_bytes(d.kind, D)) return B2B_EWORKSPACE;
   const bool inv = d.inverse != 0;
-  int rc = launch_factor(d, f, D, inv && s.y, s.launches, s.stream);
+  ScaleOp op;
+  int rc = scale_prep(d, s.workspace, D, inv && s.y, &op, s.launches, s.stream);
   if (rc != B2B_OK) return rc;
   const float sign = inv ? -1.f : 1.f;
   if (!s.y) {  // log-Jacobians only
     if (!s.logjac) return B2B_OK;
     long long g = (s.N + 255) / 256;
-    logjac_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, s.stream>>>(s.logjac, s.accumulate, f.logdet, sign, s.N);
+    logjac_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, s.stream>>>(s.logjac, s.accumulate, op.logdet, sign, s.N);
     if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
     ++*s.launches;
     return B2B_OK;
   }
-  rc = launch_map<false>(inv ? f.minv : d.p0, s.x, s.ldx, s.y, s.ldy, s.logjac, s.accumulate, f.logdet, sign, D, s.N,
-                         s.stream);
+  rc = launch_map<false>(op.tri, op.M, s.x, s.ldx, s.y, s.ldy, s.logjac, s.accumulate, op.logdet, sign, D, s.N, s.stream);
   if (rc != B2B_OK) return rc;
   ++*s.launches;
   return B2B_OK;
 }
 
 // workspace: [factor storage][chunk partials of G (P x D x D fp32)][Gd, T (D x D fp64 each)][Σ l̄ (fp64)]
-size_t b2b_scale_matrix_vjp_workspace(int D, long long N) {
+size_t b2b_scale_vjp_workspace(int kind, int D, long long N) {
   if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D || N < 0) return 0;
   const long long clen = b2b_outer_chunk_len(N), P = N > 0 ? (N + clen - 1) / clen : 1;
-  return factor_bytes(D) + al256(sizeof(float) * (size_t)P * D * D) + 2 * al256(sizeof(double) * (size_t)D * D) +
+  return prep_bytes(kind, D) + al256(sizeof(float) * (size_t)P * D * D) + 2 * al256(sizeof(double) * (size_t)D * D) +
          al256(sizeof(double));
 }
 
@@ -511,10 +760,9 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   int* const launches = s.launches;
   const cudaStream_t stream = s.stream;
   if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
-  if (!workspace || s.workspace_bytes < b2b_scale_matrix_vjp_workspace(D, N)) return B2B_EWORKSPACE;
-  const Factor f = carve(workspace, D);
-  const bool inv = d.inverse != 0;
-  char* ws = static_cast<char*>(workspace) + factor_bytes(D);
+  if (!workspace || s.workspace_bytes < b2b_scale_vjp_workspace(d.kind, D, N)) return B2B_EWORKSPACE;
+  const bool inv = d.inverse != 0, tri = d.kind == B2B_SCALE_TRIANGULAR;
+  char* ws = static_cast<char*>(workspace) + prep_bytes(d.kind, D);
   const long long clen = b2b_outer_chunk_len(N), P = (N + clen - 1) / clen;
   float* part = reinterpret_cast<float*>(ws);
   ws += al256(sizeof(float) * (size_t)P * D * D);
@@ -524,13 +772,16 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   ws += al256(sizeof(double) * (size_t)D * D);
   double* ljs = reinterpret_cast<double*>(ws);
   int rc = B2B_OK;
-  if (inv || Abar) {
-    rc = launch_factor(d, f, D, true, launches, stream);
+  ScaleOp op{};
+  if (tri || inv || Abar) {
+    rc = scale_prep(d, workspace, D, true, &op, launches, stream);
     if (rc != B2B_OK) return rc;
+  } else {
+    op.M = d.p0;  // the dense forward layer's x̄ needs A only
   }
   // x̄ = op(M)ᵀ ȳ
   if (ybar) {
-    rc = launch_map<true>(inv ? f.minv : d.p0, ybar, ldyb, xbar, ldxb, nullptr, 0, nullptr, 0.f, D, N, stream);
+    rc = launch_map<true>(op.tri, op.M, ybar, ldyb, xbar, ldxb, nullptr, 0, nullptr, 0.f, D, N, stream);
     if (rc != B2B_OK) return rc;
   } else {
     rc = (int)cudaMemset2DAsync(xbar, (size_t)ldxb * sizeof(float), 0, (size_t)D * sizeof(float), (size_t)N, stream);
@@ -539,7 +790,11 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   ++*launches;
   if (!Abar) return B2B_OK;
   if (ybar) {
-    rc = b2b_launch_outer_chunks(ybar, ldyb, x, ldx, part, nullptr, D, N, false, stream);
+    if (tri && !inv)  // G on 𝒫 only: the lower tiles of G, or of Gᵀ (operands swapped) for an upper T
+      rc = d.n0 ? b2b_launch_outer_chunks(x, ldx, ybar, ldyb, part, nullptr, D, N, true, stream)
+                : b2b_launch_outer_chunks(ybar, ldyb, x, ldx, part, nullptr, D, N, true, stream);
+    else
+      rc = b2b_launch_outer_chunks(ybar, ldyb, x, ldx, part, nullptr, D, N, false, stream);
     if (rc != B2B_OK) return rc;
     ++*launches;
   }
@@ -548,13 +803,13 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   ++*launches;
   const long long DD = (long long)D * D;
   const unsigned g = (unsigned)((DD + 255) / 256);
-  gsum_kernel<<<g, 256, 0, stream>>>(part, ybar ? (int)P : 0, ljs, f.minv, D, Abar, inv ? Gd : nullptr);
+  gsum_kernel<<<g, 256, 0, stream>>>(part, ybar ? (int)P : 0, ljs, op.minv, D, op.mask, Abar, inv ? Gd : nullptr);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
   ++*launches;
   if (!inv) return B2B_OK;
-  prod_gb_kernel<<<g, 256, 0, stream>>>(Gd, f.minv, D, Tm);
+  prod_gb_kernel<<<g, 256, 0, stream>>>(Gd, op.minv, D, op.mask, Tm);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
-  final_inv_kernel<<<g, 256, 0, stream>>>(Tm, f.minv, ljs, D, Abar);
+  final_inv_kernel<<<g, 256, 0, stream>>>(Tm, op.minv, ljs, D, op.mask, Abar);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
   *launches += 2;
   return B2B_OK;

@@ -835,6 +835,7 @@ _SLOTS = {
     _lib.MVNORMAL_TRIL: (("μ", "L"), lambda d, D: ((D,), (D, D)), (1,)),
     _lib.COUPLING_RQS: (("W", "c"), _coupling_slots, (0,)),
     _lib.SCALE_MATRIX: (("a",), lambda d, D: ((D, D),), (0,)),
+    _lib.SCALE_TRIANGULAR: (("a",), lambda d, D: ((D, D),), (0,)),
     _lib.COUPLING_MLP: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),

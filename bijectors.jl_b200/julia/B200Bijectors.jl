@@ -21,7 +21,7 @@ import Bijectors: transform, logabsdetjac, with_logabsdet_jacobian
 import Distributions
 using Distributions: MvNormal
 using PDMats: PDMat, PDiagMat, ScalMat
-using LinearAlgebra: LowerTriangular, cholesky, diagind
+using LinearAlgebra: LowerTriangular, UpperTriangular, UnitLowerTriangular, UnitUpperTriangular, cholesky, diagind
 using Functors: fmap
 using SparseArrays: findnz
 using Statistics: mean, var
@@ -47,6 +47,8 @@ const COUPLING_MLP_RQS = Int32(14)
 const COUPLING_DEEP_MLP = Int32(15)
 const COUPLING_DEEP_MLP_RQS = Int32(16)
 const ELEMENTWISE_VEC = Int32(17)
+const SCALE_TRIANGULAR = Int32(18)
+const SCALE_TRIANGULAR_MAX_D = 256
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -307,6 +309,18 @@ desc(b::VectorLaw{CuVector{Float32}}, inv::Bool) =
     LayerDesc(ELEMENTWISE_VEC, inv, vec_code(b), 0, 0, 0, 0f0, 0f0, pointer(vec_param(b)), NULLF, NULLF, NULLF, NULLI, NULLI)
 desc(b::VectorLaw{CuVector{Float64}}, inv::Bool) =
     LayerDesc64(ELEMENTWISE_VEC, inv, vec_code(b), 0, 0, 0, 0.0, 0.0, pointer(vec_param(b)), NULLD, NULLD, NULLD, NULLI, NULLI)
+# Scale(T) with T a LinearAlgebra triangular view of a CuMatrix (scale.jl:14,17,35-36): the parent matrix, column-major, with
+# n0 = upper and n1 = unit diagonal; only the triangle is read.  Float32 (D <= 256) or Float64 (D <= 2048).
+const TriMat{T} = Union{LowerTriangular{T,<:CuMatrix{T}},UpperTriangular{T,<:CuMatrix{T}},
+                        UnitLowerTriangular{T,<:CuMatrix{T}},UnitUpperTriangular{T,<:CuMatrix{T}}}
+tri_upper(a) = Int32(a isa Union{UpperTriangular,UnitUpperTriangular})
+tri_unit(a) = Int32(a isa Union{UnitLowerTriangular,UnitUpperTriangular})
+desc(b::Scale{<:TriMat{Float32}}, inv::Bool) =
+    LayerDesc(SCALE_TRIANGULAR, inv, tri_upper(b.a), tri_unit(b.a), 0, 0, 0f0, 0f0, pointer(parent(b.a)), NULLF, NULLF, NULLF,
+              NULLI, NULLI)
+desc(b::Scale{<:TriMat{Float64}}, inv::Bool) =
+    LayerDesc64(SCALE_TRIANGULAR, inv, tri_upper(b.a), tri_unit(b.a), 0, 0, 0.0, 0.0, pointer(parent(b.a)), NULLD, NULLD, NULLD,
+                NULLI, NULLI)
 # a whole-column elementwise law is a one-block Stacked
 const ElementwiseLaw = Union{Shift{<:Real},Scale{<:Real},LeakyReLU{<:Real},Logit{<:Real,<:Real},TruncatedBijector{<:Real,<:Real}}
 
@@ -321,7 +335,7 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}},
-                          Scale{<:CuMatrix{Float32}},VectorLaw{CuVector{Float32}},Permute,Stacked}
+                          Scale{<:CuMatrix{Float32}},Scale{<:TriMat{Float32}},VectorLaw{CuVector{Float32}},Permute,Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
 is_device(::DeviceLeaf) = true
@@ -544,6 +558,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
         return (z(H, d.n1), d.p1 == NULLF ? nothing : z(H), z(J, H), d.p3 == NULLF ? nothing : z(J))
     end
     d.kind == SCALE_MATRIX && return (z(D, D),)
+    d.kind == SCALE_TRIANGULAR && return (z(D, D),)  # exactly 0 outside the triangle; leaf_tangent wraps it
     d.kind == ELEMENTWISE_VEC && return (z(D),)  # Shift / Scale a, LeakyReLU α
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
@@ -681,6 +696,9 @@ function leaf_tangent(b, bar)
     names = fieldnames(typeof(b))
     return ChainRulesCore.Tangent{typeof(b)}(; (names[i] => bar[i] for i in eachindex(bar) if bar[i] !== nothing)...)
 end
+# a triangular Scale's T̄ in the triangular type of its field
+leaf_tangent(b::Scale{<:TriMat}, bar) =
+    bar[1] === nothing ? NoTangent() : ChainRulesCore.Tangent{typeof(b)}(a=Base.typename(typeof(b.a)).wrapper(bar[1]))
 # The base: μ̄, and the covariance's tangent from σ̄ or L̄ (Σ = diag(σ²): Σ̄ᵢᵢ = σ̄ᵢ/(2σᵢ); Σ = L Lᵀ: Σ̄ = sym(L⁻ᵀ Φ(Lᵀ L̄) L⁻¹)/2,
 # Φ the lower triangle with its diagonal halved).
 function base_tangent(d::MvNormal, (μ̄, p̄))

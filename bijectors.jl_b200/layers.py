@@ -8,6 +8,7 @@ launch of the matching libb2b.so kernel (include/b2b.h).  No arithmetic on the b
   InvertibleBatchNorm                src/bijectors/normalise.jl:9-37
   Permute                            src/bijectors/permute.jl:84-157
   Stacked / elementwise / Shift / Scale   src/bijectors/stacked.jl, exp_log.jl, shift.jl, scale.jl
+  LowerTriangular / UpperTriangular / UnitLowerTriangular / UnitUpperTriangular   LinearAlgebra's wrappers, for Scale(T)
   LeakyReLU                          src/bijectors/leaky_relu.jl
 """
 from __future__ import annotations
@@ -843,6 +844,40 @@ class Shift(_ElementwiseLaw):
         return Shift(-self.a)  # shift.jl:12
 
 
+class _Triangular:
+    """LinearAlgebra's triangular view of a square matrix: only the triangle is read, and the unit forms take the diagonal
+    as 1 without reading it.  `Scale` of one is the triangular layer (B2B_SCALE_TRIANGULAR); the wrapper itself only
+    holds the matrix."""
+
+    upper: bool
+    unit: bool
+
+    def __init__(self, data):
+        shape = tuple(data.shape) if isinstance(data, torch.Tensor) else np.shape(data)
+        if len(shape) != 2 or shape[0] != shape[1]:
+            raise ValueError(f"DimensionMismatch: {type(self).__name__} needs a square matrix, got {shape}")
+        self.data = data
+
+    def __repr__(self):
+        return f"{type(self).__name__}({self.data!r})"
+
+
+class LowerTriangular(_Triangular):
+    upper, unit = False, False
+
+
+class UpperTriangular(_Triangular):
+    upper, unit = True, False
+
+
+class UnitLowerTriangular(_Triangular):
+    upper, unit = False, True
+
+
+class UnitUpperTriangular(_Triangular):
+    upper, unit = True, True
+
+
 class Scale(_ElementwiseLaw):
     """Scale(a): y = a .* x, logjac = log|a| per element (scale.jl:1-39) for a scalar `a` (also a Stacked block) or a
     trainable vector a[D] (scale.jl:16,31-32).
@@ -850,11 +885,23 @@ class Scale(_ElementwiseLaw):
     A square matrix `a` gives the dense layer Scale{<:AbstractMatrix} (scale.jl:14,17,35-36): y = A x, inverse A \\ y,
     logjac = logabsdet(A)[1] per column, with A trainable (B2B_SCALE_MATRIX; Float32 only, D <= 256).  The device tensor
     `_A` holds A column-major, i.e. Aᵀ row-major (as MvNormal's scale_tril); `.a` returns A in the user's orientation.
-    A singular A is the caller's responsibility: the forward gives logjac = −Inf, the inverse non-finite values."""
+    A singular A is the caller's responsibility: the forward gives logjac = −Inf, the inverse non-finite values.
+
+    A `LowerTriangular`, `UpperTriangular`, `UnitLowerTriangular` or `UnitUpperTriangular` `a` gives the triangular layer
+    (B2B_SCALE_TRIANGULAR; Float32 D <= 256 or Float64 D <= 2048): y = T x, inverse a triangular solve, logjac = Σ log|Tᵢᵢ|
+    (0 for the unit forms), reading only the triangle.  `_A` holds T column-major as for the dense form, its entries
+    outside the triangle as given (training never changes them: T̄ is 0 there); `.a` returns the wrapper."""
 
     code = _lib.EW_SCALE
 
     def __init__(self, a, device="cuda", dtype=torch.float32):
+        self._tri = None
+        if isinstance(a, _Triangular):
+            T = a.data.detach() if isinstance(a.data, torch.Tensor) else torch.as_tensor(np.asarray(a.data, dtype=np.float64))
+            self._A = _dev_f32(T.t(), device, dtype)
+            self._tri = type(a)
+            self._a = self._s = None
+            return
         if (a.dim() if isinstance(a, torch.Tensor) else np.ndim(a)) == 2:
             if dtype != torch.float32:
                 raise TypeError(f"a dense Scale has Float32 parameters only, got {dtype}")
@@ -869,43 +916,51 @@ class Scale(_ElementwiseLaw):
 
     @property
     def dense(self) -> bool:
-        return self._A is not None
+        return self._A is not None and self._tri is None
+
+    @property
+    def triangular(self) -> bool:
+        return self._tri is not None
 
     @property
     def a(self):
+        if self.triangular:
+            return self._tri(self._A.t())
         return self._A.t() if self.dense else _ElementwiseLaw.a.fget(self)
 
     @property
     def device(self):
-        return self._A.device if self.dense else self._a.device
+        return self._A.device if self._A is not None else self._a.device
 
     def to(self, device):
         new = object.__new__(Scale)
         new.__dict__.update(self.__dict__)
-        if self.dense:
+        if self._A is not None:
             new._A = self._A.to(device)
         elif self.vector:
             new._a = self._a.to(device)
         return new
 
     def _keepalive(self):
-        return (self._A,) if self.dense else _ElementwiseLaw._keepalive(self)
+        return (self._A,) if self._A is not None else _ElementwiseLaw._keepalive(self)
 
     def _inverse(self):
         return Inverse(self)  # the scalar form included, as before: the inverse flag on the same table
 
     def _descs(self, inverse, D, dtype=torch.float32):
-        if not self.dense:
+        if self._A is None:
             return _ElementwiseLaw._descs(self, inverse, D, dtype)
         if D != self._A.shape[0]:
             raise ValueError(f"DimensionMismatch: Scale has a {self._A.shape[0]} x {self._A.shape[0]} matrix, input has {D} dims")
         _check_dtype(self._A, dtype, "Scale")
+        if self.triangular:
+            return [_desc(_lib.SCALE_TRIANGULAR, inverse, n0=int(self._tri.upper), n1=int(self._tri.unit), p0=self._A)]
         return [_desc(_lib.SCALE_MATRIX, inverse, p0=self._A)]
 
     def __eq__(self, o):
-        if not isinstance(o, Scale) or self.dense != o.dense:
+        if not isinstance(o, Scale) or self.dense != o.dense or self._tri is not o._tri:
             return False
-        return torch.equal(self._A.cpu(), o._A.cpu()) if self.dense else _ElementwiseLaw.__eq__(self, o)
+        return torch.equal(self._A.cpu(), o._A.cpu()) if self._A is not None else _ElementwiseLaw.__eq__(self, o)
 
     __hash__ = object.__hash__
 
@@ -984,7 +1039,7 @@ class Stacked(Transform):
         for b in bs:
             if not isinstance(b, (Elementwise, Shift, Scale, LeakyReLU, Logit, TruncatedBijector)) and b is not None:
                 raise B2BError(_lib.B2B_EUNSUPPORTED, f"Stacked block {type(b).__name__}")
-            if isinstance(b, Scale) and b.dense:
+            if isinstance(b, Scale) and b._A is not None:
                 raise B2BError(_lib.B2B_EUNSUPPORTED, "Stacked block Scale with a matrix (a dense layer acts on whole columns)")
             if isinstance(b, _ElementwiseLaw) and b.vector:
                 raise B2BError(_lib.B2B_EUNSUPPORTED, f"Stacked block {type(b).__name__} with a vector (one law on whole columns)")

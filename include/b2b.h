@@ -109,6 +109,10 @@ extern "C" {
 #define B2B_COUPLING_DEEP_MLP_RQS_MAX_DEPTH 4
 #define B2B_COUPLING_DEEP_MLP_RQS_MAX_D 1024
 #define B2B_ELEMENTWISE_VEC 17 /* Shift(a) / Scale(a) / LeakyReLU(a) with a trainable vector a[D]   shift.jl, scale.jl:16,31-32, leaky_relu.jl:25-29 */
+#define B2B_SCALE_TRIANGULAR 18 /* Scale(T), T triangular (Lower/Upper/UnitLower/UnitUpperTriangular): y = T*x, logjac = Σ log|Tᵢᵢ|  scale.jl:14,17,35-36 */
+/* Envelope of B2B_SCALE_TRIANGULAR: Float32 D <= 256 (the Float64 entry points: D <= 2048).  Beyond it every entry point
+ * returns B2B_EUNSUPPORTED with nothing launched and the workspace queries return 0. */
+#define B2B_SCALE_TRIANGULAR_MAX_D 256
 /* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and
  * B2B_COUPLING_DEEP_MLP_RQS (descriptor field n3) */
 #define B2B_ACT_TANH 0
@@ -217,6 +221,16 @@ extern "C" {
  *                     same a gives the same bits.  It fuses into column-local launches like STACKED_EW (same 3Dp staging,
  *                     D <= 1024), runs in both precisions, and trains a: slot 0 of b2b_chain_vjp_f32 / _f64.  a > 0 for
  *                     LeakyReLU is the caller's contract; nothing on the device checks it.)
+ * SCALE_TRIANGULAR   T[D x D]    -           -           -        -               -             tri   unit -
+ *                    (T column-major, required.  n0 = 0: lower, 1: upper -- only that triangle is read; n1 = 0: the stored
+ *                     diagonal, 1: a unit diagonal, taken as 1 and not read.  Any other n0 / n1 returns B2B_EINVAL.  Entries
+ *                     outside what is read may hold anything, NaN included.  Per column y = T x with logjac = Σᵢ log|Tᵢᵢ|,
+ *                     summed in fp64 in row order and rounded once (0 for the unit forms); inverse != 0 gives y = T⁻¹ x
+ *                     with the negated log-Jacobian.  A zero diagonal is the caller's contract, as an invertible A is for
+ *                     SCALE_MATRIX.  A prep launch writes the triangle of T (forward) or of T⁻¹ (inverse, D independent
+ *                     fp64 substitutions rounded to fp32) with zeros elsewhere; the map is exact fp32 FMA over the
+ *                     triangle only.  Float32 D <= B2B_SCALE_TRIANGULAR_MAX_D, its own launches; Float64 D <= 2048, one
+ *                     warp per column with T read through L2.  Trains T: slot 0 of b2b_chain_vjp_f32 / _f64.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -258,6 +272,11 @@ const char* b2b_status_string(int status);
  * a batch sum needs the chain to end in a fused launch (a logpdf chain ends in its MvNormal terminal).  The layer needs
  * workspace for its factor: b2b_chain_workspace_bytes adds 12·D² + 4·D + 8 bytes, each of the four parts rounded up to
  * 256 bytes, plus 256, for a chain with any SCALE_MATRIX layer (the layers share it; they run one after another).
+ * SCALE_TRIANGULAR runs the same way (D <= B2B_SCALE_TRIANGULAR_MAX_D, any N, y may alias x) in two launches: a prep
+ * launch, parallel over columns, writing M = T or T⁻¹ (fp32, zero outside the triangle) and log|det T|, then the map
+ * y = M x, which skips the k-blocks that are zero for all rows a warp owns (about D(D+1)/2 FMA per column).  With y == NULL
+ * the second launch writes the log-Jacobians only.  Its workspace is 4·D² + 8 bytes, each part rounded up to 256 bytes,
+ * plus 256; a chain holding both Scale kinds shares one region of the larger of the two sizes.
  * COUPLING_MLP runs in its own launch (any N, any ld >= D, scattered index lists, y may alias x; the envelope of
  * B2B_COUPLING_MLP_MAX_*; no workspace); like COUPLING_RQS, a batch sum needs the chain to end in a fused launch.
  * COUPLING_MLP_RQS runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x; the
@@ -408,6 +427,10 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * W_out c the same way (W̄_out ((3K−1)·n1 x H) column-major like W_out);
  * SCALE_MATRIX a (Ā, D x D column-major like A: G + (Σ l̄)·A⁻ᵀ, or −A⁻ᵀ G A⁻ᵀ − (Σ l̄)·A⁻ᵀ for the inverse layer, with
  * G = Σₙ ȳₙ uₙᵀ over the layer's inputs u; slots 1-3 return B2B_EUNSUPPORTED);
+ * SCALE_TRIANGULAR a (T̄, D x D column-major like T: the dense Ā projected on the triangle 𝒫 that T's parameters occupy --
+ * strictly below / above the diagonal for the unit forms, the diagonal included otherwise -- and exactly 0 outside 𝒫:
+ * 𝒫(G) + (Σ l̄)·diag(1/Tᵢᵢ), or −𝒫(T⁻ᵀ G T⁻ᵀ) − (Σ l̄)·diag(1/Tᵢᵢ) for the inverse layer, no diagonal term for the unit
+ * forms; slots 1-3 return B2B_EUNSUPPORTED);
  * ELEMENTWISE_VEC a (ā[D], Σₙ of ḡ·∂y/∂a + l̄·∂ℓ/∂a at the layer's output cotangent ḡ; slots 1-3 return
  * B2B_EUNSUPPORTED); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
@@ -415,7 +438,10 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * The chain is cut into segments that existing kernels differentiate -- planar runs of one direction (<= 8 layers; D not
  * in {32, 64, 128} is embedded in the next of them with zero rows), radial runs (<= 8), single RQS / coupling / spline coupling /
  * dense Scale (factor, x̄ by the transposed map, G over column chunks, an fp64 finalize; workspace: the factor of
- * b2b_chain_run_f32 plus P·D² floats, P <= 64 chunks, and 2·D² + 1 doubles) /
+ * b2b_chain_run_f32 plus P·D² floats, P <= 64 chunks, and 2·D² + 1 doubles) / triangular Scale (the prep launch, x̄ by
+ * the transposed triangular map; with T̄ requested G over column chunks -- on 𝒫 only, by the lower-triangle tiles, for the
+ * forward layer -- Σ l̄, and a masked fp64 finalize: 3 launches more for the forward layer, 5 for the inverse; workspace:
+ * its factor storage of b2b_chain_run_f32 plus P·D² floats and 2·D² + 1 doubles, each part rounded up to 256 bytes) /
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE layers (with the terminal MvNormal),
  * which one kernel differentiates (with ā requested, a second instantiation that also sweeps the run backwards, plus
  * G·V·D floats of per-CTA partials for the V ELEMENTWISE_VEC layers of the run, G <= 8 per SM); a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
@@ -545,7 +571,7 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * `ybar` (B2B_EINVAL); NULL `ybar` / `ljbar` are zeros; `param_bars` (NULL = x̄ only) holds 4*L pointers, entry 4l+i the
  * cotangent of layers[l].p<i> in its shape and layout, summed over the N columns.  Trainable slots as for Float32: PLANAR
  * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; ELEMENTWISE_VEC
- * a; BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
+ * a; SCALE_TRIANGULAR a (T̄, zero outside 𝒫); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
  * p0 is NULL) and L (D x D column-major, exactly zero above the diagonal); any other non-NULL entry returns
  * B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
  * parameter cotangents.  One warp per column recomputes the forward with the arithmetic of b2b_chain_run_f64, keeping
@@ -556,7 +582,7 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * Workspace (b2b_chain_vjp_workspace_bytes_f64; 0 exactly when the call refuses the chain) is bounded independently of N:
  * W warp slots of 8·(T + P) bytes plus 8·P, with T = Lf·D (Lf: layers before the MvNormal) and P the accumulators, per
  * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, ELEMENTWISE_VEC D, BATCHNORM / MVNORMAL_DIAG 2D, MVNORMAL_TRIL
- * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
+ * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄), SCALE_TRIANGULAR D(D+1)/2 (T̄'s packed triangle) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
  * 256 MiB but never below one CTA -- so the bound exceeds 256 MiB only when one CTA's slots do (e.g. wide couplings with
  * 2n1·n2 in the millions).  The number of warps, and with it the summation order, depends only on the chain, D and N. */
 size_t b2b_chain_vjp_workspace_bytes_f64(const b2b_layer_desc_f64* layers, int32_t L, int32_t D, int64_t N);
