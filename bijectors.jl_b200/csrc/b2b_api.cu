@@ -88,6 +88,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_COUPLING_AFFINE: ok = b2b_coupling_affine_fits(d.n0, d.n1, D); break;
     case B2B_SCALE_MATRIX: ok = D <= B2B_SCALE_MATRIX_MAX_D; break;
     case B2B_SCALE_TRIANGULAR: ok = D <= B2B_SCALE_TRIANGULAR_MAX_D; break;
+    case B2B_SCALE_LU: ok = D <= B2B_SCALE_LU_MAX_D; break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
     default: ok = !b2b_is_coupling(d.kind) || b2b_coupling_fits(d, D); break;  // the other couplings' table
   }
@@ -312,8 +313,8 @@ static bool sum_needs_logjac_ws(const b2b_layer_desc* layers, int32_t L, int nse
   return layers && L >= 1 && b2b_ends_in_terminal(layers, L) && nsegs > 1;
 }
 
-// factor storage of the dense and triangular Scale layers (one region of the largest: they run one after another); 0 for a
-// chain without one
+// factor storage of the dense, triangular and LU Scale layers (one region of the largest: they run one after another); 0
+// for a chain without one
 static size_t chain_scale_bytes(const b2b_layer_desc* layers, int32_t L, int D) {
   size_t bytes = 0;
   for (int l = 0; layers && l < L; ++l) {

@@ -31,8 +31,8 @@ struct F64Params {
   b2b_layer_desc_f64 layers[B2B_MAX_CHAIN];
 };
 
-// TRI: the chain holds a SCALE_TRIANGULAR layer (f64_layer_forward<TRI>)
-template <bool TRI>
+// TRI: the chain holds a SCALE_TRIANGULAR layer, LU: a SCALE_LU layer (f64_layer_forward<TRI, LU>)
+template <bool TRI, bool LU>
 __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_constant__ F64Params P) {
   extern __shared__ double sm64[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, D = P.D;
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(F64_WARPS * 32) chain_f64_kernel(const __grid_
     for (int i = lane; i < D; i += 32) col[i] = P.x[n * P.ldx + i];
     double lj = (P.accumulate && P.logjac) ? P.logjac[n] : 0.0;
     __syncwarp();
-    for (int l = 0; l < P.L; ++l) f64_layer_forward<TRI>(P.layers[l], D, lane, col, tmp, lj);
+    for (int l = 0; l < P.L; ++l) f64_layer_forward<TRI, LU>(P.layers[l], D, lane, col, tmp, lj);
     if (P.y)
       for (int i = lane; i < D; i += 32) P.y[n * P.ldy + i] = col[i];
     if (lane == 0) {
@@ -110,9 +110,13 @@ extern "C" int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     P.partials = static_cast<double*>(workspace);
   }
   const size_t smem = (size_t)F64_WARPS * 2 * D * sizeof(double);
-  bool tri = false;
-  for (int l = 0; l < L; ++l) tri = tri || layers[l].kind == B2B_SCALE_TRIANGULAR;
-  const auto kernel = tri ? chain_f64_kernel<true> : chain_f64_kernel<false>;
+  bool tri = false, lu = false;
+  for (int l = 0; l < L; ++l) {
+    tri = tri || layers[l].kind == B2B_SCALE_TRIANGULAR;
+    lu = lu || layers[l].kind == B2B_SCALE_LU;
+  }
+  const auto kernel =
+      lu ? chain_f64_kernel<true, true> : tri ? chain_f64_kernel<true, false> : chain_f64_kernel<false, false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   kernel<<<(int)grid, F64_WARPS * 32, smem, stream>>>(P);

@@ -120,8 +120,48 @@ __device__ __forceinline__ void law_deriv64(int op, bool inverse, double a, doub
   }
 }
 
+// v := Tᵀ v in place for a triangular T (column k of T read coalesced, a warp sum per entry): for an upper T entry k reads
+// the v_i with i < k, so k runs downwards; for a lower T upwards.
+__device__ __forceinline__ void f64_tri_tmul(const double* Tm, bool up, bool unit, int D, int lane, double* v) {
+  for (int kk = 0; kk < D; ++kk) {
+    const int k = up ? D - 1 - kk : kk;
+    double p = 0.0;
+    for (int i = (up ? 0 : k + 1) + lane; i < (up ? k : D); i += 32) p += Tm[(size_t)k * D + i] * v[i];
+    p = wsum(p);
+    if (lane == 0) v[k] = p + (unit ? v[k] : Tm[(size_t)k * D + k] * v[k]);
+    __syncwarp();
+  }
+}
+
+// v := T⁻ᵀ v in place for a triangular T: Tᵀ v̄ = v, v̄ᵢ = (vᵢ − Σ_k T(k, i)·v̄_k)/Tᵢᵢ over the finished k of column i
+__device__ __forceinline__ void f64_tri_tsolve(const double* Tm, bool up, bool unit, int D, int lane, double* v) {
+  for (int ii = 0; ii < D; ++ii) {
+    const int i = up ? ii : D - 1 - ii;
+    double p = 0.0;
+    for (int k = (up ? 0 : i + 1) + lane; k < (up ? i : D); k += 32) p += Tm[(size_t)i * D + k] * v[k];
+    p = wsum(p);
+    if (lane == 0) v[i] = (v[i] - p) / (unit ? 1.0 : Tm[(size_t)i * D + i]);
+    __syncwarp();
+  }
+}
+
+// acc(i, j) += sg·a_i·b_j on the strict lower triangle (lower) or on the upper one with the diagonal, where the diagonal
+// also takes dsg/F(j, j); acc and F are D x D column-major.  Entry (i, j) has one writer lane, (i − i₀(j)) mod 32.
+__device__ __forceinline__ void f64_lu_acc(double* acc, bool lower, const double* a, const double* b, double sg,
+                                           const double* F, double dsg, int D, int lane) {
+  for (int j = 0; j < D; ++j) {
+    double* Ac = acc + (size_t)j * D;
+    const double bj = sg * b[j];
+    for (int i = (lower ? j + 1 : 0) + lane; i < (lower ? D : j + 1); i += 32)
+      Ac[i] += i == j ? a[i] * bj + dsg / F[(size_t)j * D + j] : a[i] * bj;
+  }
+  __syncwarp();  // a and b were read with a lane mapping that shifts with j
+}
+
 // Reverse mode of one layer at its input column `col`: g (the cotangent of the layer's output) becomes the cotangent of
 // its input; `acc` (NULL: not wanted) receives this column's parameter cotangents.  All 32 lanes call it; ends synced.
+// LU = false leaves SCALE_LU out (chain_vjp_f64_kernel<false>: the chains without the layer).
+template <bool LU>
 __device__ __forceinline__ void layer_vjp(const b2b_layer_desc_f64& d, int D, int lane, const double* col, double* g,
                                           double* t1, double* t2, double lb, double* acc) {
   const bool inv = d.inverse != 0;
@@ -431,6 +471,36 @@ __device__ __forceinline__ void layer_vjp(const b2b_layer_desc_f64& d, int D, in
       __syncwarp();  // the outer product reads g with a lane mapping that shifts with j: every lane is done with it
       for (int i = lane; i < D; i += 32) g[i] = t1[i];
     } break;
+    case B2B_SCALE_LU:  // accumulators: F̄ (D x D column-major, packed like F: L̄ below the diagonal, Ū on and above it)
+      if constexpr (LU) {
+        const double* F = d.p0;
+        const b2b_layer_desc_f64 Uf = f64_lu_factor(d, true), Lf = f64_lu_factor(d, false);
+        if (!inv) {  // y = P v, v = L u, u = U x:  v̄ = Pᵀȳ, L̄ += v̄ uᵀ, ū = Lᵀv̄, Ū += ū xᵀ + l̄·diag(1/Uᵢᵢ), x̄ = Uᵀū
+          for (int i = lane; i < D; i += 32) t2[i] = col[i];
+          __syncwarp();
+          f64_tri_forward(Uf, D, lane, t2, t1);
+          for (int i = lane; i < D; i += 32) t1[i] = d.i0 ? g[d.i0[i]] : g[i];
+          __syncwarp();
+          if (acc) f64_lu_acc(acc, true, t1, t2, 1.0, F, 0.0, D, lane);
+          f64_tri_tmul(F, false, true, D, lane, t1);
+          if (acc) f64_lu_acc(acc, false, t1, col, 1.0, F, lb, D, lane);
+          f64_tri_tmul(F, true, false, D, lane, t1);
+          for (int i = lane; i < D; i += 32) g[i] = t1[i];
+        } else {  // z = U⁻¹ v, v = L⁻¹ w, w = Pᵀ y:  v̄ = U⁻ᵀz̄, Ū −= v̄ zᵀ + l̄·diag(1/Uᵢᵢ), w̄ = L⁻ᵀv̄, L̄ −= w̄ vᵀ, ȳ = P w̄
+          for (int i = lane; i < D; i += 32) t2[i] = d.i0 ? col[d.i0[i]] : col[i];
+          __syncwarp();
+          f64_tri_solve(Lf, D, lane, t2);
+          for (int i = lane; i < D; i += 32) t1[i] = t2[i];
+          __syncwarp();
+          f64_tri_solve(Uf, D, lane, t1);
+          f64_tri_tsolve(F, true, false, D, lane, g);
+          if (acc) f64_lu_acc(acc, false, g, t1, -1.0, F, -lb, D, lane);
+          f64_tri_tsolve(F, false, true, D, lane, g);
+          if (acc) f64_lu_acc(acc, true, g, t2, -1.0, F, 0.0, D, lane);
+          if (d.i0) f64_lu_permute(d.i0, false, D, lane, g, t1);
+        }
+      }
+      break;
     case B2B_PERMUTE: {
       for (int i = lane; i < D; i += 32) t1[i] = g[i];
       __syncwarp();
@@ -444,6 +514,8 @@ __device__ __forceinline__ void layer_vjp(const b2b_layer_desc_f64& d, int D, in
   __syncwarp();
 }
 
+// LU: the chain holds a SCALE_LU layer (f64_layer_forward and layer_vjp with its case)
+template <bool LU>
 __global__ void __launch_bounds__(V64_WARPS * 32) chain_vjp_f64_kernel(const __grid_constant__ V64Params P) {
   extern __shared__ double smv[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, D = P.D;
@@ -463,7 +535,7 @@ __global__ void __launch_bounds__(V64_WARPS * 32) chain_vjp_f64_kernel(const __g
     double lj = 0.0;
     for (int l = 0; l < P.Lf; ++l) {
       for (int i = lane; i < D; i += 32) tape[(size_t)l * D + i] = col[i];
-      f64_layer_forward(P.layers[l], D, lane, col, t1, lj);
+      f64_layer_forward<true, LU>(P.layers[l], D, lane, col, t1, lj);
     }
     const double lb = P.ljbar ? P.ljbar[n] : 0.0;
     for (int i = lane; i < D; i += 32) g[i] = P.ybar ? P.ybar[n * P.ldyb + i] : 0.0;
@@ -504,7 +576,7 @@ __global__ void __launch_bounds__(V64_WARPS * 32) chain_vjp_f64_kernel(const __g
     for (int l = P.Lf - 1; l >= 0; --l) {
       for (int i = lane; i < D; i += 32) col[i] = tape[(size_t)l * D + i];
       __syncwarp();
-      layer_vjp(P.layers[l], D, lane, col, g, t1, t2, lb, (P.want >> l) & 1u ? acc + P.off[l] : nullptr);
+      layer_vjp<LU>(P.layers[l], D, lane, col, g, t1, t2, lb, (P.want >> l) & 1u ? acc + P.off[l] : nullptr);
     }
     for (int i = lane; i < D; i += 32) P.xbar[n * P.ldxb + i] = g[i];
     __syncwarp();
@@ -604,6 +676,7 @@ __global__ void __launch_bounds__(V64_FIN_THREADS) vjp_f64_finalize_kernel(const
           bars[0][k] = in ? r[(d.n0 ? j * (j + 1) / 2 : j * D - j * (j + 1) / 2) + i] : 0.0;
         }
       break;
+    case B2B_SCALE_LU: copy(bars[0], r, (size_t)D * D); break;  // F̄ is accumulated in F's own layout
     default: break;
   }
 }
@@ -621,6 +694,7 @@ long long acc_len(const b2b_layer_desc_f64& d, int D) {
     case B2B_MVNORMAL_DIAG: n = 2LL * D; break;
     case B2B_MVNORMAL_TRIL: n = (long long)D + (long long)D * (D + 1) / 2; break;
     case B2B_SCALE_TRIANGULAR: n = (long long)D * (D + 1) / 2; break;
+    case B2B_SCALE_LU: n = (long long)D * D; break;
     default: break;
   }
   return (n + 31) & ~31LL;
@@ -722,9 +796,12 @@ extern "C" int b2b_chain_vjp_f64(const b2b_layer_desc_f64* layers, int32_t L, co
     P.layers[l] = layers[l];
   }
   const long long ctas = plan.warps / plan.wpc;
-  cudaError_t e = cudaFuncSetAttribute(chain_vjp_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
+  bool lu = false;
+  for (int l = 0; l < L; ++l) lu = lu || layers[l].kind == B2B_SCALE_LU;
+  const auto kernel = lu ? chain_vjp_f64_kernel<true> : chain_vjp_f64_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
   if (e != cudaSuccess) return (int)e;
-  chain_vjp_f64_kernel<<<(int)ctas, plan.wpc * 32, plan.smem, stream>>>(P);
+  kernel<<<(int)ctas, plan.wpc * 32, plan.smem, stream>>>(P);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
   ++launches;
   if (want) {

@@ -255,11 +255,49 @@ static __device__ double f64_tri_forward(const b2b_layer_desc_f64& d, int D, int
   return lp;
 }
 
+// v := P v (y[dst[r]] = v[r]) or, `inv`, Pᵀ v (v[r] = y[dst[r]]) in place through `tmp`, for dst = i0 of SCALE_LU
+static __device__ __forceinline__ void f64_lu_permute(const int32_t* dst, bool inv, int D, int lane, double* v,
+                                                      double* tmp) {
+  for (int i = lane; i < D; i += 32) tmp[i] = v[i];
+  __syncwarp();
+  for (int i = lane; i < D; i += 32) {
+    if (inv) v[i] = tmp[dst[i]];
+    else v[dst[i]] = tmp[i];
+  }
+  __syncwarp();
+}
+
+// The SCALE_TRIANGULAR descriptor of one factor of a SCALE_LU layer `d` (F in p0): U (upper) or L (unit lower)
+static __device__ __forceinline__ b2b_layer_desc_f64 f64_lu_factor(const b2b_layer_desc_f64& d, bool upper) {
+  b2b_layer_desc_f64 t = d;
+  t.kind = B2B_SCALE_TRIANGULAR;
+  t.n0 = upper ? 1 : 0;
+  t.n1 = upper ? 0 : 1;
+  return t;
+}
+
+// y = P·L·U x or U⁻¹ L⁻¹ Pᵀ x for SCALE_LU (p0 = F: L strictly below the diagonal with a unit diagonal, U on and above it;
+// i0 = dst or NULL): the steps of PERMUTE ∘ SCALE_TRIANGULAR(unit lower) ∘ SCALE_TRIANGULAR(upper) on F, by the
+// triangular layer's own functions.  Returns the log-Jacobian, ±Σ log|Uᵢᵢ|, in every lane.
+static __device__ double f64_lu_forward(const b2b_layer_desc_f64& d, int D, int lane, double* col, double* tmp) {
+  const b2b_layer_desc_f64 U = f64_lu_factor(d, true), L = f64_lu_factor(d, false);
+  if (d.inverse) {
+    if (d.i0) f64_lu_permute(d.i0, true, D, lane, col, tmp);
+    f64_tri_forward(L, D, lane, col, tmp);
+    return f64_tri_forward(U, D, lane, col, tmp);
+  }
+  const double lp = f64_tri_forward(U, D, lane, col, tmp);
+  f64_tri_forward(L, D, lane, col, tmp);
+  if (d.i0) f64_lu_permute(d.i0, false, D, lane, col, tmp);
+  return lp;
+}
+
 // Applies one layer to the column `col` (D doubles in shared memory; `tmp`: D more, scratch) and adds its log-Jacobian
 // (for MVNORMAL_DIAG: the log-density) to `lj`.  Called by all 32 lanes of a warp; ends with __syncwarp.  TRI = false
 // leaves SCALE_TRIANGULAR out: compiled in, that case costs the Float64 forward kernel registers (80 instead of 96, and a
-// spill), so b2b_chain_run_f64 uses that instantiation only for chains that hold the layer.
-template <bool TRI = true>
+// spill), so b2b_chain_run_f64 uses that instantiation only for chains that hold the layer.  LU = false leaves SCALE_LU
+// out the same way: only chains that hold it run an instantiation with that case.
+template <bool TRI = true, bool LU = false>
 static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f64& d, int D, int lane, double* col,
                                                          double* tmp, double& lj) {
   const bool inv = d.inverse != 0;
@@ -371,6 +409,9 @@ static __device__ __forceinline__ void f64_layer_forward(const b2b_layer_desc_f6
     } break;
     case B2B_SCALE_TRIANGULAR:
       if constexpr (TRI) lj += f64_tri_forward(d, D, lane, col, tmp);
+      break;
+    case B2B_SCALE_LU:
+      if constexpr (LU) lj += f64_lu_forward(d, D, lane, col, tmp);
       break;
     case B2B_MVNORMAL_TRIL:  // the column is left as it is (the terminal's y is its input); r goes to tmp
       lj += -0.5 * (double)D * 1.8378770664093453 + f64_tril_solve(d, D, lane, col, tmp);

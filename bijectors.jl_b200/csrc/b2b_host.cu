@@ -27,7 +27,7 @@ struct b2b_host_ctx {
 
 static const size_t kWsBytes = 512 * 1024;  // batch-sum partials + tensor-core W image of a coupling layer
 
-// A chain with a dense or triangular Scale also needs its factor storage, before the partials: the staging workspace grows
+// A chain with a dense, triangular or LU Scale also needs its factor storage, before the partials: the staging workspace grows
 // to hold the dense one's (the larger) at D_max, and only such chains are handed the larger size (every other chain sees
 // kWsBytes, as before).
 static size_t ctx_ws_bytes(int D_max) {

@@ -122,8 +122,8 @@ size_t b2b_tril_vjp_workspace(int D, long long N);
 long long b2b_outer_chunk_len(long long N);
 int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long long ldr, float* part, float* mup, int D,
                             long long N, bool lower, cudaStream_t stream);
-// dense and triangular Scale (b2b_scale_matrix.cu), SCALE_MATRIX or SCALE_TRIANGULAR `kind` at D <= 256: the factor
-// storage of its forward launches (0 beyond the envelope)
+// dense, triangular and LU Scale (b2b_scale_matrix.cu), SCALE_MATRIX, SCALE_TRIANGULAR or SCALE_LU `kind` at D <= 256:
+// the factor storage of its forward launches (0 beyond the envelope)
 size_t b2b_scale_workspace(int kind, int D);
 // reverse mode: b2b_scale_vjp_workspace(kind, D, N) bytes (0 beyond the envelope)
 size_t b2b_scale_vjp_workspace(int kind, int D, long long N);
@@ -195,7 +195,7 @@ struct B2BFwdSeg {
 };
 int b2b_fwd_spline(const B2BFwdSeg& s);  // b2b_coupling_rqs.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
 int b2b_fwd_mlp(const B2BFwdSeg& s);     // b2b_coupling_mlp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
-int b2b_fwd_scale(const B2BFwdSeg& s);   // b2b_scale_matrix.cu: SCALE_MATRIX, SCALE_TRIANGULAR; y == NULL: log-Jacobians only
+int b2b_fwd_scale(const B2BFwdSeg& s);   // b2b_scale_matrix.cu: SCALE_MATRIX, _TRIANGULAR, _LU; y == NULL: log-Jacobians only
 int b2b_fwd_tril(const B2BFwdSeg& s);    // b2b_mvnormal_tril.cu: copies x to y (when y != x), writes logpdf to logjac
 
 // ---- reverse-mode segment launchers ----------------------------------------------------------------------------------
@@ -236,7 +236,7 @@ int b2b_vjp_batchnorm(const B2BVjpSeg& s); // b2b_coupling_vjp.cu: eval mode
 int b2b_vjp_ew(const B2BVjpSeg& s);        // b2b_ew_vjp.cu: <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE, optionally closed by MVNORMAL_DIAG
 int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
 int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
-int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu: SCALE_MATRIX, SCALE_TRIANGULAR
+int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu: SCALE_MATRIX, SCALE_TRIANGULAR, SCALE_LU
 int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
 // One launch copying slot i of layer j from base[i] + j·step[i] to bars[4j + i], for the requested slots of a run of
 // n <= 8 layers at D (nothing is launched when none is requested).
@@ -295,6 +295,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_COUPLING_DEEP_MLP_RQS, P012 | B2B_F_I0 | B2B_F_I1, false, B2B_LC_SPLINE, B2B_VC_SPLINE, 4, B2B_F_P3, false},
       {B2B_ELEMENTWISE_VEC, B2B_F_P0,                    false, B2B_LC_FUSED,    B2B_VC_EW,       1, 0,        true},
       {B2B_SCALE_TRIANGULAR, B2B_F_P0,                   false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        true},
+      {B2B_SCALE_LU,        B2B_F_P0,                    false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        true},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -443,7 +444,8 @@ size_t b2b_slot_len(const Desc& d, int i, int D) {
     case B2B_RQS: return (size_t)D * d.n0;
     case B2B_MVNORMAL_TRIL: return i == 1 ? (size_t)D * D : D;
     case B2B_SCALE_MATRIX:
-    case B2B_SCALE_TRIANGULAR: return (size_t)D * D;
+    case B2B_SCALE_TRIANGULAR:
+    case B2B_SCALE_LU: return (size_t)D * D;
     default: return D;  // BATCHNORM b / logs, MVNORMAL_DIAG μ / σ, ELEMENTWISE_VEC a
   }
 }

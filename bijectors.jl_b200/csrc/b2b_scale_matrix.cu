@@ -20,6 +20,14 @@
 // base (all tiles), its chunks and Σ l̄ summed in a fixed order in fp64, and the two D x D products of the inverse layer
 // in fp64.  No atomics; every launch is graph-capturable.
 //
+// LU layer, B2B_SCALE_LU: y = P·L·U·x with L (unit lower) and U (upper) packed in one D x D F as getrf leaves them and P
+// the permutation y[dst[r]] = (L U x)[r].  The dense layer's map and reverse mode on M = P·L·U (forward) or U⁻¹ L⁻¹ Pᵀ:
+//   lu_prep_kernel (parallel over columns) writes M in fp32 from fp64 columns -- L·(U e_j) scattered to the rows dst[·],
+//     or Pᵀ e_j solved against L and U as inv_kernel does -- and log|det U| in row order; the map is the dense one, so a
+//     call is two launches.
+//   reverse mode: M̄ = G (forward layer) or −M⁻ᵀ G M⁻ᵀ (inverse layer, the dense finalize without its s·B term), then
+//     lu_bar_kernel takes M̄ through the factors: L̄ = 𝒮(Pᵀ M̄ Uᵀ), Ū = 𝒰(Lᵀ Pᵀ M̄) ± s·diag(1/Uᵢᵢ), packed like F.
+//
 // Triangular layer, B2B_SCALE_TRIANGULAR: Scale(T) with T lower or upper triangular, stored or unit diagonal.  The same
 // launches with the structure made explicit, selected by the descriptor's kind in scale_prep:
 //   tri_prep_kernel (parallel over columns, no serial step) writes M = T or T⁻¹ in fp32, zero outside the triangle and 1
@@ -212,6 +220,59 @@ __global__ void __launch_bounds__(kFactorThreads, 1)
   if (tid == 0) *logdet = ld;
 }
 
+// z := U⁻¹ L⁻¹ z for the kInvC columns of a warp (lanes own rows), L unit lower and U upper packed in `lu` (column-major,
+// getrf's layout, fp64 or fp32 entries): forward substitution against L (right-looking), then back substitution against U.
+// Reads L strictly below the diagonal and U on and above it; column k is read once (coalesced) for all the columns.
+template <int R, class TF>
+__device__ __forceinline__ void lu_solve_cols(double (&z)[R][kInvC], const TF* __restrict__ lu, int D, int lane) {
+  // forward substitution, unit lower L (right-looking)
+#pragma unroll
+  for (int kb = 0; kb < R; ++kb) {
+    for (int jj = 0; jj < 32; ++jj) {
+      const int k = kb * 32 + jj;
+      if (k >= D) break;
+      double v[kInvC];
+#pragma unroll
+      for (int c = 0; c < kInvC; ++c) v[c] = __shfl_sync(kFull, z[kb][c], jj);
+      const TF* Lk = lu + (size_t)k * D;
+#pragma unroll
+      for (int r = kb; r < R; ++r) {
+        const int i = lane + 32 * r;
+        if (i > k && i < D) {
+          const double l = (double)Lk[i];
+#pragma unroll
+          for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-l, v[c], z[r][c]);
+        }
+      }
+    }
+  }
+  // back substitution, upper U
+#pragma unroll
+  for (int kb = R - 1; kb >= 0; --kb) {
+    for (int jj = 31; jj >= 0; --jj) {
+      const int k = kb * 32 + jj;
+      if (k >= D) continue;
+      const TF* Uk = lu + (size_t)k * D;
+      const double ukk = (double)Uk[k];
+      double v[kInvC];
+#pragma unroll
+      for (int c = 0; c < kInvC; ++c) {
+        v[c] = __shfl_sync(kFull, z[kb][c], jj) / ukk;
+        if (lane == jj) z[kb][c] = v[c];
+      }
+#pragma unroll
+      for (int r = 0; r <= kb; ++r) {
+        const int i = lane + 32 * r;
+        if (i < k) {
+          const double u = (double)Uk[i];
+#pragma unroll
+          for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-u, v[c], z[r][c]);
+        }
+      }
+    }
+  }
+}
+
 // columns of M = A⁻¹ (fp32, column-major): solve L U z = P e_j
 template <int R>
 __global__ void __launch_bounds__(kInvWarps * 32)
@@ -227,52 +288,7 @@ __global__ void __launch_bounds__(kInvWarps * 32)
 #pragma unroll
     for (int c = 0; c < kInvC; ++c) z[r][c] = (pi == col0 + c) ? 1.0 : 0.0;
   }
-  // forward substitution, unit lower L (right-looking)
-#pragma unroll
-  for (int kb = 0; kb < R; ++kb) {
-    for (int jj = 0; jj < 32; ++jj) {
-      const int k = kb * 32 + jj;
-      if (k >= D) break;
-      double v[kInvC];
-#pragma unroll
-      for (int c = 0; c < kInvC; ++c) v[c] = __shfl_sync(kFull, z[kb][c], jj);
-      const double* Lk = lu + (size_t)k * D;
-#pragma unroll
-      for (int r = kb; r < R; ++r) {
-        const int i = lane + 32 * r;
-        if (i > k && i < D) {
-          const double l = Lk[i];
-#pragma unroll
-          for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-l, v[c], z[r][c]);
-        }
-      }
-    }
-  }
-  // back substitution, upper U
-#pragma unroll
-  for (int kb = R - 1; kb >= 0; --kb) {
-    for (int jj = 31; jj >= 0; --jj) {
-      const int k = kb * 32 + jj;
-      if (k >= D) continue;
-      const double* Uk = lu + (size_t)k * D;
-      const double ukk = Uk[k];
-      double v[kInvC];
-#pragma unroll
-      for (int c = 0; c < kInvC; ++c) {
-        v[c] = __shfl_sync(kFull, z[kb][c], jj) / ukk;
-        if (lane == jj) z[kb][c] = v[c];
-      }
-#pragma unroll
-      for (int r = 0; r <= kb; ++r) {
-        const int i = lane + 32 * r;
-        if (i < k) {
-          const double u = Uk[i];
-#pragma unroll
-          for (int c = 0; c < kInvC; ++c) z[r][c] = fma(-u, v[c], z[r][c]);
-        }
-      }
-    }
-  }
+  lu_solve_cols<R>(z, lu, D, lane);
 #pragma unroll
   for (int c = 0; c < kInvC; ++c) {
     const int j = col0 + c;
@@ -282,6 +298,21 @@ __global__ void __launch_bounds__(kInvWarps * 32)
       const int i = lane + 32 * r;
       if (i < D) minv[(size_t)j * D + i] = (float)z[r][c];
     }
+  }
+}
+
+// *logdet = Σᵢ log|Tᵢᵢ| in row order (0 for unit), by the first warp of the calling CTA
+template <int R>
+__device__ __forceinline__ void diag_logdet(const float* __restrict__ T, int D, int unit, double* __restrict__ logdet) {
+  __shared__ double lg[32 * R];
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x >= 32) return;
+  for (int i = lane; i < D; i += 32) lg[i] = unit ? 0.0 : log(fabs((double)T[(size_t)i * D + i]));
+  __syncwarp();
+  if (lane == 0) {
+    double s = 0.0;
+    for (int i = 0; i < D; ++i) s += lg[i];
+    *logdet = s;
   }
 }
 
@@ -295,15 +326,7 @@ __global__ void __launch_bounds__(kInvWarps * 32)
                     double* __restrict__ logdet) {
   const int lane = threadIdx.x & 31;
   if (blockIdx.x == gridDim.x - 1) {
-    __shared__ double lg[32 * R];
-    if (threadIdx.x >= 32) return;
-    for (int i = lane; i < D; i += 32) lg[i] = unit ? 0.0 : log(fabs((double)T[(size_t)i * D + i]));
-    __syncwarp();
-    if (lane == 0) {
-      double s = 0.0;
-      for (int i = 0; i < D; ++i) s += lg[i];
-      *logdet = s;
-    }
+    diag_logdet<R>(T, D, unit, logdet);
     return;
   }
   const int col0 = (blockIdx.x * kInvWarps + (threadIdx.x >> 5)) * kInvC;
@@ -386,6 +409,70 @@ __global__ void __launch_bounds__(kInvWarps * 32)
       const int i = lane + 32 * r;
       if (i < D) M[(size_t)j * D + i] = (float)z[r][c];
     }
+  }
+}
+
+// M = P·L·U (inv == 0) or U⁻¹ L⁻¹ Pᵀ of an LU layer, fp32: F packs L (strictly below the diagonal, unit diagonal implied)
+// and U (on and above it); y[dst[r]] = (L U x)[r], dst == NULL the identity.  Forward column j: u = U e_j, then L u
+// right-looking from the last row up (step k adds L(i, k)·u_k to the rows below k while u_k is still U's), scattered to
+// the rows dst[·].  Inverse column j: Pᵀ e_j (the 1 in the row r with dst[r] = j) solved against L and U as inv_kernel does.
+// Each entry is computed in fp64 and rounded once.  The last CTA writes log|det U| = Σ log|Uᵢᵢ| in row order.
+template <int R>
+__global__ void __launch_bounds__(kInvWarps * 32)
+    lu_prep_kernel(const float* __restrict__ F, const int* __restrict__ dst, int D, int inv, float* __restrict__ M,
+                   double* __restrict__ logdet) {
+  const int lane = threadIdx.x & 31;
+  if (blockIdx.x == gridDim.x - 1) {
+    diag_logdet<R>(F, D, 0, logdet);
+    return;
+  }
+  const int col0 = (blockIdx.x * kInvWarps + (threadIdx.x >> 5)) * kInvC;
+  if (col0 >= D) return;
+  double z[R][kInvC];
+  int row[R];  // where row i of the warp's result goes: i (inverse) or dst[i] (forward)
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int i = lane + 32 * r;
+    const int pi = i < D ? (dst ? dst[i] : i) : -1;
+    row[r] = inv ? i : pi;
+#pragma unroll
+    for (int c = 0; c < kInvC; ++c) {
+      const int j = col0 + c;
+      z[r][c] = inv ? (pi == j ? 1.0 : 0.0) : (i < D && j < D && i <= j ? (double)F[(size_t)j * D + i] : 0.0);
+    }
+  }
+  if (inv) {
+    lu_solve_cols<R>(z, F, D, lane);
+  } else {
+    const int klast = col0 + kInvC - 1;  // u_k = 0 beyond the warp's last column
+#pragma unroll
+    for (int kb = R - 1; kb >= 0; --kb) {
+      for (int jj = 31; jj >= 0; --jj) {
+        const int k = kb * 32 + jj;
+        if (k >= D || k > klast) continue;
+        const float* Lk = F + (size_t)k * D;
+        double v[kInvC];
+#pragma unroll
+        for (int c = 0; c < kInvC; ++c) v[c] = __shfl_sync(kFull, z[kb][c], jj);
+#pragma unroll
+        for (int r = kb; r < R; ++r) {
+          const int i = lane + 32 * r;
+          if (i > k && i < D) {
+            const double l = (double)Lk[i];
+#pragma unroll
+            for (int c = 0; c < kInvC; ++c) z[r][c] = fma(l, v[c], z[r][c]);
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < kInvC; ++c) {
+    const int j = col0 + c;
+    if (j >= D) break;
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if (lane + 32 * r < D) M[(size_t)j * D + row[r]] = (float)z[r][c];
   }
 }
 
@@ -606,20 +693,48 @@ __global__ void __launch_bounds__(256) prod_gb_kernel(const double* __restrict__
   Tm[idx] = a;
 }
 
-// inverse layer: Ā = −B · T − s·B, on the mask (0 elsewhere)
+// inverse layer: Ā = −B · T − s·B, on the mask (0 elsewhere).  With Ad != NULL (the LU layer): Ad = −B · T in fp64, in
+// full and without the s·B term, for lu_bar_kernel.
 __global__ void __launch_bounds__(256) final_inv_kernel(const double* __restrict__ Tm, const float* __restrict__ minv,
                                                         const double* __restrict__ ljs, int D, int mask,
-                                                        float* __restrict__ Abar) {
+                                                        float* __restrict__ Abar, double* __restrict__ Ad) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)D * D) return;
   const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
-  if (!in_mask(mask, i, j)) {
+  if (!Ad && !in_mask(mask, i, j)) {
     Abar[idx] = 0.f;
     return;
   }
   double a = 0.0;
   for (int k = 0; k < D; ++k) a = fma((double)minv[(size_t)i * D + k], Tm[(size_t)j * D + k], a);
+  if (Ad) {
+    Ad[idx] = -a;
+    return;
+  }
   Abar[idx] = (float)(-a - *ljs * (double)minv[(size_t)i * D + j]);
+}
+
+// LU layer: F̄ from M̄ (fp64, column-major: G for the forward layer, −M⁻ᵀ G M⁻ᵀ for the inverse one) through M = P L U:
+//   F̄(i, j) = (Pᵀ M̄ Uᵀ)(i, j) = Σ_{k≥j} M̄(dst[i], k)·U(j, k)                          i > j   (L̄)
+//   F̄(i, j) = (Lᵀ Pᵀ M̄)(i, j) = M̄(dst[i], j) + Σ_{k>i} L(k, i)·M̄(dst[k], j) + sg·s/Uᵢᵢ   i ≤ j   (Ū, s/Uᵢᵢ on i = j)
+// with sg = +1 for the forward layer and −1 for the inverse one, k increasing, one thread per entry.
+__global__ void __launch_bounds__(256) lu_bar_kernel(const double* __restrict__ Mb, const float* __restrict__ F,
+                                                     const int* __restrict__ dst, const double* __restrict__ ljs,
+                                                     double sg, int D, float* __restrict__ Fbar) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)D * D) return;
+  const int j = (int)(idx / D), i = (int)(idx - (long long)j * D);
+  auto prow = [&](int r) { return dst ? dst[r] : r; };
+  double a = 0.0;
+  if (i > j) {
+    const int pi = prow(i);
+    for (int k = j; k < D; ++k) a = fma(Mb[(size_t)k * D + pi], (double)F[(size_t)k * D + j], a);
+  } else {
+    a = Mb[(size_t)j * D + prow(i)];
+    for (int k = i + 1; k < D; ++k) a = fma((double)F[(size_t)i * D + k], Mb[(size_t)j * D + prow(k)], a);
+    if (i == j) a += sg * *ljs / (double)F[(size_t)i * D + i];
+  }
+  Fbar[idx] = (float)a;
 }
 
 int launch_factor(const b2b_layer_desc& d, const Factor& f, int D, bool want_inverse, int* launches, cudaStream_t stream) {
@@ -636,6 +751,20 @@ int launch_factor(const b2b_layer_desc& d, const Factor& f, int D, bool want_inv
   else if (D <= 128) inv_kernel<4><<<grid, kInvWarps * 32, 0, stream>>>(f.lu, f.perm, f.minv, D);
   else inv_kernel<8><<<grid, kInvWarps * 32, 0, stream>>>(f.lu, f.perm, f.minv, D);
   if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+  ++*launches;
+  return B2B_OK;
+}
+
+// M = P·L·U or U⁻¹ L⁻¹ Pᵀ and log|det U| of an LU layer, one launch
+int launch_lu_prep(const b2b_layer_desc& d, const TriFactor& f, int D, int* launches, cudaStream_t stream) {
+  const int grid = (D + kInvWarps * kInvC - 1) / (kInvWarps * kInvC) + 1;  // + the log|det U| CTA
+  const int inv = d.inverse != 0;
+  if (D <= 32) lu_prep_kernel<1><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, d.i0, D, inv, f.m, f.logdet);
+  else if (D <= 64) lu_prep_kernel<2><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, d.i0, D, inv, f.m, f.logdet);
+  else if (D <= 128) lu_prep_kernel<4><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, d.i0, D, inv, f.m, f.logdet);
+  else lu_prep_kernel<8><<<grid, kInvWarps * 32, 0, stream>>>(d.p0, d.i0, D, inv, f.m, f.logdet);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
   ++*launches;
   return B2B_OK;
 }
@@ -684,30 +813,39 @@ int launch_map(int tri, const float* M, const float* x, long long ldx, float* y,
   return launch_map_d<TRANS, 2>(M, x, ldx, y, ldy, logjac, accumulate, logdet, sign, D, N, stream);
 }
 
-// What the launches after the prep need, for either kind: the map operand M (A, A⁻¹, T or T⁻¹), the B = M⁻ᵀ source of the
-// finalize kernels, log|det|, the structure of M for the map and the output mask of the cotangent.
+// What the launches after the prep need, for any kind: the map operand M (A, A⁻¹, T, T⁻¹, P·L·U or U⁻¹ L⁻¹ Pᵀ), the
+// B = M⁻ᵀ source of the finalize kernels, log|det|, the structure of M for the map, the output mask of the cotangent, and
+// whether the cotangent goes through the LU factors (lu_bar_kernel).
 struct ScaleOp {
   const float* M;
   const float* minv;
   double* logdet;
   int tri;   // 0 dense, 1 lower, 2 upper
   int mask;  // kMaskFull or the triangle 𝒫
+  bool lu;
 };
 
-size_t prep_bytes(int kind, int D) { return kind == B2B_SCALE_TRIANGULAR ? tri_bytes(D) : factor_bytes(D); }
+size_t prep_bytes(int kind, int D) { return kind == B2B_SCALE_MATRIX ? factor_bytes(D) : tri_bytes(D); }
 
 // The prep launches of the layer `d` (the descriptor's kind decides them here, and nowhere else): the dense layer's LU, and
-// A⁻¹ when `want_inverse`; the triangular layer's M (always: its map must not read the entries outside the triangle).
+// A⁻¹ when `want_inverse`; the triangular layer's M (always: its map must not read the entries outside the triangle); the
+// LU layer's M (always: the map needs the product of the factors).  For the inverse LU layer M = (P L U)⁻¹ is also the
+// B = M⁻ᵀ source (minv) of final_inv_kernel.
 int scale_prep(const b2b_layer_desc& d, void* ws, int D, bool want_inverse, ScaleOp* op, int* launches,
                cudaStream_t stream) {
   const bool inv = d.inverse != 0;
   if (d.kind == B2B_SCALE_TRIANGULAR) {
     const TriFactor f = carve_tri(ws, D);
-    *op = ScaleOp{f.m, f.m, f.logdet, d.n0 ? 2 : 1, kMaskTri | (d.n0 ? kMaskUpper : 0) | (d.n1 ? kMaskStrict : 0)};
+    *op = ScaleOp{f.m, f.m, f.logdet, d.n0 ? 2 : 1, kMaskTri | (d.n0 ? kMaskUpper : 0) | (d.n1 ? kMaskStrict : 0), false};
     return launch_tri_prep(d, f, D, launches, stream);
   }
+  if (d.kind == B2B_SCALE_LU) {
+    const TriFactor f = carve_tri(ws, D);
+    *op = ScaleOp{f.m, f.m, f.logdet, 0, kMaskFull, true};
+    return launch_lu_prep(d, f, D, launches, stream);
+  }
   const Factor f = carve(ws, D);
-  *op = ScaleOp{inv ? f.minv : d.p0, f.minv, f.logdet, 0, kMaskFull};
+  *op = ScaleOp{inv ? f.minv : d.p0, f.minv, f.logdet, 0, kMaskFull, false};
   return launch_factor(d, f, D, want_inverse, launches, stream);
 }
 
@@ -720,7 +858,7 @@ size_t b2b_scale_workspace(int kind, int D) { return D >= 1 && D <= B2B_SCALE_MA
 int b2b_fwd_scale(const B2BFwdSeg& s) {
   const b2b_layer_desc& d = s.layers[0];
   const int D = s.D;
-  if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;  // = B2B_SCALE_TRIANGULAR_MAX_D
+  if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;  // = B2B_SCALE_TRIANGULAR_MAX_D = B2B_SCALE_LU_MAX_D
   if (!s.workspace || s.workspace_bytes < prep_bytes(d.kind, D)) return B2B_EWORKSPACE;
   const bool inv = d.inverse != 0;
   ScaleOp op;
@@ -761,7 +899,7 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   const cudaStream_t stream = s.stream;
   if (D < 1 || D > B2B_SCALE_MATRIX_MAX_D) return B2B_EUNSUPPORTED;
   if (!workspace || s.workspace_bytes < b2b_scale_vjp_workspace(d.kind, D, N)) return B2B_EWORKSPACE;
-  const bool inv = d.inverse != 0, tri = d.kind == B2B_SCALE_TRIANGULAR;
+  const bool inv = d.inverse != 0, tri = d.kind == B2B_SCALE_TRIANGULAR, lu = d.kind == B2B_SCALE_LU;
   char* ws = static_cast<char*>(workspace) + prep_bytes(d.kind, D);
   const long long clen = b2b_outer_chunk_len(N), P = (N + clen - 1) / clen;
   float* part = reinterpret_cast<float*>(ws);
@@ -773,7 +911,7 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   double* ljs = reinterpret_cast<double*>(ws);
   int rc = B2B_OK;
   ScaleOp op{};
-  if (tri || inv || Abar) {
+  if (tri || lu || inv || Abar) {
     rc = scale_prep(d, workspace, D, true, &op, launches, stream);
     if (rc != B2B_OK) return rc;
   } else {
@@ -803,14 +941,19 @@ int b2b_vjp_scale(const B2BVjpSeg& s) {
   ++*launches;
   const long long DD = (long long)D * D;
   const unsigned g = (unsigned)((DD + 255) / 256);
-  gsum_kernel<<<g, 256, 0, stream>>>(part, ybar ? (int)P : 0, ljs, op.minv, D, op.mask, Abar, inv ? Gd : nullptr);
+  gsum_kernel<<<g, 256, 0, stream>>>(part, ybar ? (int)P : 0, ljs, op.minv, D, op.mask, Abar, inv || lu ? Gd : nullptr);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
   ++*launches;
-  if (!inv) return B2B_OK;
-  prod_gb_kernel<<<g, 256, 0, stream>>>(Gd, op.minv, D, op.mask, Tm);
+  if (inv) {  // the LU layer's M̄ = −B G B goes back to Gd (prod_gb_kernel has read it)
+    prod_gb_kernel<<<g, 256, 0, stream>>>(Gd, op.minv, D, op.mask, Tm);
+    if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
+    final_inv_kernel<<<g, 256, 0, stream>>>(Tm, op.minv, ljs, D, op.mask, Abar, lu ? Gd : nullptr);
+    if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
+    *launches += 2;
+  }
+  if (!lu) return B2B_OK;
+  lu_bar_kernel<<<g, 256, 0, stream>>>(Gd, d.p0, d.i0, ljs, inv ? -1.0 : 1.0, D, Abar);
   if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
-  final_inv_kernel<<<g, 256, 0, stream>>>(Tm, op.minv, ljs, D, op.mask, Abar);
-  if ((rc = (int)cudaGetLastError()) != cudaSuccess) return rc;
-  *launches += 2;
+  ++*launches;
   return B2B_OK;
 }

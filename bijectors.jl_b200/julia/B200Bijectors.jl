@@ -49,6 +49,8 @@ const COUPLING_DEEP_MLP_RQS = Int32(16)
 const ELEMENTWISE_VEC = Int32(17)
 const SCALE_TRIANGULAR = Int32(18)
 const SCALE_TRIANGULAR_MAX_D = 256
+const SCALE_LU = Int32(19)
+const SCALE_LU_MAX_D = 256
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -321,6 +323,21 @@ desc(b::Scale{<:TriMat{Float32}}, inv::Bool) =
 desc(b::Scale{<:TriMat{Float64}}, inv::Bool) =
     LayerDesc64(SCALE_TRIANGULAR, inv, tri_upper(b.a), tri_unit(b.a), 0, 0, 0.0, 0.0, pointer(parent(b.a)), NULLD, NULLD, NULLD,
                 NULLI, NULLI)
+# LULinear: the LU-parameterised linear layer y = P·L·U·x, one layer for Permute(p) ∘ Scale(UnitLowerTriangular(factors)) ∘
+# Scale(UpperTriangular(factors)).  `factors` packs L (strictly below the diagonal, unit diagonal implied) and U (on and
+# above it) as lu(A).factors does, and `p` is lu(A).p (1-based; nothing: the identity), so LULinear(cu(F.factors),
+# cu(Int32.(F.p))) of F = lu(A) maps y = A x.  logjac = Σ log|Uᵢᵢ|.  Float32 (D <= 256) or Float64 (D <= 2048); `factors`
+# trains as one parameter, both triangles.
+struct LULinear{T<:Union{Float32,Float64}} <: Bijectors.Bijector
+    factors::CuMatrix{T}
+    p::Union{Nothing,CuVector{Int32}}
+end
+const LU_DST = IdDict{Any,CuVector{Int32}}()  # p .- 1, the descriptor's 0-based destination rows
+lu_dst(b::LULinear) = b.p === nothing ? NULLI : pointer(get!(() -> b.p .- Int32(1), LU_DST, b.p))
+desc(b::LULinear{Float32}, inv::Bool) =
+    LayerDesc(SCALE_LU, inv, 0, 0, 0, 0, 0f0, 0f0, pointer(b.factors), NULLF, NULLF, NULLF, lu_dst(b), NULLI)
+desc(b::LULinear{Float64}, inv::Bool) =
+    LayerDesc64(SCALE_LU, inv, 0, 0, 0, 0, 0.0, 0.0, pointer(b.factors), NULLD, NULLD, NULLD, lu_dst(b), NULLI)
 # a whole-column elementwise law is a one-block Stacked
 const ElementwiseLaw = Union{Shift{<:Real},Scale{<:Real},LeakyReLU{<:Real},Logit{<:Real,<:Real},TruncatedBijector{<:Real,<:Real}}
 
@@ -335,7 +352,8 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           Coupling{<:MLPConditioner{<:CuMatrix{Float32}}},Coupling{<:MLPSplineConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}},
-                          Scale{<:CuMatrix{Float32}},Scale{<:TriMat{Float32}},VectorLaw{CuVector{Float32}},Permute,Stacked}
+                          Scale{<:CuMatrix{Float32}},Scale{<:TriMat{Float32}},LULinear{Float32},VectorLaw{CuVector{Float32}},Permute,
+                          Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
 is_device(::DeviceLeaf) = true
@@ -559,6 +577,7 @@ function vjp_slots(d::LayerDesc, D::Integer)
     end
     d.kind == SCALE_MATRIX && return (z(D, D),)
     d.kind == SCALE_TRIANGULAR && return (z(D, D),)  # exactly 0 outside the triangle; leaf_tangent wraps it
+    d.kind == SCALE_LU && return (z(D, D),)  # factors̄, packed as factors: L̄ below the diagonal, Ū on and above it
     d.kind == ELEMENTWISE_VEC && return (z(D),)  # Shift / Scale a, LeakyReLU α
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
@@ -696,6 +715,8 @@ function leaf_tangent(b, bar)
     names = fieldnames(typeof(b))
     return ChainRulesCore.Tangent{typeof(b)}(; (names[i] => bar[i] for i in eachindex(bar) if bar[i] !== nothing)...)
 end
+# LULinear: factors̄ only (the permutation has no cotangent)
+leaf_tangent(b::LULinear, bar) = bar[1] === nothing ? NoTangent() : ChainRulesCore.Tangent{typeof(b)}(factors=bar[1])
 # a triangular Scale's T̄ in the triangular type of its field
 leaf_tangent(b::Scale{<:TriMat}, bar) =
     bar[1] === nothing ? NoTangent() : ChainRulesCore.Tangent{typeof(b)}(a=Base.typename(typeof(b.a)).wrapper(bar[1]))

@@ -9,6 +9,7 @@ launch of the matching libb2b.so kernel (include/b2b.h).  No arithmetic on the b
   Permute                            src/bijectors/permute.jl:84-157
   Stacked / elementwise / Shift / Scale   src/bijectors/stacked.jl, exp_log.jl, shift.jl, scale.jl
   LowerTriangular / UpperTriangular / UnitLowerTriangular / UnitUpperTriangular   LinearAlgebra's wrappers, for Scale(T)
+  LULinear                           Permute(p) ∘ Scale(UnitLowerTriangular(F)) ∘ Scale(UpperTriangular(F)) as one layer
   LeakyReLU                          src/bijectors/leaky_relu.jl
 """
 from __future__ import annotations
@@ -961,6 +962,85 @@ class Scale(_ElementwiseLaw):
         if not isinstance(o, Scale) or self.dense != o.dense or self._tri is not o._tri:
             return False
         return torch.equal(self._A.cpu(), o._A.cpu()) if self._A is not None else _ElementwiseLaw.__eq__(self, o)
+
+    __hash__ = object.__hash__
+
+
+class LULinear(_ParamLayer):
+    """LULinear(F, p=None): the LU-parameterised invertible linear layer of Glow (its invertible 1×1 convolution) and of
+    nflows, y = P·L·U·x, one layer for `Permute(p) ∘ Scale(UnitLowerTriangular(F)) ∘ Scale(UpperTriangular(F))`
+    (B2B_SCALE_LU; Float32 D <= 256, Float64 D <= 2048).
+
+    F packs both factors as LAPACK getrf and Julia's `lu(A).factors` do: L strictly below the diagonal (its unit diagonal
+    implied, not read), U on and above it.  `p` is 1-based like `Permute(indices)` and `lu(A).p`: row r of L·U·x goes to
+    row p[r] of y, so `LULinear(lu(A).factors, lu(A).p)` is y = A x; None is the identity.  logjac = Σ log|Uᵢᵢ| per column,
+    and `inverse(layer)` is x = U⁻¹ L⁻¹ Pᵀ y.  F trains as one parameter, both triangles (cotangent key `factors`); p is
+    fixed.  A zero Uᵢᵢ is the caller's responsibility.  `_F` holds F column-major (Fᵀ row-major), as Scale's `_A`."""
+
+    _fields = ("_F",)
+
+    def __init__(self, F, p=None, device="cuda", dtype=torch.float32):
+        shape = tuple(F.shape) if isinstance(F, torch.Tensor) else np.shape(F)
+        if len(shape) != 2 or shape[0] != shape[1]:
+            raise ValueError(f"DimensionMismatch: LULinear needs a square F, got {shape}")
+        F = F.detach() if isinstance(F, torch.Tensor) else torch.as_tensor(np.asarray(F, dtype=np.float64))
+        self._F = _dev_f32(F.t(), device, dtype)
+        self._p, self._dst = None, None
+        if p is not None:
+            p = [int(v) for v in (p.tolist() if isinstance(p, torch.Tensor) else np.asarray(p).reshape(-1).tolist())]
+            if len(p) != shape[0]:
+                raise ValueError(f"DimensionMismatch: LULinear has a {shape[0]} x {shape[0]} F and {len(p)} indices")
+            self._p = Permute._from_indices(p) + 1
+            self._dst = _dev_i32(self._p - 1, device)
+
+    @classmethod
+    def from_matrix(cls, A, device="cuda", dtype=torch.float32):
+        """The layer of A's LU factorisation with partial pivoting, computed on the host in float64 (scipy.linalg.lu):
+        `LULinear.from_matrix(A)` maps y = A x up to the rounding of F to `dtype` -- Glow's initialisation from a random
+        rotation."""
+        from scipy.linalg import lu
+
+        A = np.asarray(A.detach().cpu().numpy() if isinstance(A, torch.Tensor) else A, dtype=np.float64)
+        if A.ndim != 2 or A.shape[0] != A.shape[1]:
+            raise ValueError(f"DimensionMismatch: LULinear.from_matrix needs a square matrix, got {A.shape}")
+        P, L, U = lu(A)  # A = P·L·U, so row r of L·U is row argmax(P[:, r]) of A
+        return cls(np.tril(L, -1) + U, np.argmax(P, axis=0) + 1, device=device, dtype=dtype)
+
+    @property
+    def factors(self) -> torch.Tensor:
+        return self._F.t()
+
+    @property
+    def L(self) -> UnitLowerTriangular:
+        return UnitLowerTriangular(self._F.t())
+
+    @property
+    def U(self) -> UpperTriangular:
+        return UpperTriangular(self._F.t())
+
+    @property
+    def p(self) -> np.ndarray:
+        return np.arange(1, self._F.shape[0] + 1) if self._p is None else self._p.copy()
+
+    def to(self, device):
+        new = _ParamLayer.to(self, device)
+        if self._dst is not None:
+            new._dst = self._dst.to(device)
+        return new
+
+    def _keepalive(self):
+        return (self._F,) if self._dst is None else (self._F, self._dst)
+
+    def _descs(self, inverse, D, dtype=torch.float32):
+        if D != self._F.shape[0]:
+            raise ValueError(f"DimensionMismatch: LULinear has a {self._F.shape[0]} x {self._F.shape[0]} F, input has {D} dims")
+        _check_dtype(self._F, dtype, "LULinear")
+        if self._dst is None:
+            return [_desc(_lib.SCALE_LU, inverse, p0=self._F)]
+        return [_desc(_lib.SCALE_LU, inverse, p0=self._F, i0=self._dst)]
+
+    def __eq__(self, o):
+        return isinstance(o, LULinear) and torch.equal(self._F.cpu(), o._F.cpu()) and np.array_equal(self.p, o.p)
 
     __hash__ = object.__hash__
 

@@ -113,6 +113,10 @@ extern "C" {
 /* Envelope of B2B_SCALE_TRIANGULAR: Float32 D <= 256 (the Float64 entry points: D <= 2048).  Beyond it every entry point
  * returns B2B_EUNSUPPORTED with nothing launched and the workspace queries return 0. */
 #define B2B_SCALE_TRIANGULAR_MAX_D 256
+#define B2B_SCALE_LU 19 /* LULinear: y = P*L*U*x, L, U packed in F as lu(A).factors, P from lu(A).p; logjac = Σ log|Uᵢᵢ|  (Glow's invertible 1x1 convolution) */
+/* Envelope of B2B_SCALE_LU: Float32 D <= 256 (the Float64 entry points: D <= 2048).  Beyond it every entry point returns
+ * B2B_EUNSUPPORTED with nothing launched and the workspace queries return 0. */
+#define B2B_SCALE_LU_MAX_D 256
 /* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and
  * B2B_COUPLING_DEEP_MLP_RQS (descriptor field n3) */
 #define B2B_ACT_TANH 0
@@ -231,6 +235,18 @@ extern "C" {
  *                     fp64 substitutions rounded to fp32) with zeros elsewhere; the map is exact fp32 FMA over the
  *                     triangle only.  Float32 D <= B2B_SCALE_TRIANGULAR_MAX_D, its own launches; Float64 D <= 2048, one
  *                     warp per column with T read through L2.  Trains T: slot 0 of b2b_chain_vjp_f32 / _f64.)
+ * SCALE_LU           F[D x D]    -           -           -        dst_of_src[D]   -             -     -    -
+ *                    (F column-major, required (NULL: B2B_EINVAL); i0 NULL is the identity permutation.  F packs two
+ *                     factors as LAPACK getrf and Julia's lu(A).factors do: the strict lower triangle is L, whose unit
+ *                     diagonal is implied and not read, and the upper triangle with the diagonal is U.  Per column
+ *                     y = P·L·U·x with y[i0[r]] = (L U x)[r] (PERMUTE's index semantics), so F = lu(A).factors with
+ *                     i0 = lu(A).p .- 1 is y = A x; logjac = Σᵢ log|Uᵢᵢ|, summed in fp64 in row order and rounded once.
+ *                     inverse != 0 gives y = U⁻¹ L⁻¹ Pᵀ x with the negated log-Jacobian.  The map of the composition
+ *                     PERMUTE(i0) ∘ SCALE_TRIANGULAR(F, unit lower) ∘ SCALE_TRIANGULAR(F, upper) in one layer.  A
+ *                     permutation in i0 and a non-zero Uᵢᵢ are the caller's contract.  A prep launch writes M = P·L·U or
+ *                     U⁻¹ L⁻¹ Pᵀ (each entry in fp64, rounded once to fp32); the map is SCALE_MATRIX's.  Float32
+ *                     D <= B2B_SCALE_LU_MAX_D, its own launches; Float64 D <= 2048, one warp per column with F read
+ *                     through L2.  Trains F: slot 0 of b2b_chain_vjp_f32 / _f64, packed like F.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -277,6 +293,11 @@ const char* b2b_status_string(int status);
  * y = M x, which skips the k-blocks that are zero for all rows a warp owns (about D(D+1)/2 FMA per column).  With y == NULL
  * the second launch writes the log-Jacobians only.  Its workspace is 4·D² + 8 bytes, each part rounded up to 256 bytes,
  * plus 256; a chain holding both Scale kinds shares one region of the larger of the two sizes.
+ * SCALE_LU runs in two launches the same way (D <= B2B_SCALE_LU_MAX_D, any N, y may alias x): a prep launch, parallel
+ * over columns, writing M = P·L·U or U⁻¹ L⁻¹ Pᵀ (fp32) and log|det U|, then SCALE_MATRIX's map y = M x (D² FMA per
+ * column).  With y == NULL the second launch writes the log-Jacobians only.  Its workspace is SCALE_TRIANGULAR's,
+ * 4·D² + 8 bytes, each part rounded up to 256 bytes, plus 256; a chain holding several Scale kinds (SCALE_MATRIX,
+ * SCALE_TRIANGULAR, SCALE_LU) shares one region of the larger of the sizes.
  * COUPLING_MLP runs in its own launch (any N, any ld >= D, scattered index lists, y may alias x; the envelope of
  * B2B_COUPLING_MLP_MAX_*; no workspace); like COUPLING_RQS, a batch sum needs the chain to end in a fused launch.
  * COUPLING_MLP_RQS runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x; the
@@ -431,6 +452,10 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * strictly below / above the diagonal for the unit forms, the diagonal included otherwise -- and exactly 0 outside 𝒫:
  * 𝒫(G) + (Σ l̄)·diag(1/Tᵢᵢ), or −𝒫(T⁻ᵀ G T⁻ᵀ) − (Σ l̄)·diag(1/Tᵢᵢ) for the inverse layer, no diagonal term for the unit
  * forms; slots 1-3 return B2B_EUNSUPPORTED);
+ * SCALE_LU a (F̄, D x D column-major and packed like F: with M̄ = G for the forward layer or −M⁻ᵀ G M⁻ᵀ for the inverse
+ * one, M = P·L·U, the strict lower triangle is L̄ = 𝒮(Pᵀ M̄ Uᵀ) and the upper one with the diagonal is
+ * Ū = 𝒰(Lᵀ Pᵀ M̄) + (Σ l̄)·diag(1/Uᵢᵢ), − (Σ l̄)·diag(1/Uᵢᵢ) for the inverse layer; the permutation has no cotangent;
+ * slots 1-3 return B2B_EUNSUPPORTED);
  * ELEMENTWISE_VEC a (ā[D], Σₙ of ḡ·∂y/∂a + l̄·∂ℓ/∂a at the layer's output cotangent ḡ; slots 1-3 return
  * B2B_EUNSUPPORTED); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
@@ -442,6 +467,9 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * the transposed triangular map; with T̄ requested G over column chunks -- on 𝒫 only, by the lower-triangle tiles, for the
  * forward layer -- Σ l̄, and a masked fp64 finalize: 3 launches more for the forward layer, 5 for the inverse; workspace:
  * its factor storage of b2b_chain_run_f32 plus P·D² floats and 2·D² + 1 doubles, each part rounded up to 256 bytes) /
+ * LU Scale (the prep launch, x̄ by the transposed dense map; with F̄ requested G over column chunks, Σ l̄, the dense
+ * finalize into an fp64 M̄ and one launch taking M̄ through the factors: 4 launches more for the forward layer, 6 for the
+ * inverse; workspace as for the triangular Scale) /
  * eval-BatchNorm layers -- and runs of <= 8 STACKED_EW / ELEMENTWISE_VEC / PERMUTE layers (with the terminal MvNormal),
  * which one kernel differentiates (with ā requested, a second instantiation that also sweeps the run backwards, plus
  * G·V·D floats of per-CTA partials for the V ELEMENTWISE_VEC layers of the run, G <= 8 per SM); a terminal MVNORMAL_TRIL is a segment of its own (D <= 256).  It writes x̄ = ȳ − l̄·L⁻ᵀL⁻¹(x − μ) in one
@@ -571,7 +599,7 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * `ybar` (B2B_EINVAL); NULL `ybar` / `ljbar` are zeros; `param_bars` (NULL = x̄ only) holds 4*L pointers, entry 4l+i the
  * cotangent of layers[l].p<i> in its shape and layout, summed over the N columns.  Trainable slots as for Float32: PLANAR
  * w u b; RADIAL α_ β z_0 (raw, through log1pexp); RQS widths heights derivatives (processed); COUPLING W c; ELEMENTWISE_VEC
- * a; SCALE_TRIANGULAR a (T̄, zero outside 𝒫); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
+ * a; SCALE_TRIANGULAR a (T̄, zero outside 𝒫); SCALE_LU a (F̄, packed like F); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ (B2B_EINVAL when
  * p0 is NULL) and L (D x D column-major, exactly zero above the diagonal); any other non-NULL entry returns
  * B2B_EUNSUPPORTED.  D > 2048 returns B2B_EUNSUPPORTED with nothing launched.  N == 0 zeroes the requested
  * parameter cotangents.  One warp per column recomputes the forward with the arithmetic of b2b_chain_run_f64, keeping
@@ -582,7 +610,7 @@ int b2b_chain_run_f64(const b2b_layer_desc_f64* layers, int32_t L, const double*
  * Workspace (b2b_chain_vjp_workspace_bytes_f64; 0 exactly when the call refuses the chain) is bounded independently of N:
  * W warp slots of 8·(T + P) bytes plus 8·P, with T = Lf·D (Lf: layers before the MvNormal) and P the accumulators, per
  * layer PLANAR 2D+2, RADIAL D+2, RQS 3·D·K1, COUPLING 2n1·n2 + 2n1, ELEMENTWISE_VEC D, BATCHNORM / MVNORMAL_DIAG 2D, MVNORMAL_TRIL
- * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄), SCALE_TRIANGULAR D(D+1)/2 (T̄'s packed triangle) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
+ * D + D(D+1)/2 (μ̄ and the packed lower triangle of L̄), SCALE_TRIANGULAR D(D+1)/2 (T̄'s packed triangle), SCALE_LU D² (F̄) doubles (each rounded up to 32); W = min(ceil(N / w), 528) CTAs of w warps (w = 4, or 3 for D > 1816), lowered so that the slots stay within
  * 256 MiB but never below one CTA -- so the bound exceeds 256 MiB only when one CTA's slots do (e.g. wide couplings with
  * 2n1·n2 in the millions).  The number of warps, and with it the summation order, depends only on the chain, D and N. */
 size_t b2b_chain_vjp_workspace_bytes_f64(const b2b_layer_desc_f64* layers, int32_t L, int32_t D, int64_t N);
