@@ -13,7 +13,7 @@ from .interface import (  # noqa: F401
 from .layers import (  # noqa: F401
     AffineConditioner, Coupling, Elementwise, InvertibleBatchNorm, LeakyReLU, Logit, MLPConditioner, MLPSplineConditioner, DeepMLPConditioner, DeepMLPSplineConditioner, PartitionMask, Permute, PlanarLayer, RadialLayer,
     RationalQuadraticSpline, Scale, Shift, SplineConditioner, Stacked, TruncatedBijector, coupling, elementwise,
-    LowerTriangular, UpperTriangular, UnitLowerTriangular, UnitUpperTriangular, LULinear,
+    LowerTriangular, UpperTriangular, UnitLowerTriangular, UnitUpperTriangular, LULinear, MaskedAutoregressive,
 )
 from .transformed_distribution import (  # noqa: F401
     MvNormal, PosDefException, TransformedDistribution, logpdf, logpdf_sum, logpdf_vjp, rand, rand_logpdf, rand_vjp,

@@ -28,6 +28,7 @@ COUPLING_DEEP_MLP_RQS_MAX_DEPTH, COUPLING_DEEP_MLP_RQS_MAX_D = 4, 1024
 ELEMENTWISE_VEC = 17
 SCALE_TRIANGULAR, SCALE_TRIANGULAR_MAX_D = 18, 256
 SCALE_LU, SCALE_LU_MAX_D = 19, 256
+AUTOREGRESSIVE_MLP, AUTOREGRESSIVE_MLP_MAX_D, AUTOREGRESSIVE_MLP_MAX_H = 20, 128, 256
 ACT_TANH, ACT_LEAKY_RELU = 0, 1
 EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = 0, 1, 2, 3, 4, 5, 6, 7
 MAX_CHAIN = 24

@@ -13,7 +13,7 @@ from . import _lib
 from ._lib import B2BError
 from .interface import (Composed, Inverse, _chain_vjp_raw, _trainable_slots, batchnorm_train_vjp, batchnorm_vjp, colmajor_empty,
                         coupling_vjp, flatten, inverse, planar_chain_vjp, radial_chain_vjp, rqs_vjp, run_chain)
-from .layers import (AffineConditioner, Coupling, InvertibleBatchNorm, LULinear, PartitionMask, PlanarLayer, RadialLayer,
+from .layers import (AffineConditioner, Coupling, InvertibleBatchNorm, LULinear, MaskedAutoregressive, PartitionMask, PlanarLayer, RadialLayer,
                      RationalQuadraticSpline, Scale, _ElementwiseLaw)
 
 
@@ -377,6 +377,8 @@ def _trainable_tensors(leaf) -> List[torch.Tensor]:
         return [lay._A]
     if isinstance(lay, LULinear):
         return [lay._F]
+    if isinstance(lay, MaskedAutoregressive):
+        return list(lay._tensors())
     if isinstance(lay, _ElementwiseLaw) and lay.vector:  # Shift / Scale / LeakyReLU with a vector parameter
         return [lay._a]
     if isinstance(lay, InvertibleBatchNorm):

@@ -90,6 +90,7 @@ static int fwd_envelope(const b2b_layer_desc& d, int D) {
     case B2B_SCALE_TRIANGULAR: ok = D <= B2B_SCALE_TRIANGULAR_MAX_D; break;
     case B2B_SCALE_LU: ok = D <= B2B_SCALE_LU_MAX_D; break;
     case B2B_MVNORMAL_TRIL: ok = D <= B2B_TRIL_MAX_D; break;
+    case B2B_AUTOREGRESSIVE_MLP: ok = b2b_ar_fits(d, D); break;
     default: ok = !b2b_is_coupling(d.kind) || b2b_coupling_fits(d, D); break;  // the other couplings' table
   }
   return ok ? B2B_OK : B2B_EUNSUPPORTED;
@@ -313,14 +314,14 @@ static bool sum_needs_logjac_ws(const b2b_layer_desc* layers, int32_t L, int nse
   return layers && L >= 1 && b2b_ends_in_terminal(layers, L) && nsegs > 1;
 }
 
-// factor storage of the dense, triangular and LU Scale layers (one region of the largest: they run one after another); 0
-// for a chain without one
+// factor storage of the dense, triangular and LU Scale layers and masked weights of the autoregressive layers (one
+// region of the largest: they run one after another); 0 for a chain without one
 static size_t chain_scale_bytes(const b2b_layer_desc* layers, int32_t L, int D) {
   size_t bytes = 0;
   for (int l = 0; layers && l < L; ++l) {
     const B2BKind* k = b2b_kind(layers[l].kind);
-    if (k && k->launch == B2B_LC_SCALE) {
-      const size_t b = b2b_scale_workspace(layers[l].kind, D);
+    if (k && (k->launch == B2B_LC_SCALE || k->launch == B2B_LC_AR)) {
+      const size_t b = k->launch == B2B_LC_AR ? b2b_ar_workspace(layers[l], D) : b2b_scale_workspace(layers[l].kind, D);
       if (b > bytes) bytes = b;
     }
   }
@@ -333,7 +334,8 @@ extern "C" size_t b2b_chain_workspace_bytes(const b2b_layer_desc* layers, int32_
   // limit, or a descriptor the call finds invalid, is still sized
   for (int l = 0; layers && l < L; ++l) {
     const B2BKind* k = b2b_kind(layers[l].kind);
-    if (k && (k->launch == B2B_LC_SPLINE || k->launch == B2B_LC_SCALE || k->launch == B2B_LC_MLP || (k->launch == B2B_LC_TRIL && l == L - 1)) &&
+    if (k && (k->launch == B2B_LC_SPLINE || k->launch == B2B_LC_SCALE || k->launch == B2B_LC_MLP || k->launch == B2B_LC_AR ||
+              (k->launch == B2B_LC_TRIL && l == L - 1)) &&
         fwd_envelope(layers[l], D) != B2B_OK)
       return 0;
   }
@@ -457,7 +459,8 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
     // destination of this segment: y when given, else scratch for intermediates, nothing for the last
     float* dst = y ? y : (last_seg ? nullptr : scratch);
     const long long dst_ld = y ? ldy : D;
-    const bool cpl = g.launch == B2B_LC_COUPLING, sc = g.launch == B2B_LC_SCALE;  // the classes with a workspace slice
+    // the classes with a workspace slice
+    const bool cpl = g.launch == B2B_LC_COUPLING, sc = g.launch == B2B_LC_SCALE || g.launch == B2B_LC_AR;
     const B2BFwdSeg a{layers + g.begin, g.end - g.begin, cur, cur_ld, dst, dst_ld, logjac, lj_started ? 1 : 0, D, N,
                       g.pre >= 0 ? &layers[g.pre] : nullptr, g.post >= 0 ? &layers[g.post] : nullptr, fold_ws,
                       last_seg ? partials : nullptr, sum_out, cpl ? tc_ws : sc ? scale_ws : nullptr,
@@ -469,6 +472,7 @@ extern "C" int b2b_chain_run_f32(const b2b_layer_desc* layers, int32_t L, const 
       case B2B_LC_MLP: rc = b2b_fwd_mlp(a); break;
       case B2B_LC_SCALE: rc = b2b_fwd_scale(a); break;
       case B2B_LC_TRIL: rc = b2b_fwd_tril(a); break;  // always the last segment
+      case B2B_LC_AR: rc = b2b_fwd_ar(a); break;
       default: rc = fwd_fused(a); break;
     }
     if (rc != B2B_OK) return rc;
@@ -815,6 +819,7 @@ size_t seg_kernel_bytes(const b2b_layer_desc* layers, const VSeg& s, int D, long
     case B2B_VC_SPLINE: return b2b_coupling_rqs_vjp_workspace(d, D, N);
     case B2B_VC_MLP: return b2b_coupling_mlp_vjp_workspace(d, D, N);
     case B2B_VC_SCALE: return b2b_scale_vjp_workspace(d.kind, D, N);  // also holds the factor of the forward recompute
+    case B2B_VC_AR: return b2b_ar_vjp_workspace(d, D, N);  // also holds the masked weights of the forward recompute
     default: {
       int vec = 0;
       for (int l = s.begin; l < s.end; ++l) vec += layers[l].kind == B2B_ELEMENTWISE_VEC;
@@ -1022,10 +1027,10 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
   ws += lay.param;
   void* kws = ws;
   const size_t kws_bytes = lay.kern;
-  // 1. forward recompute: the input of every segment after the first (a dense Scale keeps its factor in the kernel
-  // workspace, free until the reverse sweep)
+  // 1. forward recompute: the input of every segment after the first (a Scale keeps its factor, an autoregressive layer
+  // its masked weights in the kernel workspace, free until the reverse sweep)
   for (int s = 0; s + 1 < S; ++s) {
-    const bool sc = segs[s].kind == B2B_VC_SCALE;
+    const bool sc = segs[s].kind == B2B_VC_SCALE || segs[s].kind == B2B_VC_AR;
     rc = b2b_chain_run_f32(layers + segs[s].begin, segs[s].end - segs[s].begin, s == 0 ? x : ckpt[s], ckpt[s + 1],
                            nullptr, nullptr, D, N, s == 0 ? ldx : D, D, 0, sc ? kws : nullptr, sc ? kws_bytes : 0, stream);
     if (rc != B2B_OK) return rc;
@@ -1049,6 +1054,7 @@ extern "C" int b2b_chain_vjp_f32(const b2b_layer_desc* layers, int32_t L, const 
       case B2B_VC_TRIL: rc = b2b_vjp_tril(a); break;
       case B2B_VC_SPLINE: rc = b2b_vjp_spline(a); break;
       case B2B_VC_SCALE: rc = b2b_vjp_scale(a); break;
+      case B2B_VC_AR: rc = b2b_vjp_ar(a); break;
       default: rc = b2b_vjp_mlp(a); break;
     }
     if (rc != B2B_OK) return rc;

@@ -15,6 +15,7 @@
 #include <cuda_runtime.h>
 
 #include "b2b_coupling_mlp.cuh"
+#include "b2b_coupling_net.cuh"
 #include "b2b_coupling_tile.cuh"
 #include "b2b_internal.h"
 
@@ -32,30 +33,6 @@ struct CmlpParams {
   const float* Wh;  // W_2 .. W_M, each H x H column-major, back to back
   int depth;        // M hidden layers
 };
-
-// dst = σ(W·src + c) for one tile: W is H x nk column-major, src [nk][CP_LD], dst [H][CP_LD], c NULL = 0.  Eight
-// hidden rows per warp and step.
-__device__ __forceinline__ void cmlp_hidden(const float* src, int nk, const float* __restrict__ W,
-                                            const float* __restrict__ c, bool vec, int H, int act, float slope,
-                                            float* dst) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  auto same = [](int k) { return k; };
-  for (int jb = 8 * warp; jb < H; jb += 8 * (CP_THREADS / 32)) {
-    float va[4][2] = {}, vb[4][2] = {};
-    coupling_gemm_block<2>(src, CP_LD, same, nk, W + jb, W + jb + 4, H, H - jb, H - jb - 4, vec, va, vb);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const int m = jb + q;
-      if (m < H) {
-        const float cm = c ? __ldg(c + m) : 0.f;
-        float dh;
-#pragma unroll
-        for (int u = 0; u < 2; ++u)
-          mlp_act(act, slope, (q < 4 ? va[q & 3][u] : vb[q & 3][u]) + cm, dst[m * CP_LD + lane + 32 * u], dh);
-      }
-    }
-  }
-}
 
 template <bool INV>
 __global__ void __launch_bounds__(CP_THREADS, 2) coupling_mlp_kernel(const __grid_constant__ CmlpParams P) {

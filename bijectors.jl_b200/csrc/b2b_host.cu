@@ -27,12 +27,19 @@ struct b2b_host_ctx {
 
 static const size_t kWsBytes = 512 * 1024;  // batch-sum partials + tensor-core W image of a coupling layer
 
-// A chain with a dense, triangular or LU Scale also needs its factor storage, before the partials: the staging workspace grows
-// to hold the dense one's (the larger) at D_max, and only such chains are handed the larger size (every other chain sees
+// A chain with a dense, triangular or LU Scale also needs its factor storage, and one with an autoregressive layer its
+// masked weights, before the partials: the staging workspace grows to hold the larger of the dense Scale's and the
+// widest autoregressive layer's at D_max, and only such chains are handed the larger size (every other chain sees
 // kWsBytes, as before).
 static size_t ctx_ws_bytes(int D_max) {
   const int d = D_max < B2B_SCALE_MATRIX_MAX_D ? D_max : B2B_SCALE_MATRIX_MAX_D;
-  const size_t scale = b2b_scale_workspace(B2B_SCALE_MATRIX, d) + 4096 * sizeof(double) + 1024;
+  size_t scale = b2b_scale_workspace(B2B_SCALE_MATRIX, d);
+  b2b_layer_desc ar{};
+  ar.kind = B2B_AUTOREGRESSIVE_MLP;
+  ar.n2 = B2B_AUTOREGRESSIVE_MLP_MAX_H;
+  const size_t arb = b2b_ar_workspace(ar, D_max < B2B_AUTOREGRESSIVE_MLP_MAX_D ? D_max : B2B_AUTOREGRESSIVE_MLP_MAX_D);
+  if (arb > scale) scale = arb;
+  scale += 4096 * sizeof(double) + 1024;
   return scale > kWsBytes ? scale : kWsBytes;
 }
 
@@ -205,7 +212,8 @@ extern "C" int b2b_chain_run_host_f32(b2b_host_ctx* c, const b2b_layer_desc* lay
   const int nseg = b2b_chain_segment_count(layers, L, D);
   if (nseg < 0) return nseg;
   const bool stage_y = y_host != nullptr || nseg > 1;
-  const size_t ws_bytes = b2b_chain_has_launch(layers, L, B2B_LC_SCALE) ? c->ws_bytes : kWsBytes;
+  const size_t ws_bytes =
+      b2b_chain_has_launch(layers, L, B2B_LC_SCALE) || b2b_chain_has_launch(layers, L, B2B_LC_AR) ? c->ws_bytes : kWsBytes;
   for (long long k = 0; k < nchunks; ++k) {
     const int s = (int)(k % c->n_streams);
     cudaStream_t st = c->streams[s];

@@ -127,6 +127,12 @@ int b2b_launch_outer_chunks(const float* S, long long lds, const float* R, long 
 size_t b2b_scale_workspace(int kind, int D);
 // reverse mode: b2b_scale_vjp_workspace(kind, D, N) bytes (0 beyond the envelope)
 size_t b2b_scale_vjp_workspace(int kind, int D, long long N);
+// masked autoregressive layer (b2b_autoregressive.cu): whether its kernels take `d` at D (the
+// B2B_AUTOREGRESSIVE_MLP_MAX_* envelope), the masked-weight storage of its forward launches and the workspace of its
+// reverse mode (0 outside the envelope; bounded independently of N)
+bool b2b_ar_fits(const b2b_layer_desc& d, int D);
+size_t b2b_ar_workspace(const b2b_layer_desc& d, int D);
+size_t b2b_ar_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
 // spline coupling, reverse mode (b2b_coupling_rqs_vjp.cu): b2b_coupling_rqs_vjp_workspace(d, D, N) bytes (0 outside the
 // envelope, bounded independently of N)
 size_t b2b_coupling_rqs_vjp_workspace(const b2b_layer_desc& d, int D, long long N);
@@ -197,6 +203,7 @@ int b2b_fwd_spline(const B2BFwdSeg& s);  // b2b_coupling_rqs.cu: COUPLING_RQS, _
 int b2b_fwd_mlp(const B2BFwdSeg& s);     // b2b_coupling_mlp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
 int b2b_fwd_scale(const B2BFwdSeg& s);   // b2b_scale_matrix.cu: SCALE_MATRIX, _TRIANGULAR, _LU; y == NULL: log-Jacobians only
 int b2b_fwd_tril(const B2BFwdSeg& s);    // b2b_mvnormal_tril.cu: copies x to y (when y != x), writes logpdf to logjac
+int b2b_fwd_ar(const B2BFwdSeg& s);      // b2b_autoregressive.cu: AUTOREGRESSIVE_MLP; workspace: its masked weights
 
 // ---- reverse-mode segment launchers ----------------------------------------------------------------------------------
 // One segment of b2b_chain_vjp_f32: `n` layers of one B2BVjpClass, their input x, the cotangent ȳ of their output, l̄ (N
@@ -238,6 +245,7 @@ int b2b_vjp_tril(const B2BVjpSeg& s);      // b2b_mvnormal_tril.cu
 int b2b_vjp_spline(const B2BVjpSeg& s);    // b2b_coupling_rqs_vjp.cu: COUPLING_RQS, _MLP_RQS and _DEEP_MLP_RQS
 int b2b_vjp_scale(const B2BVjpSeg& s);     // b2b_scale_matrix.cu: SCALE_MATRIX, SCALE_TRIANGULAR, SCALE_LU
 int b2b_vjp_mlp(const B2BVjpSeg& s);       // b2b_coupling_mlp_vjp.cu: COUPLING_MLP and COUPLING_DEEP_MLP
+int b2b_vjp_ar(const B2BVjpSeg& s);        // b2b_autoregressive.cu: AUTOREGRESSIVE_MLP
 // One launch copying slot i of layer j from base[i] + j·step[i] to bars[4j + i], for the requested slots of a run of
 // n <= 8 layers at D (nothing is launched when none is requested).
 int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, const float* const base[3],
@@ -252,11 +260,12 @@ int b2b_copy_run_bars(const b2b_layer_desc* layers, int n, float* const* bars, c
 // in b2b_coupling, which b2b_slot_len and the coupling launchers read, and a row of b2b_coupling_fits.
 
 // Forward launch class: a run of fused column-local layers, or a launch of its own.
-enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP };
+enum B2BLaunchClass { B2B_LC_FUSED, B2B_LC_COUPLING, B2B_LC_SPLINE, B2B_LC_SCALE, B2B_LC_TRIL, B2B_LC_MLP, B2B_LC_AR };
 // Reverse-mode segment class of b2b_chain_vjp_f32 (B2B_VC_EW: runs of STACKED_EW / ELEMENTWISE_VEC / PERMUTE, with
 // MVNORMAL_DIAG).
 enum B2BVjpClass {
-  B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE, B2B_VC_MLP
+  B2B_VC_PLANAR, B2B_VC_RADIAL, B2B_VC_RQS, B2B_VC_COUPLING, B2B_VC_BN, B2B_VC_EW, B2B_VC_TRIL, B2B_VC_SPLINE, B2B_VC_SCALE, B2B_VC_MLP,
+  B2B_VC_AR
 };
 // descriptor pointer fields as bits
 enum { B2B_F_P0 = 1, B2B_F_P1 = 2, B2B_F_P2 = 4, B2B_F_P3 = 8, B2B_F_I0 = 16, B2B_F_I1 = 32 };
@@ -296,6 +305,7 @@ inline const B2BKind* b2b_kind(int kind) {
       {B2B_ELEMENTWISE_VEC, B2B_F_P0,                    false, B2B_LC_FUSED,    B2B_VC_EW,       1, 0,        true},
       {B2B_SCALE_TRIANGULAR, B2B_F_P0,                   false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        true},
       {B2B_SCALE_LU,        B2B_F_P0,                    false, B2B_LC_SCALE,    B2B_VC_SCALE,    1, 0,        true},
+      {B2B_AUTOREGRESSIVE_MLP, B2B_F_P0 | B2B_F_P2 | B2B_F_I0, false, B2B_LC_AR,   B2B_VC_AR,       4, B2B_F_P1 | B2B_F_P3, false},
   };
   for (const B2BKind& k : kinds)
     if (k.kind == kind) return &k;
@@ -317,8 +327,10 @@ inline bool b2b_chain_has_launch(const b2b_layer_desc* layers, int L, int launch
 // in this order, so the slot table of b2b_coupling fixes every role's offset and every slot's length.
 enum B2BRole { B2B_W_IN, B2B_C_IN, B2B_W_HID, B2B_W_OUT, B2B_C_OUT, B2B_NROLES };
 
-// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS descriptor decoded: the one place that knows how
-// include/b2b.h packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or b2b_layer_desc_f64.
+// A COUPLING_AFFINE / _RQS / _MLP / _MLP_RQS / _DEEP_MLP / _DEEP_MLP_RQS or AUTOREGRESSIVE_MLP descriptor decoded: the one
+// place that knows how include/b2b.h packs each kind's shape, law and parameters.  Desc is b2b_layer_desc or
+// b2b_layer_desc_f64.  AUTOREGRESSIVE_MLP is the network of COUPLING_MLP with n1 = n2 = D (the batch's rows, which
+// b2b_coupling takes as its second argument) and no index lists, plus the hidden units' degrees.
 template <class Desc>
 struct B2BCoupling {
   using Ptr = decltype(Desc::p0);
@@ -331,6 +343,7 @@ struct B2BCoupling {
   size_t off[B2B_NROLES], len[B2B_NROLES];  // its offset in the slot and its elements
   Ptr W_in, c_in, W_hid, W_out, c_out;      // the roles in the descriptor (NULL: absent)
   const int32_t *idx1, *idx2;
+  const int32_t* degrees;  // AUTOREGRESSIVE_MLP: the hidden units' degrees m[H] (NULL for the couplings)
   int row1, row2;    // affine law: first rows of idx1 / idx2 when they are contiguous ranges (< 0: use the list)
 
   // role r within the arrays p[0..3] of the four slots (NULL when the kind has no role r or its slot's array is NULL)
@@ -346,25 +359,27 @@ inline bool b2b_is_coupling(int kind) {
 }
 
 template <class Desc>
-B2BCoupling<Desc> b2b_coupling(const Desc& d) {
+B2BCoupling<Desc> b2b_coupling(const Desc& d, int D = 0) {
   const int k = d.kind;
   const bool deep_rqs = k == B2B_COUPLING_DEEP_MLP_RQS, deep = k == B2B_COUPLING_DEEP_MLP || deep_rqs;
+  const bool ar = k == B2B_AUTOREGRESSIVE_MLP;
   B2BCoupling<Desc> c{};
-  c.n1 = d.n0;
-  c.n2 = d.n1;
-  c.net = k == B2B_COUPLING_MLP || k == B2B_COUPLING_MLP_RQS || deep;
+  c.n1 = ar ? D : d.n0;
+  c.n2 = ar ? D : d.n1;
+  c.net = k == B2B_COUPLING_MLP || k == B2B_COUPLING_MLP_RQS || deep || ar;
   c.spline = k == B2B_COUPLING_RQS || k == B2B_COUPLING_MLP_RQS || deep_rqs;
   // MLP_RQS: n3 = σ | K << 8; DEEP_MLP: n3 = σ | M << 8; DEEP_MLP_RQS: n3 = σ | K << 8 | M << 16
   c.K = k == B2B_COUPLING_RQS ? d.n2 : k == B2B_COUPLING_MLP_RQS ? d.n3 >> 8 : deep_rqs ? (d.n3 >> 8) & 255 : 0;
   c.M = deep_rqs ? d.n3 >> 16 : deep ? d.n3 >> 8 : c.net ? 1 : 0;
   c.B = k == B2B_COUPLING_RQS ? d.f0 : k == B2B_COUPLING_MLP_RQS || deep_rqs ? d.f1 : 0;
-  c.idx1 = d.i0;
-  c.idx2 = d.i1;
+  c.idx1 = ar ? nullptr : d.i0;
+  c.idx2 = ar ? nullptr : d.i1;
+  c.degrees = ar ? d.i0 : nullptr;
   c.row1 = k == B2B_COUPLING_AFFINE ? d.n2 : -1;
   c.row2 = k == B2B_COUPLING_AFFINE ? d.n3 : -1;
   if (c.net) {
     c.H = d.n2;
-    c.act = k == B2B_COUPLING_MLP ? d.n3 : d.n3 & 255;
+    c.act = k == B2B_COUPLING_MLP || ar ? d.n3 : d.n3 & 255;
     c.slope = d.f0;
   }
   // the slot of each role: W_in, c_in, W_hid, W_out, c_out
@@ -417,6 +432,8 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
     return d.n0 == B2B_EW_SHIFT || d.n0 == B2B_EW_SCALE || d.n0 == B2B_EW_LEAKY_RELU ? B2B_OK : B2B_EINVAL;
   if (d.kind == B2B_SCALE_TRIANGULAR)  // n0: lower / upper, n1: stored / unit diagonal
     return (d.n0 == 0 || d.n0 == 1) && (d.n1 == 0 || d.n1 == 1) ? B2B_OK : B2B_EINVAL;
+  if (d.kind == B2B_AUTOREGRESSIVE_MLP)  // n2: H, n3: σ
+    return d.n2 >= 1 && (d.n3 == B2B_ACT_TANH || d.n3 == B2B_ACT_LEAKY_RELU) ? B2B_OK : B2B_EINVAL;
   if (!b2b_is_coupling(d.kind)) return B2B_OK;
   const B2BCoupling<Desc> c = b2b_coupling(d);
   bool ok = c.n1 >= 1 && c.n2 >= 1 && c.n1 + c.n2 <= D;
@@ -431,8 +448,8 @@ int b2b_check_desc(const Desc& d, int D, bool last) {
 // elements of trainable slot i of `d` (its cotangent has the parameter's shape)
 template <class Desc>
 size_t b2b_slot_len(const Desc& d, int i, int D) {
-  if (b2b_is_coupling(d.kind)) {  // the sum of the slot's roles
-    const B2BCoupling<Desc> c = b2b_coupling(d);
+  if (b2b_is_coupling(d.kind) || d.kind == B2B_AUTOREGRESSIVE_MLP) {  // the sum of the slot's roles
+    const B2BCoupling<Desc> c = b2b_coupling(d, D);
     size_t n = 0;
     for (int r = 0; r < B2B_NROLES; ++r)
       if (c.slot[r] == i) n += c.len[r];

@@ -841,6 +841,7 @@ _SLOTS = {
     _lib.COUPLING_MLP_RQS: (("W1", "c1", "W2", "c2"), _coupling_slots, (0, 2)),
     _lib.COUPLING_DEEP_MLP: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
     _lib.COUPLING_DEEP_MLP_RQS: (("W_in", "W_hid", "W_out", "c"), _coupling_slots, (0, 1, 2)),
+    _lib.AUTOREGRESSIVE_MLP: (("W1", "c1", "W2", "c2"), lambda d, D: ((D, d.n2), (d.n2,), (d.n2, 2 * D), (2 * D,)), (0, 2)),
     _lib.ELEMENTWISE_VEC: (("a",), lambda d, D: ((D,),), ()),  # named α for the LeakyReLU law (_slot_names)
 }
 _SLOT_NAMES = {kind: names for kind, (names, _, _) in _SLOTS.items()}
@@ -948,7 +949,7 @@ def chain_vjp(t, x: torch.Tensor, ybar: Optional[torch.Tensor] = None, ljbar: Op
     One b2b_chain_vjp_f32 call -- b2b_chain_vjp_f64 when ``x`` is a Float64 batch, whose layers and cotangents must then be
     Float64 too (a mix raises TypeError).  Returns ``(xbar, grads)``: ``grads`` has one dict per leaf of ``flatten(t)``
     (application order), keyed by the reference field names -- ``w/u/b``, ``α_/β/z_0``, ``widths/heights/derivatives``
-    (D×K+1), ``W/c``, ``b/logs``, ``a`` (D×D, a dense Scale; D, a vector Shift / Scale), ``factors`` (D×D, an LULinear), ``α`` (D, a vector LeakyReLU), and ``{}`` for Permute, Stacked and
+    (D×K+1), ``W/c``, ``b/logs``, ``a`` (D×D, a dense Scale; D, a vector Shift / Scale), ``factors`` (D×D, an LULinear), ``W1/c1/W2/c2`` (a MaskedAutoregressive, exactly 0 outside its masks), ``α`` (D, a vector LeakyReLU), and ``{}`` for Permute, Stacked and
     the scalar elementwise layers -- summed over the columns of this batch."""
     D = _batch_view(x)[0]
     descs, counts = _leaf_descs(t, D, x.dtype)

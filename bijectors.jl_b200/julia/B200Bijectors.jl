@@ -51,6 +51,9 @@ const SCALE_TRIANGULAR = Int32(18)
 const SCALE_TRIANGULAR_MAX_D = 256
 const SCALE_LU = Int32(19)
 const SCALE_LU_MAX_D = 256
+const AUTOREGRESSIVE_MLP = Int32(20)
+const AUTOREGRESSIVE_MLP_MAX_D = 128
+const AUTOREGRESSIVE_MLP_MAX_H = 256
 const ACT_TANH, ACT_LEAKY_RELU = Int32(0), Int32(1)
 const EW_IDENTITY, EW_EXP, EW_LOG, EW_SHIFT, EW_SCALE, EW_LEAKY_RELU, EW_LOGIT, EW_TRUNCATED = Int32.(0:7)
 const NULLF = CuPtr{Float32}(0)
@@ -338,6 +341,52 @@ desc(b::LULinear{Float32}, inv::Bool) =
     LayerDesc(SCALE_LU, inv, 0, 0, 0, 0, 0f0, 0f0, pointer(b.factors), NULLF, NULLF, NULLF, lu_dst(b), NULLI)
 desc(b::LULinear{Float64}, inv::Bool) =
     LayerDesc64(SCALE_LU, inv, 0, 0, 0, 0, 0.0, 0.0, pointer(b.factors), NULLD, NULLD, NULLD, lu_dst(b), NULLI)
+# MaskedAutoregressive: MAF / IAF's affine layer with a MADE conditioner, y = x .* exp.(s) .+ t with
+# [s; t] = (M₂ .* W2) * σ.((M₁ .* W1) * x .+ c1) .+ c2, masks M₁[k, r] = (r <= m_k), M₂[i, k] = M₂[D+i, k] = (m_k < i) from
+# the hidden units' integer degrees m (so sᵢ, tᵢ depend on x₁..x_{i−1} only); logjac = Σ s.  W1 is (H × D), W2 (2D × H),
+# c1 / c2 === nothing is a zero shift, σ = tanh or LeakyReLU(slope).  The inverse recovers x row by row; MAF is a chain of
+# inverse(layer)s.  Float32, D <= 128, H <= 256 on the device; the same object runs on the CPU reference path.
+struct MaskedAutoregressive{M<:AbstractMatrix,V1,V2,I<:AbstractVector} <: Bijectors.Bijector
+    W1::M   # (H × D)
+    c1::V1  # H, or nothing
+    W2::M   # (2D × H)
+    c2::V2  # 2D, or nothing
+    degrees::I      # m (Int32 on the device)
+    act::Int32      # ACT_TANH or ACT_LEAKY_RELU
+    slope::Float32
+end
+function ar_shift_scale(b::MaskedAutoregressive, X::AbstractMatrix)
+    D, m = size(X, 1), collect(b.degrees)
+    W1 = ifelse.((1:D)' .<= m, b.W1, zero(eltype(b.W1)))  # entries outside the masks are never used
+    W2 = ifelse.(repeat(m' .< (1:D), 2, 1), b.W2, zero(eltype(b.W2)))
+    u = b.c1 === nothing ? W1 * X : W1 * X .+ b.c1
+    h = b.act == ACT_TANH ? tanh.(u) : ifelse.(u .>= 0, u, b.slope .* u)
+    st = b.c2 === nothing ? W2 * h : W2 * h .+ b.c2
+    return st[1:D, :], st[(D + 1):end, :]
+end
+function with_logabsdet_jacobian(b::MaskedAutoregressive, x::AbstractVecOrMat)
+    X = x isa AbstractVector ? reshape(x, :, 1) : x
+    s, t = ar_shift_scale(b, X)
+    Y, lj = X .* exp.(s) .+ t, vec(sum(s; dims=1))
+    return x isa AbstractVector ? (vec(Y), lj[1]) : (Y, lj)
+end
+function with_logabsdet_jacobian(ib::Inverse{<:MaskedAutoregressive}, y::AbstractVecOrMat)
+    Y = y isa AbstractVector ? reshape(y, :, 1) : y
+    X = zero(Y)
+    for i in axes(Y, 1)  # rows >= i of X are still 0 and do not reach sᵢ, tᵢ
+        s, t = ar_shift_scale(ib.orig, X)
+        X[i:i, :] .= (Y[i:i, :] .- t[i:i, :]) ./ exp.(s[i:i, :])
+    end
+    lj = -vec(sum(first(ar_shift_scale(ib.orig, X)); dims=1))
+    return y isa AbstractVector ? (vec(X), lj[1]) : (X, lj)
+end
+transform(b::Union{MaskedAutoregressive,Inverse{<:MaskedAutoregressive}}, x::AbstractVecOrMat) =
+    first(with_logabsdet_jacobian(b, x))
+function desc(b::MaskedAutoregressive{<:CuMatrix{Float32}}, inv::Bool)
+    ptr(c) = c === nothing ? NULLF : pointer(c)
+    LayerDesc(AUTOREGRESSIVE_MLP, inv, 0, 0, size(b.W1, 1), b.act, b.slope, 0f0, pointer(b.W1), ptr(b.c1), pointer(b.W2),
+              ptr(b.c2), pointer(b.degrees), NULLI)
+end
 # a whole-column elementwise law is a one-block Stacked
 const ElementwiseLaw = Union{Shift{<:Real},Scale{<:Real},LeakyReLU{<:Real},Logit{<:Real,<:Real},TruncatedBijector{<:Real,<:Real}}
 
@@ -353,6 +402,7 @@ const DeviceLayer = Union{PlanarLayer{<:CuVector{Float32}},RadialLayer{<:CuVecto
                           Coupling{<:DeepMLPConditioner{<:CuMatrix{Float32}}},
                           Coupling{<:DeepMLPSplineConditioner{<:CuMatrix{Float32}}},
                           Scale{<:CuMatrix{Float32}},Scale{<:TriMat{Float32}},LULinear{Float32},VectorLaw{CuVector{Float32}},Permute,
+                          MaskedAutoregressive{<:CuMatrix{Float32},<:Any,<:Any,<:CuVector{Int32}},
                           Stacked}
 const DeviceLeaf = Union{DeviceLayer,Inverse{<:DeviceLayer}}
 is_device(f::ComposedFunction) = is_device(f.inner) && is_device(f.outer)
@@ -577,7 +627,9 @@ function vjp_slots(d::LayerDesc, D::Integer)
     end
     d.kind == SCALE_MATRIX && return (z(D, D),)
     d.kind == SCALE_TRIANGULAR && return (z(D, D),)  # exactly 0 outside the triangle; leaf_tangent wraps it
-    d.kind == SCALE_LU && return (z(D, D),)  # factors̄, packed as factors: L̄ below the diagonal, Ū on and above it
+    d.kind == SCALE_LU && return (z(D, D),)
+    d.kind == AUTOREGRESSIVE_MLP &&
+        return (z(d.n2, D), d.p1 == NULLF ? nothing : z(d.n2), z(2D, d.n2), d.p3 == NULLF ? nothing : z(2D))  # factors̄, packed as factors: L̄ below the diagonal, Ū on and above it
     d.kind == ELEMENTWISE_VEC && return (z(D),)  # Shift / Scale a, LeakyReLU α
     d.kind == BATCHNORM && return (z(D), z(D))
     d.kind == MVNORMAL_DIAG && return (d.p0 == NULLF ? nothing : z(D), d.p1 == NULLF ? nothing : z(D))
@@ -717,6 +769,9 @@ function leaf_tangent(b, bar)
 end
 # LULinear: factors̄ only (the permutation has no cotangent)
 leaf_tangent(b::LULinear, bar) = bar[1] === nothing ? NoTangent() : ChainRulesCore.Tangent{typeof(b)}(factors=bar[1])
+# MaskedAutoregressive: W̄1 c̄1 W̄2 c̄2 (c̄ only where the layer has c), W̄ exactly 0 outside the masks
+leaf_tangent(b::MaskedAutoregressive, bar) = all(t -> t === nothing, bar) ? NoTangent() :
+    ChainRulesCore.Tangent{typeof(b)}(; (k => v for (k, v) in zip((:W1, :c1, :W2, :c2), bar) if v !== nothing)...)
 # a triangular Scale's T̄ in the triangular type of its field
 leaf_tangent(b::Scale{<:TriMat}, bar) =
     bar[1] === nothing ? NoTangent() : ChainRulesCore.Tangent{typeof(b)}(a=Base.typename(typeof(b.a)).wrapper(bar[1]))

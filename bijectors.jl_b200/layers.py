@@ -10,6 +10,7 @@ launch of the matching libb2b.so kernel (include/b2b.h).  No arithmetic on the b
   Stacked / elementwise / Shift / Scale   src/bijectors/stacked.jl, exp_log.jl, shift.jl, scale.jl
   LowerTriangular / UpperTriangular / UnitLowerTriangular / UnitUpperTriangular   LinearAlgebra's wrappers, for Scale(T)
   LULinear                           Permute(p) ∘ Scale(UnitLowerTriangular(F)) ∘ Scale(UpperTriangular(F)) as one layer
+  MaskedAutoregressive               MAF / IAF's affine layer with a MADE conditioner
   LeakyReLU                          src/bijectors/leaky_relu.jl
 """
 from __future__ import annotations
@@ -1041,6 +1042,109 @@ class LULinear(_ParamLayer):
 
     def __eq__(self, o):
         return isinstance(o, LULinear) and torch.equal(self._F.cpu(), o._F.cpu()) and np.array_equal(self.p, o.p)
+
+    __hash__ = object.__hash__
+
+
+class MaskedAutoregressive(_ParamLayer):
+    """MaskedAutoregressive(W1, c1, W2, c2, degrees=None, activation="tanh", slope=0.0): the affine autoregressive layer of
+    MAF (Papamakarios et al. 2017) and IAF (Kingma et al. 2016) with a one-hidden-layer MADE conditioner
+    (B2B_AUTOREGRESSIVE_MLP; Float32, D <= 128, H <= 256).  Per column, with 1-based rows r and hidden units k of
+    degree m_k, masks M₁[k, r] = (r <= m_k) and M₂[i, k] = M₂[D+i, k] = (m_k < i):
+
+        [s; t] = (M₂⊙W₂)·σ.((M₁⊙W₁)·x + c₁) + c₂,   y = x ⊙ exp.(s) + t,   logjac = Σ s
+
+    so sᵢ, tᵢ depend on x₁..x_{i−1} only.  W1 is (H × D) and W2 (2D × H), rows 1..D of W2 giving s and the rest t; c1
+    (H) and c2 (2D) may be None.  σ is tanh or LeakyReLU(slope) as for :class:`MLPConditioner`.  `degrees` are any H
+    integers, by default MADE's cyclic m_k = ((k−1) mod max(D−1, 1)) + 1; entries outside the masks are never read.
+
+    The layer itself (IAF: sampling runs it) is one network evaluation; `inverse(layer)` recovers x row by row (MAF is
+    a flow of inverse layers: its logpdf runs the forward network, rand the sequential recovery).  Rows are taken in
+    natural order: put a :class:`Permute` between layers for another.  The cotangents are keyed W1, c1, W2 and c2.
+    `_W1` / `_W2` hold W1 and W2 column-major (their transposes row-major), as the descriptor reads them."""
+
+    def __init__(self, W1, c1, W2, c2, degrees=None, activation="tanh", slope=0.0, device="cuda", dtype=torch.float32):
+        if dtype != torch.float32:
+            raise TypeError("MaskedAutoregressive: the autoregressive layer runs in Float32 only")
+        if activation not in _ACT:
+            raise ValueError(f"MaskedAutoregressive: activation must be one of {sorted(_ACT)}, got {activation!r}")
+        W1n, W2n = _host32(W1), _host32(W2)
+        if W1n.ndim != 2 or W1n.shape[0] == 0 or W1n.shape[1] == 0:
+            raise ValueError(f"DimensionMismatch: MaskedAutoregressive W1 must be (H, D), got {W1n.shape}")
+        H, D = W1n.shape
+        if W2n.shape != (2 * D, H):
+            raise ValueError(f"DimensionMismatch: MaskedAutoregressive W2 must be (2D, H) = {(2 * D, H)}, got {W2n.shape}")
+        if degrees is None:
+            degrees = np.arange(H) % max(D - 1, 1) + 1
+        deg = np.asarray(degrees.detach().cpu() if isinstance(degrees, torch.Tensor) else degrees).reshape(-1)
+        if deg.shape != (H,):
+            raise ValueError(f"DimensionMismatch: MaskedAutoregressive has {H} hidden units and {deg.size} degrees")
+        if not np.array_equal(deg, np.round(deg)):
+            raise ValueError("MaskedAutoregressive: degrees must be integers")
+        self.D, self.H, self.activation, self.slope = D, H, activation, float(slope)
+        self._W1 = _dev_f32(np.ascontiguousarray(W1n.T), device)  # column-major (H × D)
+        self._W2 = _dev_f32(np.ascontiguousarray(W2n.T), device)  # column-major (2D × H)
+        self.c1 = _bias(c1, "c1", H, device)
+        self.c2 = _bias(c2, "c2", 2 * D, device)
+        self._deg = _dev_i32(deg.astype(np.int64), device)
+
+    @property
+    def W1(self) -> torch.Tensor:
+        return self._W1.t()
+
+    @property
+    def W2(self) -> torch.Tensor:
+        return self._W2.t()
+
+    @property
+    def degrees(self) -> np.ndarray:
+        return self._deg.cpu().numpy().astype(np.int64)
+
+    @property
+    def masks(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(M₁ (H × D), M₂ (2D × H)) as boolean tensors on the layer's device."""
+        m = self._deg.to(torch.int64)
+        r = torch.arange(1, self.D + 1, device=m.device)
+        M1 = r[None, :] <= m[:, None]
+        M2 = (m[None, :] < r[:, None]).repeat(2, 1)
+        return M1, M2
+
+    @property
+    def device(self):
+        return self._W1.device
+
+    def to(self, device):
+        new = object.__new__(MaskedAutoregressive)
+        new.__dict__.update(self.__dict__)
+        for k in ("_W1", "_W2", "c1", "c2", "_deg"):
+            t = getattr(self, k)
+            setattr(new, k, None if t is None else t.to(device))
+        new._cache = {}
+        return new
+
+    def params(self) -> Dict[str, torch.Tensor]:
+        return {"W1": self.W1, "c1": self.c1, "W2": self.W2, "c2": self.c2}
+
+    def _tensors(self):
+        return tuple(t for t in (self._W1, self.c1, self._W2, self.c2) if t is not None)
+
+    def _keepalive(self):
+        return self._tensors() + (self._deg,)
+
+    def _descs(self, inverse, D, dtype=torch.float32):
+        if D != self.D:
+            raise ValueError(f"DimensionMismatch: MaskedAutoregressive has {self.D} dims, input has {D}")
+        _check_dtype(self._W1, dtype, "MaskedAutoregressive")
+        return [_desc(_lib.AUTOREGRESSIVE_MLP, inverse, p0=self._W1, p1=self.c1 if self.c1 is not None else 0,
+                      p2=self._W2, p3=self.c2 if self.c2 is not None else 0, i0=self._deg, n2=self.H,
+                      n3=_ACT[self.activation], f0=self.slope)]
+
+    def __eq__(self, o):
+        def same(a, b):
+            return (a is None and b is None) or (a is not None and b is not None and torch.equal(a.cpu(), b.cpu()))
+
+        return (isinstance(o, MaskedAutoregressive) and self.activation == o.activation and self.slope == o.slope and
+                all(same(getattr(self, k), getattr(o, k)) for k in ("_W1", "_W2", "c1", "c2", "_deg")))
 
     __hash__ = object.__hash__
 

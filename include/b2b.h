@@ -117,8 +117,14 @@ extern "C" {
 /* Envelope of B2B_SCALE_LU: Float32 D <= 256 (the Float64 entry points: D <= 2048).  Beyond it every entry point returns
  * B2B_EUNSUPPORTED with nothing launched and the workspace queries return 0. */
 #define B2B_SCALE_LU_MAX_D 256
-/* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and
- * B2B_COUPLING_DEEP_MLP_RQS (descriptor field n3) */
+#define B2B_AUTOREGRESSIVE_MLP 20 /* MaskedAutoregressive: y = x ⊙ exp.(s) + t, [s; t] from a MADE of x₁..x_{i−1} for row i  (MAF / IAF) */
+/* Envelope of B2B_AUTOREGRESSIVE_MLP (every Float32 entry point, both directions and reverse mode): D <= 128,
+ * 1 <= H <= 256.  Beyond it every entry point returns B2B_EUNSUPPORTED with nothing launched and the workspace queries
+ * return 0; the Float64 entry points refuse the kind the same way. */
+#define B2B_AUTOREGRESSIVE_MLP_MAX_D 128
+#define B2B_AUTOREGRESSIVE_MLP_MAX_H 256
+/* hidden-layer activation σ of B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP,
+ * B2B_COUPLING_DEEP_MLP_RQS and B2B_AUTOREGRESSIVE_MLP (descriptor field n3) */
 #define B2B_ACT_TANH 0
 #define B2B_ACT_LEAKY_RELU 1 /* v >= 0 ? v : a*v with a = f0 (a = 0: ReLU), the convention of B2B_EW_LEAKY_RELU */
 
@@ -247,6 +253,18 @@ extern "C" {
  *                     U⁻¹ L⁻¹ Pᵀ (each entry in fp64, rounded once to fp32); the map is SCALE_MATRIX's.  Float32
  *                     D <= B2B_SCALE_LU_MAX_D, its own launches; Float64 D <= 2048, one warp per column with F read
  *                     through L2.  Trains F: slot 0 of b2b_chain_vjp_f32 / _f64, packed like F.)
+ * AUTOREGRESSIVE_MLP W₁[H x D]  c₁[H]|NULL  W₂[2D x H] c₂[2D]|NULL m[H]           -             -     -    H    σ   a
+ *                    (a MADE layer: i0 holds the hidden units' integer degrees m_k (int32, any value), n2 = H hidden
+ *                     units, n3 = σ: B2B_ACT_TANH or B2B_ACT_LEAKY_RELU with slope a = f0; any other n3 returns
+ *                     B2B_EINVAL.  W₁, W₂ and m are required, c₁ / c₂ may be NULL (= 0); W₁ and W₂ are column-major.
+ *                     With 1-based rows r and masks M₁[k, r] = (r <= m_k), M₂[i, k] = M₂[D+i, k] = (m_k < i), per column
+ *                     [s; t] = (M₂⊙W₂)·σ.((M₁⊙W₁)·x + c₁) + c₂ and y = x ⊙ exp.(s) + t, logjac = Σ s: sᵢ and tᵢ depend
+ *                     on x₁..x_{i−1} only, so the Jacobian is lower triangular for any degrees.  Entries outside the
+ *                     masks are not read and may hold anything, NaN included.  inverse != 0 recovers x row by row,
+ *                     xᵢ = (yᵢ − tᵢ)/exp(sᵢ) with sᵢ, tᵢ from the rows already recovered, logjac = −Σ s(x).  The forward
+ *                     direction (IAF sampling, MAF's logpdf through inverse) is one network evaluation, exact fp32 FMA
+ *                     on the CUDA cores; the inverse is sequential over the D rows.  Float32 only, its own launches.
+ *                     Envelope: B2B_AUTOREGRESSIVE_MLP_MAX_*.  Trains W₁ c₁ W₂ c₂: slots 0-3 of b2b_chain_vjp_f32.)
  * Any other kind value returns B2B_EINVAL.
  */
 typedef struct b2b_layer_desc {
@@ -306,6 +324,12 @@ const char* b2b_status_string(int status);
  * envelope of B2B_COUPLING_DEEP_MLP_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
  * COUPLING_DEEP_MLP_RQS runs in its own launch the same way (any N, any ld >= D, scattered index lists, y may alias x;
  * the envelope of B2B_COUPLING_DEEP_MLP_RQS_MAX_*; no workspace; a batch sum needs the chain to end in a fused launch).
+ * AUTOREGRESSIVE_MLP runs in two launches (D <= B2B_AUTOREGRESSIVE_MLP_MAX_D, H <= B2B_AUTOREGRESSIVE_MLP_MAX_H, any
+ * N, any ld >= D, y may alias x): a prep launch writing the masked weights M₁⊙W₁, M₂⊙W₂ (zeros outside the masks) and
+ * a row-paired copy of M₂⊙W₂, then the forward network over 64-column tiles or, for inverse != 0, the sequential
+ * recovery, one warp per four columns.  Its workspace is 5·H·D floats in three parts (H·D, 2·H·D, 2·H·D), each rounded
+ * up to 256 bytes, plus 256, shared with the Scale layers' region (one region of the largest; the layers run one after
+ * another); a batch sum needs the chain to end in a fused launch.
  * The whole chain is planned before anything is enqueued: a
  * layer that fits no kernel returns B2B_EUNSUPPORTED with nothing launched and no output written.
  * If the last element is B2B_MVNORMAL_DIAG, `logjac` receives logpdf[n] = logpdf(MvNormal)(x_n) +
@@ -456,6 +480,8 @@ int b2b_rqs_vjp_f32(const b2b_layer_desc* layer, const float* x, const float* yb
  * one, M = P·L·U, the strict lower triangle is L̄ = 𝒮(Pᵀ M̄ Uᵀ) and the upper one with the diagonal is
  * Ū = 𝒰(Lᵀ Pᵀ M̄) + (Σ l̄)·diag(1/Uᵢᵢ), − (Σ l̄)·diag(1/Uᵢᵢ) for the inverse layer; the permutation has no cotangent;
  * slots 1-3 return B2B_EUNSUPPORTED);
+ * AUTOREGRESSIVE_MLP W₁ c₁ W₂ c₂ (column-major like the parameters, the W̄ entries outside the masks exactly 0; a c̄₁ /
+ * c̄₂ request whose c is NULL returns B2B_EINVAL);
  * ELEMENTWISE_VEC a (ā[D], Σₙ of ḡ·∂y/∂a + l̄·∂ℓ/∂a at the layer's output cotangent ḡ; slots 1-3 return
  * B2B_EUNSUPPORTED); BATCHNORM b logs; MVNORMAL_DIAG μ σ (only where the parameter pointer is non-NULL, else B2B_EINVAL); MVNORMAL_TRIL μ
  * (B2B_EINVAL when p0 is NULL) and L (D x D column-major, its upper triangle exactly zero).  Any other non-NULL entry
@@ -569,7 +595,8 @@ int b2b_mvnormal_diag_logpdf_f32(const float* x, const float* mu, const float* s
 /* ---- Float64 batches -------------------------------------------------------------------------------------------------
  * The reference is generic in its element type and its own tests run in Float64 (test/normalising_flows.jl:47-71 checks
  * find_alpha to 1e-14).  b2b_chain_run_f64 evaluates the same chains -- every layer kind but B2B_COUPLING_RQS,
- * B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP and B2B_COUPLING_DEEP_MLP_RQS (Float32 only: the Float64
+ * B2B_COUPLING_MLP, B2B_COUPLING_MLP_RQS, B2B_COUPLING_DEEP_MLP, B2B_COUPLING_DEEP_MLP_RQS and B2B_AUTOREGRESSIVE_MLP
+ * (Float32 only: the Float64
  * entry points and workspace
  * queries refuse them with B2B_EUNSUPPORTED / 0),
  * both directions, the terminal
